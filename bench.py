@@ -3,13 +3,13 @@
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--precision fp16|fp32]
                     [--config mnist|fmnist|celeba] [--batch B --rec_rr R --rec_iters L]
-                    [--scaling weak|strong] [--no_extra] [--no_profile]
+                    [--scaling weak|strong] [--no_extra] [--no_profile] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic images: one `gan.reconstruct` call =
 R restarts x L momentum-GD steps of generator forward + MSE + backward-to-z, then arg-min select.
 
 Workloads (BASELINE.json `configs`):
-  N=1   configs[1]: MNIST 28x28, R=10, L=200, batch=256 on one B200 - the configuration the metric is quoted on.
+  N=1   configs[1]: MNIST 28x28, R=10, L=200, batch=256 on one H100 - the configuration the metric is quoted on.
         The same line carries configs[2] (F-MNIST: the same generator class with a second weight seed, SURVEY 8d)
         and configs[3] (CelebA 64x64x3, batch 128) under `extra_configs`, and the per-GPU share of configs[4]
         (512 images on one GPU) under `weak_scaling_base`.
@@ -21,9 +21,13 @@ and is inside both timed regions.
 Prints ONE JSON line (rank 0).  `value` = images/s with inputs resident in HBM, CUDA-event timed, max over ranks;
 `e2e` = the same through the public Python API with pinned HOST buffers (H2D of the images, the all-gather and the
 D2H of the reconstructions inside the timed region); `roofline` = the dominant kernel's algorithmic FLOP/s (CUDA
-events around each launch on the launching stream, in a separate pass) against the measured bf16 tensor peak in
-MEASURED_PEAKS.json; `cpu_baseline` = the oracle restatement of the reference's TF1 CPU path on this box's host
+events around each launch on the launching stream, in a separate pass) against the bf16 tensor peak of
+MEASURED_PEAKS.json when present, else the H100 SXM data-sheet rate; `cpu_baseline` = the oracle restatement of the reference's TF1 CPU path on this box's host
 cores (bounded sample).  `--impl reference` times only that CPU port (the reference itself cannot run: no TF1/py2).
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step returned - the reconstructions
+[B_global, H, W, C] - as DIR/rec.npy (float32; a fixed, seeded sample of the images when the batch exceeds 64 MB).
+The inputs depend only on the command line, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -50,7 +54,9 @@ CONFIGS = {
 C5_GLOBAL_BATCH = 4096                    # configs[4]: MNIST R=10 L=200, batch 4096 sharded across 8 GPUs
 C5_PER_GPU = C5_GLOBAL_BATCH // 8
 FMNIST_WEIGHT_SEED = 11241991             # synthetic C3 differs from C2 only in the weights (SURVEY 8d)
-FALLBACK_PEAKS = {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0}
+# NVIDIA H100 SXM data sheet (dense, 700 W): used only when no MEASURED_PEAKS.json is present
+FALLBACK_PEAKS = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0}
+DUMP_MAX_BYTES = 64 * 1024 * 1024
 
 
 def load_peaks():
@@ -66,7 +72,7 @@ def load_peaks():
 
 
 class ClockSampler:
-    """nvidia-smi sampler running DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running DURING the timed region: the SM clock and throttle reasons the number was taken at."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -310,14 +316,19 @@ class Workload:
         self.gan.rec_rr, self.gan.rec_iters, self.gan.rec_lr = R, L, 10.0
         self.hwc = int(np.prod(self.gan.image_dim))
         self.B_global = B_local * world
-        # synthetic inputs (SURVEY 8d, S1: on-manifold + noise): generated ON DEVICE by the native generator
+        # synthetic inputs (SURVEY 8d, S1: on-manifold + noise), made by the fp32 CPU oracle generator: they depend only on
+        # the command line, not on the kernels under test, so two builds (or two precisions) see the same images
+        from oracle import defensegan_oracle as O
         g = torch.Generator(device="cpu").manual_seed(1990)
         sig = (1.0 / self.gan.latent_dim) ** 0.5
         zstar = torch.randn(self.B_global, self.gan.latent_dim, generator=g) * sig
         eps = torch.randn(self.B_global, *self.gan.image_dim, generator=g)
         lo = -1.0 if dataset == "celeba" else 0.0
-        chunks = [self.gan.generator_fn(zstar[i:i + 512].to(dev)) for i in range(0, self.B_global, 512)]
-        self.x_full = (torch.cat(chunks) + 0.1 * eps.to(dev)).clamp_(lo, 1.0).contiguous()
+        w_cpu = O.weights_to_torch(self.gan.weights, torch.float32)
+        with torch.no_grad():
+            chunks = [O.generator_forward(dataset, w_cpu, zstar[i:i + 512], use_bn=bool(self.gan.use_bn))
+                      for i in range(0, self.B_global, 512)]
+        self.x_full = (torch.cat(chunks) + 0.1 * eps).clamp_(lo, 1.0).to(dev).contiguous()
         self.z0_full = (torch.randn(self.B_global * R, self.gan.latent_dim, generator=g) * sig).to(dev)
         self.x_host = self.x_full.cpu().pin_memory()
         self.out_host = torch.empty_like(self.x_host).pin_memory()
@@ -326,8 +337,10 @@ class Workload:
         """Device-resident inputs -> full [B_global, H, W, C] result on every rank (all-gather inside)."""
         if self.world > 1:
             from defensegan_b200.parallel import reconstruct_sharded
-            return reconstruct_sharded(self.gan, self.x_full, z_init_val=self.z0_full)
-        return self.gan.reconstruct(self.x_full, z_init_val=self.z0_full)
+            self.last_out = reconstruct_sharded(self.gan, self.x_full, z_init_val=self.z0_full)
+        else:
+            self.last_out = self.gan.reconstruct(self.x_full, z_init_val=self.z0_full)
+        return self.last_out
 
     def e2e_step(self):
         """The call a user makes, host to host: pinned images -> device, projection (+ all-gather), result -> pinned host."""
@@ -394,21 +407,12 @@ def kernel_breakdown(wl, peaks, precision):
         return None, None
     dom = max(kernels, key=lambda k: k["share"])
     # a kernel that runs for tens of milliseconds settles at the power-capped clock: the sustained figure is its peak;
-    # a sub-millisecond kernel timed alone is compared with the burst figure (B200_PROFILING.md)
+    # a sub-millisecond kernel timed alone is compared with the burst figure
     long_running = dom["avg_us"] >= 5000.0
     peak = peaks["bf16_tflops_sustained" if long_running else "bf16_tflops"] if precision == "fp16" else None
-    traffic, tsrc = None, None
-    tp = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    if os.path.exists(tp):
-        with open(tp) as f:
-            tj = json.load(f)
-        ent = tj.get("workloads", {}).get("%s/%d/%s" % (wl.dataset, wl.B * wl.R, precision), {}).get(dom["kernel"])
-        if ent:
-            traffic, tsrc = ent.get("dram_bytes_per_launch"), ent.get("source")
     roofline = {"bound": "tensor", "kernel": dom["kernel"], "achieved": dom["tflops"], "peak": peak, "unit": "TFLOP/s",
-                "frac": (dom["tflops"] / peak) if peak else None, "traffic": traffic,
-                "traffic_unit": "bytes/launch (dram__bytes_read.sum + dram__bytes_write.sum; %s)" % (tsrc or "no ncu capture for this workload"),
-                "peak_source": "%s cuBLAS bf16 %s (MEASURED_PEAKS.json; fp16 and bf16 share the kind::f16 rate)" % (
+                "frac": (dom["tflops"] / peak) if peak else None,
+                "peak_source": "%s bf16 %s (MEASURED_PEAKS.json, else the H100 SXM data sheet; fp16 and bf16 share the tensor-core rate)" % (
                     peaks["_source"], "sustained: the kernel runs for %.1f ms" % (dom["avg_us"] / 1e3) if long_running else "burst"),
                 "operand_format": precision,
                 "flops_per_launch": next(k["flops_per_launch"] for k in prof if k["name"] == dom["kernel"])}
@@ -441,6 +445,17 @@ def pipeline_timeline(wl, roofline):
     return tl
 
 
+def dump_outputs(out_dir, rec):
+    """rec [B, H, W, C] -> out_dir/rec.npy in float32; a batch above DUMP_MAX_BYTES is sampled (fixed seed, sorted rows)."""
+    rec = rec.detach().float().cpu().numpy()
+    row_bytes = rec[0].nbytes
+    if rec.nbytes > DUMP_MAX_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(rec.shape[0], DUMP_MAX_BYTES // row_bytes, replace=False))
+        rec = rec[keep]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "rec.npy"), np.ascontiguousarray(rec, dtype=np.float32))
+
+
 def main():
     with _OnlyJsonOnStdout() as out:
         _main(out)
@@ -462,6 +477,8 @@ def _main(out):
     ap.add_argument("--cpu_sample", type=int, default=64, help="images of the cpu_baseline sample (0 = skip)")
     ap.add_argument("--no_profile", action="store_true")
     ap.add_argument("--no_extra", action="store_true", help="skip the configs[2]/[3]/[4]-share and batch-50 sub-measurements")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the last timed step's reconstructions to DIR/rec.npy (float32)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -485,7 +502,7 @@ def _main(out):
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
 
     dataset, B, R, L = resolve_workload(args, world)
-    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
     wl = Workload(dataset, B, R, L, args.precision, dev, rank, world,
                   weight_seed=FMNIST_WEIGHT_SEED if dataset == "f-mnist" else None)
 
@@ -502,6 +519,8 @@ def _main(out):
     launches_per_step = wl.gan._native.last_launch_count
     enqueues_per_call = wl.gan._native.last_enqueue_count
     value = wl.B_global * args.steps / (ms / 1000.0)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, wl.last_out)
 
     # ---- end-to-end through the public API with HOST buffers (`e2e`) ------------------------------------
     ms_e2e = timed(wl.e2e_step, args.steps, max(1, min(args.warmup, 2)), dev, flush, distributed)

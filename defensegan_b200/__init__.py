@@ -1,4 +1,4 @@
-"""defensegan_b200 - B200-native Defense-GAN projection loop behind the reference's Python surface.
+"""defensegan_b200 - H100-native (sm_90a) Defense-GAN projection loop behind the reference's Python surface.
 
 Public surface (mirrors kabkabm/defensegan):
     defensegan_b200.models.gan.{MnistDefenseGAN, FmnistDefenseDefenseGAN, CelebADefenseGAN}

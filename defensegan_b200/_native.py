@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI in include/defensegan_b200.h.
 
 PyTorch is used only for device memory and streams.  There is no CPU fallback: if the shared
-library is missing or no sm_100 GPU is present, every compute entry point raises.
+library is missing or no sm_90 GPU is present, every compute entry point raises.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ ARCH_IDS = {"mnist": 0, "f-mnist": 0, "fmnist": 0, "celeba": 1}
 PRECISIONS = {"fp32": 0, "fp16": 1}
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 
@@ -50,23 +50,34 @@ class dgan_rec_params(ctypes.Structure):
 ABI_VERSION = 2
 
 
-def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/ for sm_100a with nvcc into the in-tree shared library (cross-compiles
-    without a GPU).  Rebuilds when any source is newer than the library."""
+def _compile(out_path: str, extra_flags: List[str], verbose: bool, force: bool) -> str:
+    """nvcc csrc/dgan_api.cu -> out_path unless out_path is up to date: it exists, no source is newer, and it was built
+    with the same command (recorded in out_path + ".cmd", so a library built with other flags - another GPU
+    architecture, say - is rebuilt)."""
     srcs = [os.path.join(CSRC_DIR, f) for f in sorted(os.listdir(CSRC_DIR))]
     srcs.append(os.path.join(INCLUDE_DIR, "defensegan_b200.h"))
-    if not force and os.path.exists(LIB_PATH):
-        lib_m = os.path.getmtime(LIB_PATH)
-        if all(os.path.getmtime(s) <= lib_m for s in srcs):
-            return LIB_PATH
-    nvcc = os.environ.get("NVCC", "nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + [os.path.join(CSRC_DIR, "dgan_api.cu"), "-o", LIB_PATH]
+    cmd = [os.environ.get("NVCC", "nvcc")] + NVCC_FLAGS + extra_flags + [os.path.join(CSRC_DIR, "dgan_api.cu"), "-o", out_path]
+    stamp = out_path + ".cmd"
+    if not force and os.path.exists(out_path) and os.path.exists(stamp):
+        with open(stamp) as f:
+            same_cmd = f.read() == " ".join(cmd)
+        lib_m = os.path.getmtime(out_path)
+        if same_cmd and all(os.path.getmtime(s) <= lib_m for s in srcs):
+            return out_path
     if verbose:
         print(" ".join(cmd), file=sys.stderr)
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + res.stdout)
-    return LIB_PATH
+    with open(stamp, "w") as f:
+        f.write(" ".join(cmd))
+    return out_path
+
+
+def build_library(force: bool = False, verbose: bool = False) -> str:
+    """Compile csrc/ for sm_90a with nvcc into the in-tree shared library (cross-compiles
+    without a GPU).  Rebuilds when any source is newer than the library or the compile command changed."""
+    return _compile(LIB_PATH, [], verbose, force)
 
 
 PROBE_LIB_PATH = os.path.join(_PKG_DIR, "libdefensegan_b200_probe.so")
@@ -76,14 +87,7 @@ def build_probe_library(force: bool = False) -> str:
     """The same sources with -DDGAN_PROBE: per-CTA clock / %globaltimer counters in the tensor-core kernels and
     dgan_debug_probe_read().  Measurement aid only (tools/probe_step.py, the `timeline` pass of bench.py run it in a
     process of its own through DGAN_LIB); the product library carries none of it."""
-    srcs = [os.path.join(CSRC_DIR, f) for f in sorted(os.listdir(CSRC_DIR))]
-    if not force and os.path.exists(PROBE_LIB_PATH) and all(os.path.getmtime(s) <= os.path.getmtime(PROBE_LIB_PATH) for s in srcs):
-        return PROBE_LIB_PATH
-    cmd = [os.environ.get("NVCC", "nvcc")] + NVCC_FLAGS + ["-DDGAN_PROBE", os.path.join(CSRC_DIR, "dgan_api.cu"), "-o", PROBE_LIB_PATH]
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if res.returncode != 0:
-        raise RuntimeError("nvcc failed:\n" + res.stdout)
-    return PROBE_LIB_PATH
+    return _compile(PROBE_LIB_PATH, ["-DDGAN_PROBE"], False, force)
 
 
 _lib = None
@@ -167,7 +171,7 @@ class NativeGenerator:
     def __init__(self, arch: str, weights: Sequence[torch.Tensor], latent_dim: int = 128, net_dim: int = 64,
                  use_bn: bool = False, precision: str = "fp32", device: Optional[torch.device] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("defensegan_b200 needs a CUDA (sm_100) device; there is no CPU fallback")
+            raise RuntimeError("defensegan_b200 needs a CUDA (sm_90) device; there is no CPU fallback")
         if arch not in ARCH_IDS:
             raise ValueError("unknown arch %r" % (arch,))
         if precision not in PRECISIONS:

@@ -1,4 +1,4 @@
-// Shared declarations for the Defense-GAN projection-loop kernels (sm_100a only).
+// Shared declarations for the Defense-GAN projection-loop kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -9,8 +9,8 @@
 
 #include "../../include/defensegan_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "defensegan_b200 kernels are written for sm_100a only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "defensegan_b200 kernels are written for sm_90a only"
 #endif
 
 namespace dgan {

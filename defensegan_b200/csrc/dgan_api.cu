@@ -1,4 +1,4 @@
-// C-ABI of the B200-native Defense-GAN projection loop (see include/defensegan_b200.h).
+// C-ABI of the H100-native Defense-GAN projection loop (see include/defensegan_b200.h).
 // Host side: generator plan (pixel-graph tables), weight re-layout, workspace carving and the
 // on-device L-step driver.  Everything is enqueued on the caller's stream; nothing here
 // synchronises the host.
@@ -837,7 +837,7 @@ int dgan_create(dgan_handle* out, const dgan_desc* d, const float* const* weight
   int dev_major = 0, dev = 0;
   DGAN_CUDA_CHECK(cudaGetDevice(&dev));
   DGAN_CUDA_CHECK(cudaDeviceGetAttribute(&dev_major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (dev_major != 10) { set_error("defensegan_b200 requires an sm_100 (B200) device"); return DGAN_ERR_UNSUPPORTED; }
+  if (dev_major != 9) { set_error("defensegan_b200 requires an sm_90 (H100) device"); return DGAN_ERR_UNSUPPORTED; }
 
   dgan_ctx* c = new (std::nothrow) dgan_ctx();
   if (c == nullptr) { set_error("out of host memory"); return DGAN_ERR_INVALID_ARG; }
@@ -1092,20 +1092,20 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     // self-test of the validator: damage the plan of Generator.3 fwd in one specific way; the check must then fail
     if (mutate != 0 && dr.name == "Generator.3.fwd" && plan.stream_m.size() > 40) {
       TcRec& m = plan.stream_m[20];
-      TcRec* pp[2] = {&plan.stream_p[0][20], &plan.stream_p[1][20]};
+      TcRec* pp = &plan.stream_p[20];
       switch (mutate) {
         case 1: m.w[2] ^= 1u << 10; break;                                  // first-MMA flag of an op
         case 2: m.w[2] ^= 1u << 7; break;                                   // accumulator of an op
-        case 3: pp[0]->w[4] ^= 0x01; break;                                 // weight tile staged by rank 0 only
-        case 4: pp[0]->w[2] ^= 0x01; pp[1]->w[2] ^= 0x01; break;            // input pixel of an A tile
-        case 5: for (int r = 0; r < 2; ++r) pp[r]->w[0] = (pp[r]->w[0] & ~(0xFu << 8)) | ((((pp[r]->w[0] >> 8) & 0xF) ^ 1u) << 8); break;   // k-chunk
+        case 3: pp->w[4] ^= 0x01; break;                                    // weight tile of a B slot
+        case 4: pp->w[2] ^= 0x01; break;                                    // input pixel of an A tile
+        case 5: pp->w[0] = (pp->w[0] & ~(0xFu << 8)) | ((((pp->w[0] >> 8) & 0xF) ^ 1u) << 8); break;   // k-chunk
         case 6: plan.eitems[0] = -1; break;                                 // epilogue list loses an item
         case 7: for (size_t i = 0; i < plan.stream_m.size(); ++i)           // every dep -> 8: ring hazards
-                  for (int r = 0; r < 2; ++r) plan.stream_p[r][i].w[0] = (plan.stream_p[r][i].w[0] & ~(0xFu << 19)) | (8u << 19);
+                  plan.stream_p[i].w[0] = (plan.stream_p[i].w[0] & ~(0xFu << 19)) | (8u << 19);
                 break;
-        case 8: for (int r = 0; r < 2; ++r) pp[r]->w[0] = (pp[r]->w[0] & ~0xFFu) | 0xBFu; break;   // region past the ring
+        case 8: pp->w[0] = (pp->w[0] & ~0xFFu) | 0xBFu; break;              // region past the ring
         case 9: std::swap(plan.stream_m[20], plan.stream_m[21]);            // two steps out of order
-                for (int r = 0; r < 2; ++r) std::swap(plan.stream_p[r][20], plan.stream_p[r][21]);
+                std::swap(plan.stream_p[20], plan.stream_p[21]);
                 break;
         default: break;
       }
@@ -1144,7 +1144,7 @@ int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf
                             tc2_ring_bytes(dr.N, dr.epi, dr.out_bytes), &plan);
     if (rc) return -1;
     char line[256];
-    const double mb = 2.0 * (double)plan.n_bytes / 1e6;
+    const double mb = (double)plan.n_bytes / 1e6;
     total += mb;
     snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f\n", dr.name.c_str(), dr.N, dr.K,
              plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,

@@ -1,14 +1,13 @@
-// Tensor-core path (DGAN_PREC_FP16): shared pieces of the pixel-graph GEMM on tcgen05.
+// Tensor-core path (DGAN_PREC_FP16): shared pieces of the pixel-graph GEMM on Hopper wgmma.
 //
 //   out[q][n][:] = epi( sum_{(p,t) in pairs(q)} in[p][n][:] x W_t )        fp16 operands, fp32 accumulate
 //
 // Activations are pixel-major [P][N rows][C] fp16, so one input pixel x 128 latent rows x 64 channels is a dense
-// 16 KB box = one TMA box = one 128B-swizzled K-major UMMA operand; weights are stored per tap as [N][K] fp16
+// 16 KB box = one TMA box = one 128B-swizzled K-major wgmma operand; weights are stored per tap as [N][K] fp16
 // tiles.  The conv geometry is data, not code: only in-bounds (input pixel, tap) pairs are listed, so exactly the
 // algorithmic MACs are issued - no zero-insertion, no padding rows, no im2col buffer.
-// This header holds the PTX wrappers, the UMMA descriptors, the epilogue arithmetic (bias / ReLU / mask / last layer +
-// sigmoid|tanh + MSE + dL/dpre) and the weight re-layout; the CTA-pair kernel that uses them and its
-// host-side planning are in kernels_tc2.cuh.
+// This header holds the PTX wrappers, the wgmma descriptors, the weight re-layout and the helpers of the epilogue;
+// the kernel that uses them and its host-side planning are in kernels_tc2.cuh.
 #pragma once
 #include <cuda.h>  // CUtensorMap types only; the encoder is fetched through the runtime (no -lcuda)
 
@@ -30,7 +29,7 @@ struct TcState {
   float grad_scale = 64.f;      // fp16 gradient scaling (undone in the z update)
   void* encode_fn = nullptr;    // cuTensorMapEncodeTiled
   std::vector<void*>* allocs = nullptr;   // the handle's allocation list (lazily built schedules are freed with it)
-  int num_sms = 148;
+  int num_sms = 132;
 };
 
 struct TcLayerSpec {
@@ -73,60 +72,79 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait.
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16 x fp16 -> fp32, M=128, K=16
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T per warpgroup, fp16 x fp16 -> fp32, both operands K-major in shared memory.
+// d: the N/2 accumulator registers of this thread (fragment layout of the m64nNk16 f32 accumulator).
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<48> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<192> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
+template <> struct Wgmma<256> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b), "r"(scale_d));
+  }
+};
 }  // namespace ptx
 
-// K-major, 128B-swizzled operand tile: rows 128 B apart, 8-row groups 1024 B apart (SBO),
-// descriptor version 1 (sm_100), layout type 2 = SWIZZLE_128B.
+// K-major, 128B-swizzled operand tile: rows 128 B apart, 8-row groups 1024 B apart (SBO); wgmma descriptor layout
+// type 1 = SWIZZLE_128B (bits 62-63), leading byte offset unused for swizzled K-major operands (1 by convention).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// kind::f16 instruction descriptor: D = F32 (bits 4-5 = 1), A = B = F16 (0), both K-major,
-// N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
 // fp32 pair -> packed fp16, round-to-nearest, saturating to +-65504: a backward activation that exceeds the fp16 range
@@ -140,7 +158,7 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 // Extra epilogue kinds of the tensor-core path: the generator's last layer (C_out <= 3) is run as
 // a pixel-graph GEMM whose "output pixels" are 4x4 blocks of image pixels (N = 16*C_out columns =
 // the block's pre-activations), so that the output non-linearity, the squared error, its
-// derivative and the per-row loss partial are all lane-local in the epilogue
+// derivative and the per-row loss partial are all computed in the epilogue
 // (models/dataset_models.py:68-69,161-163; models/gan.py:411-414).
 enum TcEpilogue : int { EPI_FINAL_SIGMOID1 = 8, EPI_FINAL_TANH3 = 9 };
 
@@ -152,7 +170,7 @@ struct TcFinalArgs {
   int nbx, w_out;        // blocks per image row, image width
   int write_y;           // store G(z) (only the last iteration / forward-only calls consume it)
   float gscale;          // fp16 gradient scaling applied to dL/dpre
-  // 1-bit ReLU masks of the CTA-pair path: bit j of word [(q*n_pad + n)*(N/64) + g] <=> out[q][n][g*64+j] > 0.
+  // 1-bit ReLU masks of the tensor-core path: bit j of word [(q*n_pad + n)*(N/64) + g] <=> out[q][n][g*64+j] > 0.
   // Written by the forward EPI_BIAS_RELU epilogue, read by the backward EPI_MASK epilogue
   // (tf.nn.relu's gradient passes where the forward output was > 0).
   unsigned long long* mb_out;
@@ -166,112 +184,6 @@ struct TcFinalArgs {
   int m_nparts;          // partial sums per row tile
   size_t m_count;        // elements per partial-sum array (n_pad * latent)
 };
-
-// Target pixels (4x4 block of image n / R) of one row: loaded one accumulator ahead of their use.
-template <int C_OUT>
-__device__ __forceinline__ void tc_final_targets(float4 (&xq)[4 * C_OUT], const TcFinalArgs& fa, int blk, int n) {
-  if (fa.x == nullptr) return;
-  const int by = blk / fa.nbx, bx = blk % fa.nbx;
-  const int hwc = fa.w_out * fa.w_out * C_OUT;
-  const int img = min(n / fa.R, fa.B - 1);
-#pragma unroll
-  for (int li = 0; li < 4; ++li) {
-    const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * C_OUT;
-#pragma unroll
-    for (int e4 = 0; e4 < C_OUT; ++e4) xq[li * C_OUT + e4] = __ldg(reinterpret_cast<const float4*>(fa.x + (size_t)img * hwc + off) + e4);
-  }
-}
-
-template <int C_OUT, int ACT>
-__device__ __forceinline__ void tc_final_epilogue(uint32_t taddr, const TcFinalArgs& fa, const float* __restrict__ bias,
-                                                  int blk, int n, int n_pad, __half* __restrict__ dblk,
-                                                  const float4 (&xq)[4 * C_OUT]) {
-  constexpr int NV = 16 * C_OUT;
-  const int by = blk / fa.nbx, bx = blk % fa.nbx;
-  const int hwc = fa.w_out * fa.w_out * C_OUT;
-  float v[NV];
-#pragma unroll
-  for (int c = 0; c < NV; c += 16) {
-    uint32_t r[16];
-    ptx::tmem_ld16(taddr + c, r);
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[c + j] = __uint_as_float(r[j]);
-  }
-  float bsv[C_OUT];
-#pragma unroll
-  for (int co = 0; co < C_OUT; ++co) bsv[co] = __ldg(bias + co);
-  float lsum = 0.f;
-  uint32_t packed[NV / 2];   // the 16*C_OUT valid fp16 of this row of the block tensor
-#pragma unroll
-  for (int li = 0; li < 4; ++li) {
-    const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * C_OUT;
-    float yv[4 * C_OUT], dv[4 * C_OUT];
-#pragma unroll
-    for (int e = 0; e < 4 * C_OUT; ++e) {
-      const float pre = v[li * 4 * C_OUT + e] + bsv[e % C_OUT];
-      float yy, dact;
-      if (ACT == ACT_SIGMOID) { yy = __fdividef(1.f, 1.f + __expf(-pre)); dact = yy * (1.f - yy); }
-      else { const float t = __expf(-2.f * fabsf(pre)); yy = copysignf(__fdividef(1.f - t, 1.f + t), pre); dact = 1.f - yy * yy; }
-      yv[e] = yy;
-      float d = 0.f;
-      if (fa.x != nullptr) {
-        const float4 xr = xq[li * C_OUT + e / 4];
-        const float xe = (e % 4 == 0) ? xr.x : (e % 4 == 1) ? xr.y : (e % 4 == 2) ? xr.z : xr.w;
-        d = yy - xe;
-        lsum = fmaf(d, d, lsum);
-      }
-      dv[e] = d * dact * fa.gscale;
-    }
-    if (fa.write_y) {
-      float4* yp = reinterpret_cast<float4*>(fa.y + (size_t)n * hwc + off);
-#pragma unroll
-      for (int e4 = 0; e4 < C_OUT; ++e4) yp[e4] = make_float4(yv[e4 * 4], yv[e4 * 4 + 1], yv[e4 * 4 + 2], yv[e4 * 4 + 3]);
-    }
-#pragma unroll
-    for (int e2 = 0; e2 < 2 * C_OUT; ++e2) packed[li * 2 * C_OUT + e2] = pack_half2(dv[2 * e2], dv[2 * e2 + 1]);
-  }
-  if (fa.x != nullptr) {
-    uint4* dp = reinterpret_cast<uint4*>(dblk + ((size_t)blk * n_pad + n) * 64);
-#pragma unroll
-    for (int j4 = 0; j4 < NV / 8; ++j4)   // the K-padding columns [NV, 64) stay zero (cleared once per call)
-      dp[j4] = make_uint4(packed[j4 * 4], packed[j4 * 4 + 1], packed[j4 * 4 + 2], packed[j4 * 4 + 3]);
-    if (fa.write_y) fa.loss_part[(size_t)blk * n_pad + n] = lsum;   // the loss is consumed after the last forward only
-  }
-}
-
-// One 32-column chunk of an accumulator (already in registers) -> epilogue -> out[q][n][c0..c0+32)
-template <int N_TILE, int EPI, typename TOUT>
-__device__ __forceinline__ void tc_store_chunk(const uint32_t (&r)[32], int q, int c0, size_t n, int n_pad,
-                                               TOUT* __restrict__ out, const float* __restrict__ bias, int bias_pstride) {
-  const size_t orow = ((size_t)q * n_pad + n) * N_TILE;
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  if (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS) {
-    const float4* bp = reinterpret_cast<const float4*>(bias + (size_t)q * bias_pstride + c0);
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) {
-      const float4 b = __ldg(bp + j4);
-      v[j4 * 4 + 0] += b.x; v[j4 * 4 + 1] += b.y; v[j4 * 4 + 2] += b.z; v[j4 * 4 + 3] += b.w;
-    }
-    if (EPI == EPI_BIAS_RELU) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-    }
-  }
-  if (sizeof(TOUT) == 2) {
-    uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__half*>(out) + orow + c0);
-#pragma unroll
-    for (int j4 = 0; j4 < 4; ++j4)
-      op[j4] = make_uint4(pack_half2(v[j4 * 8 + 0], v[j4 * 8 + 1]), pack_half2(v[j4 * 8 + 2], v[j4 * 8 + 3]),
-                          pack_half2(v[j4 * 8 + 4], v[j4 * 8 + 5]), pack_half2(v[j4 * 8 + 6], v[j4 * 8 + 7]));
-  } else {
-    float4* op = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + orow + c0);
-#pragma unroll
-    for (int j4 = 0; j4 < 8; ++j4) op[j4] = make_float4(v[j4 * 4], v[j4 * 4 + 1], v[j4 * 4 + 2], v[j4 * 4 + 3]);
-  }
-}
 
 // ------------------------------------------------------------------------------------------
 // host side

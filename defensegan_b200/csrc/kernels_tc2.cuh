@@ -1,21 +1,17 @@
-// Tensor-core path, version 2: CTA-pair (cta_group::2) pixel-graph GEMM.
+// Tensor-core path, version 2: pixel-graph GEMM on Hopper wgmma with a host-planned operand stream.
 //
-// ncu on version 1 (profiles/r1a_*) showed the tcgen05 kernels bound by L2->SM delivery
-// (~7-8 TB/s with the tensor pipe ~29 % busy): every CTA streamed its own copy of every weight
-// tile.  Here two CTAs on the two SMs of a TPC form one MMA of M = 256 latent rows:
-//   * each CTA stages its own 128-row activation tile A and only HALF of each weight tile
-//     (N/2 rows) - the tensor cores read the other half from the peer's shared memory, so
-//     weight traffic per SM is halved;
-//   * one CTA per SM owns all 512 TMEM columns: two buffers of 256 (the MMAs of item i+1 overlap the
-//     epilogue of item i), each holding the 1-8 accumulators of a window of output pixels;
+// The CTAs come in clusters of two: CTA rank r of pair `pair` owns the 128-row latent tile 2*mp + r of every item
+// (window of 1-8 output pixels x row pair mp) that the host assigned to its pair, so both CTAs walk the same step list
+// and need the same weight tiles.  Each CTA loads one half of every weight tile and multicasts it into the shared
+// memory of both, so a pair reads each weight tile from L2 once.
 //   * operands live in a circular shared-memory ring of variable-size steps planned on the host
-//     (tc2_get_schedule): per CTA pair one contiguous stream of step records, LPT-assigned.
-// Roles per CTA: TMA producer warp / MMA issuer warp / 8 epilogue warps; only the even (leader) CTA
-// issues tcgen05.mma.cta_group::2, commits are multicast to both CTAs, TMA completions of both CTAs
-// land on the leader's "full" barrier (peer-bit mask), and the epilogue warps of both CTAs release
-// the accumulators on the leader's "acc_empty" barrier.  The epilogue warps are independent of each other: each
-// converts the 32 rows it can read from TMEM and stores them with its own TMA store; what a unit needs from global
-// memory (output pixel, bias row, mask word) is fetched ahead of time (profiles/r3_epilogue_stalls.md).
+//     (tc2_get_schedule): per CTA pair one contiguous stream of step records, LPT-assigned; a ring region is refilled
+//     only after the consumers of BOTH CTAs released it (the peer's loads write into it too);
+//   * roles per CTA: one TMA producer warp and two consumer warpgroups.  Each consumer warpgroup owns 64 of the
+//     tile's 128 rows and issues wgmma.mma_async (M = 64, K = 16) for every op of a step into register accumulators
+//     - up to 256 columns: the 1-8 accumulators of the item's window - and releases the step's ring region once its
+//     MMAs have completed; after the item's last step it runs the epilogue straight from those registers.  Each
+//     consumer warp stores the 16 rows it holds with its own TMA store (no block-level barrier on the store path).
 #pragma once
 #include "kernels_tc.cuh"
 
@@ -23,19 +19,16 @@ namespace dgan {
 
 constexpr int TC2_SMEM_MAX = 232448;         // 227 KB opt-in limit per CTA
 constexpr int TC2_TILE_BYTES = 128 * 128;    // one 128-row x 64-channel fp16 tile (TMA box, 128B swizzle)
-constexpr int TC2_BUF_COLS = 256;            // TMEM columns per accumulator buffer (2 buffers: MMA i+1 overlaps epilogue i)
-constexpr int TC2_EPI_WARPS = 8;             // two epilogue warps per TMEM lane quarter
-constexpr int TC2_THREADS = 64 + 32 * TC2_EPI_WARPS;
-constexpr int TC2_STORE_ROWS = 32;           // rows per output TMA store: each epilogue warp stores the 32 rows it holds
+constexpr int TC2_BUF_COLS = 256;            // accumulator columns of one item (128 fp32 registers per consumer thread)
+constexpr int TC2_CONSUMERS = 256;           // two consumer warpgroups
+constexpr int TC2_THREADS = TC2_CONSUMERS + 32;   // + the TMA producer warp
+constexpr int TC2_STORE_ROWS = 16;           // rows per output TMA store: each consumer warp stores the 16 rows it holds
 
-// Where each CTA pair's work starts, passed in the kernel's parameter space (constant bank): the first records and the
-// first item's header are then ONE global round trip away from the kernel's entry, and that round trip overlaps the
-// barrier set-up and the TMEM allocation (the prologue of the last CTAs to start sits on the critical path between two
-// kernels of the chain).
+// Where each CTA pair's work starts, passed in the kernel's parameter space (constant bank): the first records are then
+// ONE global round trip away from the kernel's entry, and that round trip overlaps the barrier set-up.
 constexpr int TC2_MAX_PAIRS = 80;
 struct Tc2Heads {
   uint32_t off[TC2_MAX_PAIRS + 1];    // record offsets of the pairs' step streams
-  int first[TC2_MAX_PAIRS];           // first item (window << 16 | row pair) of each pair, -1 = none
 };
 
 struct __align__(16) TcItem2 {
@@ -43,130 +36,97 @@ struct __align__(16) TcItem2 {
   uint32_t n_acc, step_beg, n_steps, pad;
 };
 
-// TMEM columns between the accumulators of one window.  N <= 32 (MNIST last layer: 16 outputs per block) packs
-// 8 accumulators into a 256-column buffer, so a window can span a whole row of blocks.
+// Accumulator columns reserved per accumulator of a window.  N <= 32 (MNIST last layer: 16 outputs per block) packs
+// 8 accumulators into the 256 columns of an item, so a window can span a whole row of blocks.
 __host__ __device__ constexpr int tc2_acc_stride(int n_tile) { return n_tile <= 32 ? 32 : (n_tile < 64 ? 64 : n_tile); }
 
-// Does this instantiation stage its output (and ReLU-mask) tiles through shared memory + TMA?
+// Does this instantiation stage its output tiles through shared memory + TMA?
 __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out_bytes) {
   return out_bytes == 2 && n_tile >= 64 && epi != EPI_FINAL_SIGMOID1 && epi != EPI_FINAL_TANH3;
 }
 
 // One step of a CTA pair's work stream (32 bytes).  The host concatenates, per CTA pair, the steps of all the items
-// assigned to it (LPT order), so producer and MMA warps read one contiguous array: 16 records per coalesced
-// warp load, staged in shared memory, the next batch always in flight - no table-load stalls on the issue path.
+// assigned to it (LPT order), so producer and consumers read one contiguous array.
 //
-// A step stages up to 4 input-pixel (A) tiles and up to 8 weight half-tiles (B slots) for one k-chunk into a
+// A step stages up to 4 input-pixel (A) tiles and up to 8 full weight tiles (B slots) for one k-chunk into a
 // variable-size region of a circular shared-memory ring (offset chosen by the host, which simulates the ring),
 // then issues up to 12 MMAs that combine them.  Several A tiles per step let one weight tile serve several input
 // pixels (stride-2 transposed conv: outputs of equal parity use the same tap with neighbouring inputs), which
-// is what the L2->SM byte count - the limiter of these kernels - cares about.
+// is what the L2->SM byte count cares about.
 //
-// producer record (per cluster rank):
+// producer record (the same for both ranks of a pair):
 //   w[0]: ring offset / 1 KB [0,8) | k-chunk [8,12) | A tiles [12,15) | B slots [15,19) | dep [19,23)
 //         dep = D: the region overlaps that of step k-D (or D = 8, barrier-slot reuse): wait until step k-D is consumed
 //   w[1]: row pair mp [0,16)
 //   w[2..3]: 4 x u16 input pixel of A tile i
-//   w[4..5]: 8 x u8 per B slot: weight tile [0,5) | half (row offset N/2) [5,6)
+//   w[4..5]: 8 x u8 weight tile [0,5) per B slot
 // MMA record:
 //   w[0]: ring offset / 1 KB [0,8) | A tiles [8,11) | ops [11,16) | flags [16,18): 1 = first step of an item, 2 = last
 //   w[2..7]: 12 x u16 per MMA: A tile [0,2) | first B slot [2,5) | slots - 1 [5,7) | accumulator [7,10) | first MMA into it [10,11)
 struct __align__(16) TcRec { uint32_t w[8]; };
 constexpr int TC2_MAX_A = 4, TC2_MAX_BSLOTS = 8, TC2_MAX_OPS = 12, TC2_NSLOT = 8;
-// Merged-N groups: when one input pixel feeds g accumulators that sit side by side in TMEM (acc, acc+1, ...) through
-// weight tiles nobody else in the step uses, the g tiles are staged back to back and ONE MMA of N = g * N_TILE
-// updates all of them.  With cta_group::2 the merged B operand [W_0 | W_1 | ...] is split in halves across the pair:
-// CTA r stages half-tiles x = r*g + j (j < g) of the sequence W_0.lo, W_0.hi, W_1.lo, ... - hence per-rank producer
-// streams.  g = 1 reduces to "each CTA stages its half of the tile".
+// Merged-N groups: when one input pixel feeds g accumulators that sit side by side (acc, acc+1, ...) through weight
+// tiles nobody else in the step uses, the g tiles are staged back to back and ONE MMA of N = g * N_TILE updates all of
+// them.
 constexpr int TC2_REC_BATCH = 16;
-constexpr int TC2_STAGING_BYTES = 2 * TC2_REC_BATCH * (int)sizeof(TcRec);   // producer + MMA warp rings
+constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // producer record ring
 
-// Output staging tiles per CTA: one per epilogue half (two per half - the next tile written while the store of the
-// previous one still reads shared memory - was measured in round 1: no gain).
+// Output staging of the TMA-store epilogues: two 16-row x 128 B buffers per consumer warp (the next unit is written
+// while the store of the previous one still reads shared memory).
 __host__ __device__ constexpr int tc2_epi_tiles(int n_tile, int epi, int out_bytes) {
   return tc2_tma_epilogue(n_tile, epi, out_bytes) ? 2 : 0;
 }
-// The item's bias row staged in shared memory by the TMA-store epilogues: N_TILE floats; a per-pixel bias (the Linear:
-// N_TILE = 256, one accumulator per item) changes from item to item and is double-buffered by item parity.
-// (Sized per instantiation: the operand ring of the N = 64 / 128 layers must stay at 192 KB = 4 steps of 48 KB.)
-__host__ __device__ constexpr int tc2_bias_bytes(int n_tile, int epi, int out_bytes) {
-  return (tc2_tma_epilogue(n_tile, epi, out_bytes) && (epi == EPI_BIAS_RELU || epi == EPI_BIAS)) ? (n_tile == 256 ? 2048 : n_tile * 4) : 0;
-}
 __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
-  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - tc2_bias_bytes(n_tile, epi, out_bytes) - TC2_STAGING_BYTES - epi_b) / 1024) * 1024;
+  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b) / 1024) * 1024;
   return raw > 255 * 1024 ? 255 * 1024 : raw;
 }
 
 template <int N_TILE, int EPI = EPI_NONE, int OUT_BYTES = 2>
 struct Tc2Cfg {
-  static constexpr int HALF_B = (N_TILE / 2) * 128;                      // bytes of this CTA's half weight tile
-  static constexpr int ACC_STRIDE = tc2_acc_stride(N_TILE);
-  static constexpr int MAXB = TC2_BUF_COLS / ACC_STRIDE;                  // = accumulators per window (8 / 4 / 2 / 1)
+  static constexpr int B_TILE = N_TILE * 128;                             // bytes of one staged weight tile
+  static constexpr int MAXB = TC2_BUF_COLS / tc2_acc_stride(N_TILE);      // = accumulators per window (8 / 4 / 2 / 1)
+  static constexpr int MAXG = N_TILE >= 64 ? (256 / N_TILE < 4 ? 256 / N_TILE : 4) : 1;   // tiles of a merged MMA
+  static constexpr int ACC_REGS = MAXB * N_TILE / 2;                      // accumulator registers per consumer thread
   static constexpr bool TMA_EPI = tc2_tma_epilogue(N_TILE, EPI, OUT_BYTES);
-  static constexpr int EPI_TILES = tc2_epi_tiles(N_TILE, EPI, OUT_BYTES);   // output staging tiles (0 or 2)
+  static constexpr int EPI_TILES = tc2_epi_tiles(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_BYTES = EPI_TILES * TC2_TILE_BYTES;
   static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, EPI, OUT_BYTES);          // operand ring (offsets are 8-bit KB)
-  static constexpr int SMEM_BYTES = RING_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256 + tc2_bias_bytes(N_TILE, EPI, OUT_BYTES);
+  static constexpr int SMEM_BYTES = RING_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
 };
 
 namespace ptx {
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Execution barrier of the pair without the GPU-scope fence of a releasing arrive (end of the kernel: nothing another CTA
-// reads depends on it - shared-memory and TMEM lifetimes are ordered by the mbarriers and tcgen05 fences).
-__device__ __forceinline__ void cluster_sync_relaxed() {
-  asm volatile("barrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-}
-// TMA load executed by either CTA of the pair into its OWN shared memory; the transaction bytes
-// are credited to the barrier of the even CTA (peer bit cleared).
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {   // arrives on the barrier at this offset in BOTH CTAs
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
                ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// TMA load into the same shared-memory offset of both CTAs of the pair; each CTA's barrier at `bar` receives the bytes
+// that land in it.
+__device__ __forceinline__ void tma_load_3d_mc2(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"((uint16_t)3) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t local_bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(local_bar), "r"(cta) : "memory");
+}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_local(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
@@ -193,12 +153,6 @@ __device__ __forceinline__ bool elect_one() {
   asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.u32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t local_bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(local_bar), "r"(cta) : "memory");
-}
 }  // namespace ptx
 
 // k-th item (window << 16 | row pair) of CTA pair `pair` from the host-computed table [slot][pair] (-1 = no more work).
@@ -207,11 +161,29 @@ __device__ __forceinline__ int tc2_item_at(const int* __restrict__ order, int k,
   return k < n_slots ? __ldg(order + (size_t)k * n_pairs + pair) : -1;
 }
 
+// One op of a step: the 4 k16 MMAs of a 64-channel k-chunk into accumulators [a, a + g).  The accumulator registers
+// must be named at compile time, so the (a, g) pair of the record selects one of the unrolled instantiations.
+template <int NT, int MAXB, int MAXG, int A = 0, int G = 1, int NREG>
+__device__ __forceinline__ void tc2_mma_op(float (&acc)[NREG], int a, int g, uint64_t da, uint64_t db, uint32_t first) {
+  if constexpr (A < MAXB) {
+    if constexpr (A + G <= MAXB) {
+      if (a == A && g == G) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          ptx::Wgmma<NT * G>::mma(acc + A * (NT / 2), da + 2u * k, db + 2u * k, (k > 0 || !first) ? 1u : 0u);
+        return;
+      }
+    }
+    if constexpr (G < MAXG) tc2_mma_op<NT, MAXB, MAXG, A, G + 1>(acc, a, g, da, db, first);
+    else tc2_mma_op<NT, MAXB, MAXG, A + 1, 1>(acc, a, g, da, db, first);
+  }
+}
+
 #ifdef DGAN_PROBE
 // Developer build only (-DDGAN_PROBE): per kernel instantiation and CTA, summed over launches: cycles from the PDL wait to
-// the end of the CTA's work, launches, cycles from kernel entry to the PDL wait, cycles the MMA warp waited for operands.
-// [4] cycles of the set-up (kernel entry to the PDL trigger), [5] / [6] %globaltimer (ns) at kernel entry / at the end of
-// the CTA's work in the LAST launch, [7] %globaltimer when the CTA's first operands had landed (leaders, last launch).
+// the end of the CTA's work, launches, cycles from kernel entry to the PDL wait, cycles the first consumer warp waited
+// for operands.  [4] cycles of the set-up (kernel entry to the PDL trigger), [5] / [6] %globaltimer (ns) at kernel entry
+// / at the end of the CTA's work in the LAST launch, [7] %globaltimer when the CTA's first operands had landed.
 __device__ unsigned long long g_tc2_probe[48][160][8];
 __device__ __forceinline__ unsigned long long probe_gtime() {
   unsigned long long t;
@@ -227,78 +199,51 @@ template <int N_TILE, int EPI, typename TOUT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC2_THREADS, 1)
 tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const __grid_constant__ CUtensorMap tm_out,
-                  const TcItem2* __restrict__ items, const TcRec* __restrict__ stream_p0, const TcRec* __restrict__ stream_p1,
+                  const TcItem2* __restrict__ items, const TcRec* __restrict__ stream_p,
                   const TcRec* __restrict__ stream_m, const __grid_constant__ Tc2Heads heads,
                   const int* __restrict__ eitems, int n_slots,
                   TOUT* __restrict__ out, int n_pad, const float* __restrict__ bias, int bias_pstride, const TcFinalArgs fa) {
   using Cfg = Tc2Cfg<N_TILE, EPI, (int)sizeof(TOUT)>;
   constexpr bool TMA_EPI = Cfg::TMA_EPI;
-  constexpr int HALF_B = Cfg::HALF_B, ACC_STRIDE = Cfg::ACC_STRIDE;
+  constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3);
+  constexpr bool HAS_BIAS = (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
+  constexpr int B_TILE = Cfg::B_TILE;
+  constexpr int PRODUCER = TC2_CONSUMERS / 32;     // warp index of the TMA producer
   extern __shared__ uint8_t smem_raw[];
 #ifdef DGAN_PROBE
   const long long probe_t_start = clock64();
   const unsigned long long probe_g_start = probe_gtime();
+  long long probe_wait_full = 0;
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t epi_base = smem_base + Cfg::RING_BYTES;            // output staging tiles: EPI_TILES / 2 per epilogue half
-  const uint32_t stg_base = epi_base + Cfg::EPI_BYTES;              // [producer ring][MMA ring] of TcRec
+  const uint32_t epi_base = smem_base + Cfg::RING_BYTES;            // output staging: 4 KB per consumer warp
+  const uint32_t stg_base = epi_base + Cfg::EPI_BYTES;              // producer ring of TcRec
   const uint32_t bar_base = stg_base + TC2_STAGING_BYTES;
-  // full[s] @ +8s (s<8), empty[s] @ +64+8s, acc_full[2] @ +128, acc_empty[2] @ +144, tmem slot @ +160, momentum-tail flag @ +200
-  const uint32_t bar_full = bar_base, bar_empty = bar_base + 64, bar_acc_full = bar_base + 128, bar_acc_empty = bar_base + 144;
-  const uint32_t tmem_slot = bar_base + 160;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - ptx::smem_u32(smem_raw)));
+  // full[s] @ +8s (s<8), empty[s] @ +64+8s, momentum-tail flag @ +200
+  const uint32_t bar_full = bar_base, bar_empty = bar_base + 64;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = ptx::cluster_ctarank();
-  const bool leader = rank == 0;
   const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
+  const uint32_t rbeg = heads.off[pair], rend = heads.off[pair + 1];
 
-  // The schedule tables are constants: each role's first entries are requested before anything else, so that their
+  // The schedule tables are constants: the producer's first records are requested before anything else, so that their
   // latency overlaps the set-up below (and, for CTAs that start early, the previous kernel's tail).
-  uint32_t rbeg = 0, rend = 0;
   uint4 mine = make_uint4(0, 0, 0, 0);
-  int item_first = -1;
-  constexpr bool HAS_BIAS = TMA_EPI && (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
-  const int et = (warp - 2) * 32 + lane;              // 0..255 over the epilogue threads
-  uint32_t q_next = 0, nacc_next = 0;                 // epilogue: output pixel of accumulator `lane` (lanes 0..15), accumulator count
-  float bias_next = 0.f;                              // epilogue: element `et` of the next item's bias row
-  const TcRec* __restrict__ stream = warp == 1 ? stream_m : (rank ? stream_p1 : stream_p0);
-  if (warp <= 1) {
-    rbeg = heads.off[pair]; rend = heads.off[pair + 1];
-    if (2 * rbeg + lane < 2 * rend) mine = __ldg(reinterpret_cast<const uint4*>(stream + rbeg) + lane);   // lane = 16-byte half
-  } else {
-    item_first = heads.first[pair];
-    if (item_first >= 0) {           // header of the first item (see the epilogue): tables and bias are constants too
-      const TcItem2* ip0 = items + (item_first >> 16);
-      if (lane < 16) q_next = (uint32_t)__ldg(&ip0->q[lane]);
-      nacc_next = __ldg(&ip0->n_acc);
-      if (HAS_BIAS && bias_pstride == 0 && et < N_TILE) bias_next = __ldg(bias + et);
+  if (warp == PRODUCER) {
+    if (2 * rbeg + lane < 2 * rend) mine = __ldg(reinterpret_cast<const uint4*>(stream_p + rbeg) + lane);   // lane = 16-byte half
+    if (lane == 0) {
+      ptx::prefetch_tmap(&tm_a);
+      ptx::prefetch_tmap(&tm_b);
+      if (TMA_EPI) ptx::prefetch_tmap(&tm_out);
+      for (int s = 0; s < TC2_NSLOT; ++s) {
+        ptx::mbar_init(bar_full + 8 * s, 1);                   // producer's arrive.expect_tx
+        ptx::mbar_init(bar_empty + 8 * s, 2 * TC2_CONSUMERS / 32);   // one arrive per consumer warp of both CTAs
+      }
+      ptx::fence_barrier_init();
     }
   }
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tm_a);
-    ptx::prefetch_tmap(&tm_b);
-    for (int s = 0; s < TC2_NSLOT; ++s) {
-      ptx::mbar_init(bar_full + 8 * s, 1);    // leader's producer arrive.expect_tx (bytes of both CTAs)
-      ptx::mbar_init(bar_empty + 8 * s, 1);   // one multicast commit per CTA
-    }
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(bar_acc_full + 8 * b, 1);
-      ptx::mbar_init(bar_acc_empty + 8 * b, 2 * TC2_EPI_WARPS);   // epilogue warps of both CTAs (used on the leader only)
-    }
-    if (TMA_EPI) ptx::prefetch_tmap(&tm_out);
-    ptx::fence_barrier_init();
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc_2sm(tmem_slot, 512);
-    ptx::tmem_relinquish_2sm();
-  }
-  ptx::tc_fence_before();
-  ptx::cluster_sync_all();                     // barriers of BOTH CTAs initialised before any remote signal
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  if (HAS_BIAS && warp >= 2 && bias_pstride != 0 && item_first >= 0 && et < N_TILE)   // per-pixel bias: row of the first item's pixel
-    bias_next = __ldg(bias + (size_t)__shfl_sync(0xffffffffu, q_next, 0) * bias_pstride + et);
+  ptx::cluster_sync();                         // barriers of BOTH CTAs initialised before any remote signal
   // everything above overlapped the previous kernel's tail (PDL); from here on we read what it wrote
 #ifdef DGAN_PROBE
   const long long probe_t_entry = clock64();
@@ -307,14 +252,13 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   pdl_wait();
 #ifdef DGAN_PROBE
   const long long probe_t_go = clock64();
-  long long probe_wait_full = 0;
 #endif
 
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    // The whole warp walks the step list convergently; every table value is loaded from a
-    // warp-uniform address so the TMA operands live in uniform registers (no per-instruction
-    // R2UR/ELECT loop), and one elected lane issues.
+  if (warp == PRODUCER) {
+    // ===================== TMA producer =====================
+    // The whole warp walks the step list convergently; every table value is loaded from a warp-uniform address, and
+    // one elected lane issues.
+    const TcRec* __restrict__ stream = stream_p;
     uint32_t it = 0;
     const uint32_t ring = stg_base;
     for (uint32_t base = rbeg; base < rend; base += TC2_REC_BATCH) {
@@ -331,24 +275,24 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         const int row0 = (2 * (int)(r0.y & 0xFFFFu) + (int)rank) * kRowTile;
         if (it >= dep) ptx::mbar_wait(bar_empty + 8 * ((it - dep) & (TC2_NSLOT - 1)), ((it - dep) >> 3) & 1);   // step it-dep consumed
         // implied by the wait above (steps are consumed in order); observing every phase of this slot exactly once
-        // before it is re-armed keeps the barrier protocol checkable (compute-sanitizer synccheck)
+        // before it is re-armed keeps the barrier protocol simple to check
         if (dep != TC2_NSLOT && it >= TC2_NSLOT) ptx::mbar_wait(bar_empty + 8 * slot, ((it - TC2_NSLOT) >> 3) & 1);
         const uint32_t full = bar_full + 8 * slot;
         const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
         if (ptx::elect_one()) {
-          if (leader) ptx::mbar_expect_tx(full, 2u * (uint32_t)(nA * TC_A_BYTES + nB * HALF_B));
+          ptx::mbar_expect_tx(full, (uint32_t)(nA * TC_A_BYTES + nB * B_TILE));
 #pragma unroll
           for (int a = 0; a < TC2_MAX_A; ++a) {
             if (a >= nA) break;
             const int p = (int)((((a < 2) ? r0.z : r0.w) >> (16 * (a & 1))) & 0xFFFFu);
-            ptx::tma_load_3d_2sm(sa + a * TC_A_BYTES, &tm_a, full, kc * 64, row0, p);
+            ptx::tma_load_3d(sa + a * TC_A_BYTES, &tm_a, full, kc * 64, row0, p);
           }
           const uint32_t sb = sa + nA * TC_A_BYTES;
 #pragma unroll
-          for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {
+          for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {     // this CTA's half of each weight tile, into both CTAs
             if (b >= nB) break;
             const uint32_t e = ((b < 4) ? r1.x : r1.y) >> (8 * (b & 3));
-            ptx::tma_load_3d_2sm(sb + b * HALF_B, &tm_b, full, kc * 64, (int)((e >> 5) & 1u) * (N_TILE / 2), (int)(e & 0x1Fu));
+            ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
           }
         }
         __syncwarp();
@@ -357,248 +301,214 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     }
     // drain: the last steps' "consumed" signals are otherwise never observed (nobody leaves while MMAs still read smem)
     for (uint32_t j = it > TC2_NSLOT ? it - TC2_NSLOT : 0; j < it; ++j) ptx::mbar_wait(bar_empty + 8 * (j & (TC2_NSLOT - 1)), (j >> 3) & 1);
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader) {
-      constexpr uint32_t idesc = make_idesc_f16(256, N_TILE);
-      uint32_t it = 0, item_count = 0;
-      const uint32_t ring = stg_base + TC2_REC_BATCH * (uint32_t)sizeof(TcRec);
-      const uint64_t desc0 = make_smem_desc_sw128(smem_base);
-      const uint32_t desc_lo0 = (uint32_t)desc0, desc_hi = (uint32_t)(desc0 >> 32);
-      uint32_t buf = 0;
-      for (uint32_t base = rbeg; base < rend; base += TC2_REC_BATCH) {
-        ptx::st_shared_v4(ring + lane * 16u, mine.x, mine.y, mine.z, mine.w);
-        __syncwarp();
-        if (2 * (base + TC2_REC_BATCH) + lane < 2 * rend) mine = __ldg(reinterpret_cast<const uint4*>(stream + base + TC2_REC_BATCH) + lane);
-        const uint32_t cnt = min((uint32_t)TC2_REC_BATCH, rend - base);
-        for (uint32_t i = 0; i < cnt; ++i, ++it) {
-          const uint4 r0 = ptx::ld_shared_v4(ring + i * 32u);
-          const uint4 r1 = ptx::ld_shared_v4(ring + i * 32u + 16u);
-          const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
-          const int nA = (r0.x >> 8) & 0x7, n_ops = (r0.x >> 11) & 0x1F;
-          const uint32_t flags = (r0.x >> 16) & 0x3u;
-          if (flags & 1u) {                                   // first step of an item: its accumulator buffer must be drained
-            buf = item_count & 1;
-            ptx::mbar_wait(bar_acc_empty + 8 * buf, ((item_count >> 1) & 1) ^ 1);
-          }
-#ifdef DGAN_PROBE
-          const long long probe_w0 = clock64();
-#endif
-          ptx::mbar_wait(bar_full + 8 * slot, phase);
-#ifdef DGAN_PROBE
-          probe_wait_full += clock64() - probe_w0;
-          if (it == 0 && lane == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
-#endif
-          ptx::tc_fence_after();
-          // descriptors differ only in the 14-bit start-address field: one 32-bit add each (smem < 256 KB, no carry)
-          const uint32_t a_lo0 = desc_lo0 + ((r0.x & 0xFFu) << 6);
-          const uint32_t b_lo0 = a_lo0 + (uint32_t)nA * (uint32_t)(TC_A_BYTES >> 4);
-          if (ptx::elect_one()) {
-            const uint32_t d0 = tmem_base + buf * TC2_BUF_COLS;
-            const uint32_t opw[6] = {r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-            for (int oi = 0; oi < TC2_MAX_OPS; ++oi) {
-              if (oi >= n_ops) break;
-              const uint32_t e = opw[oi >> 1] >> (16 * (oi & 1));
-              const uint32_t first = (e >> 10) & 1u;
-              const uint32_t a_lo = a_lo0 + (e & 3u) * (uint32_t)(TC_A_BYTES >> 4);
-              const uint32_t b_lo = b_lo0 + ((e >> 2) & 7u) * (uint32_t)(HALF_B >> 4);
-              const uint32_t d = d0 + ((e >> 7) & 7u) * ACC_STRIDE;
-              const uint32_t idg = idesc + ((e >> 5) & 3u) * ((uint32_t)(N_TILE >> 3) << 17);   // N = slots * N_TILE
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                ptx::umma_f16_2sm(d, ((uint64_t)desc_hi << 32) | (a_lo + 2u * k), ((uint64_t)desc_hi << 32) | (b_lo + 2u * k), idg,
-                                  (k > 0 || !first) ? 1u : 0u);
-            }
-            ptx::umma_commit_2sm(bar_empty + 8 * slot);           // this step is consumed (both CTAs)
-            if (flags & 2u) ptx::umma_commit_2sm(bar_acc_full + 8 * buf);   // last step: accumulators complete in both CTAs
-          }
-          __syncwarp();
-          if (flags & 2u) ++item_count;
-        }
-        __syncwarp();
-      }
-      // drain: observe the release of the last (up to two) accumulator buffers by the epilogue warps of both CTAs
-      for (uint32_t j = item_count > 2 ? item_count - 2 : 0; j < item_count; ++j) ptx::mbar_wait(bar_acc_empty + 8 * (j & 1), (j >> 1) & 1);
-    }
   } else {
-    // ===================== epilogue (warps 2..9, both CTAs) =====================
-    // Two warps per TMEM lane quarter split the (accumulator, 32-column chunk) units of an item;
-    // the TMEM load of a warp's next unit is in flight while it converts and stores the current one.
-    // Nothing on the per-unit path depends on a global load issued in the same unit (ncu source counters of the
-    // round-2 build: a third of the epilogue's time went to the chain item header -> output pixel -> bias / mask word):
-    // the window's output pixels live in lanes 0..15 (one shuffle per use), fetched one item ahead; the item's bias row
-    // is staged in shared memory before the accumulators are awaited; mask words are fetched two units ahead.
-    const int lq = warp & 3;                          // TMEM lanes this warp may access
-    const int half = (warp - 2) >> 2;                 // 0 | 1: which of the two warps of this quarter
-    const int row = lq * 32 + lane;
-    const uint32_t bias_s = bar_base + 256;           // [2][256] floats
-    uint32_t item_count = 0;
-    for (int kk = 0, item_e = item_first, item_next; item_e >= 0; ++kk, ++item_count, item_e = item_next) {
-      item_next = tc2_item_at(eitems, kk + 1, pair, n_pairs, n_slots);      // (window << 16 | row pair), one item ahead
+    // ===================== consumer warpgroups (warps 0..7) =====================
+    const int wg = warp >> 2, wl = warp & 3;
+    const int r_lo = wg * 64 + wl * 16 + (lane >> 2);      // this thread's rows of the 128-row tile: r_lo and r_lo + 8
+    float acc[Cfg::ACC_REGS];
+#pragma unroll
+    for (int i = 0; i < Cfg::ACC_REGS; ++i) acc[i] = 0.f;
+    uint32_t item_count = 0, store_count = 0;
+    int item_e = -1;
+    uint32_t it = 0;
+    for (uint32_t ri = rbeg; ri < rend; ++ri, ++it) {
+      const uint4* rp = reinterpret_cast<const uint4*>(stream_m + ri);
+      const uint4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
+      const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
+      const int nA = (r0.x >> 8) & 0x7, n_ops = (r0.x >> 11) & 0x1F;
+      const uint32_t flags = (r0.x >> 16) & 0x3u;
+      if (flags & 1u) item_e = tc2_item_at(eitems, (int)item_count, pair, n_pairs, n_slots);
+#ifdef DGAN_PROBE
+      const long long probe_w0 = clock64();
+#endif
+      ptx::mbar_wait(bar_full + 8 * slot, phase);
+#ifdef DGAN_PROBE
+      probe_wait_full += clock64() - probe_w0;
+      if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
+#endif
+      const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
+      const uint64_t da0 = make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u);   // this warpgroup's 64 rows of the A tiles
+      const uint64_t db0 = make_smem_desc_sw128(sa + (uint32_t)nA * TC_A_BYTES);
+      uint32_t w0 = r0.z, w1 = r0.w, w2 = r1.x, w3 = r1.y, w4 = r1.z, w5 = r1.w;
+      ptx::fence_operands(acc);
+      ptx::wgmma_fence();
+      for (int oi = 0; oi < n_ops; ++oi) {
+        const uint32_t e = (oi & 1) ? (w0 >> 16) : (w0 & 0xFFFFu);
+        if (oi & 1) { w0 = w1; w1 = w2; w2 = w3; w3 = w4; w4 = w5; }
+        // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
+        const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(TC_A_BYTES >> 4));
+        const uint64_t db = db0 + (uint64_t)(((e >> 2) & 7u) * (uint32_t)(B_TILE >> 4));
+        tc2_mma_op<N_TILE, Cfg::MAXB, Cfg::MAXG>(acc, (int)((e >> 7) & 7u), (int)((e >> 5) & 3u) + 1, da, db, (e >> 10) & 1u);
+      }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait0();
+      ptx::fence_operands(acc);
+      __syncwarp();
+      if (lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * slot, (uint32_t)lane);   // this warp's MMAs no longer read the region
+      if (!(flags & 2u)) continue;
+
+      // ---- epilogue of the item: accumulator registers -> (bias | ReLU | mask | last layer) -> global memory.
+      //      Register i of accumulator a holds column (i % (N_TILE/2)) / 4 * 8 + (lane % 4) * 2 + (i % 2) of row
+      //      r_lo + 8 * ((i / 2) % 2) (the m64nNk16 accumulator fragment).
+      const TcItem2* ip = items + (item_e >> 16);
       const int mp = item_e & 0xFFFF;
-      const uint32_t q_mine = q_next;
-      const int n_acc = (int)nacc_next;
+      const int n_acc = (int)__ldg(&ip->n_acc);
+      const uint32_t q_mine = lane < 16 ? (uint32_t)__ldg(&ip->q[lane]) : 0u;
       auto q_of = [&](int a) { return (int)__shfl_sync(0xffffffffu, q_mine, a); };
-      if (HAS_BIAS && (item_count == 0 || bias_pstride != 0)) {
-        // a per-pixel bias (Linear) comes with one accumulator per item (N_TILE = 256): the row of q[0] serves the item
-        if (et < N_TILE) ptx::st_shared_u32(bias_s + (item_count & 1u) * 1024u + (uint32_t)et * 4u, __float_as_uint(bias_next));
-        ptx::named_bar_sync(4, 32 * TC2_EPI_WARPS);   // also: every warp is done with the row of item_count - 2
-      }
-      if (item_next >= 0) {                            // next item's header, in flight during this item
-        const TcItem2* ipn = items + (item_next >> 16);
-        if (lane < 16) q_next = (uint32_t)__ldg(&ipn->q[lane]);
-        nacc_next = __ldg(&ipn->n_acc);
-        if (HAS_BIAS && bias_pstride != 0 && et < N_TILE)
-          bias_next = __ldg(bias + (size_t)__shfl_sync(0xffffffffu, q_next, 0) * bias_pstride + et);
-      }
-      const size_t n = (size_t)(2 * mp + (int)rank) * kRowTile + row;
-      const uint32_t buf = item_count & 1;
-      const uint32_t tbuf = tmem_base + ((uint32_t)(lq * 32) << 16) + buf * TC2_BUF_COLS;
-      constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3);
-      float4 xq_next[FINAL ? (EPI == EPI_FINAL_SIGMOID1 ? 4 : 12) : 1];
-      if (FINAL && half < n_acc)     // first block's target pixels: in flight while the MMAs finish
-        tc_final_targets<(EPI == EPI_FINAL_SIGMOID1 ? 1 : 3)>(reinterpret_cast<float4(&)[EPI == EPI_FINAL_SIGMOID1 ? 4 : 12]>(xq_next), fa, q_of(half < n_acc ? half : 0), (int)n);
-      // EPI_MASK: mask words are fetched two units ahead; the first two are in flight while the MMAs finish
-      unsigned long long mbits = ~0ull, mbits_next = ~0ull, mbits_next2 = ~0ull;
-      if (TMA_EPI && EPI == EPI_MASK) {
-        constexpr int G0 = N_TILE >= 64 ? N_TILE / 64 : 1;
-        const int nu = n_acc * G0, u1 = half + 2;
-        const int q0 = q_of(half < nu ? half / G0 : 0), q1 = q_of(u1 < nu ? u1 / G0 : 0);
-        if (half < nu) mbits_next = __ldg(fa.mb_in + ((size_t)q0 * n_pad + n) * G0 + half % G0);
-        if (u1 < nu) mbits_next2 = __ldg(fa.mb_in + ((size_t)q1 * n_pad + n) * G0 + u1 % G0);
-      }
-      ptx::mbar_wait(bar_acc_full + 8 * buf, (item_count >> 1) & 1);
-      ptx::tc_fence_after();
-      if (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3) {
+      const int tile_row0 = (2 * mp + (int)rank) * kRowTile;
+      const size_t n_lo = (size_t)(tile_row0 + r_lo);
+      if constexpr (FINAL) {
         constexpr int CO = (EPI == EPI_FINAL_SIGMOID1) ? 1 : 3;
-        float4 xq[4 * CO];
-        for (int a = half; a < n_acc; a += 2) {
+        const int hwc = fa.w_out * fa.w_out * CO;
+        float bsv[CO];
 #pragma unroll
-          for (int j = 0; j < 4 * CO; ++j) xq[j] = xq_next[j];
-          const int qa = q_of(a), qa2 = q_of(a + 2 < n_acc ? a + 2 : a);
-          if (a + 2 < n_acc) tc_final_targets<CO>(reinterpret_cast<float4(&)[4 * CO]>(xq_next), fa, qa2, (int)n);   // next block's targets in flight
-          const uint32_t taddr = tbuf + (uint32_t)(a * ACC_STRIDE);
-          if (EPI == EPI_FINAL_SIGMOID1)
-            tc_final_epilogue<1, ACT_SIGMOID>(taddr, fa, bias, qa, (int)n, n_pad, reinterpret_cast<__half*>(out),
-                                              reinterpret_cast<const float4(&)[4]>(xq));
-          else
-            tc_final_epilogue<3, ACT_TANH>(taddr, fa, bias, qa, (int)n, n_pad, reinterpret_cast<__half*>(out),
-                                           reinterpret_cast<const float4(&)[12]>(xq));
-        }
-      } else if (TMA_EPI) {
-        // ---- 64-column units through shared memory: TMEM -> regs -> (bias|ReLU|mask) -> fp16 -> this warp's 32-row
-        //      slice of a 128B-swizzled tile -> one TMA store of 32 rows x 64 channels per warp.  The warps of a half
-        //      share nothing: no block-level barrier on the unit path, each warp waits for its own previous store.
-        constexpr int G = N_TILE >= 64 ? N_TILE / 64 : 1;   // 64-column groups per accumulator
-        const int n_units = n_acc * G;
-        const int row0 = (2 * mp + (int)rank) * kRowTile + lq * 32;
-        const uint32_t swz = (uint32_t)(lane & 7);
-        const uint32_t s_out = epi_base + (uint32_t)half * TC2_TILE_BYTES + (uint32_t)lq * 4096u;
-        const uint32_t bias_row = bias_s + ((bias_pstride != 0) ? (item_count & 1u) * 1024u : 0u);
-        uint32_t r0[32], r1[32];
-        if (half < n_units) {
-          const int a = half / G, g = half % G;
-          ptx::tmem_ld32(tbuf + (uint32_t)(a * ACC_STRIDE + g * 64), r0);
-          ptx::tmem_ld32(tbuf + (uint32_t)(a * ACC_STRIDE + g * 64 + 32), r1);
-        }
-        for (int u = half; u < n_units; u += 2) {
-          const int a = u / G, g = u % G, q = q_of(a);
-          mbits = mbits_next; mbits_next = mbits_next2;
-          ptx::tmem_ld_wait();
-          uint32_t pk[32];
-          unsigned long long bits = 0ull;
-          {
-            float v[64];
+        for (int co = 0; co < CO; ++co) bsv[co] = __ldg(bias + co);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) { v[j] = __uint_as_float(r0[j]); v[32 + j] = __uint_as_float(r1[j]); }
-            if (HAS_BIAS) {
+        for (int a = 0; a < Cfg::MAXB; ++a) {
+          if (a >= n_acc) break;
+          const int blk = q_of(a);
+          const int by = blk / fa.nbx, bx = blk % fa.nbx;
 #pragma unroll
-              for (int j4 = 0; j4 < 16; ++j4) {
-                const uint4 b = ptx::ld_shared_v4(bias_row + (uint32_t)(g * 256 + j4 * 16));
-                v[j4 * 4 + 0] += __uint_as_float(b.x); v[j4 * 4 + 1] += __uint_as_float(b.y);
-                v[j4 * 4 + 2] += __uint_as_float(b.z); v[j4 * 4 + 3] += __uint_as_float(b.w);
+          for (int h = 0; h < 2; ++h) {
+            const size_t n = n_lo + 8 * h;
+            const int img = min((int)(n / fa.R), fa.B - 1);
+            float lsum = 0.f;
+#pragma unroll
+            for (int j = 0; j < N_TILE / 8; ++j) {
+              const int col = j * 8 + (lane & 3) * 2;     // (li * 4 + lj) * CO + co of the 4x4 block
+              const int li = col / (4 * CO), e = col % (4 * CO);
+              const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * CO + e;
+              float2 xv = make_float2(0.f, 0.f);
+              if (fa.x != nullptr) xv = __ldg(reinterpret_cast<const float2*>(fa.x + (size_t)img * hwc + off));
+              float yv[2], dv[2];
+#pragma unroll
+              for (int c = 0; c < 2; ++c) {
+                const float pre = acc[a * (N_TILE / 2) + j * 4 + h * 2 + c] + bsv[(e + c) % CO];
+                float yy, dact;
+                if (EPI == EPI_FINAL_SIGMOID1) { yy = __fdividef(1.f, 1.f + __expf(-pre)); dact = yy * (1.f - yy); }
+                else { const float t = __expf(-2.f * fabsf(pre)); yy = copysignf(__fdividef(1.f - t, 1.f + t), pre); dact = 1.f - yy * yy; }
+                yv[c] = yy;
+                float d = 0.f;
+                if (fa.x != nullptr) { d = yy - (c ? xv.y : xv.x); lsum = fmaf(d, d, lsum); }
+                dv[c] = d * dact * fa.gscale;
               }
-              if (EPI == EPI_BIAS_RELU) {
-#pragma unroll
-                for (int j = 0; j < 64; ++j) v[j] = fmaxf(v[j], 0.f);
-              }
+              if (fa.write_y) *reinterpret_cast<float2*>(fa.y + n * hwc + off) = make_float2(yv[0], yv[1]);
+              // the K-padding columns [16*CO, 64) of the block tensor stay zero (cleared once per call)
+              if (fa.x != nullptr)
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(out) + ((size_t)blk * n_pad + n) * 64 + col) = pack_half2(dv[0], dv[1]);
             }
-            if (EPI == EPI_BIAS_RELU && fa.mb_out != nullptr) {
+            lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
+            lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
+            // the loss is consumed after the last forward only
+            if (fa.x != nullptr && fa.write_y && (lane & 3) == 0) fa.loss_part[(size_t)blk * n_pad + n] = lsum;
+          }
+        }
+      } else if constexpr (TMA_EPI) {
+        // 64-column units: registers -> fp16 -> this warp's 16-row slice of a 128B-swizzled tile -> one TMA store
+        constexpr int G = N_TILE / 64;                 // 64-column groups per accumulator
+        const int row_w = tile_row0 + wg * 64 + wl * 16;
+        const uint32_t s_warp = epi_base + (uint32_t)warp * 4096u;
+        const uint32_t swz = (uint32_t)(lane >> 2);
 #pragma unroll
-              for (int j = 0; j < 64; ++j) bits |= (unsigned long long)(v[j] > 0.f) << j;
-            }
+        for (int a = 0; a < Cfg::MAXB; ++a) {
+          if (a >= n_acc) break;
+          const int q = q_of(a);
+#pragma unroll
+          for (int g = 0; g < G; ++g) {
+            unsigned long long mk[2] = {~0ull, ~0ull}, bits[2] = {0ull, 0ull};
             if (EPI == EPI_MASK) {
 #pragma unroll
-              for (int j = 0; j < 64; ++j)
-                if (!((mbits >> j) & 1ull)) v[j] = 0.f;
+              for (int h = 0; h < 2; ++h) mk[h] = __ldg(fa.mb_in + ((size_t)q * n_pad + n_lo + 8 * h) * G + g);
             }
+            uint32_t pk[2][8];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) pk[j] = pack_half2(v[2 * j], v[2 * j + 1]);
-          }
-          if (u + 2 < n_units) {                           // next unit's accumulator columns: in flight during the store phase
-            const int a2 = (u + 2) / G, g2 = (u + 2) % G;
-            ptx::tmem_ld32(tbuf + (uint32_t)(a2 * ACC_STRIDE + g2 * 64), r0);
-            ptx::tmem_ld32(tbuf + (uint32_t)(a2 * ACC_STRIDE + g2 * 64 + 32), r1);
-          }
-          if (lane == 0) ptx::bulk_wait_read0();           // this warp's previous store has read its slice
-          __syncwarp();
+            for (int j = 0; j < 8; ++j) {
+              const int cl = j * 8 + (lane & 3) * 2;   // column within the 64-column group
+              float2 bv = make_float2(0.f, 0.f);
+              if (HAS_BIAS) bv = __ldg(reinterpret_cast<const float2*>(bias + (size_t)q * bias_pstride + g * 64 + cl));
 #pragma unroll
-          for (int c = 0; c < 8; ++c)
-            ptx::st_shared_v4(s_out + (uint32_t)lane * 128u + (((uint32_t)c ^ swz) << 4), pk[c * 4], pk[c * 4 + 1], pk[c * 4 + 2], pk[c * 4 + 3]);
-          ptx::fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            ptx::tma_store_3d(&tm_out, s_out, g * 64, row0, q);
-            ptx::bulk_commit();
-          }
-          // global traffic of this unit after the proxy fence (which waits for the thread's outstanding accesses)
-          if (EPI == EPI_BIAS_RELU && fa.mb_out != nullptr) fa.mb_out[((size_t)q * n_pad + n) * G + g] = bits;
-          if (EPI == EPI_MASK && u + 4 < n_units) {
-            const int a4 = (u + 4) / G, g4 = (u + 4) % G;
-            mbits_next2 = __ldg(fa.mb_in + ((size_t)q_of(a4) * n_pad + n) * G + g4);
+              for (int h = 0; h < 2; ++h) {
+                float v0 = acc[a * (N_TILE / 2) + (g * 8 + j) * 4 + h * 2];
+                float v1 = acc[a * (N_TILE / 2) + (g * 8 + j) * 4 + h * 2 + 1];
+                if (HAS_BIAS) { v0 += bv.x; v1 += bv.y; }
+                if (EPI == EPI_BIAS_RELU) {
+                  v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                  bits[h] |= ((unsigned long long)(v0 > 0.f) << cl) | ((unsigned long long)(v1 > 0.f) << (cl + 1));
+                }
+                if (EPI == EPI_MASK) {
+                  if (!((mk[h] >> cl) & 1ull)) v0 = 0.f;
+                  if (!((mk[h] >> (cl + 1)) & 1ull)) v1 = 0.f;
+                }
+                pk[h][j] = pack_half2(v0, v1);
+              }
+            }
+            const uint32_t buf = s_warp + (store_count & 1u) * 2048u;
+            if (lane == 0) ptx::bulk_wait_read1();     // the store that used this buffer two units ago has read it
+            __syncwarp();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int j = 0; j < 8; ++j)
+                ptx::st_shared_u32(buf + (swz + 8u * h) * 128u + (((uint32_t)j ^ swz) << 4) + (uint32_t)(lane & 3) * 4u, pk[h][j]);
+            ptx::fence_proxy_async_smem();
+            __syncwarp();
+            if (lane == 0) {
+              ptx::tma_store_3d(&tm_out, buf, g * 64, row_w, q);
+              ptx::bulk_commit();
+            }
+            ++store_count;
+            if (EPI == EPI_BIAS_RELU && fa.mb_out != nullptr) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
+                bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
+              }
+              if ((lane & 3) < 2) fa.mb_out[((size_t)q * n_pad + n_lo + 8 * (lane & 1)) * G + g] = (lane & 1) ? bits[1] : bits[0];
+            }
           }
         }
       } else {
-        constexpr int CH = N_TILE >= 32 ? N_TILE / 32 : 1;     // 32-column chunks per accumulator
-        const int n_units = n_acc * CH;
-        uint32_t rA[32], rB[32];
-        int u = half;
-        if (u < n_units) ptx::tmem_ld32(tbuf + (uint32_t)((u / CH) * ACC_STRIDE + (u % CH) * 32), rA);
-        for (; u < n_units; u += 4) {
-          ptx::tmem_ld_wait();
-          if (u + 2 < n_units) ptx::tmem_ld32(tbuf + (uint32_t)(((u + 2) / CH) * ACC_STRIDE + ((u + 2) % CH) * 32), rB);
-          tc_store_chunk<N_TILE, EPI, TOUT>(rA, q_of(u / CH), (u % CH) * 32, n, n_pad, out, bias, bias_pstride);
-          if (u + 2 < n_units) {
-            ptx::tmem_ld_wait();
-            if (u + 4 < n_units) ptx::tmem_ld32(tbuf + (uint32_t)(((u + 4) / CH) * ACC_STRIDE + ((u + 4) % CH) * 32), rA);
-            tc_store_chunk<N_TILE, EPI, TOUT>(rB, q_of((u + 2) / CH), ((u + 2) % CH) * 32, n, n_pad, out, bias, bias_pstride);
+        // fp32 outputs (BatchNorm pre-activations, the Linear backward's partial sums): straight from the registers
+#pragma unroll
+        for (int a = 0; a < Cfg::MAXB; ++a) {
+          if (a >= n_acc) break;
+          const int q = q_of(a);
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            const int col = j * 8 + (lane & 3) * 2;
+            float2 bv = make_float2(0.f, 0.f);
+            if (HAS_BIAS) bv = __ldg(reinterpret_cast<const float2*>(bias + (size_t)q * bias_pstride + col));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = acc[a * (N_TILE / 2) + j * 4 + h * 2] + bv.x, v1 = acc[a * (N_TILE / 2) + j * 4 + h * 2 + 1] + bv.y;
+              if (EPI == EPI_BIAS_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+              const size_t o = ((size_t)q * n_pad + n_lo + 8 * h) * N_TILE + col;
+              if (sizeof(TOUT) == 4) *reinterpret_cast<float2*>(reinterpret_cast<float*>(out) + o) = make_float2(v0, v1);
+              else *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(out) + o) = pack_half2(v0, v1);
+            }
           }
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive_remote(bar_acc_empty + 8 * buf, 0);
       if (EPI == EPI_NONE && sizeof(TOUT) == 4 && fa.m_counter != nullptr) {
-        // ---- momentum in the tail of the split-K Linear backward.  Every epilogue thread has stored its share of this
+        // ---- momentum in the tail of the split-K Linear backward.  Every consumer thread has stored its share of this
         //      item's partial sums; the CTA that completes the last partial of its 128-row tile applies the update
         //      (same arithmetic and summation order as momentum_kernel: parts 0, 1, 2, ...).
         const uint32_t flag_addr = bar_base + 200;
         const unsigned rt = 2u * (unsigned)mp + rank;
         __threadfence();
-        ptx::named_bar_sync(3, 32 * TC2_EPI_WARPS);
-        if (warp == 2 && lane == 0) {
+        ptx::named_bar_sync(3, TC2_CONSUMERS);
+        if (threadIdx.x == 0) {
           const unsigned ticket = atomicAdd(fa.m_counter + rt, 1u);
           ptx::st_shared_u32(flag_addr, ticket == (unsigned)TC_LINEAR_SPLIT - 1u ? 1u : 0u);
         }
-        ptx::named_bar_sync(3, 32 * TC2_EPI_WARPS);
+        ptx::named_bar_sync(3, TC2_CONSUMERS);
         if (ptx::ld_shared_u32(flag_addr) != 0u) {
           __threadfence();
           const float* __restrict__ gp = reinterpret_cast<const float*>(out);
           const size_t base = (size_t)rt * kRowTile * N_TILE;
-          const int tid = (warp - 2) * 32 + lane;
+          const int tid = threadIdx.x;
           // 4 float4 positions per thread in flight at a time (the loop is latency-bound: 6 L2 reads per position)
-          constexpr int STRIDE = 4 * 32 * TC2_EPI_WARPS, UNR = 4;
+          constexpr int STRIDE = 4 * TC2_CONSUMERS, UNR = 4;
           for (int e0 = tid * 4; e0 < kRowTile * N_TILE; e0 += UNR * STRIDE) {
             float4 gs[UNR], vv[UNR], zz[UNR];
 #pragma unroll
@@ -634,14 +544,15 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           if (tid == 0) fa.m_counter[rt] = 0u;             // ready for the next launch
         }
       }
+      ++item_count;
     }
-    if (TMA_EPI && lane == 0) ptx::bulk_wait_read0();   // shared memory no longer read; the writes complete with the grid
+    if (TMA_EPI && lane == 0) ptx::bulk_wait_all0();   // this warp's output stores are complete before the CTA retires
   }
 
 #ifdef DGAN_PROBE
   {
     constexpr int key = tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT));
-    if (warp == 1 && lane == 0) atomicAdd(&g_tc2_probe[key][blockIdx.x][3], (unsigned long long)probe_wait_full);
+    if (threadIdx.x == 0) atomicAdd(&g_tc2_probe[key][blockIdx.x][3], (unsigned long long)probe_wait_full);
     __syncthreads();
     if (threadIdx.x == 0) {
       atomicAdd(&g_tc2_probe[key][blockIdx.x][0], (unsigned long long)(clock64() - probe_t_go));
@@ -653,12 +564,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     }
   }
 #endif
-  ptx::tc_fence_before();
-  ptx::cluster_sync_relaxed();   // the leader's MMAs read the peer's shared memory and TMEM is freed for the pair: nobody leaves early
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc_2sm(tmem_base, 512);
-  }
+  ptx::cluster_sync();   // the peer's multicasts and barrier arrivals target this CTA's shared memory: nobody leaves early
 }
 
 // ------------------------------------------------------------------------------------------
@@ -666,16 +572,16 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 // ------------------------------------------------------------------------------------------
 struct Tc2Schedule {           // one window tiling of a layer-direction + its item -> CTA-pair assignment, uploaded
   TcItem2* items = nullptr;
-  TcRec* stream_p[2] = {nullptr, nullptr};   // producer records per cluster rank; per CTA pair: its items' steps, concatenated
+  TcRec* stream_p = nullptr;       // producer records (both ranks of a pair); per CTA pair: its items' steps, concatenated
   TcRec* stream_m = nullptr;       // MMA records, same indexing
-  Tc2Heads heads{};                // per pair: record offsets into the streams, first item (kernel parameter)
-  int* eitems = nullptr;           // [n_slots][n_pairs] (window << 16 | row pair) for the epilogue warps, or -1
+  Tc2Heads heads{};                // per pair: record offsets into the streams (kernel parameter)
+  int* eitems = nullptr;           // [n_slots][n_pairs] (window << 16 | row pair) for the consumer epilogues, or -1
   int n_slots = 0, n_pairs = 0;
   int n_windows = 0;
   int wh = 0, ww = 0, sy = 1, sx = 1;
 };
 struct TcWeights2 {
-  CUtensorMap tm_b;            // box {64, N/2, 1}
+  CUtensorMap tm_b;            // box {64, N/2, 1}: the half of a weight tile one CTA of the pair loads
   PairTable tab;               // host copy: schedules are built lazily per batch size
   int h_grid = 0, w_grid = 0, max_acc = 1;
   mutable std::vector<std::pair<int, Tc2Schedule>> by_mpairs;   // chosen schedule per n_mpairs (lazy cache)
@@ -687,7 +593,7 @@ static int tc2_maxb(int N) { return TC2_BUF_COLS / tc2_acc_stride(N); }
 struct Tc2HostStep {
   int kc = 0, nA = 0, nB = 0, n_ops = 0;
   int a_pix[TC2_MAX_A] = {0, 0, 0, 0};
-  uint8_t b_ent[2][TC2_MAX_BSLOTS] = {{0}, {0}};
+  uint8_t b_ent[TC2_MAX_BSLOTS] = {0};   // weight tile per B slot
   uint16_t ops[TC2_MAX_OPS] = {0};
   int n_tile_mmas = 0;         // un-merged count (statistics)
   int bytes = 0;               // operand bytes staged per CTA
@@ -704,7 +610,7 @@ struct Tc2HostItem {
 // the step uses (and whose first-MMA flags agree) become one merged-N MMA.
 static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int N, int K, int max_g, int max_a,
                            int step_max_bytes, Tc2HostItem* out) {
-  const int kch = K / 64, half_b = (N / 2) * 128;
+  const int kch = K / 64, b_tile = N * 128;
   out->hdr = TcItem2{};
   out->hdr.n_acc = (uint32_t)qs.size();
   for (size_t a = 0; a < qs.size(); ++a) out->hdr.q[a] = (uint16_t)qs[a];
@@ -724,13 +630,13 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     std::stable_sort(g.second.begin(), g.second.end(), [](const auto& l, const auto& r) { return l.second < r.second; });
   // a pixel with more entries than one step can hold is split (Linear layers: 16 tiles per input "pixel")
   std::vector<std::pair<int, std::vector<std::pair<int, int>>>> px;
-  const int ent_cap = std::min({TC2_MAX_BSLOTS, TC2_MAX_OPS, std::max(1, (step_max_bytes - TC_A_BYTES) / half_b)});
+  const int ent_cap = std::min({TC2_MAX_BSLOTS, TC2_MAX_OPS, std::max(1, (step_max_bytes - TC_A_BYTES) / b_tile)});
   for (auto& g : by_p)
     for (size_t b0 = 0; b0 < g.second.size(); b0 += (size_t)ent_cap)
       px.push_back({g.first, std::vector<std::pair<int, int>>(g.second.begin() + b0,
                                                                g.second.begin() + std::min(g.second.size(), b0 + (size_t)ent_cap))});
-  // ---- phase 1: greedy groups.  (Re-using the weight tiles of the PREVIOUS step as well was measured in round 1:
-  //      5-15 % fewer bytes, but 2 % slower - less ring capacity in flight, fewer merged-N MMAs - and is gone.)
+  // ---- phase 1: greedy groups (each step stages its own weight tiles: re-using the previous step's would save bytes but
+  //      hold ring capacity and split merged-N MMAs).
   struct Group { size_t i0, i1; std::vector<int> staged; };
   std::vector<Group> groups;
   {
@@ -750,7 +656,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
         const int nA = (int)(i1 - i0) + 1, nB = (int)staged.size() + fresh;
         const bool dup_pixel = (i1 > i0 && px[i1].first == px[i1 - 1].first);   // split halves of one pixel stay apart
         if (i1 > i0 && (dup_pixel || nB > TC2_MAX_BSLOTS || n_ent + (int)px[i1].second.size() > TC2_MAX_OPS ||
-                        nA * TC_A_BYTES + nB * half_b > step_max_bytes))
+                        nA * TC_A_BYTES + nB * b_tile > step_max_bytes))
           break;
         for (int t : fresh_tiles) staged.push_back(t);
         n_ent += (int)px[i1].second.size();
@@ -761,7 +667,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     }
   }
   // ---- phase 2: ops + B slots.  A tile is "single use" (mergeable into an N = g*N_TILE MMA) only if no other pixel of
-  //      its group needs it in the plain half-per-CTA layout.
+  //      its group needs it on its own.
   uint32_t seen = 0;
   for (size_t gi = 0; gi < groups.size(); ++gi) {
     const Group& G = groups[gi];
@@ -786,17 +692,13 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
                  (!(seen & (1u << ent[e + g].second))) == f0)
             ++g;
           slot = st.nB;
-          for (int r = 0; r < 2; ++r)
-            for (size_t jj = 0; jj < g; ++jj) {
-              const size_t x = (size_t)r * g + jj;              // half-tile index in W_0.lo, W_0.hi, W_1.lo, ...
-              st.b_ent[r][slot + jj] = (uint8_t)((ent[e + x / 2].first & 0x1F) | ((x & 1) << 5));
-            }
+          for (size_t jj = 0; jj < g; ++jj) st.b_ent[slot + jj] = (uint8_t)(ent[e + jj].first & 0x1F);   // W_0, W_1, ...
           st.nB += (int)g;
         } else if (slot_of[t0] >= 0) {
           slot = slot_of[t0];
         } else {
           slot = slot_of[t0] = st.nB;
-          for (int r = 0; r < 2; ++r) st.b_ent[r][slot] = (uint8_t)((t0 & 0x1F) | (r << 5));
+          st.b_ent[slot] = (uint8_t)(t0 & 0x1F);
           st.nB += 1;
         }
         st.ops[st.n_ops++] = (uint16_t)((i - G.i0) | (slot << 2) | ((g - 1) << 5) | (acc0 << 7) | ((f0 ? 1 : 0) << 10));
@@ -805,7 +707,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
         e += g;
       }
     }
-    st.bytes = st.nA * TC_A_BYTES + st.nB * half_b;
+    st.bytes = st.nA * TC_A_BYTES + st.nB * b_tile;
     out->steps.push_back(st);
   }
   // k-chunk outermost: every accumulator then sums its (k-chunk, input pixel) contributions in one canonical order
@@ -876,7 +778,7 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   int shape[4] = {1, 1, 1, 1};   // wh, ww, sy, sx
   int n_slots = 0, n_pairs = 0;
   std::vector<TcItem2> hdrs;
-  std::vector<TcRec> stream_p[2], stream_m;
+  std::vector<TcRec> stream_p, stream_m;
   std::vector<uint32_t> stream_off;
   std::vector<int> eitems;
   long long n_mma = 0, n_single = 0, n_steps = 0, n_bytes = 0;
@@ -888,11 +790,8 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   const int max_g = (N >= 64) ? std::min(4, 256 / N) : 1;      // merged-N MMAs (see TC2_MAX_A above)
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
-  // ring); measured on C2: 32 KB (= one A tile per step) 5359, 40 KB 5466, 48-56 KB 5660, 64 KB 5553, 96 KB 5385 images/s.
-  // (second sweep, final round-2 epilogue: 40 KB 5679, 48 KB 6047 / 6004, 56 KB 6064, 64 KB 6041 - flat from 48 KB on, except that
-  //  the N = 64, K = 128 layer (Generator.3 forward: 4 KB weight half-tiles, 3 activation tiles + their taps per 64 KB step)
-  //  gains 2 - 3 us per launch with 64 KB steps while the N = 128 layers lose as much: configs[1] 5912 -> 5965 images/s on one
-  //  box; CelebA's layer of that shape is indifferent: 1556 vs 1546)
+  // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
+  // forward: 8 KB weight tiles) packs 3 activation tiles and their taps into 64 KB steps.
   const int step_kb = (N == 64 && K == 128) ? DGAN_STEP_MAX_KB_N64 : DGAN_STEP_MAX_KB;
   const int step_max = std::min((ring_bytes / 2) & ~1023, step_kb * 1024);
   double best_cost = 1e300;
@@ -985,9 +884,9 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   eitems.assign(n_slots * (size_t)n_pairs, -1);
   std::vector<uint32_t>& stream_off = plan->stream_off;
   stream_off.assign((size_t)n_pairs + 1, 0);
-  std::vector<TcRec>* stream_p = plan->stream_p;
+  std::vector<TcRec>& stream_p = plan->stream_p;
   std::vector<TcRec>& stream_m = plan->stream_m;
-  stream_p[0].clear(); stream_p[1].clear(); stream_m.clear();
+  stream_p.clear(); stream_m.clear();
   long long n_mma = 0, n_single = 0, n_steps = 0, n_bytes = 0;
   for (size_t pr = 0; pr < best_lists.size(); ++pr) {
     stream_off[pr] = (uint32_t)stream_m.size();
@@ -1020,15 +919,14 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         rm.w[0] = (uint32_t)beg | ((uint32_t)hs.nA << 8) | ((uint32_t)hs.n_ops << 11) | (flags << 16);
         for (int o = 0; o < hs.n_ops; ++o) rm.w[2 + o / 2] |= (uint32_t)hs.ops[o] << (16 * (o & 1));
         stream_m.push_back(rm);
-        for (int r = 0; r < 2; ++r) {
-          TcRec rp{};
-          rp.w[0] = (uint32_t)beg | ((uint32_t)hs.kc << 8) | ((uint32_t)hs.nA << 12) | ((uint32_t)hs.nB << 15) | ((uint32_t)dep << 19);
-          rp.w[1] = (uint32_t)mp;
-          for (int a = 0; a < hs.nA; ++a) rp.w[2 + a / 2] |= (uint32_t)(hs.a_pix[a] & 0xFFFF) << (16 * (a & 1));
-          for (int b = 0; b < hs.nB; ++b) rp.w[4 + b / 4] |= (uint32_t)hs.b_ent[r][b] << (8 * (b & 3));
-          stream_p[r].push_back(rp);
-        }
-        n_mma += hs.n_ops; n_single += hs.n_tile_mmas; n_steps += 1; n_bytes += hs.bytes;
+        TcRec rp{};
+        rp.w[0] = (uint32_t)beg | ((uint32_t)hs.kc << 8) | ((uint32_t)hs.nA << 12) | ((uint32_t)hs.nB << 15) | ((uint32_t)dep << 19);
+        rp.w[1] = (uint32_t)mp;
+        for (int a = 0; a < hs.nA; ++a) rp.w[2 + a / 2] |= (uint32_t)(hs.a_pix[a] & 0xFFFF) << (16 * (a & 1));
+        for (int b = 0; b < hs.nB; ++b) rp.w[4 + b / 4] |= (uint32_t)hs.b_ent[b] << (8 * (b & 3));
+        stream_p.push_back(rp);
+        // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
+        n_mma += hs.n_ops; n_single += hs.n_tile_mmas; n_steps += 1; n_bytes += 2LL * hs.nA * TC_A_BYTES + (long long)hs.nB * N * 128;
       }
     }
   }
@@ -1042,7 +940,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 // Independent validation of a plan against the pair table it was built from (host only; used by
 // dgan_debug_check_plans and the CPU tests).  Re-derives from the uploaded records alone:
 //  * every (output pixel, input pixel, tap, k-chunk) contribution of every item happens exactly once, into the right
-//    accumulator, with the weight half-tiles each CTA stages forming exactly the operand the MMA reads;
+//    accumulator, with the weight tiles each CTA stages forming exactly the operand the MMA reads;
 //  * the first MMA into an accumulator - and only that one - overwrites it;
 //  * every accumulator sums in the canonical order (k-chunk major, input pixel ascending): results then do not
 //    depend on the schedule (batch-size / sharding invariance);
@@ -1051,10 +949,10 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //  * every (window, row pair) item is assigned to exactly one CTA pair.
 static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int ring_bytes, const Tc2Plan& pl, std::string* err) {
   auto fail = [&](const std::string& m) { *err = m; return DGAN_ERR_INVALID_ARG; };
-  const int kch = K / 64, half_b = (N / 2) * 128, acc_stride = tc2_acc_stride(N), max_acc = TC2_BUF_COLS / acc_stride;
+  const int kch = K / 64, b_tile = N * 128, acc_stride = tc2_acc_stride(N), max_acc = TC2_BUF_COLS / acc_stride;
   const size_t n_pairs = (size_t)pl.n_pairs;
   if (pl.stream_off.size() != n_pairs + 1) return fail("stream_off size");
-  if (pl.stream_p[0].size() != pl.stream_m.size() || pl.stream_p[1].size() != pl.stream_m.size()) return fail("stream sizes differ");
+  if (pl.stream_p.size() != pl.stream_m.size()) return fail("stream sizes differ");
   if (pl.eitems.size() != (size_t)pl.n_slots * n_pairs) return fail("eitems size");
   std::vector<int> assigned(pl.hdrs.size() * (size_t)n_mpairs, 0);
   for (const TcItem2& h : pl.hdrs) {
@@ -1062,7 +960,7 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
     for (uint32_t a = 0; a < h.n_acc; ++a)
       if ((size_t)h.q[a] + 1 >= tab.off.size()) return fail("window pixel out of range");
   }
-  struct Step { int beg, end, nB, kc; uint8_t b0[8], b1[8]; };
+  struct Step { int beg, end, nB, kc; uint8_t b[8]; };
   for (size_t pr = 0; pr < n_pairs; ++pr) {
     const uint32_t r_beg = pl.stream_off[pr], r_end = pl.stream_off[pr + 1];
     if (r_beg > r_end || r_end > pl.stream_m.size()) return fail("stream_off not monotone");
@@ -1073,19 +971,18 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
     std::vector<std::pair<int, int>> last_kp;                     // per accumulator: last (kc, p)
     std::vector<std::vector<std::pair<int, int>>> contrib;        // per accumulator: (p * 32 + tile, kc)
     for (uint32_t ri = r_beg; ri < r_end; ++ri) {
-      const TcRec &m = pl.stream_m[ri], &p0 = pl.stream_p[0][ri], &p1 = pl.stream_p[1][ri];
+      const TcRec &m = pl.stream_m[ri], &p0 = pl.stream_p[ri];
       const int k = (int)steps.size();
       Step st{};
       st.beg = (int)(p0.w[0] & 0xFF);
       const int nA = (int)((p0.w[0] >> 12) & 7), nB = (int)((p0.w[0] >> 15) & 0xF), dep = (int)((p0.w[0] >> 19) & 0xF);
       st.kc = (int)((p0.w[0] >> 8) & 0xF); st.nB = nB;
-      if (p1.w[0] != p0.w[0] || p1.w[1] != p0.w[1] || p1.w[2] != p0.w[2] || p1.w[3] != p0.w[3]) return fail("producer records of the two ranks disagree");
       if ((int)(m.w[0] & 0xFF) != st.beg || (int)((m.w[0] >> 8) & 7) != nA) return fail("MMA record disagrees with the producer record");
       if (nA < 1 || nA > TC2_MAX_A || nB > TC2_MAX_BSLOTS || st.kc >= kch) return fail("step field out of range");
-      st.end = st.beg + (nA * TC_A_BYTES + nB * half_b + 1023) / 1024;
+      st.end = st.beg + (nA * TC_A_BYTES + nB * b_tile + 1023) / 1024;
       if (st.end * 1024 > ring_bytes) return fail("step region outside the ring");
       if (dep < 1 || dep > TC2_NSLOT) return fail("dep out of range");
-      for (int b = 0; b < 8; ++b) { st.b0[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3))); st.b1[b] = (uint8_t)(p1.w[4 + b / 4] >> (8 * (b & 3))); }
+      for (int b = 0; b < 8; ++b) st.b[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3)));
       const uint32_t flags = (m.w[0] >> 16) & 3u;
       const int n_ops = (int)((m.w[0] >> 11) & 0x1F);
       if (n_ops > TC2_MAX_OPS) return fail("too many ops in a step");
@@ -1118,11 +1015,8 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
         {
           if (slot + g > nB) return fail("op reads a B slot the step does not stage");
           for (int i = 0; i < g; ++i) {
-            const int x0 = 2 * i, x1 = 2 * i + 1;
-            const uint8_t* lo = (x0 / g) ? st.b1 : st.b0; const uint8_t* hi = (x1 / g) ? st.b1 : st.b0;
-            const uint8_t el = lo[slot + x0 % g], eh = hi[slot + x1 % g];
-            if ((el & 0x20) != 0 || (eh & 0x20) == 0 || (el & 0x1F) != (eh & 0x1F)) return fail("staged weight halves do not form the MMA operand");
-            tiles[i] = el & 0x1F;
+            if (st.b[slot + i] & 0xE0) return fail("weight tile entry out of range");
+            tiles[i] = st.b[slot + i];
           }
         }
         for (int i = 0; i < g; ++i) {
@@ -1177,12 +1071,10 @@ static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& 
   sc.wh = plan.shape[0]; sc.ww = plan.shape[1]; sc.sy = plan.shape[2]; sc.sx = plan.shape[3];
   sc.n_windows = (int)plan.hdrs.size(); sc.n_pairs = n_pairs; sc.n_slots = plan.n_slots;
   if ((rc = tc_upload(allocs, plan.hdrs.data(), plan.hdrs.size() * sizeof(TcItem2), (void**)&sc.items, s))) return rc;
-  for (int r = 0; r < 2; ++r)
-    if ((rc = tc_upload(allocs, plan.stream_p[r].data(), plan.stream_p[r].size() * sizeof(TcRec), (void**)&sc.stream_p[r], s))) return rc;
+  if ((rc = tc_upload(allocs, plan.stream_p.data(), plan.stream_p.size() * sizeof(TcRec), (void**)&sc.stream_p, s))) return rc;
   if ((rc = tc_upload(allocs, plan.stream_m.data(), plan.stream_m.size() * sizeof(TcRec), (void**)&sc.stream_m, s))) return rc;
   if (n_pairs > TC2_MAX_PAIRS) { set_error("more CTA pairs than the kernel's parameter block holds"); return DGAN_ERR_UNSUPPORTED; }
   for (int pr = 0; pr <= n_pairs; ++pr) sc.heads.off[pr] = plan.stream_off[(size_t)pr];
-  for (int pr = 0; pr < n_pairs; ++pr) sc.heads.first[pr] = plan.n_slots > 0 ? plan.eitems[(size_t)pr] : -1;
   if ((rc = tc_upload(allocs, plan.eitems.data(), plan.eitems.size() * sizeof(int), (void**)&sc.eitems, s))) return rc;
   w2.by_mpairs.push_back({n_mpairs, sc});
   *out = &w2.by_mpairs.back().second;
@@ -1235,10 +1127,10 @@ static int tc2_launch_impl(TcState& st, int64_t* launches, const TcWeights& w, c
   cudaError_t le = cudaSuccess;
 #define TC2_GO(NT, EP)                                                                                                 \
   le = launch_pdl(tc_bsgemm2_kernel<NT, EP, TOUT>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, EP, (int)sizeof(TOUT)>::SMEM_BYTES, s, \
-                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p[0], w2s.stream_p[1], w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, bias, w.bias_pstride, fa)
+                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, bias, w.bias_pstride, fa)
 #define TC2_GO_H(NT, EP)                                                                                               \
   le = launch_pdl(tc_bsgemm2_kernel<NT, EP, __half>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, EP, 2>::SMEM_BYTES, s,   \
-                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p[0], w2s.stream_p[1], w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, reinterpret_cast<__half*>(out), n_pad, bias, 0, fa)
+                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, reinterpret_cast<__half*>(out), n_pad, bias, 0, fa)
 #define TC2_BY_N(EP)                    \
   do {                                  \
     if (w.N == 64) TC2_GO(64, EP);      \

@@ -2,7 +2,7 @@
 
 Same class names, attribute names, defaults, argument meaning and error behaviour as
 `DefenseGANBase` and its dataset subclasses (reference models/gan.py:39-135,333-449,649-765),
-with the TF1 graph machinery replaced by eager calls into the native sm_100a library:
+with the TF1 graph machinery replaced by eager calls into the native sm_90a library:
 
     gan = MnistDefenseGAN(cfg=cfg, test_mode=True)
     gan.load_generator()                      # reference models/gan.py:86-87
@@ -114,7 +114,7 @@ class DefenseGANBase(object):
         self.attribute = "gender"
         self.output_dir = "output"
         # additions of this implementation
-        self.precision = "fp32"            # 'fp32' (CUDA-core, reference arithmetic) | 'fp16' (tcgen05 operands)
+        self.precision = "fp32"            # 'fp32' (CUDA-core, reference arithmetic) | 'fp16' (wgmma operands)
         self.rec_momentum = 0.7            # tf.train.MomentumOptimizer(momentum=0.7), models/gan.py:389-391
         self.rec_decay_lr = False          # the reference's decay is dead code (SURVEY F3); True = intended schedule
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
@@ -300,7 +300,7 @@ class DefenseGANBase(object):
             raise TypeError("expected a torch.Tensor or numpy array")
         if not t.is_cuda:
             if not torch.cuda.is_available():
-                raise RuntimeError("defensegan_b200 needs a CUDA (sm_100) device; there is no CPU fallback")
+                raise RuntimeError("defensegan_b200 needs a CUDA (sm_90) device; there is no CPU fallback")
             t = t.cuda(non_blocking=True)
         return t.to(torch.float32)
 

@@ -1,5 +1,5 @@
 /*
- * defensegan_b200.h - C ABI of the B200-native Defense-GAN projection loop.
+ * defensegan_b200.h - C ABI of the H100-native Defense-GAN projection loop.
  *
  * The reference (kabkabm/defensegan) has no FFI/plugin interface: the boundary is the Python
  * method DefenseGANBase.reconstruct (models/gan.py:333-449) plus the eval driver
@@ -41,7 +41,7 @@ enum dgan_arch { DGAN_ARCH_MNIST = 0, DGAN_ARCH_CELEBA = 1 };
 /* arithmetic of the contractions.  State (z, momentum, loss, accumulators) is always fp32. */
 enum dgan_precision {
   DGAN_PREC_FP32 = 0, /* fp32 operands, CUDA-core FMA: the reference's arithmetic type */
-  DGAN_PREC_FP16 = 1  /* fp16 operands, fp32 accumulate, tcgen05 tensor cores */
+  DGAN_PREC_FP16 = 1  /* fp16 operands, fp32 accumulate, wgmma tensor cores */
 };
 
 typedef struct dgan_desc {

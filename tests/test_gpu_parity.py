@@ -1,10 +1,10 @@
-"""GPU parity tests (run on the B200 box with -m gpu): every call goes through the C-ABI
+"""GPU parity tests (run on an H100 with -m gpu): every call goes through the C-ABI
 (ctypes -> libdefensegan_b200.so) and is checked against the CPU oracle / golden vectors.
 
 Tolerances (stated per precision):
   fp32 (CUDA-core FMA, the reference's arithmetic type): elementwise |rec - rec_oracle64| <= 1e-4,
        identical arg-min indices, |loss_min - oracle| <= 1e-6 at the C1 horizon.
-  fp16 (tcgen05 operands, fp32 accumulate): per-image |MSE_min - oracle| <= 1e-4 (BASELINE.json's
+  fp16 (wgmma operands, fp32 accumulate): per-image |MSE_min - oracle| <= 1e-4 (BASELINE.json's
        bar), elementwise |rec - rec_oracle| <= 2e-2 at the C1 horizon.
 """
 import ctypes

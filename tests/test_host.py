@@ -517,7 +517,7 @@ def test_load_generator_from_tf_checkpoint_dir(tmp_path):
 # ---------------------------------------------------------------------------------------------------
 # tensor-core schedule planner (host code of the CUDA library; needs no GPU)
 # ---------------------------------------------------------------------------------------------------
-def _check_plans(arch, n_rows, n_pairs=74, net_dim=64, mutate=0, use_bn=0):
+def _check_plans(arch, n_rows, n_pairs=66, net_dim=64, mutate=0, use_bn=0):
     import ctypes
     from defensegan_b200 import _native
     lib = _native.load_library()
@@ -593,7 +593,7 @@ def test_plan_statistics_entry_point():
     lib.dgan_debug_plan_stats.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
     desc = _native.dgan_desc(_native.ABI_VERSION, 0, 128, 64, 0, 1)
     buf = ctypes.create_string_buffer(1 << 16)
-    assert lib.dgan_debug_plan_stats(ctypes.byref(desc), 2560, 74, buf, len(buf)) > 0
+    assert lib.dgan_debug_plan_stats(ctypes.byref(desc), 2560, 66, buf, len(buf)) > 0
     rows = [l.split(" | ") for l in buf.value.decode().strip().splitlines()[1:]]
     by = {r[0]: r for r in rows}
     assert float(by["total staged MB per L-step"][1]) < 1900.0

@@ -1,4 +1,4 @@
-"""Per-kernel SASS mnemonic histogram of the built library (evidence that tcgen05 / TMEM / TMA are on the hot path).
+"""Per-kernel SASS mnemonic histogram of the built library (evidence that wgmma / TMA are on the hot path).
 Usage: python tools/sass_histogram.py [library.so] > profiles/<name>.md"""
 import collections
 import re
@@ -16,7 +16,7 @@ for line in sass.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_.]*)", line)
     if m and fn:
         hist[fn][m.group(1)] += 1
-keys = ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMASTG", "LDTM", "UTCATOMSWS", "SYNCS", "STL", "LDL", "USETMAXREG", "MEMBAR",
+keys = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "SYNCS", "STL", "LDL", "MEMBAR",
         "FENCE", "RED", "ATOMG", "LDG", "STG", "BAR", "ELECT"]
 print("| kernel | total | " + " | ".join(keys) + " |")
 print("|---|---|" + "---|" * len(keys))
