@@ -1094,8 +1094,18 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
       TcRec& m = plan.stream_m[20];
       TcRec* pp = &plan.stream_p[20];
       switch (mutate) {
-        case 1: m.w[2] ^= 1u << 10; break;                                  // first-MMA flag of an op
-        case 2: m.w[2] ^= 1u << 7; break;                                   // accumulator of an op
+        case 1: m.w[2] ^= 1u << 6; break;                                   // first-MMA flag of an op
+        case 2: {                                                           // accumulator of an op: swap two ops of round 0
+                  const int nb = (int)m.w[1];
+                  for (int j = 1; j < nb; ++j) {
+                    const uint32_t b0 = m.w[2] & 0xFFu, bj = (m.w[2 + j / 4] >> (8 * (j & 3))) & 0xFFu;
+                    if (bj == b0) continue;
+                    m.w[2] = (m.w[2] & ~0xFFu) | bj;
+                    m.w[2 + j / 4] = (m.w[2 + j / 4] & ~(0xFFu << (8 * (j & 3)))) | (b0 << (8 * (j & 3)));
+                    break;
+                  }
+                  break;
+                }
         case 3: pp->w[4] ^= 0x01; break;                                    // weight tile of a B slot
         case 4: pp->w[2] ^= 0x01; break;                                    // input pixel of an A tile
         case 5: pp->w[0] = (pp->w[0] & ~(0xFu << 8)) | ((((pp->w[0] >> 8) & 0xF) ^ 1u) << 8); break;   // k-chunk
@@ -1134,7 +1144,8 @@ int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
-  std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load\n";
+  std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load"
+                    " | zero-tile MMA %\n";
   double total = 0.0;
   for (const PlanDir& dr : plan_dirs(d)) {
     int max_acc = tc2_maxb(dr.N);
@@ -1146,9 +1157,10 @@ int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf
     char line[256];
     const double mb = (double)plan.n_bytes / 1e6;
     total += mb;
-    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f\n", dr.name.c_str(), dr.N, dr.K,
+    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f\n", dr.name.c_str(), dr.N, dr.K,
              plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,
-             plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0));
+             plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0),
+             100.0 * (double)plan.n_pad / (double)std::max(plan.n_mma, 1LL));
     out += line;
   }
   char line[64];

@@ -7,11 +7,15 @@
 //   * operands live in a circular shared-memory ring of variable-size steps planned on the host
 //     (tc2_get_schedule): per CTA pair one contiguous stream of step records, LPT-assigned; a ring region is refilled
 //     only after the consumers of BOTH CTAs released it (the peer's loads write into it too);
-//   * roles per CTA: one TMA producer warp and two consumer warpgroups.  Each consumer warpgroup owns 64 of the
-//     tile's 128 rows and issues wgmma.mma_async (M = 64, K = 16) for every op of a step into register accumulators
-//     - up to 256 columns: the 1-8 accumulators of the item's window - and releases the step's ring region once its
-//     MMAs have completed; after the item's last step it runs the epilogue straight from those registers.  Each
-//     consumer warp stores the 16 rows it holds with its own TMA store (no block-level barrier on the store path).
+//   * roles per CTA: one producer warpgroup (one warp issues the TMA loads) and two consumer warpgroups.  The producer
+//     gives up registers (setmaxnreg) so that the consumers can hold accumulators and epilogue without spilling.  Each
+//     consumer warpgroup owns 64 of the tile's 128 rows and issues wgmma.mma_async (M = 64, K = 16) into register
+//     accumulators - up to 256 columns: the 1-8 accumulators of the item's window.  A step is a run-time number of
+//     rounds, and a round is one MMA into EVERY accumulator in compile-time order, so the compiler never has to choose
+//     an accumulator at run time (an accumulator with nothing to add in a round reads an all-zero weight tile).  One
+//     wgmma group is committed per step and a step's ring region is released once the NEXT step's MMAs are issued and
+//     the step's own group has retired; after the item's last step the consumer waits for all MMAs and runs the
+//     epilogue straight from the registers.  Each consumer warp stores the 16 rows it holds with its own TMA store.
 #pragma once
 #include "kernels_tc.cuh"
 
@@ -21,7 +25,10 @@ constexpr int TC2_SMEM_MAX = 232448;         // 227 KB opt-in limit per CTA
 constexpr int TC2_TILE_BYTES = 128 * 128;    // one 128-row x 64-channel fp16 tile (TMA box, 128B swizzle)
 constexpr int TC2_BUF_COLS = 256;            // accumulator columns of one item (128 fp32 registers per consumer thread)
 constexpr int TC2_CONSUMERS = 256;           // two consumer warpgroups
-constexpr int TC2_THREADS = TC2_CONSUMERS + 32;   // + the TMA producer warp
+constexpr int TC2_THREADS = TC2_CONSUMERS + 128;   // + the producer warpgroup
+// Register split of the 64K-entry register file (setmaxnreg): 128 x 40 + 256 x 232 = 64512.  Every thread starts at
+// the launch's 168.
+constexpr int TC2_PRODUCER_REGS = 40, TC2_CONSUMER_REGS = 232;
 constexpr int TC2_STORE_ROWS = 16;           // rows per output TMA store: each consumer warp stores the 16 rows it holds
 
 // Where each CTA pair's work starts, passed in the kernel's parameter space (constant bank): the first records are then
@@ -50,7 +57,7 @@ __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out
 //
 // A step stages up to 4 input-pixel (A) tiles and up to 8 full weight tiles (B slots) for one k-chunk into a
 // variable-size region of a circular shared-memory ring (offset chosen by the host, which simulates the ring),
-// then issues up to 12 MMAs that combine them.  Several A tiles per step let one weight tile serve several input
+// then issues rounds of MMAs that combine them.  Several A tiles per step let one weight tile serve several input
 // pixels (stride-2 transposed conv: outputs of equal parity use the same tap with neighbouring inputs), which
 // is what the L2->SM byte count cares about.
 //
@@ -61,13 +68,13 @@ __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out
 //   w[2..3]: 4 x u16 input pixel of A tile i
 //   w[4..5]: 8 x u8 weight tile [0,5) per B slot
 // MMA record:
-//   w[0]: ring offset / 1 KB [0,8) | A tiles [8,11) | ops [11,16) | flags [16,18): 1 = first step of an item, 2 = last
-//   w[2..7]: 12 x u16 per MMA: A tile [0,2) | first B slot [2,5) | slots - 1 [5,7) | accumulator [7,10) | first MMA into it [10,11)
+//   w[0]: ring offset / 1 KB [0,8) | A tiles [8,11) | rounds [11,16) | flags [16,18): 1 = first step of an item, 2 = last
+//   w[1]: accumulators per round (MAXB of the instantiation; checked by the validator only)
+//   w[2..7]: 24 x u8, round-major, one per (round, accumulator): A tile [0,2) | B slot [2,6) | first MMA into the
+//            accumulator [6,7).  B slot 15 = the all-zero tile outside the ring (the accumulator has nothing to add in
+//            this round; never a first MMA).
 struct __align__(16) TcRec { uint32_t w[8]; };
-constexpr int TC2_MAX_A = 4, TC2_MAX_BSLOTS = 8, TC2_MAX_OPS = 12, TC2_NSLOT = 8;
-// Merged-N groups: when one input pixel feeds g accumulators that sit side by side (acc, acc+1, ...) through weight
-// tiles nobody else in the step uses, the g tiles are staged back to back and ONE MMA of N = g * N_TILE updates all of
-// them.
+constexpr int TC2_MAX_A = 4, TC2_MAX_BSLOTS = 8, TC2_OP_BYTES = 24, TC2_ZERO_SLOT = 15, TC2_NSLOT = 8;
 constexpr int TC2_REC_BATCH = 16;
 constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // producer record ring
 
@@ -76,9 +83,14 @@ constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // produ
 __host__ __device__ constexpr int tc2_epi_tiles(int n_tile, int epi, int out_bytes) {
   return tc2_tma_epilogue(n_tile, epi, out_bytes) ? 2 : 0;
 }
+// The all-zero weight tile read by the MMAs of an accumulator with nothing to add in a round (instantiations with more
+// than one accumulator per window).  It sits right after the ring and is written once per CTA.
+__host__ __device__ constexpr int tc2_zero_bytes(int n_tile) {
+  return TC2_BUF_COLS / tc2_acc_stride(n_tile) > 1 ? n_tile * 128 : 0;
+}
 __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
-  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b) / 1024) * 1024;
+  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile)) / 1024) * 1024;
   return raw > 255 * 1024 ? 255 * 1024 : raw;
 }
 
@@ -86,13 +98,13 @@ template <int N_TILE, int EPI = EPI_NONE, int OUT_BYTES = 2>
 struct Tc2Cfg {
   static constexpr int B_TILE = N_TILE * 128;                             // bytes of one staged weight tile
   static constexpr int MAXB = TC2_BUF_COLS / tc2_acc_stride(N_TILE);      // = accumulators per window (8 / 4 / 2 / 1)
-  static constexpr int MAXG = N_TILE >= 64 ? (256 / N_TILE < 4 ? 256 / N_TILE : 4) : 1;   // tiles of a merged MMA
   static constexpr int ACC_REGS = MAXB * N_TILE / 2;                      // accumulator registers per consumer thread
   static constexpr bool TMA_EPI = tc2_tma_epilogue(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_TILES = tc2_epi_tiles(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_BYTES = EPI_TILES * TC2_TILE_BYTES;
+  static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE);
   static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, EPI, OUT_BYTES);          // operand ring (offsets are 8-bit KB)
-  static constexpr int SMEM_BYTES = RING_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = RING_BYTES + ZERO_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
 };
 
 namespace ptx {
@@ -147,6 +159,9 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // true in exactly one lane of a converged warp
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -161,21 +176,36 @@ __device__ __forceinline__ int tc2_item_at(const int* __restrict__ order, int k,
   return k < n_slots ? __ldg(order + (size_t)k * n_pairs + pair) : -1;
 }
 
-// One op of a step: the 4 k16 MMAs of a 64-channel k-chunk into accumulators [a, a + g).  The accumulator registers
-// must be named at compile time, so the (a, g) pair of the record selects one of the unrolled instantiations.
-template <int NT, int MAXB, int MAXG, int A = 0, int G = 1, int NREG>
-__device__ __forceinline__ void tc2_mma_op(float (&acc)[NREG], int a, int g, uint64_t da, uint64_t db, uint32_t first) {
-  if constexpr (A < MAXB) {
-    if constexpr (A + G <= MAXB) {
-      if (a == A && g == G) {
+// One round of a step: for every accumulator a, in compile-time order, the 4 k16 MMAs of a 64-channel k-chunk.  Only
+// the operand descriptors and the overwrite predicate come from the record byte of (round, a), so the sequence of
+// wgmma instructions and the registers they name are fixed.
+//   da0 / db0: descriptors of the step's first A tile (this warpgroup's rows) and first B slot; zoff: the zero tile's
+//   distance from db0 in 16-byte units.
+template <int NT, int MAXB, int NREG>
+__device__ __forceinline__ void tc2_mma_round(float (&acc)[NREG], const uint32_t (&q)[6], uint64_t da0, uint64_t db0, uint32_t zoff) {
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          ptx::Wgmma<NT * G>::mma(acc + A * (NT / 2), da + 2u * k, db + 2u * k, (k > 0 || !first) ? 1u : 0u);
-        return;
-      }
-    }
-    if constexpr (G < MAXG) tc2_mma_op<NT, MAXB, MAXG, A, G + 1>(acc, a, g, da, db, first);
-    else tc2_mma_op<NT, MAXB, MAXG, A + 1, 1>(acc, a, g, da, db, first);
+  for (int a = 0; a < MAXB; ++a) {
+    const uint32_t e = (q[a >> 2] >> (8 * (a & 3))) & 0xFFu;
+    const uint32_t bs = (e >> 2) & 0xFu;
+    // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
+    const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(TC_A_BYTES >> 4));
+    const uint64_t db = db0 + (uint64_t)(bs == (uint32_t)TC2_ZERO_SLOT ? zoff : bs * (uint32_t)(NT * 128 >> 4));
+    const uint32_t keep = ((e >> 6) & 1u) ^ 1u;      // 0: first MMA into the accumulator, overwrite it
+#pragma unroll
+    for (int k = 0; k < 4; ++k) ptx::Wgmma<NT>::mma(acc + a * (NT / 2), da + 2u * k, db + 2u * k, k > 0 ? 1u : keep);
+  }
+}
+
+// Drop the record bytes of one round (MAXB of them) from the front of the op queue.
+template <int MAXB>
+__device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
+  if constexpr (MAXB >= 4) {
+#pragma unroll
+    for (int i = 0; i < 6; ++i) q[i] = (i + MAXB / 4 < 6) ? q[i + MAXB / 4] : 0u;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 5; ++i) q[i] = __funnelshift_r(q[i], q[i + 1], 8 * MAXB);
+    q[5] >>= 8 * MAXB;
   }
 }
 
@@ -216,7 +246,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   long long probe_wait_full = 0;
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t epi_base = smem_base + Cfg::RING_BYTES;            // output staging: 4 KB per consumer warp
+  const uint32_t zero_base = smem_base + Cfg::RING_BYTES;           // the all-zero weight tile
+  const uint32_t epi_base = zero_base + Cfg::ZERO_BYTES;            // output staging: 4 KB per consumer warp
   const uint32_t stg_base = epi_base + Cfg::EPI_BYTES;              // producer ring of TcRec
   const uint32_t bar_base = stg_base + TC2_STAGING_BYTES;
   // full[s] @ +8s (s<8), empty[s] @ +64+8s, momentum-tail flag @ +200
@@ -243,6 +274,12 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       ptx::fence_barrier_init();
     }
   }
+  if constexpr (Cfg::ZERO_BYTES > 0) {
+    if (threadIdx.x < TC2_CONSUMERS) {
+      for (uint32_t i = threadIdx.x; i < (uint32_t)Cfg::ZERO_BYTES / 16u; i += TC2_CONSUMERS) ptx::st_shared_v4(zero_base + 16u * i, 0u, 0u, 0u, 0u);
+      ptx::fence_proxy_async_smem();           // the MMAs read it through the async proxy
+    }
+  }
   ptx::cluster_sync();                         // barriers of BOTH CTAs initialised before any remote signal
   // everything above overlapped the previous kernel's tail (PDL); from here on we read what it wrote
 #ifdef DGAN_PROBE
@@ -254,98 +291,117 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   const long long probe_t_go = clock64();
 #endif
 
-  if (warp == PRODUCER) {
-    // ===================== TMA producer =====================
-    // The whole warp walks the step list convergently; every table value is loaded from a warp-uniform address, and
-    // one elected lane issues.
-    const TcRec* __restrict__ stream = stream_p;
-    uint32_t it = 0;
-    const uint32_t ring = stg_base;
-    for (uint32_t base = rbeg; base < rend; base += TC2_REC_BATCH) {
-      ptx::st_shared_v4(ring + lane * 16u, mine.x, mine.y, mine.z, mine.w);
-      __syncwarp();
-      if (2 * (base + TC2_REC_BATCH) + lane < 2 * rend) mine = __ldg(reinterpret_cast<const uint4*>(stream + base + TC2_REC_BATCH) + lane);
-      const uint32_t cnt = min((uint32_t)TC2_REC_BATCH, rend - base);
-      for (uint32_t i = 0; i < cnt; ++i, ++it) {
-        const uint4 r0 = ptx::ld_shared_v4(ring + i * 32u);
-        const uint2 r1 = ptx::ld_shared_v2(ring + i * 32u + 16u);
-        const uint32_t slot = it & (TC2_NSLOT - 1);
-        const int kc = (r0.x >> 8) & 0xF, nA = (r0.x >> 12) & 0x7, nB = (r0.x >> 15) & 0xF;
-        const uint32_t dep = (r0.x >> 19) & 0xF;
-        const int row0 = (2 * (int)(r0.y & 0xFFFFu) + (int)rank) * kRowTile;
-        if (it >= dep) ptx::mbar_wait(bar_empty + 8 * ((it - dep) & (TC2_NSLOT - 1)), ((it - dep) >> 3) & 1);   // step it-dep consumed
-        // implied by the wait above (steps are consumed in order); observing every phase of this slot exactly once
-        // before it is re-armed keeps the barrier protocol simple to check
-        if (dep != TC2_NSLOT && it >= TC2_NSLOT) ptx::mbar_wait(bar_empty + 8 * slot, ((it - TC2_NSLOT) >> 3) & 1);
-        const uint32_t full = bar_full + 8 * slot;
-        const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
-        if (ptx::elect_one()) {
-          ptx::mbar_expect_tx(full, (uint32_t)(nA * TC_A_BYTES + nB * B_TILE));
+  if (warp >= PRODUCER) {
+    // ===================== producer warpgroup =====================
+    // It hands registers to the consumer warpgroups.  Only its first warp has work; the other three wait at the final
+    // cluster barrier.
+    ptx::setmaxnreg_dec<TC2_PRODUCER_REGS>();
+    if (warp == PRODUCER) {
+      // The whole warp walks the step list convergently; every table value is loaded from a warp-uniform address, and
+      // one elected lane issues.
+      const TcRec* __restrict__ stream = stream_p;
+      uint32_t it = 0;
+      const uint32_t ring = stg_base;
+      for (uint32_t base = rbeg; base < rend; base += TC2_REC_BATCH) {
+        ptx::st_shared_v4(ring + lane * 16u, mine.x, mine.y, mine.z, mine.w);
+        __syncwarp();
+        if (2 * (base + TC2_REC_BATCH) + lane < 2 * rend) mine = __ldg(reinterpret_cast<const uint4*>(stream + base + TC2_REC_BATCH) + lane);
+        const uint32_t cnt = min((uint32_t)TC2_REC_BATCH, rend - base);
+        for (uint32_t i = 0; i < cnt; ++i, ++it) {
+          const uint4 r0 = ptx::ld_shared_v4(ring + i * 32u);
+          const uint2 r1 = ptx::ld_shared_v2(ring + i * 32u + 16u);
+          const uint32_t slot = it & (TC2_NSLOT - 1);
+          const int kc = (r0.x >> 8) & 0xF, nA = (r0.x >> 12) & 0x7, nB = (r0.x >> 15) & 0xF;
+          const uint32_t dep = (r0.x >> 19) & 0xF;
+          const int row0 = (2 * (int)(r0.y & 0xFFFFu) + (int)rank) * kRowTile;
+          if (it >= dep) ptx::mbar_wait(bar_empty + 8 * ((it - dep) & (TC2_NSLOT - 1)), ((it - dep) >> 3) & 1);   // step it-dep consumed
+          // implied by the wait above (steps are consumed in order); observing every phase of this slot exactly once
+          // before it is re-armed keeps the barrier protocol simple to check
+          if (dep != TC2_NSLOT && it >= TC2_NSLOT) ptx::mbar_wait(bar_empty + 8 * slot, ((it - TC2_NSLOT) >> 3) & 1);
+          const uint32_t full = bar_full + 8 * slot;
+          const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
+          if (ptx::elect_one()) {
+            ptx::mbar_expect_tx(full, (uint32_t)(nA * TC_A_BYTES + nB * B_TILE));
 #pragma unroll
-          for (int a = 0; a < TC2_MAX_A; ++a) {
-            if (a >= nA) break;
-            const int p = (int)((((a < 2) ? r0.z : r0.w) >> (16 * (a & 1))) & 0xFFFFu);
-            ptx::tma_load_3d(sa + a * TC_A_BYTES, &tm_a, full, kc * 64, row0, p);
-          }
-          const uint32_t sb = sa + nA * TC_A_BYTES;
+            for (int a = 0; a < TC2_MAX_A; ++a) {
+              if (a >= nA) break;
+              const int p = (int)((((a < 2) ? r0.z : r0.w) >> (16 * (a & 1))) & 0xFFFFu);
+              ptx::tma_load_3d(sa + a * TC_A_BYTES, &tm_a, full, kc * 64, row0, p);
+            }
+            const uint32_t sb = sa + nA * TC_A_BYTES;
 #pragma unroll
-          for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {     // this CTA's half of each weight tile, into both CTAs
-            if (b >= nB) break;
-            const uint32_t e = ((b < 4) ? r1.x : r1.y) >> (8 * (b & 3));
-            ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+            for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {     // this CTA's half of each weight tile, into both CTAs
+              if (b >= nB) break;
+              const uint32_t e = ((b < 4) ? r1.x : r1.y) >> (8 * (b & 3));
+              ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+            }
           }
+          __syncwarp();
         }
         __syncwarp();
       }
-      __syncwarp();
+      // drain: the last steps' "consumed" signals are otherwise never observed (nobody leaves while MMAs still read smem)
+      for (uint32_t j = it > TC2_NSLOT ? it - TC2_NSLOT : 0; j < it; ++j) ptx::mbar_wait(bar_empty + 8 * (j & (TC2_NSLOT - 1)), (j >> 3) & 1);
     }
-    // drain: the last steps' "consumed" signals are otherwise never observed (nobody leaves while MMAs still read smem)
-    for (uint32_t j = it > TC2_NSLOT ? it - TC2_NSLOT : 0; j < it; ++j) ptx::mbar_wait(bar_empty + 8 * (j & (TC2_NSLOT - 1)), (j >> 3) & 1);
   } else {
     // ===================== consumer warpgroups (warps 0..7) =====================
+    ptx::setmaxnreg_inc<TC2_CONSUMER_REGS>();
     const int wg = warp >> 2, wl = warp & 3;
     const int r_lo = wg * 64 + wl * 16 + (lane >> 2);      // this thread's rows of the 128-row tile: r_lo and r_lo + 8
     float acc[Cfg::ACC_REGS];
 #pragma unroll
     for (int i = 0; i < Cfg::ACC_REGS; ++i) acc[i] = 0.f;
     uint32_t item_count = 0, store_count = 0;
-    int item_e = -1;
-    uint32_t it = 0;
-    for (uint32_t ri = rbeg; ri < rend; ++ri, ++it) {
-      const uint4* rp = reinterpret_cast<const uint4*>(stream_m + ri);
-      const uint4 r0 = __ldg(rp), r1 = __ldg(rp + 1);
-      const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
-      const int nA = (r0.x >> 8) & 0x7, n_ops = (r0.x >> 11) & 0x1F;
-      const uint32_t flags = (r0.x >> 16) & 0x3u;
-      if (flags & 1u) item_e = tc2_item_at(eitems, (int)item_count, pair, n_pairs, n_slots);
+    uint32_t ri = rbeg, it = 0;
+    while (ri < rend) {
+      const int item_e = tc2_item_at(eitems, (int)item_count, pair, n_pairs, n_slots);
+      // MMA record of the next step, loaded one step ahead within the item: no global-load latency between two steps'
+      // MMAs (and no record held in registers across the epilogue)
+      uint4 n0 = __ldg(reinterpret_cast<const uint4*>(stream_m + ri)), n1 = __ldg(reinterpret_cast<const uint4*>(stream_m + ri) + 1);
+      uint32_t flags;
+      do {    // the steps of one item
+        const uint4 r0 = n0, r1 = n1;
+        flags = (r0.x >> 16) & 0x3u;
+        if (!(flags & 2u)) {            // not the item's last step: another step of the item follows
+          const uint4* rp = reinterpret_cast<const uint4*>(stream_m + ri + 1);
+          n0 = __ldg(rp); n1 = __ldg(rp + 1);
+        }
+        const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
+        const int nA = (r0.x >> 8) & 0x7, n_rounds = (r0.x >> 11) & 0x1F;
 #ifdef DGAN_PROBE
-      const long long probe_w0 = clock64();
+        const long long probe_w0 = clock64();
 #endif
-      ptx::mbar_wait(bar_full + 8 * slot, phase);
+        ptx::mbar_wait(bar_full + 8 * slot, phase);
 #ifdef DGAN_PROBE
-      probe_wait_full += clock64() - probe_w0;
-      if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
+        probe_wait_full += clock64() - probe_w0;
+        if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
 #endif
-      const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
-      const uint64_t da0 = make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u);   // this warpgroup's 64 rows of the A tiles
-      const uint64_t db0 = make_smem_desc_sw128(sa + (uint32_t)nA * TC_A_BYTES);
-      uint32_t w0 = r0.z, w1 = r0.w, w2 = r1.x, w3 = r1.y, w4 = r1.z, w5 = r1.w;
-      ptx::fence_operands(acc);
-      ptx::wgmma_fence();
-      for (int oi = 0; oi < n_ops; ++oi) {
-        const uint32_t e = (oi & 1) ? (w0 >> 16) : (w0 & 0xFFFFu);
-        if (oi & 1) { w0 = w1; w1 = w2; w2 = w3; w3 = w4; w4 = w5; }
-        // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
-        const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(TC_A_BYTES >> 4));
-        const uint64_t db = db0 + (uint64_t)(((e >> 2) & 7u) * (uint32_t)(B_TILE >> 4));
-        tc2_mma_op<N_TILE, Cfg::MAXB, Cfg::MAXG>(acc, (int)((e >> 7) & 7u), (int)((e >> 5) & 3u) + 1, da, db, (e >> 10) & 1u);
-      }
-      ptx::wgmma_commit();
+        const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
+        const uint64_t da0 = make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u);   // this warpgroup's 64 rows of the A tiles
+        const uint32_t sb = sa + (uint32_t)nA * TC_A_BYTES;
+        const uint64_t db0 = make_smem_desc_sw128(sb);
+        const uint32_t zoff = (zero_base - sb) >> 4;    // zero tile after the ring: always above the step's B slots
+        uint32_t q[6] = {r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+        ptx::fence_operands(acc);
+        ptx::wgmma_fence();
+        for (int r = 0; r < n_rounds; ++r) {
+          tc2_mma_round<N_TILE, Cfg::MAXB>(acc, q, da0, db0, zoff);
+          tc2_pop_round<Cfg::MAXB>(q);
+        }
+        ptx::wgmma_commit();
+        // one group stays in flight across steps: with at most this step's group pending, the previous step's has retired
+        ptx::wgmma_wait1();
+        ptx::fence_operands(acc);
+        __syncwarp();
+        // this warp's MMAs no longer read the previous step's region (the previous item's last step was released below)
+        if (!(flags & 1u) && lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
+        ++ri; ++it;
+      } while (!(flags & 2u));
+      // the epilogue reads the registers: wait for all MMAs, then release the item's last step
       ptx::wgmma_wait0();
       ptx::fence_operands(acc);
       __syncwarp();
-      if (lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * slot, (uint32_t)lane);   // this warp's MMAs no longer read the region
-      if (!(flags & 2u)) continue;
+      if (lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
 
       // ---- epilogue of the item: accumulator registers -> (bias | ReLU | mask | last layer) -> global memory.
       //      Register i of accumulator a holds column (i % (N_TILE/2)) / 4 * 8 + (lane % 4) * 2 + (i % 2) of row
@@ -591,13 +647,14 @@ static int tc2_maxb(int N) { return TC2_BUF_COLS / tc2_acc_stride(N); }
 
 // host-side description of one step (same for every row pair; ring offset and dep are filled per CTA-pair stream)
 struct Tc2HostStep {
-  int kc = 0, nA = 0, nB = 0, n_ops = 0;
+  int kc = 0, nA = 0, nB = 0, n_rounds = 0;
   int a_pix[TC2_MAX_A] = {0, 0, 0, 0};
   uint8_t b_ent[TC2_MAX_BSLOTS] = {0};   // weight tile per B slot
-  uint16_t ops[TC2_MAX_OPS] = {0};
-  int n_tile_mmas = 0;         // un-merged count (statistics)
+  uint8_t ops[TC2_OP_BYTES] = {0};       // [round][accumulator] record bytes
+  int n_real = 0;              // ops that do not read the zero tile (statistics)
   int bytes = 0;               // operand bytes staged per CTA
 };
+constexpr uint8_t TC2_PAD_OP = (uint8_t)(TC2_ZERO_SLOT << 2);   // A tile 0 x zero tile, accumulate
 struct Tc2HostItem {
   TcItem2 hdr{};
   std::vector<Tc2HostStep> steps;
@@ -606,9 +663,10 @@ struct Tc2HostItem {
 
 // Steps of one window (accumulator a <-> output pixel qs[a]).  Input pixels are taken in ascending order and packed
 // greedily into steps of <= max_a A tiles (max_a = 1: one input pixel per step); a weight tile needed by several
-// pixels of a step is staged once.  Within a pixel, runs of consecutive accumulators whose tiles nobody else in
-// the step uses (and whose first-MMA flags agree) become one merged-N MMA.
-static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int N, int K, int max_g, int max_a,
+// pixels of a step is staged once.  The kernel issues a step as rounds of max_b MMAs, one per accumulator slot of the
+// instantiation: an accumulator's r-th contribution in the step (pixel order) goes to round r, and a slot with nothing
+// to add in a round - or beyond the window's accumulators - reads the zero tile.
+static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int N, int K, int max_b, int max_a,
                            int step_max_bytes, Tc2HostItem* out) {
   const int kch = K / 64, b_tile = N * 128;
   out->hdr = TcItem2{};
@@ -630,81 +688,72 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     std::stable_sort(g.second.begin(), g.second.end(), [](const auto& l, const auto& r) { return l.second < r.second; });
   // a pixel with more entries than one step can hold is split (Linear layers: 16 tiles per input "pixel")
   std::vector<std::pair<int, std::vector<std::pair<int, int>>>> px;
-  const int ent_cap = std::min({TC2_MAX_BSLOTS, TC2_MAX_OPS, std::max(1, (step_max_bytes - TC_A_BYTES) / b_tile)});
+  const int ent_cap = std::min(TC2_MAX_BSLOTS, std::max(1, (step_max_bytes - TC_A_BYTES) / b_tile));
   for (auto& g : by_p)
     for (size_t b0 = 0; b0 < g.second.size(); b0 += (size_t)ent_cap)
       px.push_back({g.first, std::vector<std::pair<int, int>>(g.second.begin() + b0,
                                                                g.second.begin() + std::min(g.second.size(), b0 + (size_t)ent_cap))});
+  const int max_rounds = TC2_OP_BYTES / max_b;
   // ---- phase 1: greedy groups (each step stages its own weight tiles: re-using the previous step's would save bytes but
-  //      hold ring capacity and split merged-N MMAs).
-  struct Group { size_t i0, i1; std::vector<int> staged; };
+  //      hold ring capacity).
+  struct Group { size_t i0, i1; };
   std::vector<Group> groups;
   {
     size_t i0 = 0;
     while (i0 < px.size()) {
       size_t i1 = i0;
       std::vector<int> staged;      // tiles this group loads itself
-      int n_ent = 0;
+      int cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // contributions per accumulator = rounds it needs
       auto have = [&](int t) { return std::find(staged.begin(), staged.end(), t) != staged.end(); };
       while (i1 < px.size() && (int)(i1 - i0) < max_a) {
         int fresh = 0;
         std::vector<int> fresh_tiles;
-        for (auto& ta : px[i1].second)
+        int c2[8];
+        std::copy(cnt, cnt + 8, c2);
+        int rounds = 0;
+        for (auto& ta : px[i1].second) {
           if (!have(ta.first) && std::find(fresh_tiles.begin(), fresh_tiles.end(), ta.first) == fresh_tiles.end()) {
             fresh_tiles.push_back(ta.first); ++fresh;
           }
+          ++c2[ta.second];
+        }
+        for (int a = 0; a < 8; ++a) rounds = std::max(rounds, c2[a]);
         const int nA = (int)(i1 - i0) + 1, nB = (int)staged.size() + fresh;
         const bool dup_pixel = (i1 > i0 && px[i1].first == px[i1 - 1].first);   // split halves of one pixel stay apart
-        if (i1 > i0 && (dup_pixel || nB > TC2_MAX_BSLOTS || n_ent + (int)px[i1].second.size() > TC2_MAX_OPS ||
+        if (i1 > i0 && (dup_pixel || nB > TC2_MAX_BSLOTS || rounds > max_rounds ||
                         nA * TC_A_BYTES + nB * b_tile > step_max_bytes))
           break;
         for (int t : fresh_tiles) staged.push_back(t);
-        n_ent += (int)px[i1].second.size();
+        std::copy(c2, c2 + 8, cnt);
         ++i1;
       }
-      groups.push_back({i0, i1, staged});
+      groups.push_back({i0, i1});
       i0 = i1;
     }
   }
-  // ---- phase 2: ops + B slots.  A tile is "single use" (mergeable into an N = g*N_TILE MMA) only if no other pixel of
-  //      its group needs it on its own.
+  // ---- phase 2: B slots + the [round][accumulator] ops
   uint32_t seen = 0;
   for (size_t gi = 0; gi < groups.size(); ++gi) {
     const Group& G = groups[gi];
-    std::vector<int> use(32, 0);
-    for (size_t i = G.i0; i < G.i1; ++i)
-      for (auto& ta : px[i].second) ++use[ta.first];
     Tc2HostStep st;
     st.nA = (int)(G.i1 - G.i0);
-    int slot_of[32];
+    std::fill(st.ops, st.ops + TC2_OP_BYTES, TC2_PAD_OP);
+    int slot_of[32], cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (int t = 0; t < 32; ++t) slot_of[t] = -1;
     for (size_t i = G.i0; i < G.i1; ++i) {
       st.a_pix[i - G.i0] = px[i].first;
-      const auto& ent = px[i].second;
-      for (size_t e = 0; e < ent.size();) {
-        const int acc0 = ent[e].second, t0 = ent[e].first;
-        const bool f0 = !(seen & (1u << acc0));
-        size_t g = 1;
-        int slot;
-        if (use[t0] == 1) {
-          while ((int)g < max_g && e + g < ent.size() && ent[e + g].second == acc0 + (int)g && use[ent[e + g].first] == 1 &&
-                 std::find(G.staged.begin(), G.staged.end(), ent[e + g].first) != G.staged.end() &&
-                 (!(seen & (1u << ent[e + g].second))) == f0)
-            ++g;
-          slot = st.nB;
-          for (size_t jj = 0; jj < g; ++jj) st.b_ent[slot + jj] = (uint8_t)(ent[e + jj].first & 0x1F);   // W_0, W_1, ...
-          st.nB += (int)g;
-        } else if (slot_of[t0] >= 0) {
-          slot = slot_of[t0];
-        } else {
-          slot = slot_of[t0] = st.nB;
-          st.b_ent[slot] = (uint8_t)(t0 & 0x1F);
-          st.nB += 1;
+      for (auto& ta : px[i].second) {
+        const int t = ta.first, acc = ta.second;
+        if (slot_of[t] < 0) {
+          slot_of[t] = st.nB;
+          st.b_ent[st.nB++] = (uint8_t)(t & 0x1F);
         }
-        st.ops[st.n_ops++] = (uint16_t)((i - G.i0) | (slot << 2) | ((g - 1) << 5) | (acc0 << 7) | ((f0 ? 1 : 0) << 10));
-        st.n_tile_mmas += (int)g;
-        for (size_t jj = 0; jj < g; ++jj) seen |= 1u << ent[e + jj].second;
-        e += g;
+        const bool first = !(seen & (1u << acc));
+        const int r = cnt[acc]++;
+        st.ops[r * max_b + acc] = (uint8_t)((i - G.i0) | (slot_of[t] << 2) | ((first ? 1 : 0) << 6));
+        st.n_rounds = std::max(st.n_rounds, r + 1);
+        st.n_real += 1;
+        seen |= 1u << acc;
       }
     }
     st.bytes = st.nA * TC_A_BYTES + st.nB * b_tile;
@@ -718,7 +767,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     for (size_t gi = 0; gi < n_groups; ++gi) {
       Tc2HostStep sk = out->steps[gi];
       sk.kc = kc;
-      for (int o = 0; o < sk.n_ops; ++o) sk.ops[o] &= (uint16_t)~(1u << 10);
+      for (int o = 0; o < TC2_OP_BYTES; ++o) sk.ops[o] &= (uint8_t)~(1u << 6);
       out->steps.push_back(sk);
     }
   out->stage_bytes = 0.0;
@@ -781,19 +830,21 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   std::vector<TcRec> stream_p, stream_m;
   std::vector<uint32_t> stream_off;
   std::vector<int> eitems;
-  long long n_mma = 0, n_single = 0, n_steps = 0, n_bytes = 0;
+  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;   // 64-channel MMA ops issued, those reading the zero tile
   double load_max = 0.0, load_mean = 0.0;   // cost-model load of the busiest CTA pair / the mean over pairs (balance of the LPT assignment)
 };
 
 static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int n_mpairs, int n_pairs,
                     int ring_bytes, Tc2Plan* plan) {
-  const int max_g = (N >= 64) ? std::min(4, 256 / N) : 1;      // merged-N MMAs (see TC2_MAX_A above)
+  const int max_b = tc2_maxb(N);        // accumulator slots of the kernel instantiation: MMAs per round
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
-  // forward: 8 KB weight tiles) packs 3 activation tiles and their taps into 64 KB steps.
+  // forward: 8 KB weight tiles) packs 3 activation tiles and their taps into steps of up to 64 KB.  Three steps always
+  // fit the ring, so a step's region never overlaps the previous step's: that one is released only after this step's
+  // MMAs have been issued.
   const int step_kb = (N == 64 && K == 128) ? DGAN_STEP_MAX_KB_N64 : DGAN_STEP_MAX_KB;
-  const int step_max = std::min((ring_bytes / 2) & ~1023, step_kb * 1024);
+  const int step_max = std::min((ring_bytes / 3) & ~1023, step_kb * 1024);
   double best_cost = 1e300;
   int best_shape[4] = {1, 1, 1, 1};
   std::vector<Tc2HostItem> best_items;
@@ -806,7 +857,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
           if (wh * ww > max_acc || wh > h_grid || ww > std::max(w_grid, 1)) continue;
           tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
           std::vector<Tc2HostItem> items(wins.size());
-          for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, max_g, max_a, step_max, &items[i]);
+          for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, max_b, max_a, step_max, &items[i]);
           std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
           std::vector<double> icost(items.size());
           for (size_t i = 0; i < items.size(); ++i)
@@ -887,7 +938,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   std::vector<TcRec>& stream_p = plan->stream_p;
   std::vector<TcRec>& stream_m = plan->stream_m;
   stream_p.clear(); stream_m.clear();
-  long long n_mma = 0, n_single = 0, n_steps = 0, n_bytes = 0;
+  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;
   for (size_t pr = 0; pr < best_lists.size(); ++pr) {
     stream_off[pr] = (uint32_t)stream_m.size();
     // circular operand ring of this CTA pair: sequential allocation, wrap when the step does not fit
@@ -913,11 +964,13 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
           const auto& rg = region[(size_t)(kidx - d)];
           if (rg.first < end && beg < rg.second) { dep = d; break; }
         }
+        if (dep == 1 && j > 0) { set_error("tensor-core step overlaps the step before it (ring too small)"); return DGAN_ERR_UNSUPPORTED; }
         region.push_back({beg, end});
         const uint32_t flags = (j == 0 ? 1u : 0u) | (j + 1 == itm.steps.size() ? 2u : 0u);
         TcRec rm{};
-        rm.w[0] = (uint32_t)beg | ((uint32_t)hs.nA << 8) | ((uint32_t)hs.n_ops << 11) | (flags << 16);
-        for (int o = 0; o < hs.n_ops; ++o) rm.w[2 + o / 2] |= (uint32_t)hs.ops[o] << (16 * (o & 1));
+        rm.w[0] = (uint32_t)beg | ((uint32_t)hs.nA << 8) | ((uint32_t)hs.n_rounds << 11) | (flags << 16);
+        rm.w[1] = (uint32_t)max_b;
+        for (int o = 0; o < hs.n_rounds * max_b; ++o) rm.w[2 + o / 4] |= (uint32_t)hs.ops[o] << (8 * (o & 3));
         stream_m.push_back(rm);
         TcRec rp{};
         rp.w[0] = (uint32_t)beg | ((uint32_t)hs.kc << 8) | ((uint32_t)hs.nA << 12) | ((uint32_t)hs.nB << 15) | ((uint32_t)dep << 19);
@@ -926,14 +979,15 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         for (int b = 0; b < hs.nB; ++b) rp.w[4 + b / 4] |= (uint32_t)hs.b_ent[b] << (8 * (b & 3));
         stream_p.push_back(rp);
         // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
-        n_mma += hs.n_ops; n_single += hs.n_tile_mmas; n_steps += 1; n_bytes += 2LL * hs.nA * TC_A_BYTES + (long long)hs.nB * N * 128;
+        n_mma += hs.n_rounds * max_b; n_pad += hs.n_rounds * max_b - hs.n_real;
+        n_steps += 1; n_bytes += 2LL * hs.nA * TC_A_BYTES + (long long)hs.nB * N * 128;
       }
     }
   }
   stream_off[(size_t)n_pairs] = (uint32_t)stream_m.size();
   plan->hdrs.resize(best_items.size());
   for (size_t i = 0; i < best_items.size(); ++i) plan->hdrs[i] = best_items[i].hdr;
-  plan->n_mma = n_mma; plan->n_single = n_single; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
+  plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
   return 0;
 }
 
@@ -944,8 +998,11 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //  * the first MMA into an accumulator - and only that one - overwrites it;
 //  * every accumulator sums in the canonical order (k-chunk major, input pixel ascending): results then do not
 //    depend on the schedule (batch-size / sharding invariance);
+//  * an op that reads the zero tile never overwrites its accumulator;
 //  * ring safety: when a step's loads may start (step k - dep consumed), no earlier step that can still be read
 //    overlaps its region, regions stay inside the ring, dep <= number of barrier slots;
+//  * progress: a step's region is released only once the next step's MMAs are issued (unless it ends its item), so
+//    no step inside an item may wait for the step right before it (dep >= 2);
 //  * every (window, row pair) item is assigned to exactly one CTA pair.
 static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int ring_bytes, const Tc2Plan& pl, std::string* err) {
   auto fail = [&](const std::string& m) { *err = m; return DGAN_ERR_INVALID_ARG; };
@@ -984,8 +1041,10 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
       if (dep < 1 || dep > TC2_NSLOT) return fail("dep out of range");
       for (int b = 0; b < 8; ++b) st.b[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3)));
       const uint32_t flags = (m.w[0] >> 16) & 3u;
-      const int n_ops = (int)((m.w[0] >> 11) & 0x1F);
-      if (n_ops > TC2_MAX_OPS) return fail("too many ops in a step");
+      const int n_rounds = (int)((m.w[0] >> 11) & 0x1F);
+      if ((int)m.w[1] != max_acc) return fail("MMA record for another instantiation (accumulators per round)");
+      if (n_rounds < 1 || n_rounds * max_acc > TC2_OP_BYTES) return fail("round count out of range");
+      if (dep == 1 && !(flags & 1u)) return fail("ring deadlock: a step waits for the step before it, which is released only after it");
       if (flags & 1u) {
         if (in_item) return fail("item starts inside an item");
         in_item = true; ++item_k;
@@ -1002,33 +1061,29 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
       if (!in_item) return fail("step outside an item");
       if ((int)(p0.w[1] & 0xFFFF) != mp) return fail("row pair of a step differs from its item");
       const TcItem2& hdr = pl.hdrs[win];
-      for (int oi = 0; oi < n_ops; ++oi) {
-        const uint32_t e = (m.w[2 + oi / 2] >> (16 * (oi & 1))) & 0xFFFFu;
-        const int a_idx = e & 3, slot = (e >> 2) & 7, g = ((e >> 5) & 3) + 1, acc0 = (e >> 7) & 7;
-        const bool first = (e >> 10) & 1, prev = (e >> 11) & 1;
+      // the kernel issues round by round, accumulator 0 .. max_acc - 1 within a round
+      for (int oi = 0; oi < n_rounds * max_acc; ++oi) {
+        const uint32_t e = (m.w[2 + oi / 4] >> (8 * (oi & 3))) & 0xFFu;
+        const int a_idx = e & 3, slot = (e >> 2) & 0xF, acc = oi % max_acc;
+        const bool first = (e >> 6) & 1;
+        if (e & 0x80u) return fail("op field out of range");
+        if (slot == TC2_ZERO_SLOT) {
+          if (max_acc == 1) return fail("zero-tile op in an instantiation without a zero tile");
+          if (first) return fail("zero-tile op overwrites its accumulator");
+          continue;
+        }
         if (a_idx >= nA) return fail("op reads an A tile the step does not stage");
-        if (acc0 + g > (int)hdr.n_acc) return fail("op writes past the window's accumulators");
-        if (g > 1 && (acc_stride != N || g * N > 256)) return fail("merged MMA too wide");
+        if (acc >= (int)hdr.n_acc) return fail("op writes past the window's accumulators");
+        if (slot >= nB) return fail("op reads a B slot the step does not stage");
+        if (st.b[slot] & 0xE0) return fail("weight tile entry out of range");
         const int p = (int)((p0.w[2 + a_idx / 2] >> (16 * (a_idx & 1))) & 0xFFFF);
-        int tiles[4];
-        if (prev) return fail("op refers to a previous step's weight tiles (not supported)");
-        {
-          if (slot + g > nB) return fail("op reads a B slot the step does not stage");
-          for (int i = 0; i < g; ++i) {
-            if (st.b[slot + i] & 0xE0) return fail("weight tile entry out of range");
-            tiles[i] = st.b[slot + i];
-          }
-        }
-        for (int i = 0; i < g; ++i) {
-          const int acc = acc0 + i;
-          const bool unseen = !(seen & (1u << acc));
-          if (first != unseen) return fail(first ? "overwrite of a live accumulator" : "accumulate into an uninitialised accumulator");
-          const std::pair<int, int> kp{st.kc, p};
-          if (!(last_kp[acc] < kp)) return fail("accumulation order is not canonical (k-chunk major, pixel ascending)");
-          last_kp[acc] = kp;
-          contrib[acc].push_back({p * 32 + tiles[i], st.kc});
-        }
-        for (int i = 0; i < g; ++i) seen |= 1u << (acc0 + i);
+        const bool unseen = !(seen & (1u << acc));
+        if (first != unseen) return fail(first ? "overwrite of a live accumulator" : "accumulate into an uninitialised accumulator");
+        const std::pair<int, int> kp{st.kc, p};
+        if (!(last_kp[acc] < kp)) return fail("accumulation order is not canonical (k-chunk major, pixel ascending)");
+        last_kp[acc] = kp;
+        contrib[acc].push_back({p * 32 + st.b[slot], st.kc});
+        seen |= 1u << acc;
       }
       // ring safety
       for (int c = k - 1; c >= 0 && c >= k - 4 * TC2_NSLOT; --c) {
