@@ -860,25 +860,33 @@ int dgan_destroy(dgan_handle h) {
 // fp16 path: plan and upload the schedules of every layer-direction for this many latent rows (cached in the handle).
 // Planning allocates and synchronises; it happens here - a caller needs the workspace size before its first
 // dgan_reconstruct of a batch size anyway - so that dgan_reconstruct itself only enqueues kernels.
+struct TcDir { const TcWeights* w1; TcWeights2* w2; int epi, out_bytes; };
+// The tensor-core layer-directions of the fp16 path with the epilogue and output type they launch with, in the order of
+// plan_dirs: layer l forward, layer l backward, ..., last layer forward, last layer backward.
+static std::vector<TcDir> tc_dirs(dgan_ctx* c) {
+  std::vector<TcDir> dirs;
+  const int nl = (int)c->layers.size();
+  for (int l = 0; l < nl; ++l) {
+    GemmLayer& L = c->layers[(size_t)l];
+    const bool bn = L.bn_scale != nullptr;        // BN layers: float epilogue (fp32 pre-activations), see run_forward
+    dirs.push_back({&L.tc_f, &L.tc2_f, (L.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2});
+    if (l == 0) dirs.push_back({&L.tc_b, &L.tc2_b, EPI_NONE, 4});
+    else dirs.push_back({&L.tc_b, &L.tc2_b, c->layers[(size_t)l - 1].relu ? EPI_MASK : EPI_NONE, 2});
+  }
+  dirs.push_back({&c->tc_fin.f, &c->tc2_fin_f, c->tc_fin.C_out == 1 ? EPI_FINAL_SIGMOID1 : EPI_FINAL_TANH3, 2});
+  dirs.push_back({&c->tc_fin.b, &c->tc2_fin_b, c->layers[(size_t)nl - 1].relu ? EPI_MASK : EPI_NONE, 2});
+  return dirs;
+}
+
 static int plan_all(dgan_ctx* c, int n_rows) {
   if (c->desc.precision != DGAN_PREC_FP16) return 0;
   const int n_pad = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile), n_mpairs = n_pad / (2 * kRowTile);
   const int n_pairs = c->tc.num_sms / 2;
   const Tc2Schedule* sc = nullptr;
   int rc;
-  auto one = [&](const TcWeights& w1, const TcWeights2& w2, int epi, int out_bytes) {
-    return tc2_get_schedule(c->tc, w1, w2, n_mpairs, n_pairs, tc2_ring_bytes(w1.N, epi, out_bytes), c->tc.allocs, (cudaStream_t)0, &sc);
-  };
-  const int nl = (int)c->layers.size();
-  for (int l = 0; l < nl; ++l) {
-    const GemmLayer& L = c->layers[(size_t)l];
-    const bool bn = L.bn_scale != nullptr;        // BN layers: float epilogue (fp32 pre-activations), see run_forward
-    if ((rc = one(L.tc_f, L.tc2_f, (L.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2))) return rc;
-    if (l == 0) { if ((rc = one(L.tc_b, L.tc2_b, EPI_NONE, 4))) return rc; }
-    else if ((rc = one(L.tc_b, L.tc2_b, c->layers[(size_t)l - 1].relu ? EPI_MASK : EPI_NONE, 2))) return rc;
-  }
-  if ((rc = one(c->tc_fin.f, c->tc2_fin_f, c->tc_fin.C_out == 1 ? EPI_FINAL_SIGMOID1 : EPI_FINAL_TANH3, 2))) return rc;
-  return one(c->tc_fin.b, c->tc2_fin_b, c->layers[(size_t)nl - 1].relu ? EPI_MASK : EPI_NONE, 2);
+  for (const TcDir& d : tc_dirs(c))
+    if ((rc = tc2_get_schedule(c->tc, *d.w1, *d.w2, n_mpairs, n_pairs, d.epi, d.out_bytes, c->tc.allocs, (cudaStream_t)0, &sc))) return rc;
+  return 0;
 }
 
 size_t dgan_workspace_bytes(dgan_handle h, int batch, int rec_rr) {
@@ -1085,9 +1093,8 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     if (dr.N != 16 && dr.N != 48 && dr.N != 64 && dr.N != 128 && dr.N != 256) { set_error(dr.name + ": unsupported N"); return DGAN_ERR_UNSUPPORTED; }
     int max_acc = tc2_maxb(dr.N);
     if (dr.force_acc > 0) max_acc = std::min(max_acc, dr.force_acc);
-    const int ring = tc2_ring_bytes(dr.N, dr.epi, dr.out_bytes);
     Tc2Plan plan;
-    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, n_mpairs, n_pairs, ring, &plan);
+    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
     // self-test of the validator: damage the plan of Generator.3 fwd in one specific way; the check must then fail
     if (mutate != 0 && dr.name == "Generator.3.fwd" && plan.stream_m.size() > 40) {
@@ -1117,15 +1124,67 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
         case 9: std::swap(plan.stream_m[20], plan.stream_m[21]);            // two steps out of order
                 std::swap(plan.stream_p[20], plan.stream_p[21]);
                 break;
+        case 10: plan.maxb = 3;                                              // slots per round without an instantiation
+                 for (TcRec& r : plan.stream_m) r.w[1] = 3;
+                 break;
+        case 11: for (TcRec& r : plan.stream_m) r.w[1] = 2;                 // records disagree with the plan's slots
+                 break;
         default: break;
       }
     }
     std::string err;
-    if ((rc = tc2_check_plan(dr.N, dr.K, dr.tab, n_mpairs, ring, plan, &err))) { set_error(dr.name + ": " + err); return rc; }
+    if ((rc = tc2_check_plan(dr.N, dr.K, dr.tab, n_mpairs, dr.epi, dr.out_bytes, plan, &err))) { set_error(dr.name + ": " + err); return rc; }
+    if (mutate != 0) continue;
+    // the plans dgan_debug_force_slots can select: every other slot count this direction has an instantiation for
+    for (const Tc2Kind& k : kTc2Kinds) {
+      if (k.n != dr.N || k.epi != dr.epi || k.out_bytes != dr.out_bytes || k.maxb == plan.maxb) continue;
+      Tc2Plan forced;
+      if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &forced))) {
+        set_error(dr.name + " (" + std::to_string(k.maxb) + " slots): " + dgan_last_error());
+        return rc;
+      }
+      if ((rc = tc2_check_plan(dr.N, dr.K, dr.tab, n_mpairs, dr.epi, dr.out_bytes, forced, &err))) {
+        set_error(dr.name + " (" + std::to_string(k.maxb) + " slots): " + err);
+        return rc;
+      }
+    }
   }
   return 0;
 }
 
+
+// Host-side test aid (not in the public header): plan layer-direction `dir` (plan_dirs order) of an fp16 handle with
+// exactly `maxb` accumulator slots per round from now on (0: the planner chooses again).  Schedules and captured loops
+// are re-made on the next call, so any instantiation of TC2_KINDS can be run at any batch size; the results must not
+// change, because every accumulator keeps its summation order.
+int dgan_debug_force_slots(dgan_handle h, int dir, int maxb) {
+  if (h == nullptr || h->desc.precision != DGAN_PREC_FP16 || maxb < 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
+  const std::vector<TcDir> dirs = tc_dirs(h);
+  if (dir < 0 || dir >= (int)dirs.size()) { set_error("layer-direction out of range"); return DGAN_ERR_INVALID_ARG; }
+  const TcDir& d = dirs[(size_t)dir];
+  if (maxb > 0 && !tc2_has_kind(d.w1->N, maxb, d.epi, d.out_bytes)) {
+    set_error("no kernel instantiation with " + std::to_string(maxb) + " accumulator slots per round for this layer-direction");
+    return DGAN_ERR_UNSUPPORTED;
+  }
+  d.w2->force_maxb = maxb;
+  d.w2->by_mpairs.clear();                  // the uploaded tables stay in h->allocs until dgan_destroy
+  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  h->graphs.clear();
+  return DGAN_OK;
+}
+
+// Host-side test aid: the accumulator slots per round the instantiations of TC2_KINDS offer for layer-direction `dir`,
+// written to out[0 .. n).  Returns n, or -1.
+int dgan_debug_slot_choices(dgan_handle h, int dir, int* out, int max_n) {
+  if (h == nullptr || h->desc.precision != DGAN_PREC_FP16 || out == nullptr) return -1;
+  const std::vector<TcDir> dirs = tc_dirs(h);
+  if (dir < 0 || dir >= (int)dirs.size()) return -1;
+  const TcDir& d = dirs[(size_t)dir];
+  int n = 0;
+  for (const Tc2Kind& k : kTc2Kinds)
+    if (k.n == d.w1->N && k.epi == d.epi && k.out_bytes == d.out_bytes && n < max_n) out[n++] = k.maxb;
+  return n;
+}
 
 #ifdef DGAN_PROBE
 // Developer build only: copy (and clear) the per-CTA cycle counters of the tensor-core kernels.  out: [48][160][8] u64.
@@ -1139,28 +1198,33 @@ int dgan_debug_probe_read(unsigned long long* out) {
 #endif
 
 // Host-only developer aid (not in the public header): the plan of every layer-direction in numbers - window shape, items,
-// steps, MMAs, operand bytes staged from L2 into shared memory (both CTAs of every pair) - as text.  Returns the length.
-int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {
+// steps, MMAs, operand bytes staged from L2 into shared memory (both CTAs of every pair), accumulator slots per round -
+// as text.  Layer-direction `force_dir` (plan_dirs order; -1: none) is planned with exactly `force_maxb` slots per
+// round, as dgan_debug_force_slots would.  Returns the length.
+int dgan_debug_plan_stats_slots(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, char* buf, int buf_len) {
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
   std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load"
-                    " | zero-tile MMA %\n";
+                    " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us\n";
   double total = 0.0;
-  for (const PlanDir& dr : plan_dirs(d)) {
+  const std::vector<PlanDir> dirs = plan_dirs(d);
+  for (size_t di = 0; di < dirs.size(); ++di) {
+    const PlanDir& dr = dirs[di];
     int max_acc = tc2_maxb(dr.N);
     if (dr.force_acc > 0) max_acc = std::min(max_acc, dr.force_acc);
     Tc2Plan plan;
-    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, n_mpairs, n_pairs,
-                            tc2_ring_bytes(dr.N, dr.epi, dr.out_bytes), &plan);
+    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, (int)di == force_dir ? force_maxb : 0, dr.epi, dr.out_bytes,
+                            n_mpairs, n_pairs, &plan);
     if (rc) return -1;
     char line[256];
     const double mb = (double)plan.n_bytes / 1e6;
     total += mb;
-    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f\n", dr.name.c_str(), dr.N, dr.K,
-             plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,
+    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f | %d | %.1f | %.1f\n", dr.name.c_str(),
+             dr.N, dr.K, plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,
              plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0),
-             100.0 * (double)plan.n_pad / (double)std::max(plan.n_mma, 1LL));
+             100.0 * (double)plan.n_pad / (double)std::max(plan.n_mma, 1LL), plan.maxb, plan.op_ns_max / 1e3,
+             plan.load_max / 1e3);
     out += line;
   }
   char line[64];
@@ -1170,6 +1234,10 @@ int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf
   memcpy(buf, out.data(), (size_t)n);
   buf[n] = 0;
   return n;
+}
+
+int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {
+  return dgan_debug_plan_stats_slots(d, n_rows, n_pairs, -1, 0, buf, buf_len);
 }
 
 }  // extern "C"

@@ -17,6 +17,7 @@
 //     the step's own group has retired; after the item's last step the consumer waits for all MMAs and runs the
 //     epilogue straight from the registers.  Each consumer warp stores the 16 rows it holds with its own TMA store.
 #pragma once
+#include <type_traits>
 #include "kernels_tc.cuh"
 
 namespace dgan {
@@ -84,28 +85,54 @@ __host__ __device__ constexpr int tc2_epi_tiles(int n_tile, int epi, int out_byt
   return tc2_tma_epilogue(n_tile, epi, out_bytes) ? 2 : 0;
 }
 // The all-zero weight tile read by the MMAs of an accumulator with nothing to add in a round (instantiations with more
-// than one accumulator per window).  It sits right after the ring and is written once per CTA.
-__host__ __device__ constexpr int tc2_zero_bytes(int n_tile) {
-  return TC2_BUF_COLS / tc2_acc_stride(n_tile) > 1 ? n_tile * 128 : 0;
-}
-__host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int epi, int out_bytes) {
+// than one accumulator per round).  It sits right after the ring and is written once per CTA.
+__host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb) { return maxb > 1 ? n_tile * 128 : 0; }
+__host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
-  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile)) / 1024) * 1024;
+  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb)) / 1024) * 1024;
   return raw > 255 * 1024 ? 255 * 1024 : raw;
 }
 
-template <int N_TILE, int EPI = EPI_NONE, int OUT_BYTES = 2>
+// MAXB_: accumulator slots of the instantiation = MMAs per round = the most accumulators a window may have.  Fewer slots
+// than fit the 256 accumulator columns issue fewer zero-tile MMAs but allow only smaller windows (more staged bytes);
+// the planner weighs the two (tc2_plan).
+template <int N_TILE, int MAXB_, int EPI = EPI_NONE, int OUT_BYTES = 2>
 struct Tc2Cfg {
+  static_assert(MAXB_ >= 1 && MAXB_ <= TC2_BUF_COLS / tc2_acc_stride(N_TILE), "more accumulator slots than columns");
   static constexpr int B_TILE = N_TILE * 128;                             // bytes of one staged weight tile
-  static constexpr int MAXB = TC2_BUF_COLS / tc2_acc_stride(N_TILE);      // = accumulators per window (8 / 4 / 2 / 1)
+  static constexpr int MAXB = MAXB_;
   static constexpr int ACC_REGS = MAXB * N_TILE / 2;                      // accumulator registers per consumer thread
   static constexpr bool TMA_EPI = tc2_tma_epilogue(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_TILES = tc2_epi_tiles(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_BYTES = EPI_TILES * TC2_TILE_BYTES;
-  static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE);
-  static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, EPI, OUT_BYTES);          // operand ring (offsets are 8-bit KB)
+  static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE, MAXB);
+  static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, MAXB, EPI, OUT_BYTES);    // operand ring (offsets are 8-bit KB)
   static constexpr int SMEM_BYTES = RING_BYTES + ZERO_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
 };
+
+// Every instantiation of tc_bsgemm2_kernel: (N, accumulator slots per round, epilogue, output type).  tc2_optin_all,
+// the launch dispatch and the planner's candidate set (tc2_plan) all read this list.  For each (N, epilogue, output
+// type) it holds the largest slot count, which every window shape can use, and the smaller ones the planner picks for
+// the shipped generators.
+#define TC2_KINDS(X)                                                                                                   \
+  X(256, 1, EPI_BIAS_RELU, __half) X(256, 1, EPI_BIAS, __half) X(256, 1, EPI_MASK, __half) X(256, 1, EPI_NONE, __half) \
+  X(256, 1, EPI_NONE, float) X(256, 1, EPI_BIAS, float)                                                                \
+  X(128, 2, EPI_BIAS_RELU, __half) X(128, 2, EPI_BIAS, __half) X(128, 2, EPI_MASK, __half) X(128, 2, EPI_NONE, __half) \
+  X(128, 2, EPI_NONE, float) X(128, 2, EPI_BIAS, float) X(128, 1, EPI_NONE, float)                                    \
+  X(64, 4, EPI_BIAS_RELU, __half) X(64, 4, EPI_BIAS, __half) X(64, 4, EPI_MASK, __half) X(64, 4, EPI_NONE, __half)     \
+  X(64, 4, EPI_NONE, float) X(64, 4, EPI_BIAS, float)                                                                  \
+  X(16, 8, EPI_FINAL_SIGMOID1, __half) X(16, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, EPI_FINAL_TANH3, __half)
+
+struct Tc2Kind { int n, maxb, epi, out_bytes; };
+#define TC2_KIND_ROW(NT, MB, EP, T) {NT, MB, EP, (int)sizeof(T)},
+static constexpr Tc2Kind kTc2Kinds[] = {TC2_KINDS(TC2_KIND_ROW)};
+#undef TC2_KIND_ROW
+// Is there an instantiation with these template arguments?
+static inline bool tc2_has_kind(int n, int maxb, int epi, int out_bytes) {
+  for (const Tc2Kind& k : kTc2Kinds)
+    if (k.n == n && k.maxb == maxb && k.epi == epi && k.out_bytes == out_bytes) return true;
+  return false;
+}
 
 namespace ptx {
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2) {
@@ -225,7 +252,7 @@ __host__ __device__ constexpr int tc2_probe_key(int n_tile, int epi, int out_byt
 }
 #endif
 
-template <int N_TILE, int EPI, typename TOUT>
+template <int N_TILE, int MAXB, int EPI, typename TOUT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC2_THREADS, 1)
 tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const __grid_constant__ CUtensorMap tm_out,
@@ -233,7 +260,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                   const TcRec* __restrict__ stream_m, const __grid_constant__ Tc2Heads heads,
                   const int* __restrict__ eitems, int n_slots,
                   TOUT* __restrict__ out, int n_pad, const float* __restrict__ bias, int bias_pstride, const TcFinalArgs fa) {
-  using Cfg = Tc2Cfg<N_TILE, EPI, (int)sizeof(TOUT)>;
+  using Cfg = Tc2Cfg<N_TILE, MAXB, EPI, (int)sizeof(TOUT)>;
   constexpr bool TMA_EPI = Cfg::TMA_EPI;
   constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3);
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
@@ -635,11 +662,13 @@ struct Tc2Schedule {           // one window tiling of a layer-direction + its i
   int n_slots = 0, n_pairs = 0;
   int n_windows = 0;
   int wh = 0, ww = 0, sy = 1, sx = 1;
+  int maxb = 1;                    // accumulator slots per round: selects the kernel instantiation
 };
 struct TcWeights2 {
   CUtensorMap tm_b;            // box {64, N/2, 1}: the half of a weight tile one CTA of the pair loads
   PairTable tab;               // host copy: schedules are built lazily per batch size
   int h_grid = 0, w_grid = 0, max_acc = 1;
+  int force_maxb = 0;          // > 0: plan with exactly this many accumulator slots per round (dgan_debug_force_slots)
   mutable std::vector<std::pair<int, Tc2Schedule>> by_mpairs;   // chosen schedule per n_mpairs (lazy cache)
 };
 
@@ -659,6 +688,7 @@ struct Tc2HostItem {
   TcItem2 hdr{};
   std::vector<Tc2HostStep> steps;
   double stage_bytes = 0.0;
+  long long n_ops = 0;         // 64-channel MMAs issued (rounds x slots), zero-tile ones included
 };
 
 // Steps of one window (accumulator a <-> output pixel qs[a]).  Input pixels are taken in ascending order and packed
@@ -771,7 +801,8 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
       out->steps.push_back(sk);
     }
   out->stage_bytes = 0.0;
-  for (auto& stp : out->steps) out->stage_bytes += stp.bytes;
+  out->n_ops = 0;
+  for (auto& stp : out->steps) { out->stage_bytes += stp.bytes; out->n_ops += (long long)stp.n_rounds * max_b; }
 }
 
 // Windows of wh x ww accumulators with strides (sy, sx) over the output grid.  Stride 2 gathers outputs of equal
@@ -814,14 +845,31 @@ static int tc2_build_direction(TcState& st, const TcWeights& w1, TcWeights2* w2,
 #ifndef DGAN_COST_FIXED_KB
 #define DGAN_COST_FIXED_KB 48.0
 #endif
+// Time model of an item (DESIGN.md section 3, least-squares fit to per-kernel times on an H100): NS_PER_KB per KB of
+// the cost above (staged bytes + epilogue and fixed charges), OP_NS per 64-channel MMA at N = 64, scaled by
+// max(N, OP_MIN_N) / 64 for other widths, and STEP_NS per step (the consumers' full-barrier wait, wgmma commit and
+// wait, region release and record load of a step).
+#ifndef DGAN_COST_NS_PER_KB
+#define DGAN_COST_NS_PER_KB 6.8
+#endif
+#ifndef DGAN_COST_OP_NS
+#define DGAN_COST_OP_NS 103.0
+#endif
+#ifndef DGAN_COST_STEP_NS
+#define DGAN_COST_STEP_NS 942.0
+#endif
+#ifndef DGAN_COST_OP_MIN_N
+#define DGAN_COST_OP_MIN_N 32
+#endif
 #ifndef TC2_REFINE_BUDGET
 #define TC2_REFINE_BUDGET (1LL << 26)    // candidate evaluations of the assignment refinement per window shape (tc2_plan)
 #endif
 
-// Pick (and build on first use) the window tiling for `n_mpairs` row pairs on `n_pairs` CTA pairs: every candidate
-// shape (wh x ww accumulators, strides 1 or 2) is scored by an LPT assignment of its items (window, row pair) to the
-// CTA pairs with cost = operand bytes staged + a per-accumulator epilogue charge + a fixed per-item charge;
-// the smallest makespan wins.  Then each pair's items are concatenated into its step streams, the circular operand
+// Pick (and build on first use) the accumulator slots per round and the window tiling for `n_mpairs` row pairs on
+// `n_pairs` CTA pairs: every candidate - an instantiation of TC2_KINDS for (N, epilogue, output type) and a shape of
+// wh x ww <= its slots accumulators, strides 1 or 2 - is scored by an LPT assignment of its items (window, row pair)
+// to the CTA pairs with the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed
+// per-item charge, and the MMAs issued, zero-tile ones included); the smallest makespan wins.  Then each pair's items are concatenated into its step streams, the circular operand
 // ring is simulated to give every step its offset and its dependency distance, and everything is uploaded.
 struct Tc2Plan {               // host result of the planner (what tc2_get_schedule uploads)
   int shape[4] = {1, 1, 1, 1};   // wh, ww, sy, sx
@@ -832,11 +880,14 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   std::vector<int> eitems;
   long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;   // 64-channel MMA ops issued, those reading the zero tile
   double load_max = 0.0, load_mean = 0.0;   // cost-model load of the busiest CTA pair / the mean over pairs (balance of the LPT assignment)
+  double op_ns_max = 0.0;      // the MMA term of the busiest pair's load (estimated tensor time, ns)
+  int maxb = 1, ring_bytes = 0;   // accumulator slots per round of the chosen instantiation, its operand ring
 };
 
-static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int n_mpairs, int n_pairs,
-                    int ring_bytes, Tc2Plan* plan) {
-  const int max_b = tc2_maxb(N);        // accumulator slots of the kernel instantiation: MMAs per round
+static double tc2_op_ns(int N) { return DGAN_COST_OP_NS * (double)std::max(N, DGAN_COST_OP_MIN_N) / 64.0; }
+
+static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
+                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan) {
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
@@ -844,24 +895,33 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   // fit the ring, so a step's region never overlaps the previous step's: that one is released only after this step's
   // MMAs have been issued.
   const int step_kb = (N == 64 && K == 128) ? DGAN_STEP_MAX_KB_N64 : DGAN_STEP_MAX_KB;
-  const int step_max = std::min((ring_bytes / 3) & ~1023, step_kb * 1024);
+  const double op_ns = tc2_op_ns(N);
   double best_cost = 1e300;
-  int best_shape[4] = {1, 1, 1, 1};
+  int best_shape[4] = {1, 1, 1, 1}, max_b = 0, ring_bytes = 0;
   std::vector<Tc2HostItem> best_items;
   std::vector<std::vector<int>> best_lists;
   std::vector<std::vector<int>> wins;
+  for (const Tc2Kind& kind : kTc2Kinds) {
+    if (kind.n != N || kind.epi != epi || kind.out_bytes != out_bytes) continue;
+    if (force_maxb > 0 && kind.maxb != force_maxb) continue;
+    const int mb = kind.maxb, ring = tc2_ring_bytes(N, mb, epi, out_bytes);
+    const int step_max = std::min((ring / 3) & ~1023, step_kb * 1024);
   for (int wh = 1; wh <= 2; ++wh)
     for (int ww = 1; ww <= 8; ++ww)
       for (int sy = 1; sy <= (wh > 1 ? 2 : 1); ++sy)
         for (int sx = 1; sx <= (ww > 1 ? 2 : 1); ++sx) {
-          if (wh * ww > max_acc || wh > h_grid || ww > std::max(w_grid, 1)) continue;
+          if (wh * ww > std::min(max_acc, mb) || wh > h_grid || ww > std::max(w_grid, 1)) continue;
           tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
           std::vector<Tc2HostItem> items(wins.size());
-          for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, max_b, max_a, step_max, &items[i]);
-          std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
+          for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, mb, max_a, step_max, &items[i]);
           std::vector<double> icost(items.size());
-          for (size_t i = 0; i < items.size(); ++i)
-            icost[i] = items[i].stage_bytes + DGAN_COST_EPI_KB * 1024.0 * items[i].hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0;
+          auto cost_item = [&](const Tc2HostItem& it) {
+            return DGAN_COST_NS_PER_KB / 1024.0 *
+                       (it.stage_bytes + DGAN_COST_EPI_KB * 1024.0 * it.hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0) +
+                   op_ns * (double)it.n_ops + DGAN_COST_STEP_NS * (double)it.steps.size();
+          };
+          std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
+          for (size_t i = 0; i < items.size(); ++i) icost[i] = cost_item(items[i]);
           // LPT: items (window, mp) largest-first, each to the currently least-loaded CTA pair
           const long long total = (long long)items.size() * n_mpairs;
           std::vector<double> load((size_t)n_pairs, 0.0);
@@ -923,9 +983,19 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
             plan->load_max = makespan;
             plan->load_mean = std::accumulate(load.begin(), load.end(), 0.0) / (double)n_pairs;
             best_shape[0] = wh; best_shape[1] = ww; best_shape[2] = sy; best_shape[3] = sx;
+            max_b = mb; ring_bytes = ring;
+            plan->op_ns_max = 0.0;
+            for (size_t pr = 0; pr < lists.size(); ++pr)
+              if (load[pr] == makespan) {
+                for (int idx : lists[pr]) plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
+                break;
+              }
             best_items.swap(items); best_lists.swap(lists);
           }
         }
+  }
+  if (max_b == 0) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
+  plan->maxb = max_b; plan->ring_bytes = ring_bytes;
   plan->shape[0] = best_shape[0]; plan->shape[1] = best_shape[1]; plan->shape[2] = best_shape[2]; plan->shape[3] = best_shape[3];
   plan->n_pairs = n_pairs;
   size_t n_slots = 0;
@@ -1003,10 +1073,16 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //    overlaps its region, regions stay inside the ring, dep <= number of barrier slots;
 //  * progress: a step's region is released only once the next step's MMAs are issued (unless it ends its item), so
 //    no step inside an item may wait for the step right before it (dep >= 2);
-//  * every (window, row pair) item is assigned to exactly one CTA pair.
-static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int ring_bytes, const Tc2Plan& pl, std::string* err) {
+//  * every (window, row pair) item is assigned to exactly one CTA pair;
+//  * the accumulator slots per round name an instantiation of TC2_KINDS, and every MMA record carries the plan's count
+//    (the launch dispatches on the plan's count, the kernel decodes the records with it).
+static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int epi, int out_bytes, const Tc2Plan& pl,
+                          std::string* err) {
   auto fail = [&](const std::string& m) { *err = m; return DGAN_ERR_INVALID_ARG; };
-  const int kch = K / 64, b_tile = N * 128, acc_stride = tc2_acc_stride(N), max_acc = TC2_BUF_COLS / acc_stride;
+  const int kch = K / 64, b_tile = N * 128;
+  const int max_acc = pl.maxb;
+  if (!tc2_has_kind(N, max_acc, epi, out_bytes)) return fail("no kernel instantiation with these accumulator slots per round");
+  const int ring_bytes = tc2_ring_bytes(N, max_acc, epi, out_bytes);
   const size_t n_pairs = (size_t)pl.n_pairs;
   if (pl.stream_off.size() != n_pairs + 1) return fail("stream_off size");
   if (pl.stream_p.size() != pl.stream_m.size()) return fail("stream sizes differ");
@@ -1042,7 +1118,7 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
       for (int b = 0; b < 8; ++b) st.b[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3)));
       const uint32_t flags = (m.w[0] >> 16) & 3u;
       const int n_rounds = (int)((m.w[0] >> 11) & 0x1F);
-      if ((int)m.w[1] != max_acc) return fail("MMA record for another instantiation (accumulators per round)");
+      if ((int)m.w[1] != max_acc) return fail("MMA record disagrees with the plan on the accumulator slots per round");
       if (n_rounds < 1 || n_rounds * max_acc > TC2_OP_BYTES) return fail("round count out of range");
       if (dep == 1 && !(flags & 1u)) return fail("ring deadlock: a step waits for the step before it, which is released only after it");
       if (flags & 1u) {
@@ -1114,15 +1190,17 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
 }
 
 // Pick (and build on first use) the schedule of one layer-direction for `n_mpairs` row pairs and upload it.
-static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& w2, int n_mpairs, int n_pairs, int ring_bytes,
-                            std::vector<void*>* allocs, cudaStream_t s, const Tc2Schedule** out) {
+static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& w2, int n_mpairs, int n_pairs, int epi,
+                            int out_bytes, std::vector<void*>* allocs, cudaStream_t s, const Tc2Schedule** out) {
   (void)st;
   for (auto& kv : w2.by_mpairs)
     if (kv.first == n_mpairs) { *out = &kv.second; return 0; }
   Tc2Plan plan;
   int rc;
-  if ((rc = tc2_plan(w1.N, w1.K, w2.tab, w2.h_grid, w2.w_grid, w2.max_acc, n_mpairs, n_pairs, ring_bytes, &plan))) return rc;
+  if ((rc = tc2_plan(w1.N, w1.K, w2.tab, w2.h_grid, w2.w_grid, w2.max_acc, w2.force_maxb, epi, out_bytes, n_mpairs, n_pairs, &plan)))
+    return rc;
   Tc2Schedule sc;
+  sc.maxb = plan.maxb;
   sc.wh = plan.shape[0]; sc.ww = plan.shape[1]; sc.sy = plan.shape[2]; sc.sx = plan.shape[3];
   sc.n_windows = (int)plan.hdrs.size(); sc.n_pairs = n_pairs; sc.n_slots = plan.n_slots;
   if ((rc = tc_upload(allocs, plan.hdrs.data(), plan.hdrs.size() * sizeof(TcItem2), (void**)&sc.items, s))) return rc;
@@ -1136,21 +1214,15 @@ static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& 
   return 0;
 }
 
-template <int NT, int EP, typename TOUT>
+template <int NT, int MB, int EP, typename TOUT>
 static cudaError_t tc2_optin() {
-  return cudaFuncSetAttribute(tc_bsgemm2_kernel<NT, EP, TOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              Tc2Cfg<NT, EP, (int)sizeof(TOUT)>::SMEM_BYTES);
+  return cudaFuncSetAttribute(tc_bsgemm2_kernel<NT, MB, EP, TOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              Tc2Cfg<NT, MB, EP, (int)sizeof(TOUT)>::SMEM_BYTES);
 }
 
 static int tc2_optin_all() {
-#define TC2_OPTIN(NT, EP, T) DGAN_CUDA_CHECK((tc2_optin<NT, EP, T>()))
-  TC2_OPTIN(64, EPI_BIAS_RELU, __half); TC2_OPTIN(128, EPI_BIAS_RELU, __half); TC2_OPTIN(256, EPI_BIAS_RELU, __half);
-  TC2_OPTIN(64, EPI_BIAS, __half); TC2_OPTIN(128, EPI_BIAS, __half); TC2_OPTIN(256, EPI_BIAS, __half);
-  TC2_OPTIN(64, EPI_MASK, __half); TC2_OPTIN(128, EPI_MASK, __half); TC2_OPTIN(256, EPI_MASK, __half);
-  TC2_OPTIN(64, EPI_NONE, __half); TC2_OPTIN(128, EPI_NONE, __half); TC2_OPTIN(256, EPI_NONE, __half);
-  TC2_OPTIN(64, EPI_NONE, float); TC2_OPTIN(128, EPI_NONE, float); TC2_OPTIN(256, EPI_NONE, float);
-  TC2_OPTIN(64, EPI_BIAS, float); TC2_OPTIN(128, EPI_BIAS, float); TC2_OPTIN(256, EPI_BIAS, float);   // use_bn: fp32 pre-activations
-  TC2_OPTIN(16, EPI_FINAL_SIGMOID1, __half); TC2_OPTIN(48, EPI_FINAL_TANH3, __half);
+#define TC2_OPTIN(NT, MB, EP, T) DGAN_CUDA_CHECK((tc2_optin<NT, MB, EP, T>()));
+  TC2_KINDS(TC2_OPTIN)
 #undef TC2_OPTIN
   return 0;
 }
@@ -1175,33 +1247,23 @@ static int tc2_launch_impl(TcState& st, int64_t* launches, const TcWeights& w, c
   const int n_mpairs = n_pad / (2 * kRowTile);
   const Tc2Schedule* schp = nullptr;
   const int pairs_avail = st.num_sms / 2;
-  const int ring_bytes = tc2_ring_bytes(w.N, epi, (int)sizeof(TOUT));
-  if ((rc = tc2_get_schedule(st, w, w2m, n_mpairs, pairs_avail, ring_bytes, st.allocs, s, &schp))) return rc;
+  if ((rc = tc2_get_schedule(st, w, w2m, n_mpairs, pairs_avail, epi, (int)sizeof(TOUT), st.allocs, s, &schp))) return rc;
   const Tc2Schedule& w2s = *schp;
   const int grid = 2 * w2s.n_pairs;       // pairs without work find -1 in slot 0 and fall through
   cudaError_t le = cudaSuccess;
-#define TC2_GO(NT, EP)                                                                                                 \
-  le = launch_pdl(tc_bsgemm2_kernel<NT, EP, TOUT>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, EP, (int)sizeof(TOUT)>::SMEM_BYTES, s, \
-                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, bias, w.bias_pstride, fa)
-#define TC2_GO_H(NT, EP)                                                                                               \
-  le = launch_pdl(tc_bsgemm2_kernel<NT, EP, __half>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, EP, 2>::SMEM_BYTES, s,   \
-                  tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, reinterpret_cast<__half*>(out), n_pad, bias, 0, fa)
-#define TC2_BY_N(EP)                    \
-  do {                                  \
-    if (w.N == 64) TC2_GO(64, EP);      \
-    else if (w.N == 128) TC2_GO(128, EP); \
-    else TC2_GO(256, EP);               \
-  } while (0)
-  if (sizeof(TOUT) == 4) { if (epi == EPI_BIAS) TC2_BY_N(EPI_BIAS); else TC2_BY_N(EPI_NONE); }
-  else if (epi == EPI_FINAL_SIGMOID1) { TC2_GO_H(16, EPI_FINAL_SIGMOID1); }
-  else if (epi == EPI_FINAL_TANH3) { TC2_GO_H(48, EPI_FINAL_TANH3); }
-  else if (epi == EPI_BIAS_RELU) { TC2_BY_N(EPI_BIAS_RELU); }
-  else if (epi == EPI_BIAS) { TC2_BY_N(EPI_BIAS); }
-  else if (epi == EPI_MASK) { TC2_BY_N(EPI_MASK); }
-  else { TC2_BY_N(EPI_NONE); }
-#undef TC2_BY_N
+  bool found = false;
+#define TC2_GO(NT, MB, EP, T)                                                                                          \
+  if constexpr (std::is_same<T, TOUT>::value) {                                                                      \
+    if (!found && w.N == NT && w2s.maxb == MB && epi == EP) {                                                         \
+      found = true;                                                                                                   \
+      le = launch_pdl(tc_bsgemm2_kernel<NT, MB, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
+                      tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, \
+                      bias, (EP == EPI_FINAL_SIGMOID1 || EP == EPI_FINAL_TANH3) ? 0 : w.bias_pstride, fa);              \
+    }                                                                                                                 \
+  }
+  TC2_KINDS(TC2_GO)
 #undef TC2_GO
-#undef TC2_GO_H
+  if (!found) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
   (*launches)++;
   cudaError_t e = (le != cudaSuccess) ? le : cudaGetLastError();
   if (e != cudaSuccess) { set_error(std::string("tc_bsgemm2 launch: ") + cudaGetErrorString(e)); return DGAN_ERR_CUDA; }

@@ -1,5 +1,6 @@
 """Developer aid (no GPU needed): print the planner's numbers for every tensor-core layer-direction.
-Usage: python tools/plan_stats.py [mnist|celeba] [batch] [R] [CTA pairs] [library]"""
+Usage: python tools/plan_stats.py [mnist|celeba] [batch] [R] [CTA pairs] [library] [--slots DIR=MAXB]
+--slots plans layer-direction DIR (the row index of the table, from 0) with exactly MAXB accumulator slots per round."""
 import ctypes
 import os
 import sys
@@ -7,6 +8,11 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from defensegan_b200 import _native
 
+force_dir, force_maxb = -1, 0
+if "--slots" in sys.argv:
+    i = sys.argv.index("--slots")
+    force_dir, force_maxb = (int(v) for v in sys.argv[i + 1].split("="))
+    del sys.argv[i:i + 2]
 dataset = sys.argv[1] if len(sys.argv) > 1 else "mnist"
 batch = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 R = int(sys.argv[3]) if len(sys.argv) > 3 else 10
@@ -14,8 +20,9 @@ pairs = int(sys.argv[4]) if len(sys.argv) > 4 else 74
 lib = ctypes.CDLL(sys.argv[5]) if len(sys.argv) > 5 else ctypes.CDLL(_native.build_library())
 desc = _native.dgan_desc(_native.ABI_VERSION, _native.ARCH_IDS[dataset], 128, 64, 0, _native.PRECISIONS["fp16"])
 buf = ctypes.create_string_buffer(1 << 16)
-lib.dgan_debug_plan_stats.restype = ctypes.c_int
-lib.dgan_debug_plan_stats.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-n = lib.dgan_debug_plan_stats(ctypes.byref(desc), batch * R, pairs, buf, len(buf))
+lib.dgan_debug_plan_stats_slots.restype = ctypes.c_int
+lib.dgan_debug_plan_stats_slots.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                            ctypes.c_char_p, ctypes.c_int]
+n = lib.dgan_debug_plan_stats_slots(ctypes.byref(desc), batch * R, pairs, force_dir, force_maxb, buf, len(buf))
 assert n > 0
 print(buf.value.decode())
