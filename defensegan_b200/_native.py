@@ -12,6 +12,7 @@ import sys
 from typing import Dict, List, Optional, Sequence
 
 import torch
+from torch.autograd.function import once_differentiable
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_NAME = "libdefensegan_b200.so"
@@ -30,7 +31,7 @@ NVCC_FLAGS = [
 # Every symbol include/defensegan_b200.h declares.
 ABI_SYMBOLS = [
     "dgan_abi_version", "dgan_last_error", "dgan_num_weights", "dgan_create", "dgan_destroy",
-    "dgan_workspace_bytes", "dgan_reconstruct", "dgan_sample_z0", "dgan_forward", "dgan_loss_grad",
+    "dgan_workspace_bytes", "dgan_reconstruct", "dgan_sample_z0", "dgan_forward", "dgan_loss_grad", "dgan_vjp",
     "dgan_last_launch_count", "dgan_last_enqueue_count", "dgan_macs_per_row", "dgan_profile_enable", "dgan_profile_num_kinds",
     "dgan_profile_kind_name", "dgan_profile_read",
 ]
@@ -128,6 +129,8 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_forward.argtypes = [vp, vp, i32, vp, vp, sz, vp]
     lib.dgan_loss_grad.restype = i32
     lib.dgan_loss_grad.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_vjp.restype = i32
+    lib.dgan_vjp.argtypes = [vp, vp, i32, vp, vp, vp, vp, sz, vp]
     lib.dgan_last_launch_count.restype = ctypes.c_int64
     lib.dgan_last_launch_count.argtypes = [vp]
     lib.dgan_last_enqueue_count.restype = ctypes.c_int64
@@ -326,3 +329,48 @@ class NativeGenerator:
             _check(self.lib, self.lib.dgan_loss_grad(self._handle, _ptr(x), batch, rec_rr, _ptr(zc), _ptr(y), _ptr(loss),
                                                      _ptr(grad), ws, need, ctypes.c_void_p(stream)), "dgan_loss_grad")
         return y, loss, grad
+
+    def vjp(self, z: torch.Tensor, dy: torch.Tensor, want_y: bool = False):
+        """Vector-Jacobian product of the generator at z: dz = (dG/dz)^T dy for a cotangent dy shaped like G(z)
+        ([N,H,W,C] or [N,H*W*C]).  The forward is recomputed; with want_y it is returned too, as (y, dz), bit-identical
+        to forward(z).  With use_bn the batch statistics of the N rows are differentiated."""
+        zc = _require_cuda_f32(z, "z")
+        dyc = _require_cuda_f32(dy, "dy")
+        n = zc.shape[0]
+        if zc.numel() != n * self.latent_dim:
+            raise ValueError("z must be [N, %d]" % self.latent_dim)
+        if dyc.numel() != n * self.hwc or dyc.shape[0] != n:
+            raise ValueError("dy must be [N,%d,%d,%d] with the rows of z" % self.image_dim)
+        with torch.cuda.device(self.device):
+            y = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device) if want_y else None
+            dz = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
+            ws, need = self._workspace(n, 1)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _check(self.lib, self.lib.dgan_vjp(self._handle, _ptr(zc), n, _ptr(dyc), _ptr(y), _ptr(dz), ws, need,
+                                               ctypes.c_void_p(stream)), "dgan_vjp")
+        return (y, dz) if want_y else dz
+
+
+class GeneratorFunction(torch.autograd.Function):
+    """y = G(z) through a NativeGenerator (or anything with its forward / vjp methods), differentiable in z.  The
+    backward recomputes the forward inside `native.vjp` on the current stream; the weights are frozen (no gradient),
+    as in the projection.  Only first derivatives are available."""
+
+    @staticmethod
+    def forward(ctx, z, native):
+        ctx.native = native
+        ctx.save_for_backward(z)
+        return native.forward(z)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        (z,) = ctx.saved_tensors
+        return ctx.native.vjp(z, dy).reshape(z.shape), None
+
+
+def generator(native, z: torch.Tensor) -> torch.Tensor:
+    """G(z): a tensor with a grad_fn when z requires grad and grad mode is on, else exactly native.forward(z)."""
+    if z.requires_grad and torch.is_grad_enabled():
+        return GeneratorFunction.apply(z, native)
+    return native.forward(z)

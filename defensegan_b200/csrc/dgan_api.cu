@@ -13,6 +13,7 @@
 #include "kernels_simt.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_tc2.cuh"
+#include "kernels_vjp.cuh"
 
 namespace dgan {
 
@@ -200,13 +201,18 @@ __global__ void transpose_tiles_kernel(const float* __restrict__ in, float* __re
   out[t * per + (size_t)cc * rows + r] = in[i];
 }
 
+// out = s * (sum of the n_parts partial sums, fixed order); with row_scale, row r (row_len values) is also divided by
+// row_scale[r] (dgan_vjp: its power-of-two cotangent scales, so the division is exact)
 __global__ void scale_copy_kernel(const float* __restrict__ in, int n_parts, size_t part_stride,
-                                  float* __restrict__ out, float s, size_t n) {
+                                  float* __restrict__ out, float s, size_t n,
+                                  const float* __restrict__ row_scale, int row_len) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float g = in[i];
   for (int p = 1; p < n_parts; ++p) g += in[i + (size_t)p * part_stride];
-  out[i] = g * s;
+  float m = s;
+  if (row_scale != nullptr) m /= row_scale[i / row_len];
+  out[i] = g * m;
 }
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -232,7 +238,8 @@ struct Workspace {
   __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][64] scaled dL/dpre of the last layer
   int n_loss_parts = 0, n_g_parts = 1;
   size_t loss_stride_n = 1, loss_stride_b = 1;   // loss_part index = n * stride_n + part * stride_b
-  float *y = nullptr, *dpre = nullptr, *loss_part = nullptr, *loss = nullptr;
+  float *y = nullptr, *dpre = nullptr, *loss_part = nullptr;
+  float* loss = nullptr;               // [n_pad] per-row loss; dgan_vjp (which computes no loss) keeps its row scales here
   float* x = nullptr;                  // [batch][H*W*C] copy of the call's images (the captured loop reads them from here)
   size_t bytes = 0;
 };
@@ -569,6 +576,32 @@ static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t
     DGAN_CUDA_CHECK(cudaMemsetAsync(w.dpre + (size_t)w.n_rows * c->hwc, 0, (size_t)(w.n_pad - w.n_rows) * c->hwc * sizeof(float), s));
   init_z_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, s>>>(w.z, w.v, w.z_h, z0, w.n_rows, w.n_pad, latent, seed,
                                                                  sqrtf(1.0f / (float)latent), row_offset * latent);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// ---- a caller's cotangent dy [n_rows][H*W*C] -> the last layer's d(pre), after a forward that wrote w.y ----------
+// fp16 path: per-row power-of-two scales (one shared scale with BatchNorm) in w.loss, d(pre) * scale in w.dblk;
+// fp32 path: d(pre) unscaled in w.dpre.  See kernels_vjp.cuh.
+static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cudaStream_t s) {
+  const FinalLayer& f = c->fin;
+  const bool tc = c->desc.precision == DGAN_PREC_FP16;
+  const bool sigmoid = f.C_out == 1 && f.act == ACT_SIGMOID;
+  if (!sigmoid && !(f.C_out == 3 && f.act == ACT_TANH)) { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
+  if (tc) {
+    if (sigmoid) cotangent_rowmax_kernel<ACT_SIGMOID><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
+    else cotangent_rowmax_kernel<ACT_TANH><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
+    DGAN_LAUNCH_CHECK(c);
+    cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, w.n_rows, c->desc.use_bn ? 1 : 0);
+    DGAN_LAUNCH_CHECK(c);
+  }
+  const size_t total = (size_t)w.n_rows * c->hwc;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  const int w_out = 2 * f.w_in;
+#define CT(ACT, CO, BLK) cotangent_kernel<ACT, CO, BLK><<<grid, 256, 0, s>>>(w.y, dy, w.n_rows, w_out, w.loss, w.dpre, w.dblk, w.n_pad)
+  if (sigmoid) { if (tc) CT(ACT_SIGMOID, 1, true); else CT(ACT_SIGMOID, 1, false); }
+  else { if (tc) CT(ACT_TANH, 3, true); else CT(ACT_TANH, 3, false); }
+#undef CT
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
@@ -929,9 +962,34 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
   if (grad_dev) {
     const size_t n = (size_t)n_rows * h->desc.latent_dim;
     scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->desc.latent_dim,
-                                                                  grad_dev, grad_multiplier(h), n);
+                                                                  grad_dev, grad_multiplier(h), n, nullptr, 1);
     DGAN_LAUNCH_CHECK(h);
   }
+  return DGAN_OK;
+}
+
+int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev, void* ws,
+             size_t ws_bytes, void* stream) {
+  if (h == nullptr || z_dev == nullptr || dy_dev == nullptr || dz_dev == nullptr || n_rows <= 0) {
+    set_error("invalid argument");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  Workspace w;
+  int rc;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  h->n_rows_cur = n_rows;     // the FLOPs dgan_profile_read reports refer to this call
+  // the forward of dgan_forward, keeping the ReLU masks; the cotangent replaces the loss's (y - x) in the last layer
+  if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
+  if ((rc = run_forward(h, w, nullptr, 1, 1, true, s))) return rc;
+  if ((rc = launch_cotangent(h, w, dy_dev, s))) return rc;
+  if ((rc = run_backward(h, w, s))) return rc;
+  const size_t n = (size_t)n_rows * h->desc.latent_dim;
+  const bool tc = h->desc.precision == DGAN_PREC_FP16;
+  scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->desc.latent_dim, dz_dev,
+                                                                1.f, n, tc ? w.loss : nullptr, h->desc.latent_dim);
+  DGAN_LAUNCH_CHECK(h);
+  if (y_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(y_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
   return DGAN_OK;
 }
 

@@ -286,11 +286,13 @@ class DefenseGANBase(object):
         raise NotImplementedError
 
     def generator_fn(self, z=None, is_training=False):
-        """G(z) (reference models/gan.py:657-665,726-735): z [N, latent] -> images [N,H,W,C]."""
+        """G(z) (reference models/gan.py:657-665,726-735): z [N, latent] -> images [N,H,W,C].
+        Differentiable in z like the reference's graph: when z requires grad (and grad mode is on) the result has a
+        grad_fn whose backward is the native vector-Jacobian product; otherwise it is a plain tensor."""
         if z is None:
             raise ValueError("z must be given (sampling inside generator_fn is a training-time feature)")
         z = self._as_cuda(z)
-        return self._get_native(z.device).forward(z)
+        return _native.generator(self._get_native(z.device), z)
 
     @staticmethod
     def _as_cuda(t):

@@ -71,7 +71,7 @@ int dgan_create(dgan_handle* out, const dgan_desc* desc, const float* const* wei
                 int n_weights, void* stream);
 int dgan_destroy(dgan_handle h);
 
-/* Bytes of caller-owned scratch needed by dgan_reconstruct / dgan_forward / dgan_loss_grad
+/* Bytes of caller-owned scratch needed by dgan_reconstruct / dgan_forward / dgan_loss_grad / dgan_vjp
  * for `batch` images x `rec_rr` restarts.  Also plans and uploads the launch schedules for that many latent rows
  * (cached in the handle; this is where the one-time allocation and synchronisation of a batch size happen). */
 size_t dgan_workspace_bytes(dgan_handle h, int batch, int rec_rr);
@@ -119,6 +119,16 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
 int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, const float* z_dev,
                    float* y_dev, float* loss_dev, float* grad_dev, void* workspace,
                    size_t workspace_bytes, void* stream);
+
+/* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
+ *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
+ *   y_dev [n_rows, H*W*C] = G(z) (nullable; bit-identical to dgan_forward).  The forward is recomputed.
+ *   Workspace: dgan_workspace_bytes(h, n_rows, 1).  With use_bn the batch statistics of the n_rows rows are
+ *   differentiated (rows are coupled, as in the reference).  No host synchronisation, no allocation.
+ * DGAN_PREC_FP16 scales each row's cotangent by a power of two before its fp16 backward (one scale for the call with
+ * use_bn) and divides it out of dz, so dz does not depend on the magnitude of dy beyond the fp32/fp16 range limits. */
+int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev,
+             void* workspace, size_t workspace_bytes, void* stream);
 
 /* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack). */
 int64_t dgan_last_launch_count(dgan_handle h);
