@@ -235,7 +235,7 @@ struct Workspace {
   std::vector<CUtensorMap> map_in, map_out;
   bool have_maps = false;
   unsigned* mom_counter = nullptr;     // fp16 path: [n_pad / 128] tickets of the split-K Linear backward's momentum tail
-  __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][64] scaled dL/dpre of the last layer
+  __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][16 * C_out] scaled dL/dpre of the last layer
   int n_loss_parts = 0, n_g_parts = 1;
   size_t loss_stride_n = 1, loss_stride_b = 1;   // loss_part index = n * stride_n + part * stride_b
   float *y = nullptr, *dpre = nullptr, *loss_part = nullptr;
@@ -264,7 +264,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base) {
   w.g = (float*)take(np * latent * 4 * w.n_g_parts);
   if (tc) w.z_h = (__half*)take(np * latent * 2);
   if (tc) w.mom_counter = (unsigned*)take(np / kRowTile * sizeof(unsigned));
-  if (tc) w.dblk = (__half*)take((size_t)c->tc_fin.n_blocks * np * 64 * 2);
+  if (tc) w.dblk = (__half*)take((size_t)c->tc_fin.n_blocks * np * 16 * c->tc_fin.C_out * 2);
   w.n_loss_parts = tc ? c->tc_fin.n_blocks : c->fin.n_bands;
   w.loss_stride_n = tc ? 1 : (size_t)w.n_loss_parts;          // fp16 path: [block][n_pad] (coalesced epilogue stores)
   w.loss_stride_b = tc ? (size_t)np : 1;
@@ -391,7 +391,7 @@ static int build_maps(dgan_ctx* c, Workspace& w) {
   w.map_out.assign((size_t)2 * nl + 2, CUtensorMap{});
   int rc;
   auto mk = [&](CUtensorMap* m, const void* base, int K, int P, uint32_t box_rows = 128) {
-    return tc_make_map(c->tc, m, base, (uint64_t)K, (uint64_t)w.n_pad, (uint64_t)P, box_rows);
+    return tc_make_map(c->tc, m, base, (uint64_t)K, (uint64_t)w.n_pad, (uint64_t)P, box_rows, tc2_box_k(K));
   };
   for (int l = 0; l < nl; ++l) {
     const GemmLayer& L = c->layers[l];
@@ -403,7 +403,7 @@ static int build_maps(dgan_ctx* c, Workspace& w) {
   }
   const GemmLayer& last = c->layers[nl - 1];
   if ((rc = mk(&w.map_in[2 * nl], w.act_h[nl - 1], c->fin.C_in, last.P_out))) return rc;
-  if ((rc = mk(&w.map_in[2 * nl + 1], w.dblk, 64, c->tc_fin.n_blocks))) return rc;
+  if ((rc = mk(&w.map_in[2 * nl + 1], w.dblk, 16 * c->tc_fin.C_out, c->tc_fin.n_blocks))) return rc;   // 16-channel boxes
   if ((rc = mk(&w.map_out[2 * nl + 1], w.dact_h[nl - 1], last.C_out, last.P_out, TC2_STORE_ROWS))) return rc;
   w.have_maps = true;
   return 0;
@@ -567,8 +567,6 @@ static int run_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s, Momentu
 static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t seed, cudaStream_t s, size_t row_offset = 0) {
   const int latent = c->desc.latent_dim;
   const size_t total4 = (size_t)w.n_pad * latent / 4;
-  // the last layer's block tensor is K-padded to 64 columns; the epilogue only ever writes the 16*C_out valid ones
-  if (w.dblk != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.dblk, 0, (size_t)c->tc_fin.n_blocks * w.n_pad * 64 * sizeof(__half), s));
   if (w.mom_counter != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.mom_counter, 0, (size_t)w.n_pad / kRowTile * sizeof(unsigned), s));
   // fp32 path: the last layer's forward writes dL/dpre for the real rows only while its backward walks all n_pad rows;
   // the tile-padding rows are never observed, but they must not be read uninitialised
@@ -594,6 +592,13 @@ static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cu
     DGAN_LAUNCH_CHECK(c);
     cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, w.n_rows, c->desc.use_bn ? 1 : 0);
     DGAN_LAUNCH_CHECK(c);
+  }
+  if (tc && w.n_pad > w.n_rows) {
+    // the cotangent covers the real rows; the block tensor's tile-padding rows get zeros (the last layer's backward
+    // reads all n_pad rows)
+    const size_t row_b = (size_t)16 * f.C_out * sizeof(__half);
+    DGAN_CUDA_CHECK(cudaMemset2DAsync(w.dblk + (size_t)w.n_rows * 16 * f.C_out, (size_t)w.n_pad * row_b, 0,
+                                      (size_t)(w.n_pad - w.n_rows) * row_b, (size_t)c->tc_fin.n_blocks, s));
   }
   const size_t total = (size_t)w.n_rows * c->hwc;
   const unsigned grid = (unsigned)((total + 255) / 256);
@@ -679,7 +684,7 @@ std::vector<PlanDir> plan_dirs(const dgan_desc* d) {
   }
   const int fh = celeba ? 32 : 14, c_img = celeba ? 3 : 1;
   dirs.push_back({"last.fwd", 16 * c_img, nd, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2, 0, celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2});
-  dirs.push_back({"last.bwd", nd, 64, final_block_bwd_pairs(fh, fh), fh, fh, 0, celeba ? EPI_NONE : EPI_MASK, 2});
+  dirs.push_back({"last.bwd", nd, 16 * c_img, final_block_bwd_pairs(fh, fh), fh, fh, 0, celeba ? EPI_NONE : EPI_MASK, 2});
   return dirs;
 }
 }  // namespace
@@ -1154,8 +1159,16 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     Tc2Plan plan;
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
-    // self-test of the validator: damage the plan of Generator.3 fwd in one specific way; the check must then fail
-    if (mutate != 0 && dr.name == "Generator.3.fwd" && plan.stream_m.size() > 40) {
+    // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd, faults 12-13
+    // (specific to narrow ops) that of the last layer's backward; the check must then fail
+    if (mutate >= 12 && dr.name == "last.bwd" && plan.stream_m.size() > 40) {
+      switch (mutate) {
+        case 12: for (TcRec& r : plan.stream_m) r.w[1] = (r.w[1] & 0xFFu) | ((uint32_t)(plan.ksub == 1 ? 2 : 1) << 8); break;   // k16 per op
+        case 13: plan.stream_p[20].w[0] |= 1u << 8; break;                 // a k-chunk >= 1 (a narrow K has one)
+        default: break;
+      }
+    }
+    if (mutate != 0 && mutate < 12 && dr.name == "Generator.3.fwd" && plan.stream_m.size() > 40) {
       TcRec& m = plan.stream_m[20];
       TcRec* pp = &plan.stream_p[20];
       switch (mutate) {
@@ -1195,7 +1208,7 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     if (mutate != 0) continue;
     // the plans dgan_debug_force_slots can select: every other slot count this direction has an instantiation for
     for (const Tc2Kind& k : kTc2Kinds) {
-      if (k.n != dr.N || k.epi != dr.epi || k.out_bytes != dr.out_bytes || k.maxb == plan.maxb) continue;
+      if (k.n != dr.N || k.ksub != plan.ksub || k.epi != dr.epi || k.out_bytes != dr.out_bytes || k.maxb == plan.maxb) continue;
       Tc2Plan forced;
       if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &forced))) {
         set_error(dr.name + " (" + std::to_string(k.maxb) + " slots): " + dgan_last_error());
@@ -1220,7 +1233,7 @@ int dgan_debug_force_slots(dgan_handle h, int dir, int maxb) {
   const std::vector<TcDir> dirs = tc_dirs(h);
   if (dir < 0 || dir >= (int)dirs.size()) { set_error("layer-direction out of range"); return DGAN_ERR_INVALID_ARG; }
   const TcDir& d = dirs[(size_t)dir];
-  if (maxb > 0 && !tc2_has_kind(d.w1->N, maxb, d.epi, d.out_bytes)) {
+  if (maxb > 0 && !tc2_has_kind(d.w1->N, maxb, tc2_ksub(d.w1->K), d.epi, d.out_bytes)) {
     set_error("no kernel instantiation with " + std::to_string(maxb) + " accumulator slots per round for this layer-direction");
     return DGAN_ERR_UNSUPPORTED;
   }
@@ -1240,7 +1253,7 @@ int dgan_debug_slot_choices(dgan_handle h, int dir, int* out, int max_n) {
   const TcDir& d = dirs[(size_t)dir];
   int n = 0;
   for (const Tc2Kind& k : kTc2Kinds)
-    if (k.n == d.w1->N && k.epi == d.epi && k.out_bytes == d.out_bytes && n < max_n) out[n++] = k.maxb;
+    if (k.n == d.w1->N && k.ksub == tc2_ksub(d.w1->K) && k.epi == d.epi && k.out_bytes == d.out_bytes && n < max_n) out[n++] = k.maxb;
   return n;
 }
 
@@ -1256,15 +1269,17 @@ int dgan_debug_probe_read(unsigned long long* out) {
 #endif
 
 // Host-only developer aid (not in the public header): the plan of every layer-direction in numbers - window shape, items,
-// steps, MMAs, operand bytes staged from L2 into shared memory (both CTAs of every pair), accumulator slots per round -
-// as text.  Layer-direction `force_dir` (plan_dirs order; -1: none) is planned with exactly `force_maxb` slots per
-// round, as dgan_debug_force_slots would.  Returns the length.
-int dgan_debug_plan_stats_slots(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, char* buf, int buf_len) {
+// steps, MMAs (ops of KSUB k16 each, and k16 MMAs), operand bytes staged from L2 into shared memory (both CTAs of every
+// pair), accumulator slots per round - as text.  Layer-direction `force_dir` (plan_dirs order; -1: none) is planned
+// with exactly `force_maxb` slots per round, as dgan_debug_force_slots would, and, when force_shape is not NULL, with
+// exactly that window shape {wh, ww, sy, sx}.  Returns the length.
+static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, const int* force_shape,
+                           char* buf, int buf_len) {
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
   std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load"
-                    " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us\n";
+                    " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us | k16 MMAs\n";
   double total = 0.0;
   const std::vector<PlanDir> dirs = plan_dirs(d);
   for (size_t di = 0; di < dirs.size(); ++di) {
@@ -1272,17 +1287,18 @@ int dgan_debug_plan_stats_slots(const dgan_desc* d, int n_rows, int n_pairs, int
     int max_acc = tc2_maxb(dr.N);
     if (dr.force_acc > 0) max_acc = std::min(max_acc, dr.force_acc);
     Tc2Plan plan;
-    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, (int)di == force_dir ? force_maxb : 0, dr.epi, dr.out_bytes,
-                            n_mpairs, n_pairs, &plan);
+    const bool forced = (int)di == force_dir;
+    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, forced ? force_maxb : 0, dr.epi, dr.out_bytes,
+                            n_mpairs, n_pairs, &plan, forced ? force_shape : nullptr);
     if (rc) return -1;
     char line[256];
     const double mb = (double)plan.n_bytes / 1e6;
     total += mb;
-    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f | %d | %.1f | %.1f\n", dr.name.c_str(),
+    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f | %d | %.1f | %.1f | %lld\n", dr.name.c_str(),
              dr.N, dr.K, plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,
              plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0),
              100.0 * (double)plan.n_pad / (double)std::max(plan.n_mma, 1LL), plan.maxb, plan.op_ns_max / 1e3,
-             plan.load_max / 1e3);
+             plan.load_max / 1e3, plan.n_mma * plan.ksub);
     out += line;
   }
   char line[64];
@@ -1292,6 +1308,18 @@ int dgan_debug_plan_stats_slots(const dgan_desc* d, int n_rows, int n_pairs, int
   memcpy(buf, out.data(), (size_t)n);
   buf[n] = 0;
   return n;
+}
+
+int dgan_debug_plan_stats_slots(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, char* buf, int buf_len) {
+  return plan_stats_impl(d, n_rows, n_pairs, force_dir, force_maxb, nullptr, buf, buf_len);
+}
+
+// As dgan_debug_plan_stats_slots, with layer-direction `force_dir` also planned on exactly the window shape wh x ww with
+// strides (sy, sx) (force_maxb = 0: any slot count that fits it): plans of two builds compared at the same window.
+int dgan_debug_plan_stats_window(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, int wh, int ww,
+                                 int sy, int sx, char* buf, int buf_len) {
+  const int shape[4] = {wh, ww, sy, sx};
+  return plan_stats_impl(d, n_rows, n_pairs, force_dir, force_maxb, shape, buf, buf_len);
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -15,7 +15,6 @@
 
 namespace dgan {
 
-constexpr int TC_A_BYTES = 128 * 128;        // one activation tile: 128 rows x 64 fp16
 constexpr int TC_LINEAR_SPLIT = 4;           // partial sums of the Linear backward (dz)
 
 // One direction (forward or backward) of one layer on the tensor-core path.
@@ -146,6 +145,11 @@ template <> struct Wgmma<256> {
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
+// K-major, 32B-swizzled operand sub-tile of 16 channels (one k16): rows 32 B apart, 8-row groups 256 B apart (SBO);
+// layout type 3 = SWIZZLE_32B.  The k16 spans the whole 32 B swizzle width, so the leading byte offset is unused.
+__device__ __forceinline__ uint64_t make_smem_desc_sw32(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)3 << 62);
+}
 
 // fp32 pair -> packed fp16, round-to-nearest, saturating to +-65504: a backward activation that exceeds the fp16 range
 // (trained filters, |y - x| up to 2 on CelebA) must not become inf and turn z into NaN for the rest of the loop.
@@ -209,17 +213,20 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// 3-D fp16 tensor [d2][d1][d0] (d0 contiguous), box {64, box1, 1}, 128B swizzle.
+// 3-D fp16 tensor [d2][d1][d0] (d0 contiguous), box {box0, box1, 1}: box0 = 64 channels with 128B swizzle (the
+// 64-channel operand), or 16 channels with 32B swizzle (one 16-channel sub-tile of a narrow operand).
 static int tc_make_map(const TcState& st, CUtensorMap* map, const void* base, uint64_t d0, uint64_t d1, uint64_t d2,
-                       uint32_t box1) {
+                       uint32_t box1, uint32_t box0 = 64) {
   if (st.encode_fn == nullptr) { set_error("cuTensorMapEncodeTiled unavailable"); return DGAN_ERR_CUDA; }
   const cuuint64_t dims[3] = {d0, d1, d2};
   const cuuint64_t strides[2] = {d0 * 2, d0 * d1 * 2};
-  const cuuint32_t box[3] = {64, box1, 1};
+  if (box0 != 64 && box0 != 16) { set_error("tensor map box must be 64 or 16 channels wide"); return DGAN_ERR_UNSUPPORTED; }
+  const cuuint32_t box[3] = {box0, box1, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = ((PFN_encodeTiled)st.encode_fn)(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims,
                                                strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                               box0 == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_32B,
+                                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
@@ -239,7 +246,8 @@ static int tc_upload(std::vector<void*>* allocs, const void* host, size_t bytes,
 
 static int tc_set_direction(TcWeights* w, int N, int K, int n_tiles, int P_in, int P_out) {
   if (N != 16 && N != 48 && N != 64 && N != 128 && N != 256) { set_error("tensor-core path needs 64/128/256 output channels per pixel"); return DGAN_ERR_UNSUPPORTED; }
-  if (K % 64 != 0) { set_error("tensor-core path needs input channels in multiples of 64"); return DGAN_ERR_UNSUPPORTED; }
+  // K < 64: the narrow operand of the last layer's backward (16 * C_out channels, k16 sub-tiles)
+  if (K % 64 != 0 && !(K == 16 || K == 48)) { set_error("tensor-core path needs input channels in multiples of 64, or 16 / 48"); return DGAN_ERR_UNSUPPORTED; }
   if (n_tiles > 32 || P_in > 65535 || P_out > 65535) { set_error("tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
   w->N = N; w->K = K; w->P_in = P_in; w->P_out = P_out; w->n_tiles = n_tiles;
   return 0;
@@ -249,10 +257,10 @@ static int tc_set_direction(TcWeights* w, int N, int K, int n_tiles, int P_in, i
 // Image pixels are grouped into 4x4 blocks; block (by,bx) receives from the 4x4 input pixels
 // o = 2by-1+ry, p = 2bx-1+rx (ry,rx in 0..3): out row 4by+li = 2o+ka-1  =>  ka = li - 2ry + 3.
 // Weight tile (ry,rx), forward:  rows (li*4+lj)*C_out+co, cols ci   = F[ka][kb][co][ci] or 0
-//                      backward: rows ci, cols (li*4+lj)*C_out+co (zero padded to 64)
+//                      backward: rows ci, cols (li*4+lj)*C_out+co
 __global__ void tc_final_tiles_kernel(const float* __restrict__ F /*[25][C_out][C_in]*/, int C_out, int C_in,
                                       __half* __restrict__ wf /*[16][16*C_out][C_in]*/,
-                                      __half* __restrict__ wb /*[16][C_in][64]*/) {
+                                      __half* __restrict__ wb /*[16][C_in][16*C_out]*/) {
   const int tile = blockIdx.x, ry = tile >> 2, rx = tile & 3;
   const int nrow = 16 * C_out;
   for (int e = threadIdx.x; e < nrow * C_in; e += blockDim.x) {
@@ -263,15 +271,13 @@ __global__ void tc_final_tiles_kernel(const float* __restrict__ F /*[25][C_out][
     if (ka >= 0 && ka < 5 && kb >= 0 && kb < 5) v = F[((size_t)(ka * 5 + kb) * C_out + co) * C_in + ci];
     wf[((size_t)tile * nrow + r) * C_in + ci] = __float2half_rn(v);
   }
-  for (int e = threadIdx.x; e < C_in * 64; e += blockDim.x) {
-    const int ci = e / 64, k = e % 64;
+  for (int e = threadIdx.x; e < C_in * nrow; e += blockDim.x) {
+    const int ci = e / nrow, k = e % nrow;
+    const int co = k % C_out, l = k / C_out, li = l >> 2, lj = l & 3;
+    const int ka = li - 2 * ry + 3, kb = lj - 2 * rx + 3;
     float v = 0.f;
-    if (k < nrow) {
-      const int co = k % C_out, l = k / C_out, li = l >> 2, lj = l & 3;
-      const int ka = li - 2 * ry + 3, kb = lj - 2 * rx + 3;
-      if (ka >= 0 && ka < 5 && kb >= 0 && kb < 5) v = F[((size_t)(ka * 5 + kb) * C_out + co) * C_in + ci];
-    }
-    wb[((size_t)tile * C_in + ci) * 64 + k] = __float2half_rn(v);
+    if (ka >= 0 && ka < 5 && kb >= 0 && kb < 5) v = F[((size_t)(ka * 5 + kb) * C_out + co) * C_in + ci];
+    wb[((size_t)tile * C_in + ci) * nrow + k] = __float2half_rn(v);
   }
 }
 
@@ -349,13 +355,14 @@ static int tc_build_final(TcState& st, TcFinal* tf, const float* F, int h_in, in
   tf->C_out = C_out; tf->act = act; tf->nbx = w_in / 2; tf->n_blocks = (h_in / 2) * (w_in / 2); tf->w_out = 2 * w_in;
   const int nrow = 16 * C_out;
   DGAN_CUDA_CHECK(cudaMalloc((void**)&tf->f.w, (size_t)16 * nrow * C_in * 2)); allocs->push_back(tf->f.w);
-  DGAN_CUDA_CHECK(cudaMalloc((void**)&tf->b.w, (size_t)16 * C_in * 64 * 2)); allocs->push_back(tf->b.w);
+  DGAN_CUDA_CHECK(cudaMalloc((void**)&tf->b.w, (size_t)16 * C_in * nrow * 2)); allocs->push_back(tf->b.w);
   tc_final_tiles_kernel<<<16, 256, 0, s>>>(F, C_out, C_in, tf->f.w, tf->b.w);
   DGAN_CUDA_CHECK(cudaGetLastError());
   int rc;
   (void)st;
   if ((rc = tc_set_direction(&tf->f, nrow, C_in, 16, h_in * w_in, tf->n_blocks))) return rc;
-  if ((rc = tc_set_direction(&tf->b, C_in, 64, 16, tf->n_blocks, h_in * w_in))) return rc;
+  // backward: K = the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
+  if ((rc = tc_set_direction(&tf->b, C_in, nrow, 16, tf->n_blocks, h_in * w_in))) return rc;
   return 0;
 }
 

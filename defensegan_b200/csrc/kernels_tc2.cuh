@@ -70,7 +70,8 @@ __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out
 //   w[4..5]: 8 x u8 weight tile [0,5) per B slot
 // MMA record:
 //   w[0]: ring offset / 1 KB [0,8) | A tiles [8,11) | rounds [11,16) | flags [16,18): 1 = first step of an item, 2 = last
-//   w[1]: accumulators per round (MAXB of the instantiation; checked by the validator only)
+//   w[1]: accumulators per round [0,8) (MAXB of the instantiation) | k16 MMAs per op [8,11) (KSUB); checked by the
+//         validator only
 //   w[2..7]: 24 x u8, round-major, one per (round, accumulator): A tile [0,2) | B slot [2,6) | first MMA into the
 //            accumulator [6,7).  B slot 15 = the all-zero tile outside the ring (the accumulator has nothing to add in
 //            this round; never a first MMA).
@@ -84,53 +85,70 @@ constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // produ
 __host__ __device__ constexpr int tc2_epi_tiles(int n_tile, int epi, int out_bytes) {
   return tc2_tma_epilogue(n_tile, epi, out_bytes) ? 2 : 0;
 }
+// k16 MMAs per op (KSUB) of a direction with K input channels: 4 = a 64-channel k-chunk, one 128B-swizzled operand per
+// tile; 1..3 = a narrow operand (the last layer's backward, K = 16 * C_out) of KSUB 16-channel 32B-swizzled sub-tiles.
+__host__ __device__ constexpr int tc2_ksub(int K) { return K % 64 == 0 ? 4 : K / 16; }
+// Staged bytes of one A tile (128 rows) and one weight tile (N rows) of an op.
+__host__ __device__ constexpr int tc2_a_bytes(int ksub) { return 128 * 32 * ksub; }
+__host__ __device__ constexpr int tc2_b_bytes(int n_tile, int ksub) { return n_tile * 32 * ksub; }
 // The all-zero weight tile read by the MMAs of an accumulator with nothing to add in a round (instantiations with more
-// than one accumulator per round).  It sits right after the ring and is written once per CTA.
-__host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb) { return maxb > 1 ? n_tile * 128 : 0; }
-__host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int epi, int out_bytes) {
+// than one accumulator per round).  It sits right after the ring, has the shape of a weight tile and is written once
+// per CTA.
+__host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb, int ksub) { return maxb > 1 ? tc2_b_bytes(n_tile, ksub) : 0; }
+__host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int ksub, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
-  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb)) / 1024) * 1024;
+  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb, ksub)) / 1024) * 1024;
   return raw > 255 * 1024 ? 255 * 1024 : raw;
 }
 
 // MAXB_: accumulator slots of the instantiation = MMAs per round = the most accumulators a window may have.  Fewer slots
 // than fit the 256 accumulator columns issue fewer zero-tile MMAs but allow only smaller windows (more staged bytes);
 // the planner weighs the two (tc2_plan).
-template <int N_TILE, int MAXB_, int EPI = EPI_NONE, int OUT_BYTES = 2>
+// KSUB_: k16 MMAs per op (tc2_ksub).  4: A and weight tiles are 64-channel 128B-swizzled boxes and the op's k16 step
+// through each 128 B row.  1..3: each tile is KSUB sub-tiles of 16 channels (32 B rows, 32B swizzle), one per k16, so a
+// narrow K stages and multiplies only its real channels.
+template <int N_TILE, int MAXB_, int KSUB_ = 4, int EPI = EPI_NONE, int OUT_BYTES = 2>
 struct Tc2Cfg {
   static_assert(MAXB_ >= 1 && MAXB_ <= TC2_BUF_COLS / tc2_acc_stride(N_TILE), "more accumulator slots than columns");
-  static constexpr int B_TILE = N_TILE * 128;                             // bytes of one staged weight tile
+  static_assert(KSUB_ >= 1 && KSUB_ <= 4, "k16 MMAs per op");
+  static constexpr int KSUB = KSUB_;
+  static constexpr int A_BYTES = tc2_a_bytes(KSUB);                      // bytes of one staged activation tile
+  static constexpr int B_TILE = tc2_b_bytes(N_TILE, KSUB);               // bytes of one staged weight tile
+  static constexpr int A_SUB = 128 * 32, B_SUB = N_TILE * 32;            // narrow ops: bytes of one 16-channel sub-tile
   static constexpr int MAXB = MAXB_;
   static constexpr int ACC_REGS = MAXB * N_TILE / 2;                      // accumulator registers per consumer thread
   static constexpr bool TMA_EPI = tc2_tma_epilogue(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_TILES = tc2_epi_tiles(N_TILE, EPI, OUT_BYTES);
   static constexpr int EPI_BYTES = EPI_TILES * TC2_TILE_BYTES;
-  static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE, MAXB);
-  static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, MAXB, EPI, OUT_BYTES);    // operand ring (offsets are 8-bit KB)
+  static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE, MAXB, KSUB);
+  static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, MAXB, KSUB, EPI, OUT_BYTES);    // operand ring (offsets are 8-bit KB)
   static constexpr int SMEM_BYTES = RING_BYTES + ZERO_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
 };
 
-// Every instantiation of tc_bsgemm2_kernel: (N, accumulator slots per round, epilogue, output type).  tc2_optin_all,
-// the launch dispatch and the planner's candidate set (tc2_plan) all read this list.  For each (N, epilogue, output
-// type) it holds the largest slot count, which every window shape can use, and the smaller ones the planner picks for
-// the shipped generators.
+// Every instantiation of tc_bsgemm2_kernel: (N, accumulator slots per round, k16 MMAs per op, epilogue, output type).
+// tc2_optin_all, the launch dispatch and the planner's candidate set (tc2_plan) all read this list.  For each
+// (N, k16 per op, epilogue, output type) it holds the largest slot count, which every window shape can use, and the
+// smaller ones the planner picks for the shipped generators.  The narrow kinds (k16 per op < 4) are the last layer's
+// backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA).
 #define TC2_KINDS(X)                                                                                                   \
-  X(256, 1, EPI_BIAS_RELU, __half) X(256, 1, EPI_BIAS, __half) X(256, 1, EPI_MASK, __half) X(256, 1, EPI_NONE, __half) \
-  X(256, 1, EPI_NONE, float) X(256, 1, EPI_BIAS, float)                                                                \
-  X(128, 2, EPI_BIAS_RELU, __half) X(128, 2, EPI_BIAS, __half) X(128, 2, EPI_MASK, __half) X(128, 2, EPI_NONE, __half) \
-  X(128, 2, EPI_NONE, float) X(128, 2, EPI_BIAS, float) X(128, 1, EPI_NONE, float)                                    \
-  X(64, 4, EPI_BIAS_RELU, __half) X(64, 4, EPI_BIAS, __half) X(64, 4, EPI_MASK, __half) X(64, 4, EPI_NONE, __half)     \
-  X(64, 4, EPI_NONE, float) X(64, 4, EPI_BIAS, float)                                                                  \
-  X(16, 8, EPI_FINAL_SIGMOID1, __half) X(16, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, EPI_FINAL_TANH3, __half)
+  X(256, 1, 4, EPI_BIAS_RELU, __half) X(256, 1, 4, EPI_BIAS, __half) X(256, 1, 4, EPI_MASK, __half)                    \
+  X(256, 1, 4, EPI_NONE, __half) X(256, 1, 4, EPI_NONE, float) X(256, 1, 4, EPI_BIAS, float)                           \
+  X(128, 2, 4, EPI_BIAS_RELU, __half) X(128, 2, 4, EPI_BIAS, __half) X(128, 2, 4, EPI_MASK, __half)                    \
+  X(128, 2, 4, EPI_NONE, __half) X(128, 2, 4, EPI_NONE, float) X(128, 2, 4, EPI_BIAS, float)                           \
+  X(128, 1, 4, EPI_NONE, float)                                                                                        \
+  X(64, 4, 4, EPI_BIAS_RELU, __half) X(64, 4, 4, EPI_BIAS, __half) X(64, 4, 4, EPI_MASK, __half)                      \
+  X(64, 4, 4, EPI_NONE, __half) X(64, 4, 4, EPI_NONE, float) X(64, 4, 4, EPI_BIAS, float)                              \
+  X(64, 4, 1, EPI_MASK, __half) X(64, 4, 1, EPI_NONE, __half) X(64, 4, 3, EPI_NONE, __half)                            \
+  X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)
 
-struct Tc2Kind { int n, maxb, epi, out_bytes; };
-#define TC2_KIND_ROW(NT, MB, EP, T) {NT, MB, EP, (int)sizeof(T)},
+struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
+#define TC2_KIND_ROW(NT, MB, KS, EP, T) {NT, MB, KS, EP, (int)sizeof(T)},
 static constexpr Tc2Kind kTc2Kinds[] = {TC2_KINDS(TC2_KIND_ROW)};
 #undef TC2_KIND_ROW
 // Is there an instantiation with these template arguments?
-static inline bool tc2_has_kind(int n, int maxb, int epi, int out_bytes) {
+static inline bool tc2_has_kind(int n, int maxb, int ksub, int epi, int out_bytes) {
   for (const Tc2Kind& k : kTc2Kinds)
-    if (k.n == n && k.maxb == maxb && k.epi == epi && k.out_bytes == out_bytes) return true;
+    if (k.n == n && k.maxb == maxb && k.ksub == ksub && k.epi == epi && k.out_bytes == out_bytes) return true;
   return false;
 }
 
@@ -203,23 +221,25 @@ __device__ __forceinline__ int tc2_item_at(const int* __restrict__ order, int k,
   return k < n_slots ? __ldg(order + (size_t)k * n_pairs + pair) : -1;
 }
 
-// One round of a step: for every accumulator a, in compile-time order, the 4 k16 MMAs of a 64-channel k-chunk.  Only
-// the operand descriptors and the overwrite predicate come from the record byte of (round, a), so the sequence of
-// wgmma instructions and the registers they name are fixed.
+// One round of a step: for every accumulator a, in compile-time order, the KSUB k16 MMAs of one op (a 64-channel
+// k-chunk, or a narrow operand's 16-channel sub-tiles).  Only the operand descriptors and the overwrite predicate come
+// from the record byte of (round, a), so the sequence of wgmma instructions and the registers they name are fixed.
 //   da0 / db0: descriptors of the step's first A tile (this warpgroup's rows) and first B slot; zoff: the zero tile's
 //   distance from db0 in 16-byte units.
-template <int NT, int MAXB, int NREG>
+template <int NT, int MAXB, int KSUB, int NREG>
 __device__ __forceinline__ void tc2_mma_round(float (&acc)[NREG], const uint32_t (&q)[6], uint64_t da0, uint64_t db0, uint32_t zoff) {
+  // the next k16: 32 B further along the 128 B row of a 128B-swizzled tile, or the next 16-channel sub-tile
+  constexpr uint32_t DA_K = KSUB == 4 ? 2u : (uint32_t)(128 * 32 >> 4), DB_K = KSUB == 4 ? 2u : (uint32_t)(NT * 32 >> 4);
 #pragma unroll
   for (int a = 0; a < MAXB; ++a) {
     const uint32_t e = (q[a >> 2] >> (8 * (a & 3))) & 0xFFu;
     const uint32_t bs = (e >> 2) & 0xFu;
     // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
-    const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(TC_A_BYTES >> 4));
-    const uint64_t db = db0 + (uint64_t)(bs == (uint32_t)TC2_ZERO_SLOT ? zoff : bs * (uint32_t)(NT * 128 >> 4));
+    const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(tc2_a_bytes(KSUB) >> 4));
+    const uint64_t db = db0 + (uint64_t)(bs == (uint32_t)TC2_ZERO_SLOT ? zoff : bs * (uint32_t)(tc2_b_bytes(NT, KSUB) >> 4));
     const uint32_t keep = ((e >> 6) & 1u) ^ 1u;      // 0: first MMA into the accumulator, overwrite it
 #pragma unroll
-    for (int k = 0; k < 4; ++k) ptx::Wgmma<NT>::mma(acc + a * (NT / 2), da + 2u * k, db + 2u * k, k > 0 ? 1u : keep);
+    for (int k = 0; k < KSUB; ++k) ptx::Wgmma<NT>::mma(acc + a * (NT / 2), da + DA_K * k, db + DB_K * k, k > 0 ? 1u : keep);
   }
 }
 
@@ -252,7 +272,7 @@ __host__ __device__ constexpr int tc2_probe_key(int n_tile, int epi, int out_byt
 }
 #endif
 
-template <int N_TILE, int MAXB, int EPI, typename TOUT>
+template <int N_TILE, int MAXB, int KSUB, int EPI, typename TOUT>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC2_THREADS, 1)
 tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const __grid_constant__ CUtensorMap tm_out,
@@ -260,11 +280,11 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                   const TcRec* __restrict__ stream_m, const __grid_constant__ Tc2Heads heads,
                   const int* __restrict__ eitems, int n_slots,
                   TOUT* __restrict__ out, int n_pad, const float* __restrict__ bias, int bias_pstride, const TcFinalArgs fa) {
-  using Cfg = Tc2Cfg<N_TILE, MAXB, EPI, (int)sizeof(TOUT)>;
+  using Cfg = Tc2Cfg<N_TILE, MAXB, KSUB, EPI, (int)sizeof(TOUT)>;
   constexpr bool TMA_EPI = Cfg::TMA_EPI;
   constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3);
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
-  constexpr int B_TILE = Cfg::B_TILE;
+  constexpr int B_TILE = Cfg::B_TILE, A_BYTES = Cfg::A_BYTES;
   constexpr int PRODUCER = TC2_CONSUMERS / 32;     // warp index of the TMA producer
   extern __shared__ uint8_t smem_raw[];
 #ifdef DGAN_PROBE
@@ -348,19 +368,32 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           const uint32_t full = bar_full + 8 * slot;
           const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
           if (ptx::elect_one()) {
-            ptx::mbar_expect_tx(full, (uint32_t)(nA * TC_A_BYTES + nB * B_TILE));
+            ptx::mbar_expect_tx(full, (uint32_t)(nA * A_BYTES + nB * B_TILE));
 #pragma unroll
             for (int a = 0; a < TC2_MAX_A; ++a) {
               if (a >= nA) break;
               const int p = (int)((((a < 2) ? r0.z : r0.w) >> (16 * (a & 1))) & 0xFFFFu);
-              ptx::tma_load_3d(sa + a * TC_A_BYTES, &tm_a, full, kc * 64, row0, p);
+              if constexpr (KSUB == 4) {
+                ptx::tma_load_3d(sa + a * A_BYTES, &tm_a, full, kc * 64, row0, p);
+              } else {
+#pragma unroll
+                for (int k = 0; k < KSUB; ++k)           // one 16-channel box per sub-tile
+                  ptx::tma_load_3d(sa + a * A_BYTES + k * Cfg::A_SUB, &tm_a, full, (kc * KSUB + k) * 16, row0, p);
+              }
             }
-            const uint32_t sb = sa + nA * TC_A_BYTES;
+            const uint32_t sb = sa + nA * A_BYTES;
 #pragma unroll
             for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {     // this CTA's half of each weight tile, into both CTAs
               if (b >= nB) break;
               const uint32_t e = ((b < 4) ? r1.x : r1.y) >> (8 * (b & 3));
-              ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+              if constexpr (KSUB == 4) {
+                ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+              } else {
+#pragma unroll
+                for (int k = 0; k < KSUB; ++k)           // this CTA's half of every sub-tile
+                  ptx::tma_load_3d_mc2(sb + b * B_TILE + k * Cfg::B_SUB + rank * (Cfg::B_SUB / 2), &tm_b, full, (kc * KSUB + k) * 16,
+                                       (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+              }
             }
           }
           __syncwarp();
@@ -404,15 +437,16 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
 #endif
         const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
-        const uint64_t da0 = make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u);   // this warpgroup's 64 rows of the A tiles
-        const uint32_t sb = sa + (uint32_t)nA * TC_A_BYTES;
-        const uint64_t db0 = make_smem_desc_sw128(sb);
+        // this warpgroup's 64 rows of the A tiles (of their first sub-tile when narrow)
+        const uint64_t da0 = KSUB == 4 ? make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u) : make_smem_desc_sw32(sa + (uint32_t)wg * 64u * 32u);
+        const uint32_t sb = sa + (uint32_t)nA * A_BYTES;
+        const uint64_t db0 = KSUB == 4 ? make_smem_desc_sw128(sb) : make_smem_desc_sw32(sb);
         const uint32_t zoff = (zero_base - sb) >> 4;    // zero tile after the ring: always above the step's B slots
         uint32_t q[6] = {r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
         ptx::fence_operands(acc);
         ptx::wgmma_fence();
         for (int r = 0; r < n_rounds; ++r) {
-          tc2_mma_round<N_TILE, Cfg::MAXB>(acc, q, da0, db0, zoff);
+          tc2_mma_round<N_TILE, Cfg::MAXB, KSUB>(acc, q, da0, db0, zoff);
           tc2_pop_round<Cfg::MAXB>(q);
         }
         ptx::wgmma_commit();
@@ -476,9 +510,9 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                 dv[c] = d * dact * fa.gscale;
               }
               if (fa.write_y) *reinterpret_cast<float2*>(fa.y + n * hwc + off) = make_float2(yv[0], yv[1]);
-              // the K-padding columns [16*CO, 64) of the block tensor stay zero (cleared once per call)
+              // d(pre) block tensor [n_blocks][n_pad][16 * CO]: the last layer's backward reads it as its narrow operand
               if (fa.x != nullptr)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(out) + ((size_t)blk * n_pad + n) * 64 + col) = pack_half2(dv[0], dv[1]);
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(out) + ((size_t)blk * n_pad + n) * N_TILE + col) = pack_half2(dv[0], dv[1]);
             }
             lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
             lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
@@ -664,8 +698,10 @@ struct Tc2Schedule {           // one window tiling of a layer-direction + its i
   int wh = 0, ww = 0, sy = 1, sx = 1;
   int maxb = 1;                    // accumulator slots per round: selects the kernel instantiation
 };
+// 64-channel or 16-channel TMA box for operands of K channels (tc_make_map)
+static uint32_t tc2_box_k(int K) { return tc2_ksub(K) == 4 ? 64u : 16u; }
 struct TcWeights2 {
-  CUtensorMap tm_b;            // box {64, N/2, 1}: the half of a weight tile one CTA of the pair loads
+  CUtensorMap tm_b;            // box {64 | 16, N/2, 1}: the half of a weight tile (sub-tile) one CTA of the pair loads
   PairTable tab;               // host copy: schedules are built lazily per batch size
   int h_grid = 0, w_grid = 0, max_acc = 1;
   int force_maxb = 0;          // > 0: plan with exactly this many accumulator slots per round (dgan_debug_force_slots)
@@ -688,7 +724,7 @@ struct Tc2HostItem {
   TcItem2 hdr{};
   std::vector<Tc2HostStep> steps;
   double stage_bytes = 0.0;
-  long long n_ops = 0;         // 64-channel MMAs issued (rounds x slots), zero-tile ones included
+  long long n_ops = 0;         // ops issued (rounds x slots, KSUB k16 MMAs each), zero-tile ones included
 };
 
 // Steps of one window (accumulator a <-> output pixel qs[a]).  Input pixels are taken in ascending order and packed
@@ -698,7 +734,7 @@ struct Tc2HostItem {
 // to add in a round - or beyond the window's accumulators - reads the zero tile.
 static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int N, int K, int max_b, int max_a,
                            int step_max_bytes, Tc2HostItem* out) {
-  const int kch = K / 64, b_tile = N * 128;
+  const int ksub = tc2_ksub(K), kch = K / (16 * ksub), a_bytes = tc2_a_bytes(ksub), b_tile = tc2_b_bytes(N, ksub);
   out->hdr = TcItem2{};
   out->hdr.n_acc = (uint32_t)qs.size();
   for (size_t a = 0; a < qs.size(); ++a) out->hdr.q[a] = (uint16_t)qs[a];
@@ -718,7 +754,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     std::stable_sort(g.second.begin(), g.second.end(), [](const auto& l, const auto& r) { return l.second < r.second; });
   // a pixel with more entries than one step can hold is split (Linear layers: 16 tiles per input "pixel")
   std::vector<std::pair<int, std::vector<std::pair<int, int>>>> px;
-  const int ent_cap = std::min(TC2_MAX_BSLOTS, std::max(1, (step_max_bytes - TC_A_BYTES) / b_tile));
+  const int ent_cap = std::min(TC2_MAX_BSLOTS, std::max(1, (step_max_bytes - a_bytes) / b_tile));
   for (auto& g : by_p)
     for (size_t b0 = 0; b0 < g.second.size(); b0 += (size_t)ent_cap)
       px.push_back({g.first, std::vector<std::pair<int, int>>(g.second.begin() + b0,
@@ -751,7 +787,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
         const int nA = (int)(i1 - i0) + 1, nB = (int)staged.size() + fresh;
         const bool dup_pixel = (i1 > i0 && px[i1].first == px[i1 - 1].first);   // split halves of one pixel stay apart
         if (i1 > i0 && (dup_pixel || nB > TC2_MAX_BSLOTS || rounds > max_rounds ||
-                        nA * TC_A_BYTES + nB * b_tile > step_max_bytes))
+                        nA * a_bytes + nB * b_tile > step_max_bytes))
           break;
         for (int t : fresh_tiles) staged.push_back(t);
         std::copy(c2, c2 + 8, cnt);
@@ -786,7 +822,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
         seen |= 1u << acc;
       }
     }
-    st.bytes = st.nA * TC_A_BYTES + st.nB * b_tile;
+    st.bytes = st.nA * a_bytes + st.nB * b_tile;
     out->steps.push_back(st);
   }
   // k-chunk outermost: every accumulator then sums its (k-chunk, input pixel) contributions in one canonical order
@@ -830,7 +866,7 @@ static int tc2_build_direction(TcState& st, const TcWeights& w1, TcWeights2* w2,
   int max_acc = tc2_maxb(N);
   if (force_max_acc > 0) max_acc = std::min(max_acc, force_max_acc);
   w2->tab = tab; w2->h_grid = h_grid; w2->w_grid = w_grid; w2->max_acc = max_acc;
-  return tc_make_map(st, &w2->tm_b, w1.w, (uint64_t)K, (uint64_t)N, (uint64_t)w1.n_tiles, (uint32_t)(N / 2));
+  return tc_make_map(st, &w2->tm_b, w1.w, (uint64_t)K, (uint64_t)N, (uint64_t)w1.n_tiles, (uint32_t)(N / 2), tc2_box_k(K));
 }
 
 #ifndef DGAN_STEP_MAX_KB
@@ -846,8 +882,8 @@ static int tc2_build_direction(TcState& st, const TcWeights& w1, TcWeights2* w2,
 #define DGAN_COST_FIXED_KB 48.0
 #endif
 // Time model of an item (DESIGN.md section 3, least-squares fit to per-kernel times on an H100): NS_PER_KB per KB of
-// the cost above (staged bytes + epilogue and fixed charges), OP_NS per 64-channel MMA at N = 64, scaled by
-// max(N, OP_MIN_N) / 64 for other widths, and STEP_NS per step (the consumers' full-barrier wait, wgmma commit and
+// the cost above (staged bytes + epilogue and fixed charges), OP_NS per 64-channel op (4 k16 MMAs) at N = 64, scaled by
+// max(N, OP_MIN_N) / 64 for other widths and by KSUB / 4 for narrow ops, and STEP_NS per step (the consumers' full-barrier wait, wgmma commit and
 // wait, region release and record load of a step).
 #ifndef DGAN_COST_NS_PER_KB
 #define DGAN_COST_NS_PER_KB 6.8
@@ -878,16 +914,20 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   std::vector<TcRec> stream_p, stream_m;
   std::vector<uint32_t> stream_off;
   std::vector<int> eitems;
-  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;   // 64-channel MMA ops issued, those reading the zero tile
+  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;   // ops issued (KSUB k16 MMAs each), those reading the zero tile
   double load_max = 0.0, load_mean = 0.0;   // cost-model load of the busiest CTA pair / the mean over pairs (balance of the LPT assignment)
   double op_ns_max = 0.0;      // the MMA term of the busiest pair's load (estimated tensor time, ns)
   int maxb = 1, ring_bytes = 0;   // accumulator slots per round of the chosen instantiation, its operand ring
+  int ksub = 4;                   // k16 MMAs per op of the instantiation (tc2_ksub)
 };
 
-static double tc2_op_ns(int N) { return DGAN_COST_OP_NS * (double)std::max(N, DGAN_COST_OP_MIN_N) / 64.0; }
+static double tc2_op_ns(int N, int ksub) {
+  return DGAN_COST_OP_NS * (double)std::max(N, DGAN_COST_OP_MIN_N) / 64.0 * (double)ksub / 4.0;
+}
 
+// force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
 static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
-                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan) {
+                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan, const int* force_shape = nullptr) {
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
@@ -895,22 +935,24 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   // fit the ring, so a step's region never overlaps the previous step's: that one is released only after this step's
   // MMAs have been issued.
   const int step_kb = (N == 64 && K == 128) ? DGAN_STEP_MAX_KB_N64 : DGAN_STEP_MAX_KB;
-  const double op_ns = tc2_op_ns(N);
+  const int ksub = tc2_ksub(K);
+  const double op_ns = tc2_op_ns(N, ksub);
   double best_cost = 1e300;
   int best_shape[4] = {1, 1, 1, 1}, max_b = 0, ring_bytes = 0;
   std::vector<Tc2HostItem> best_items;
   std::vector<std::vector<int>> best_lists;
   std::vector<std::vector<int>> wins;
   for (const Tc2Kind& kind : kTc2Kinds) {
-    if (kind.n != N || kind.epi != epi || kind.out_bytes != out_bytes) continue;
+    if (kind.n != N || kind.ksub != ksub || kind.epi != epi || kind.out_bytes != out_bytes) continue;
     if (force_maxb > 0 && kind.maxb != force_maxb) continue;
-    const int mb = kind.maxb, ring = tc2_ring_bytes(N, mb, epi, out_bytes);
+    const int mb = kind.maxb, ring = tc2_ring_bytes(N, mb, ksub, epi, out_bytes);
     const int step_max = std::min((ring / 3) & ~1023, step_kb * 1024);
   for (int wh = 1; wh <= 2; ++wh)
     for (int ww = 1; ww <= 8; ++ww)
       for (int sy = 1; sy <= (wh > 1 ? 2 : 1); ++sy)
         for (int sx = 1; sx <= (ww > 1 ? 2 : 1); ++sx) {
           if (wh * ww > std::min(max_acc, mb) || wh > h_grid || ww > std::max(w_grid, 1)) continue;
+          if (force_shape != nullptr && (wh != force_shape[0] || ww != force_shape[1] || sy != force_shape[2] || sx != force_shape[3])) continue;
           tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
           std::vector<Tc2HostItem> items(wins.size());
           for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, mb, max_a, step_max, &items[i]);
@@ -995,7 +1037,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         }
   }
   if (max_b == 0) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
-  plan->maxb = max_b; plan->ring_bytes = ring_bytes;
+  plan->maxb = max_b; plan->ring_bytes = ring_bytes; plan->ksub = ksub;
   plan->shape[0] = best_shape[0]; plan->shape[1] = best_shape[1]; plan->shape[2] = best_shape[2]; plan->shape[3] = best_shape[3];
   plan->n_pairs = n_pairs;
   size_t n_slots = 0;
@@ -1039,7 +1081,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         const uint32_t flags = (j == 0 ? 1u : 0u) | (j + 1 == itm.steps.size() ? 2u : 0u);
         TcRec rm{};
         rm.w[0] = (uint32_t)beg | ((uint32_t)hs.nA << 8) | ((uint32_t)hs.n_rounds << 11) | (flags << 16);
-        rm.w[1] = (uint32_t)max_b;
+        rm.w[1] = (uint32_t)max_b | ((uint32_t)ksub << 8);
         for (int o = 0; o < hs.n_rounds * max_b; ++o) rm.w[2 + o / 4] |= (uint32_t)hs.ops[o] << (8 * (o & 3));
         stream_m.push_back(rm);
         TcRec rp{};
@@ -1050,7 +1092,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         stream_p.push_back(rp);
         // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
         n_mma += hs.n_rounds * max_b; n_pad += hs.n_rounds * max_b - hs.n_real;
-        n_steps += 1; n_bytes += 2LL * hs.nA * TC_A_BYTES + (long long)hs.nB * N * 128;
+        n_steps += 1; n_bytes += 2LL * hs.nA * tc2_a_bytes(ksub) + (long long)hs.nB * tc2_b_bytes(N, ksub);
       }
     }
   }
@@ -1074,15 +1116,17 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //  * progress: a step's region is released only once the next step's MMAs are issued (unless it ends its item), so
 //    no step inside an item may wait for the step right before it (dep >= 2);
 //  * every (window, row pair) item is assigned to exactly one CTA pair;
-//  * the accumulator slots per round name an instantiation of TC2_KINDS, and every MMA record carries the plan's count
-//    (the launch dispatches on the plan's count, the kernel decodes the records with it).
+//  * the accumulator slots per round and the k16 MMAs per op name an instantiation of TC2_KINDS, and every MMA record
+//    carries the plan's counts (the launch dispatches on them, the kernel decodes the records and stages its operands
+//    with them).
 static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int epi, int out_bytes, const Tc2Plan& pl,
                           std::string* err) {
   auto fail = [&](const std::string& m) { *err = m; return DGAN_ERR_INVALID_ARG; };
-  const int kch = K / 64, b_tile = N * 128;
+  const int ksub = tc2_ksub(K), kch = K / (16 * ksub), a_bytes = tc2_a_bytes(ksub), b_tile = tc2_b_bytes(N, ksub);
   const int max_acc = pl.maxb;
-  if (!tc2_has_kind(N, max_acc, epi, out_bytes)) return fail("no kernel instantiation with these accumulator slots per round");
-  const int ring_bytes = tc2_ring_bytes(N, max_acc, epi, out_bytes);
+  if (pl.ksub != ksub) return fail("plan's k16 MMAs per op disagree with the direction's channels");
+  if (!tc2_has_kind(N, max_acc, ksub, epi, out_bytes)) return fail("no kernel instantiation with these accumulator slots per round");
+  const int ring_bytes = tc2_ring_bytes(N, max_acc, ksub, epi, out_bytes);
   const size_t n_pairs = (size_t)pl.n_pairs;
   if (pl.stream_off.size() != n_pairs + 1) return fail("stream_off size");
   if (pl.stream_p.size() != pl.stream_m.size()) return fail("stream sizes differ");
@@ -1112,13 +1156,14 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
       st.kc = (int)((p0.w[0] >> 8) & 0xF); st.nB = nB;
       if ((int)(m.w[0] & 0xFF) != st.beg || (int)((m.w[0] >> 8) & 7) != nA) return fail("MMA record disagrees with the producer record");
       if (nA < 1 || nA > TC2_MAX_A || nB > TC2_MAX_BSLOTS || st.kc >= kch) return fail("step field out of range");
-      st.end = st.beg + (nA * TC_A_BYTES + nB * b_tile + 1023) / 1024;
+      st.end = st.beg + (nA * a_bytes + nB * b_tile + 1023) / 1024;
       if (st.end * 1024 > ring_bytes) return fail("step region outside the ring");
       if (dep < 1 || dep > TC2_NSLOT) return fail("dep out of range");
       for (int b = 0; b < 8; ++b) st.b[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3)));
       const uint32_t flags = (m.w[0] >> 16) & 3u;
       const int n_rounds = (int)((m.w[0] >> 11) & 0x1F);
-      if ((int)m.w[1] != max_acc) return fail("MMA record disagrees with the plan on the accumulator slots per round");
+      if ((int)(m.w[1] & 0xFFu) != max_acc) return fail("MMA record disagrees with the plan on the accumulator slots per round");
+      if ((int)(m.w[1] >> 8) != ksub) return fail("MMA record disagrees with the instantiation on the k16 sub-tiles per op");
       if (n_rounds < 1 || n_rounds * max_acc > TC2_OP_BYTES) return fail("round count out of range");
       if (dep == 1 && !(flags & 1u)) return fail("ring deadlock: a step waits for the step before it, which is released only after it");
       if (flags & 1u) {
@@ -1214,14 +1259,14 @@ static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& 
   return 0;
 }
 
-template <int NT, int MB, int EP, typename TOUT>
+template <int NT, int MB, int KS, int EP, typename TOUT>
 static cudaError_t tc2_optin() {
-  return cudaFuncSetAttribute(tc_bsgemm2_kernel<NT, MB, EP, TOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              Tc2Cfg<NT, MB, EP, (int)sizeof(TOUT)>::SMEM_BYTES);
+  return cudaFuncSetAttribute(tc_bsgemm2_kernel<NT, MB, KS, EP, TOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              Tc2Cfg<NT, MB, KS, EP, (int)sizeof(TOUT)>::SMEM_BYTES);
 }
 
 static int tc2_optin_all() {
-#define TC2_OPTIN(NT, MB, EP, T) DGAN_CUDA_CHECK((tc2_optin<NT, MB, EP, T>()));
+#define TC2_OPTIN(NT, MB, KS, EP, T) DGAN_CUDA_CHECK((tc2_optin<NT, MB, KS, EP, T>()));
   TC2_KINDS(TC2_OPTIN)
 #undef TC2_OPTIN
   return 0;
@@ -1236,7 +1281,7 @@ static int tc2_launch_impl(TcState& st, int64_t* launches, const TcWeights& w, c
   CUtensorMap tm_a;
   int rc;
   if (pre_a != nullptr) tm_a = *pre_a;          // encoded once per workspace by the caller
-  else if ((rc = tc_make_map(st, &tm_a, in, (uint64_t)w.K, (uint64_t)n_pad, (uint64_t)w.P_in, 128))) return rc;
+  else if ((rc = tc_make_map(st, &tm_a, in, (uint64_t)w.K, (uint64_t)n_pad, (uint64_t)w.P_in, 128, tc2_box_k(w.K)))) return rc;
   CUtensorMap tm_out = tm_a;                     // placeholder when unused
   if (tc2_tma_epilogue(w.N, epi, (int)sizeof(TOUT))) {
     if (pre_out != nullptr) tm_out = *pre_out;
@@ -1252,11 +1297,12 @@ static int tc2_launch_impl(TcState& st, int64_t* launches, const TcWeights& w, c
   const int grid = 2 * w2s.n_pairs;       // pairs without work find -1 in slot 0 and fall through
   cudaError_t le = cudaSuccess;
   bool found = false;
-#define TC2_GO(NT, MB, EP, T)                                                                                          \
+  const int ksub = tc2_ksub(w.K);
+#define TC2_GO(NT, MB, KS, EP, T)                                                                                      \
   if constexpr (std::is_same<T, TOUT>::value) {                                                                      \
-    if (!found && w.N == NT && w2s.maxb == MB && epi == EP) {                                                         \
+    if (!found && w.N == NT && w2s.maxb == MB && ksub == KS && epi == EP) {                                           \
       found = true;                                                                                                   \
-      le = launch_pdl(tc_bsgemm2_kernel<NT, MB, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
+      le = launch_pdl(tc_bsgemm2_kernel<NT, MB, KS, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, KS, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
                       tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, \
                       bias, (EP == EPI_FINAL_SIGMOID1 || EP == EPI_FINAL_TANH3) ? 0 : w.bias_pstride, fa);              \
     }                                                                                                                 \

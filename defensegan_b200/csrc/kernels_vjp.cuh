@@ -3,7 +3,7 @@
 //   d(pre) = dy * act'(y)        act' = y(1-y) (sigmoid) | 1 - y^2 (tanh), from the same fp32 y the epilogues use
 //
 // fp32 path: d(pre) goes to the [n_pad][H*W*C] buffer the last layer's backward reads.
-// fp16 path: it goes to the last layer's 4x4 block tensor [n_blocks][n_pad][64] (column (li*4+lj)*C_out + co), scaled
+// fp16 path: it goes to the last layer's 4x4 block tensor [n_blocks][n_pad][16*C_out] (column (li*4+lj)*C_out + co), scaled
 // per row by a power of two s_n chosen so that the row's largest |d(pre)| * s_n lies in [8, 16) - the ceiling the
 // MNIST MSE cotangent reaches with the projection's fixed scale.  Being powers of two, the scales are exact: undoing
 // them after the backward (scale_copy_kernel) makes the result independent of |dy| up to the fp32/fp16 range limits.
@@ -69,8 +69,8 @@ __global__ void __launch_bounds__(1024) cotangent_scale_kernel(float* __restrict
 }
 
 // One thread per element of y [n_rows][w_out][w_out][CO].  BLOCKS (fp16 path): dblk[blk][n][(li*4+lj)*CO + co] =
-// fp16(d(pre) * scale[n]) for pixel (4*by+li, 4*bx+lj), blk = by * (w_out/4) + bx; the K-padding columns are not
-// touched.  Otherwise dpre[n][i] = d(pre) (rows share y's layout).
+// fp16(d(pre) * scale[n]) for pixel (4*by+li, 4*bx+lj), blk = by * (w_out/4) + bx.  Otherwise dpre[n][i] = d(pre)
+// (rows share y's layout).
 template <int ACT, int CO, bool BLOCKS>
 __global__ void __launch_bounds__(256)
 cotangent_kernel(const float* __restrict__ y, const float* __restrict__ dy, int n_rows, int w_out,
@@ -84,7 +84,7 @@ cotangent_kernel(const float* __restrict__ y, const float* __restrict__ dy, int 
   const int pix = r / CO, co = r % CO, row = pix / w_out, col = pix % w_out;
   const int blk = (row >> 2) * (w_out >> 2) + (col >> 2);
   const int k = ((row & 3) * 4 + (col & 3)) * CO + co;
-  dblk[((size_t)blk * n_pad + n) * 64 + k] = __float2half_rn(d * scale[n]);
+  dblk[((size_t)blk * n_pad + n) * (16 * CO) + k] = __float2half_rn(d * scale[n]);
 }
 
 }  // namespace dgan
