@@ -82,6 +82,68 @@ PairTable linear_bwd_pairs(int n_pix) {
   return t;
 }
 
+// The generator's transposed convs between the Linear (4x4 pixels of 4 * net_dim channels) and the last layer, whose
+// input is the last one's output: channels in and out, valid input rows, output rows, input raster, ReLU after the bias.
+struct DeconvSpec { int c_in, c_out, h_in, h_used, in_raster; bool relu; };
+static std::vector<DeconvSpec> deconv_specs(const dgan_desc* d) {
+  const int nd = d->net_dim;
+  if (d->arch == DGAN_ARCH_CELEBA) return {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 8, 16, 8, true}, {nd, nd, 16, 32, 16, false}};
+  if (d->use_bn)   // BN2's batch statistics cover all 8x8 outputs of Generator.2; the 7x7 crop comes after BN+ReLU
+    return {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 7, 14, 8, true}};
+  return {{4 * nd, 2 * nd, 4, 7, 4, true}, {2 * nd, nd, 7, 14, 7, true}};
+}
+
+// Every layer-direction of the fp16 path, in launch-site and profile-kind order: layer l forward, layer l backward, ...,
+// last layer forward, last layer backward.  A function of the desc alone: the CPU tests plan without a GPU.
+// With BatchNorm after a layer (use_bn: the Linear, Generator.2 and Generator.3) its forward writes fp32 pre-activations
+// without the ReLU, and the backward into its output applies no mask (the BN backward does both).
+static std::vector<TcDir> tc_directions(const dgan_desc* d) {
+  const bool celeba = d->arch == DGAN_ARCH_CELEBA;
+  const int nd = d->net_dim, c_img = celeba ? 3 : 1;
+  std::vector<TcDir> dirs;
+  auto add = [&](const std::string& name, const std::string& kind, int N, int K, int P_in, int P_out, int n_tiles,
+                 PairTable tab, int h_grid, int w_grid, int epi, int out_bytes) {
+    TcDir t;
+    t.name = name; t.kind = kind; t.N = N; t.K = K; t.P_in = P_in; t.P_out = P_out; t.n_tiles = n_tiles;
+    t.tab = std::move(tab); t.h_grid = h_grid; t.w_grid = w_grid; t.max_acc = tc2_maxb(N);
+    t.epi = epi; t.out_bytes = out_bytes;
+    dirs.push_back(std::move(t));
+  };
+  // a GEMM layer's directions have one weight tile more than their pairs use: the all-zero tile of tc_with_zero_tile()
+  const bool bn0 = d->use_bn != 0;
+  add("Linear.fwd", "Linear.fwd", 4 * nd, d->latent_dim, 1, 16, 17, tc_with_zero_tile(linear_fwd_pairs(16), 16), 4, 4,
+      bn0 ? EPI_BIAS : EPI_BIAS_RELU, bn0 ? 4 : 2);
+  dirs.back().bias_pstride = 4 * nd;                 // bias index f = pixel * C_out + c
+  // dz as TC_LINEAR_SPLIT partial sums over the 16 pixels, one accumulator per window
+  add("Linear.bwd", "Linear.bwd", d->latent_dim, 4 * nd, 16, TC_LINEAR_SPLIT, 17, linear_split_pairs(16), 1, TC_LINEAR_SPLIT,
+      EPI_NONE, 4);
+  dirs.back().max_acc = 1;
+  bool mask_in = !bn0;                               // the backward into the previous layer's output applies its ReLU mask
+  const std::vector<DeconvSpec> specs = deconv_specs(d);
+  int li = 2;
+  for (const DeconvSpec& sp : specs) {
+    const std::string nm = "Generator." + std::to_string(li == 4 ? 5 : li);
+    const bool bn = d->use_bn && li <= 3;
+    add(nm + ".fwd", nm + ".fwd", sp.c_out, sp.c_in, sp.in_raster * sp.in_raster, sp.h_used * sp.h_used, kTaps + 1,
+        tc_with_zero_tile(deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.h_used, sp.h_used,
+        (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2);
+    add(nm + ".bwd", nm + ".bwd", sp.c_in, sp.c_out, sp.h_used * sp.h_used, sp.in_raster * sp.in_raster, kTaps + 1,
+        tc_with_zero_tile(deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.in_raster,
+        sp.in_raster, mask_in ? EPI_MASK : EPI_NONE, 2);
+    mask_in = sp.relu && !bn;
+    ++li;
+  }
+  // the last layer on 4x4 blocks of image pixels (16 weight tiles per direction); its forward computes the loss
+  const int fh = specs.back().h_used, n_blocks = (fh / 2) * (fh / 2);
+  const std::string fn = celeba ? "Generator.6" : "Generator.5";
+  add("last.fwd", fn + "+loss.fwd", 16 * c_img, nd, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2,
+      celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2);
+  // K: the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
+  add("last.bwd", fn + ".bwd", nd, 16 * c_img, n_blocks, fh * fh, 16, final_block_bwd_pairs(fh, fh), fh, fh,
+      mask_in ? EPI_MASK : EPI_NONE, 2);
+  return dirs;
+}
+
 // ---------------------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------------------
@@ -95,7 +157,6 @@ struct DevTable {
 struct GemmLayer {
   // forward: [P_in][N][C_in] -> [P_out][N][C_out]
   int P_in, C_in, P_out, C_out;
-  int h_in, w_in, h_used, w_used;  // spatial geometry (Linear: 1x1 -> 4x4)
   bool relu;                       // ReLU after bias (false: CelebA Generator.5)
   DevTable fwd, bwd;
   PairTable fwd_host, bwd_host;
@@ -107,9 +168,6 @@ struct GemmLayer {
   const float* bn_offset = nullptr;   // use_bn: Generator.BN{1,2,3}.offset / .scale (else null)
   const float* bn_scale = nullptr;
   int bn_per_pixel = 0;               // BN1 normalises each flat feature (axes [0]); BN2/3 each channel (axes [0,1,2])
-  // fp16 K-major tiles for the tensor-core path (kernels_tc.cuh): [tile][N rows][K cols]
-  TcWeights tc_f, tc_b;
-  TcWeights2 tc2_f, tc2_b;
 };
 
 struct FinalLayer {
@@ -117,6 +175,7 @@ struct FinalLayer {
   const float* w = nullptr;  // [25][C_out][C_in] == the TF filter layout
   const float* bias = nullptr;
   int n_bands = 0;
+  int n_blocks = 0;          // fp16 path: the 4x4 blocks of image pixels its GEMMs treat as pixels
   size_t fwd_smem = 0, bwd_smem = 0;
 };
 
@@ -134,8 +193,7 @@ struct dgan_ctx {
   int64_t last_launches = 0;
   int64_t launches = 0;
   TcState tc;
-  TcFinal tc_fin;
-  TcWeights2 tc2_fin_f, tc2_fin_b;
+  std::vector<TcDir> tc_dirs;          // fp16 path: tc_directions() with weight tiles and schedules
   // optional per-launch CUDA-event timing (dgan_profile_*): serialises nothing by itself but
   // adds two event records per launch, so it is never enabled in a timed benchmark pass
   bool profile = false;
@@ -230,10 +288,8 @@ struct Workspace {
   std::vector<float*> pre_h;           // fp16 path, use_bn: pre-normalisation outputs, fp32 (null otherwise)
   __half* z_h = nullptr;
   std::vector<unsigned long long*> maskbits;   // fp16 path: 1-bit ReLU masks per hidden layer output
-  // fp16 CTA-pair path: TMA descriptors of every launch site, encoded once per workspace
-  // index 2l = forward of layer l (in, out), 2l+1 = backward of layer l; 2nl = last-layer forward, 2nl+1 = its backward
+  // fp16 path: the TMA descriptors of each layer-direction's input and output, indexed as tc_dirs (build_maps)
   std::vector<CUtensorMap> map_in, map_out;
-  bool have_maps = false;
   unsigned* mom_counter = nullptr;     // fp16 path: [n_pad / 128] tickets of the split-K Linear backward's momentum tail
   __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][16 * C_out] scaled dL/dpre of the last layer
   int n_loss_parts = 0, n_g_parts = 1;
@@ -264,8 +320,8 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base) {
   w.g = (float*)take(np * latent * 4 * w.n_g_parts);
   if (tc) w.z_h = (__half*)take(np * latent * 2);
   if (tc) w.mom_counter = (unsigned*)take(np / kRowTile * sizeof(unsigned));
-  if (tc) w.dblk = (__half*)take((size_t)c->tc_fin.n_blocks * np * 16 * c->tc_fin.C_out * 2);
-  w.n_loss_parts = tc ? c->tc_fin.n_blocks : c->fin.n_bands;
+  if (tc) w.dblk = (__half*)take((size_t)c->fin.n_blocks * np * 16 * c->fin.C_out * 2);
+  w.n_loss_parts = tc ? c->fin.n_blocks : c->fin.n_bands;
   w.loss_stride_n = tc ? 1 : (size_t)w.n_loss_parts;          // fp16 path: [block][n_pad] (coalesced epilogue stores)
   w.loss_stride_b = tc ? (size_t)np : 1;
   for (const GemmLayer& l : c->layers) {
@@ -378,35 +434,46 @@ static int launch_final_bwd(dgan_ctx* c, const Workspace& w, const TOUT* mask_sr
   return 0;
 }
 
-static int tcx_launch(dgan_ctx* c, const TcWeights& w1, const TcWeights2& w2, const __half* in, __half* out, int n_pad,
-                      int epi, const float* bias, cudaStream_t s,
-                      unsigned long long* mb_out = nullptr, const unsigned long long* mb_in = nullptr,
-                      const CUtensorMap* pre_a = nullptr, const CUtensorMap* pre_out = nullptr);
+// What layer-direction i of the fp16 path (tc_dirs order) reads and writes in workspace w.  mask: the 1-bit ReLU masks
+// of the activation it writes (forward) or whose gradient it writes (backward); bias: its epilogue's.
+struct TcIo { const void* in; void* out; unsigned long long* mask; const float* bias; };
+static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i) {
+  const int nl = (int)c->layers.size(), l = i / 2;
+  if (i == 2 * nl) return {w.act_h[nl - 1], w.dblk, nullptr, c->fin.bias};
+  if (i % 2 == 0)       // a BatchNorm layer's GEMM writes its fp32 pre-activations
+    return {l == 0 ? (const void*)w.z_h : w.act_h[l - 1], w.pre_h[l] ? (void*)w.pre_h[l] : w.act_h[l], w.maskbits[l],
+            c->layers[l].bias};
+  if (l == 0) return {w.dact_h[0], w.g, nullptr, nullptr};
+  return {l == nl ? w.dblk : w.dact_h[l], w.dact_h[l - 1], w.maskbits[l - 1], nullptr};
+}
 
-// Encode the TMA descriptors of all launch sites for this workspace (once per call instead of per launch).
+// Encode the TMA descriptors of every layer-direction's input and output for this workspace.
 static int build_maps(dgan_ctx* c, Workspace& w) {
   if (c->desc.precision != DGAN_PREC_FP16) return 0;
-  const int nl = (int)c->layers.size();
-  w.map_in.assign((size_t)2 * nl + 2, CUtensorMap{});
-  w.map_out.assign((size_t)2 * nl + 2, CUtensorMap{});
+  w.map_in.assign(c->tc_dirs.size(), CUtensorMap{});
+  w.map_out.assign(c->tc_dirs.size(), CUtensorMap{});
   int rc;
-  auto mk = [&](CUtensorMap* m, const void* base, int K, int P, uint32_t box_rows = 128) {
-    return tc_make_map(c->tc, m, base, (uint64_t)K, (uint64_t)w.n_pad, (uint64_t)P, box_rows, tc2_box_k(K));
-  };
-  for (int l = 0; l < nl; ++l) {
-    const GemmLayer& L = c->layers[l];
-    const void* fin = (l == 0) ? (const void*)w.z_h : (const void*)w.act_h[l - 1];
-    if ((rc = mk(&w.map_in[2 * l], fin, L.C_in, L.P_in))) return rc;
-    if ((rc = mk(&w.map_out[2 * l], w.act_h[l], L.C_out, L.P_out, TC2_STORE_ROWS))) return rc;   // unused by BN layers (float epilogue)
-    if ((rc = mk(&w.map_in[2 * l + 1], w.dact_h[l], L.C_out, L.P_out))) return rc;
-    if (l >= 1 && (rc = mk(&w.map_out[2 * l + 1], w.dact_h[l - 1], L.C_in, L.P_in, TC2_STORE_ROWS))) return rc;
+  for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
+    const TcDir& t = c->tc_dirs[i];
+    const TcIo io = tc_io(c, w, (int)i);
+    if ((rc = tc_make_map(c->tc, &w.map_in[i], io.in, (uint64_t)t.K, (uint64_t)w.n_pad, (uint64_t)t.P_in, 128, tc2_box_k(t.K))))
+      return rc;
+    w.map_out[i] = w.map_in[i];      // a placeholder where the epilogue does not store through TMA
+    if (tc2_tma_epilogue(t.N, t.epi, t.out_bytes) &&
+        (rc = tc_make_map(c->tc, &w.map_out[i], io.out, (uint64_t)t.N, (uint64_t)w.n_pad, (uint64_t)t.P_out, TC2_STORE_ROWS)))
+      return rc;
   }
-  const GemmLayer& last = c->layers[nl - 1];
-  if ((rc = mk(&w.map_in[2 * nl], w.act_h[nl - 1], c->fin.C_in, last.P_out))) return rc;
-  if ((rc = mk(&w.map_in[2 * nl + 1], w.dblk, 16 * c->tc_fin.C_out, c->tc_fin.n_blocks))) return rc;   // 16-channel boxes
-  if ((rc = mk(&w.map_out[2 * nl + 1], w.dact_h[nl - 1], last.C_out, last.P_out, TC2_STORE_ROWS))) return rc;
-  w.have_maps = true;
   return 0;
+}
+
+// Layer-direction i of the fp16 path on workspace w, with the epilogue, output type and masks its table entry implies.
+// want_mask: a forward with the ReLU also stores its masks.  fa: the last layer's and the momentum tail's arguments.
+static int tc_launch(dgan_ctx* c, const Workspace& w, int i, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{}) {
+  const TcDir& t = c->tc_dirs[(size_t)i];
+  const TcIo io = tc_io(c, w, i);
+  if (t.epi == EPI_BIAS_RELU && want_mask) fa.mb_out = io.mask;
+  if (t.epi == EPI_MASK) fa.mb_in = io.mask;
+  return tc2_launch(&c->launches, t, w.map_in[(size_t)i], w.map_out[(size_t)i], io.out, w.n_pad, io.bias, s, fa);
 }
 
 // ---- batch-statistics BatchNorm of layer l on either path's activations (tflib/ops/batchnorm.py:80-93) ----
@@ -454,30 +521,17 @@ static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, i
   int rc;
   const int nl = (int)c->layers.size();
   if (c->desc.precision == DGAN_PREC_FP16) {
-    const __half* in = w.z_h;
     for (int l = 0; l < nl; ++l) {
-      const GemmLayer& L = c->layers[l];
       ProfScope ps(c, 2 * l, s);
-      if (L.bn_scale != nullptr) {               // pre = GEMM + bias (fp32 out);  act = relu(BN_batchstat(pre)) (fp16)
-        TcFinalArgs fa{};
-        if ((rc = tc2_launch_impl<float>(c->tc, &c->launches, L.tc_f, L.tc2_f, in, w.pre_h[l], w.n_pad, EPI_BIAS, L.bias, s, &fa,
-                                         w.have_maps ? &w.map_in[2 * l] : nullptr, nullptr)))
-          return rc;
-        if ((rc = bn_forward_t<float, __half>(c, w, l, w.pre_h[l], w.act_h[l], s))) return rc;
-      } else if ((rc = tcx_launch(c, L.tc_f, L.tc2_f, in, w.act_h[l], w.n_pad, L.relu ? EPI_BIAS_RELU : EPI_BIAS, L.bias, s,
-                                  (L.relu && want_grad) ? w.maskbits[l] : nullptr, nullptr,
-                                  w.have_maps ? &w.map_in[2 * l] : nullptr, w.have_maps ? &w.map_out[2 * l] : nullptr))) {
-        return rc;
-      }
-      in = w.act_h[l];
+      if ((rc = tc_launch(c, w, 2 * l, s, want_grad))) return rc;
+      // with BatchNorm the GEMM wrote pre = GEMM + bias (fp32):  act = relu(BN_batchstat(pre)) (fp16)
+      if (c->layers[l].bn_scale != nullptr && (rc = bn_forward_t<float, __half>(c, w, l, w.pre_h[l], w.act_h[l], s))) return rc;
     }
     ProfScope ps(c, 2 * nl, s);
     TcFinalArgs fa{};
     fa.x = x; fa.y = w.y; fa.loss_part = w.loss_part; fa.R = R; fa.B = B; fa.n_rows = w.n_rows;
-    fa.nbx = c->tc_fin.nbx; fa.w_out = c->tc_fin.w_out; fa.gscale = c->tc.grad_scale; fa.write_y = want_y ? 1 : 0;
-    return tc2_launch_impl<__half>(c->tc, &c->launches, c->tc_fin.f, c->tc2_fin_f, in, w.dblk, w.n_pad,
-                                   c->tc_fin.C_out == 1 ? EPI_FINAL_SIGMOID1 : EPI_FINAL_TANH3, c->fin.bias, s, &fa,
-                                   w.have_maps ? &w.map_in[2 * nl] : nullptr, nullptr);
+    fa.nbx = c->fin.w_in / 2; fa.w_out = 2 * c->fin.w_in; fa.gscale = c->tc.grad_scale; fa.write_y = want_y ? 1 : 0;
+    return tc_launch(c, w, 2 * nl, s, false, fa);
   }
   const float* in = w.z;
   for (int l = 0; l < nl; ++l) {
@@ -508,37 +562,22 @@ static int run_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s, Momentu
   int rc;
   const int nl = (int)c->layers.size();
   if (c->desc.precision == DGAN_PREC_FP16) {
-    const GemmLayer& last = c->layers[nl - 1];
     // with BatchNorm after layer j the GEMM writes d(act_j) unmasked and the BN backward turns it into d(pre_j) in place
-    auto bn_backward_h = [&](int j) -> int { return bn_backward_t<float, __half>(c, w, j, w.pre_h[j], w.act_h[j], w.dact_h[j], s); };
-    {
-      ProfScope ps(c, 2 * nl + 1, s);
-      const bool bn = last.bn_scale != nullptr, mask = last.relu && !bn;
-      if ((rc = tcx_launch(c, c->tc_fin.b, c->tc2_fin_b, w.dblk, w.dact_h[nl - 1], w.n_pad, mask ? EPI_MASK : EPI_NONE,
-                           nullptr, s, nullptr, mask ? w.maskbits[nl - 1] : nullptr,
-                           w.have_maps ? &w.map_in[2 * nl + 1] : nullptr, w.have_maps ? &w.map_out[2 * nl + 1] : nullptr)))
-        return rc;
-      if (bn && (rc = bn_backward_h(nl - 1))) return rc;
-    }
-    for (int l = nl - 1; l >= 1; --l) {
-      const GemmLayer& L = c->layers[l];
-      const bool bn = c->layers[l - 1].bn_scale != nullptr, mask = c->layers[l - 1].relu && !bn;
+    for (int l = nl; l >= 1; --l) {       // l = nl: the last layer
       ProfScope ps(c, 2 * l + 1, s);
-      if ((rc = tcx_launch(c, L.tc_b, L.tc2_b, w.dact_h[l], w.dact_h[l - 1], w.n_pad, mask ? EPI_MASK : EPI_NONE, nullptr,
-                           s, nullptr, mask ? w.maskbits[l - 1] : nullptr,
-                           w.have_maps ? &w.map_in[2 * l + 1] : nullptr, w.have_maps ? &w.map_out[2 * l + 1] : nullptr)))
+      if ((rc = tc_launch(c, w, 2 * l + 1, s))) return rc;
+      const int j = l - 1;
+      if (c->layers[j].bn_scale != nullptr &&
+          (rc = bn_backward_t<float, __half>(c, w, j, w.pre_h[j], w.act_h[j], w.dact_h[j], s)))
         return rc;
-      if (bn && (rc = bn_backward_h(l - 1))) return rc;
     }
-    const GemmLayer& L0 = c->layers[0];
     ProfScope ps(c, 1, s);
     TcFinalArgs fa{};
     if (mom.tail) {      // the CTA that completes a row tile's partial sums applies the momentum update
       fa.mz = w.z; fa.mv = w.v; fa.mz_h = w.z_h; fa.m_gmul = grad_multiplier(c); fa.m_lr = mom.lr; fa.m_mu = mom.mu;
       fa.m_counter = w.mom_counter; fa.m_nparts = w.n_g_parts; fa.m_count = (size_t)w.n_pad * c->desc.latent_dim;
     }
-    return tc2_launch_impl<float>(c->tc, &c->launches, L0.tc_b, L0.tc2_b, w.dact_h[0], w.g, w.n_pad, EPI_NONE, nullptr, s,
-                                  &fa, w.have_maps ? &w.map_in[1] : nullptr, nullptr);
+    return tc_launch(c, w, 1, s, false, fa);
   }
   auto bn_backward = [&](int l) -> int { return bn_backward_t<float, float>(c, w, l, w.pre[l], w.act[l], w.dact[l], s); };
   const GemmLayer& last = c->layers[nl - 1];
@@ -598,7 +637,7 @@ static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cu
     // reads all n_pad rows)
     const size_t row_b = (size_t)16 * f.C_out * sizeof(__half);
     DGAN_CUDA_CHECK(cudaMemset2DAsync(w.dblk + (size_t)w.n_rows * 16 * f.C_out, (size_t)w.n_pad * row_b, 0,
-                                      (size_t)(w.n_pad - w.n_rows) * row_b, (size_t)c->tc_fin.n_blocks, s));
+                                      (size_t)(w.n_pad - w.n_rows) * row_b, (size_t)f.n_blocks, s));
   }
   const size_t total = (size_t)w.n_rows * c->hwc;
   const unsigned grid = (unsigned)((total + 255) / 256);
@@ -611,24 +650,31 @@ static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cu
   return 0;
 }
 
-static int check_ws(const dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out) {
+// fp16 path: plan and upload the schedules of every layer-direction for this many latent rows (cached in the handle).
+// Planning allocates and synchronises, so it happens before any kernel of a call is enqueued (and never while the L-step
+// loop is captured); a caller that sized its workspace with dgan_workspace_bytes has had it done there.
+static int plan_all(dgan_ctx* c, int n_rows) {
+  if (c->desc.precision != DGAN_PREC_FP16) return 0;
+  const int n_mpairs = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile) / (2 * kRowTile);
+  int rc;
+  for (TcDir& t : c->tc_dirs)
+    if ((rc = tc2_get_schedule(t, n_mpairs, c->tc.num_sms / 2, &c->allocs))) return rc;
+  return 0;
+}
+
+// Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
+// workspace's tensor maps.
+static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
+  int rc;
+  if ((rc = plan_all(c, n_rows))) return rc;
   *out = carve(c, n_rows, ws);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes));
     return DGAN_ERR_WORKSPACE;
   }
-  return 0;
-}
-
-// one hidden layer-direction on the tensor cores
-static int tcx_launch(dgan_ctx* c, const TcWeights& w1, const TcWeights2& w2, const __half* in, __half* out, int n_pad,
-                      int epi, const float* bias, cudaStream_t s, unsigned long long* mb_out,
-                      const unsigned long long* mb_in, const CUtensorMap* pre_a, const CUtensorMap* pre_out) {
-  TcFinalArgs fa{};
-  fa.mb_out = mb_out; fa.mb_in = mb_in;
-  return tc2_launch_impl<__half>(c->tc, &c->launches, w1, w2, in, out, n_pad, epi, bias, s, &fa, pre_a, pre_out);
+  return build_maps(c, *out);
 }
 
 // element counts of the weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights)
@@ -656,39 +702,6 @@ static float grad_multiplier(const dgan_ctx* c) {
 // =========================================================================================
 // C ABI
 // =========================================================================================
-namespace {
-struct PlanDir { std::string name; int N, K; dgan::PairTable tab; int h, w, force_acc, epi, out_bytes; };
-// every tensor-core layer-direction of the fp16 path, as create_impl sets it up (host only)
-std::vector<PlanDir> plan_dirs(const dgan_desc* d) {
-  using namespace dgan;
-  typedef PlanDir Dir;
-  const bool celeba = d->arch == DGAN_ARCH_CELEBA;
-  const int nd = d->net_dim, latent = d->latent_dim;
-  std::vector<Dir> dirs;
-  dirs.push_back({"Linear.fwd", 4 * nd, latent, linear_fwd_pairs(16), 4, 4, 0, EPI_BIAS_RELU, 2});
-  dirs.push_back({"Linear.bwd", latent, 4 * nd, linear_split_pairs(16), 1, TC_LINEAR_SPLIT, 1, EPI_NONE, 4});
-  struct DSpec { int c_in, c_out, h_in, h_used, in_raster; bool relu; };
-  std::vector<DSpec> specs;
-  if (celeba) specs = {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 8, 16, 8, true}, {nd, nd, 16, 32, 16, false}};
-  else if (d->use_bn) specs = {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 7, 14, 8, true}};   // BN2 sees the 8x8 raster (create_impl)
-  else specs = {{4 * nd, 2 * nd, 4, 7, 4, true}, {2 * nd, nd, 7, 14, 7, true}};
-  int li = 2;
-  for (const DSpec& sp : specs) {
-    const std::string nm = "Generator." + std::to_string(li == 4 ? 5 : li);
-    const bool bn = d->use_bn && li <= 3;          // a BN layer's GEMMs neither apply the ReLU nor its mask
-    dirs.push_back({nm + ".fwd", sp.c_out, sp.c_in, tc_with_zero_tile(deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps),
-                    sp.h_used, sp.h_used, 0, (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, 2});
-    dirs.push_back({nm + ".bwd", sp.c_in, sp.c_out, tc_with_zero_tile(deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps),
-                    sp.in_raster, sp.in_raster, 0, d->use_bn ? EPI_NONE : EPI_MASK, 2});
-    ++li;
-  }
-  const int fh = celeba ? 32 : 14, c_img = celeba ? 3 : 1;
-  dirs.push_back({"last.fwd", 16 * c_img, nd, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2, 0, celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2});
-  dirs.push_back({"last.bwd", nd, 16 * c_img, final_block_bwd_pairs(fh, fh), fh, fh, 0, celeba ? EPI_NONE : EPI_MASK, 2});
-  return dirs;
-}
-}  // namespace
-
 extern "C" {
 
 int dgan_abi_version(void) { return DGAN_ABI_VERSION; }
@@ -730,7 +743,7 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
   // ---- Linear (Generator.Input): [1][N][latent] -> [16][N][4*nd]
   {
     GemmLayer L{};
-    L.P_in = 1; L.C_in = latent; L.P_out = 16; L.C_out = 4 * nd; L.h_in = 1; L.w_in = 1; L.h_used = 4; L.w_used = 4;
+    L.P_in = 1; L.C_in = latent; L.P_out = 16; L.C_out = 4 * nd;
     L.relu = true;
     L.fwd_host = linear_fwd_pairs(16); L.bwd_host = linear_bwd_pairs(16);
     const float* W = weights[0];             // (latent, 16*4nd), column f = pixel*4nd + c
@@ -745,18 +758,13 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
     c->layers.push_back(L);
   }
   // ---- hidden deconvs
-  struct DSpec { int c_in, c_out, h_in, h_used; bool relu; int in_raster; };
-  std::vector<DSpec> specs;
-  if (celeba) specs = {{4 * nd, 2 * nd, 4, 8, true, 4}, {2 * nd, nd, 8, 16, true, 8}, {nd, nd, 16, 32, false, 16}};
-  else if (d->use_bn)   // BN2's batch statistics cover all 8x8 outputs of Generator.2; the 7x7 crop comes after BN+ReLU
-    specs = {{4 * nd, 2 * nd, 4, 8, true, 4}, {2 * nd, nd, 7, 14, true, 8}};
-  else specs = {{4 * nd, 2 * nd, 4, 7, true, 4}, {2 * nd, nd, 7, 14, true, 7}};
+  const std::vector<DeconvSpec> specs = deconv_specs(d);
   int wi = d->use_bn ? 4 : 2;
   int di = 0;
-  for (const DSpec& sp : specs) {
+  for (const DeconvSpec& sp : specs) {
     GemmLayer L{};
     L.P_in = sp.in_raster * sp.in_raster; L.C_in = sp.c_in; L.P_out = sp.h_used * sp.h_used; L.C_out = sp.c_out;
-    L.h_in = L.w_in = sp.in_raster; L.h_used = L.w_used = sp.h_used; L.relu = sp.relu;
+    L.relu = sp.relu;
     L.fwd_host = deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster);
     L.bwd_host = deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster);
     const float* F = weights[wi];            // (5,5,C_out,C_in)
@@ -778,9 +786,10 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
   // ---- final layer
   {
     FinalLayer& f = c->fin;
-    f.h_in = f.w_in = celeba ? 32 : 14; f.C_in = nd; f.C_out = c->C; f.act = celeba ? ACT_TANH : ACT_SIGMOID;
+    f.h_in = f.w_in = specs.back().h_used; f.C_in = nd; f.C_out = c->C; f.act = celeba ? ACT_TANH : ACT_SIGMOID;
     f.w = weights[wi]; f.bias = weights[wi + 1];
     f.n_bands = (2 * f.h_in + kBandRows - 1) / kBandRows;
+    f.n_blocks = (f.h_in / 2) * (f.w_in / 2);
     f.fwd_smem = ((size_t)kTaps * f.C_out * f.C_in + (size_t)(kBandRows / 2 + 2) * f.w_in * (f.C_in + 4)) * 4;
     f.bwd_smem = (size_t)kTaps * f.C_out * f.C_in * 4;
   }
@@ -803,58 +812,47 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
   OPTIN((final_fwd_loss_kernel<__half, 3, ACT_TANH>), 100 * 1024);
 #undef OPTIN
   if (d->precision == DGAN_PREC_FP16) {
-    std::vector<TcLayerSpec> tspecs;
-    for (GemmLayer& L : c->layers) {
-      TcLayerSpec t{};
-      t.P_in = L.P_in; t.C_in = L.C_in; t.P_out = L.P_out; t.C_out = L.C_out;
-      t.h_in = L.h_in; t.w_in = L.w_in; t.h_used = L.h_used; t.w_used = L.w_used;
-      t.fwd = &L.fwd_host; t.bwd = &L.bwd_host;
-      t.w_fwd_kmajor_src = (&L == &c->layers[0]) ? nullptr : L.wb;  // F[t][co][ci]: rows co (N), cols ci (K)
-      t.w_bwd_kmajor_src = (&L == &c->layers[0]) ? nullptr : L.wf;  // Ff[t][ci][co]: rows ci (N), cols co (K)
-      t.linear_W = (&L == &c->layers[0]) ? weights[0] : nullptr;
-      t.linear_Wt = (&L == &c->layers[0]) ? L.wb : nullptr;
-      t.out_f = &L.tc_f; t.out_b = &L.tc_b; t.bias_pstride = L.bias_pstride;
-      tspecs.push_back(t);
-    }
-    if ((rc = tc_build(c->tc, tspecs, latent, &c->allocs, s))) return fail(rc);
-    if ((rc = tc_build_final(c->tc, &c->tc_fin, c->fin.w, c->fin.h_in, c->fin.w_in, c->fin.C_in, c->fin.C_out,
-                             c->fin.act, &c->allocs, s)))
-      return fail(rc);
-    c->tc.allocs = &c->allocs;
-    {
-      if ((rc = tc2_optin_all())) return fail(rc);
-      for (size_t l = 0; l < c->layers.size(); ++l) {
-        GemmLayer& L = c->layers[l];
-        if ((rc = tc2_build_direction(c->tc, L.tc_f, &L.tc2_f, tc_with_zero_tile(L.fwd_host, L.tc_f.n_tiles - 1), L.h_used, L.w_used, 0, &c->allocs, s))) return fail(rc);
-        if (l == 0) {
-          const PairTable split = linear_split_pairs(L.P_out);
-          if ((rc = tc2_build_direction(c->tc, L.tc_b, &L.tc2_b, split, 1, TC_LINEAR_SPLIT, 1, &c->allocs, s))) return fail(rc);
-        } else if ((rc = tc2_build_direction(c->tc, L.tc_b, &L.tc2_b, tc_with_zero_tile(L.bwd_host, L.tc_b.n_tiles - 1), L.h_in, L.w_in, 0, &c->allocs, s))) {
-          return fail(rc);
-        }
+    if ((rc = tc_init(c->tc))) return fail(rc);
+    if ((rc = tc2_optin_all())) return fail(rc);
+    c->tc_dirs = tc_directions(d);
+    const int nl = (int)c->layers.size();
+    for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
+      TcDir& t = c->tc_dirs[i];
+      if (t.N != 16 && t.N != 48 && t.N != 64 && t.N != 128 && t.N != 256) { set_error("tensor-core path needs 64/128/256 output channels per pixel"); return fail(DGAN_ERR_UNSUPPORTED); }
+      // K < 64: the narrow operand of the last layer's backward (16 * C_out channels, k16 sub-tiles)
+      if (t.K % 64 != 0 && !(t.K == 16 || t.K == 48)) { set_error("tensor-core path needs input channels in multiples of 64, or 16 / 48"); return fail(DGAN_ERR_UNSUPPORTED); }
+      if (t.n_tiles > 32 || t.P_in > 65535 || t.P_out > 65535) { set_error("tensor-core schedule limits exceeded"); return fail(DGAN_ERR_UNSUPPORTED); }
+      // fp16 K-major weight tiles [n_tiles][N rows][K cols]
+      const size_t tile = (size_t)t.N * t.K;
+      if ((rc = dev_alloc(c, (void**)&t.w, (size_t)t.n_tiles * tile * 2))) return fail(rc);
+      if ((int)i < 2 * nl) {     // a GEMM layer: its tiles, then the all-zero tile of tc_with_zero_tile()
+        const GemmLayer& L = c->layers[i / 2];
+        const size_t elems = (size_t)(t.n_tiles - 1) * tile;
+        const unsigned blocks = (unsigned)((elems + 255) / 256);
+        DGAN_CUDA_CHECK(cudaMemsetAsync(t.w + elems, 0, tile * 2, s));
+        if (i % 2 == 0) tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wb, t.w, elems);        // F[t][co][ci]; Linear: Wt[q*C + c][k]
+        else if (i == 1) tc_linear_bwd_tiles_kernel<<<blocks, 256, 0, s>>>(weights[0], t.w, latent, L.C_out, L.P_out);   // W[k][q*C + c]
+        else tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wf, t.w, elems);                   // Ff[t][ci][co]
+        DGAN_CUDA_CHECK(cudaGetLastError());
       }
-      const PairTable ft = final_block_fwd_pairs(c->fin.h_in, c->fin.w_in), bt = final_block_bwd_pairs(c->fin.h_in, c->fin.w_in);
-      if ((rc = tc2_build_direction(c->tc, c->tc_fin.f, &c->tc2_fin_f, ft, c->fin.h_in / 2, c->fin.w_in / 2, 0, &c->allocs, s))) return fail(rc);
-      if ((rc = tc2_build_direction(c->tc, c->tc_fin.b, &c->tc2_fin_b, bt, c->fin.h_in, c->fin.w_in, 0, &c->allocs, s))) return fail(rc);
+      if ((rc = tc_make_map(c->tc, &t.tm_b, t.w, (uint64_t)t.K, (uint64_t)t.N, (uint64_t)t.n_tiles, (uint32_t)(t.N / 2), tc2_box_k(t.K))))
+        return fail(rc);
     }
+    if (nd != 64) { set_error("tensor-core final layer needs net_dim == 64"); return fail(DGAN_ERR_UNSUPPORTED); }
+    tc_final_tiles_kernel<<<16, 256, 0, s>>>(c->fin.w, c->fin.C_out, c->fin.C_in, c->tc_dirs[2 * nl].w, c->tc_dirs[2 * nl + 1].w);
+    DGAN_CUDA_CHECK(cudaGetLastError());
   }
-  {
-    static const char* lname_m[] = {"Linear", "Generator.2", "Generator.3"};
-    static const char* lname_c[] = {"Linear", "Generator.2", "Generator.3", "Generator.5"};
-    for (size_t l = 0; l < c->layers.size(); ++l) {
-      const std::string nm = celeba ? lname_c[l] : lname_m[l];
-      const double macs = (double)c->layers[l].fwd_host.pairs.size() * c->layers[l].C_in * c->layers[l].C_out;
-      c->kind_names.push_back(nm + ".fwd"); c->kind_macs_per_row.push_back(macs);
-      c->kind_names.push_back(nm + ".bwd"); c->kind_macs_per_row.push_back(macs);
-    }
-    double fmacs = 0;
-    for (const GemmLayer& L : c->layers) fmacs += (double)L.fwd_host.pairs.size() * L.C_in * L.C_out;
-    fmacs = (double)c->macs_per_row - fmacs;
-    const std::string fn = celeba ? "Generator.6" : "Generator.5";
-    c->kind_names.push_back(fn + "+loss.fwd"); c->kind_macs_per_row.push_back(fmacs);
-    c->kind_names.push_back(fn + ".bwd"); c->kind_macs_per_row.push_back(fmacs);
-    c->kind_names.push_back("momentum"); c->kind_macs_per_row.push_back(0.0);
+  // profile kinds: the layer-directions in tc_directions() order (both paths), then the momentum update
+  for (const TcDir& t : tc_directions(d)) c->kind_names.push_back(t.kind);
+  c->kind_names.push_back("momentum");
+  double fmacs = (double)c->macs_per_row;
+  for (const GemmLayer& L : c->layers) {
+    const double macs = (double)L.fwd_host.pairs.size() * L.C_in * L.C_out;
+    c->kind_macs_per_row.insert(c->kind_macs_per_row.end(), 2, macs);      // forward, backward
+    fmacs -= macs;
   }
+  c->kind_macs_per_row.insert(c->kind_macs_per_row.end(), 2, fmacs);        // the last layer's forward, backward
+  c->kind_macs_per_row.push_back(0.0);
   DGAN_CUDA_CHECK(cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking));
   DGAN_CUDA_CHECK(cudaGetLastError());
   return DGAN_OK;
@@ -893,38 +891,6 @@ int dgan_destroy(dgan_handle h) {
   for (void* p : h->allocs) cudaFree(p);
   delete h;
   return DGAN_OK;
-}
-
-// fp16 path: plan and upload the schedules of every layer-direction for this many latent rows (cached in the handle).
-// Planning allocates and synchronises; it happens here - a caller needs the workspace size before its first
-// dgan_reconstruct of a batch size anyway - so that dgan_reconstruct itself only enqueues kernels.
-struct TcDir { const TcWeights* w1; TcWeights2* w2; int epi, out_bytes; };
-// The tensor-core layer-directions of the fp16 path with the epilogue and output type they launch with, in the order of
-// plan_dirs: layer l forward, layer l backward, ..., last layer forward, last layer backward.
-static std::vector<TcDir> tc_dirs(dgan_ctx* c) {
-  std::vector<TcDir> dirs;
-  const int nl = (int)c->layers.size();
-  for (int l = 0; l < nl; ++l) {
-    GemmLayer& L = c->layers[(size_t)l];
-    const bool bn = L.bn_scale != nullptr;        // BN layers: float epilogue (fp32 pre-activations), see run_forward
-    dirs.push_back({&L.tc_f, &L.tc2_f, (L.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2});
-    if (l == 0) dirs.push_back({&L.tc_b, &L.tc2_b, EPI_NONE, 4});
-    else dirs.push_back({&L.tc_b, &L.tc2_b, c->layers[(size_t)l - 1].relu ? EPI_MASK : EPI_NONE, 2});
-  }
-  dirs.push_back({&c->tc_fin.f, &c->tc2_fin_f, c->tc_fin.C_out == 1 ? EPI_FINAL_SIGMOID1 : EPI_FINAL_TANH3, 2});
-  dirs.push_back({&c->tc_fin.b, &c->tc2_fin_b, c->layers[(size_t)nl - 1].relu ? EPI_MASK : EPI_NONE, 2});
-  return dirs;
-}
-
-static int plan_all(dgan_ctx* c, int n_rows) {
-  if (c->desc.precision != DGAN_PREC_FP16) return 0;
-  const int n_pad = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile), n_mpairs = n_pad / (2 * kRowTile);
-  const int n_pairs = c->tc.num_sms / 2;
-  const Tc2Schedule* sc = nullptr;
-  int rc;
-  for (const TcDir& d : tc_dirs(c))
-    if ((rc = tc2_get_schedule(c->tc, *d.w1, *d.w2, n_mpairs, n_pairs, d.epi, d.out_bytes, c->tc.allocs, (cudaStream_t)0, &sc))) return rc;
-  return 0;
 }
 
 size_t dgan_workspace_bytes(dgan_handle h, int batch, int rec_rr) {
@@ -1015,17 +981,11 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
   const float rec_lr = prm->rec_lr, momentum = prm->momentum;
   const uint64_t seed = prm->seed;
   if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
-  if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
-  if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
-  if (dgan_workspace_bytes(h, batch, rec_rr) > ws_bytes) {
-    set_error("workspace too small: need " + std::to_string(dgan_workspace_bytes(h, batch, rec_rr)) + " bytes, got " + std::to_string(ws_bytes));
-    return DGAN_ERR_WORKSPACE;
-  }
   cudaStream_t s = (cudaStream_t)stream;
   const int latent = h->desc.latent_dim;
-  Workspace w = carve(h, batch * rec_rr, ws);
+  Workspace w;
   int rc;
-  if ((rc = build_maps(h, w))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w))) return rc;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
@@ -1150,14 +1110,10 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
-  typedef PlanDir Dir;
-  const std::vector<Dir> dirs = plan_dirs(d);
-  for (const Dir& dr : dirs) {
+  for (const TcDir& dr : tc_directions(d)) {
     if (dr.N != 16 && dr.N != 48 && dr.N != 64 && dr.N != 128 && dr.N != 256) { set_error(dr.name + ": unsupported N"); return DGAN_ERR_UNSUPPORTED; }
-    int max_acc = tc2_maxb(dr.N);
-    if (dr.force_acc > 0) max_acc = std::min(max_acc, dr.force_acc);
     Tc2Plan plan;
-    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
+    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
     // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd, faults 12-13
     // (specific to narrow ops) that of the last layer's backward; the check must then fail
@@ -1210,7 +1166,7 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     for (const Tc2Kind& k : kTc2Kinds) {
       if (k.n != dr.N || k.ksub != plan.ksub || k.epi != dr.epi || k.out_bytes != dr.out_bytes || k.maxb == plan.maxb) continue;
       Tc2Plan forced;
-      if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &forced))) {
+      if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &forced))) {
         set_error(dr.name + " (" + std::to_string(k.maxb) + " slots): " + dgan_last_error());
         return rc;
       }
@@ -1224,21 +1180,20 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
 }
 
 
-// Host-side test aid (not in the public header): plan layer-direction `dir` (plan_dirs order) of an fp16 handle with
+// Host-side test aid (not in the public header): plan layer-direction `dir` (tc_directions order) of an fp16 handle with
 // exactly `maxb` accumulator slots per round from now on (0: the planner chooses again).  Schedules and captured loops
 // are re-made on the next call, so any instantiation of TC2_KINDS can be run at any batch size; the results must not
 // change, because every accumulator keeps its summation order.
 int dgan_debug_force_slots(dgan_handle h, int dir, int maxb) {
   if (h == nullptr || h->desc.precision != DGAN_PREC_FP16 || maxb < 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
-  const std::vector<TcDir> dirs = tc_dirs(h);
-  if (dir < 0 || dir >= (int)dirs.size()) { set_error("layer-direction out of range"); return DGAN_ERR_INVALID_ARG; }
-  const TcDir& d = dirs[(size_t)dir];
-  if (maxb > 0 && !tc2_has_kind(d.w1->N, maxb, tc2_ksub(d.w1->K), d.epi, d.out_bytes)) {
+  if (dir < 0 || dir >= (int)h->tc_dirs.size()) { set_error("layer-direction out of range"); return DGAN_ERR_INVALID_ARG; }
+  TcDir& d = h->tc_dirs[(size_t)dir];
+  if (maxb > 0 && !tc2_has_kind(d.N, maxb, tc2_ksub(d.K), d.epi, d.out_bytes)) {
     set_error("no kernel instantiation with " + std::to_string(maxb) + " accumulator slots per round for this layer-direction");
     return DGAN_ERR_UNSUPPORTED;
   }
-  d.w2->force_maxb = maxb;
-  d.w2->by_mpairs.clear();                  // the uploaded tables stay in h->allocs until dgan_destroy
+  d.force_maxb = maxb;
+  d.by_mpairs.clear();                      // the uploaded tables stay in h->allocs until dgan_destroy
   for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
   h->graphs.clear();
   return DGAN_OK;
@@ -1248,12 +1203,11 @@ int dgan_debug_force_slots(dgan_handle h, int dir, int maxb) {
 // written to out[0 .. n).  Returns n, or -1.
 int dgan_debug_slot_choices(dgan_handle h, int dir, int* out, int max_n) {
   if (h == nullptr || h->desc.precision != DGAN_PREC_FP16 || out == nullptr) return -1;
-  const std::vector<TcDir> dirs = tc_dirs(h);
-  if (dir < 0 || dir >= (int)dirs.size()) return -1;
-  const TcDir& d = dirs[(size_t)dir];
+  if (dir < 0 || dir >= (int)h->tc_dirs.size()) return -1;
+  const TcDir& d = h->tc_dirs[(size_t)dir];
   int n = 0;
   for (const Tc2Kind& k : kTc2Kinds)
-    if (k.n == d.w1->N && k.ksub == tc2_ksub(d.w1->K) && k.epi == d.epi && k.out_bytes == d.out_bytes && n < max_n) out[n++] = k.maxb;
+    if (k.n == d.N && k.ksub == tc2_ksub(d.K) && k.epi == d.epi && k.out_bytes == d.out_bytes && n < max_n) out[n++] = k.maxb;
   return n;
 }
 
@@ -1270,7 +1224,8 @@ int dgan_debug_probe_read(unsigned long long* out) {
 
 // Host-only developer aid (not in the public header): the plan of every layer-direction in numbers - window shape, items,
 // steps, MMAs (ops of KSUB k16 each, and k16 MMAs), operand bytes staged from L2 into shared memory (both CTAs of every
-// pair), accumulator slots per round - as text.  Layer-direction `force_dir` (plan_dirs order; -1: none) is planned
+// pair), accumulator slots per round, epilogue and output type - as text.  Layer-direction `force_dir` (tc_directions
+// order; -1: none) is planned
 // with exactly `force_maxb` slots per round, as dgan_debug_force_slots would, and, when force_shape is not NULL, with
 // exactly that window shape {wh, ww, sy, sx}.  Returns the length.
 static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, const int* force_shape,
@@ -1279,26 +1234,35 @@ static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int forc
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
   std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load"
-                    " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us | k16 MMAs\n";
+                    " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us | k16 MMAs"
+                    " | epilogue/output\n";
+  auto epi_name = [](int epi) {
+    switch (epi) {
+      case EPI_BIAS_RELU: return "bias_relu";
+      case EPI_BIAS: return "bias";
+      case EPI_MASK: return "mask";
+      case EPI_FINAL_SIGMOID1: return "final_sigmoid";
+      case EPI_FINAL_TANH3: return "final_tanh";
+      default: return "none";
+    }
+  };
   double total = 0.0;
-  const std::vector<PlanDir> dirs = plan_dirs(d);
+  const std::vector<TcDir> dirs = tc_directions(d);
   for (size_t di = 0; di < dirs.size(); ++di) {
-    const PlanDir& dr = dirs[di];
-    int max_acc = tc2_maxb(dr.N);
-    if (dr.force_acc > 0) max_acc = std::min(max_acc, dr.force_acc);
+    const TcDir& dr = dirs[di];
     Tc2Plan plan;
     const bool forced = (int)di == force_dir;
-    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h, dr.w, max_acc, forced ? force_maxb : 0, dr.epi, dr.out_bytes,
+    const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, forced ? force_maxb : 0, dr.epi, dr.out_bytes,
                             n_mpairs, n_pairs, &plan, forced ? force_shape : nullptr);
     if (rc) return -1;
-    char line[256];
+    char line[320];
     const double mb = (double)plan.n_bytes / 1e6;
     total += mb;
-    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f | %d | %.1f | %.1f | %lld\n", dr.name.c_str(),
-             dr.N, dr.K, plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3], plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots,
-             plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0),
+    snprintf(line, sizeof line, "%s | %d | %d | %dx%d, %dx%d | %zu | %d | %lld | %lld | %.1f | %.3f | %.1f | %d | %.1f | %.1f | %lld | %s/f%d\n",
+             dr.name.c_str(), dr.N, dr.K, plan.shape[0], plan.shape[1], plan.shape[2], plan.shape[3],
+             plan.hdrs.size() * (size_t)n_mpairs, plan.n_slots, plan.n_steps, plan.n_mma, mb, plan.load_max / std::max(plan.load_mean, 1.0),
              100.0 * (double)plan.n_pad / (double)std::max(plan.n_mma, 1LL), plan.maxb, plan.op_ns_max / 1e3,
-             plan.load_max / 1e3, plan.n_mma * plan.ksub);
+             plan.load_max / 1e3, plan.n_mma * plan.ksub, epi_name(dr.epi), 8 * dr.out_bytes);
     out += line;
   }
   char line[64];

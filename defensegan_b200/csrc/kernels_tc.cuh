@@ -17,26 +17,10 @@ namespace dgan {
 
 constexpr int TC_LINEAR_SPLIT = 4;           // partial sums of the Linear backward (dz)
 
-// One direction (forward or backward) of one layer on the tensor-core path.
-struct TcWeights {
-  __half* w = nullptr;          // [tiles][N][K] fp16, K contiguous
-  int N = 0, K = 0, P_in = 0, P_out = 0, n_tiles = 0;
-  int bias_pstride = 0;
-};
-
 struct TcState {
   float grad_scale = 64.f;      // fp16 gradient scaling (undone in the z update)
   void* encode_fn = nullptr;    // cuTensorMapEncodeTiled
-  std::vector<void*>* allocs = nullptr;   // the handle's allocation list (lazily built schedules are freed with it)
   int num_sms = 132;
-};
-
-struct TcLayerSpec {
-  int P_in, C_in, P_out, C_out, h_in, w_in, h_used, w_used;
-  const PairTable *fwd, *bwd;
-  const float *w_fwd_kmajor_src, *w_bwd_kmajor_src, *linear_W, *linear_Wt;
-  TcWeights *out_f, *out_b;
-  int bias_pstride;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -244,12 +228,16 @@ static int tc_upload(std::vector<void*>* allocs, const void* host, size_t bytes,
   return 0;
 }
 
-static int tc_set_direction(TcWeights* w, int N, int K, int n_tiles, int P_in, int P_out) {
-  if (N != 16 && N != 48 && N != 64 && N != 128 && N != 256) { set_error("tensor-core path needs 64/128/256 output channels per pixel"); return DGAN_ERR_UNSUPPORTED; }
-  // K < 64: the narrow operand of the last layer's backward (16 * C_out channels, k16 sub-tiles)
-  if (K % 64 != 0 && !(K == 16 || K == 48)) { set_error("tensor-core path needs input channels in multiples of 64, or 16 / 48"); return DGAN_ERR_UNSUPPORTED; }
-  if (n_tiles > 32 || P_in > 65535 || P_out > 65535) { set_error("tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
-  w->N = N; w->K = K; w->P_in = P_in; w->P_out = P_out; w->n_tiles = n_tiles;
+// The tensor-map encoder and the SM count of the current device.
+static int tc_init(TcState& st) {
+  cudaDriverEntryPointQueryResult qres;
+  void* fn = nullptr;
+  DGAN_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+  if (fn == nullptr || qres != cudaDriverEntryPointSuccess) { set_error("cuTensorMapEncodeTiled not found in the driver"); return DGAN_ERR_CUDA; }
+  st.encode_fn = fn;
+  int dev = 0;
+  DGAN_CUDA_CHECK(cudaGetDevice(&dev));
+  DGAN_CUDA_CHECK(cudaDeviceGetAttribute(&st.num_sms, cudaDevAttrMultiProcessorCount, dev));
   return 0;
 }
 
@@ -341,73 +329,6 @@ static PairTable final_block_bwd_pairs(int h_in, int w_in) {
       t.off.push_back((int)t.pairs.size());
     }
   return t;
-}
-
-struct TcFinal {
-  TcWeights f, b;
-  int n_blocks = 0, nbx = 0, w_out = 0, C_out = 0, act = 0;
-};
-
-static int tc_build_final(TcState& st, TcFinal* tf, const float* F, int h_in, int w_in, int C_in, int C_out, int act,
-                          std::vector<void*>* allocs, cudaStream_t s) {
-  if (C_in != 64) { set_error("tensor-core final layer needs net_dim == 64"); return DGAN_ERR_UNSUPPORTED; }
-  if ((h_in % 2) || (w_in % 2) || h_in != w_in) { set_error("final layer geometry unsupported"); return DGAN_ERR_UNSUPPORTED; }
-  tf->C_out = C_out; tf->act = act; tf->nbx = w_in / 2; tf->n_blocks = (h_in / 2) * (w_in / 2); tf->w_out = 2 * w_in;
-  const int nrow = 16 * C_out;
-  DGAN_CUDA_CHECK(cudaMalloc((void**)&tf->f.w, (size_t)16 * nrow * C_in * 2)); allocs->push_back(tf->f.w);
-  DGAN_CUDA_CHECK(cudaMalloc((void**)&tf->b.w, (size_t)16 * C_in * nrow * 2)); allocs->push_back(tf->b.w);
-  tc_final_tiles_kernel<<<16, 256, 0, s>>>(F, C_out, C_in, tf->f.w, tf->b.w);
-  DGAN_CUDA_CHECK(cudaGetLastError());
-  int rc;
-  (void)st;
-  if ((rc = tc_set_direction(&tf->f, nrow, C_in, 16, h_in * w_in, tf->n_blocks))) return rc;
-  // backward: K = the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
-  if ((rc = tc_set_direction(&tf->b, C_in, nrow, 16, tf->n_blocks, h_in * w_in))) return rc;
-  return 0;
-}
-
-static int tc_build(TcState& st, std::vector<TcLayerSpec>& specs, int latent, std::vector<void*>* allocs, cudaStream_t s) {
-  cudaDriverEntryPointQueryResult qres;
-  void* fn = nullptr;
-  DGAN_CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-  if (fn == nullptr || qres != cudaDriverEntryPointSuccess) { set_error("cuTensorMapEncodeTiled not found in the driver"); return DGAN_ERR_CUDA; }
-  st.encode_fn = fn;
-  int dev = 0;
-  DGAN_CUDA_CHECK(cudaGetDevice(&dev));
-  DGAN_CUDA_CHECK(cudaDeviceGetAttribute(&st.num_sms, cudaDevAttrMultiProcessorCount, dev));
-  int rc;
-  for (TcLayerSpec& sp : specs) {
-    const bool linear = sp.linear_W != nullptr;
-    const int n_tiles = linear ? sp.P_out : kTaps;
-    const size_t elems = (size_t)n_tiles * sp.C_out * sp.C_in;
-    // one extra, all-zero tile per direction: tc_with_zero_tile() gives output pixels that receive nothing a single
-    // (pixel 0, zero tile) contribution, so their accumulators hold exact zeros and every item has a step
-    const size_t tile_elems = (size_t)sp.C_out * sp.C_in;
-    __half *wf = nullptr, *wb = nullptr;
-    DGAN_CUDA_CHECK(cudaMalloc((void**)&wf, (elems + tile_elems) * 2)); allocs->push_back(wf);
-    DGAN_CUDA_CHECK(cudaMalloc((void**)&wb, (elems + tile_elems) * 2)); allocs->push_back(wb);
-    DGAN_CUDA_CHECK(cudaMemsetAsync(wf + elems, 0, tile_elems * 2, s));
-    DGAN_CUDA_CHECK(cudaMemsetAsync(wb + elems, 0, tile_elems * 2, s));
-    const unsigned blocks = (unsigned)((elems + 255) / 256);
-    if (linear) {
-      // forward tile q: rows c (N = C_out), cols k (K = latent) = Wt[q*C + c][k]
-      tc_convert_kernel<<<blocks, 256, 0, s>>>(sp.linear_Wt, wf, elems);
-      // backward tile q: rows k (N = latent), cols c (K = C_out) = W[k][q*C + c]
-      tc_linear_bwd_tiles_kernel<<<blocks, 256, 0, s>>>(sp.linear_W, wb, latent, sp.C_out, sp.P_out);
-    } else {
-      tc_convert_kernel<<<blocks, 256, 0, s>>>(sp.w_fwd_kmajor_src, wf, elems);   // F[t][co][ci]
-      tc_convert_kernel<<<blocks, 256, 0, s>>>(sp.w_bwd_kmajor_src, wb, elems);   // Ff[t][ci][co]
-    }
-    DGAN_CUDA_CHECK(cudaGetLastError());
-    sp.out_f->w = wf; sp.out_b->w = wb;
-    sp.out_f->bias_pstride = sp.bias_pstride;
-    // forward: N = C_out, K = C_in;  backward: N = C_in, K = C_out (the Linear's dz is summed over its 16 pixels as
-    // TC_LINEAR_SPLIT partial outputs: more items, and the z update adds the partials in a fixed order)
-    if ((rc = tc_set_direction(sp.out_f, sp.C_out, sp.C_in, n_tiles + 1, sp.P_in, sp.P_out))) return rc;
-    if ((rc = tc_set_direction(sp.out_b, sp.C_in, sp.C_out, n_tiles + 1, sp.P_out, linear ? TC_LINEAR_SPLIT : sp.P_in))) return rc;
-  }
-  (void)latent;
-  return 0;
 }
 
 }  // namespace dgan

@@ -17,7 +17,6 @@
 //     the step's own group has retired; after the item's last step the consumer waits for all MMAs and runs the
 //     epilogue straight from the registers.  Each consumer warp stores the 16 rows it holds with its own TMA store.
 #pragma once
-#include <type_traits>
 #include "kernels_tc.cuh"
 
 namespace dgan {
@@ -700,12 +699,20 @@ struct Tc2Schedule {           // one window tiling of a layer-direction + its i
 };
 // 64-channel or 16-channel TMA box for operands of K channels (tc_make_map)
 static uint32_t tc2_box_k(int K) { return tc2_ksub(K) == 4 ? 64u : 16u; }
-struct TcWeights2 {
-  CUtensorMap tm_b;            // box {64 | 16, N/2, 1}: the half of a weight tile (sub-tile) one CTA of the pair loads
-  PairTable tab;               // host copy: schedules are built lazily per batch size
-  int h_grid = 0, w_grid = 0, max_acc = 1;
+// One layer-direction of the fp16 path: out[P_out][rows][N] = epi(pixel graph `tab` over in[P_in][rows][K] and n_tiles
+// [N][K] weight tiles).  dgan_api.cu's tc_directions() fills the description from the generator's desc alone; a handle
+// adds the weight tiles, their tensor map and the schedules planned for its row counts.
+struct TcDir {
+  std::string name, kind;      // plan-statistics row, profile kind
+  int N = 0, K = 0, P_in = 0, P_out = 0, n_tiles = 0;
+  PairTable tab;               // an output pixel that receives nothing has (pixel 0, zero tile)
+  int h_grid = 0, w_grid = 0;  // the output pixels as the grid the planner's windows tile
+  int max_acc = 1;             // most accumulators per window
+  int epi = EPI_NONE, out_bytes = 2, bias_pstride = 0;
+  __half* w = nullptr;         // [n_tiles][N][K] fp16, K contiguous
+  CUtensorMap tm_b{};          // box {64 | 16, N/2, 1}: the half of a weight tile (sub-tile) one CTA of the pair loads
   int force_maxb = 0;          // > 0: plan with exactly this many accumulator slots per round (dgan_debug_force_slots)
-  mutable std::vector<std::pair<int, Tc2Schedule>> by_mpairs;   // chosen schedule per n_mpairs (lazy cache)
+  std::vector<std::pair<int, Tc2Schedule>> by_mpairs;   // uploaded schedule per n_mpairs (tc2_get_schedule)
 };
 
 static int tc2_maxb(int N) { return TC2_BUF_COLS / tc2_acc_stride(N); }
@@ -857,16 +864,6 @@ static void tc2_enumerate_windows(int h_grid, int w_grid, int wh, int ww, int sy
             }
           if (!qs.empty()) wins->push_back(qs);
         }
-}
-
-static int tc2_build_direction(TcState& st, const TcWeights& w1, TcWeights2* w2, const PairTable& tab, int h_grid,
-                               int w_grid, int force_max_acc, std::vector<void*>* allocs, cudaStream_t s) {
-  (void)allocs; (void)s;
-  const int N = w1.N, K = w1.K;
-  int max_acc = tc2_maxb(N);
-  if (force_max_acc > 0) max_acc = std::min(max_acc, force_max_acc);
-  w2->tab = tab; w2->h_grid = h_grid; w2->w_grid = w_grid; w2->max_acc = max_acc;
-  return tc_make_map(st, &w2->tm_b, w1.w, (uint64_t)K, (uint64_t)N, (uint64_t)w1.n_tiles, (uint32_t)(N / 2), tc2_box_k(K));
 }
 
 #ifndef DGAN_STEP_MAX_KB
@@ -1234,16 +1231,16 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
   return 0;
 }
 
-// Pick (and build on first use) the schedule of one layer-direction for `n_mpairs` row pairs and upload it.
-static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& w2, int n_mpairs, int n_pairs, int epi,
-                            int out_bytes, std::vector<void*>* allocs, cudaStream_t s, const Tc2Schedule** out) {
-  (void)st;
-  for (auto& kv : w2.by_mpairs)
-    if (kv.first == n_mpairs) { *out = &kv.second; return 0; }
+// Plan the schedule of layer-direction d for `n_mpairs` row pairs on `n_pairs` CTA pairs and upload it (allocates and
+// synchronises), unless d already has one for that many row pairs.
+static int tc2_get_schedule(TcDir& d, int n_mpairs, int n_pairs, std::vector<void*>* allocs) {
+  for (auto& kv : d.by_mpairs)
+    if (kv.first == n_mpairs) return 0;
   Tc2Plan plan;
   int rc;
-  if ((rc = tc2_plan(w1.N, w1.K, w2.tab, w2.h_grid, w2.w_grid, w2.max_acc, w2.force_maxb, epi, out_bytes, n_mpairs, n_pairs, &plan)))
+  if ((rc = tc2_plan(d.N, d.K, d.tab, d.h_grid, d.w_grid, d.max_acc, d.force_maxb, d.epi, d.out_bytes, n_mpairs, n_pairs, &plan)))
     return rc;
+  const cudaStream_t s = 0;
   Tc2Schedule sc;
   sc.maxb = plan.maxb;
   sc.wh = plan.shape[0]; sc.ww = plan.shape[1]; sc.sy = plan.shape[2]; sc.sx = plan.shape[3];
@@ -1254,8 +1251,7 @@ static int tc2_get_schedule(TcState& st, const TcWeights& w1, const TcWeights2& 
   if (n_pairs > TC2_MAX_PAIRS) { set_error("more CTA pairs than the kernel's parameter block holds"); return DGAN_ERR_UNSUPPORTED; }
   for (int pr = 0; pr <= n_pairs; ++pr) sc.heads.off[pr] = plan.stream_off[(size_t)pr];
   if ((rc = tc_upload(allocs, plan.eitems.data(), plan.eitems.size() * sizeof(int), (void**)&sc.eitems, s))) return rc;
-  w2.by_mpairs.push_back({n_mpairs, sc});
-  *out = &w2.by_mpairs.back().second;
+  d.by_mpairs.push_back({n_mpairs, sc});
   return 0;
 }
 
@@ -1272,40 +1268,27 @@ static int tc2_optin_all() {
   return 0;
 }
 
-template <typename TOUT>
-static int tc2_launch_impl(TcState& st, int64_t* launches, const TcWeights& w, const TcWeights2& w2m, const __half* in,
-                           TOUT* out, int n_pad, int epi, const float* bias, cudaStream_t s, const TcFinalArgs* final_args = nullptr, const CUtensorMap* pre_a = nullptr,
-                           const CUtensorMap* pre_out = nullptr) {
-  TcFinalArgs fa{};
-  if (final_args) fa = *final_args;
-  CUtensorMap tm_a;
-  int rc;
-  if (pre_a != nullptr) tm_a = *pre_a;          // encoded once per workspace by the caller
-  else if ((rc = tc_make_map(st, &tm_a, in, (uint64_t)w.K, (uint64_t)n_pad, (uint64_t)w.P_in, 128, tc2_box_k(w.K)))) return rc;
-  CUtensorMap tm_out = tm_a;                     // placeholder when unused
-  if (tc2_tma_epilogue(w.N, epi, (int)sizeof(TOUT))) {
-    if (pre_out != nullptr) tm_out = *pre_out;
-    else if ((rc = tc_make_map(st, &tm_out, out, (uint64_t)w.N, (uint64_t)n_pad, (uint64_t)w.P_out, TC2_STORE_ROWS))) return rc;
-  }
+// Launch layer-direction d on n_pad rows with the schedule tc2_get_schedule made for them.  tm_a, tm_out: the tensor
+// maps of its input and output; out: its output, of d.out_bytes per element.
+static int tc2_launch(int64_t* launches, const TcDir& d, const CUtensorMap& tm_a, const CUtensorMap& tm_out, void* out,
+                      int n_pad, const float* bias, cudaStream_t s, const TcFinalArgs& fa) {
   if (n_pad % (2 * kRowTile) != 0) { set_error("pair kernel needs n_pad % 256 == 0"); return DGAN_ERR_INVALID_ARG; }
-  if (w.bias_pstride != 0 && w.N != 256) { set_error("a per-pixel bias needs one accumulator per item (N = 256)"); return DGAN_ERR_UNSUPPORTED; }
+  if (d.bias_pstride != 0 && d.N != 256) { set_error("a per-pixel bias needs one accumulator per item (N = 256)"); return DGAN_ERR_UNSUPPORTED; }
   const int n_mpairs = n_pad / (2 * kRowTile);
-  const Tc2Schedule* schp = nullptr;
-  const int pairs_avail = st.num_sms / 2;
-  if ((rc = tc2_get_schedule(st, w, w2m, n_mpairs, pairs_avail, epi, (int)sizeof(TOUT), st.allocs, s, &schp))) return rc;
-  const Tc2Schedule& w2s = *schp;
-  const int grid = 2 * w2s.n_pairs;       // pairs without work find -1 in slot 0 and fall through
+  const Tc2Schedule* sc = nullptr;
+  for (auto& kv : d.by_mpairs)
+    if (kv.first == n_mpairs) sc = &kv.second;
+  if (sc == nullptr) { set_error(d.name + ": no schedule planned for " + std::to_string(n_pad) + " rows"); return DGAN_ERR_INVALID_ARG; }
+  const int grid = 2 * sc->n_pairs;       // pairs without work find -1 in slot 0 and fall through
   cudaError_t le = cudaSuccess;
   bool found = false;
-  const int ksub = tc2_ksub(w.K);
+  const int ksub = tc2_ksub(d.K);
 #define TC2_GO(NT, MB, KS, EP, T)                                                                                      \
-  if constexpr (std::is_same<T, TOUT>::value) {                                                                      \
-    if (!found && w.N == NT && w2s.maxb == MB && ksub == KS && epi == EP) {                                           \
-      found = true;                                                                                                   \
-      le = launch_pdl(tc_bsgemm2_kernel<NT, MB, KS, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, KS, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
-                      tm_a, w2m.tm_b, tm_out, w2s.items, w2s.stream_p, w2s.stream_m, w2s.heads, w2s.eitems, w2s.n_slots, out, n_pad, \
-                      bias, (EP == EPI_FINAL_SIGMOID1 || EP == EPI_FINAL_TANH3) ? 0 : w.bias_pstride, fa);              \
-    }                                                                                                                 \
+  if (!found && d.N == NT && sc->maxb == MB && ksub == KS && d.epi == EP && d.out_bytes == (int)sizeof(T)) {           \
+    found = true;                                                                                                     \
+    le = launch_pdl(tc_bsgemm2_kernel<NT, MB, KS, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, KS, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
+                    tm_a, d.tm_b, tm_out, sc->items, sc->stream_p, sc->stream_m, sc->heads, sc->eitems, sc->n_slots,     \
+                    static_cast<T*>(out), n_pad, bias, d.bias_pstride, fa);                                            \
   }
   TC2_KINDS(TC2_GO)
 #undef TC2_GO

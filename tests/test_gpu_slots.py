@@ -31,12 +31,15 @@ def _force(gen, d, maxb):
     assert rc == 0, lib.dgan_last_error()
 
 
-@pytest.mark.parametrize("arch,B,R", [("mnist", 6, 5), ("celeba", 3, 4)])
-def test_every_slot_count_reconstructs_bit_identically(arch, B, R):
+@pytest.mark.parametrize("arch,use_bn,B,R", [pytest.param("mnist", False, 6, 5, id="mnist-6-5"),
+                                             pytest.param("celeba", False, 3, 4, id="celeba-3-4"),
+                                             pytest.param("mnist", True, 6, 5, id="mnist-bn-6-5")])
+def test_every_slot_count_reconstructs_bit_identically(arch, use_bn, B, R):
     from defensegan_b200 import _native
     dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, random_bias=True)
-    gen = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], precision="fp16", device=dev)
+    w = O.init_generator_weights(arch, random_bias=True, use_bn=use_bn)
+    gen = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], use_bn=use_bn, precision="fp16",
+                                  device=dev)
     try:
         imgs = torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=11)).to(dev)
         z0 = torch.tensor(O.sample_z0(B * R, 128, seed=12)).to(dev)

@@ -601,6 +601,42 @@ def test_plan_statistics_entry_point():
         assert float(by[name][9]) < 1.12, (name, by[name])
 
 
+# The epilogue and output type each layer-direction of the fp16 path launches with.  With BatchNorm after a layer
+# (use_bn: the Linear, Generator.2 and Generator.3) its forward stores fp32 pre-activations without the ReLU, and the
+# backward into its output applies no ReLU mask: the BN backward does both.
+_EPILOGUES = {           # direction: MNIST, MNIST + BN, CelebA, CelebA + BN (None: no such direction)
+    "Linear.fwd": ("bias_relu/f16", "bias/f32", "bias_relu/f16", "bias/f32"),
+    "Linear.bwd": ("none/f32", "none/f32", "none/f32", "none/f32"),
+    "Generator.2.fwd": ("bias_relu/f16", "bias/f32", "bias_relu/f16", "bias/f32"),
+    "Generator.2.bwd": ("mask/f16", "none/f16", "mask/f16", "none/f16"),
+    "Generator.3.fwd": ("bias_relu/f16", "bias/f32", "bias_relu/f16", "bias/f32"),
+    "Generator.3.bwd": ("mask/f16", "none/f16", "mask/f16", "none/f16"),
+    "Generator.5.fwd": (None, None, "bias/f16", "bias/f16"),
+    "Generator.5.bwd": (None, None, "mask/f16", "none/f16"),
+    "last.fwd": ("final_sigmoid/f16", "final_sigmoid/f16", "final_tanh/f16", "final_tanh/f16"),
+    "last.bwd": ("mask/f16", "none/f16", "none/f16", "none/f16"),
+}
+
+
+@pytest.mark.parametrize("arch,use_bn", [("mnist", 0), ("mnist", 1), ("celeba", 0), ("celeba", 1)])
+def test_plans_are_made_for_the_epilogue_each_direction_launches_with(arch, use_bn):
+    """The epilogue and output type set a plan's instantiation and ring size, so the plans the validator checks and the
+    statistics describe must be made for the ones the launch uses.  The statistics name them in their last column."""
+    import ctypes
+    from defensegan_b200 import _native
+    lib = _native.load_library()
+    lib.dgan_debug_plan_stats.restype = ctypes.c_int
+    lib.dgan_debug_plan_stats.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
+    desc = _native.dgan_desc(_native.ABI_VERSION, _native.ARCH_IDS[arch], 128, 64, use_bn, _native.PRECISIONS["fp16"])
+    buf = ctypes.create_string_buffer(1 << 16)
+    assert lib.dgan_debug_plan_stats(ctypes.byref(desc), 256, 66, buf, len(buf)) > 0
+    lines = [l.split(" | ") for l in buf.value.decode().strip().splitlines()]
+    assert len(lines[0]) == 16 and lines[0][15] == "epilogue/output", lines[0]
+    col = 2 * (arch == "celeba") + use_bn
+    want = {name: v[col] for name, v in _EPILOGUES.items() if v[col] is not None}
+    assert [(r[0], r[15]) for r in lines[1:-1]] == list(want.items())     # in launch order
+
+
 def test_schedule_validator_rejects_damaged_plans():
     """The validator is not vacuous: nine single faults injected into a valid plan (wrong first-MMA flag, accumulator,
     staged weight tile, input pixel, k-chunk, lost epilogue item, unsafe ring dependencies, region outside the ring,
