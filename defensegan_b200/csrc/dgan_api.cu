@@ -1116,46 +1116,42 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
     // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd, faults 12-13
-    // (specific to narrow ops) that of the last layer's backward; the check must then fail
-    if (mutate >= 12 && dr.name == "last.bwd" && plan.stream_m.size() > 40) {
+    // (specific to narrow ops) that of the last layer's backward; the check must then fail.  Each fault but 6 and 9
+    // decodes records, changes one field and encodes them again.
+    const bool narrow = mutate >= 12 && dr.name == "last.bwd", wide = mutate != 0 && mutate < 12 && dr.name == "Generator.3.fwd";
+    if ((narrow || wide) && plan.stream_m.size() > 40) {
+      auto mma = [&](size_t i, auto f) { TcMmaRec m = TcMmaRec::decode(plan.stream_m[i]); f(m); plan.stream_m[i] = m.encode(); };
+      auto producer = [&](size_t i, auto f) { TcProducerRec p = TcProducerRec::decode(plan.stream_p[i]); f(p); plan.stream_p[i] = p.encode(); };
+      auto every_mma = [&](auto f) { for (size_t i = 0; i < plan.stream_m.size(); ++i) mma(i, f); };
       switch (mutate) {
-        case 12: for (TcRec& r : plan.stream_m) r.w[1] = (r.w[1] & 0xFFu) | ((uint32_t)(plan.ksub == 1 ? 2 : 1) << 8); break;   // k16 per op
-        case 13: plan.stream_p[20].w[0] |= 1u << 8; break;                 // a k-chunk >= 1 (a narrow K has one)
-        default: break;
-      }
-    }
-    if (mutate != 0 && mutate < 12 && dr.name == "Generator.3.fwd" && plan.stream_m.size() > 40) {
-      TcRec& m = plan.stream_m[20];
-      TcRec* pp = &plan.stream_p[20];
-      switch (mutate) {
-        case 1: m.w[2] ^= 1u << 6; break;                                   // first-MMA flag of an op
-        case 2: {                                                           // accumulator of an op: swap two ops of round 0
-                  const int nb = (int)m.w[1];
-                  for (int j = 1; j < nb; ++j) {
-                    const uint32_t b0 = m.w[2] & 0xFFu, bj = (m.w[2 + j / 4] >> (8 * (j & 3))) & 0xFFu;
-                    if (bj == b0) continue;
-                    m.w[2] = (m.w[2] & ~0xFFu) | bj;
-                    m.w[2 + j / 4] = (m.w[2 + j / 4] & ~(0xFFu << (8 * (j & 3)))) | (b0 << (8 * (j & 3)));
-                    break;
-                  }
-                  break;
-                }
-        case 3: pp->w[4] ^= 0x01; break;                                    // weight tile of a B slot
-        case 4: pp->w[2] ^= 0x01; break;                                    // input pixel of an A tile
-        case 5: pp->w[0] = (pp->w[0] & ~(0xFu << 8)) | ((((pp->w[0] >> 8) & 0xF) ^ 1u) << 8); break;   // k-chunk
-        case 6: plan.eitems[0] = -1; break;                                 // epilogue list loses an item
-        case 7: for (size_t i = 0; i < plan.stream_m.size(); ++i)           // every dep -> 8: ring hazards
-                  plan.stream_p[i].w[0] = (plan.stream_p[i].w[0] & ~(0xFu << 19)) | (8u << 19);
+        case 1: mma(20, [](TcMmaRec& m) {                                    // first-MMA flag of an op
+                  TcOp op = TcOp::decode(m.ops[0]);
+                  op.first ^= 1u;
+                  m.ops[0] = op.encode();
+                });
                 break;
-        case 8: pp->w[0] = (pp->w[0] & ~0xFFu) | 0xBFu; break;              // region past the ring
-        case 9: std::swap(plan.stream_m[20], plan.stream_m[21]);            // two steps out of order
+        case 2: mma(20, [](TcMmaRec& m) {                                    // accumulator of an op: swap two ops of round 0
+                  for (uint32_t j = 1; j < m.maxb; ++j)
+                    if (m.ops[j] != m.ops[0]) { std::swap(m.ops[0], m.ops[j]); break; }
+                });
+                break;
+        case 3: producer(20, [](TcProducerRec& p) { p.tile[0] ^= 1u; }); break;   // weight tile of a B slot
+        case 4: producer(20, [](TcProducerRec& p) { p.pix[0] ^= 1u; }); break;    // input pixel of an A tile
+        case 5: producer(20, [](TcProducerRec& p) { p.kc ^= 1u; }); break;        // k-chunk
+        case 6: plan.eitems[0] = -1; break;                                       // epilogue list loses an item
+        case 7: for (size_t i = 0; i < plan.stream_p.size(); ++i)                 // every dep -> 8: ring hazards
+                  producer(i, [](TcProducerRec& p) { p.dep = TC2_NSLOT; });
+                break;
+        case 8: producer(20, [](TcProducerRec& p) { p.off = 0xBF; }); break;      // region past the ring
+        case 9: std::swap(plan.stream_m[20], plan.stream_m[21]);                  // two steps out of order
                 std::swap(plan.stream_p[20], plan.stream_p[21]);
                 break;
-        case 10: plan.maxb = 3;                                              // slots per round without an instantiation
-                 for (TcRec& r : plan.stream_m) r.w[1] = 3;
+        case 10: plan.maxb = 3;                                                   // slots per round without an instantiation
+                 every_mma([](TcMmaRec& m) { m.maxb = 3; });
                  break;
-        case 11: for (TcRec& r : plan.stream_m) r.w[1] = 2;                 // records disagree with the plan's slots
-                 break;
+        case 11: every_mma([](TcMmaRec& m) { m.maxb = 2; }); break;               // records disagree with the plan's slots
+        case 12: every_mma([&](TcMmaRec& m) { m.ksub = plan.ksub == 1 ? 2 : 1; }); break;   // k16 per op
+        case 13: producer(20, [](TcProducerRec& p) { p.kc |= 1u; }); break;      // a k-chunk >= 1 (a narrow K has one)
         default: break;
       }
     }

@@ -18,6 +18,7 @@
 //     epilogue straight from the registers.  Each consumer warp stores the 16 rows it holds with its own TMA store.
 #pragma once
 #include "kernels_tc.cuh"
+#include "tc_records.cuh"
 
 namespace dgan {
 
@@ -38,10 +39,12 @@ struct Tc2Heads {
   uint32_t off[TC2_MAX_PAIRS + 1];    // record offsets of the pairs' step streams
 };
 
+// A window's output pixels, one per accumulator (the consumers' epilogue reads it).
 struct __align__(16) TcItem2 {
   uint16_t q[16];
-  uint32_t n_acc, step_beg, n_steps, pad;
+  uint32_t n_acc;
 };
+static_assert(sizeof(TcItem2) == 48 && offsetof(TcItem2, n_acc) == 32, "the kernel's item loads");
 
 // Accumulator columns reserved per accumulator of a window.  N <= 32 (MNIST last layer: 16 outputs per block) packs
 // 8 accumulators into the 256 columns of an item, so a window can span a whole row of blocks.
@@ -52,32 +55,8 @@ __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out
   return out_bytes == 2 && n_tile >= 64 && epi != EPI_FINAL_SIGMOID1 && epi != EPI_FINAL_TANH3;
 }
 
-// One step of a CTA pair's work stream (32 bytes).  The host concatenates, per CTA pair, the steps of all the items
-// assigned to it (LPT order), so producer and consumers read one contiguous array.
-//
-// A step stages up to 4 input-pixel (A) tiles and up to 8 full weight tiles (B slots) for one k-chunk into a
-// variable-size region of a circular shared-memory ring (offset chosen by the host, which simulates the ring),
-// then issues rounds of MMAs that combine them.  Several A tiles per step let one weight tile serve several input
-// pixels (stride-2 transposed conv: outputs of equal parity use the same tap with neighbouring inputs), which
-// is what the L2->SM byte count cares about.
-//
-// producer record (the same for both ranks of a pair):
-//   w[0]: ring offset / 1 KB [0,8) | k-chunk [8,12) | A tiles [12,15) | B slots [15,19) | dep [19,23)
-//         dep = D: the region overlaps that of step k-D (or D = 8, barrier-slot reuse): wait until step k-D is consumed
-//   w[1]: row pair mp [0,16)
-//   w[2..3]: 4 x u16 input pixel of A tile i
-//   w[4..5]: 8 x u8 weight tile [0,5) per B slot
-// MMA record:
-//   w[0]: ring offset / 1 KB [0,8) | A tiles [8,11) | rounds [11,16) | flags [16,18): 1 = first step of an item, 2 = last
-//   w[1]: accumulators per round [0,8) (MAXB of the instantiation) | k16 MMAs per op [8,11) (KSUB); checked by the
-//         validator only
-//   w[2..7]: 24 x u8, round-major, one per (round, accumulator): A tile [0,2) | B slot [2,6) | first MMA into the
-//            accumulator [6,7).  B slot 15 = the all-zero tile outside the ring (the accumulator has nothing to add in
-//            this round; never a first MMA).
-struct __align__(16) TcRec { uint32_t w[8]; };
-constexpr int TC2_MAX_A = 4, TC2_MAX_BSLOTS = 8, TC2_OP_BYTES = 24, TC2_ZERO_SLOT = 15, TC2_NSLOT = 8;
 constexpr int TC2_REC_BATCH = 16;
-constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // producer record ring
+constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // producer record ring (records: tc_records.cuh)
 
 // Output staging of the TMA-store epilogues: two 16-row x 128 B buffers per consumer warp (the next unit is written
 // while the store of the previous one still reads shared memory).
@@ -97,7 +76,7 @@ __host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb, int ksub)
 __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int ksub, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
   const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb, ksub)) / 1024) * 1024;
-  return raw > 255 * 1024 ? 255 * 1024 : raw;
+  return raw > TC2_RING_MAX_KB * 1024 ? TC2_RING_MAX_KB * 1024 : raw;
 }
 
 // MAXB_: accumulator slots of the instantiation = MMAs per round = the most accumulators a window may have.  Fewer slots
@@ -144,6 +123,13 @@ struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
 #define TC2_KIND_ROW(NT, MB, KS, EP, T) {NT, MB, KS, EP, (int)sizeof(T)},
 static constexpr Tc2Kind kTc2Kinds[] = {TC2_KINDS(TC2_KIND_ROW)};
 #undef TC2_KIND_ROW
+// The MMA records carry every instantiation's slots per round and k16 MMAs per op.
+constexpr bool tc2_kinds_fit_records() {
+  for (const Tc2Kind& k : kTc2Kinds)
+    if ((uint32_t)k.maxb > TcMmaRec::MaxB::mask || (uint32_t)k.ksub > TcMmaRec::Ksub::mask) return false;
+  return true;
+}
+static_assert(tc2_kinds_fit_records(), "an instantiation's MAXB or KSUB does not fit the MMA record");
 // Is there an instantiation with these template arguments?
 static inline bool tc2_has_kind(int n, int maxb, int ksub, int epi, int out_bytes) {
   for (const Tc2Kind& k : kTc2Kinds)
@@ -214,8 +200,8 @@ __device__ __forceinline__ bool elect_one() {
 }
 }  // namespace ptx
 
-// k-th item (window << 16 | row pair) of CTA pair `pair` from the host-computed table [slot][pair] (-1 = no more work).
-// The host assigns items largest-first to the least-loaded pair (LPT) with the cost model of tc2_get_schedule.
+// k-th item word (tc2_item_word) of CTA pair `pair` from the host-computed table [slot][pair] (-1 = no more work).
+// The host assigns items largest-first to the least-loaded pair (LPT) with the cost model of tc2_plan.
 __device__ __forceinline__ int tc2_item_at(const int* __restrict__ order, int k, int pair, int n_pairs, int n_slots) {
   return k < n_slots ? __ldg(order + (size_t)k * n_pairs + pair) : -1;
 }
@@ -231,27 +217,29 @@ __device__ __forceinline__ void tc2_mma_round(float (&acc)[NREG], const uint32_t
   constexpr uint32_t DA_K = KSUB == 4 ? 2u : (uint32_t)(128 * 32 >> 4), DB_K = KSUB == 4 ? 2u : (uint32_t)(NT * 32 >> 4);
 #pragma unroll
   for (int a = 0; a < MAXB; ++a) {
-    const uint32_t e = (q[a >> 2] >> (8 * (a & 3))) & 0xFFu;
-    const uint32_t bs = (e >> 2) & 0xFu;
+    const uint32_t e = TcMmaRec::Ops::get(q[a / TcMmaRec::Ops::PER_WORD], a);
+    const uint32_t bs = TcOp::Slot::get(e);
     // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
-    const uint64_t da = da0 + (uint64_t)((e & 3u) * (uint32_t)(tc2_a_bytes(KSUB) >> 4));
+    const uint64_t da = da0 + (uint64_t)(TcOp::A::get(e) * (uint32_t)(tc2_a_bytes(KSUB) >> 4));
     const uint64_t db = db0 + (uint64_t)(bs == (uint32_t)TC2_ZERO_SLOT ? zoff : bs * (uint32_t)(tc2_b_bytes(NT, KSUB) >> 4));
-    const uint32_t keep = ((e >> 6) & 1u) ^ 1u;      // 0: first MMA into the accumulator, overwrite it
+    const uint32_t keep = TcOp::First::get(e) ^ 1u;  // 0: first MMA into the accumulator, overwrite it
 #pragma unroll
     for (int k = 0; k < KSUB; ++k) ptx::Wgmma<NT>::mma(acc + a * (NT / 2), da + DA_K * k, db + DB_K * k, k > 0 ? 1u : keep);
   }
 }
 
-// Drop the record bytes of one round (MAXB of them) from the front of the op queue.
+// Drop the op bytes of one round (MAXB of them) from the front of the op queue (the MMA record's words 2..7).
 template <int MAXB>
 __device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
-  if constexpr (MAXB >= 4) {
+  using Ops = TcMmaRec::Ops;
+  static_assert(Ops::WORDS == 6, "the op queue holds every op word");
+  if constexpr (MAXB >= Ops::PER_WORD) {
 #pragma unroll
-    for (int i = 0; i < 6; ++i) q[i] = (i + MAXB / 4 < 6) ? q[i + MAXB / 4] : 0u;
+    for (int i = 0; i < 6; ++i) q[i] = (i + MAXB / Ops::PER_WORD < 6) ? q[i + MAXB / Ops::PER_WORD] : 0u;
   } else {
 #pragma unroll
-    for (int i = 0; i < 5; ++i) q[i] = __funnelshift_r(q[i], q[i + 1], 8 * MAXB);
-    q[5] >>= 8 * MAXB;
+    for (int i = 0; i < 5; ++i) q[i] = __funnelshift_r(q[i], q[i + 1], Ops::BITS * MAXB);
+    q[5] >>= Ops::BITS * MAXB;
   }
 }
 
@@ -357,21 +345,23 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           const uint4 r0 = ptx::ld_shared_v4(ring + i * 32u);
           const uint2 r1 = ptx::ld_shared_v2(ring + i * 32u + 16u);
           const uint32_t slot = it & (TC2_NSLOT - 1);
-          const int kc = (r0.x >> 8) & 0xF, nA = (r0.x >> 12) & 0x7, nB = (r0.x >> 15) & 0xF;
-          const uint32_t dep = (r0.x >> 19) & 0xF;
-          const int row0 = (2 * (int)(r0.y & 0xFFFFu) + (int)rank) * kRowTile;
+          using P = TcProducerRec;
+          const int kc = P::Kc::get(r0.x), nA = P::NA::get(r0.x), nB = P::NB::get(r0.x);
+          // not P::Dep::get(r0.x): the same value, but ptxas then orders this warp's record loads differently
+          const uint32_t dep = (r0.x >> P::Dep::shift) & P::Dep::mask;
+          const int row0 = (2 * (int)P::Mp::get(r0.y) + (int)rank) * kRowTile;
           if (it >= dep) ptx::mbar_wait(bar_empty + 8 * ((it - dep) & (TC2_NSLOT - 1)), ((it - dep) >> 3) & 1);   // step it-dep consumed
           // implied by the wait above (steps are consumed in order); observing every phase of this slot exactly once
           // before it is re-armed keeps the barrier protocol simple to check
           if (dep != TC2_NSLOT && it >= TC2_NSLOT) ptx::mbar_wait(bar_empty + 8 * slot, ((it - TC2_NSLOT) >> 3) & 1);
           const uint32_t full = bar_full + 8 * slot;
-          const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
+          const uint32_t sa = smem_base + (P::Off::get(r0.x) << 10);
           if (ptx::elect_one()) {
             ptx::mbar_expect_tx(full, (uint32_t)(nA * A_BYTES + nB * B_TILE));
 #pragma unroll
             for (int a = 0; a < TC2_MAX_A; ++a) {
               if (a >= nA) break;
-              const int p = (int)((((a < 2) ? r0.z : r0.w) >> (16 * (a & 1))) & 0xFFFFu);
+              const int p = (int)P::Pix::get(a < P::Pix::PER_WORD ? r0.z : r0.w, a);
               if constexpr (KSUB == 4) {
                 ptx::tma_load_3d(sa + a * A_BYTES, &tm_a, full, kc * 64, row0, p);
               } else {
@@ -384,14 +374,14 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #pragma unroll
             for (int b = 0; b < TC2_MAX_BSLOTS; ++b) {     // this CTA's half of each weight tile, into both CTAs
               if (b >= nB) break;
-              const uint32_t e = ((b < 4) ? r1.x : r1.y) >> (8 * (b & 3));
+              const uint32_t t = P::Tile::get(b < P::Tile::PER_WORD ? r1.x : r1.y, b);
               if constexpr (KSUB == 4) {
-                ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+                ptx::tma_load_3d_mc2(sb + b * B_TILE + rank * (B_TILE / 2), &tm_b, full, kc * 64, (int)rank * (N_TILE / 2), (int)t);
               } else {
 #pragma unroll
                 for (int k = 0; k < KSUB; ++k)           // this CTA's half of every sub-tile
                   ptx::tma_load_3d_mc2(sb + b * B_TILE + k * Cfg::B_SUB + rank * (Cfg::B_SUB / 2), &tm_b, full, (kc * KSUB + k) * 16,
-                                       (int)rank * (N_TILE / 2), (int)(e & 0x1Fu));
+                                       (int)rank * (N_TILE / 2), (int)t);
               }
             }
           }
@@ -420,13 +410,13 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       uint32_t flags;
       do {    // the steps of one item
         const uint4 r0 = n0, r1 = n1;
-        flags = (r0.x >> 16) & 0x3u;
-        if (!(flags & 2u)) {            // not the item's last step: another step of the item follows
+        flags = TcMmaRec::Flags::get(r0.x);
+        if (!(flags & TcMmaRec::LAST)) {     // not the item's last step: another step of the item follows
           const uint4* rp = reinterpret_cast<const uint4*>(stream_m + ri + 1);
           n0 = __ldg(rp); n1 = __ldg(rp + 1);
         }
         const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
-        const int nA = (r0.x >> 8) & 0x7, n_rounds = (r0.x >> 11) & 0x1F;
+        const int nA = TcMmaRec::NA::get(r0.x), n_rounds = TcMmaRec::Rounds::get(r0.x);
 #ifdef DGAN_PROBE
         const long long probe_w0 = clock64();
 #endif
@@ -435,7 +425,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         probe_wait_full += clock64() - probe_w0;
         if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
 #endif
-        const uint32_t sa = smem_base + ((r0.x & 0xFFu) << 10);
+        const uint32_t sa = smem_base + (TcMmaRec::Off::get(r0.x) << 10);
         // this warpgroup's 64 rows of the A tiles (of their first sub-tile when narrow)
         const uint64_t da0 = KSUB == 4 ? make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u) : make_smem_desc_sw32(sa + (uint32_t)wg * 64u * 32u);
         const uint32_t sb = sa + (uint32_t)nA * A_BYTES;
@@ -454,9 +444,9 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         ptx::fence_operands(acc);
         __syncwarp();
         // this warp's MMAs no longer read the previous step's region (the previous item's last step was released below)
-        if (!(flags & 1u) && lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
+        if (!(flags & TcMmaRec::FIRST) && lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
         ++ri; ++it;
-      } while (!(flags & 2u));
+      } while (!(flags & TcMmaRec::LAST));
       // the epilogue reads the registers: wait for all MMAs, then release the item's last step
       ptx::wgmma_wait0();
       ptx::fence_operands(acc);
@@ -466,8 +456,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       // ---- epilogue of the item: accumulator registers -> (bias | ReLU | mask | last layer) -> global memory.
       //      Register i of accumulator a holds column (i % (N_TILE/2)) / 4 * 8 + (lane % 4) * 2 + (i % 2) of row
       //      r_lo + 8 * ((i / 2) % 2) (the m64nNk16 accumulator fragment).
-      const TcItem2* ip = items + (item_e >> 16);
-      const int mp = item_e & 0xFFFF;
+      const TcItem2* ip = items + tc2_item_window(item_e);
+      const int mp = tc2_item_mp(item_e);
       const int n_acc = (int)__ldg(&ip->n_acc);
       const uint32_t q_mine = lane < 16 ? (uint32_t)__ldg(&ip->q[lane]) : 0u;
       auto q_of = [&](int a) { return (int)__shfl_sync(0xffffffffu, q_mine, a); };
@@ -691,10 +681,8 @@ struct Tc2Schedule {           // one window tiling of a layer-direction + its i
   TcRec* stream_p = nullptr;       // producer records (both ranks of a pair); per CTA pair: its items' steps, concatenated
   TcRec* stream_m = nullptr;       // MMA records, same indexing
   Tc2Heads heads{};                // per pair: record offsets into the streams (kernel parameter)
-  int* eitems = nullptr;           // [n_slots][n_pairs] (window << 16 | row pair) for the consumer epilogues, or -1
+  int* eitems = nullptr;           // [n_slots][n_pairs] item words (tc2_item_word) for the consumer epilogues, or -1
   int n_slots = 0, n_pairs = 0;
-  int n_windows = 0;
-  int wh = 0, ww = 0, sy = 1, sx = 1;
   int maxb = 1;                    // accumulator slots per round: selects the kernel instantiation
 };
 // 64-channel or 16-channel TMA box for operands of K channels (tc_make_map)
@@ -722,11 +710,10 @@ struct Tc2HostStep {
   int kc = 0, nA = 0, nB = 0, n_rounds = 0;
   int a_pix[TC2_MAX_A] = {0, 0, 0, 0};
   uint8_t b_ent[TC2_MAX_BSLOTS] = {0};   // weight tile per B slot
-  uint8_t ops[TC2_OP_BYTES] = {0};       // [round][accumulator] record bytes
+  uint8_t ops[TC2_OP_BYTES] = {0};       // [round][accumulator] op bytes (TcOp)
   int n_real = 0;              // ops that do not read the zero tile (statistics)
   int bytes = 0;               // operand bytes staged per CTA
 };
-constexpr uint8_t TC2_PAD_OP = (uint8_t)(TC2_ZERO_SLOT << 2);   // A tile 0 x zero tile, accumulate
 struct Tc2HostItem {
   TcItem2 hdr{};
   std::vector<Tc2HostStep> steps;
@@ -819,11 +806,11 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
         const int t = ta.first, acc = ta.second;
         if (slot_of[t] < 0) {
           slot_of[t] = st.nB;
-          st.b_ent[st.nB++] = (uint8_t)(t & 0x1F);
+          st.b_ent[st.nB++] = (uint8_t)t;
         }
         const bool first = !(seen & (1u << acc));
         const int r = cnt[acc]++;
-        st.ops[r * max_b + acc] = (uint8_t)((i - G.i0) | (slot_of[t] << 2) | ((first ? 1 : 0) << 6));
+        st.ops[r * max_b + acc] = TcOp{(uint32_t)(i - G.i0), (uint32_t)slot_of[t], first ? 1u : 0u}.encode();
         st.n_rounds = std::max(st.n_rounds, r + 1);
         st.n_real += 1;
         seen |= 1u << acc;
@@ -840,7 +827,7 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     for (size_t gi = 0; gi < n_groups; ++gi) {
       Tc2HostStep sk = out->steps[gi];
       sk.kc = kc;
-      for (int o = 0; o < TC2_OP_BYTES; ++o) sk.ops[o] &= (uint8_t)~(1u << 6);
+      for (int o = 0; o < TC2_OP_BYTES; ++o) sk.ops[o] = (uint8_t)TcOp::First::put(sk.ops[o], 0u);
       out->steps.push_back(sk);
     }
   out->stage_bytes = 0.0;
@@ -895,15 +882,12 @@ static void tc2_enumerate_windows(int h_grid, int w_grid, int wh, int ww, int sy
 #define DGAN_COST_OP_MIN_N 32
 #endif
 #ifndef TC2_REFINE_BUDGET
-#define TC2_REFINE_BUDGET (1LL << 26)    // candidate evaluations of the assignment refinement per window shape (tc2_plan)
+#define TC2_REFINE_BUDGET (1LL << 26)    // candidate evaluations of the assignment refinement per window shape (tc2_search)
 #endif
 
-// Pick (and build on first use) the accumulator slots per round and the window tiling for `n_mpairs` row pairs on
-// `n_pairs` CTA pairs: every candidate - an instantiation of TC2_KINDS for (N, epilogue, output type) and a shape of
-// wh x ww <= its slots accumulators, strides 1 or 2 - is scored by an LPT assignment of its items (window, row pair)
-// to the CTA pairs with the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed
-// per-item charge, and the MMAs issued, zero-tile ones included); the smallest makespan wins.  Then each pair's items are concatenated into its step streams, the circular operand
-// ring is simulated to give every step its offset and its dependency distance, and everything is uploaded.
+// The planner.  tc2_search picks the accumulator slots per round and the window tiling for `n_mpairs` row pairs on
+// `n_pairs` CTA pairs and assigns the items to the pairs; tc2_encode_streams lays each pair's steps out in its operand
+// ring and writes the records; tc2_get_schedule uploads the result.
 struct Tc2Plan {               // host result of the planner (what tc2_get_schedule uploads)
   int shape[4] = {1, 1, 1, 1};   // wh, ww, sy, sx
   int n_slots = 0, n_pairs = 0;
@@ -922,9 +906,15 @@ static double tc2_op_ns(int N, int ksub) {
   return DGAN_COST_OP_NS * (double)std::max(N, DGAN_COST_OP_MIN_N) / 64.0 * (double)ksub / 4.0;
 }
 
+// Every candidate - an instantiation of TC2_KINDS for (N, epilogue, output type) and a shape of wh x ww <= its slots
+// accumulators, strides 1 or 2 - is scored by an LPT assignment of its items (window, row pair) to the CTA pairs with
+// the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed per-item charge, and the MMAs
+// issued, zero-tile ones included); the smallest makespan wins.  Fills the plan's shape, slots, ring and loads, and
+// returns the winner's items and, per CTA pair, its item indices (window * n_mpairs + row pair) in issue order.
 // force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
-static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
-                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan, const int* force_shape = nullptr) {
+static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
+                      int out_bytes, int n_mpairs, int n_pairs, const int* force_shape, Tc2Plan* plan,
+                      std::vector<Tc2HostItem>* best_items, std::vector<std::vector<int>>* best_lists) {
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
@@ -935,110 +925,116 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   const int ksub = tc2_ksub(K);
   const double op_ns = tc2_op_ns(N, ksub);
   double best_cost = 1e300;
-  int best_shape[4] = {1, 1, 1, 1}, max_b = 0, ring_bytes = 0;
-  std::vector<Tc2HostItem> best_items;
-  std::vector<std::vector<int>> best_lists;
+  plan->maxb = 0;
   std::vector<std::vector<int>> wins;
   for (const Tc2Kind& kind : kTc2Kinds) {
     if (kind.n != N || kind.ksub != ksub || kind.epi != epi || kind.out_bytes != out_bytes) continue;
     if (force_maxb > 0 && kind.maxb != force_maxb) continue;
     const int mb = kind.maxb, ring = tc2_ring_bytes(N, mb, ksub, epi, out_bytes);
     const int step_max = std::min((ring / 3) & ~1023, step_kb * 1024);
-  for (int wh = 1; wh <= 2; ++wh)
-    for (int ww = 1; ww <= 8; ++ww)
-      for (int sy = 1; sy <= (wh > 1 ? 2 : 1); ++sy)
-        for (int sx = 1; sx <= (ww > 1 ? 2 : 1); ++sx) {
-          if (wh * ww > std::min(max_acc, mb) || wh > h_grid || ww > std::max(w_grid, 1)) continue;
-          if (force_shape != nullptr && (wh != force_shape[0] || ww != force_shape[1] || sy != force_shape[2] || sx != force_shape[3])) continue;
-          tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
-          std::vector<Tc2HostItem> items(wins.size());
-          for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, mb, max_a, step_max, &items[i]);
-          std::vector<double> icost(items.size());
-          auto cost_item = [&](const Tc2HostItem& it) {
-            return DGAN_COST_NS_PER_KB / 1024.0 *
-                       (it.stage_bytes + DGAN_COST_EPI_KB * 1024.0 * it.hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0) +
-                   op_ns * (double)it.n_ops + DGAN_COST_STEP_NS * (double)it.steps.size();
-          };
-          std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
-          for (size_t i = 0; i < items.size(); ++i) icost[i] = cost_item(items[i]);
-          // LPT: items (window, mp) largest-first, each to the currently least-loaded CTA pair
-          const long long total = (long long)items.size() * n_mpairs;
-          std::vector<double> load((size_t)n_pairs, 0.0);
-          std::vector<std::vector<int>> lists((size_t)n_pairs);
-          for (long long idx = 0; idx < total; ++idx) {        // items[] is sorted by cost, mp is the fast index: cost-descending
-            size_t best = 0;
-            for (size_t pr = 1; pr < (size_t)n_pairs; ++pr)
-              if (load[pr] < load[best]) best = pr;
-            load[best] += icost[(size_t)(idx / n_mpairs)];
-            lists[best].push_back((int)idx);
-          }
-          // Refinement: while the busiest pair can hand an item to - or swap one with - another pair so that both end
-          // up below its load, do the best such move (LPT alone leaves e.g. 35 on a mean of 30.4 for Generator.2 bwd's
-          // 160 items of cost 4..25).
-          auto cost_of = [&](int idx) { return icost[(size_t)(idx / n_mpairs)]; };
-          // One pass looks at |P| x (1 + |Q|) candidates for every other pair Q: quadratic in the items per pair.  With many
-          // items per pair (large batches: 160 row pairs x 1024 windows) LPT alone is already within one small item of
-          // the mean and the search would take minutes, so it runs on a budget of candidate evaluations that the
-          // benchmarked sizes (<= 20 row pairs) never reach.
-          long long work = 0;
-          for (int iter = 0; iter < 4096 && work < TC2_REFINE_BUDGET; ++iter) {
-            const size_t P = (size_t)(std::max_element(load.begin(), load.end()) - load.begin());
-            double best_peak = load[P];
-            size_t bq = P; int bi = -1, bj = -1;
-            for (size_t Q = 0; Q < (size_t)n_pairs; ++Q) {
-              if (Q == P) continue;
-              work += (long long)lists[P].size() * (long long)(1 + lists[Q].size());
-              for (size_t i = 0; i < lists[P].size(); ++i) {
-                const double ci = cost_of(lists[P][i]);
-                double peak = std::max(load[P] - ci, load[Q] + ci);           // move i: P -> Q
-                if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = -1; }
-                for (size_t j = 0; j < lists[Q].size(); ++j) {                 // swap i <-> j
-                  const double cj = cost_of(lists[Q][j]);
-                  if (cj >= ci) continue;
-                  peak = std::max(load[P] - ci + cj, load[Q] + ci - cj);
-                  if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = (int)j; }
+    for (int wh = 1; wh <= 2; ++wh)
+      for (int ww = 1; ww <= 8; ++ww)
+        for (int sy = 1; sy <= (wh > 1 ? 2 : 1); ++sy)
+          for (int sx = 1; sx <= (ww > 1 ? 2 : 1); ++sx) {
+            if (wh * ww > std::min(max_acc, mb) || wh > h_grid || ww > std::max(w_grid, 1)) continue;
+            if (force_shape != nullptr && (wh != force_shape[0] || ww != force_shape[1] || sy != force_shape[2] || sx != force_shape[3])) continue;
+            tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
+            std::vector<Tc2HostItem> items(wins.size());
+            for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, mb, max_a, step_max, &items[i]);
+            std::vector<double> icost(items.size());
+            auto cost_item = [&](const Tc2HostItem& it) {
+              return DGAN_COST_NS_PER_KB / 1024.0 *
+                         (it.stage_bytes + DGAN_COST_EPI_KB * 1024.0 * it.hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0) +
+                     op_ns * (double)it.n_ops + DGAN_COST_STEP_NS * (double)it.steps.size();
+            };
+            std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
+            for (size_t i = 0; i < items.size(); ++i) icost[i] = cost_item(items[i]);
+            // LPT: items (window, mp) largest-first, each to the currently least-loaded CTA pair
+            const long long total = (long long)items.size() * n_mpairs;
+            std::vector<double> load((size_t)n_pairs, 0.0);
+            std::vector<std::vector<int>> lists((size_t)n_pairs);
+            for (long long idx = 0; idx < total; ++idx) {        // items[] is sorted by cost, mp is the fast index: cost-descending
+              size_t best = 0;
+              for (size_t pr = 1; pr < (size_t)n_pairs; ++pr)
+                if (load[pr] < load[best]) best = pr;
+              load[best] += icost[(size_t)(idx / n_mpairs)];
+              lists[best].push_back((int)idx);
+            }
+            // Refinement: while the busiest pair can hand an item to - or swap one with - another pair so that both end
+            // up below its load, do the best such move (LPT alone leaves e.g. 35 on a mean of 30.4 for Generator.2 bwd's
+            // 160 items of cost 4..25).
+            auto cost_of = [&](int idx) { return icost[(size_t)(idx / n_mpairs)]; };
+            // One pass looks at |P| x (1 + |Q|) candidates for every other pair Q: quadratic in the items per pair.  With many
+            // items per pair (large batches: 160 row pairs x 1024 windows) LPT alone is already within one small item of
+            // the mean and the search would take minutes, so it runs on a budget of candidate evaluations that the
+            // benchmarked sizes (<= 20 row pairs) never reach.
+            long long work = 0;
+            for (int iter = 0; iter < 4096 && work < TC2_REFINE_BUDGET; ++iter) {
+              const size_t P = (size_t)(std::max_element(load.begin(), load.end()) - load.begin());
+              double best_peak = load[P];
+              size_t bq = P; int bi = -1, bj = -1;
+              for (size_t Q = 0; Q < (size_t)n_pairs; ++Q) {
+                if (Q == P) continue;
+                work += (long long)lists[P].size() * (long long)(1 + lists[Q].size());
+                for (size_t i = 0; i < lists[P].size(); ++i) {
+                  const double ci = cost_of(lists[P][i]);
+                  double peak = std::max(load[P] - ci, load[Q] + ci);           // move i: P -> Q
+                  if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = -1; }
+                  for (size_t j = 0; j < lists[Q].size(); ++j) {                 // swap i <-> j
+                    const double cj = cost_of(lists[Q][j]);
+                    if (cj >= ci) continue;
+                    peak = std::max(load[P] - ci + cj, load[Q] + ci - cj);
+                    if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = (int)j; }
+                  }
                 }
               }
-            }
-            if (bi < 0) break;
-            const int it_i = lists[P][(size_t)bi];
-            const double ci = cost_of(it_i);
-            if (bj < 0) {
-              lists[P].erase(lists[P].begin() + bi);
-              lists[bq].push_back(it_i);
-              load[P] -= ci; load[bq] += ci;
-            } else {
-              const int it_j = lists[bq][(size_t)bj];
-              const double cj = cost_of(it_j);
-              lists[P][(size_t)bi] = it_j; lists[bq][(size_t)bj] = it_i;
-              load[P] += cj - ci; load[bq] += ci - cj;
-            }
-          }
-          for (auto& l : lists)      // biggest first: a pair's last item is its smallest (shortest un-overlapped epilogue)
-            std::stable_sort(l.begin(), l.end(), [&](int a, int b) { return cost_of(a) > cost_of(b); });
-          const double makespan = *std::max_element(load.begin(), load.end());
-          if (makespan < best_cost) {
-            best_cost = makespan;
-            plan->load_max = makespan;
-            plan->load_mean = std::accumulate(load.begin(), load.end(), 0.0) / (double)n_pairs;
-            best_shape[0] = wh; best_shape[1] = ww; best_shape[2] = sy; best_shape[3] = sx;
-            max_b = mb; ring_bytes = ring;
-            plan->op_ns_max = 0.0;
-            for (size_t pr = 0; pr < lists.size(); ++pr)
-              if (load[pr] == makespan) {
-                for (int idx : lists[pr]) plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
-                break;
+              if (bi < 0) break;
+              const int it_i = lists[P][(size_t)bi];
+              const double ci = cost_of(it_i);
+              if (bj < 0) {
+                lists[P].erase(lists[P].begin() + bi);
+                lists[bq].push_back(it_i);
+                load[P] -= ci; load[bq] += ci;
+              } else {
+                const int it_j = lists[bq][(size_t)bj];
+                const double cj = cost_of(it_j);
+                lists[P][(size_t)bi] = it_j; lists[bq][(size_t)bj] = it_i;
+                load[P] += cj - ci; load[bq] += ci - cj;
               }
-            best_items.swap(items); best_lists.swap(lists);
+            }
+            for (auto& l : lists)      // biggest first: a pair's last item is its smallest (shortest un-overlapped epilogue)
+              std::stable_sort(l.begin(), l.end(), [&](int a, int b) { return cost_of(a) > cost_of(b); });
+            const double makespan = *std::max_element(load.begin(), load.end());
+            if (makespan < best_cost) {
+              best_cost = makespan;
+              plan->load_max = makespan;
+              plan->load_mean = std::accumulate(load.begin(), load.end(), 0.0) / (double)n_pairs;
+              plan->shape[0] = wh; plan->shape[1] = ww; plan->shape[2] = sy; plan->shape[3] = sx;
+              plan->maxb = mb; plan->ring_bytes = ring;
+              plan->op_ns_max = 0.0;
+              for (size_t pr = 0; pr < lists.size(); ++pr)
+                if (load[pr] == makespan) {
+                  for (int idx : lists[pr]) plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
+                  break;
+                }
+              best_items->swap(items); best_lists->swap(lists);
+            }
           }
-        }
   }
-  if (max_b == 0) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
-  plan->maxb = max_b; plan->ring_bytes = ring_bytes; plan->ksub = ksub;
-  plan->shape[0] = best_shape[0]; plan->shape[1] = best_shape[1]; plan->shape[2] = best_shape[2]; plan->shape[3] = best_shape[3];
+  if (plan->maxb == 0) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
+  plan->ksub = ksub;
+  return 0;
+}
+
+// Per CTA pair, its items' steps in issue order: simulate the pair's circular operand ring to give every step its
+// region and dependency distance, and encode the producer and MMA records and the epilogue item list.  The only
+// writer of the records.
+static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vector<Tc2HostItem>& items,
+                              const std::vector<std::vector<int>>& lists, Tc2Plan* plan) {
+  const int max_b = plan->maxb, ring_bytes = plan->ring_bytes, ksub = plan->ksub;
   plan->n_pairs = n_pairs;
   size_t n_slots = 0;
-  for (auto& l : best_lists) n_slots = std::max(n_slots, l.size());
+  for (auto& l : lists) n_slots = std::max(n_slots, l.size());
   plan->n_slots = (int)n_slots;
   std::vector<int>& eitems = plan->eitems;
   eitems.assign(n_slots * (size_t)n_pairs, -1);
@@ -1048,16 +1044,16 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
   std::vector<TcRec>& stream_m = plan->stream_m;
   stream_p.clear(); stream_m.clear();
   long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;
-  for (size_t pr = 0; pr < best_lists.size(); ++pr) {
+  for (size_t pr = 0; pr < lists.size(); ++pr) {
     stream_off[pr] = (uint32_t)stream_m.size();
     // circular operand ring of this CTA pair: sequential allocation, wrap when the step does not fit
     std::vector<std::pair<int, int>> region;     // [begin, end) in KB of every step of this stream
     int cursor = 0;
-    for (size_t k = 0; k < best_lists[pr].size(); ++k) {
-      const int win = best_lists[pr][k] / n_mpairs, mp = best_lists[pr][k] % n_mpairs;
-      if (win > 0x7FFF || mp > 0xFFFF) { set_error("tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
-      eitems[k * (size_t)n_pairs + pr] = (win << 16) | mp;
-      const Tc2HostItem& itm = best_items[(size_t)win];
+    for (size_t k = 0; k < lists[pr].size(); ++k) {
+      const int win = lists[pr][k] / n_mpairs, mp = lists[pr][k] % n_mpairs;
+      if ((uint32_t)win > TcItemWindow::mask || (uint32_t)mp > TcItemMp::mask) { set_error("tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
+      eitems[k * (size_t)n_pairs + pr] = tc2_item_word(win, mp);
+      const Tc2HostItem& itm = items[(size_t)win];
       for (size_t j = 0; j < itm.steps.size(); ++j) {
         const Tc2HostStep& hs = itm.steps[j];
         const int kb = (hs.bytes + 1023) / 1024;
@@ -1075,18 +1071,16 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
         }
         if (dep == 1 && j > 0) { set_error("tensor-core step overlaps the step before it (ring too small)"); return DGAN_ERR_UNSUPPORTED; }
         region.push_back({beg, end});
-        const uint32_t flags = (j == 0 ? 1u : 0u) | (j + 1 == itm.steps.size() ? 2u : 0u);
-        TcRec rm{};
-        rm.w[0] = (uint32_t)beg | ((uint32_t)hs.nA << 8) | ((uint32_t)hs.n_rounds << 11) | (flags << 16);
-        rm.w[1] = (uint32_t)max_b | ((uint32_t)ksub << 8);
-        for (int o = 0; o < hs.n_rounds * max_b; ++o) rm.w[2 + o / 4] |= (uint32_t)hs.ops[o] << (8 * (o & 3));
-        stream_m.push_back(rm);
-        TcRec rp{};
-        rp.w[0] = (uint32_t)beg | ((uint32_t)hs.kc << 8) | ((uint32_t)hs.nA << 12) | ((uint32_t)hs.nB << 15) | ((uint32_t)dep << 19);
-        rp.w[1] = (uint32_t)mp;
-        for (int a = 0; a < hs.nA; ++a) rp.w[2 + a / 2] |= (uint32_t)(hs.a_pix[a] & 0xFFFF) << (16 * (a & 1));
-        for (int b = 0; b < hs.nB; ++b) rp.w[4 + b / 4] |= (uint32_t)hs.b_ent[b] << (8 * (b & 3));
-        stream_p.push_back(rp);
+        TcMmaRec m;
+        m.off = (uint32_t)beg; m.nA = (uint32_t)hs.nA; m.n_rounds = (uint32_t)hs.n_rounds; m.maxb = (uint32_t)max_b; m.ksub = (uint32_t)ksub;
+        m.flags = (j == 0 ? TcMmaRec::FIRST : 0u) | (j + 1 == itm.steps.size() ? TcMmaRec::LAST : 0u);
+        std::copy(hs.ops, hs.ops + hs.n_rounds * max_b, m.ops);    // the op bytes of later rounds stay 0
+        stream_m.push_back(m.encode());
+        TcProducerRec p;
+        p.off = (uint32_t)beg; p.kc = (uint32_t)hs.kc; p.nA = (uint32_t)hs.nA; p.nB = (uint32_t)hs.nB; p.dep = (uint32_t)dep; p.mp = (uint32_t)mp;
+        std::copy(hs.a_pix, hs.a_pix + TC2_MAX_A, p.pix);
+        std::copy(hs.b_ent, hs.b_ent + TC2_MAX_BSLOTS, p.tile);
+        stream_p.push_back(p.encode());
         // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
         n_mma += hs.n_rounds * max_b; n_pad += hs.n_rounds * max_b - hs.n_real;
         n_steps += 1; n_bytes += 2LL * hs.nA * tc2_a_bytes(ksub) + (long long)hs.nB * tc2_b_bytes(N, ksub);
@@ -1094,10 +1088,20 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
     }
   }
   stream_off[(size_t)n_pairs] = (uint32_t)stream_m.size();
-  plan->hdrs.resize(best_items.size());
-  for (size_t i = 0; i < best_items.size(); ++i) plan->hdrs[i] = best_items[i].hdr;
+  plan->hdrs.resize(items.size());
+  for (size_t i = 0; i < items.size(); ++i) plan->hdrs[i] = items[i].hdr;
   plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
   return 0;
+}
+
+// The plan of one layer-direction.  force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
+static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
+                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan, const int* force_shape = nullptr) {
+  std::vector<Tc2HostItem> items;
+  std::vector<std::vector<int>> lists;
+  const int rc = tc2_search(N, K, tab, h_grid, w_grid, max_acc, force_maxb, epi, out_bytes, n_mpairs, n_pairs, force_shape,
+                            plan, &items, &lists);
+  return rc ? rc : tc2_encode_streams(N, n_mpairs, n_pairs, items, lists, plan);
 }
 
 // Independent validation of a plan against the pair table it was built from (host only; used by
@@ -1134,7 +1138,7 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
     for (uint32_t a = 0; a < h.n_acc; ++a)
       if ((size_t)h.q[a] + 1 >= tab.off.size()) return fail("window pixel out of range");
   }
-  struct Step { int beg, end, nB, kc; uint8_t b[8]; };
+  struct Step { int beg, end; };
   for (size_t pr = 0; pr < n_pairs; ++pr) {
     const uint32_t r_beg = pl.stream_off[pr], r_end = pl.stream_off[pr + 1];
     if (r_beg > r_end || r_end > pl.stream_m.size()) return fail("stream_off not monotone");
@@ -1145,31 +1149,29 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
     std::vector<std::pair<int, int>> last_kp;                     // per accumulator: last (kc, p)
     std::vector<std::vector<std::pair<int, int>>> contrib;        // per accumulator: (p * 32 + tile, kc)
     for (uint32_t ri = r_beg; ri < r_end; ++ri) {
-      const TcRec &m = pl.stream_m[ri], &p0 = pl.stream_p[ri];
+      const TcMmaRec m = TcMmaRec::decode(pl.stream_m[ri]);
+      const TcProducerRec p0 = TcProducerRec::decode(pl.stream_p[ri]);
       const int k = (int)steps.size();
-      Step st{};
-      st.beg = (int)(p0.w[0] & 0xFF);
-      const int nA = (int)((p0.w[0] >> 12) & 7), nB = (int)((p0.w[0] >> 15) & 0xF), dep = (int)((p0.w[0] >> 19) & 0xF);
-      st.kc = (int)((p0.w[0] >> 8) & 0xF); st.nB = nB;
-      if ((int)(m.w[0] & 0xFF) != st.beg || (int)((m.w[0] >> 8) & 7) != nA) return fail("MMA record disagrees with the producer record");
-      if (nA < 1 || nA > TC2_MAX_A || nB > TC2_MAX_BSLOTS || st.kc >= kch) return fail("step field out of range");
+      const int nA = (int)p0.nA, nB = (int)p0.nB, dep = (int)p0.dep, kc = (int)p0.kc;
+      Step st{(int)p0.off, 0};
+      if (m.off != p0.off || m.nA != p0.nA) return fail("MMA record disagrees with the producer record");
+      if (nA < 1 || nA > TC2_MAX_A || nB > TC2_MAX_BSLOTS || kc >= kch) return fail("step field out of range");
       st.end = st.beg + (nA * a_bytes + nB * b_tile + 1023) / 1024;
       if (st.end * 1024 > ring_bytes) return fail("step region outside the ring");
       if (dep < 1 || dep > TC2_NSLOT) return fail("dep out of range");
-      for (int b = 0; b < 8; ++b) st.b[b] = (uint8_t)(p0.w[4 + b / 4] >> (8 * (b & 3)));
-      const uint32_t flags = (m.w[0] >> 16) & 3u;
-      const int n_rounds = (int)((m.w[0] >> 11) & 0x1F);
-      if ((int)(m.w[1] & 0xFFu) != max_acc) return fail("MMA record disagrees with the plan on the accumulator slots per round");
-      if ((int)(m.w[1] >> 8) != ksub) return fail("MMA record disagrees with the instantiation on the k16 sub-tiles per op");
+      const uint32_t flags = m.flags;
+      const int n_rounds = (int)m.n_rounds;
+      if ((int)m.maxb != max_acc) return fail("MMA record disagrees with the plan on the accumulator slots per round");
+      if ((int)m.ksub != ksub) return fail("MMA record disagrees with the instantiation on the k16 sub-tiles per op");
       if (n_rounds < 1 || n_rounds * max_acc > TC2_OP_BYTES) return fail("round count out of range");
-      if (dep == 1 && !(flags & 1u)) return fail("ring deadlock: a step waits for the step before it, which is released only after it");
-      if (flags & 1u) {
+      if (dep == 1 && !(flags & TcMmaRec::FIRST)) return fail("ring deadlock: a step waits for the step before it, which is released only after it");
+      if (flags & TcMmaRec::FIRST) {
         if (in_item) return fail("item starts inside an item");
         in_item = true; ++item_k;
         if (item_k >= pl.n_slots) return fail("more items than slots");
         const int e = pl.eitems[(size_t)item_k * n_pairs + pr];
         if (e < 0) return fail("stream has an item the epilogue list lacks");
-        win = e >> 16; mp = e & 0xFFFF;
+        win = tc2_item_window(e); mp = tc2_item_mp(e);
         if ((size_t)win >= pl.hdrs.size() || mp >= n_mpairs) return fail("item index out of range");
         if (assigned[(size_t)win * n_mpairs + mp]++) return fail("item assigned twice");
         seen = 0;
@@ -1177,14 +1179,14 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
         contrib.assign(pl.hdrs[win].n_acc, {});
       }
       if (!in_item) return fail("step outside an item");
-      if ((int)(p0.w[1] & 0xFFFF) != mp) return fail("row pair of a step differs from its item");
+      if ((int)p0.mp != mp) return fail("row pair of a step differs from its item");
       const TcItem2& hdr = pl.hdrs[win];
       // the kernel issues round by round, accumulator 0 .. max_acc - 1 within a round
       for (int oi = 0; oi < n_rounds * max_acc; ++oi) {
-        const uint32_t e = (m.w[2 + oi / 4] >> (8 * (oi & 3))) & 0xFFu;
-        const int a_idx = e & 3, slot = (e >> 2) & 0xF, acc = oi % max_acc;
-        const bool first = (e >> 6) & 1;
-        if (e & 0x80u) return fail("op field out of range");
+        const TcOp op = TcOp::decode(m.ops[oi]);
+        const int a_idx = (int)op.a, slot = (int)op.slot, acc = oi % max_acc;
+        const bool first = op.first != 0;
+        if (m.ops[oi] & ~TcOp::USED) return fail("op field out of range");
         if (slot == TC2_ZERO_SLOT) {
           if (max_acc == 1) return fail("zero-tile op in an instantiation without a zero tile");
           if (first) return fail("zero-tile op overwrites its accumulator");
@@ -1193,14 +1195,14 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
         if (a_idx >= nA) return fail("op reads an A tile the step does not stage");
         if (acc >= (int)hdr.n_acc) return fail("op writes past the window's accumulators");
         if (slot >= nB) return fail("op reads a B slot the step does not stage");
-        if (st.b[slot] & 0xE0) return fail("weight tile entry out of range");
-        const int p = (int)((p0.w[2 + a_idx / 2] >> (16 * (a_idx & 1))) & 0xFFFF);
+        if (p0.tile[slot] > TcProducerRec::Tile::mask) return fail("weight tile entry out of range");
+        const int p = (int)p0.pix[a_idx];
         const bool unseen = !(seen & (1u << acc));
         if (first != unseen) return fail(first ? "overwrite of a live accumulator" : "accumulate into an uninitialised accumulator");
-        const std::pair<int, int> kp{st.kc, p};
+        const std::pair<int, int> kp{kc, p};
         if (!(last_kp[acc] < kp)) return fail("accumulation order is not canonical (k-chunk major, pixel ascending)");
         last_kp[acc] = kp;
-        contrib[acc].push_back({p * 32 + st.b[slot], st.kc});
+        contrib[acc].push_back({p * 32 + (int)p0.tile[slot], kc});
         seen |= 1u << acc;
       }
       // ring safety
@@ -1210,7 +1212,7 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
         if (c > k - dep) return fail("ring hazard: a region may be overwritten while it can still be read");
       }
       steps.push_back(st);
-      if (flags & 2u) {
+      if (flags & TcMmaRec::LAST) {
         for (uint32_t a = 0; a < hdr.n_acc; ++a) {
           std::vector<std::pair<int, int>> want;
           for (int kc = 0; kc < kch; ++kc)
@@ -1243,8 +1245,7 @@ static int tc2_get_schedule(TcDir& d, int n_mpairs, int n_pairs, std::vector<voi
   const cudaStream_t s = 0;
   Tc2Schedule sc;
   sc.maxb = plan.maxb;
-  sc.wh = plan.shape[0]; sc.ww = plan.shape[1]; sc.sy = plan.shape[2]; sc.sx = plan.shape[3];
-  sc.n_windows = (int)plan.hdrs.size(); sc.n_pairs = n_pairs; sc.n_slots = plan.n_slots;
+  sc.n_pairs = n_pairs; sc.n_slots = plan.n_slots;
   if ((rc = tc_upload(allocs, plan.hdrs.data(), plan.hdrs.size() * sizeof(TcItem2), (void**)&sc.items, s))) return rc;
   if ((rc = tc_upload(allocs, plan.stream_p.data(), plan.stream_p.size() * sizeof(TcRec), (void**)&sc.stream_p, s))) return rc;
   if ((rc = tc_upload(allocs, plan.stream_m.data(), plan.stream_m.size() * sizeof(TcRec), (void**)&sc.stream_m, s))) return rc;
