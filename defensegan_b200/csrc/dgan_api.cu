@@ -82,66 +82,147 @@ PairTable linear_bwd_pairs(int n_pix) {
   return t;
 }
 
-// The generator's transposed convs between the Linear (4x4 pixels of 4 * net_dim channels) and the last layer, whose
+// The generator's channel widths: the latent and the outputs of the Linear (4 * net_dim), of Generator.2 (2 * net_dim)
+// and of the later layers (net_dim).
+struct Widths { int latent, c4, c2, c1; };
+static Widths real_widths(const dgan_desc* d) { return {d->latent_dim, 4 * d->net_dim, 2 * d->net_dim, d->net_dim}; }
+
+// Shared memory of the fp32 last layer's forward (final_fwd_loss_kernel): all 25 taps of the filter and the input rows of
+// one band of output rows.
+static size_t final_fwd_smem(int c_in, int c_out, int w_in) {
+  return ((size_t)kTaps * c_out * c_in + (size_t)(kBandRows / 2 + 2) * w_in * (c_in + 4)) * 4;
+}
+// dynamic shared memory the fp32 last layer opts in to: the 227 KB a block may have on an H100, less 1 KB for the
+// kernels' static shared memory, which counts against the same limit
+constexpr int kFinalSmemMax = TC2_SMEM_MAX - 1024;
+
+// The width rule: every channel width a handle stores, padded with exact zeros (weight rows and columns, biases, BN
+// offset and scale), so that the padded activations and gradients are exactly 0 and every real output is the unpadded
+// sum with zero terms appended - its bits do not change.
+//   fp32 path: the next multiple of 64, the output tile of bsgemm_f32_kernel (a width it served before is not padded).
+//   fp16 path: the smallest of 64, 128 and 256 that holds the width, the N of a tensor-core instantiation; above 256, the
+//              next multiple of 256, computed in column blocks of 256 (tc_directions).  The Linear's output is at least
+//              256 wide: its per-pixel bias is served by the N = 256 instantiations only (tc_dir_supported).
+//              latent_dim <= 256 and net_dim <= 128 keep every K within 512 channels, 8 k-chunks (tc_records.cuh).
+// Returns 0 with the padded widths, or DGAN_ERR_UNSUPPORTED naming the limit.  Creation, tc_directions, carve (through
+// the handle) and the plan validator all take their widths from here.
+static int padded_widths(const dgan_desc* d, Widths* out) {
+  if (d->latent_dim <= 0 || d->net_dim <= 0) { set_error("unsupported widths: latent_dim and net_dim must be positive"); return DGAN_ERR_UNSUPPORTED; }
+  const Widths r = real_widths(d);
+  if (d->precision == DGAN_PREC_FP16) {
+    if (d->latent_dim > 256) { set_error("unsupported latent_dim " + std::to_string(d->latent_dim) + ": the fp16 path takes latent_dim <= 256"); return DGAN_ERR_UNSUPPORTED; }
+    if (d->net_dim > 128) { set_error("unsupported net_dim " + std::to_string(d->net_dim) + ": the fp16 path takes net_dim <= 128 (K <= 512 channels)"); return DGAN_ERR_UNSUPPORTED; }
+    auto pad = [](int w) { return w <= 64 ? 64 : w <= 128 ? 128 : (w + 255) / 256 * 256; };
+    *out = {pad(r.latent), std::max(256, pad(r.c4)), pad(r.c2), pad(r.c1)};
+    return 0;
+  }
+  auto pad = [](int w) { return (w + 63) / 64 * 64; };
+  *out = {pad(r.latent), pad(r.c4), pad(r.c2), pad(r.c1)};
+  const bool celeba = d->arch == DGAN_ARCH_CELEBA;
+  const int c_img = celeba ? 3 : 1, w_in = celeba ? 32 : 14;
+  if (final_fwd_smem(out->c1, c_img, w_in) > (size_t)kFinalSmemMax) {
+    int max_nd = 64;
+    while (final_fwd_smem(max_nd + 64, c_img, w_in) <= (size_t)kFinalSmemMax) max_nd += 64;
+    set_error("unsupported net_dim " + std::to_string(d->net_dim) + ": the fp32 last layer holds its filter and input rows in "
+              "shared memory, which allows net_dim <= " + std::to_string(max_nd) + (celeba ? " on CelebA" : " on MNIST"));
+    return DGAN_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+
+// The generator's transposed convs between the Linear (4x4 pixels of c4 channels) and the last layer, whose
 // input is the last one's output: channels in and out, valid input rows, output rows, input raster, ReLU after the bias.
 struct DeconvSpec { int c_in, c_out, h_in, h_used, in_raster; bool relu; };
-static std::vector<DeconvSpec> deconv_specs(const dgan_desc* d) {
-  const int nd = d->net_dim;
-  if (d->arch == DGAN_ARCH_CELEBA) return {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 8, 16, 8, true}, {nd, nd, 16, 32, 16, false}};
+static std::vector<DeconvSpec> deconv_specs(const dgan_desc* d, const Widths& w) {
+  if (d->arch == DGAN_ARCH_CELEBA) return {{w.c4, w.c2, 4, 8, 4, true}, {w.c2, w.c1, 8, 16, 8, true}, {w.c1, w.c1, 16, 32, 16, false}};
   if (d->use_bn)   // BN2's batch statistics cover all 8x8 outputs of Generator.2; the 7x7 crop comes after BN+ReLU
-    return {{4 * nd, 2 * nd, 4, 8, 4, true}, {2 * nd, nd, 7, 14, 8, true}};
-  return {{4 * nd, 2 * nd, 4, 7, 4, true}, {2 * nd, nd, 7, 14, 7, true}};
+    return {{w.c4, w.c2, 4, 8, 4, true}, {w.c2, w.c1, 7, 14, 8, true}};
+  return {{w.c4, w.c2, 4, 7, 4, true}, {w.c2, w.c1, 7, 14, 7, true}};
 }
 
 // Every layer-direction of the fp16 path, in launch-site and profile-kind order: layer l forward, layer l backward, ...,
 // last layer forward, last layer backward.  A function of the desc alone: the CPU tests plan without a GPU.
 // With BatchNorm after a layer (use_bn: the Linear, Generator.2 and Generator.3) its forward writes fp32 pre-activations
 // without the ReLU, and the backward into its output applies no mask (the BN backward does both).
+// Widths are the padded ones of padded_widths(); a desc it refuses has no directions.  A layer-direction with more than
+// 256 output channels becomes one entry per column block of 256, named and profiled as e.g. "Linear.fwd[256:512]".
 static std::vector<TcDir> tc_directions(const dgan_desc* d) {
   const bool celeba = d->arch == DGAN_ARCH_CELEBA;
-  const int nd = d->net_dim, c_img = celeba ? 3 : 1;
+  const int c_img = celeba ? 3 : 1;
   std::vector<TcDir> dirs;
+  Widths wd;
+  if (padded_widths(d, &wd) != 0) return dirs;
+  const Widths rw = real_widths(d);
+  int ld = 0;
+  // n_real: the real output channels of the layer-direction
   auto add = [&](const std::string& name, const std::string& kind, int N, int K, int P_in, int P_out, int n_tiles,
-                 PairTable tab, int h_grid, int w_grid, int epi, int out_bytes) {
-    TcDir t;
-    t.name = name; t.kind = kind; t.N = N; t.K = K; t.P_in = P_in; t.P_out = P_out; t.n_tiles = n_tiles;
-    t.tab = std::move(tab); t.h_grid = h_grid; t.w_grid = w_grid; t.max_acc = tc2_maxb(N);
-    t.epi = epi; t.out_bytes = out_bytes;
-    dirs.push_back(std::move(t));
+                 PairTable tab, int h_grid, int w_grid, int epi, int out_bytes, int n_real) {
+    for (int col0 = 0; col0 < N; col0 += 256) {
+      const int nb = std::min(256, N - col0);
+      const std::string blk = nb == N ? "" : "[" + std::to_string(col0) + ":" + std::to_string(col0 + nb) + "]";
+      TcDir t;
+      t.name = name + blk; t.kind = kind + blk; t.base_kind = kind; t.N = nb; t.K = K; t.P_in = P_in; t.P_out = P_out;
+      t.n_tiles = n_tiles; t.tab = tab; t.h_grid = h_grid; t.w_grid = w_grid; t.max_acc = tc2_maxb(nb);
+      t.epi = epi; t.out_bytes = out_bytes; t.ld = ld; t.col0 = col0; t.out_ld = N; t.n_real = n_real;
+      dirs.push_back(std::move(t));
+    }
+    ++ld;
   };
   // a GEMM layer's directions have one weight tile more than their pairs use: the all-zero tile of tc_with_zero_tile()
   const bool bn0 = d->use_bn != 0;
-  add("Linear.fwd", "Linear.fwd", 4 * nd, d->latent_dim, 1, 16, 17, tc_with_zero_tile(linear_fwd_pairs(16), 16), 4, 4,
-      bn0 ? EPI_BIAS : EPI_BIAS_RELU, bn0 ? 4 : 2);
-  dirs.back().bias_pstride = 4 * nd;                 // bias index f = pixel * C_out + c
+  add("Linear.fwd", "Linear.fwd", wd.c4, wd.latent, 1, 16, 17, tc_with_zero_tile(linear_fwd_pairs(16), 16), 4, 4,
+      bn0 ? EPI_BIAS : EPI_BIAS_RELU, bn0 ? 4 : 2, rw.c4);
+  for (TcDir& t : dirs) t.bias_pstride = wd.c4;     // bias index f = pixel * C_out + c
   // dz as TC_LINEAR_SPLIT partial sums over the 16 pixels, one accumulator per window
-  add("Linear.bwd", "Linear.bwd", d->latent_dim, 4 * nd, 16, TC_LINEAR_SPLIT, 17, linear_split_pairs(16), 1, TC_LINEAR_SPLIT,
-      EPI_NONE, 4);
+  add("Linear.bwd", "Linear.bwd", wd.latent, wd.c4, 16, TC_LINEAR_SPLIT, 17, linear_split_pairs(16), 1, TC_LINEAR_SPLIT,
+      EPI_NONE, 4, rw.latent);
   dirs.back().max_acc = 1;
   bool mask_in = !bn0;                               // the backward into the previous layer's output applies its ReLU mask
-  const std::vector<DeconvSpec> specs = deconv_specs(d);
+  const std::vector<DeconvSpec> specs = deconv_specs(d, wd), real_specs = deconv_specs(d, rw);
   int li = 2;
   for (const DeconvSpec& sp : specs) {
     const std::string nm = "Generator." + std::to_string(li == 4 ? 5 : li);
     const bool bn = d->use_bn && li <= 3;
+    const DeconvSpec& rs = real_specs[(size_t)(li - 2)];
     add(nm + ".fwd", nm + ".fwd", sp.c_out, sp.c_in, sp.in_raster * sp.in_raster, sp.h_used * sp.h_used, kTaps + 1,
         tc_with_zero_tile(deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.h_used, sp.h_used,
-        (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2);
+        (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2, rs.c_out);
     add(nm + ".bwd", nm + ".bwd", sp.c_in, sp.c_out, sp.h_used * sp.h_used, sp.in_raster * sp.in_raster, kTaps + 1,
         tc_with_zero_tile(deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.in_raster,
-        sp.in_raster, mask_in ? EPI_MASK : EPI_NONE, 2);
+        sp.in_raster, mask_in ? EPI_MASK : EPI_NONE, 2, rs.c_in);
     mask_in = sp.relu && !bn;
     ++li;
   }
   // the last layer on 4x4 blocks of image pixels (16 weight tiles per direction); its forward computes the loss
   const int fh = specs.back().h_used, n_blocks = (fh / 2) * (fh / 2);
   const std::string fn = celeba ? "Generator.6" : "Generator.5";
-  add("last.fwd", fn + "+loss.fwd", 16 * c_img, nd, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2,
-      celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2);
+  add("last.fwd", fn + "+loss.fwd", 16 * c_img, wd.c1, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2,
+      celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2, 16 * c_img);
   // K: the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
-  add("last.bwd", fn + ".bwd", nd, 16 * c_img, n_blocks, fh * fh, 16, final_block_bwd_pairs(fh, fh), fh, fh,
-      mask_in ? EPI_MASK : EPI_NONE, 2);
+  add("last.bwd", fn + ".bwd", wd.c1, 16 * c_img, n_blocks, fh * fh, 16, final_block_bwd_pairs(fh, fh), fh, fh,
+      mask_in ? EPI_MASK : EPI_NONE, 2, rw.c1);
   return dirs;
+}
+
+// Can the tensor-core path run layer-direction t?  One check for dgan_create and the plan validator: an instantiation of
+// TC2_KINDS has its N, k16 MMAs per op, epilogue and output type; K is whole 64-channel k-chunks, at most 512 channels
+// (the 4-bit k-chunk field of the producer record is not checked at run time, tc_records.cuh), or a narrow operand of
+// 16-channel sub-tiles; and the planner's tables hold its tiles and pixels.
+static int tc_dir_supported(const TcDir& t) {
+  const int ksub = tc2_ksub(t.K);
+  bool kind = false;
+  for (const Tc2Kind& k : kTc2Kinds) kind = kind || (k.n == t.N && k.ksub == ksub && k.epi == t.epi && k.out_bytes == t.out_bytes);
+  if (!kind) {
+    set_error(t.name + ": unsupported N = " + std::to_string(t.N) + ", K = " + std::to_string(t.K) + ": no tensor-core instantiation");
+    return DGAN_ERR_UNSUPPORTED;
+  }
+  if (t.K <= 0 || t.K > 512 || (t.K % 64 != 0 && (t.K > 48 || t.K % 16 != 0))) {
+    set_error(t.name + ": unsupported K = " + std::to_string(t.K) + ": the tensor-core path takes multiples of 64 up to 512 input channels, or 16 / 32 / 48");
+    return DGAN_ERR_UNSUPPORTED;
+  }
+  if (t.n_tiles > 32 || t.P_in > 65535 || t.P_out > 65535) { set_error(t.name + ": unsupported geometry: tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
+  if (t.bias_pstride != 0 && t.N != 256) { set_error(t.name + ": unsupported N = " + std::to_string(t.N) + ": a per-pixel bias needs N = 256"); return DGAN_ERR_UNSUPPORTED; }
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -168,6 +249,7 @@ struct GemmLayer {
   const float* bn_offset = nullptr;   // use_bn: Generator.BN{1,2,3}.offset / .scale (else null)
   const float* bn_scale = nullptr;
   int bn_per_pixel = 0;               // BN1 normalises each flat feature (axes [0]); BN2/3 each channel (axes [0,1,2])
+  int64_t macs = 0;                   // algorithmic MACs per latent row, at the real widths (padding is not work)
 };
 
 struct FinalLayer {
@@ -185,6 +267,7 @@ using namespace dgan;
 
 struct dgan_ctx {
   dgan_desc desc;
+  Widths wd{};                         // the padded widths the handle stores (padded_widths)
   int H = 0, W = 0, C = 0, hwc = 0;
   std::vector<GemmLayer> layers;
   FinalLayer fin;
@@ -217,7 +300,7 @@ namespace dgan {
 
 struct ProfScope {
   dgan_ctx* c; cudaStream_t s; bool on; dgan_ctx::ProfRec r;
-  ProfScope(dgan_ctx* c_, int kind, cudaStream_t s_) : c(c_), s(s_), on(c_->profile) {
+  ProfScope(dgan_ctx* c_, int kind, cudaStream_t s_) : c(c_), s(s_), on(c_->profile && kind >= 0) {
     if (!on) return;
     r.kind = kind;
     cudaEventCreate(&r.a); cudaEventCreate(&r.b);
@@ -259,18 +342,29 @@ __global__ void transpose_tiles_kernel(const float* __restrict__ in, float* __re
   out[t * per + (size_t)cc * rows + r] = in[i];
 }
 
-// out = s * (sum of the n_parts partial sums, fixed order); with row_scale, row r (row_len values) is also divided by
-// row_scale[r] (dgan_vjp: its power-of-two cotangent scales, so the division is exact)
+// out[r][c] = s * (sum of the n_parts partial sums of in[r][c], fixed order) for rows of row_len values, read at the
+// row stride in_ld (the padded latent width); with row_scale, row r is also divided by row_scale[r] (dgan_vjp: its
+// power-of-two cotangent scales, so the division is exact)
 __global__ void scale_copy_kernel(const float* __restrict__ in, int n_parts, size_t part_stride,
                                   float* __restrict__ out, float s, size_t n,
-                                  const float* __restrict__ row_scale, int row_len) {
+                                  const float* __restrict__ row_scale, int row_len, int in_ld) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  float g = in[i];
-  for (int p = 1; p < n_parts; ++p) g += in[i + (size_t)p * part_stride];
+  const size_t r = i / row_len, j = r * in_ld + i % row_len;
+  float g = in[j];
+  for (int p = 1; p < n_parts; ++p) g += in[j + (size_t)p * part_stride];
   float m = s;
-  if (row_scale != nullptr) m /= row_scale[i / row_len];
+  if (row_scale != nullptr) m /= row_scale[r];
   out[i] = g * m;
+}
+
+// The width rule on a weight tensor: dst [A_p][B_p][C_p] = src [A][B][C] where every index is in range, 0 elsewhere.
+__global__ void pad_copy_kernel(const float* __restrict__ src, float* __restrict__ dst, int A, int B, int C, int Ap, int Bp,
+                                int Cp) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)Ap * Bp * Cp) return;
+  const int c = (int)(i % Cp), b = (int)((i / Cp) % Bp), a = (int)(i / ((size_t)Cp * Bp));
+  dst[i] = (a < A && b < B && c < C) ? src[((size_t)a * B + b) * C + c] : 0.f;
 }
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -312,7 +406,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base) {
     return p;
   };
   const size_t np = (size_t)w.n_pad;
-  const int latent = c->desc.latent_dim;
+  const int latent = c->wd.latent;                 // z, v, g and z_h are stored at the padded latent width
   w.z = (float*)take(np * latent * 4);
   w.v = (float*)take(np * latent * 4);
   const bool tc = c->desc.precision == DGAN_PREC_FP16;
@@ -434,8 +528,8 @@ static int launch_final_bwd(dgan_ctx* c, const Workspace& w, const TOUT* mask_sr
   return 0;
 }
 
-// What layer-direction i of the fp16 path (tc_dirs order) reads and writes in workspace w.  mask: the 1-bit ReLU masks
-// of the activation it writes (forward) or whose gradient it writes (backward); bias: its epilogue's.
+// What logical layer-direction i of the fp16 path (TcDir::ld) reads and writes in workspace w, at full width.  mask: the
+// 1-bit ReLU masks of the activation it writes (forward) or whose gradient it writes (backward); bias: its epilogue's.
 struct TcIo { const void* in; void* out; unsigned long long* mask; const float* bias; };
 static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i) {
   const int nl = (int)c->layers.size(), l = i / 2;
@@ -455,25 +549,48 @@ static int build_maps(dgan_ctx* c, Workspace& w) {
   int rc;
   for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
     const TcDir& t = c->tc_dirs[i];
-    const TcIo io = tc_io(c, w, (int)i);
+    const TcIo io = tc_io(c, w, t.ld);
     if ((rc = tc_make_map(c->tc, &w.map_in[i], io.in, (uint64_t)t.K, (uint64_t)w.n_pad, (uint64_t)t.P_in, 128, tc2_box_k(t.K))))
       return rc;
     w.map_out[i] = w.map_in[i];      // a placeholder where the epilogue does not store through TMA
+    // the full-width output: a column block stores at its channel offset (TcFinalArgs::col0)
     if (tc2_tma_epilogue(t.N, t.epi, t.out_bytes) &&
-        (rc = tc_make_map(c->tc, &w.map_out[i], io.out, (uint64_t)t.N, (uint64_t)w.n_pad, (uint64_t)t.P_out, TC2_STORE_ROWS)))
+        (rc = tc_make_map(c->tc, &w.map_out[i], io.out, (uint64_t)t.out_ld, (uint64_t)w.n_pad, (uint64_t)t.P_out, TC2_STORE_ROWS)))
       return rc;
   }
   return 0;
 }
 
-// Layer-direction i of the fp16 path on workspace w, with the epilogue, output type and masks its table entry implies.
-// want_mask: a forward with the ReLU also stores its masks.  fa: the last layer's and the momentum tail's arguments.
-static int tc_launch(dgan_ctx* c, const Workspace& w, int i, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{}) {
-  const TcDir& t = c->tc_dirs[(size_t)i];
-  const TcIo io = tc_io(c, w, i);
-  if (t.epi == EPI_BIAS_RELU && want_mask) fa.mb_out = io.mask;
-  if (t.epi == EPI_MASK) fa.mb_in = io.mask;
-  return tc2_launch(&c->launches, t, w.map_in[(size_t)i], w.map_out[(size_t)i], io.out, w.n_pad, io.bias, s, fa);
+// Logical layer-direction ld of the fp16 path on workspace w: every column block of it, with the epilogue, output type
+// and masks its table entries imply.  want_mask: a forward with the ReLU also stores its masks.  fa: the last layer's and
+// the momentum tail's arguments.  Each block of a split layer-direction is profiled as its own kind (its tc_dirs index);
+// an unsplit one is profiled by the caller, together with the BatchNorm kernels that follow it.
+static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{}) {
+  const TcIo io = tc_io(c, w, ld);
+  for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
+    const TcDir& t = c->tc_dirs[i];
+    if (t.ld != ld) continue;
+    ProfScope ps(c, t.N == t.out_ld ? -1 : (int)i, s);
+    TcFinalArgs f = fa;
+    const size_t words = (size_t)t.col0 / 64;          // mask words before the block's channels
+    if (t.epi == EPI_BIAS_RELU && want_mask) f.mb_out = io.mask + words;
+    if (t.epi == EPI_MASK) f.mb_in = io.mask + words;
+    f.out_ld = t.out_ld;
+    f.col0 = t.col0;
+    void* out = t.out_bytes == 4 ? (void*)((float*)io.out + t.col0) : (void*)((__half*)io.out + t.col0);
+    const float* bias = io.bias != nullptr ? io.bias + t.col0 : nullptr;
+    if (int rc = tc2_launch(&c->launches, t, w.map_in[i], w.map_out[i], out, w.n_pad, bias, s, f)) return rc;
+  }
+  return 0;
+}
+
+// The profile kind of logical layer-direction ld when it is one launch (-1 when it is split into column blocks: those
+// are profiled by tc_launch).  fp16 kinds are the tc_dirs entries, fp32 kinds the logical layer-directions.
+static int prof_kind(const dgan_ctx* c, int ld) {
+  if (c->desc.precision != DGAN_PREC_FP16) return ld;
+  for (size_t i = 0; i < c->tc_dirs.size(); ++i)
+    if (c->tc_dirs[i].ld == ld) return c->tc_dirs[i].N == c->tc_dirs[i].out_ld ? (int)i : -1;
+  return -1;
 }
 
 // ---- batch-statistics BatchNorm of layer l on either path's activations (tflib/ops/batchnorm.py:80-93) ----
@@ -522,12 +639,12 @@ static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, i
   const int nl = (int)c->layers.size();
   if (c->desc.precision == DGAN_PREC_FP16) {
     for (int l = 0; l < nl; ++l) {
-      ProfScope ps(c, 2 * l, s);
+      ProfScope ps(c, prof_kind(c, 2 * l), s);
       if ((rc = tc_launch(c, w, 2 * l, s, want_grad))) return rc;
       // with BatchNorm the GEMM wrote pre = GEMM + bias (fp32):  act = relu(BN_batchstat(pre)) (fp16)
       if (c->layers[l].bn_scale != nullptr && (rc = bn_forward_t<float, __half>(c, w, l, w.pre_h[l], w.act_h[l], s))) return rc;
     }
-    ProfScope ps(c, 2 * nl, s);
+    ProfScope ps(c, prof_kind(c, 2 * nl), s);
     TcFinalArgs fa{};
     fa.x = x; fa.y = w.y; fa.loss_part = w.loss_part; fa.R = R; fa.B = B; fa.n_rows = w.n_rows;
     fa.nbx = c->fin.w_in / 2; fa.w_out = 2 * c->fin.w_in; fa.gscale = c->tc.grad_scale; fa.write_y = want_y ? 1 : 0;
@@ -564,18 +681,18 @@ static int run_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s, Momentu
   if (c->desc.precision == DGAN_PREC_FP16) {
     // with BatchNorm after layer j the GEMM writes d(act_j) unmasked and the BN backward turns it into d(pre_j) in place
     for (int l = nl; l >= 1; --l) {       // l = nl: the last layer
-      ProfScope ps(c, 2 * l + 1, s);
+      ProfScope ps(c, prof_kind(c, 2 * l + 1), s);
       if ((rc = tc_launch(c, w, 2 * l + 1, s))) return rc;
       const int j = l - 1;
       if (c->layers[j].bn_scale != nullptr &&
           (rc = bn_backward_t<float, __half>(c, w, j, w.pre_h[j], w.act_h[j], w.dact_h[j], s)))
         return rc;
     }
-    ProfScope ps(c, 1, s);
+    ProfScope ps(c, prof_kind(c, 1), s);
     TcFinalArgs fa{};
     if (mom.tail) {      // the CTA that completes a row tile's partial sums applies the momentum update
       fa.mz = w.z; fa.mv = w.v; fa.mz_h = w.z_h; fa.m_gmul = grad_multiplier(c); fa.m_lr = mom.lr; fa.m_mu = mom.mu;
-      fa.m_counter = w.mom_counter; fa.m_nparts = w.n_g_parts; fa.m_count = (size_t)w.n_pad * c->desc.latent_dim;
+      fa.m_counter = w.mom_counter; fa.m_nparts = w.n_g_parts; fa.m_count = (size_t)w.n_pad * c->wd.latent;
     }
     return tc_launch(c, w, 1, s, false, fa);
   }
@@ -603,16 +720,17 @@ static int run_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s, Momentu
                            L0.C_in, nullptr, 0, nullptr, s);
 }
 
+// z (at the padded latent width) from the caller's z0 [n_rows][latent_dim] or the Philox stream, v = 0
 static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t seed, cudaStream_t s, size_t row_offset = 0) {
-  const int latent = c->desc.latent_dim;
-  const size_t total4 = (size_t)w.n_pad * latent / 4;
+  const int latent = c->desc.latent_dim, ld = c->wd.latent;
+  const size_t total = (size_t)w.n_pad * ld;
   if (w.mom_counter != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.mom_counter, 0, (size_t)w.n_pad / kRowTile * sizeof(unsigned), s));
   // fp32 path: the last layer's forward writes dL/dpre for the real rows only while its backward walks all n_pad rows;
   // the tile-padding rows are never observed, but they must not be read uninitialised
   if (w.dblk == nullptr && w.n_pad > w.n_rows)
     DGAN_CUDA_CHECK(cudaMemsetAsync(w.dpre + (size_t)w.n_rows * c->hwc, 0, (size_t)(w.n_pad - w.n_rows) * c->hwc * sizeof(float), s));
-  init_z_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, s>>>(w.z, w.v, w.z_h, z0, w.n_rows, w.n_pad, latent, seed,
-                                                                 sqrtf(1.0f / (float)latent), row_offset * latent);
+  init_z_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w.z, w.v, w.z_h, z0, w.n_rows, w.n_pad, latent, ld, seed,
+                                                                sqrtf(1.0f / (float)latent), row_offset * latent);
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
@@ -677,16 +795,21 @@ static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspac
   return build_maps(c, *out);
 }
 
-// element counts of the weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights)
-static std::vector<size_t> weight_counts(const dgan_desc* d) {
-  const size_t nd = (size_t)d->net_dim, latent = (size_t)d->latent_dim, feat = 16 * 4 * nd;
-  std::vector<size_t> n = {latent * feat, feat};
-  if (d->use_bn) { n.push_back(feat); n.push_back(feat); }
-  std::vector<std::pair<size_t, size_t>> dc = {{4 * nd, 2 * nd}, {2 * nd, nd}};
-  if (d->arch == DGAN_ARCH_CELEBA) { dc.push_back({nd, nd}); dc.push_back({nd, 3}); } else dc.push_back({nd, 1});
+// The weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights) as 3-D arrays: the caller's shape
+// [a][b][c] at the real widths and the handle's [ap][bp][cp] at the padded ones.
+struct WeightShape { int a, b, c, ap, bp, cp; };
+static std::vector<WeightShape> weight_shapes(const dgan_desc* d, const Widths& p) {
+  const Widths r = real_widths(d);
+  std::vector<WeightShape> n = {{r.latent, 16, r.c4, p.latent, 16, p.c4}, {1, 16, r.c4, 1, 16, p.c4}};   // W [latent][pixel][c]
+  if (d->use_bn) { n.push_back(n.back()); n.push_back(n.back()); }
+  const int c_img = d->arch == DGAN_ARCH_CELEBA ? 3 : 1;
+  std::vector<std::pair<int, int>> dc = {{r.c4, r.c2}, {r.c2, r.c1}}, dp = {{p.c4, p.c2}, {p.c2, p.c1}};   // (C_in, C_out)
+  if (d->arch == DGAN_ARCH_CELEBA) { dc.push_back({r.c1, r.c1}); dp.push_back({p.c1, p.c1}); }
+  dc.push_back({r.c1, c_img}); dp.push_back({p.c1, c_img});
   for (size_t i = 0; i < dc.size(); ++i) {
-    n.push_back(25 * dc[i].first * dc[i].second); n.push_back(dc[i].second);
-    if (d->use_bn && i < 2) { n.push_back(dc[i].second); n.push_back(dc[i].second); }
+    n.push_back({kTaps, dc[i].second, dc[i].first, kTaps, dp[i].second, dp[i].first});   // filters (5,5,C_out,C_in)
+    n.push_back({1, 1, dc[i].second, 1, 1, dp[i].second});
+    if (d->use_bn && i < 2) { n.push_back(n.back()); n.push_back(n.back()); }
   }
   return n;
 }
@@ -716,39 +839,50 @@ int dgan_num_weights(const dgan_desc* d) {
 static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weights_in, cudaStream_t s) {
   c->desc = *d;
   const bool celeba = d->arch == DGAN_ARCH_CELEBA;
-  const int nd = d->net_dim, latent = d->latent_dim;
+  int rc = 0;
+  if ((rc = padded_widths(d, &c->wd))) return rc;
+  const Widths real = real_widths(d);
+  const int latent = c->wd.latent;
   c->H = celeba ? 64 : 28; c->W = c->H; c->C = celeba ? 3 : 1;
   c->hwc = c->H * c->W * c->C;
-  int rc = 0;
   auto fail = [](int code) { return code; };   // the caller destroys the half-built handle
-  // The handle owns copies of every weight tensor: the caller may free or reuse `weights_dev` as soon as the
-  // copies enqueued here have run (i.e. after synchronising `stream`).
+  // The handle owns copies of every weight tensor, at the padded widths: the caller may free or reuse `weights_dev` as
+  // soon as the copies enqueued here have run (i.e. after synchronising `stream`).
   std::vector<const float*> wown;
   {
-    const std::vector<size_t> counts = weight_counts(d);
+    const std::vector<WeightShape> shapes = weight_shapes(d, c->wd);
     size_t total = 0;
-    for (size_t n : counts) total += align_up(n * sizeof(float), 256);
+    for (const WeightShape& w : shapes) total += align_up((size_t)w.ap * w.bp * w.cp * sizeof(float), 256);
     char* base = nullptr;
     if ((rc = dev_alloc(c, (void**)&base, total))) return fail(rc);
     size_t off = 0;
-    for (size_t i = 0; i < counts.size(); ++i) {
-      cudaError_t e = cudaMemcpyAsync(base + off, weights_in[i], counts[i] * sizeof(float), cudaMemcpyDeviceToDevice, s);
-      if (e != cudaSuccess) { set_error(std::string("weight copy: ") + cudaGetErrorString(e)); return fail(DGAN_ERR_CUDA); }
-      wown.push_back((const float*)(base + off));
-      off += align_up(counts[i] * sizeof(float), 256);
+    for (size_t i = 0; i < shapes.size(); ++i) {
+      const WeightShape& w = shapes[i];
+      const size_t n = (size_t)w.ap * w.bp * w.cp;
+      float* dst = (float*)(base + off);
+      if (w.a == w.ap && w.b == w.bp && w.c == w.cp) {
+        cudaError_t e = cudaMemcpyAsync(dst, weights_in[i], n * sizeof(float), cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) { set_error(std::string("weight copy: ") + cudaGetErrorString(e)); return fail(DGAN_ERR_CUDA); }
+      } else {
+        pad_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(weights_in[i], dst, w.a, w.b, w.c, w.ap, w.bp, w.cp);
+        DGAN_CUDA_CHECK(cudaGetLastError());
+      }
+      wown.push_back(dst);
+      off += align_up(n * sizeof(float), 256);
     }
   }
   const float* const* weights = wown.data();
 
-  // ---- Linear (Generator.Input): [1][N][latent] -> [16][N][4*nd]
+  // ---- Linear (Generator.Input): [1][N][latent] -> [16][N][c4]
   {
     GemmLayer L{};
-    L.P_in = 1; L.C_in = latent; L.P_out = 16; L.C_out = 4 * nd;
+    L.P_in = 1; L.C_in = latent; L.P_out = 16; L.C_out = c->wd.c4;
     L.relu = true;
     L.fwd_host = linear_fwd_pairs(16); L.bwd_host = linear_bwd_pairs(16);
-    const float* W = weights[0];             // (latent, 16*4nd), column f = pixel*4nd + c
+    L.macs = (int64_t)16 * real.latent * real.c4;
+    const float* W = weights[0];             // (latent, 16*c4), column f = pixel*c4 + c
     L.wf = W; L.wf_tile_stride = L.C_out; L.wf_ld = 16 * L.C_out;
-    float* Wt = nullptr;                     // [16*4nd][latent]: backward tile q rows = c, cols = latent
+    float* Wt = nullptr;                     // [16*c4][latent]: backward tile q rows = c, cols = latent
     if ((rc = dev_alloc(c, (void**)&Wt, (size_t)latent * 16 * L.C_out * 4))) return fail(rc);
     const size_t total = (size_t)latent * 16 * L.C_out;
     transpose_tiles_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, Wt, latent, 16 * L.C_out, total);
@@ -758,7 +892,7 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
     c->layers.push_back(L);
   }
   // ---- hidden deconvs
-  const std::vector<DeconvSpec> specs = deconv_specs(d);
+  const std::vector<DeconvSpec> specs = deconv_specs(d, c->wd), real_specs = deconv_specs(d, real);
   int wi = d->use_bn ? 4 : 2;
   int di = 0;
   for (const DeconvSpec& sp : specs) {
@@ -767,6 +901,7 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
     L.relu = sp.relu;
     L.fwd_host = deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster);
     L.bwd_host = deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster);
+    L.macs = (int64_t)L.fwd_host.pairs.size() * real_specs[(size_t)di].c_in * real_specs[(size_t)di].c_out;
     const float* F = weights[wi];            // (5,5,C_out,C_in)
     float* Ff = nullptr;                     // [25][C_in][C_out]
     const size_t total = (size_t)kTaps * sp.c_out * sp.c_in;
@@ -786,30 +921,33 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
   // ---- final layer
   {
     FinalLayer& f = c->fin;
-    f.h_in = f.w_in = specs.back().h_used; f.C_in = nd; f.C_out = c->C; f.act = celeba ? ACT_TANH : ACT_SIGMOID;
+    f.h_in = f.w_in = specs.back().h_used; f.C_in = c->wd.c1; f.C_out = c->C; f.act = celeba ? ACT_TANH : ACT_SIGMOID;
     f.w = weights[wi]; f.bias = weights[wi + 1];
     f.n_bands = (2 * f.h_in + kBandRows - 1) / kBandRows;
     f.n_blocks = (f.h_in / 2) * (f.w_in / 2);
-    f.fwd_smem = ((size_t)kTaps * f.C_out * f.C_in + (size_t)(kBandRows / 2 + 2) * f.w_in * (f.C_in + 4)) * 4;
+    f.fwd_smem = final_fwd_smem(f.C_in, f.C_out, f.w_in);     // <= kFinalSmemMax: padded_widths refuses more
     f.bwd_smem = (size_t)kTaps * f.C_out * f.C_in * 4;
   }
-  // exact in-bounds MACs per latent row (SURVEY 8d / Appendix B)
+  // exact in-bounds MACs per latent row at the real widths (SURVEY 8d / Appendix B)
   c->macs_per_row = 0;
-  for (const GemmLayer& L : c->layers) c->macs_per_row += (int64_t)L.fwd_host.pairs.size() * L.C_in * L.C_out;
+  for (const GemmLayer& L : c->layers) c->macs_per_row += L.macs;
   {
     PairTable ft = deconv_fwd_pairs(c->fin.h_in, c->fin.w_in, 2 * c->fin.h_in, 2 * c->fin.w_in);
-    c->macs_per_row += (int64_t)ft.pairs.size() * c->fin.C_in * c->fin.C_out;
+    c->macs_per_row += (int64_t)ft.pairs.size() * real.c1 * c->fin.C_out;
   }
   for (GemmLayer& L : c->layers) {
     if ((rc = upload_table(c, L.fwd_host, &L.fwd, s))) return fail(rc);
     if ((rc = upload_table(c, L.bwd_host, &L.bwd, s))) return fail(rc);
   }
-  // opt in to > 48 KB dynamic shared memory where needed
+  // opt in to > 48 KB dynamic shared memory where needed: the fp32 last layer's footprint grows with net_dim, up to what
+  // an H100 block can have (padded_widths refuses wider generators)
 #define OPTIN(K, BYTES) DGAN_CUDA_CHECK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(BYTES)))
-  OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID>), 100 * 1024);
-  OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH>), 100 * 1024);
+  OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID>), kFinalSmemMax);
+  OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<__half, 1, ACT_SIGMOID>), 100 * 1024);
   OPTIN((final_fwd_loss_kernel<__half, 3, ACT_TANH>), 100 * 1024);
+  OPTIN((final_bwd_kernel<float, 1>), kFinalSmemMax);
+  OPTIN((final_bwd_kernel<float, 3>), kFinalSmemMax);
 #undef OPTIN
   if (d->precision == DGAN_PREC_FP16) {
     if ((rc = tc_init(c->tc))) return fail(rc);
@@ -818,40 +956,51 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
     const int nl = (int)c->layers.size();
     for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
       TcDir& t = c->tc_dirs[i];
-      if (t.N != 16 && t.N != 48 && t.N != 64 && t.N != 128 && t.N != 256) { set_error("tensor-core path needs 64/128/256 output channels per pixel"); return fail(DGAN_ERR_UNSUPPORTED); }
-      // K < 64: the narrow operand of the last layer's backward (16 * C_out channels, k16 sub-tiles)
-      if (t.K % 64 != 0 && !(t.K == 16 || t.K == 48)) { set_error("tensor-core path needs input channels in multiples of 64, or 16 / 48"); return fail(DGAN_ERR_UNSUPPORTED); }
-      if (t.n_tiles > 32 || t.P_in > 65535 || t.P_out > 65535) { set_error("tensor-core schedule limits exceeded"); return fail(DGAN_ERR_UNSUPPORTED); }
+      if ((rc = tc_dir_supported(t))) return fail(rc);
       // fp16 K-major weight tiles [n_tiles][N rows][K cols]
       const size_t tile = (size_t)t.N * t.K;
       if ((rc = dev_alloc(c, (void**)&t.w, (size_t)t.n_tiles * tile * 2))) return fail(rc);
-      if ((int)i < 2 * nl) {     // a GEMM layer: its tiles, then the all-zero tile of tc_with_zero_tile()
-        const GemmLayer& L = c->layers[i / 2];
+      if (t.ld < 2 * nl) {       // a GEMM layer: its tiles (rows col0 .. col0 + N), then the all-zero tile of tc_with_zero_tile()
+        const GemmLayer& L = c->layers[(size_t)(t.ld / 2)];
         const size_t elems = (size_t)(t.n_tiles - 1) * tile;
         const unsigned blocks = (unsigned)((elems + 255) / 256);
         DGAN_CUDA_CHECK(cudaMemsetAsync(t.w + elems, 0, tile * 2, s));
-        if (i % 2 == 0) tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wb, t.w, elems);        // F[t][co][ci]; Linear: Wt[q*C + c][k]
-        else if (i == 1) tc_linear_bwd_tiles_kernel<<<blocks, 256, 0, s>>>(weights[0], t.w, latent, L.C_out, L.P_out);   // W[k][q*C + c]
-        else tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wf, t.w, elems);                   // Ff[t][ci][co]
+        if (t.ld % 2 == 0)         // F[t][co][ci]; Linear: Wt[q*C + c][k]
+          tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wb, t.w, elems, L.C_out, t.col0, t.N, t.K);
+        else if (t.ld == 1)        // W[k][q*C + c]
+          tc_linear_bwd_tiles_kernel<<<blocks, 256, 0, s>>>(weights[0], t.w, latent, L.C_out, L.P_out);
+        else                       // Ff[t][ci][co]
+          tc_convert_kernel<<<blocks, 256, 0, s>>>(L.wf, t.w, elems, L.C_in, t.col0, t.N, t.K);
         DGAN_CUDA_CHECK(cudaGetLastError());
       }
       if ((rc = tc_make_map(c->tc, &t.tm_b, t.w, (uint64_t)t.K, (uint64_t)t.N, (uint64_t)t.n_tiles, (uint32_t)(t.N / 2), tc2_box_k(t.K))))
         return fail(rc);
     }
-    if (nd != 64) { set_error("tensor-core final layer needs net_dim == 64"); return fail(DGAN_ERR_UNSUPPORTED); }
-    tc_final_tiles_kernel<<<16, 256, 0, s>>>(c->fin.w, c->fin.C_out, c->fin.C_in, c->tc_dirs[2 * nl].w, c->tc_dirs[2 * nl + 1].w);
+    // the last layer's two directions (never split: N <= 128) are the table's last two entries
+    const size_t nd = c->tc_dirs.size();
+    tc_final_tiles_kernel<<<16, 256, 0, s>>>(c->fin.w, c->fin.C_out, c->fin.C_in, c->tc_dirs[nd - 2].w, c->tc_dirs[nd - 1].w);
     DGAN_CUDA_CHECK(cudaGetLastError());
   }
-  // profile kinds: the layer-directions in tc_directions() order (both paths), then the momentum update
-  for (const TcDir& t : tc_directions(d)) c->kind_names.push_back(t.kind);
-  c->kind_names.push_back("momentum");
+  // profile kinds, then the momentum update: fp16, the tc_directions() entries (a column block of a split layer-direction
+  // is a kind of its own, with the share of the MACs that falls on its real channels); fp32, the layer-directions
+  std::vector<double> lmacs;        // per logical layer-direction
   double fmacs = (double)c->macs_per_row;
   for (const GemmLayer& L : c->layers) {
-    const double macs = (double)L.fwd_host.pairs.size() * L.C_in * L.C_out;
-    c->kind_macs_per_row.insert(c->kind_macs_per_row.end(), 2, macs);      // forward, backward
-    fmacs -= macs;
+    lmacs.insert(lmacs.end(), 2, (double)L.macs);      // forward, backward
+    fmacs -= (double)L.macs;
   }
-  c->kind_macs_per_row.insert(c->kind_macs_per_row.end(), 2, fmacs);        // the last layer's forward, backward
+  lmacs.insert(lmacs.end(), 2, fmacs);                 // the last layer's forward, backward
+  for (const TcDir& t : tc_directions(d)) {
+    if (d->precision == DGAN_PREC_FP16) {
+      const int real_in_block = std::max(0, std::min(t.N, t.n_real - t.col0));
+      c->kind_names.push_back(t.kind);
+      c->kind_macs_per_row.push_back(lmacs[(size_t)t.ld] * real_in_block / t.n_real);
+    } else if (t.col0 == 0) {
+      c->kind_names.push_back(t.base_kind);
+      c->kind_macs_per_row.push_back(lmacs[(size_t)t.ld]);
+    }
+  }
+  c->kind_names.push_back("momentum");
   c->kind_macs_per_row.push_back(0.0);
   DGAN_CUDA_CHECK(cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking));
   DGAN_CUDA_CHECK(cudaGetLastError());
@@ -865,8 +1014,8 @@ int dgan_create(dgan_handle* out, const dgan_desc* d, const float* const* weight
   if (d->abi_version != DGAN_ABI_VERSION) { set_error("ABI version mismatch"); return DGAN_ERR_INVALID_ARG; }
   if (d->arch != DGAN_ARCH_MNIST && d->arch != DGAN_ARCH_CELEBA) { set_error("unknown arch"); return DGAN_ERR_INVALID_ARG; }
   if (d->precision != DGAN_PREC_FP32 && d->precision != DGAN_PREC_FP16) { set_error("unknown precision"); return DGAN_ERR_INVALID_ARG; }
-  if (d->net_dim <= 0 || d->net_dim % 64 != 0) { set_error("net_dim must be a positive multiple of 64"); return DGAN_ERR_UNSUPPORTED; }
-  if (d->latent_dim <= 0 || d->latent_dim % 64 != 0) { set_error("latent_dim must be a positive multiple of 64"); return DGAN_ERR_UNSUPPORTED; }
+  Widths wd;
+  if (const int rc = padded_widths(d, &wd)) return rc;
   if (n_weights != dgan_num_weights(d)) { set_error("wrong number of weight tensors"); return DGAN_ERR_INVALID_ARG; }
   for (int i = 0; i < n_weights; ++i)
     if (weights[i] == nullptr) { set_error("NULL weight pointer"); return DGAN_ERR_INVALID_ARG; }
@@ -932,8 +1081,9 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
   if (loss_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(loss_dev, w.loss, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, s));
   if (grad_dev) {
     const size_t n = (size_t)n_rows * h->desc.latent_dim;
-    scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->desc.latent_dim,
-                                                                  grad_dev, grad_multiplier(h), n, nullptr, 1);
+    scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->wd.latent,
+                                                                  grad_dev, grad_multiplier(h), n, nullptr, h->desc.latent_dim,
+                                                                  h->wd.latent);
     DGAN_LAUNCH_CHECK(h);
   }
   return DGAN_OK;
@@ -957,8 +1107,8 @@ int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev,
   if ((rc = run_backward(h, w, s))) return rc;
   const size_t n = (size_t)n_rows * h->desc.latent_dim;
   const bool tc = h->desc.precision == DGAN_PREC_FP16;
-  scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->desc.latent_dim, dz_dev,
-                                                                1.f, n, tc ? w.loss : nullptr, h->desc.latent_dim);
+  scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->wd.latent, dz_dev,
+                                                                1.f, n, tc ? w.loss : nullptr, h->desc.latent_dim, h->wd.latent);
   DGAN_LAUNCH_CHECK(h);
   if (y_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(y_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
   return DGAN_OK;
@@ -967,9 +1117,10 @@ int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev,
 int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_rows, float* z_dev, void* stream) {
   if (h == nullptr || z_dev == nullptr || n_rows <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int latent = h->desc.latent_dim;
-  const size_t total4 = (size_t)n_rows * latent / 4;
-  init_z_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(z_dev, nullptr, nullptr, nullptr, n_rows, n_rows, latent, seed,
-                                                                                      sqrtf(1.0f / (float)latent), (size_t)z_row_offset * latent);
+  const size_t total = (size_t)n_rows * latent;
+  init_z_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(z_dev, nullptr, nullptr, nullptr, n_rows, n_rows, latent,
+                                                                                   latent, seed, sqrtf(1.0f / (float)latent),
+                                                                                   (size_t)z_row_offset * latent);
   DGAN_LAUNCH_CHECK(h);
   return DGAN_OK;
 }
@@ -982,7 +1133,7 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
   const uint64_t seed = prm->seed;
   if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
-  const int latent = h->desc.latent_dim;
+  const int latent = h->wd.latent;
   Workspace w;
   int rc;
   if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w))) return rc;
@@ -1110,8 +1261,10 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
+  Widths wd;
+  if (int rc = padded_widths(d, &wd)) return rc;
   for (const TcDir& dr : tc_directions(d)) {
-    if (dr.N != 16 && dr.N != 48 && dr.N != 64 && dr.N != 128 && dr.N != 256) { set_error(dr.name + ": unsupported N"); return DGAN_ERR_UNSUPPORTED; }
+    if (int rc = tc_dir_supported(dr)) return rc;
     Tc2Plan plan;
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
@@ -1229,6 +1382,8 @@ static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int forc
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
+  Widths wd;
+  if (padded_widths(d, &wd) != 0) return -1;
   std::string out = "direction | N | K | window (h x w, stride) | items | slots | steps | MMAs | staged MB | busiest pair / mean load"
                     " | zero-tile MMA % | MMAs per round | busiest pair: est. tensor us | busiest pair: est. us | k16 MMAs"
                     " | epilogue/output\n";
@@ -1280,6 +1435,17 @@ int dgan_debug_plan_stats_window(const dgan_desc* d, int n_rows, int n_pairs, in
                                  int sy, int sx, char* buf, int buf_len) {
   const int shape[4] = {wh, ww, sy, sx};
   return plan_stats_impl(d, n_rows, n_pairs, force_dir, force_maxb, shape, buf, buf_len);
+}
+
+// Host-only aid (not in the public header): the widths a handle for `d` stores - out[0..4) = latent, 4 * net_dim,
+// 2 * net_dim, net_dim, padded by padded_widths().  Returns 0, or its error code with the limit in dgan_last_error().
+int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
+  using namespace dgan;
+  if (d == nullptr || out == nullptr) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
+  Widths w;
+  if (int rc = padded_widths(d, &w)) return rc;
+  out[0] = w.latent; out[1] = w.c4; out[2] = w.c2; out[3] = w.c1;
+  return 0;
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -305,37 +305,38 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
 
 // z_hat / momentum-slot initialisation = tf.local_variables_initializer() per batch
 // (utils/gan_defense.py:119; models/gan.py:370-377,424-428): z ~ N(0, 1/latent) or z0, v = 0.
-// Rows >= n_rows (tile padding) are zeroed.
+// z is [n_pad][ld] with ld >= latent (the padded latent width); rows >= n_rows (tile padding) and columns >= latent are
+// zeroed.  Element (row, col) of the draw is value e % 4 of Philox block e / 4 with e = elem_offset + row * latent + col,
+// the index of the real [rows][latent] array: the draw does not depend on the padding or on how the batch is chained.
 __global__ void init_z_kernel(float* __restrict__ z, float* __restrict__ v, __half* __restrict__ z_h,
-                              const float* __restrict__ z0, int n_rows, int n_pad, int latent,
+                              const float* __restrict__ z0, int n_rows, int n_pad, int latent, int ld,
                               uint64_t seed, float stddev, size_t elem_offset) {
-  const size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // one thread = 4 consecutive values
-  const size_t total4 = (size_t)n_pad * latent / 4;
-  if (q >= total4) return;
-  const size_t e = q * 4;
-  const int row = (int)(e / latent);
-  float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (row < n_rows) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)n_pad * ld) return;
+  const int row = (int)(i / ld), col = (int)(i % ld);
+  float val = 0.f;
+  if (row < n_rows && col < latent) {
+    const size_t e = (size_t)row * latent + col;
     if (z0 != nullptr) {
-      val = *reinterpret_cast<const float4*>(z0 + e);
+      val = z0[e];
     } else {
-      const size_t gq = q + elem_offset / 4;   // counter = global element index / 4: independent of how the batch is chained
+      const size_t g = e + elem_offset, gq = g / 4;
+      const int lane = (int)(g % 4);
       const uint4 r = philox4x32_10(make_uint4((uint32_t)gq, (uint32_t)(gq >> 32), 0u, 0u),
                                     make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-      const float u0 = ((float)r.x + 0.5f) * 2.3283064365386963e-10f;
-      const float u1 = ((float)r.y + 0.5f) * 2.3283064365386963e-10f;
-      const float u2 = ((float)r.z + 0.5f) * 2.3283064365386963e-10f;
-      const float u3 = ((float)r.w + 0.5f) * 2.3283064365386963e-10f;
-      const float m0 = sqrtf(-2.f * logf(u0)) * stddev, m1 = sqrtf(-2.f * logf(u2)) * stddev;
-      float s0, c0, s1, c1;
-      sincosf(6.283185307179586f * u1, &s0, &c0);
-      sincosf(6.283185307179586f * u3, &s1, &c1);
-      val = make_float4(m0 * c0, m0 * s0, m1 * c1, m1 * s1);
+      // Box-Muller on (u0, u1) -> values 0, 1 and on (u2, u3) -> values 2, 3
+      const uint32_t ra = lane < 2 ? r.x : r.z, rb = lane < 2 ? r.y : r.w;
+      const float ua = ((float)ra + 0.5f) * 2.3283064365386963e-10f;
+      const float ub = ((float)rb + 0.5f) * 2.3283064365386963e-10f;
+      const float m = sqrtf(-2.f * logf(ua)) * stddev;
+      float sn, cs;
+      sincosf(6.283185307179586f * ub, &sn, &cs);
+      val = (lane & 1) ? m * sn : m * cs;
     }
   }
-  *reinterpret_cast<float4*>(z + e) = val;
-  if (v != nullptr) *reinterpret_cast<float4*>(v + e) = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (z_h != nullptr) store4(z_h + e, val);
+  z[i] = val;
+  if (v != nullptr) v[i] = 0.f;
+  if (z_h != nullptr) z_h[i] = __float2half_rn(val);
 }
 
 // loss[n] = (sum of band partials, fixed order) / (H*W*C)            (models/gan.py:411-413)

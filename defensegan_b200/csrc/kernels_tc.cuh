@@ -171,15 +171,23 @@ struct TcFinalArgs {
   unsigned* m_counter;   // [n_pad / 128] arrival tickets, self-resetting; NULL = plain partial sums
   int m_nparts;          // partial sums per row tile
   size_t m_count;        // elements per partial-sum array (n_pad * latent)
+  // A column block of a layer-direction wider than one tile (tc_directions): the output's row stride in channels (its
+  // full width) and the block's first channel.  The TMA store adds col0 to its channel coordinate; the other outputs,
+  // the bias and the ReLU masks are passed already offset to the block.
+  int out_ld, col0;
 };
 
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-// fp32 [tiles][rows][cols] -> fp16, same layout
-__global__ void tc_convert_kernel(const float* __restrict__ in, __half* __restrict__ out, size_t n) {
+// fp32 [tiles][rows_full][cols] -> fp16 [tiles][rows][cols]: rows row0 .. row0 + rows of every tile (a column block of a
+// layer-direction's weight tiles; rows == rows_full: all of them)
+__global__ void tc_convert_kernel(const float* __restrict__ in, __half* __restrict__ out, size_t n, int rows_full, int row0,
+                                  int rows, int cols) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __float2half_rn(in[i]);
+  if (i >= n) return;
+  const size_t per = (size_t)rows * cols, t = i / per, rem = i % per;
+  out[i] = __float2half_rn(in[(t * rows_full + row0) * cols + rem]);
 }
 // Linear backward tiles: out[q][k][c] = W[k][q*C + c]   (W is (latent, 16*C))
 __global__ void tc_linear_bwd_tiles_kernel(const float* __restrict__ W, __half* __restrict__ out, int latent, int C,

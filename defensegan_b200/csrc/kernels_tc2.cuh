@@ -107,7 +107,8 @@ struct Tc2Cfg {
 // tc2_optin_all, the launch dispatch and the planner's candidate set (tc2_plan) all read this list.  For each
 // (N, k16 per op, epilogue, output type) it holds the largest slot count, which every window shape can use, and the
 // smaller ones the planner picks for the shipped generators.  The narrow kinds (k16 per op < 4) are the last layer's
-// backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA).
+// backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA), at N = 64 (net_dim <= 64) and
+// N = 128 (64 < net_dim <= 128).
 #define TC2_KINDS(X)                                                                                                   \
   X(256, 1, 4, EPI_BIAS_RELU, __half) X(256, 1, 4, EPI_BIAS, __half) X(256, 1, 4, EPI_MASK, __half)                    \
   X(256, 1, 4, EPI_NONE, __half) X(256, 1, 4, EPI_NONE, float) X(256, 1, 4, EPI_BIAS, float)                           \
@@ -117,6 +118,7 @@ struct Tc2Cfg {
   X(64, 4, 4, EPI_BIAS_RELU, __half) X(64, 4, 4, EPI_BIAS, __half) X(64, 4, 4, EPI_MASK, __half)                      \
   X(64, 4, 4, EPI_NONE, __half) X(64, 4, 4, EPI_NONE, float) X(64, 4, 4, EPI_BIAS, float)                              \
   X(64, 4, 1, EPI_MASK, __half) X(64, 4, 1, EPI_NONE, __half) X(64, 4, 3, EPI_NONE, __half)                            \
+  X(128, 2, 1, EPI_MASK, __half) X(128, 2, 1, EPI_NONE, __half) X(128, 2, 3, EPI_NONE, __half)                         \
   X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)
 
 struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
@@ -512,6 +514,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       } else if constexpr (TMA_EPI) {
         // 64-column units: registers -> fp16 -> this warp's 16-row slice of a 128B-swizzled tile -> one TMA store
         constexpr int G = N_TILE / 64;                 // 64-column groups per accumulator
+        const int GT = fa.out_ld >> 6;                 // 64-column groups per output row (mask words)
         const int row_w = tile_row0 + wg * 64 + wl * 16;
         const uint32_t s_warp = epi_base + (uint32_t)warp * 4096u;
         const uint32_t swz = (uint32_t)(lane >> 2);
@@ -524,7 +527,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
             unsigned long long mk[2] = {~0ull, ~0ull}, bits[2] = {0ull, 0ull};
             if (EPI == EPI_MASK) {
 #pragma unroll
-              for (int h = 0; h < 2; ++h) mk[h] = __ldg(fa.mb_in + ((size_t)q * n_pad + n_lo + 8 * h) * G + g);
+              for (int h = 0; h < 2; ++h) mk[h] = __ldg(fa.mb_in + ((size_t)q * n_pad + n_lo + 8 * h) * GT + g);
             }
             uint32_t pk[2][8];
 #pragma unroll
@@ -559,7 +562,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
             ptx::fence_proxy_async_smem();
             __syncwarp();
             if (lane == 0) {
-              ptx::tma_store_3d(&tm_out, buf, g * 64, row_w, q);
+              ptx::tma_store_3d(&tm_out, buf, fa.col0 + g * 64, row_w, q);
               ptx::bulk_commit();
             }
             ++store_count;
@@ -569,7 +572,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                 bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
                 bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
               }
-              if ((lane & 3) < 2) fa.mb_out[((size_t)q * n_pad + n_lo + 8 * (lane & 1)) * G + g] = (lane & 1) ? bits[1] : bits[0];
+              if ((lane & 3) < 2) fa.mb_out[((size_t)q * n_pad + n_lo + 8 * (lane & 1)) * GT + g] = (lane & 1) ? bits[1] : bits[0];
             }
           }
         }
@@ -588,7 +591,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
             for (int h = 0; h < 2; ++h) {
               float v0 = acc[a * (N_TILE / 2) + j * 4 + h * 2] + bv.x, v1 = acc[a * (N_TILE / 2) + j * 4 + h * 2 + 1] + bv.y;
               if (EPI == EPI_BIAS_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-              const size_t o = ((size_t)q * n_pad + n_lo + 8 * h) * N_TILE + col;
+              const size_t o = ((size_t)q * n_pad + n_lo + 8 * h) * fa.out_ld + col;
               if (sizeof(TOUT) == 4) *reinterpret_cast<float2*>(reinterpret_cast<float*>(out) + o) = make_float2(v0, v1);
               else *reinterpret_cast<uint32_t*>(reinterpret_cast<__half*>(out) + o) = pack_half2(v0, v1);
             }
@@ -697,6 +700,12 @@ struct TcDir {
   int h_grid = 0, w_grid = 0;  // the output pixels as the grid the planner's windows tile
   int max_acc = 1;             // most accumulators per window
   int epi = EPI_NONE, out_bytes = 2, bias_pstride = 0;
+  // The logical layer-direction (layer l forward = 2l, backward = 2l + 1) this entry computes.  A layer-direction with
+  // more than 256 output channels is split into column blocks of 256: entry i writes channels [col0, col0 + N) of the
+  // one out_ld-wide output tensor that the next layer reads.
+  int ld = 0, col0 = 0, out_ld = 0;
+  int n_real = 0;              // real (unpadded) output channels of the logical layer-direction
+  std::string base_kind;       // profile kind of the logical layer-direction (kind without the block's channel range)
   __half* w = nullptr;         // [n_tiles][N][K] fp16, K contiguous
   CUtensorMap tm_b{};          // box {64 | 16, N/2, 1}: the half of a weight tile (sub-tile) one CTA of the pair loads
   int force_maxb = 0;          // > 0: plan with exactly this many accumulator slots per round (dgan_debug_force_slots)
@@ -1274,7 +1283,6 @@ static int tc2_optin_all() {
 static int tc2_launch(int64_t* launches, const TcDir& d, const CUtensorMap& tm_a, const CUtensorMap& tm_out, void* out,
                       int n_pad, const float* bias, cudaStream_t s, const TcFinalArgs& fa) {
   if (n_pad % (2 * kRowTile) != 0) { set_error("pair kernel needs n_pad % 256 == 0"); return DGAN_ERR_INVALID_ARG; }
-  if (d.bias_pstride != 0 && d.N != 256) { set_error("a per-pixel bias needs one accumulator per item (N = 256)"); return DGAN_ERR_UNSUPPORTED; }
   const int n_mpairs = n_pad / (2 * kRowTile);
   const Tc2Schedule* sc = nullptr;
   for (auto& kv : d.by_mpairs)

@@ -26,7 +26,7 @@
 //            in this round; never a first MMA).
 // Item word (the consumers' epilogue list): window [16,31) | row pair [0,16); -1 = no item.
 //
-// The k-chunk needs no run-time check: dgan_create refuses K > 256, i.e. more than 4 k-chunks.
+// The k-chunk needs no run-time check: tc_dir_supported (dgan_api.cu) refuses K > 512, i.e. more than 8 k-chunks.
 #pragma once
 #include <cstdint>
 

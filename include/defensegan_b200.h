@@ -48,7 +48,14 @@ typedef struct dgan_desc {
   int32_t abi_version; /* DGAN_ABI_VERSION */
   int32_t arch;        /* dgan_arch */
   int32_t latent_dim;  /* LATENT_DIM (experiments/cfgs/gans/default.yml:4) */
-  int32_t net_dim;     /* NET_DIM    (default.yml:7) */
+  int32_t net_dim;     /* NET_DIM    (default.yml:7)
+                        * Accepted widths (others: DGAN_ERR_UNSUPPORTED, the limit named in dgan_last_error):
+                        *   DGAN_PREC_FP32: any latent_dim >= 1; net_dim >= 1 up to what the last layer's shared memory
+                        *                   holds: 704 (MNIST), 256 (CelebA).
+                        *   DGAN_PREC_FP16: 1 <= latent_dim <= 256, 1 <= net_dim <= 128.
+                        * Callers always see the real widths (weights, z, gradients); the handle stores each channel width
+                        * padded with exact zeros (fp32: to a multiple of 64; fp16: to 64, 128, 256 or 512), which leaves
+                        * every result's bits as the unpadded computation would give them. */
   int32_t use_bn;      /* USE_BN     (default.yml:3); batch-statistics BN, tflib/ops/batchnorm.py:80-93 (both precisions; fp16 path: fp32 pre-activations and statistics, fp16 activations) */
   int32_t precision;   /* dgan_precision */
 } dgan_desc;
@@ -130,7 +137,9 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev,
              void* workspace, size_t workspace_bytes, void* stream);
 
-/* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack). */
+/* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack
+ * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
+ * 256 channels, 1 + 10 L - 5 + 2). */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA

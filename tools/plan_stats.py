@@ -1,5 +1,8 @@
 """Developer aid (no GPU needed): print the planner's numbers for every tensor-core layer-direction.
 Usage: python tools/plan_stats.py [mnist|celeba] [batch] [R] [CTA pairs] [library] [--slots DIR=MAXB] [--window DIR=WH,WW,SY,SX]
+                                 [--latent_dim N] [--net_dim N] [--use_bn]
+--latent_dim / --net_dim / --use_bn plan that generator (default 128 / 64 / no BN); the handle pads each width (see
+DESIGN.md section 2), and the last column shows the share of each direction's k16 MMAs that multiply real channels;
 --slots plans layer-direction DIR (the row index of the table, from 0) with exactly MAXB accumulator slots per round;
 --window plans it on exactly the window WH x WW with strides (SY, SX), e.g. to compare two builds at the same window."""
 import ctypes
@@ -14,6 +17,15 @@ if "--slots" in sys.argv:
     i = sys.argv.index("--slots")
     force_dir, force_maxb = (int(v) for v in sys.argv[i + 1].split("="))
     del sys.argv[i:i + 2]
+widths = {"--latent_dim": 128, "--net_dim": 64}
+for flag in widths:
+    if flag in sys.argv:
+        i = sys.argv.index(flag)
+        widths[flag] = int(sys.argv[i + 1])
+        del sys.argv[i:i + 2]
+use_bn = "--use_bn" in sys.argv
+if use_bn:
+    sys.argv.remove("--use_bn")
 window = None
 if "--window" in sys.argv:
     i = sys.argv.index("--window")
@@ -25,7 +37,8 @@ batch = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 R = int(sys.argv[3]) if len(sys.argv) > 3 else 10
 pairs = int(sys.argv[4]) if len(sys.argv) > 4 else 74
 lib = ctypes.CDLL(sys.argv[5]) if len(sys.argv) > 5 else ctypes.CDLL(_native.build_library())
-desc = _native.dgan_desc(_native.ABI_VERSION, _native.ARCH_IDS[dataset], 128, 64, 0, _native.PRECISIONS["fp16"])
+latent, nd = widths["--latent_dim"], widths["--net_dim"]
+desc = _native.dgan_desc(_native.ABI_VERSION, _native.ARCH_IDS[dataset], latent, nd, int(use_bn), _native.PRECISIONS["fp16"])
 buf = ctypes.create_string_buffer(1 << 16)
 lib.dgan_debug_plan_stats_slots.restype = ctypes.c_int
 lib.dgan_debug_plan_stats_slots.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
@@ -35,5 +48,24 @@ if window is None:
 else:
     lib.dgan_debug_plan_stats_window.restype = ctypes.c_int
     n = lib.dgan_debug_plan_stats_window(ctypes.byref(desc), batch * R, pairs, force_dir, force_maxb, *window, buf, len(buf))
-assert n > 0
-print(buf.value.decode())
+if n <= 0:
+    lib.dgan_last_error.restype = ctypes.c_char_p
+    raise SystemExit((lib.dgan_last_error() or b"planning failed").decode())
+# real (unpadded) N and K of each layer-direction; a column block "name[a:b]" has the real channels of [a, b)
+img = 48 if dataset == "celeba" else 16
+real = {"Linear.fwd": (4 * nd, latent), "Linear.bwd": (latent, 4 * nd), "Generator.2.fwd": (2 * nd, 4 * nd),
+        "Generator.2.bwd": (4 * nd, 2 * nd), "Generator.3.fwd": (nd, 2 * nd), "Generator.3.bwd": (2 * nd, nd),
+        "Generator.5.fwd": (nd, nd), "Generator.5.bwd": (nd, nd), "last.fwd": (img, nd), "last.bwd": (nd, img)}
+lines = buf.value.decode().strip().splitlines()
+out = [lines[0] + " | real k16 MMAs (share)"]
+for line in lines[1:-1]:
+    col = line.split(" | ")
+    name, n, k = col[0], int(col[1]), int(col[2])
+    rn, rk = real[name.split("[")[0]]
+    if "[" in name:
+        a, b = (int(v) for v in name[name.index("[") + 1:-1].split(":"))
+        rn = max(0, min(b, rn) - a)
+    share = min(rn, n) * min(rk, k) / (n * k)
+    out.append(line + " | %d (%.2f)" % (round(int(col[14]) * share), share))
+out.append(lines[-1])
+print("\n".join(out))
