@@ -12,6 +12,7 @@ import sys
 from typing import Dict, List, Optional, Sequence
 
 import torch
+import torch.autograd.forward_ad as fwAD
 from torch.autograd.function import once_differentiable
 
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
@@ -31,7 +32,7 @@ NVCC_FLAGS = [
 # Every symbol include/defensegan_b200.h declares.
 ABI_SYMBOLS = [
     "dgan_abi_version", "dgan_last_error", "dgan_num_weights", "dgan_create", "dgan_destroy",
-    "dgan_workspace_bytes", "dgan_reconstruct", "dgan_sample_z0", "dgan_forward", "dgan_loss_grad", "dgan_vjp",
+    "dgan_workspace_bytes", "dgan_reconstruct", "dgan_sample_z0", "dgan_forward", "dgan_loss_grad", "dgan_vjp", "dgan_jvp",
     "dgan_last_launch_count", "dgan_last_enqueue_count", "dgan_macs_per_row", "dgan_profile_enable", "dgan_profile_num_kinds",
     "dgan_profile_kind_name", "dgan_profile_read",
 ]
@@ -131,6 +132,8 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_loss_grad.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_vjp.restype = i32
     lib.dgan_vjp.argtypes = [vp, vp, i32, vp, vp, vp, vp, sz, vp]
+    lib.dgan_jvp.restype = i32
+    lib.dgan_jvp.argtypes = [vp, vp, i32, vp, vp, vp, vp, sz, vp]
     lib.dgan_last_launch_count.restype = ctypes.c_int64
     lib.dgan_last_launch_count.argtypes = [vp]
     lib.dgan_last_enqueue_count.restype = ctypes.c_int64
@@ -183,6 +186,7 @@ class NativeGenerator:
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.arch, self.precision = arch, precision
         self.latent_dim, self.net_dim = int(latent_dim), int(net_dim)
+        self.use_bn = bool(use_bn)
         self.image_dim = (64, 64, 3) if ARCH_IDS[arch] == 1 else (28, 28, 1)
         self.hwc = self.image_dim[0] * self.image_dim[1] * self.image_dim[2]
         self._handle = ctypes.c_void_p(0)
@@ -350,17 +354,65 @@ class NativeGenerator:
                                                ctypes.c_void_p(stream)), "dgan_vjp")
         return (y, dz) if want_y else dz
 
+    def jvp(self, z: torch.Tensor, t: torch.Tensor, want_y: bool = False):
+        """Jacobian-vector product of the generator at z: ty = (dG/dz) t for a tangent t shaped like z ([N, latent_dim]),
+        returned as [N,H,W,C].  The forward is recomputed; with want_y it is returned too, as (y, ty), bit-identical to
+        forward(z).  With use_bn the batch statistics of the N rows are differentiated."""
+        zc = _require_cuda_f32(z, "z")
+        tc = _require_cuda_f32(t, "t")
+        n = zc.shape[0]
+        if zc.numel() != n * self.latent_dim:
+            raise ValueError("z must be [N, %d]" % self.latent_dim)
+        if tc.numel() != n * self.latent_dim or tc.shape[0] != n:
+            raise ValueError("t must be [N, %d] with the rows of z" % self.latent_dim)
+        with torch.cuda.device(self.device):
+            y = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device) if want_y else None
+            ty = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
+            ws, need = self._workspace(n, 1)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _check(self.lib, self.lib.dgan_jvp(self._handle, _ptr(zc), n, _ptr(tc), _ptr(y), _ptr(ty), ws, need,
+                                               ctypes.c_void_p(stream)), "dgan_jvp")
+        return (y, ty) if want_y else ty
+
+    def jacobian(self, z: torch.Tensor, max_rows: int = 4096) -> torch.Tensor:
+        """dG/dz at each row of z ([N, latent_dim]) as [N, H, W, C, latent_dim]: column k of image i is jvp(z_i, e_k).
+        Runs jvp on each row repeated latent_dim times with identity tangents, whole images per call and at most
+        max_rows (at least one image) rows per call; rows are independent, so the chunking does not change a bit.
+        Refused with use_bn: the batch statistics couple the rows, so G has no per-row Jacobian."""
+        if self.use_bn:
+            raise ValueError("generator_jacobian is undefined with BatchNorm (use_bn): its batch statistics couple the "
+                             "rows, so the Jacobian of one row depends on the others")
+        zc = _require_cuda_f32(z, "z")
+        n, k = zc.shape[0], self.latent_dim
+        if zc.numel() != n * k:
+            raise ValueError("z must be [N, %d]" % k)
+        per_call = max(1, int(max_rows) // k)
+        eye = torch.eye(k, dtype=torch.float32, device=zc.device)
+        out = torch.empty((n, k) + self.image_dim, dtype=torch.float32, device=zc.device)
+        for i in range(0, n, per_call):
+            m = min(per_call, n - i)
+            rows = zc.view(n, k)[i:i + m].repeat_interleave(k, dim=0)
+            out[i:i + m] = self.jvp(rows, eye.repeat(m, 1)).view((m, k) + self.image_dim)
+        return out.movedim(1, -1).contiguous()
+
 
 class GeneratorFunction(torch.autograd.Function):
-    """y = G(z) through a NativeGenerator (or anything with its forward / vjp methods), differentiable in z.  The
-    backward recomputes the forward inside `native.vjp` on the current stream; the weights are frozen (no gradient),
-    as in the projection.  Only first derivatives are available."""
+    """y = G(z) through a NativeGenerator (or anything with its forward / vjp / jvp methods), differentiable in z in
+    both modes.  The backward recomputes the forward inside `native.vjp`, and the forward-mode rule (`jvp`, used by
+    torch.autograd.forward_ad and torch.func.jvp) recomputes it inside `native.jvp`, so a forward-mode call computes G(z)
+    twice; both run on the current stream.  The weights are frozen (no gradient), as in the projection.  Only first
+    derivatives are available."""
 
     @staticmethod
-    def forward(ctx, z, native):
+    def forward(z, native):
+        return native.forward(z)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        z, native = inputs
         ctx.native = native
         ctx.save_for_backward(z)
-        return native.forward(z)
+        ctx.save_for_forward(z)
 
     @staticmethod
     @once_differentiable
@@ -368,9 +420,31 @@ class GeneratorFunction(torch.autograd.Function):
         (z,) = ctx.saved_tensors
         return ctx.native.vjp(z, dy).reshape(z.shape), None
 
+    @staticmethod
+    def jvp(ctx, t, _native_t):
+        (z,) = ctx.saved_tensors
+        z, t = _unwrap_functorch(z), _unwrap_functorch(t)
+        with torch._C._DisableFuncTorch():      # the result buffers must be plain tensors too
+            return ctx.native.jvp(z, t)
+
+
+def _is_functorch_wrapped(z: torch.Tensor) -> bool:
+    return bool(torch._C._functorch.is_functorch_wrapped_tensor(z))
+
+
+def _unwrap_functorch(t: torch.Tensor) -> torch.Tensor:
+    """Under torch.func.jvp the forward-mode rule receives functorch-wrapped tensors, which have no storage of their own
+    (and tensors it allocates would be wrapped too, unless functorch is disabled); the library reads the tensor they
+    wrap."""
+    while _is_functorch_wrapped(t):
+        t = torch._C._functorch.get_unwrapped(t)
+    return t
+
 
 def generator(native, z: torch.Tensor) -> torch.Tensor:
-    """G(z): a tensor with a grad_fn when z requires grad and grad mode is on, else exactly native.forward(z)."""
-    if z.requires_grad and torch.is_grad_enabled():
+    """G(z): a tensor with a grad_fn when z requires grad and grad mode is on, a dual tensor carrying J t when z carries a
+    forward tangent t (torch.autograd.forward_ad, torch.func.jvp), else exactly native.forward(z)."""
+    if ((z.requires_grad and torch.is_grad_enabled()) or _is_functorch_wrapped(z)
+            or fwAD.unpack_dual(z).tangent is not None):
         return GeneratorFunction.apply(z, native)
     return native.forward(z)

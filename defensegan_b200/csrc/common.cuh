@@ -54,7 +54,8 @@ enum Epilogue : int {
   EPI_NONE = 3        // out = acc                                       (backward into a linear output / dz)
 };
 
-enum FinalAct : int { ACT_SIGMOID = 0, ACT_TANH = 1 };
+// ACT_NONE: the last layer's linear part alone, no bias (dgan_jvp's tangent of the pre-activation)
+enum FinalAct : int { ACT_SIGMOID = 0, ACT_TANH = 1, ACT_NONE = 2 };
 
 // One (input pixel, weight tile) contribution to an output pixel.  Every layer of the generator -
 // Linear, 5x5/stride-2 transposed conv forward, and their backward-to-input - is expressed as

@@ -146,7 +146,11 @@ static std::vector<DeconvSpec> deconv_specs(const dgan_desc* d, const Widths& w)
 // without the ReLU, and the backward into its output applies no mask (the BN backward does both).
 // Widths are the padded ones of padded_widths(); a desc it refuses has no directions.  A layer-direction with more than
 // 256 output channels becomes one entry per column block of 256, named and profiled as e.g. "Linear.fwd[256:512]".
-static std::vector<TcDir> tc_directions(const dgan_desc* d) {
+// tangent: dgan_jvp's pass instead - each layer's forward becomes its tangent direction "<layer>.jvp" (same geometry,
+// pair table and weight tiles, no bias, the tangent epilogue: the ReLU mask of the primal forward, none before a
+// BatchNorm or without an activation, fp32 for the last layer), and the backward directions are left out (their logical
+// indices stay reserved, so an entry's ld names the same layer-direction in both lists).
+static std::vector<TcDir> tc_directions(const dgan_desc* d, bool tangent = false) {
   const bool celeba = d->arch == DGAN_ARCH_CELEBA;
   const int c_img = celeba ? 3 : 1;
   std::vector<TcDir> dirs;
@@ -168,15 +172,27 @@ static std::vector<TcDir> tc_directions(const dgan_desc* d) {
     }
     ++ld;
   };
+  // a forward of the projection, or its tangent direction t_name with epilogue t_epi and output type t_bytes
+  auto fwd = [&](const std::string& name, const std::string& kind, const std::string& t_name, int N, int K, int P_in,
+                 int P_out, int n_tiles, PairTable tab, int h_grid, int w_grid, int epi, int out_bytes, int t_epi, int t_bytes,
+                 int n_real) {
+    if (tangent) add(t_name, t_name, N, K, P_in, P_out, n_tiles, std::move(tab), h_grid, w_grid, t_epi, t_bytes, n_real);
+    else add(name, kind, N, K, P_in, P_out, n_tiles, std::move(tab), h_grid, w_grid, epi, out_bytes, n_real);
+  };
   // a GEMM layer's directions have one weight tile more than their pairs use: the all-zero tile of tc_with_zero_tile()
   const bool bn0 = d->use_bn != 0;
-  add("Linear.fwd", "Linear.fwd", wd.c4, wd.latent, 1, 16, 17, tc_with_zero_tile(linear_fwd_pairs(16), 16), 4, 4,
-      bn0 ? EPI_BIAS : EPI_BIAS_RELU, bn0 ? 4 : 2, rw.c4);
-  for (TcDir& t : dirs) t.bias_pstride = wd.c4;     // bias index f = pixel * C_out + c
+  fwd("Linear.fwd", "Linear.fwd", "Linear.jvp", wd.c4, wd.latent, 1, 16, 17, tc_with_zero_tile(linear_fwd_pairs(16), 16), 4, 4,
+      bn0 ? EPI_BIAS : EPI_BIAS_RELU, bn0 ? 4 : 2, bn0 ? EPI_NONE : EPI_MASK, 2, rw.c4);
+  if (!tangent)
+    for (TcDir& t : dirs) t.bias_pstride = wd.c4;   // bias index f = pixel * C_out + c
   // dz as TC_LINEAR_SPLIT partial sums over the 16 pixels, one accumulator per window
-  add("Linear.bwd", "Linear.bwd", wd.latent, wd.c4, 16, TC_LINEAR_SPLIT, 17, linear_split_pairs(16), 1, TC_LINEAR_SPLIT,
-      EPI_NONE, 4, rw.latent);
-  dirs.back().max_acc = 1;
+  if (tangent) {
+    ++ld;
+  } else {
+    add("Linear.bwd", "Linear.bwd", wd.latent, wd.c4, 16, TC_LINEAR_SPLIT, 17, linear_split_pairs(16), 1, TC_LINEAR_SPLIT,
+        EPI_NONE, 4, rw.latent);
+    dirs.back().max_acc = 1;
+  }
   bool mask_in = !bn0;                               // the backward into the previous layer's output applies its ReLU mask
   const std::vector<DeconvSpec> specs = deconv_specs(d, wd), real_specs = deconv_specs(d, rw);
   int li = 2;
@@ -184,10 +200,11 @@ static std::vector<TcDir> tc_directions(const dgan_desc* d) {
     const std::string nm = "Generator." + std::to_string(li == 4 ? 5 : li);
     const bool bn = d->use_bn && li <= 3;
     const DeconvSpec& rs = real_specs[(size_t)(li - 2)];
-    add(nm + ".fwd", nm + ".fwd", sp.c_out, sp.c_in, sp.in_raster * sp.in_raster, sp.h_used * sp.h_used, kTaps + 1,
+    fwd(nm + ".fwd", nm + ".fwd", nm + ".jvp", sp.c_out, sp.c_in, sp.in_raster * sp.in_raster, sp.h_used * sp.h_used, kTaps + 1,
         tc_with_zero_tile(deconv_fwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.h_used, sp.h_used,
-        (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2, rs.c_out);
-    add(nm + ".bwd", nm + ".bwd", sp.c_in, sp.c_out, sp.h_used * sp.h_used, sp.in_raster * sp.in_raster, kTaps + 1,
+        (sp.relu && !bn) ? EPI_BIAS_RELU : EPI_BIAS, bn ? 4 : 2, (sp.relu && !bn) ? EPI_MASK : EPI_NONE, 2, rs.c_out);
+    if (tangent) ++ld;
+    else add(nm + ".bwd", nm + ".bwd", sp.c_in, sp.c_out, sp.h_used * sp.h_used, sp.in_raster * sp.in_raster, kTaps + 1,
         tc_with_zero_tile(deconv_bwd_pairs(sp.h_in, sp.h_in, sp.h_used, sp.h_used, sp.in_raster), kTaps), sp.in_raster,
         sp.in_raster, mask_in ? EPI_MASK : EPI_NONE, 2, rs.c_in);
     mask_in = sp.relu && !bn;
@@ -196,8 +213,10 @@ static std::vector<TcDir> tc_directions(const dgan_desc* d) {
   // the last layer on 4x4 blocks of image pixels (16 weight tiles per direction); its forward computes the loss
   const int fh = specs.back().h_used, n_blocks = (fh / 2) * (fh / 2);
   const std::string fn = celeba ? "Generator.6" : "Generator.5";
-  add("last.fwd", fn + "+loss.fwd", 16 * c_img, wd.c1, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2, fh / 2,
-      celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2, 16 * c_img);
+  // its tangent: the fp32 tangent of the pre-activation as a block tensor (dgan_jvp applies act'(y))
+  fwd("last.fwd", fn + "+loss.fwd", "last.jvp", 16 * c_img, wd.c1, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2,
+      fh / 2, celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2, EPI_NONE, 4, 16 * c_img);
+  if (tangent) return dirs;
   // K: the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
   add("last.bwd", fn + ".bwd", wd.c1, 16 * c_img, n_blocks, fh * fh, 16, final_block_bwd_pairs(fh, fh), fh, fh,
       mask_in ? EPI_MASK : EPI_NONE, 2, rw.c1);
@@ -277,6 +296,8 @@ struct dgan_ctx {
   int64_t launches = 0;
   TcState tc;
   std::vector<TcDir> tc_dirs;          // fp16 path: tc_directions() with weight tiles and schedules
+  // fp16 path: dgan_jvp's tangent directions (tc_directions(desc, true)) on tc_dirs' weight tiles; made on the first jvp
+  std::vector<TcDir> tc_jvp_dirs;
   // optional per-launch CUDA-event timing (dgan_profile_*): serialises nothing by itself but
   // adds two event records per launch, so it is never enabled in a timed benchmark pass
   bool profile = false;
@@ -384,6 +405,7 @@ struct Workspace {
   std::vector<unsigned long long*> maskbits;   // fp16 path: 1-bit ReLU masks per hidden layer output
   // fp16 path: the TMA descriptors of each layer-direction's input and output, indexed as tc_dirs (build_maps)
   std::vector<CUtensorMap> map_in, map_out;
+  std::vector<CUtensorMap> jmap_in, jmap_out;   // the same for the tangent directions (tc_jvp_dirs), dgan_jvp only
   unsigned* mom_counter = nullptr;     // fp16 path: [n_pad / 128] tickets of the split-K Linear backward's momentum tail
   __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][16 * C_out] scaled dL/dpre of the last layer
   int n_loss_parts = 0, n_g_parts = 1;
@@ -531,8 +553,13 @@ static int launch_final_bwd(dgan_ctx* c, const Workspace& w, const TOUT* mask_sr
 // What logical layer-direction i of the fp16 path (TcDir::ld) reads and writes in workspace w, at full width.  mask: the
 // 1-bit ReLU masks of the activation it writes (forward) or whose gradient it writes (backward); bias: its epilogue's.
 struct TcIo { const void* in; void* out; unsigned long long* mask; const float* bias; };
-static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i) {
+// tangent (dgan_jvp, forward slots only): the tangent of z (in z_h) and of each layer's output (in dact_h), the last
+// layer's into w.dpre; masks are the primal forward's.
+static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i, bool tangent = false) {
   const int nl = (int)c->layers.size(), l = i / 2;
+  if (tangent)
+    return i == 2 * nl ? TcIo{w.dact_h[nl - 1], w.dpre, nullptr, nullptr}
+                       : TcIo{l == 0 ? (const void*)w.z_h : w.dact_h[l - 1], w.dact_h[l], w.maskbits[l], nullptr};
   if (i == 2 * nl) return {w.act_h[nl - 1], w.dblk, nullptr, c->fin.bias};
   if (i % 2 == 0)       // a BatchNorm layer's GEMM writes its fp32 pre-activations
     return {l == 0 ? (const void*)w.z_h : w.act_h[l - 1], w.pre_h[l] ? (void*)w.pre_h[l] : w.act_h[l], w.maskbits[l],
@@ -541,21 +568,25 @@ static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i) {
   return {l == nl ? w.dblk : w.dact_h[l], w.dact_h[l - 1], w.maskbits[l - 1], nullptr};
 }
 
-// Encode the TMA descriptors of every layer-direction's input and output for this workspace.
-static int build_maps(dgan_ctx* c, Workspace& w) {
+// Encode the TMA descriptors of every layer-direction's input and output for this workspace (tangent: of the tangent
+// directions).
+static int build_maps(dgan_ctx* c, Workspace& w, bool tangent = false) {
   if (c->desc.precision != DGAN_PREC_FP16) return 0;
-  w.map_in.assign(c->tc_dirs.size(), CUtensorMap{});
-  w.map_out.assign(c->tc_dirs.size(), CUtensorMap{});
+  const std::vector<TcDir>& dirs = tangent ? c->tc_jvp_dirs : c->tc_dirs;
+  std::vector<CUtensorMap>& map_in = tangent ? w.jmap_in : w.map_in;
+  std::vector<CUtensorMap>& map_out = tangent ? w.jmap_out : w.map_out;
+  map_in.assign(dirs.size(), CUtensorMap{});
+  map_out.assign(dirs.size(), CUtensorMap{});
   int rc;
-  for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
-    const TcDir& t = c->tc_dirs[i];
-    const TcIo io = tc_io(c, w, t.ld);
-    if ((rc = tc_make_map(c->tc, &w.map_in[i], io.in, (uint64_t)t.K, (uint64_t)w.n_pad, (uint64_t)t.P_in, 128, tc2_box_k(t.K))))
+  for (size_t i = 0; i < dirs.size(); ++i) {
+    const TcDir& t = dirs[i];
+    const TcIo io = tc_io(c, w, t.ld, tangent);
+    if ((rc = tc_make_map(c->tc, &map_in[i], io.in, (uint64_t)t.K, (uint64_t)w.n_pad, (uint64_t)t.P_in, 128, tc2_box_k(t.K))))
       return rc;
-    w.map_out[i] = w.map_in[i];      // a placeholder where the epilogue does not store through TMA
+    map_out[i] = map_in[i];          // a placeholder where the epilogue does not store through TMA
     // the full-width output: a column block stores at its channel offset (TcFinalArgs::col0)
     if (tc2_tma_epilogue(t.N, t.epi, t.out_bytes) &&
-        (rc = tc_make_map(c->tc, &w.map_out[i], io.out, (uint64_t)t.out_ld, (uint64_t)w.n_pad, (uint64_t)t.P_out, TC2_STORE_ROWS)))
+        (rc = tc_make_map(c->tc, &map_out[i], io.out, (uint64_t)t.out_ld, (uint64_t)w.n_pad, (uint64_t)t.P_out, TC2_STORE_ROWS)))
       return rc;
   }
   return 0;
@@ -564,13 +595,16 @@ static int build_maps(dgan_ctx* c, Workspace& w) {
 // Logical layer-direction ld of the fp16 path on workspace w: every column block of it, with the epilogue, output type
 // and masks its table entries imply.  want_mask: a forward with the ReLU also stores its masks.  fa: the last layer's and
 // the momentum tail's arguments.  Each block of a split layer-direction is profiled as its own kind (its tc_dirs index);
-// an unsplit one is profiled by the caller, together with the BatchNorm kernels that follow it.
-static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{}) {
-  const TcIo io = tc_io(c, w, ld);
-  for (size_t i = 0; i < c->tc_dirs.size(); ++i) {
-    const TcDir& t = c->tc_dirs[i];
+// an unsplit one is profiled by the caller, together with the BatchNorm kernels that follow it.  tangent: the tangent
+// direction of ld (dgan_jvp; not profiled).
+static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{},
+                     bool tangent = false) {
+  const TcIo io = tc_io(c, w, ld, tangent);
+  const std::vector<TcDir>& dirs = tangent ? c->tc_jvp_dirs : c->tc_dirs;
+  for (size_t i = 0; i < dirs.size(); ++i) {
+    const TcDir& t = dirs[i];
     if (t.ld != ld) continue;
-    ProfScope ps(c, t.N == t.out_ld ? -1 : (int)i, s);
+    ProfScope ps(c, t.N == t.out_ld || tangent ? -1 : (int)i, s);
     TcFinalArgs f = fa;
     const size_t words = (size_t)t.col0 / 64;          // mask words before the block's channels
     if (t.epi == EPI_BIAS_RELU && want_mask) f.mb_out = io.mask + words;
@@ -579,7 +613,9 @@ static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bo
     f.col0 = t.col0;
     void* out = t.out_bytes == 4 ? (void*)((float*)io.out + t.col0) : (void*)((__half*)io.out + t.col0);
     const float* bias = io.bias != nullptr ? io.bias + t.col0 : nullptr;
-    if (int rc = tc2_launch(&c->launches, t, w.map_in[i], w.map_out[i], out, w.n_pad, bias, s, f)) return rc;
+    const CUtensorMap& m_in = tangent ? w.jmap_in[i] : w.map_in[i];
+    const CUtensorMap& m_out = tangent ? w.jmap_out[i] : w.map_out[i];
+    if (int rc = tc2_launch(&c->launches, t, m_in, m_out, out, w.n_pad, bias, s, f)) return rc;
   }
   return 0;
 }
@@ -614,20 +650,32 @@ static int bn_forward_t(dgan_ctx* c, const Workspace& w, int l, const TP* pre, T
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
+// tangent (dgan_jvp): dact holds the tangent of pre and becomes the tangent of act, in place (bn_apply_jvp_kernel)
 template <typename TP, typename T>
-static int bn_backward_t(dgan_ctx* c, const Workspace& w, int l, const TP* pre, const T* act, T* dact, cudaStream_t s) {
+static int bn_backward_t(dgan_ctx* c, const Workspace& w, int l, const TP* pre, const T* act, T* dact, cudaStream_t s,
+                         bool tangent = false) {
   const GemmLayer& L = c->layers[l];
   const int G = L.bn_per_pixel ? L.P_out * L.C_out : L.C_out;
   float* part = w.bn_part[l];
   float *mean_p = part, *var_p = part + (size_t)kBnSplits * G, *s1_p = part + (size_t)2 * kBnSplits * G,
         *s2_p = part + (size_t)3 * kBnSplits * G;
   dim3 rgrid(G / 32, kBnSplits);
+  const size_t total = (size_t)L.P_out * w.n_pad * L.C_out;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  if (tangent) {
+    bn_reduce_kernel<3, TP, T><<<rgrid, 256, 0, s>>>(pre, act, dact, mean_p, var_p, L.P_out, w.n_rows, w.n_pad, L.C_out,
+                                                 L.bn_per_pixel, s1_p, s2_p);
+    DGAN_LAUNCH_CHECK(c);
+    bn_apply_jvp_kernel<TP, T><<<grid, 256, 0, s>>>(pre, act, mean_p, var_p, s1_p, s2_p, L.bn_scale, L.P_out, w.n_rows, w.n_pad,
+                                                   L.C_out, L.bn_per_pixel, dact);
+    DGAN_LAUNCH_CHECK(c);
+    return 0;
+  }
   bn_reduce_kernel<2, TP, T><<<rgrid, 256, 0, s>>>(pre, act, dact, mean_p, var_p, L.P_out, w.n_rows, w.n_pad, L.C_out,
                                                L.bn_per_pixel, s1_p, s2_p);
   DGAN_LAUNCH_CHECK(c);
-  const size_t total = (size_t)L.P_out * w.n_pad * L.C_out;
-  bn_apply_bwd_kernel<TP, T><<<(unsigned)((total + 255) / 256), 256, 0, s>>>(pre, act, mean_p, var_p, s1_p, s2_p, L.bn_scale, L.P_out,
-                                                                          w.n_rows, w.n_pad, L.C_out, L.bn_per_pixel, dact);
+  bn_apply_bwd_kernel<TP, T><<<grid, 256, 0, s>>>(pre, act, mean_p, var_p, s1_p, s2_p, L.bn_scale, L.P_out,
+                                                 w.n_rows, w.n_pad, L.C_out, L.bn_per_pixel, dact);
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
@@ -720,6 +768,46 @@ static int run_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s, Momentu
                            L0.C_in, nullptr, 0, nullptr, s);
 }
 
+// ---- dgan_jvp's tangent pass, after a forward that kept its ReLU masks (run_forward with want_grad): the tangent of z
+// (fp32 path: w.v; fp16 path: z_h, scaled per row) through every layer's forward weights without bias, masked by the
+// primal forward (BatchNorm: bn_backward_t's tangent mode), into the tangent of the last layer's pre-activation in w.dpre
+// (fp32 path: [n_pad][H*W*C]; fp16 path: the fp32 block tensor [n_blocks][n_pad][16 * C_out]).  The hidden layers'
+// tangents live in the gradient buffers (dact, dact_h), which a jvp does not otherwise use.
+static int run_tangent(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  int rc;
+  const int nl = (int)c->layers.size();
+  if (c->desc.precision == DGAN_PREC_FP16) {
+    for (int l = 0; l < nl; ++l) {
+      if ((rc = tc_launch(c, w, 2 * l, s, false, TcFinalArgs{}, true))) return rc;
+      if (c->layers[l].bn_scale != nullptr &&
+          (rc = bn_backward_t<float, __half>(c, w, l, w.pre_h[l], w.act_h[l], w.dact_h[l], s, true)))
+        return rc;
+    }
+    return tc_launch(c, w, 2 * nl, s, false, TcFinalArgs{}, true);
+  }
+  const float* in = w.v;
+  for (int l = 0; l < nl; ++l) {
+    const GemmLayer& L = c->layers[l];
+    const bool bn = L.bn_scale != nullptr, mask = L.relu && !bn;
+    if ((rc = launch_bsgemm_f32(c, mask ? EPI_MASK : EPI_NONE, in, L.C_in, w.n_pad, L.wf, L.wf_tile_stride, L.wf_ld, L.fwd,
+                                w.dact[l], L.C_out, nullptr, 0, mask ? w.act[l] : nullptr, s)))
+      return rc;
+    if (bn && (rc = bn_backward_t<float, float>(c, w, l, w.pre[l], w.act[l], w.dact[l], s, true))) return rc;
+    in = w.dact[l];
+  }
+  // the last layer's linear part (ACT_NONE: no bias, no activation) writes t(pre) where its forward writes y
+  const FinalLayer& f = c->fin;
+  dim3 grid(w.n_rows, f.n_bands), block(128);
+  if (f.C_out == 1)
+    final_fwd_loss_kernel<float, 1, ACT_NONE><<<grid, block, f.fwd_smem, s>>>(in, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, f.bias,
+                                                                             nullptr, 1, 1, w.dpre, nullptr, nullptr);
+  else
+    final_fwd_loss_kernel<float, 3, ACT_NONE><<<grid, block, f.fwd_smem, s>>>(in, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, f.bias,
+                                                                             nullptr, 1, 1, w.dpre, nullptr, nullptr);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
 // z (at the padded latent width) from the caller's z0 [n_rows][latent_dim] or the Philox stream, v = 0
 static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t seed, cudaStream_t s, size_t row_offset = 0) {
   const int latent = c->desc.latent_dim, ld = c->wd.latent;
@@ -747,7 +835,7 @@ static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cu
     if (sigmoid) cotangent_rowmax_kernel<ACT_SIGMOID><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
     else cotangent_rowmax_kernel<ACT_TANH><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
     DGAN_LAUNCH_CHECK(c);
-    cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, w.n_rows, c->desc.use_bn ? 1 : 0);
+    cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, w.n_rows, c->desc.use_bn ? 1 : 0, 4);
     DGAN_LAUNCH_CHECK(c);
   }
   if (tc && w.n_pad > w.n_rows) {
@@ -776,6 +864,27 @@ static int plan_all(dgan_ctx* c, int n_rows) {
   const int n_mpairs = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile) / (2 * kRowTile);
   int rc;
   for (TcDir& t : c->tc_dirs)
+    if ((rc = tc2_get_schedule(t, n_mpairs, c->tc.num_sms / 2, &c->allocs))) return rc;
+  return 0;
+}
+
+// fp16 path: dgan_jvp's tangent directions, made on the first jvp from tc_directions(desc, true) with the projection's
+// weight tiles (same layer-direction and column block), then planned for this many latent rows like plan_all.  A handle
+// that never runs a jvp plans nothing for them and holds no schedule.
+static int plan_tangent(dgan_ctx* c, int n_rows) {
+  if (c->desc.precision != DGAN_PREC_FP16) return 0;
+  int rc;
+  if (c->tc_jvp_dirs.empty()) {
+    std::vector<TcDir> dirs = tc_directions(&c->desc, true);
+    for (TcDir& t : dirs) {
+      if ((rc = tc_dir_supported(t))) return rc;
+      for (const TcDir& p : c->tc_dirs)
+        if (p.ld == t.ld && p.col0 == t.col0) { t.w = p.w; t.tm_b = p.tm_b; }
+    }
+    c->tc_jvp_dirs = std::move(dirs);
+  }
+  const int n_mpairs = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile) / (2 * kRowTile);
+  for (TcDir& t : c->tc_jvp_dirs)
     if ((rc = tc2_get_schedule(t, n_mpairs, c->tc.num_sms / 2, &c->allocs))) return rc;
   return 0;
 }
@@ -944,6 +1053,8 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
 #define OPTIN(K, BYTES) DGAN_CUDA_CHECK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(BYTES)))
   OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH>), kFinalSmemMax);
+  OPTIN((final_fwd_loss_kernel<float, 1, ACT_NONE>), kFinalSmemMax);    // dgan_jvp's tangent of the last layer
+  OPTIN((final_fwd_loss_kernel<float, 3, ACT_NONE>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<__half, 1, ACT_SIGMOID>), 100 * 1024);
   OPTIN((final_fwd_loss_kernel<__half, 3, ACT_TANH>), 100 * 1024);
   OPTIN((final_bwd_kernel<float, 1>), kFinalSmemMax);
@@ -1114,6 +1225,52 @@ int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev,
   return DGAN_OK;
 }
 
+int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, float* y_dev, float* ty_dev, void* ws,
+             size_t ws_bytes, void* stream) {
+  if (h == nullptr || z_dev == nullptr || t_dev == nullptr || ty_dev == nullptr || n_rows <= 0) {
+    set_error("invalid argument");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  Workspace w;
+  int rc;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  if ((rc = plan_tangent(h, n_rows)) || (rc = build_maps(h, w, true))) return rc;
+  h->n_rows_cur = n_rows;
+  const FinalLayer& f = h->fin;
+  const bool tc = h->desc.precision == DGAN_PREC_FP16;
+  const bool sigmoid = f.C_out == 1 && f.act == ACT_SIGMOID;
+  if (!sigmoid && !(f.C_out == 3 && f.act == ACT_TANH)) { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
+  // the forward of dgan_forward, keeping the ReLU masks the tangent pass reads
+  if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
+  if ((rc = run_forward(h, w, nullptr, 1, 1, true, s))) return rc;
+  // the tangent of z, now that the primal Linear has read z_h: fp16 path, row n scaled by 2^e_n with its largest
+  // |t| * 2^e_n in [0.25, 0.5) (one scale for the call with BatchNorm), the scales in w.loss
+  const int latent = h->desc.latent_dim, ld = h->wd.latent;
+  if (tc) {
+    cotangent_rowmax_kernel<ACT_NONE><<<n_rows, 256, 0, s>>>(nullptr, t_dev, latent, w.loss);
+    DGAN_LAUNCH_CHECK(h);
+    cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, n_rows, h->desc.use_bn ? 1 : 0, -1);
+    DGAN_LAUNCH_CHECK(h);
+  }
+  const size_t n_in = (size_t)w.n_pad * ld;
+  tangent_in_kernel<<<(unsigned)((n_in + 255) / 256), 256, 0, s>>>(t_dev, tc ? w.loss : nullptr, n_rows, w.n_pad, latent, ld,
+                                                                   tc ? nullptr : w.v, tc ? w.z_h : nullptr);
+  DGAN_LAUNCH_CHECK(h);
+  if ((rc = run_tangent(h, w, s))) return rc;
+  // ty = t(pre) * act'(y) / scale
+  const size_t total = (size_t)n_rows * h->hwc;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  const int w_out = 2 * f.w_in;
+#define TO(ACT, CO, BLK) tangent_out_kernel<ACT, CO, BLK><<<grid, 256, 0, s>>>(w.y, w.dpre, n_rows, w_out, BLK ? w.loss : nullptr, w.n_pad, ty_dev)
+  if (sigmoid) { if (tc) TO(ACT_SIGMOID, 1, true); else TO(ACT_SIGMOID, 1, false); }
+  else { if (tc) TO(ACT_TANH, 3, true); else TO(ACT_TANH, 3, false); }
+#undef TO
+  DGAN_LAUNCH_CHECK(h);
+  if (y_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(y_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
+  return DGAN_OK;
+}
+
 int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_rows, float* z_dev, void* stream) {
   if (h == nullptr || z_dev == nullptr || n_rows <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int latent = h->desc.latent_dim;
@@ -1257,21 +1414,23 @@ int dgan_profile_read(dgan_handle h, int max_kinds, double* ms_out, int64_t* lau
 // Host-only developer/test aid (not in the public header): plan every tensor-core layer-direction of the fp16 path for
 // `n_rows` latent rows on `n_pairs` CTA pairs exactly as dgan_create/dgan_reconstruct would, and validate each plan
 // with tc2_check_plan.  Needs no GPU.  Returns 0, or an error code with the failing direction in dgan_last_error().
-int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
+static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mutate, bool tangent) {
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
   Widths wd;
   if (int rc = padded_widths(d, &wd)) return rc;
-  for (const TcDir& dr : tc_directions(d)) {
+  const std::string wide_target = tangent ? "Generator.3.jvp" : "Generator.3.fwd";
+  for (const TcDir& dr : tc_directions(d, tangent)) {
     if (int rc = tc_dir_supported(dr)) return rc;
     Tc2Plan plan;
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
-    // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd, faults 12-13
-    // (specific to narrow ops) that of the last layer's backward; the check must then fail.  Each fault but 6 and 9
-    // decodes records, changes one field and encodes them again.
-    const bool narrow = mutate >= 12 && dr.name == "last.bwd", wide = mutate != 0 && mutate < 12 && dr.name == "Generator.3.fwd";
+    // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd (of its
+    // tangent direction Generator.3.jvp for the tangent pass), faults 12-13 (specific to narrow ops) that of the last
+    // layer's backward; the check must then fail.  Each fault but 6 and 9 decodes records, changes one field and encodes
+    // them again.
+    const bool narrow = mutate >= 12 && dr.name == "last.bwd", wide = mutate != 0 && mutate < 12 && dr.name == wide_target;
     if ((narrow || wide) && plan.stream_m.size() > 40) {
       auto mma = [&](size_t i, auto f) { TcMmaRec m = TcMmaRec::decode(plan.stream_m[i]); f(m); plan.stream_m[i] = m.encode(); };
       auto producer = [&](size_t i, auto f) { TcProducerRec p = TcProducerRec::decode(plan.stream_p[i]); f(p); plan.stream_p[i] = p.encode(); };
@@ -1326,6 +1485,15 @@ int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int muta
     }
   }
   return 0;
+}
+
+int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
+  return check_plans_impl(d, n_rows, n_pairs, mutate, false);
+}
+
+// The same for dgan_jvp's tangent directions (tc_directions(d, true)); faults 1-11 damage Generator.3.jvp.
+int dgan_debug_check_tangent_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
+  return check_plans_impl(d, n_rows, n_pairs, mutate, true);
 }
 
 

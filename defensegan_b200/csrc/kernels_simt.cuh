@@ -107,7 +107,8 @@ bsgemm_f32_kernel(const float* __restrict__ in, int C_in, int n_pad, const float
 // Block = (band of 4 output rows, one latent row); the <=4 input rows it needs are staged in
 // shared memory (row stride C_in+4 words: conflict-free 16-byte reads), threads are ordered by
 // sub-pixel phase so that filter reads are (nearly) warp-uniform broadcasts.
-// TIN = float (fp32 path) or __half (tensor-core path activations).
+// TIN = float (fp32 path) or __half (tensor-core path activations).  ACT_NONE (dgan_jvp, fp32 path): y = the deconv alone,
+// without bias - the tangent of the pre-activation, from the tangent of the input.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float4 load4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ float4 load4(const __half* p) {
@@ -169,7 +170,7 @@ final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in
     if (i >= h_out) continue;
     float acc[C_OUT];
 #pragma unroll
-    for (int co = 0; co < C_OUT; ++co) acc[co] = bias[co];
+    for (int co = 0; co < C_OUT; ++co) acc[co] = ACT == ACT_NONE ? 0.f : bias[co];
     // i = 2o + ka - 1  =>  ka has the parity of i+1
     for (int ka = (i + 1) & 1; ka < 5; ka += 2) {
       const int o = (i + 1 - ka) >> 1;
@@ -195,7 +196,8 @@ final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in
     for (int co = 0; co < C_OUT; ++co) {
       float yv, dact;
       if (ACT == ACT_SIGMOID) { yv = 1.f / (1.f + expf(-acc[co])); dact = yv * (1.f - yv); }
-      else { yv = tanhf(acc[co]); dact = 1.f - yv * yv; }
+      else if (ACT == ACT_TANH) { yv = tanhf(acc[co]); dact = 1.f - yv * yv; }
+      else { yv = acc[co]; dact = 1.f; }
       y[ob + co] = yv;
       if (x != nullptr) {
         const float d = yv - x[(size_t)img * h_out * px_per_row + (size_t)i * px_per_row + j * C_OUT + co];
@@ -402,6 +404,7 @@ __device__ __forceinline__ void bn_st(__half* p, size_t i, float v) {   // satur
 
 // MODE 0: sum x            MODE 1: sum (x - mean)^2
 // MODE 2: S1 = sum dy, S2 = sum dy * xhat with dy = dact * (act > 0), xhat = (pre - mean) * inv
+// MODE 3: as MODE 2 with dy = dact, unmasked (dgan_jvp: dact holds the tangent of pre)
 template <int MODE, typename TP, typename T>
 __global__ void __launch_bounds__(256)
 bn_reduce_kernel(const TP* __restrict__ x, const T* __restrict__ act, const T* __restrict__ dact,
@@ -419,7 +422,7 @@ bn_reduce_kernel(const TP* __restrict__ x, const T* __restrict__ act, const T* _
     for (int k = 0; k < kBnSplits; ++k) s += mean_part[(size_t)k * G + g];
     mean = s / (float)M;
   }
-  if (MODE == 2) {
+  if (MODE >= 2) {
     float s = 0.f;
     for (int k = 0; k < kBnSplits; ++k) s += var_part[(size_t)k * G + g];
     inv = rsqrtf(s / (float)M + 1e-5f);
@@ -433,8 +436,8 @@ bn_reduce_kernel(const TP* __restrict__ x, const T* __restrict__ act, const T* _
     const size_t idx = ((size_t)p * n_pad + n) * C + c;
     if (MODE == 0) a0 += bn_ld(x, idx);
     if (MODE == 1) { const float d = bn_ld(x, idx) - mean; a0 = fmaf(d, d, a0); }
-    if (MODE == 2) {
-      const float dy = bn_ld(act, idx) > 0.f ? bn_ld(dact, idx) : 0.f;
+    if (MODE >= 2) {
+      const float dy = (MODE == 3 || bn_ld(act, idx) > 0.f) ? bn_ld(dact, idx) : 0.f;
       a0 += dy;
       a1 = fmaf(dy, (bn_ld(x, idx) - mean) * inv, a1);
     }
@@ -445,7 +448,7 @@ bn_reduce_kernel(const TP* __restrict__ x, const T* __restrict__ act, const T* _
     float s0 = 0.f, s1 = 0.f;
     for (int k = 0; k < 8; ++k) { s0 += red0[k][tx]; s1 += red1[k][tx]; }
     out0[(size_t)split * G + g] = s0;
-    if (MODE == 2) out1[(size_t)split * G + g] = s1;
+    if (MODE >= 2) out1[(size_t)split * G + g] = s1;
   }
 }
 
@@ -496,6 +499,33 @@ __global__ void bn_apply_bwd_kernel(const TP* __restrict__ pre, const T* __restr
   const float xhat = (bn_ld(pre, i) - mean) * inv;
   const float dy = bn_ld(act, i) > 0.f ? bn_ld(dact, i) : 0.f;
   bn_st(dact, i, scale[g] * inv * (dy - s1 / M - xhat * (s2 / M)));
+}
+
+// tangent through BN + ReLU (dgan_jvp), in place:  t = [act > 0] * scale*inv * (t - S1/M - xhat * S2/M) with S1 = sum t,
+// S2 = sum t * xhat over the same rows (and pixels) as the forward statistics (bn_reduce_kernel MODE 3)
+template <typename TP, typename T>
+__global__ void bn_apply_jvp_kernel(const TP* __restrict__ pre, const T* __restrict__ act,
+                                    const float* __restrict__ mean_part, const float* __restrict__ var_part,
+                                    const float* __restrict__ s1_part, const float* __restrict__ s2_part,
+                                    const float* __restrict__ scale, int P, int n_rows, int n_pad, int C, int per_pixel,
+                                    T* __restrict__ t /*in: tangent of pre, out: tangent of act*/) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t total = (size_t)P * n_pad * C;
+  if (i >= total) return;
+  const int c = (int)(i % C);
+  const int n = (int)((i / C) % n_pad);
+  const int p = (int)(i / ((size_t)C * n_pad));
+  if (n >= n_rows || !(bn_ld(act, i) > 0.f)) { bn_st(t, i, 0.f); return; }
+  const int G = per_pixel ? P * C : C, g = per_pixel ? p * C + c : c;
+  const float M = per_pixel ? (float)n_rows : (float)P * (float)n_rows;
+  float sm = 0.f, sv = 0.f, s1 = 0.f, s2 = 0.f;
+  for (int k = 0; k < kBnSplits; ++k) {
+    sm += mean_part[(size_t)k * G + g]; sv += var_part[(size_t)k * G + g];
+    s1 += s1_part[(size_t)k * G + g]; s2 += s2_part[(size_t)k * G + g];
+  }
+  const float mean = sm / M, inv = rsqrtf(sv / M + 1e-5f);
+  const float xhat = (bn_ld(pre, i) - mean) * inv;
+  bn_st(t, i, scale[g] * inv * (bn_ld(t, i) - s1 / M - xhat * (s2 / M)));
 }
 
 }  // namespace dgan

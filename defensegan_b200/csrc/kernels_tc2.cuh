@@ -108,7 +108,8 @@ struct Tc2Cfg {
 // (N, k16 per op, epilogue, output type) it holds the largest slot count, which every window shape can use, and the
 // smaller ones the planner picks for the shipped generators.  The narrow kinds (k16 per op < 4) are the last layer's
 // backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA), at N = 64 (net_dim <= 64) and
-// N = 128 (64 < net_dim <= 128).
+// N = 128 (64 < net_dim <= 128).  N = 16 / 48 with EPI_NONE and fp32 output: dgan_jvp's tangent of the last layer's
+// pre-activation (last.jvp), on the last layer's forward geometry.
 #define TC2_KINDS(X)                                                                                                   \
   X(256, 1, 4, EPI_BIAS_RELU, __half) X(256, 1, 4, EPI_BIAS, __half) X(256, 1, 4, EPI_MASK, __half)                    \
   X(256, 1, 4, EPI_NONE, __half) X(256, 1, 4, EPI_NONE, float) X(256, 1, 4, EPI_BIAS, float)                           \
@@ -119,7 +120,8 @@ struct Tc2Cfg {
   X(64, 4, 4, EPI_NONE, __half) X(64, 4, 4, EPI_NONE, float) X(64, 4, 4, EPI_BIAS, float)                              \
   X(64, 4, 1, EPI_MASK, __half) X(64, 4, 1, EPI_NONE, __half) X(64, 4, 3, EPI_NONE, __half)                            \
   X(128, 2, 1, EPI_MASK, __half) X(128, 2, 1, EPI_NONE, __half) X(128, 2, 3, EPI_NONE, __half)                         \
-  X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)
+  X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)   \
+  X(16, 8, 4, EPI_NONE, float) X(48, 4, 4, EPI_NONE, float)
 
 struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
 #define TC2_KIND_ROW(NT, MB, KS, EP, T) {NT, MB, KS, EP, (int)sizeof(T)},

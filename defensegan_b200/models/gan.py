@@ -294,6 +294,12 @@ class DefenseGANBase(object):
         z = self._as_cuda(z)
         return _native.generator(self._get_native(z.device), z)
 
+    def generator_jacobian(self, z):
+        """dG/dz at each row of z [N, latent] as [N,H,W,C,latent] (NativeGenerator.jacobian: forward-mode products with
+        identity tangents).  Its columns span the tangent space of the range of G at G(z).  Refused with use_bn."""
+        z = self._as_cuda(z)
+        return self._get_native(z.device).jacobian(z)
+
     @staticmethod
     def _as_cuda(t):
         if isinstance(t, np.ndarray):

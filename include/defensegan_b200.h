@@ -137,6 +137,17 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev,
              void* workspace, size_t workspace_bytes, void* stream);
 
+/* The linearisation of generator_fn at z (models/gan.py:657-665,726-735):
+ *   z_dev [n_rows, latent] fp32, t_dev [n_rows, latent] fp32 (tangent) -> ty_dev [n_rows, H*W*C] fp32 = J_G(z) t,
+ *   y_dev [n_rows, H*W*C] = G(z) (nullable; bit-identical to dgan_forward).
+ *   Workspace: dgan_workspace_bytes(h, n_rows, 1).  With use_bn the batch statistics of the n_rows rows are
+ *   differentiated (rows are coupled).  No host synchronisation; no allocation once this row count has been planned
+ *   (the first dgan_jvp at a row count plans the tangent pass for it).
+ * The forward is recomputed.  DGAN_PREC_FP16 scales each row's tangent by a power of two that puts its largest entry in
+ * [0.25, 0.5) (one scale for the call with use_bn) and divides it out of ty, so jvp(z, 2^k t) == 2^k jvp(z, t). */
+int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, float* y_dev, float* ty_dev,
+             void* workspace, size_t workspace_bytes, void* stream);
+
 /* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack
  * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
  * 256 channels, 1 + 10 L - 5 + 2). */
