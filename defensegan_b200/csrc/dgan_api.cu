@@ -416,62 +416,84 @@ struct Workspace {
   size_t bytes = 0;
 };
 
-static Workspace carve(const dgan_ctx* c, int n_rows, void* base) {
+// The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer - name, element type, byte
+// offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.
+static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
   size_t off = 0;
   char* b = (char*)base;
-  auto take = [&](size_t bytes) -> void* {
+  // a buffer of the dims' product of elements of type `type`, one of the element types below
+  struct ElemType { const char* name; size_t bytes; };
+  static const ElemType kTypes[] = {{"f32", 4}, {"f16", 2}, {"u64", 8}, {"u32", 4}};
+  auto take = [&](const std::string& name, const char* type, std::initializer_list<size_t> dims) -> void* {
+    size_t bytes = 0;
+    for (const ElemType& t : kTypes)
+      if (strcmp(t.name, type) == 0) bytes = t.bytes;
+    for (size_t d : dims) bytes *= d;
+    if (layout != nullptr) {
+      *layout += name + " " + type + " " + std::to_string(off);
+      for (size_t d : dims) *layout += " " + std::to_string(d);
+      *layout += "\n";
+    }
     void* p = b ? (void*)(b + off) : nullptr;
     off += align_up(bytes, 1024);
     return p;
   };
   const size_t np = (size_t)w.n_pad;
-  const int latent = c->wd.latent;                 // z, v, g and z_h are stored at the padded latent width
-  w.z = (float*)take(np * latent * 4);
-  w.v = (float*)take(np * latent * 4);
+  const size_t latent = (size_t)c->wd.latent;      // z, v, g and z_h are stored at the padded latent width
   const bool tc = c->desc.precision == DGAN_PREC_FP16;
   w.n_g_parts = tc ? TC_LINEAR_SPLIT : 1;
-  w.g = (float*)take(np * latent * 4 * w.n_g_parts);
-  if (tc) w.z_h = (__half*)take(np * latent * 2);
-  if (tc) w.mom_counter = (unsigned*)take(np / kRowTile * sizeof(unsigned));
-  if (tc) w.dblk = (__half*)take((size_t)c->fin.n_blocks * np * 16 * c->fin.C_out * 2);
   w.n_loss_parts = tc ? c->fin.n_blocks : c->fin.n_bands;
+  if (layout != nullptr) {
+    *layout += "n_rows " + std::to_string(n_rows) + "\nn_pad " + std::to_string(np) + "\nwidths " +
+               std::to_string(c->wd.latent) + " " + std::to_string(c->wd.c4) + " " + std::to_string(c->wd.c2) + " " +
+               std::to_string(c->wd.c1) + "\ng_parts " + std::to_string(w.n_g_parts) + "\n";
+  }
+  w.z = (float*)take("z", "f32", {np, latent});
+  w.v = (float*)take("v", "f32", {np, latent});
+  w.g = (float*)take("g", "f32", {(size_t)w.n_g_parts, np, latent});
+  if (tc) w.z_h = (__half*)take("z_h", "f16", {np, latent});
+  if (tc) w.mom_counter = (unsigned*)take("mom_counter", "u32", {np / kRowTile});
+  if (tc) w.dblk = (__half*)take("dblk", "f16", {(size_t)c->fin.n_blocks, np, (size_t)16 * c->fin.C_out});
   w.loss_stride_n = tc ? 1 : (size_t)w.n_loss_parts;          // fp16 path: [block][n_pad] (coalesced epilogue stores)
   w.loss_stride_b = tc ? (size_t)np : 1;
-  for (const GemmLayer& l : c->layers) {
-    const size_t elems = (size_t)l.P_out * np * l.C_out;
+  for (size_t i = 0; i < c->layers.size(); ++i) {
+    const GemmLayer& l = c->layers[i];
+    const std::string li = "." + std::to_string(i);
+    const size_t P = (size_t)l.P_out, C = (size_t)l.C_out;
+    const size_t G = l.bn_per_pixel ? P * C : C;
     if (tc) {
-      w.act_h.push_back((__half*)take(elems * 2));
-      w.dact_h.push_back((__half*)take(elems * 2));
-      w.maskbits.push_back((unsigned long long*)take(elems / 8));
+      w.act_h.push_back((__half*)take("act_h" + li, "f16", {P, np, C}));
+      w.dact_h.push_back((__half*)take("dact_h" + li, "f16", {P, np, C}));
+      w.maskbits.push_back((unsigned long long*)take("mask" + li, "u64", {P, np, C / 64}));
       if (l.bn_scale != nullptr) {
-        const size_t G = l.bn_per_pixel ? (size_t)l.P_out * l.C_out : (size_t)l.C_out;
-        w.pre_h.push_back((float*)take(elems * 4));
-        w.bn_part.push_back((float*)take((size_t)4 * kBnSplits * G * 4));
+        w.pre_h.push_back((float*)take("pre_h" + li, "f32", {P, np, C}));
+        w.bn_part.push_back((float*)take("bn_part" + li, "f32", {4, (size_t)kBnSplits, G}));
       } else {
         w.pre_h.push_back(nullptr);
         w.bn_part.push_back(nullptr);
       }
     } else {
-      w.act.push_back((float*)take(elems * 4));
-      w.dact.push_back((float*)take(elems * 4));
+      w.act.push_back((float*)take("act" + li, "f32", {P, np, C}));
+      w.dact.push_back((float*)take("dact" + li, "f32", {P, np, C}));
       if (l.bn_scale != nullptr) {
-        const size_t G = l.bn_per_pixel ? (size_t)l.P_out * l.C_out : (size_t)l.C_out;
-        w.pre.push_back((float*)take(elems * 4));
-        w.bn_part.push_back((float*)take((size_t)4 * kBnSplits * G * 4));
+        w.pre.push_back((float*)take("pre" + li, "f32", {P, np, C}));
+        w.bn_part.push_back((float*)take("bn_part" + li, "f32", {4, (size_t)kBnSplits, G}));
       } else {
         w.pre.push_back(nullptr);
         w.bn_part.push_back(nullptr);
       }
     }
   }
-  w.x = (float*)take(np * c->hwc * 4);     // batch <= n_pad
-  w.y = (float*)take(np * c->hwc * 4);
-  w.dpre = (float*)take(np * c->hwc * 4);
-  w.loss_part = (float*)take(np * w.n_loss_parts * 4);
-  w.loss = (float*)take(np * 4);
+  const size_t hwc = (size_t)c->hwc;
+  w.x = (float*)take("x", "f32", {np, hwc});     // batch <= n_pad
+  w.y = (float*)take("y", "f32", {np, hwc});
+  w.dpre = (float*)take("dpre", "f32", {np, hwc});
+  if (tc) w.loss_part = (float*)take("loss_part", "f32", {(size_t)w.n_loss_parts, np});
+  else w.loss_part = (float*)take("loss_part", "f32", {np, (size_t)w.n_loss_parts});
+  w.loss = (float*)take("loss", "f32", {np});
   w.bytes = off;
   return w;
 }
@@ -1614,6 +1636,19 @@ int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
   if (int rc = padded_widths(d, &w)) return rc;
   out[0] = w.latent; out[1] = w.c4; out[2] = w.c2; out[3] = w.c1;
   return 0;
+}
+
+// Host-only test aid (not in the public header): the workspace of handle h for n_rows latent rows as text, from carve()
+// itself - lines "n_rows N", "n_pad N", "widths latent c4 c2 c1" (padded), "g_parts N", then one line per buffer:
+// "name type byte_offset dim0 dim1 ..." (type f32, f16, u64 or u32; dims in storage order, outermost first; the mask
+// words of layer l are "mask.l" [P_out][n_pad][C_out / 64]).  Returns the length, or -1 when buf is too small.
+int dgan_debug_workspace_layout(dgan_handle h, int n_rows, char* buf, int buf_len) {
+  if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
+  std::string out;
+  carve(h, n_rows, nullptr, &out);
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {
