@@ -35,6 +35,7 @@ ABI_SYMBOLS = [
     "dgan_workspace_bytes", "dgan_reconstruct", "dgan_sample_z0", "dgan_forward", "dgan_loss_grad", "dgan_vjp", "dgan_jvp",
     "dgan_last_launch_count", "dgan_last_enqueue_count", "dgan_macs_per_row", "dgan_profile_enable", "dgan_profile_num_kinds",
     "dgan_profile_kind_name", "dgan_profile_read",
+    "dgan_workspace_bytes_weighted", "dgan_reconstruct_weighted", "dgan_loss_grad_weighted",
 ]
 
 
@@ -124,6 +125,12 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_workspace_bytes.argtypes = [vp, i32, i32]
     lib.dgan_reconstruct.restype = i32
     lib.dgan_reconstruct.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_workspace_bytes_weighted.restype = sz
+    lib.dgan_workspace_bytes_weighted.argtypes = [vp, i32, i32]
+    lib.dgan_reconstruct_weighted.restype = i32
+    lib.dgan_reconstruct_weighted.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_weighted.restype = i32
+    lib.dgan_loss_grad_weighted.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -220,8 +227,9 @@ class NativeGenerator:
             pass
 
     # -- helpers -------------------------------------------------------------------------
-    def _workspace(self, batch: int, rec_rr: int):
-        need = int(self.lib.dgan_workspace_bytes(self._handle, batch, rec_rr))
+    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False):
+        sizer = self.lib.dgan_workspace_bytes_weighted if weighted else self.lib.dgan_workspace_bytes
+        need = int(sizer(self._handle, batch, rec_rr))
         if need == 0:
             raise RuntimeError("dgan_workspace_bytes returned 0 (invalid batch / rec_rr)")
         if self._ws is None or self._ws.numel() < need + 1024:
@@ -265,13 +273,17 @@ class NativeGenerator:
     def reconstruct(self, images: torch.Tensor, rec_rr: int, rec_iters: int, rec_lr: float = 10.0,
                     z_init_val: Optional[torch.Tensor] = None, seed: int = 0, momentum: float = 0.7,
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
-                    z_row_offset: int = 0):
+                    z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None):
+        """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
+        the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
+        (dgan_reconstruct_weighted)."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
             raise ValueError("images must be [B,%d,%d,%d]" % self.image_dim)
         if rec_rr <= 0 or rec_iters <= 0 or batch <= 0:
             raise ValueError("batch, rec_rr and rec_iters must be positive")
+        pw = self._pixel_weights(pixel_weights, batch)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -283,13 +295,18 @@ class NativeGenerator:
                 raise ValueError("out must be a contiguous CUDA float32 tensor shaped like images")
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr)
+            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            rc = self.lib.dgan_reconstruct(self._handle, ctypes.byref(prm), _ptr(x), _ptr(z0), _ptr(rec), _ptr(loss),
-                                           _ptr(idx), ws, need, ctypes.c_void_p(stream))
-            _check(self.lib, rc, "dgan_reconstruct")
+            if pw is None:
+                rc = self.lib.dgan_reconstruct(self._handle, ctypes.byref(prm), _ptr(x), _ptr(z0), _ptr(rec), _ptr(loss),
+                                               _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct")
+            else:
+                rc = self.lib.dgan_reconstruct_weighted(self._handle, ctypes.byref(prm), _ptr(x), _ptr(pw), _ptr(z0),
+                                                        _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_weighted")
         rec = rec.view(images.shape) if out is None else rec
         if return_aux:
             return rec, loss, idx
@@ -317,21 +334,38 @@ class NativeGenerator:
                    "dgan_forward")
         return y
 
-    def loss_grad(self, images: torch.Tensor, z: torch.Tensor, rec_rr: int):
+    def _pixel_weights(self, pixel_weights: Optional[torch.Tensor], batch: int) -> Optional[torch.Tensor]:
+        """The weights as a contiguous CUDA float32 [batch, H, W, C] tensor (None stays None)."""
+        if pixel_weights is None:
+            return None
+        pw = _require_cuda_f32(pixel_weights, "pixel_weights")
+        if pw.numel() != batch * self.hwc or pw.shape[0] != batch:
+            raise ValueError("pixel_weights must be [B,%d,%d,%d] like the images" % self.image_dim)
+        return pw
+
+    def loss_grad(self, images: torch.Tensor, z: torch.Tensor, rec_rr: int, pixel_weights: Optional[torch.Tensor] = None):
+        """(G(z), per-row loss, d(sum loss)/dz) at z [batch*rec_rr, latent]; with pixel_weights [B,H,W,C] the loss is the
+        weighted one of reconstruct (dgan_loss_grad_weighted)."""
         x = _require_cuda_f32(images, "images")
         zc = _require_cuda_f32(z, "z")
         batch = x.shape[0]
         n = batch * rec_rr
         if zc.shape[0] != n:
             raise ValueError("z must have batch*rec_rr rows")
+        pw = self._pixel_weights(pixel_weights, batch)
         with torch.cuda.device(self.device):
             y = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
             loss = torch.empty(n, dtype=torch.float32, device=self.device)
             grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr)
+            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            _check(self.lib, self.lib.dgan_loss_grad(self._handle, _ptr(x), batch, rec_rr, _ptr(zc), _ptr(y), _ptr(loss),
-                                                     _ptr(grad), ws, need, ctypes.c_void_p(stream)), "dgan_loss_grad")
+            if pw is None:
+                _check(self.lib, self.lib.dgan_loss_grad(self._handle, _ptr(x), batch, rec_rr, _ptr(zc), _ptr(y), _ptr(loss),
+                                                         _ptr(grad), ws, need, ctypes.c_void_p(stream)), "dgan_loss_grad")
+            else:
+                _check(self.lib, self.lib.dgan_loss_grad_weighted(self._handle, _ptr(x), _ptr(pw), batch, rec_rr, _ptr(zc),
+                                                                  _ptr(y), _ptr(loss), _ptr(grad), ws, need,
+                                                                  ctypes.c_void_p(stream)), "dgan_loss_grad_weighted")
         return y, loss, grad
 
     def vjp(self, z: torch.Tensor, dy: torch.Tensor, want_y: bool = False):

@@ -150,7 +150,11 @@ static std::vector<DeconvSpec> deconv_specs(const dgan_desc* d, const Widths& w)
 // pair table and weight tiles, no bias, the tangent epilogue: the ReLU mask of the primal forward, none before a
 // BatchNorm or without an activation, fp32 for the last layer), and the backward directions are left out (their logical
 // indices stay reserved, so an entry's ld names the same layer-direction in both lists).
-static std::vector<TcDir> tc_directions(const dgan_desc* d, bool tangent = false) {
+// weighted: dgan_reconstruct_weighted's pass - the last layer's forward alone, "last.fwd.w", with the weighted final
+// epilogue (per-pixel weights of the squared error); its ld and geometry are those of last.fwd.
+enum TcPass { TC_PASS_PROJ, TC_PASS_TANGENT, TC_PASS_WEIGHTED };
+static std::vector<TcDir> tc_directions(const dgan_desc* d, TcPass pass = TC_PASS_PROJ) {
+  const bool tangent = pass == TC_PASS_TANGENT;
   const bool celeba = d->arch == DGAN_ARCH_CELEBA;
   const int c_img = celeba ? 3 : 1;
   std::vector<TcDir> dirs;
@@ -217,6 +221,12 @@ static std::vector<TcDir> tc_directions(const dgan_desc* d, bool tangent = false
   fwd("last.fwd", fn + "+loss.fwd", "last.jvp", 16 * c_img, wd.c1, fh * fh, n_blocks, 16, final_block_fwd_pairs(fh, fh), fh / 2,
       fh / 2, celeba ? EPI_FINAL_TANH3 : EPI_FINAL_SIGMOID1, 2, EPI_NONE, 4, 16 * c_img);
   if (tangent) return dirs;
+  if (pass == TC_PASS_WEIGHTED) {      // last.fwd is never split (N = 16 * C_out): one entry
+    TcDir t = dirs.back();
+    t.name = "last.fwd.w"; t.kind = t.base_kind = fn + "+wloss.fwd";
+    t.epi = celeba ? EPI_FINAL_TANH3_W : EPI_FINAL_SIGMOID1_W;
+    return {t};
+  }
   // K: the 16 * C_out real channels of d(pre), no padding (narrow k16 sub-tiles, see Tc2Cfg)
   add("last.bwd", fn + ".bwd", wd.c1, 16 * c_img, n_blocks, fh * fh, 16, final_block_bwd_pairs(fh, fh), fh, fh,
       mask_in ? EPI_MASK : EPI_NONE, 2, rw.c1);
@@ -296,16 +306,20 @@ struct dgan_ctx {
   int64_t launches = 0;
   TcState tc;
   std::vector<TcDir> tc_dirs;          // fp16 path: tc_directions() with weight tiles and schedules
-  // fp16 path: dgan_jvp's tangent directions (tc_directions(desc, true)) on tc_dirs' weight tiles; made on the first jvp
+  // fp16 path: dgan_jvp's tangent directions (tc_directions(desc, TC_PASS_TANGENT)) on tc_dirs' weight tiles; made on the
+  // first jvp
   std::vector<TcDir> tc_jvp_dirs;
+  // fp16 path: the weighted last-layer forward (tc_directions(desc, TC_PASS_WEIGHTED)) on last.fwd's weight tiles; made on
+  // the first weighted call
+  std::vector<TcDir> tc_w_dirs;
   // optional per-launch CUDA-event timing (dgan_profile_*): serialises nothing by itself but
   // adds two event records per launch, so it is never enabled in a timed benchmark pass
   bool profile = false;
   int n_rows_cur = 0;
-  // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay) on a
-  // private stream, replayed with one cudaGraphLaunch per call.
+  // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
+  // weighted) on a private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
-    const void* ws; int batch, rec_rr, rec_iters, decay_lr; float rec_lr, momentum;
+    const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted; float rec_lr, momentum;
     cudaGraphExec_t exec; int64_t kernels;
   };
   std::vector<LoopGraph> graphs;
@@ -406,6 +420,7 @@ struct Workspace {
   // fp16 path: the TMA descriptors of each layer-direction's input and output, indexed as tc_dirs (build_maps)
   std::vector<CUtensorMap> map_in, map_out;
   std::vector<CUtensorMap> jmap_in, jmap_out;   // the same for the tangent directions (tc_jvp_dirs), dgan_jvp only
+  std::vector<CUtensorMap> wmap_in, wmap_out;   // the same for the weighted last-layer forward (tc_w_dirs), weighted calls only
   unsigned* mom_counter = nullptr;     // fp16 path: [n_pad / 128] tickets of the split-K Linear backward's momentum tail
   __half* dblk = nullptr;              // fp16 path: [n_blocks][n_pad][16 * C_out] scaled dL/dpre of the last layer
   int n_loss_parts = 0, n_g_parts = 1;
@@ -413,12 +428,14 @@ struct Workspace {
   float *y = nullptr, *dpre = nullptr, *loss_part = nullptr;
   float* loss = nullptr;               // [n_pad] per-row loss; dgan_vjp (which computes no loss) keeps its row scales here
   float* x = nullptr;                  // [batch][H*W*C] copy of the call's images (the captured loop reads them from here)
+  float* xw = nullptr;                 // weighted workspaces: [batch][H*W*C] copy of the call's per-pixel weights
   size_t bytes = 0;
 };
 
 // The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer - name, element type, byte
-// offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.
-static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr) {
+// offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.  weighted: the workspace of the
+// weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.
+static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -494,6 +511,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
   if (tc) w.loss_part = (float*)take("loss_part", "f32", {(size_t)w.n_loss_parts, np});
   else w.loss_part = (float*)take("loss_part", "f32", {np, (size_t)w.n_loss_parts});
   w.loss = (float*)take("loss", "f32", {np});
+  if (weighted) w.xw = (float*)take("xw", "f32", {np, hwc});   // batch <= n_pad
   w.bytes = off;
   return w;
 }
@@ -537,19 +555,21 @@ static int launch_bsgemm_f32(dgan_ctx* c, int epi, const float* in, int C_in, in
   return 0;
 }
 
+// xw (not NULL, with x): the per-pixel weights of the squared error (the WEIGHTED instantiations)
 template <typename TIN>
 static int launch_final_fwd(dgan_ctx* c, const TIN* hin, const Workspace& w, const float* x, int R, int B,
-                            bool want_grad, cudaStream_t s) {
+                            bool want_grad, cudaStream_t s, const float* xw = nullptr) {
   const FinalLayer& f = c->fin;
   dim3 grid(w.n_rows, f.n_bands), block(128);
   const size_t smem = f.fwd_smem;
   float* dpre = want_grad ? w.dpre : nullptr;
   float* lp = x ? w.loss_part : nullptr;
-#define FF(CO, ACT)                                                                                         \
-  final_fwd_loss_kernel<TIN, CO, ACT><<<grid, block, smem, s>>>(hin, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, \
-                                                                f.bias, x, R, B, w.y, dpre ? dpre : w.dpre, lp)
-  if (f.C_out == 1 && f.act == ACT_SIGMOID) FF(1, ACT_SIGMOID);
-  else if (f.C_out == 3 && f.act == ACT_TANH) FF(3, ACT_TANH);
+#define FF(CO, ACT, WT)                                                                                         \
+  final_fwd_loss_kernel<TIN, CO, ACT, WT><<<grid, block, smem, s>>>(hin, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, \
+                                                                    f.bias, x, R, B, w.y, dpre ? dpre : w.dpre, lp, xw)
+  const bool wt = xw != nullptr && x != nullptr;
+  if (f.C_out == 1 && f.act == ACT_SIGMOID) { if (wt) FF(1, ACT_SIGMOID, true); else FF(1, ACT_SIGMOID, false); }
+  else if (f.C_out == 3 && f.act == ACT_TANH) { if (wt) FF(3, ACT_TANH, true); else FF(3, ACT_TANH, false); }
   else { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
 #undef FF
   DGAN_LAUNCH_CHECK(c);
@@ -576,10 +596,10 @@ static int launch_final_bwd(dgan_ctx* c, const Workspace& w, const TOUT* mask_sr
 // 1-bit ReLU masks of the activation it writes (forward) or whose gradient it writes (backward); bias: its epilogue's.
 struct TcIo { const void* in; void* out; unsigned long long* mask; const float* bias; };
 // tangent (dgan_jvp, forward slots only): the tangent of z (in z_h) and of each layer's output (in dact_h), the last
-// layer's into w.dpre; masks are the primal forward's.
-static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i, bool tangent = false) {
+// layer's into w.dpre; masks are the primal forward's.  The weighted pass reads and writes what the projection's does.
+static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i, TcPass pass = TC_PASS_PROJ) {
   const int nl = (int)c->layers.size(), l = i / 2;
-  if (tangent)
+  if (pass == TC_PASS_TANGENT)
     return i == 2 * nl ? TcIo{w.dact_h[nl - 1], w.dpre, nullptr, nullptr}
                        : TcIo{l == 0 ? (const void*)w.z_h : w.dact_h[l - 1], w.dact_h[l], w.maskbits[l], nullptr};
   if (i == 2 * nl) return {w.act_h[nl - 1], w.dblk, nullptr, c->fin.bias};
@@ -590,19 +610,31 @@ static TcIo tc_io(const dgan_ctx* c, const Workspace& w, int i, bool tangent = f
   return {l == nl ? w.dblk : w.dact_h[l], w.dact_h[l - 1], w.maskbits[l - 1], nullptr};
 }
 
-// Encode the TMA descriptors of every layer-direction's input and output for this workspace (tangent: of the tangent
-// directions).
-static int build_maps(dgan_ctx* c, Workspace& w, bool tangent = false) {
+// The layer-directions of a pass and the workspace's tensor maps of them.
+static const std::vector<TcDir>& pass_dirs(const dgan_ctx* c, TcPass pass) {
+  return pass == TC_PASS_TANGENT ? c->tc_jvp_dirs : pass == TC_PASS_WEIGHTED ? c->tc_w_dirs : c->tc_dirs;
+}
+template <typename WS>   // Workspace or const Workspace
+static auto& pass_maps_in(WS& w, TcPass pass) {
+  return pass == TC_PASS_TANGENT ? w.jmap_in : pass == TC_PASS_WEIGHTED ? w.wmap_in : w.map_in;
+}
+template <typename WS>
+static auto& pass_maps_out(WS& w, TcPass pass) {
+  return pass == TC_PASS_TANGENT ? w.jmap_out : pass == TC_PASS_WEIGHTED ? w.wmap_out : w.map_out;
+}
+
+// Encode the TMA descriptors of every layer-direction's input and output for this workspace (of the pass's directions).
+static int build_maps(dgan_ctx* c, Workspace& w, TcPass pass = TC_PASS_PROJ) {
   if (c->desc.precision != DGAN_PREC_FP16) return 0;
-  const std::vector<TcDir>& dirs = tangent ? c->tc_jvp_dirs : c->tc_dirs;
-  std::vector<CUtensorMap>& map_in = tangent ? w.jmap_in : w.map_in;
-  std::vector<CUtensorMap>& map_out = tangent ? w.jmap_out : w.map_out;
+  const std::vector<TcDir>& dirs = pass_dirs(c, pass);
+  std::vector<CUtensorMap>& map_in = pass_maps_in(w, pass);
+  std::vector<CUtensorMap>& map_out = pass_maps_out(w, pass);
   map_in.assign(dirs.size(), CUtensorMap{});
   map_out.assign(dirs.size(), CUtensorMap{});
   int rc;
   for (size_t i = 0; i < dirs.size(); ++i) {
     const TcDir& t = dirs[i];
-    const TcIo io = tc_io(c, w, t.ld, tangent);
+    const TcIo io = tc_io(c, w, t.ld, pass);
     if ((rc = tc_make_map(c->tc, &map_in[i], io.in, (uint64_t)t.K, (uint64_t)w.n_pad, (uint64_t)t.P_in, 128, tc2_box_k(t.K))))
       return rc;
     map_out[i] = map_in[i];          // a placeholder where the epilogue does not store through TMA
@@ -617,16 +649,18 @@ static int build_maps(dgan_ctx* c, Workspace& w, bool tangent = false) {
 // Logical layer-direction ld of the fp16 path on workspace w: every column block of it, with the epilogue, output type
 // and masks its table entries imply.  want_mask: a forward with the ReLU also stores its masks.  fa: the last layer's and
 // the momentum tail's arguments.  Each block of a split layer-direction is profiled as its own kind (its tc_dirs index);
-// an unsplit one is profiled by the caller, together with the BatchNorm kernels that follow it.  tangent: the tangent
-// direction of ld (dgan_jvp; not profiled).
+// an unsplit one is profiled by the caller, together with the BatchNorm kernels that follow it.  pass: the tangent
+// direction of ld (dgan_jvp; not profiled) or its weighted one (the last layer's forward; profiled by the caller).
 static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bool want_mask = false, TcFinalArgs fa = TcFinalArgs{},
-                     bool tangent = false) {
-  const TcIo io = tc_io(c, w, ld, tangent);
-  const std::vector<TcDir>& dirs = tangent ? c->tc_jvp_dirs : c->tc_dirs;
+                     TcPass pass = TC_PASS_PROJ) {
+  const TcIo io = tc_io(c, w, ld, pass);
+  const std::vector<TcDir>& dirs = pass_dirs(c, pass);
+  const std::vector<CUtensorMap>& maps_in = pass_maps_in(w, pass);
+  const std::vector<CUtensorMap>& maps_out = pass_maps_out(w, pass);
   for (size_t i = 0; i < dirs.size(); ++i) {
     const TcDir& t = dirs[i];
     if (t.ld != ld) continue;
-    ProfScope ps(c, t.N == t.out_ld || tangent ? -1 : (int)i, s);
+    ProfScope ps(c, t.N == t.out_ld || pass != TC_PASS_PROJ ? -1 : (int)i, s);
     TcFinalArgs f = fa;
     const size_t words = (size_t)t.col0 / 64;          // mask words before the block's channels
     if (t.epi == EPI_BIAS_RELU && want_mask) f.mb_out = io.mask + words;
@@ -635,9 +669,7 @@ static int tc_launch(dgan_ctx* c, const Workspace& w, int ld, cudaStream_t s, bo
     f.col0 = t.col0;
     void* out = t.out_bytes == 4 ? (void*)((float*)io.out + t.col0) : (void*)((__half*)io.out + t.col0);
     const float* bias = io.bias != nullptr ? io.bias + t.col0 : nullptr;
-    const CUtensorMap& m_in = tangent ? w.jmap_in[i] : w.map_in[i];
-    const CUtensorMap& m_out = tangent ? w.jmap_out[i] : w.map_out[i];
-    if (int rc = tc2_launch(&c->launches, t, m_in, m_out, out, w.n_pad, bias, s, f)) return rc;
+    if (int rc = tc2_launch(&c->launches, t, maps_in[i], maps_out[i], out, w.n_pad, bias, s, f)) return rc;
   }
   return 0;
 }
@@ -702,9 +734,9 @@ static int bn_backward_t(dgan_ctx* c, const Workspace& w, int l, const TP* pre, 
   return 0;
 }
 
-// ---- one generator forward (+ loss and dL/dpre when x != null) ---------------------------
+// ---- one generator forward (+ loss and dL/dpre when x != null; weighted per pixel by xw when that is not null too) ----
 static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, int B, bool want_grad,
-                       cudaStream_t s, bool want_y = true) {
+                       cudaStream_t s, bool want_y = true, const float* xw = nullptr) {
   int rc;
   const int nl = (int)c->layers.size();
   if (c->desc.precision == DGAN_PREC_FP16) {
@@ -718,7 +750,9 @@ static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, i
     TcFinalArgs fa{};
     fa.x = x; fa.y = w.y; fa.loss_part = w.loss_part; fa.R = R; fa.B = B; fa.n_rows = w.n_rows;
     fa.nbx = c->fin.w_in / 2; fa.w_out = 2 * c->fin.w_in; fa.gscale = c->tc.grad_scale; fa.write_y = want_y ? 1 : 0;
-    return tc_launch(c, w, 2 * nl, s, false, fa);
+    const bool weighted = x != nullptr && xw != nullptr;
+    fa.xw = weighted ? xw : nullptr;
+    return tc_launch(c, w, 2 * nl, s, false, fa, weighted ? TC_PASS_WEIGHTED : TC_PASS_PROJ);
   }
   const float* in = w.z;
   for (int l = 0; l < nl; ++l) {
@@ -737,7 +771,7 @@ static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, i
     in = w.act[l];
   }
   ProfScope ps(c, 2 * nl, s);
-  return launch_final_fwd<float>(c, in, w, x, R, B, want_grad, s);
+  return launch_final_fwd<float>(c, in, w, x, R, B, want_grad, s, xw);
 }
 
 // ---- backward-to-z: w.g = J^T dpre (unscaled by 2/HWC; fp16 path additionally x gscale) -----
@@ -800,12 +834,12 @@ static int run_tangent(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   const int nl = (int)c->layers.size();
   if (c->desc.precision == DGAN_PREC_FP16) {
     for (int l = 0; l < nl; ++l) {
-      if ((rc = tc_launch(c, w, 2 * l, s, false, TcFinalArgs{}, true))) return rc;
+      if ((rc = tc_launch(c, w, 2 * l, s, false, TcFinalArgs{}, TC_PASS_TANGENT))) return rc;
       if (c->layers[l].bn_scale != nullptr &&
           (rc = bn_backward_t<float, __half>(c, w, l, w.pre_h[l], w.act_h[l], w.dact_h[l], s, true)))
         return rc;
     }
-    return tc_launch(c, w, 2 * nl, s, false, TcFinalArgs{}, true);
+    return tc_launch(c, w, 2 * nl, s, false, TcFinalArgs{}, TC_PASS_TANGENT);
   }
   const float* in = w.v;
   for (int l = 0; l < nl; ++l) {
@@ -890,40 +924,46 @@ static int plan_all(dgan_ctx* c, int n_rows) {
   return 0;
 }
 
-// fp16 path: dgan_jvp's tangent directions, made on the first jvp from tc_directions(desc, true) with the projection's
-// weight tiles (same layer-direction and column block), then planned for this many latent rows like plan_all.  A handle
-// that never runs a jvp plans nothing for them and holds no schedule.
-static int plan_tangent(dgan_ctx* c, int n_rows) {
+// fp16 path: the directions of dgan_jvp's tangent pass or of the weighted last-layer forward, made on the first call that
+// needs them from tc_directions(desc, pass) with the projection's weight tiles (same layer-direction and column block),
+// then planned for this many latent rows like plan_all.  A handle that never runs such a call plans nothing for them and
+// holds no schedule.
+static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
   if (c->desc.precision != DGAN_PREC_FP16) return 0;
   int rc;
-  if (c->tc_jvp_dirs.empty()) {
-    std::vector<TcDir> dirs = tc_directions(&c->desc, true);
+  std::vector<TcDir>& have = pass == TC_PASS_TANGENT ? c->tc_jvp_dirs : c->tc_w_dirs;
+  if (have.empty()) {
+    std::vector<TcDir> dirs = tc_directions(&c->desc, pass);
     for (TcDir& t : dirs) {
       if ((rc = tc_dir_supported(t))) return rc;
       for (const TcDir& p : c->tc_dirs)
         if (p.ld == t.ld && p.col0 == t.col0) { t.w = p.w; t.tm_b = p.tm_b; }
     }
-    c->tc_jvp_dirs = std::move(dirs);
+    have = std::move(dirs);
   }
   const int n_mpairs = (int)align_up((size_t)std::max(n_rows, 1), 2 * kRowTile) / (2 * kRowTile);
-  for (TcDir& t : c->tc_jvp_dirs)
+  for (TcDir& t : have)
     if ((rc = tc2_get_schedule(t, n_mpairs, c->tc.num_sms / 2, &c->allocs))) return rc;
   return 0;
 }
 
 // Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
-// workspace's tensor maps.
-static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out) {
+// workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
+// planned and mapped too.
+static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
   if ((rc = plan_all(c, n_rows))) return rc;
-  *out = carve(c, n_rows, ws);
+  if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
+  *out = carve(c, n_rows, ws, nullptr, weighted);
   if (out->bytes > ws_bytes) {
-    set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes));
+    set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
+              (weighted ? " (dgan_workspace_bytes_weighted)" : ""));
     return DGAN_ERR_WORKSPACE;
   }
-  return build_maps(c, *out);
+  if ((rc = build_maps(c, *out))) return rc;
+  return weighted ? build_maps(c, *out, TC_PASS_WEIGHTED) : 0;
 }
 
 // The weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights) as 3-D arrays: the caller's shape
@@ -1075,6 +1115,8 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
 #define OPTIN(K, BYTES) DGAN_CUDA_CHECK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(BYTES)))
   OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH>), kFinalSmemMax);
+  OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID, true>), kFinalSmemMax);   // the weighted loss
+  OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH, true>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<float, 1, ACT_NONE>), kFinalSmemMax);    // dgan_jvp's tangent of the last layer
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_NONE>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<__half, 1, ACT_SIGMOID>), 100 * 1024);
@@ -1181,6 +1223,12 @@ size_t dgan_workspace_bytes(dgan_handle h, int batch, int rec_rr) {
   return carve(h, batch * rec_rr, nullptr).bytes;
 }
 
+size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
+  if (plan_all(h, batch * rec_rr) != 0 || plan_pass(h, batch * rec_rr, TC_PASS_WEIGHTED) != 0) return 0;
+  return carve(h, batch * rec_rr, nullptr, nullptr, true).bytes;
+}
+
 int64_t dgan_last_launch_count(dgan_handle h) { return h ? h->last_launches : 0; }
 int64_t dgan_last_enqueue_count(dgan_handle h) { return h ? h->last_enqueues : 0; }
 int64_t dgan_macs_per_row(dgan_handle h) { return h ? h->macs_per_row : 0; }
@@ -1197,16 +1245,17 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
   return DGAN_OK;
 }
 
-int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, const float* z_dev, float* y_dev,
-                   float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+// dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place
+static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
+                          float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   if (h == nullptr || x_dev == nullptr || z_dev == nullptr || batch <= 0 || rec_rr <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, w_dev != nullptr))) return rc;
   if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
-  if ((rc = run_forward(h, w, x_dev, rec_rr, batch, true, s))) return rc;
+  if ((rc = run_forward(h, w, x_dev, rec_rr, batch, true, s, true, w_dev))) return rc;
   if ((rc = run_backward(h, w, s))) return rc;
   loss_finish_kernel<<<(n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b, 1.0f / (float)h->hwc, n_rows, w.loss);
   DGAN_LAUNCH_CHECK(h);
@@ -1220,6 +1269,17 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
     DGAN_LAUNCH_CHECK(h);
   }
   return DGAN_OK;
+}
+
+int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, const float* z_dev, float* y_dev,
+                   float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+  return loss_grad_impl(h, x_dev, nullptr, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
+}
+
+int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
+                            float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (w_dev == nullptr) { set_error("NULL weights"); return DGAN_ERR_INVALID_ARG; }
+  return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev, void* ws,
@@ -1257,7 +1317,7 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
   Workspace w;
   int rc;
   if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
-  if ((rc = plan_tangent(h, n_rows)) || (rc = build_maps(h, w, true))) return rc;
+  if ((rc = plan_pass(h, n_rows, TC_PASS_TANGENT)) || (rc = build_maps(h, w, TC_PASS_TANGENT))) return rc;
   h->n_rows_cur = n_rows;
   const FinalLayer& f = h->fin;
   const bool tc = h->desc.precision == DGAN_PREC_FP16;
@@ -1304,9 +1364,13 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
   return DGAN_OK;
 }
 
-int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* z0_dev, float* rec_dev,
-                     float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+// dgan_reconstruct (w_dev NULL) and dgan_reconstruct_weighted: the weights are copied into the workspace next to the
+// images, so the captured loop reads the workspace only
+static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
+                            const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                            void* stream) {
   if (h == nullptr || prm == nullptr || x_dev == nullptr || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  const bool weighted = w_dev != nullptr;
   const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters, decay_lr = prm->decay_lr;
   const float rec_lr = prm->rec_lr, momentum = prm->momentum;
   const uint64_t seed = prm->seed;
@@ -1315,13 +1379,17 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
   const int latent = h->wd.latent;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted))) return rc;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
   if ((rc = run_init_z(h, w, z0_dev, seed, s, (size_t)prm->z_row_offset))) return rc;
   DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
   enqueues += (h->launches - launches0) + 1;
+  if (weighted) {
+    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    enqueues += 1;
+  }
   // The L-step loop (a function of the workspace and the hyper-parameters only): everything it reads or writes lives in
   // the workspace, so it can be captured once and replayed.
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
@@ -1337,7 +1405,7 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
       // The loop returns the pre-update forward of iteration L-1 (models/gan.py:419-421, SURVEY F4):
       // the L-th update is never observed, so its backward pass is not run.
       int r2;
-      if ((r2 = run_forward(h, w, w.x, rec_rr, batch, !last, ls, /*want_y=*/last))) return r2;
+      if ((r2 = run_forward(h, w, w.x, rec_rr, batch, !last, ls, /*want_y=*/last, w.xw))) return r2;
       if (last) continue;
       MomentumArgs mom;
       mom.lr = lr; mom.mu = momentum; mom.tail = tail;
@@ -1357,7 +1425,7 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
     dgan_ctx::LoopGraph* g = nullptr;
     for (auto& e : h->graphs)
       if (e.ws == ws && e.batch == batch && e.rec_rr == rec_rr && e.rec_iters == rec_iters && e.decay_lr == decay_lr &&
-          e.rec_lr == rec_lr && e.momentum == momentum) { g = &e; break; }
+          e.weighted == (int)weighted && e.rec_lr == rec_lr && e.momentum == momentum) { g = &e; break; }
     if (g == nullptr) {
       const int64_t k0 = h->launches;
       cudaGraph_t graph = nullptr;
@@ -1367,7 +1435,7 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
         cudaGraphExec_t exec = nullptr;
         if (crc == 0 && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
           if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, rec_lr, momentum, exec, h->launches - k0});
+          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, rec_lr, momentum, exec, h->launches - k0});
           g = &h->graphs.back();
         }
         if (graph) cudaGraphDestroy(graph);
@@ -1398,6 +1466,18 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_d
   h->last_enqueues = enqueues;
   h->last_launches = h->launches - launches0;
   return DGAN_OK;
+}
+
+int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* z0_dev, float* rec_dev,
+                     float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  return reconstruct_impl(h, prm, x_dev, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
+}
+
+int dgan_reconstruct_weighted(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
+                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                              size_t ws_bytes, void* stream) {
+  if (w_dev == nullptr) { set_error("NULL weights"); return DGAN_ERR_INVALID_ARG; }
+  return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -1436,14 +1516,14 @@ int dgan_profile_read(dgan_handle h, int max_kinds, double* ms_out, int64_t* lau
 // Host-only developer/test aid (not in the public header): plan every tensor-core layer-direction of the fp16 path for
 // `n_rows` latent rows on `n_pairs` CTA pairs exactly as dgan_create/dgan_reconstruct would, and validate each plan
 // with tc2_check_plan.  Needs no GPU.  Returns 0, or an error code with the failing direction in dgan_last_error().
-static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mutate, bool tangent) {
+static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mutate, TcPass pass) {
   using namespace dgan;
   if (d == nullptr || n_rows <= 0 || n_pairs <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
   Widths wd;
   if (int rc = padded_widths(d, &wd)) return rc;
-  const std::string wide_target = tangent ? "Generator.3.jvp" : "Generator.3.fwd";
-  for (const TcDir& dr : tc_directions(d, tangent)) {
+  const std::string wide_target = pass == TC_PASS_TANGENT ? "Generator.3.jvp" : pass == TC_PASS_WEIGHTED ? "last.fwd.w" : "Generator.3.fwd";
+  for (const TcDir& dr : tc_directions(d, pass)) {
     if (int rc = tc_dir_supported(dr)) return rc;
     Tc2Plan plan;
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
@@ -1510,12 +1590,17 @@ static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mut
 }
 
 int dgan_debug_check_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
-  return check_plans_impl(d, n_rows, n_pairs, mutate, false);
+  return check_plans_impl(d, n_rows, n_pairs, mutate, TC_PASS_PROJ);
 }
 
-// The same for dgan_jvp's tangent directions (tc_directions(d, true)); faults 1-11 damage Generator.3.jvp.
+// The same for dgan_jvp's tangent directions (tc_directions(d, TC_PASS_TANGENT)); faults 1-11 damage Generator.3.jvp.
 int dgan_debug_check_tangent_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
-  return check_plans_impl(d, n_rows, n_pairs, mutate, true);
+  return check_plans_impl(d, n_rows, n_pairs, mutate, TC_PASS_TANGENT);
+}
+
+// The same for the weighted last-layer forward (tc_directions(d, TC_PASS_WEIGHTED)); faults 1-11 damage last.fwd.w.
+int dgan_debug_check_weighted_plans(const dgan_desc* d, int n_rows, int n_pairs, int mutate) {
+  return check_plans_impl(d, n_rows, n_pairs, mutate, TC_PASS_WEIGHTED);
 }
 
 
@@ -1642,13 +1727,22 @@ int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
 // itself - lines "n_rows N", "n_pad N", "widths latent c4 c2 c1" (padded), "g_parts N", then one line per buffer:
 // "name type byte_offset dim0 dim1 ..." (type f32, f16, u64 or u32; dims in storage order, outermost first; the mask
 // words of layer l are "mask.l" [P_out][n_pad][C_out / 64]).  Returns the length, or -1 when buf is too small.
-int dgan_debug_workspace_layout(dgan_handle h, int n_rows, char* buf, int buf_len) {
+static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted) {
   if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   std::string out;
-  carve(h, n_rows, nullptr, &out);
+  carve(h, n_rows, nullptr, &out, weighted);
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();
+}
+
+int dgan_debug_workspace_layout(dgan_handle h, int n_rows, char* buf, int buf_len) {
+  return workspace_layout_impl(h, n_rows, buf, buf_len, false);
+}
+
+// The same for the workspace of the weighted entries (dgan_workspace_bytes_weighted): the weights are "xw" [n_pad][H*W*C].
+int dgan_debug_workspace_layout_weighted(dgan_handle h, int n_rows, char* buf, int buf_len) {
+  return workspace_layout_impl(h, n_rows, buf, buf_len, true);
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -128,14 +128,17 @@ __device__ __forceinline__ void store4(__half* p, float4 v) {
 
 constexpr int kBandRows = 4;
 
-template <typename TIN, int C_OUT, int ACT>
+// WEIGHTED (dgan_reconstruct_weighted): xw [B][P_out*C_OUT] weights each pixel's squared error, e = xw (y - x): the loss
+// takes e (y - x) and dpre = e act'(y).  With xw = 1, e == y - x, so every output is the unweighted kernel's.
+template <typename TIN, int C_OUT, int ACT, bool WEIGHTED = false>
 __global__ void __launch_bounds__(128)
 final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in, int C_in,
                       const float* __restrict__ w /*[25][C_OUT][C_in]*/, const float* __restrict__ bias,
                       const float* __restrict__ x /*[B][P_out*C_OUT] or null*/, int R, int B,
                       float* __restrict__ y /*[n_pad][P_out*C_OUT]*/,
                       float* __restrict__ dpre /*[n_pad][P_out*C_OUT] or null*/,
-                      float* __restrict__ loss_part /*[n_pad][n_bands] or null*/) {
+                      float* __restrict__ loss_part /*[n_pad][n_bands] or null*/,
+                      const float* __restrict__ xw = nullptr /*[B][P_out*C_OUT], WEIGHTED only*/) {
   extern __shared__ __align__(16) float smem_f[];
   const int ldh = C_in + 4;
   float* ws = smem_f;                                  // [25*C_OUT][C_in]
@@ -199,7 +202,13 @@ final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in
       else if (ACT == ACT_TANH) { yv = tanhf(acc[co]); dact = 1.f - yv * yv; }
       else { yv = acc[co]; dact = 1.f; }
       y[ob + co] = yv;
-      if (x != nullptr) {
+      if (WEIGHTED) {
+        const size_t xi = (size_t)img * h_out * px_per_row + (size_t)i * px_per_row + j * C_OUT + co;
+        const float d = yv - x[xi];
+        const float e = xw[xi] * d;
+        lsum = fmaf(e, d, lsum);
+        dpre[ob + co] = e * dact;
+      } else if (x != nullptr) {
         const float d = yv - x[(size_t)img * h_out * px_per_row + (size_t)i * px_per_row + j * C_OUT + co];
         lsum = fmaf(d, d, lsum);
         dpre[ob + co] = d * dact;

@@ -148,7 +148,9 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 // the block's pre-activations), so that the output non-linearity, the squared error, its
 // derivative and the per-row loss partial are all computed in the epilogue
 // (models/dataset_models.py:68-69,161-163; models/gan.py:411-414).
-enum TcEpilogue : int { EPI_FINAL_SIGMOID1 = 8, EPI_FINAL_TANH3 = 9 };
+// The _W kinds weight the squared error per pixel (dgan_reconstruct_weighted): e = w (y - x), loss part += e (y - x),
+// d(pre) = e act'(y); with w = 1, e == y - x and every stored value is the unweighted kind's.
+enum TcEpilogue : int { EPI_FINAL_SIGMOID1 = 8, EPI_FINAL_TANH3 = 9, EPI_FINAL_SIGMOID1_W = 10, EPI_FINAL_TANH3_W = 11 };
 
 struct TcFinalArgs {
   const float* x;        // [B][H*W*C] target images (NULL: forward only)
@@ -175,6 +177,9 @@ struct TcFinalArgs {
   // full width) and the block's first channel.  The TMA store adds col0 to its channel coordinate; the other outputs,
   // the bias and the ReLU masks are passed already offset to the block.
   int out_ld, col0;
+  // The weighted last-layer epilogues: [B][H*W*C] per-pixel weights of the squared error, indexed as x.  Last, so that
+  // every other field keeps its offset.
+  const float* xw;
 };
 
 // ------------------------------------------------------------------------------------------

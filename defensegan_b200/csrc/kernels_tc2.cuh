@@ -52,7 +52,8 @@ __host__ __device__ constexpr int tc2_acc_stride(int n_tile) { return n_tile <= 
 
 // Does this instantiation stage its output tiles through shared memory + TMA?
 __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out_bytes) {
-  return out_bytes == 2 && n_tile >= 64 && epi != EPI_FINAL_SIGMOID1 && epi != EPI_FINAL_TANH3;
+  return out_bytes == 2 && n_tile >= 64 && epi != EPI_FINAL_SIGMOID1 && epi != EPI_FINAL_TANH3 && epi != EPI_FINAL_SIGMOID1_W &&
+         epi != EPI_FINAL_TANH3_W;
 }
 
 constexpr int TC2_REC_BATCH = 16;
@@ -109,7 +110,8 @@ struct Tc2Cfg {
 // smaller ones the planner picks for the shipped generators.  The narrow kinds (k16 per op < 4) are the last layer's
 // backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA), at N = 64 (net_dim <= 64) and
 // N = 128 (64 < net_dim <= 128).  N = 16 / 48 with EPI_NONE and fp32 output: dgan_jvp's tangent of the last layer's
-// pre-activation (last.jvp), on the last layer's forward geometry.
+// pre-activation (last.jvp), on the last layer's forward geometry.  The _W final kinds: the weighted last-layer forward
+// (last.fwd.w, dgan_reconstruct_weighted), at the N / slots / k16 of the unweighted final kinds.
 #define TC2_KINDS(X)                                                                                                   \
   X(256, 1, 4, EPI_BIAS_RELU, __half) X(256, 1, 4, EPI_BIAS, __half) X(256, 1, 4, EPI_MASK, __half)                    \
   X(256, 1, 4, EPI_NONE, __half) X(256, 1, 4, EPI_NONE, float) X(256, 1, 4, EPI_BIAS, float)                           \
@@ -121,7 +123,8 @@ struct Tc2Cfg {
   X(64, 4, 1, EPI_MASK, __half) X(64, 4, 1, EPI_NONE, __half) X(64, 4, 3, EPI_NONE, __half)                            \
   X(128, 2, 1, EPI_MASK, __half) X(128, 2, 1, EPI_NONE, __half) X(128, 2, 3, EPI_NONE, __half)                         \
   X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)   \
-  X(16, 8, 4, EPI_NONE, float) X(48, 4, 4, EPI_NONE, float)
+  X(16, 8, 4, EPI_NONE, float) X(48, 4, 4, EPI_NONE, float)                                                              \
+  X(16, 8, 4, EPI_FINAL_SIGMOID1_W, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1_W, __half) X(48, 4, 4, EPI_FINAL_TANH3_W, __half)
 
 struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
 #define TC2_KIND_ROW(NT, MB, KS, EP, T) {NT, MB, KS, EP, (int)sizeof(T)},
@@ -273,7 +276,9 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                   TOUT* __restrict__ out, int n_pad, const float* __restrict__ bias, int bias_pstride, const TcFinalArgs fa) {
   using Cfg = Tc2Cfg<N_TILE, MAXB, KSUB, EPI, (int)sizeof(TOUT)>;
   constexpr bool TMA_EPI = Cfg::TMA_EPI;
-  constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3);
+  constexpr bool WEIGHTED = (EPI == EPI_FINAL_SIGMOID1_W || EPI == EPI_FINAL_TANH3_W);
+  constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3 || WEIGHTED);
+  constexpr bool SIGMOID1 = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_SIGMOID1_W);
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
   constexpr int B_TILE = Cfg::B_TILE, A_BYTES = Cfg::A_BYTES;
   constexpr int PRODUCER = TC2_CONSUMERS / 32;     // warp index of the TMA producer
@@ -468,7 +473,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       const int tile_row0 = (2 * mp + (int)rank) * kRowTile;
       const size_t n_lo = (size_t)(tile_row0 + r_lo);
       if constexpr (FINAL) {
-        constexpr int CO = (EPI == EPI_FINAL_SIGMOID1) ? 1 : 3;
+        constexpr int CO = SIGMOID1 ? 1 : 3;
         const int hwc = fa.w_out * fa.w_out * CO;
         float bsv[CO];
 #pragma unroll
@@ -490,16 +495,23 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
               const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * CO + e;
               float2 xv = make_float2(0.f, 0.f);
               if (fa.x != nullptr) xv = __ldg(reinterpret_cast<const float2*>(fa.x + (size_t)img * hwc + off));
+              float2 wv = make_float2(1.f, 1.f);      // the weight pair next to the image pair (weighted kinds)
+              if (WEIGHTED) wv = __ldg(reinterpret_cast<const float2*>(fa.xw + (size_t)img * hwc + off));
               float yv[2], dv[2];
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
                 const float pre = acc[a * (N_TILE / 2) + j * 4 + h * 2 + c] + bsv[(e + c) % CO];
                 float yy, dact;
-                if (EPI == EPI_FINAL_SIGMOID1) { yy = __fdividef(1.f, 1.f + __expf(-pre)); dact = yy * (1.f - yy); }
+                if (SIGMOID1) { yy = __fdividef(1.f, 1.f + __expf(-pre)); dact = yy * (1.f - yy); }
                 else { const float t = __expf(-2.f * fabsf(pre)); yy = copysignf(__fdividef(1.f - t, 1.f + t), pre); dact = 1.f - yy * yy; }
                 yv[c] = yy;
                 float d = 0.f;
-                if (fa.x != nullptr) { d = yy - (c ? xv.y : xv.x); lsum = fmaf(d, d, lsum); }
+                if (WEIGHTED) {           // e = w d: the loss part takes e d, d(pre) e act'(y)
+                  d = yy - (c ? xv.y : xv.x);
+                  const float ew = (c ? wv.y : wv.x) * d;
+                  lsum = fmaf(ew, d, lsum);
+                  d = ew;
+                } else if (fa.x != nullptr) { d = yy - (c ? xv.y : xv.x); lsum = fmaf(d, d, lsum); }
                 dv[c] = d * dact * fa.gscale;
               }
               if (fa.write_y) *reinterpret_cast<float2*>(fa.y + n * hwc + off) = make_float2(yv[0], yv[1]);

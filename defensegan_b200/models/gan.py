@@ -318,26 +318,50 @@ class DefenseGANBase(object):
         return (int(self.seed) * 1000003 + int(reconstructor_id) * 7919 + self._call_counter) & (2 ** 63 - 1)
 
     def reconstruct(self, images, batch_size=None, back_prop=True, reconstructor_id=0, z_init_val=None,
-                    return_aux=False, out=None, z_row_offset=0):
+                    return_aux=False, out=None, z_row_offset=0, pixel_weights=None):
         """Defense-GAN projection of `images` onto the generator's range (reference
         models/gan.py:333-449): rec_rr restarts x rec_iters momentum-GD steps on
         ||G(z) - x||^2, returns G(z) of the min-loss restart.  Hyper-parameters are read from the
         object at call time.  Fresh z0 ~ N(0, 1/latent_dim) and zero momentum on every call
         (utils/gan_defense.py:119) unless `z_init_val` [B*rec_rr, latent_dim] is given
         (models/gan.py:395-397).  `z_row_offset` (sharded callers only): index of the first latent row of `images`
-        in the call's z0 stream, so that a batch split over several GPUs draws what one GPU would."""
+        in the call's z0 stream, so that a batch split over several GPUs draws what one GPU would.
+
+        `pixel_weights` (an extension; the reference has none): a tensor or array that broadcasts to the images' shape,
+        with finite values in [0, 1], to fit G(z) to part of each image - occluded or missing pixels (weight 0), pixels a
+        detector flagged as corrupted, per-channel or per-region weighting.  The R restarts of an image share its weights.
+        Each restart minimises (1/HWC) sum_p w_p (G(z)_p - x_p)^2: the normaliser stays H*W*C, so rec_lr means what it
+        means unweighted, and weights covering a fraction f of the pixels give gradients about f times smaller (there is
+        no renormalisation).  The returned loss and the arg-min restart use the weighted loss; an image whose weights are
+        all 0 keeps its z0 and restart 0 is chosen.  With weights of 1 the result is bit-identical to the unweighted
+        call.  The weights are checked before any native call - a ValueError for non-finite values or values outside
+        [0, 1] - at the cost of one device reduction and one host read, on the weighted path only."""
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
         if batch_size is not None and int(batch_size) != x.shape[0]:
             raise ValueError("batch_size (%d) does not match images.shape[0] (%d)" % (int(batch_size), x.shape[0]))
+        pw = self._pixel_weights(pixel_weights, x) if pixel_weights is not None else None
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(x.device)
         self.last_seed = seed = self._next_seed(reconstructor_id)
+        kw = {} if pw is None else {"pixel_weights": pw}
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
-                                 return_aux=return_aux, z_row_offset=int(z_row_offset))
+                                 return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
         return res
+
+    def _pixel_weights(self, pixel_weights, x):
+        """pixel_weights broadcast to x's shape and materialised once, after one check of all values (finite, in [0, 1])."""
+        w = self._as_cuda(pixel_weights)
+        try:
+            w = torch.broadcast_to(w.to(x.device), x.shape).contiguous()
+        except RuntimeError as e:
+            raise ValueError("pixel_weights of shape %s do not broadcast to the images' shape %s"
+                             % (tuple(w.shape), tuple(x.shape))) from e
+        if not bool((torch.isfinite(w) & (w >= 0) & (w <= 1)).all()):
+            raise ValueError("pixel_weights must be finite and in [0, 1]")
+        return w
 
     # -- bulk offline reconstruction + its on-disk cache (reference models/gan.py:451-587, 604-646) --------------
     def set_dataset_generators(self, train: Optional[Callable] = None, dev: Optional[Callable] = None,

@@ -27,11 +27,13 @@ def shard_bounds(n_images: int, world_size: int) -> List[int]:
 
 
 def sharded_apply(local_fn: Callable, images: torch.Tensor, rec_rr: int, z_init_val: Optional[torch.Tensor] = None,
-                  group=None) -> torch.Tensor:
+                  group=None, pixel_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Run `local_fn(images_shard, z0_shard, out_view, first_image)` on this rank's shard and all-gather.
 
     `local_fn` must write its [b_local, ...] result into `out_view` (a view of the gather
     buffer).  `images` (and `z_init_val` [B*rec_rr, latent]) hold the FULL batch on every rank.
+    With `pixel_weights` (anything that broadcasts to the images' shape) the shard's weights are sliced with its images
+    and passed as `local_fn(..., pixel_weights=weights_shard)`.
     Returns the full [B, ...] result on every rank.
     """
     world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -48,7 +50,11 @@ def sharded_apply(local_fn: Callable, images: torch.Tensor, rec_rr: int, z_init_
         z0 = None
         if z_init_val is not None:
             z0 = z_init_val.reshape(n * rec_rr, -1)[lo * rec_rr:hi * rec_rr]
-        local_fn(images[lo:hi], z0, gather[rank, :hi - lo], lo)
+        if pixel_weights is None:
+            local_fn(images[lo:hi], z0, gather[rank, :hi - lo], lo)
+        else:
+            pw = torch.broadcast_to(torch.as_tensor(pixel_weights, device=images.device), images.shape)
+            local_fn(images[lo:hi], z0, gather[rank, :hi - lo], lo, pixel_weights=pw[lo:hi])
     if hi - lo < per:
         gather[rank, hi - lo:].zero_()
     if world > 1:
@@ -59,9 +65,11 @@ def sharded_apply(local_fn: Callable, images: torch.Tensor, rec_rr: int, z_init_
     return out
 
 
-def reconstruct_sharded(gan, images: torch.Tensor, z_init_val: Optional[torch.Tensor] = None, group=None) -> torch.Tensor:
+def reconstruct_sharded(gan, images: torch.Tensor, z_init_val: Optional[torch.Tensor] = None, group=None,
+                        pixel_weights: Optional[torch.Tensor] = None) -> torch.Tensor:
     """gan.reconstruct over all ranks of `group` (NCCL): identical to the single-GPU result
     row for row (no BatchNorm), with `z_init_val` given or drawn (the shards index one common z0 stream).
+    `pixel_weights` (see DefenseGANBase.reconstruct) are sliced with the images.
     Ranks with an empty shard still advance the call counter so that later calls stay in step."""
     if bool(gan.use_bn):
         raise RuntimeError("use_bn=True couples all latent rows through batch statistics (SURVEY F2); "
@@ -69,8 +77,11 @@ def reconstruct_sharded(gan, images: torch.Tensor, z_init_val: Optional[torch.Te
 
     # every rank advances the model's call counter identically, so all shards draw from ONE Philox stream; the shard's
     # first row in that stream is (first image) * rec_rr: row for row the single-GPU draw
-    def local_fn(x, z0, out_view, first_image):
-        gan.reconstruct(x, z_init_val=z0, out=out_view, z_row_offset=first_image * int(gan.rec_rr))
+    if pixel_weights is not None:       # checked on the full batch, so every rank raises before any collective
+        pixel_weights = gan._pixel_weights(pixel_weights, images)
+
+    def local_fn(x, z0, out_view, first_image, **kw):
+        gan.reconstruct(x, z_init_val=z0, out=out_view, z_row_offset=first_image * int(gan.rec_rr), **kw)
 
     local_fn.skip = gan._next_seed      # a rank without images must still consume this call's seed
-    return sharded_apply(local_fn, images, int(gan.rec_rr), z_init_val=z_init_val, group=group)
+    return sharded_apply(local_fn, images, int(gan.rec_rr), z_init_val=z_init_val, group=group, pixel_weights=pixel_weights)

@@ -111,6 +111,26 @@ int dgan_reconstruct(dgan_handle h, const dgan_rec_params* params, const float* 
                      const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* Projection onto the generator's range with a per-pixel weighted loss (an extension: the reference has no weighting),
+ * for partially observed images - occluded or missing pixels, pixels flagged as corrupted, per-channel weighting:
+ *   w_dev [batch, H, W, C] fp32, finite, 0 <= w <= 1 (not checked here); the rec_rr restarts of image i share its map.
+ *   Row n's loss is (1/HWC) sum_p w[n / rec_rr, p] (G(z_n)_p - x_p)^2: the normaliser stays H*W*C, so rec_lr keeps its
+ *   meaning and weights covering a fraction f of the pixels give gradients about f times smaller.  Evaluation order per
+ *   pixel: d = y - x, e = w * d, loss += e * d, d(pre) = e * act'(y); with w == 1 every output is bit-identical to
+ *   dgan_reconstruct's.  loss_dev and the arg-min select use the weighted loss; an image whose weights are all 0 keeps
+ *   z0 (its gradient is 0) and restart 0 is chosen (lowest index on ties).  Weights above 1 could saturate the fp16
+ *   path's fixed d(pre) scale, which is sized for |y - x| <= 1.
+ * Workspace: dgan_workspace_bytes_weighted.  The weights are copied into it next to the images: one stream operation
+ * more than dgan_reconstruct, no host synchronisation, no allocation once the size has been planned. */
+int dgan_reconstruct_weighted(dgan_handle h, const dgan_rec_params* params, const float* x_dev, const float* w_dev,
+                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
+                              void* workspace, size_t workspace_bytes, void* stream);
+
+/* Bytes of scratch for dgan_reconstruct_weighted / dgan_loss_grad_weighted: dgan_workspace_bytes plus one weight buffer
+ * of batch images.  Also plans the weighted last-layer forward for batch x rec_rr latent rows (a handle that never
+ * weights plans nothing for it). */
+size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -126,6 +146,12 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
 int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, const float* z_dev,
                    float* y_dev, float* loss_dev, float* grad_dev, void* workspace,
                    size_t workspace_bytes, void* stream);
+
+/* dgan_loss_grad with the weighted loss of dgan_reconstruct_weighted (w_dev [batch, H, W, C], read in place).
+ * Workspace: dgan_workspace_bytes_weighted(h, batch, rec_rr). */
+int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr,
+                            const float* z_dev, float* y_dev, float* loss_dev, float* grad_dev, void* workspace,
+                            size_t workspace_bytes, void* stream);
 
 /* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
  *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
