@@ -1636,11 +1636,12 @@ int dgan_debug_slot_choices(dgan_handle h, int dir, int* out, int max_n) {
 }
 
 #ifdef DGAN_PROBE
-// Developer build only: copy (and clear) the per-CTA cycle counters of the tensor-core kernels.  out: [48][160][8] u64.
+// Developer build only: copy (and clear) the per-CTA cycle counters of the tensor-core kernels.
+// out: [48][160][TC2_PROBE_WORDS] u64.
 int dgan_debug_probe_read(unsigned long long* out) {
   if (cudaDeviceSynchronize() != cudaSuccess) return -1;
   if (cudaMemcpyFromSymbol(out, dgan::g_tc2_probe, sizeof(dgan::g_tc2_probe)) != cudaSuccess) return -1;
-  static unsigned long long zeros[48 * 160 * 8];
+  static unsigned long long zeros[48 * 160 * dgan::TC2_PROBE_WORDS];
   if (cudaMemcpyToSymbol(dgan::g_tc2_probe, zeros, sizeof(zeros)) != cudaSuccess) return -1;
   return 0;
 }

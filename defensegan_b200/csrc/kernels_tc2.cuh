@@ -13,9 +13,10 @@
 //     accumulators - up to 256 columns: the 1-8 accumulators of the item's window.  A step is a run-time number of
 //     rounds, and a round is one MMA into EVERY accumulator in compile-time order, so the compiler never has to choose
 //     an accumulator at run time (an accumulator with nothing to add in a round reads an all-zero weight tile).  One
-//     wgmma group is committed per step and a step's ring region is released once the NEXT step's MMAs are issued and
-//     the step's own group has retired; after the item's last step the consumer waits for all MMAs and runs the
-//     epilogue straight from the registers.  Each consumer warp stores the 16 rows it holds with its own TMA store.
+//     wgmma group is committed per round and one stays in flight, across step boundaries too; a step's ring region is
+//     released once the NEXT step's first round is issued and every earlier group has retired; after the item's last
+//     step the consumer waits for all MMAs and runs the epilogue straight from the registers.  Each consumer warp
+//     stores the 16 rows it holds with its own TMA store.
 #pragma once
 #include "kernels_tc.cuh"
 #include "tc_records.cuh"
@@ -168,11 +169,15 @@ __device__ __forceinline__ void tma_load_3d_mc2(uint32_t dst, const CUtensorMap*
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"((uint16_t)3) : "memory");
 }
+// Arrive on the barrier at `local_bar` in CTA `cta` of the cluster.  Release at CTA scope (the default): the consumers'
+// only accesses it orders are their MMAs' shared-memory reads, which wgmma.wait_group has already completed.
+// .release.cluster compiles to MEMBAR.ALL.GPU, which also waits for the warp's outstanding global loads (the next
+// step's record), once per step.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t local_bar, uint32_t cta) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(local_bar), "r"(cta) : "memory");
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(local_bar), "r"(cta) : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -255,7 +260,12 @@ __device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
 // the end of the CTA's work, launches, cycles from kernel entry to the PDL wait, cycles the first consumer warp waited
 // for operands.  [4] cycles of the set-up (kernel entry to the PDL trigger), [5] / [6] %globaltimer (ns) at kernel entry
 // / at the end of the CTA's work in the LAST launch, [7] %globaltimer when the CTA's first operands had landed.
-__device__ unsigned long long g_tc2_probe[48][160][8];
+// Where the first consumer warp's cycles go, besides the operand wait [3]: [8] issuing a step's MMAs (full barrier
+// passed -> last round waited for, minus [9]; the previous step's release included), [9] the wgmma_wait1 after each
+// round, [10] the wgmma_wait0 at the end of each item, [11] the item epilogues (registers -> global memory, momentum
+// tail included).
+constexpr int TC2_PROBE_WORDS = 12;
+__device__ unsigned long long g_tc2_probe[48][160][TC2_PROBE_WORDS];
 __device__ __forceinline__ unsigned long long probe_gtime() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -286,7 +296,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #ifdef DGAN_PROBE
   const long long probe_t_start = clock64();
   const unsigned long long probe_g_start = probe_gtime();
-  long long probe_wait_full = 0;
+  long long probe_wait_full = 0, probe_issue = 0, probe_wait1 = 0, probe_wait0 = 0, probe_epi = 0;
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t zero_base = smem_base + Cfg::RING_BYTES;           // the all-zero weight tile
@@ -431,7 +441,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #endif
         ptx::mbar_wait(bar_full + 8 * slot, phase);
 #ifdef DGAN_PROBE
-        probe_wait_full += clock64() - probe_w0;
+        const long long probe_w1 = clock64();
+        probe_wait_full += probe_w1 - probe_w0;
         if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
 #endif
         const uint32_t sa = smem_base + (TcMmaRec::Off::get(r0.x) << 10);
@@ -441,24 +452,49 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         const uint64_t db0 = KSUB == 4 ? make_smem_desc_sw128(sb) : make_smem_desc_sw32(sb);
         const uint32_t zoff = (zero_base - sb) >> 4;    // zero tile after the ring: always above the step's B slots
         uint32_t q[6] = {r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+#ifdef DGAN_PROBE
+        long long probe_step_wait = 0;
+#endif
         ptx::fence_operands(acc);
         ptx::wgmma_fence();
+        // One wgmma group per round, and one group in flight.  ptxas closes a hardware group at the end of every
+        // iteration of this run-time loop whatever the commits say, so a single commit per step would make its wait
+        // drain the whole step and idle the tensor pipe at every step boundary.
         for (int r = 0; r < n_rounds; ++r) {
           tc2_mma_round<N_TILE, Cfg::MAXB, KSUB>(acc, q, da0, db0, zoff);
           tc2_pop_round<Cfg::MAXB>(q);
+          ptx::wgmma_commit();
+#ifdef DGAN_PROBE
+          const long long probe_c0 = clock64();
+#endif
+          ptx::wgmma_wait1();           // every group but this round's has retired
+#ifdef DGAN_PROBE
+          probe_step_wait += clock64() - probe_c0;
+#endif
+          if (r == 0) {
+            __syncwarp();
+            // this warp's MMAs no longer read the previous step's region (the previous item's last step was released
+            // after its wgmma_wait0 below)
+            if (!(flags & TcMmaRec::FIRST) && lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
+          }
         }
-        ptx::wgmma_commit();
-        // one group stays in flight across steps: with at most this step's group pending, the previous step's has retired
-        ptx::wgmma_wait1();
         ptx::fence_operands(acc);
-        __syncwarp();
-        // this warp's MMAs no longer read the previous step's region (the previous item's last step was released below)
-        if (!(flags & TcMmaRec::FIRST) && lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
+#ifdef DGAN_PROBE
+        probe_wait1 += probe_step_wait;
+        probe_issue += clock64() - probe_w1 - probe_step_wait;
+#endif
         ++ri; ++it;
       } while (!(flags & TcMmaRec::LAST));
       // the epilogue reads the registers: wait for all MMAs, then release the item's last step
+#ifdef DGAN_PROBE
+      const long long probe_d0 = clock64();
+#endif
       ptx::wgmma_wait0();
       ptx::fence_operands(acc);
+#ifdef DGAN_PROBE
+      const long long probe_e0 = clock64();
+      probe_wait0 += probe_e0 - probe_d0;
+#endif
       __syncwarp();
       if (lane < 2) ptx::mbar_arrive_cluster(bar_empty + 8 * ((it - 1) & (TC2_NSLOT - 1)), (uint32_t)lane);
 
@@ -667,6 +703,9 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           if (tid == 0) fa.m_counter[rt] = 0u;             // ready for the next launch
         }
       }
+#ifdef DGAN_PROBE
+      probe_epi += clock64() - probe_e0;
+#endif
       ++item_count;
     }
     if (TMA_EPI && lane == 0) ptx::bulk_wait_all0();   // this warp's output stores are complete before the CTA retires
@@ -675,7 +714,13 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #ifdef DGAN_PROBE
   {
     constexpr int key = tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT));
-    if (threadIdx.x == 0) atomicAdd(&g_tc2_probe[key][blockIdx.x][3], (unsigned long long)probe_wait_full);
+    if (threadIdx.x == 0) {
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][3], (unsigned long long)probe_wait_full);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][8], (unsigned long long)probe_issue);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][9], (unsigned long long)probe_wait1);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][10], (unsigned long long)probe_wait0);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][11], (unsigned long long)probe_epi);
+    }
     __syncthreads();
     if (threadIdx.x == 0) {
       atomicAdd(&g_tc2_probe[key][blockIdx.x][0], (unsigned long long)(clock64() - probe_t_go));
@@ -943,7 +988,7 @@ static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
   // forward: 8 KB weight tiles) packs 3 activation tiles and their taps into steps of up to 64 KB.  Three steps always
   // fit the ring, so a step's region never overlaps the previous step's: that one is released only after this step's
-  // MMAs have been issued.
+  // first round has been issued.
   const int step_kb = (N == 64 && K == 128) ? DGAN_STEP_MAX_KB_N64 : DGAN_STEP_MAX_KB;
   const int ksub = tc2_ksub(K);
   const double op_ns = tc2_op_ns(N, ksub);
@@ -1137,7 +1182,7 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //  * an op that reads the zero tile never overwrites its accumulator;
 //  * ring safety: when a step's loads may start (step k - dep consumed), no earlier step that can still be read
 //    overlaps its region, regions stay inside the ring, dep <= number of barrier slots;
-//  * progress: a step's region is released only once the next step's MMAs are issued (unless it ends its item), so
+//  * progress: a step's region is released only once the next step's first round is issued (unless it ends its item), so
 //    no step inside an item may wait for the step right before it (dep >= 2);
 //  * every (window, row pair) item is assigned to exactly one CTA pair;
 //  * the accumulator slots per round and the k16 MMAs per op name an instantiation of TC2_KINDS, and every MMA record

@@ -1,6 +1,8 @@
 """Developer aid, needs a library built with -DDGAN_PROBE (DGAN_LIB=...): per tensor-core kernel instantiation, the
 distribution over CTAs of the cycles from the PDL wait to the end of the CTA's work (mean over the launches of one
 projection): a wide distribution = the static item assignment leaves SMs idle at the kernel boundary.
+The second table splits the first consumer warp's cycles into the operand wait, MMA issue, the wgmma_wait1 after each
+round, the wgmma_wait0 at the end of each item and the epilogues, as shares of its busy cycles.
 Usage: DGAN_LIB=build_ab/probe.so python tools/probe_step.py [mnist|celeba] [batch] [L] [--json]
 (--json: one JSON object with the time-ordered busy / hand-over table instead of the text tables; bench.py uses it)"""
 import ctypes
@@ -29,14 +31,15 @@ lib = gan._native.lib if hasattr(gan, "_native") and gan._native is not None els
 gan.reconstruct(x, z_init_val=z0)
 torch.cuda.synchronize()
 lib = gan._native.lib
-buf = (ctypes.c_ulonglong * (48 * 160 * 8))()
+W = 12                                              # counters per CTA (TC2_PROBE_WORDS)
+buf = (ctypes.c_ulonglong * (48 * 160 * W))()
 lib.dgan_debug_probe_read.restype = ctypes.c_int
 lib.dgan_debug_probe_read.argtypes = [ctypes.POINTER(ctypes.c_ulonglong)]
 assert lib.dgan_debug_probe_read(buf) == 0          # discard the first call (schedule upload, graph capture)
 gan.reconstruct(x, z_init_val=z0)
 torch.cuda.synchronize()
 assert lib.dgan_debug_probe_read(buf) == 0
-a = np.frombuffer(buf, dtype=np.uint64).reshape(48, 160, 8).astype(np.float64)
+a = np.frombuffer(buf, dtype=np.uint64).reshape(48, 160, W).astype(np.float64)
 # algorithmic MACs per launch of the MNIST kernels (in-bounds pairs x C_in x C_out x rows), for the busy-time TFLOP/s column
 rows = B * 10
 kind_flops, layer_names = {}, {}
@@ -49,9 +52,9 @@ if dataset != "celeba":
                   (16, "final-sigmoid"): 287296.0 * rows, (64, "mask"): 287296.0 * rows}
 NT = [256, 128, 64, 48, 16]
 EP = ["bias+relu", "bias", "mask", "none", "final-sigmoid", "final-tanh", "float-out", "?"]
-raw = np.frombuffer(buf, dtype=np.uint64).reshape(48, 160, 8)
+raw = np.frombuffer(buf, dtype=np.uint64).reshape(48, 160, W)
 print("kernel <N, epilogue> | launches | cycles from PDL wait to CTA end: mean / min / max over CTAs | (max-mean)/max | trigger->wait mean | MMA operand wait mean (leaders) | set-up cycles mean | last launch, ns from its first CTA entry: last entry / first operands (mean, leaders) / first CTA end / last CTA end")
-timeline = []
+timeline, split = [], {}
 for k in range(48):
     cnt = a[k, :, 1]
     act = cnt > 0
@@ -67,6 +70,10 @@ for k in range(48):
     print("<%d, %s> | %d | %.0f / %.0f / %.0f | %.3f | %.0f | %.0f | %.0f | %d / %.0f / %d / %d   [abs first entry %d, last end %d]" % (
         NT[k // 8], EP[k % 8], int(cnt[act].max()), dur.mean(), dur.min(), dur.max(), (dur.max() - dur.mean()) / dur.max(), pre.mean(),
         wf[lead].mean() if lead.any() else 0, setup.mean(), g0.max() - t0, (gf[gf > 0] - t0).mean() if (gf > 0).any() else -1, g1.min() - t0, g1.max() - t0, t0, g1.max()))
+    # the first consumer warp of each CTA (thread 0): shares of its busy cycles, means over CTAs
+    sh = [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (3, 8, 9, 10, 11)]
+    split[layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8]))] = dict(
+        zip(("operand_wait", "issue", "wgmma_wait1", "wgmma_wait0", "epilogue"), [round(v, 3) for v in sh]))
     timeline.append((int(t0), layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8])), int(g0.max()), float(gf[gf > 0].mean()) if (gf > 0).any() else float(g0.max()),
                      int(g1.max()), 2.0 * kind_flops.get((NT[k // 8], EP[k % 8]), 0.0)))
 # the last launches of the kernels, in time order: how long each was busy and what the hand-over from its predecessor cost
@@ -84,6 +91,11 @@ for t0, name, last_entry, first_full, last_end, flops in timeline:
         tot_gap += gap
     prev_end = last_end
 print("sum | %.1f | %.1f |" % (tot_busy, tot_gap))
+print()
+print("first consumer warp, share of its busy cycles | operand wait | MMA issue | wgmma_wait1 | wgmma_wait0 | epilogue | rest")
+for name, d in split.items():
+    v = list(d.values())
+    print("%s | %s | %.3f" % (name, " | ".join("%.3f" % x for x in v), 1.0 - sum(v)))
 if as_json:
     import json
     rows_out, prev_end = [], None
@@ -91,7 +103,7 @@ if as_json:
         busy = (last_end - last_entry) / 1e3
         gap = (first_full - prev_end) / 1e3 if prev_end is not None and abs(first_full - prev_end) < 1e5 else None
         rows_out.append({"kernel": name, "busy_us": round(busy, 2), "handover_us": None if gap is None else round(gap, 2),
-                         "tflops_while_busy": round(flops / busy / 1e6, 1) if flops else None})
+                         "tflops_while_busy": round(flops / busy / 1e6, 1) if flops else None, "consumer_share": split.get(name)})
         prev_end = last_end
     sys.stdout = _stdout
     print(json.dumps({"dataset": dataset, "batch": B, "rec_rr": 10, "rec_iters": L, "kernels": rows_out,
