@@ -7,6 +7,8 @@
 //   * operands live in a circular shared-memory ring of variable-size steps planned on the host
 //     (tc2_get_schedule): per CTA pair one contiguous stream of step records, LPT-assigned; a ring region is refilled
 //     only after the consumers of BOTH CTAs released it (the peer's loads write into it too);
+//   * a step's MMA record reaches the consumers as its operands do: the producer copies it into a shared-memory slot,
+//     and the copy completes on the step's full barrier, so the consumers' step loop loads nothing from global memory;
 //   * roles per CTA: one producer warpgroup (one warp issues the TMA loads) and two consumer warpgroups.  The producer
 //     gives up registers (setmaxnreg) so that the consumers can hold accumulators and epilogue without spilling.  Each
 //     consumer warpgroup owns 64 of the tile's 128 rows and issues wgmma.mma_async (M = 64, K = 16) into register
@@ -59,6 +61,9 @@ __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out
 
 constexpr int TC2_REC_BATCH = 16;
 constexpr int TC2_STAGING_BYTES = TC2_REC_BATCH * (int)sizeof(TcRec);   // producer record ring (records: tc_records.cuh)
+// The consumers' MMA records: one slot per barrier slot.  The producer copies a step's record there with the step's
+// operands, on the same full barrier.
+constexpr int TC2_MREC_BYTES = TC2_NSLOT * (int)sizeof(TcRec);
 
 // Output staging of the TMA-store epilogues: two 16-row x 128 B buffers per consumer warp (the next unit is written
 // while the store of the previous one still reads shared memory).
@@ -77,7 +82,7 @@ __host__ __device__ constexpr int tc2_b_bytes(int n_tile, int ksub) { return n_t
 __host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb, int ksub) { return maxb > 1 ? tc2_b_bytes(n_tile, ksub) : 0; }
 __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int ksub, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
-  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb, ksub)) / 1024) * 1024;
+  const int raw = ((TC2_SMEM_MAX - 1024 - 256 - TC2_MREC_BYTES - TC2_STAGING_BYTES - epi_b - tc2_zero_bytes(n_tile, maxb, ksub)) / 1024) * 1024;
   return raw > TC2_RING_MAX_KB * 1024 ? TC2_RING_MAX_KB * 1024 : raw;
 }
 
@@ -102,7 +107,7 @@ struct Tc2Cfg {
   static constexpr int EPI_BYTES = EPI_TILES * TC2_TILE_BYTES;
   static constexpr int ZERO_BYTES = tc2_zero_bytes(N_TILE, MAXB, KSUB);
   static constexpr int RING_BYTES = tc2_ring_bytes(N_TILE, MAXB, KSUB, EPI, OUT_BYTES);    // operand ring (offsets are 8-bit KB)
-  static constexpr int SMEM_BYTES = RING_BYTES + ZERO_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256;
+  static constexpr int SMEM_BYTES = RING_BYTES + ZERO_BYTES + EPI_BYTES + TC2_STAGING_BYTES + 1024 + 256 + TC2_MREC_BYTES;
 };
 
 // Every instantiation of tc_bsgemm2_kernel: (N, accumulator slots per round, k16 MMAs per op, epilogue, output type).
@@ -201,6 +206,18 @@ __device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
   return v;
 }
+// As ld_shared_v4, but ordered after the barrier wait before it (the data was written by an asynchronous copy that
+// completed on that barrier).
+__device__ __forceinline__ uint4 ld_shared_v4_ordered(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+// Copy `bytes` (a multiple of 16) from global memory into this CTA's shared memory; the barrier at `bar` receives them.
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
 __device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
@@ -263,12 +280,22 @@ __device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
 // Where the first consumer warp's cycles go, besides the operand wait [3]: [8] issuing a step's MMAs (full barrier
 // passed -> last round waited for, minus [9]; the previous step's release included), [9] the wgmma_wait1 after each
 // round, [10] the wgmma_wait0 at the end of each item, [11] the item epilogues (registers -> global memory, momentum
-// tail included).
-constexpr int TC2_PROBE_WORDS = 12;
+// tail included; [8] excludes [12]).  What is left of the warp's cycles after those spans: [12] record wait (full barrier
+// passed -> the step's MMA record read from shared memory and first used), [13] item head (end of the previous item's
+// epilogue, or the PDL wait, -> the first step's operand wait), [14] end wait (end of the last epilogue -> every warp of
+// the CTA has finished, the producer's drain included).  [15] steps the CTA ran.
+constexpr int TC2_PROBE_WORDS = 16;
 __device__ unsigned long long g_tc2_probe[48][160][TC2_PROBE_WORDS];
 __device__ __forceinline__ unsigned long long probe_gtime() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// clock64() once the load that produces record word 0 `w0` has returned: the clock read is predicated on a bit of the
+// word (bit 31, which no record sets), so it cannot be scheduled ahead of the load's arrival.
+__device__ __forceinline__ long long probe_clock_after(uint32_t w0) {
+  long long t;
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ge.s32 p, %1, 0;\n\tmov.u64 %0, 0;\n\t@p mov.u64 %0, %%clock64;\n\t}" : "=l"(t) : "r"(w0) : "memory");
   return t;
 }
 __host__ __device__ constexpr int tc2_probe_key(int n_tile, int epi, int out_bytes) {
@@ -297,14 +324,15 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   const long long probe_t_start = clock64();
   const unsigned long long probe_g_start = probe_gtime();
   long long probe_wait_full = 0, probe_issue = 0, probe_wait1 = 0, probe_wait0 = 0, probe_epi = 0;
+  unsigned probe_rec = 0, probe_head = 0, probe_steps = 0;     // 32-bit cycle counts: a launch is far shorter than 2^32 cycles
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t zero_base = smem_base + Cfg::RING_BYTES;           // the all-zero weight tile
   const uint32_t epi_base = zero_base + Cfg::ZERO_BYTES;            // output staging: 4 KB per consumer warp
   const uint32_t stg_base = epi_base + Cfg::EPI_BYTES;              // producer ring of TcRec
   const uint32_t bar_base = stg_base + TC2_STAGING_BYTES;
-  // full[s] @ +8s (s<8), empty[s] @ +64+8s, momentum-tail flag @ +200
-  const uint32_t bar_full = bar_base, bar_empty = bar_base + 64;
+  // full[s] @ +8s (s<8), empty[s] @ +64+8s, momentum-tail flag @ +200, MMA record of the step in barrier slot s @ +256+32s
+  const uint32_t bar_full = bar_base, bar_empty = bar_base + 64, mrec_base = bar_base + 256;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = ptx::cluster_ctarank();
@@ -342,6 +370,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   pdl_wait();
 #ifdef DGAN_PROBE
   const long long probe_t_go = clock64();
+  unsigned probe_h0 = (unsigned)probe_t_go;     // start of the item head
+  bool probe_new_item = true;
 #endif
 
   if (warp >= PRODUCER) {
@@ -376,7 +406,10 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           const uint32_t full = bar_full + 8 * slot;
           const uint32_t sa = smem_base + (P::Off::get(r0.x) << 10);
           if (ptx::elect_one()) {
-            ptx::mbar_expect_tx(full, (uint32_t)(nA * A_BYTES + nB * B_TILE));
+            ptx::mbar_expect_tx(full, (uint32_t)(nA * A_BYTES + nB * B_TILE) + (uint32_t)sizeof(TcRec));
+            // the consumers' record of this step (this CTA's own copy, not multicast).  Its slot is free: step it - 8 is
+            // consumed (waited for above), and a consumer warp holds a record in registers before it says so
+            ptx::bulk_load(mrec_base + slot * (uint32_t)sizeof(TcRec), stream_m + rbeg + it, (uint32_t)sizeof(TcRec), full);
 #pragma unroll
             for (int a = 0; a < TC2_MAX_A; ++a) {
               if (a >= nA) break;
@@ -423,21 +456,17 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     uint32_t ri = rbeg, it = 0;
     while (ri < rend) {
       const int item_e = tc2_item_at(eitems, (int)item_count, pair, n_pairs, n_slots);
-      // MMA record of the next step, loaded one step ahead within the item: no global-load latency between two steps'
-      // MMAs (and no record held in registers across the epilogue)
-      uint4 n0 = __ldg(reinterpret_cast<const uint4*>(stream_m + ri)), n1 = __ldg(reinterpret_cast<const uint4*>(stream_m + ri) + 1);
+      // what the epilogue needs to know of the item, requested now: two chained global loads that overlap the item's MMAs
+      const TcItem2* ip = items + tc2_item_window(item_e);
+      const int n_acc = (int)__ldg(&ip->n_acc);
+      const uint32_t q_mine = lane < 16 ? (uint32_t)__ldg(&ip->q[lane]) : 0u;
       uint32_t flags;
       do {    // the steps of one item
-        const uint4 r0 = n0, r1 = n1;
-        flags = TcMmaRec::Flags::get(r0.x);
-        if (!(flags & TcMmaRec::LAST)) {     // not the item's last step: another step of the item follows
-          const uint4* rp = reinterpret_cast<const uint4*>(stream_m + ri + 1);
-          n0 = __ldg(rp); n1 = __ldg(rp + 1);
-        }
         const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
-        const int nA = TcMmaRec::NA::get(r0.x), n_rounds = TcMmaRec::Rounds::get(r0.x);
 #ifdef DGAN_PROBE
         const long long probe_w0 = clock64();
+        if (probe_new_item) probe_head += (unsigned)probe_w0 - probe_h0;
+        probe_new_item = false;
 #endif
         ptx::mbar_wait(bar_full + 8 * slot, phase);
 #ifdef DGAN_PROBE
@@ -445,6 +474,15 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         probe_wait_full += probe_w1 - probe_w0;
         if (it == 0 && threadIdx.x == 0) g_tc2_probe[tc2_probe_key(N_TILE, EPI, (int)sizeof(TOUT))][blockIdx.x][7] = probe_gtime();
 #endif
+        // the step's MMA record arrived with its operands, in the barrier slot's record slot: no global load in this loop
+        const uint4 r0 = ptx::ld_shared_v4_ordered(mrec_base + slot * (uint32_t)sizeof(TcRec));
+        const uint4 r1 = ptx::ld_shared_v4_ordered(mrec_base + slot * (uint32_t)sizeof(TcRec) + 16u);
+        flags = TcMmaRec::Flags::get(r0.x);
+#ifdef DGAN_PROBE
+        const unsigned probe_rec_step = (unsigned)probe_clock_after(r0.x) - (unsigned)probe_w1;
+        probe_rec += probe_rec_step;
+#endif
+        const int nA = TcMmaRec::NA::get(r0.x), n_rounds = TcMmaRec::Rounds::get(r0.x);
         const uint32_t sa = smem_base + (TcMmaRec::Off::get(r0.x) << 10);
         // this warpgroup's 64 rows of the A tiles (of their first sub-tile when narrow)
         const uint64_t da0 = KSUB == 4 ? make_smem_desc_sw128(sa + (uint32_t)wg * 64u * 128u) : make_smem_desc_sw32(sa + (uint32_t)wg * 64u * 32u);
@@ -481,7 +519,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         ptx::fence_operands(acc);
 #ifdef DGAN_PROBE
         probe_wait1 += probe_step_wait;
-        probe_issue += clock64() - probe_w1 - probe_step_wait;
+        probe_issue += clock64() - probe_w1 - probe_step_wait - probe_rec_step;
 #endif
         ++ri; ++it;
       } while (!(flags & TcMmaRec::LAST));
@@ -501,10 +539,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       // ---- epilogue of the item: accumulator registers -> (bias | ReLU | mask | last layer) -> global memory.
       //      Register i of accumulator a holds column (i % (N_TILE/2)) / 4 * 8 + (lane % 4) * 2 + (i % 2) of row
       //      r_lo + 8 * ((i / 2) % 2) (the m64nNk16 accumulator fragment).
-      const TcItem2* ip = items + tc2_item_window(item_e);
       const int mp = tc2_item_mp(item_e);
-      const int n_acc = (int)__ldg(&ip->n_acc);
-      const uint32_t q_mine = lane < 16 ? (uint32_t)__ldg(&ip->q[lane]) : 0u;
       auto q_of = [&](int a) { return (int)__shfl_sync(0xffffffffu, q_mine, a); };
       const int tile_row0 = (2 * mp + (int)rank) * kRowTile;
       const size_t n_lo = (size_t)(tile_row0 + r_lo);
@@ -704,7 +739,11 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         }
       }
 #ifdef DGAN_PROBE
-      probe_epi += clock64() - probe_e0;
+      const long long probe_e1 = clock64();
+      probe_epi += probe_e1 - probe_e0;
+      probe_h0 = (unsigned)probe_e1;
+      probe_new_item = true;
+      probe_steps = it;
 #endif
       ++item_count;
     }
@@ -723,6 +762,10 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     }
     __syncthreads();
     if (threadIdx.x == 0) {
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][12], (unsigned long long)probe_rec);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][13], (unsigned long long)probe_head);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][15], (unsigned long long)probe_steps);
+      if (probe_steps != 0) atomicAdd(&g_tc2_probe[key][blockIdx.x][14], (unsigned long long)((unsigned)clock64() - probe_h0));
       atomicAdd(&g_tc2_probe[key][blockIdx.x][0], (unsigned long long)(clock64() - probe_t_go));
       atomicAdd(&g_tc2_probe[key][blockIdx.x][1], 1ull);
       atomicAdd(&g_tc2_probe[key][blockIdx.x][2], (unsigned long long)(probe_t_go - probe_t_entry));

@@ -2,7 +2,8 @@
 Usage: python tools/plan_stats.py [mnist|celeba] [batch] [R] [CTA pairs] [library] [--slots DIR=MAXB] [--window DIR=WH,WW,SY,SX]
                                  [--latent_dim N] [--net_dim N] [--use_bn]
 --latent_dim / --net_dim / --use_bn plan that generator (default 128 / 64 / no BN); the handle pads each width (see
-DESIGN.md section 2), and the last column shows the share of each direction's k16 MMAs that multiply real channels;
+DESIGN.md section 2), and the last two columns show the share of each direction's k16 MMAs that multiply real channels
+and its steps per CTA pair (what each consumer warp pays a fixed per-step cost for);
 --slots plans layer-direction DIR (the row index of the table, from 0) with exactly MAXB accumulator slots per round;
 --window plans it on exactly the window WH x WW with strides (SY, SX), e.g. to compare two builds at the same window."""
 import ctypes
@@ -57,7 +58,7 @@ real = {"Linear.fwd": (4 * nd, latent), "Linear.bwd": (latent, 4 * nd), "Generat
         "Generator.2.bwd": (4 * nd, 2 * nd), "Generator.3.fwd": (nd, 2 * nd), "Generator.3.bwd": (2 * nd, nd),
         "Generator.5.fwd": (nd, nd), "Generator.5.bwd": (nd, nd), "last.fwd": (img, nd), "last.bwd": (nd, img)}
 lines = buf.value.decode().strip().splitlines()
-out = [lines[0] + " | real k16 MMAs (share)"]
+out = [lines[0] + " | real k16 MMAs (share) | steps per CTA pair"]
 for line in lines[1:-1]:
     col = line.split(" | ")
     name, n, k = col[0], int(col[1]), int(col[2])
@@ -66,6 +67,6 @@ for line in lines[1:-1]:
         a, b = (int(v) for v in name[name.index("[") + 1:-1].split(":"))
         rn = max(0, min(b, rn) - a)
     share = min(rn, n) * min(rk, k) / (n * k)
-    out.append(line + " | %d (%.2f)" % (round(int(col[14]) * share), share))
+    out.append(line + " | %d (%.2f) | %.1f" % (round(int(col[14]) * share), share, int(col[6]) / pairs))
 out.append(lines[-1])
 print("\n".join(out))
