@@ -1528,11 +1528,12 @@ static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mut
     Tc2Plan plan;
     int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
-    // self-test of the validator: damage one plan in one specific way - faults 1-11 that of Generator.3 fwd (of its
-    // tangent direction Generator.3.jvp for the tangent pass), faults 12-13 (specific to narrow ops) that of the last
+    // self-test of the validator: damage one plan in one specific way - faults 1-11 and 14-15 that of Generator.3 fwd (of
+    // its tangent direction Generator.3.jvp for the tangent pass), faults 12-13 (specific to narrow ops) that of the last
     // layer's backward; the check must then fail.  Each fault but 6 and 9 decodes records, changes one field and encodes
     // them again.
-    const bool narrow = mutate >= 12 && dr.name == "last.bwd", wide = mutate != 0 && mutate < 12 && dr.name == wide_target;
+    const bool narrow = (mutate == 12 || mutate == 13) && dr.name == "last.bwd";
+    const bool wide = mutate != 0 && mutate != 12 && mutate != 13 && dr.name == wide_target;
     if ((narrow || wide) && plan.stream_m.size() > 40) {
       auto mma = [&](size_t i, auto f) { TcMmaRec m = TcMmaRec::decode(plan.stream_m[i]); f(m); plan.stream_m[i] = m.encode(); };
       auto producer = [&](size_t i, auto f) { TcProducerRec p = TcProducerRec::decode(plan.stream_p[i]); f(p); plan.stream_p[i] = p.encode(); };
@@ -1566,6 +1567,22 @@ static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mut
         case 11: every_mma([](TcMmaRec& m) { m.maxb = 2; }); break;               // records disagree with the plan's slots
         case 12: every_mma([&](TcMmaRec& m) { m.ksub = plan.ksub == 1 ? 2 : 1; }); break;   // k16 per op
         case 13: producer(20, [](TcProducerRec& p) { p.kc |= 1u; }); break;      // a k-chunk >= 1 (a narrow K has one)
+        case 14: mma(20, [](TcMmaRec& m) {                                   // a round without a real op
+                   for (uint32_t j = 0; j < m.maxb; ++j) m.ops[j] = TC2_PAD_OP;
+                 });
+                 break;
+        case 15: {                                                            // a zero-tile op that overwrites
+                   bool done = false;
+                   for (size_t i = 20; i < plan.stream_m.size() && !done; ++i)
+                     mma(i, [&](TcMmaRec& m) {
+                       for (uint32_t j = 0; j < m.n_rounds * m.maxb && !done; ++j)
+                         if (TcOp::decode(m.ops[j]).slot == (uint32_t)TC2_ZERO_SLOT) {
+                           m.ops[j] = (uint8_t)TcOp::First::put(m.ops[j], 1u);
+                           done = true;
+                         }
+                     });
+                   break;
+                 }
         default: break;
       }
     }
@@ -1649,10 +1666,11 @@ int dgan_debug_probe_read(unsigned long long* out) {
 
 // Host-only developer aid (not in the public header): the plan of every layer-direction in numbers - window shape, items,
 // steps, MMAs (ops of KSUB k16 each, and k16 MMAs), operand bytes staged from L2 into shared memory (both CTAs of every
-// pair), accumulator slots per round, epilogue and output type - as text.  Layer-direction `force_dir` (tc_directions
-// order; -1: none) is planned
-// with exactly `force_maxb` slots per round, as dgan_debug_force_slots would, and, when force_shape is not NULL, with
-// exactly that window shape {wh, ww, sy, sx}.  Returns the length.
+// pair), accumulator slots per round, epilogue and output type - as text.  The MMA columns count every slot of every
+// round, as the time model does; what the kernel issues and skips is in dgan_debug_plan_issue_stats.  Layer-direction
+// `force_dir` (tc_directions order; -1: none) is planned with exactly `force_maxb` slots per round, as
+// dgan_debug_force_slots would, and, when force_shape is not NULL, with exactly that window shape {wh, ww, sy, sx}.
+// Returns the length.
 static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int force_dir, int force_maxb, const int* force_shape,
                            char* buf, int buf_len) {
   using namespace dgan;
@@ -1711,6 +1729,32 @@ int dgan_debug_plan_stats_window(const dgan_desc* d, int n_rows, int n_pairs, in
                                  int sy, int sx, char* buf, int buf_len) {
   const int shape[4] = {wh, ww, sy, sx};
   return plan_stats_impl(d, n_rows, n_pairs, force_dir, force_maxb, shape, buf, buf_len);
+}
+
+// Host-only developer aid (not in the public header): what the kernel issues for the plan of every layer-direction -
+// the slots per round, the k16 MMAs issued (the real ones, and the zero-tile ones where the round is fixed:
+// tc2_issues_zero_ops), the zero-tile k16 MMAs the kernel skips, and the MMA term of the busiest CTA pair's load for the
+// MMAs issued (est. tensor us) - as text, one line per layer-direction in the order of dgan_debug_plan_stats.  The plans
+// are the ones dgan_debug_plan_stats describes.  Returns the length, or -1.
+int dgan_debug_plan_issue_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {
+  using namespace dgan;
+  if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
+  const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
+  Widths wd;
+  if (padded_widths(d, &wd) != 0) return -1;
+  std::string out = "direction | slots | k16 MMAs issued | zero-tile k16 MMAs skipped | busiest pair: est. tensor us, issued\n";
+  for (const TcDir& dr : tc_directions(d)) {
+    Tc2Plan plan;
+    if (tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan)) return -1;
+    char line[200];
+    snprintf(line, sizeof line, "%s | %d | %lld | %lld | %.1f\n", dr.name.c_str(), plan.maxb, plan.n_issued * plan.ksub,
+             (plan.n_mma - plan.n_issued) * plan.ksub, plan.op_ns_issued_max / 1e3);
+    out += line;
+  }
+  const int n = (int)std::min(out.size(), (size_t)buf_len - 1);
+  memcpy(buf, out.data(), (size_t)n);
+  buf[n] = 0;
+  return n;
 }
 
 // Host-only aid (not in the public header): the widths a handle for `d` stores - out[0..4) = latent, 4 * net_dim,

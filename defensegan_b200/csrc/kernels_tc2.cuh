@@ -13,8 +13,10 @@
 //     gives up registers (setmaxnreg) so that the consumers can hold accumulators and epilogue without spilling.  Each
 //     consumer warpgroup owns 64 of the tile's 128 rows and issues wgmma.mma_async (M = 64, K = 16) into register
 //     accumulators - up to 256 columns: the 1-8 accumulators of the item's window.  A step is a run-time number of
-//     rounds, and a round is one MMA into EVERY accumulator in compile-time order, so the compiler never has to choose
-//     an accumulator at run time (an accumulator with nothing to add in a round reads an all-zero weight tile).  One
+//     rounds, and a round is one op per accumulator with something to add, in compile-time order: the consumers branch
+//     on the round's active set to a straight-line variant, so the compiler never has to choose an accumulator at run
+//     time (the 8-slot and the narrow instantiations issue into every accumulator, and one with nothing to add reads
+//     an all-zero weight tile).  One
 //     wgmma group is committed per round and one stays in flight, across step boundaries too; a step's ring region is
 //     released once the NEXT step's first round is issued and every earlier group has retired; after the item's last
 //     step the consumer waits for all MMAs and runs the epilogue straight from the registers.  Each consumer warp
@@ -76,9 +78,16 @@ __host__ __device__ constexpr int tc2_ksub(int K) { return K % 64 == 0 ? 4 : K /
 // Staged bytes of one A tile (128 rows) and one weight tile (N rows) of an op.
 __host__ __device__ constexpr int tc2_a_bytes(int ksub) { return 128 * 32 * ksub; }
 __host__ __device__ constexpr int tc2_b_bytes(int n_tile, int ksub) { return n_tile * 32 * ksub; }
-// The all-zero weight tile read by the MMAs of an accumulator with nothing to add in a round (instantiations with more
-// than one accumulator per round).  It sits right after the ring, has the shape of a weight tile and is written once
-// per CTA.
+// Does an instantiation with `maxb` accumulator slots and `ksub` k16 MMAs per op issue zero-tile ops?  With 2 or 4
+// slots and 64-channel ops, a round issues only its real ops: the consumers branch on the round's active set to one of
+// at most 15 straight-line variants (tc2_mma_round).  The others keep the fixed round, in which an accumulator with
+// nothing to add reads the zero tile: the 8-slot instantiations (N = 16), and the narrow ones (the last layer's
+// backward, 1 or 3 k16 MMAs per op), where the dispatch measured slower than the zero-tile MMAs it saves.
+__host__ __device__ constexpr bool tc2_issues_zero_ops(int maxb, int ksub) { return maxb > 4 || (maxb > 1 && ksub < 4); }
+// The all-zero weight tile read by the zero-tile ops of the instantiations that issue them.  It sits right after the
+// ring, has the shape of a weight tile and is written once per CTA.  The instantiations that skip zero-tile ops keep
+// its space too: the ring size caps the step size (tc2_search), so dropping it would move the plans, and the time
+// model's constants were fitted to these rings.
 __host__ __device__ constexpr int tc2_zero_bytes(int n_tile, int maxb, int ksub) { return maxb > 1 ? tc2_b_bytes(n_tile, ksub) : 0; }
 __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int ksub, int epi, int out_bytes) {
   const int epi_b = tc2_epi_tiles(n_tile, epi, out_bytes) * TC2_TILE_BYTES;
@@ -86,9 +95,10 @@ __host__ __device__ constexpr int tc2_ring_bytes(int n_tile, int maxb, int ksub,
   return raw > TC2_RING_MAX_KB * 1024 ? TC2_RING_MAX_KB * 1024 : raw;
 }
 
-// MAXB_: accumulator slots of the instantiation = MMAs per round = the most accumulators a window may have.  Fewer slots
-// than fit the 256 accumulator columns issue fewer zero-tile MMAs but allow only smaller windows (more staged bytes);
-// the planner weighs the two (tc2_plan).
+// MAXB_: accumulator slots of the instantiation = the most ops per round = the most accumulators a window may have.
+// With 2 or 4 slots and 64-channel ops a round issues only its real ops.  Where the round is fixed (8 slots, narrow
+// ops), fewer slots issue fewer zero-tile MMAs but allow only smaller windows (more staged bytes), and the planner
+// weighs the two (tc2_plan).
 // KSUB_: k16 MMAs per op (tc2_ksub).  4: A and weight tiles are 64-channel 128B-swizzled boxes and the op's k16 step
 // through each 128 B row.  1..3: each tile is KSUB sub-tiles of 16 channels (32 B rows, 32B swizzle), one per k16, so a
 // narrow K stages and multiplies only its real channels.
@@ -235,25 +245,63 @@ __device__ __forceinline__ int tc2_item_at(const int* __restrict__ order, int k,
   return k < n_slots ? __ldg(order + (size_t)k * n_pairs + pair) : -1;
 }
 
-// One round of a step: for every accumulator a, in compile-time order, the KSUB k16 MMAs of one op (a 64-channel
-// k-chunk, or a narrow operand's 16-channel sub-tiles).  Only the operand descriptors and the overwrite predicate come
-// from the record byte of (round, a), so the sequence of wgmma instructions and the registers they name are fixed.
+// The ops of one round into the accumulators of the set MASK (bit a = accumulator a), in compile-time order: for each,
+// the KSUB k16 MMAs of one op (a 64-channel k-chunk, or a narrow operand's 16-channel sub-tiles).  Only the operand
+// descriptors and the overwrite predicate come from the record byte of (round, a), so the sequence of wgmma
+// instructions and the registers they name are fixed.
 //   da0 / db0: descriptors of the step's first A tile (this warpgroup's rows) and first B slot; zoff: the zero tile's
-//   distance from db0 in 16-byte units.
-template <int NT, int MAXB, int KSUB, int NREG>
-__device__ __forceinline__ void tc2_mma_round(float (&acc)[NREG], const uint32_t (&q)[6], uint64_t da0, uint64_t db0, uint32_t zoff) {
+//   distance from db0 in 16-byte units (instantiations that issue zero-tile ops).
+template <int NT, int MAXB, int KSUB, uint32_t MASK, int NREG>
+__device__ __forceinline__ void tc2_mma_ops(float (&acc)[NREG], const uint32_t (&q)[6], uint64_t da0, uint64_t db0, uint32_t zoff) {
   // the next k16: 32 B further along the 128 B row of a 128B-swizzled tile, or the next 16-channel sub-tile
   constexpr uint32_t DA_K = KSUB == 4 ? 2u : (uint32_t)(128 * 32 >> 4), DB_K = KSUB == 4 ? 2u : (uint32_t)(NT * 32 >> 4);
 #pragma unroll
   for (int a = 0; a < MAXB; ++a) {
+    if (!((MASK >> a) & 1u)) continue;
     const uint32_t e = TcMmaRec::Ops::get(q[a / TcMmaRec::Ops::PER_WORD], a);
     const uint32_t bs = TcOp::Slot::get(e);
     // descriptors differ only in the 14-bit start-address field (smem < 256 KB, no carry)
     const uint64_t da = da0 + (uint64_t)(TcOp::A::get(e) * (uint32_t)(tc2_a_bytes(KSUB) >> 4));
-    const uint64_t db = db0 + (uint64_t)(bs == (uint32_t)TC2_ZERO_SLOT ? zoff : bs * (uint32_t)(tc2_b_bytes(NT, KSUB) >> 4));
+    const uint32_t boff = bs * (uint32_t)(tc2_b_bytes(NT, KSUB) >> 4);
+    const uint64_t db = db0 + (uint64_t)(tc2_issues_zero_ops(MAXB, KSUB) && bs == (uint32_t)TC2_ZERO_SLOT ? zoff : boff);
     const uint32_t keep = TcOp::First::get(e) ^ 1u;  // 0: first MMA into the accumulator, overwrite it
 #pragma unroll
     for (int k = 0; k < KSUB; ++k) ptx::Wgmma<NT>::mma(acc + a * (NT / 2), da + DA_K * k, db + DB_K * k, k > 0 ? 1u : keep);
+  }
+  // in the variant itself: a commit where the variants' paths join would close a hardware group of its own, an empty
+  // HGMMA
+  ptx::wgmma_commit();
+}
+
+// One round of a step, committed as one wgmma group.  Where the instantiation issues zero-tile ops
+// (tc2_issues_zero_ops): one op into every accumulator (a slot with nothing to add reads the zero tile).  Otherwise only
+// the round's real ops.  The round's active set - the accumulators whose op byte names a B slot, not the zero tile - is
+// the same in every thread of the warpgroup (it comes from the step's record), and the branch on it leads to a
+// straight-line variant per set.  A guard predicate per MMA would instead make ptxas branch around every
+// HGMMA and close a hardware wgmma group at each, so that the round's wait_group 1 would drain the pipe.  The plan
+// validator rejects a round without a real op (it would commit an empty group).
+template <int NT, int MAXB, int KSUB, int NREG>
+__device__ __forceinline__ void tc2_mma_round(float (&acc)[NREG], const uint32_t (&q)[6], uint64_t da0, uint64_t db0, uint32_t zoff) {
+  if constexpr (tc2_issues_zero_ops(MAXB, KSUB) || MAXB == 1) {
+    tc2_mma_ops<NT, MAXB, KSUB, (1u << MAXB) - 1u>(acc, q, da0, db0, zoff);
+  } else {
+    static_assert(MAXB <= TcMmaRec::Ops::PER_WORD, "a round's op bytes share the queue's first word");
+    uint32_t set = 0;
+#pragma unroll
+    for (int a = 0; a < MAXB; ++a)
+      set |= (TcOp::Slot::get(TcMmaRec::Ops::get(q[0], a)) != (uint32_t)TC2_ZERO_SLOT ? 1u : 0u) << a;
+    switch (set) {
+#define TC2_ROUND_VARIANT(M) \
+  case M:                    \
+    if constexpr (M < (1u << MAXB)) tc2_mma_ops<NT, MAXB, KSUB, M>(acc, q, da0, db0, zoff); \
+    break;
+      TC2_ROUND_VARIANT(1u) TC2_ROUND_VARIANT(2u) TC2_ROUND_VARIANT(3u) TC2_ROUND_VARIANT(4u) TC2_ROUND_VARIANT(5u)
+      TC2_ROUND_VARIANT(6u) TC2_ROUND_VARIANT(7u) TC2_ROUND_VARIANT(8u) TC2_ROUND_VARIANT(9u) TC2_ROUND_VARIANT(10u)
+      TC2_ROUND_VARIANT(11u) TC2_ROUND_VARIANT(12u) TC2_ROUND_VARIANT(13u) TC2_ROUND_VARIANT(14u) TC2_ROUND_VARIANT(15u)
+#undef TC2_ROUND_VARIANT
+      // an empty set (rejected by the validator) would commit a group without an MMA: ptxas would add an empty HGMMA
+      default: __builtin_unreachable();
+    }
   }
 }
 
@@ -355,7 +403,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       ptx::fence_barrier_init();
     }
   }
-  if constexpr (Cfg::ZERO_BYTES > 0) {
+  if constexpr (Cfg::ZERO_BYTES > 0 && tc2_issues_zero_ops(MAXB, KSUB)) {    // only where zero-tile ops read it
     if (threadIdx.x < TC2_CONSUMERS) {
       for (uint32_t i = threadIdx.x; i < (uint32_t)Cfg::ZERO_BYTES / 16u; i += TC2_CONSUMERS) ptx::st_shared_v4(zero_base + 16u * i, 0u, 0u, 0u, 0u);
       ptx::fence_proxy_async_smem();           // the MMAs read it through the async proxy
@@ -499,9 +547,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         // iteration of this run-time loop whatever the commits say, so a single commit per step would make its wait
         // drain the whole step and idle the tensor pipe at every step boundary.
         for (int r = 0; r < n_rounds; ++r) {
-          tc2_mma_round<N_TILE, Cfg::MAXB, KSUB>(acc, q, da0, db0, zoff);
+          tc2_mma_round<N_TILE, Cfg::MAXB, KSUB>(acc, q, da0, db0, zoff);    // commits the round's group
           tc2_pop_round<Cfg::MAXB>(q);
-          ptx::wgmma_commit();
 #ifdef DGAN_PROBE
           const long long probe_c0 = clock64();
 #endif
@@ -829,14 +876,17 @@ struct Tc2HostItem {
   TcItem2 hdr{};
   std::vector<Tc2HostStep> steps;
   double stage_bytes = 0.0;
-  long long n_ops = 0;         // ops issued (rounds x slots, KSUB k16 MMAs each), zero-tile ones included
+  long long n_ops = 0;         // ops of the rounds' slots (rounds x slots, KSUB k16 MMAs each): what the time model charges
+  long long n_issued = 0;      // ops the kernel issues: the real ones, and the zero-tile ones where the instantiation
+                               // issues them (tc2_issues_zero_ops)
 };
 
 // Steps of one window (accumulator a <-> output pixel qs[a]).  Input pixels are taken in ascending order and packed
 // greedily into steps of <= max_a A tiles (max_a = 1: one input pixel per step); a weight tile needed by several
-// pixels of a step is staged once.  The kernel issues a step as rounds of max_b MMAs, one per accumulator slot of the
+// pixels of a step is staged once.  The kernel issues a step as rounds over the max_b accumulator slots of the
 // instantiation: an accumulator's r-th contribution in the step (pixel order) goes to round r, and a slot with nothing
-// to add in a round - or beyond the window's accumulators - reads the zero tile.
+// to add in a round - or beyond the window's accumulators - holds a zero-tile op, which only the fixed-round
+// instantiations issue (tc2_issues_zero_ops).
 static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int N, int K, int max_b, int max_a,
                            int step_max_bytes, Tc2HostItem* out) {
   const int ksub = tc2_ksub(K), kch = K / (16 * ksub), a_bytes = tc2_a_bytes(ksub), b_tile = tc2_b_bytes(N, ksub);
@@ -943,7 +993,12 @@ static void tc2_build_item(const PairTable& tab, const std::vector<int>& qs, int
     }
   out->stage_bytes = 0.0;
   out->n_ops = 0;
-  for (auto& stp : out->steps) { out->stage_bytes += stp.bytes; out->n_ops += (long long)stp.n_rounds * max_b; }
+  out->n_issued = 0;
+  for (auto& stp : out->steps) {
+    out->stage_bytes += stp.bytes;
+    out->n_ops += (long long)stp.n_rounds * max_b;
+    out->n_issued += tc2_issues_zero_ops(max_b, ksub) ? (long long)stp.n_rounds * max_b : (long long)stp.n_real;
+  }
 }
 
 // Windows of wh x ww accumulators with strides (sy, sx) over the output grid.  Stride 2 gathers outputs of equal
@@ -1006,9 +1061,12 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   std::vector<TcRec> stream_p, stream_m;
   std::vector<uint32_t> stream_off;
   std::vector<int> eitems;
-  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;   // ops issued (KSUB k16 MMAs each), those reading the zero tile
+  // ops of the rounds' slots (rounds x slots, KSUB k16 MMAs each), the zero-tile ones among them, ops issued (the real
+  // ones, and the zero-tile ones where the instantiation issues them)
+  long long n_mma = 0, n_pad = 0, n_issued = 0, n_steps = 0, n_bytes = 0;
   double load_max = 0.0, load_mean = 0.0;   // cost-model load of the busiest CTA pair / the mean over pairs (balance of the LPT assignment)
   double op_ns_max = 0.0;      // the MMA term of the busiest pair's load (estimated tensor time, ns)
+  double op_ns_issued_max = 0.0;   // the same term for the ops the kernel issues (n_issued)
   int maxb = 1, ring_bytes = 0;   // accumulator slots per round of the chosen instantiation, its operand ring
   int ksub = 4;                   // k16 MMAs per op of the instantiation (tc2_ksub)
 };
@@ -1019,8 +1077,9 @@ static double tc2_op_ns(int N, int ksub) {
 
 // Every candidate - an instantiation of TC2_KINDS for (N, epilogue, output type) and a shape of wh x ww <= its slots
 // accumulators, strides 1 or 2 - is scored by an LPT assignment of its items (window, row pair) to the CTA pairs with
-// the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed per-item charge, and the MMAs
-// issued, zero-tile ones included); the smallest makespan wins.  Fills the plan's shape, slots, ring and loads, and
+// the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed per-item charge, and the ops
+// of the rounds' slots, zero-tile ones included even where the kernel skips them: the constants were fitted to kernels
+// that issued them); the smallest makespan wins.  Fills the plan's shape, slots, ring and loads, and
 // returns the winner's items and, per CTA pair, its item indices (window * n_mpairs + row pair) in issue order.
 // force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
 static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
@@ -1123,9 +1182,13 @@ static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid
               plan->shape[0] = wh; plan->shape[1] = ww; plan->shape[2] = sy; plan->shape[3] = sx;
               plan->maxb = mb; plan->ring_bytes = ring;
               plan->op_ns_max = 0.0;
+              plan->op_ns_issued_max = 0.0;
               for (size_t pr = 0; pr < lists.size(); ++pr)
                 if (load[pr] == makespan) {
-                  for (int idx : lists[pr]) plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
+                  for (int idx : lists[pr]) {
+                    plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
+                    plan->op_ns_issued_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_issued;
+                  }
                   break;
                 }
               best_items->swap(items); best_lists->swap(lists);
@@ -1154,7 +1217,7 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
   std::vector<TcRec>& stream_p = plan->stream_p;
   std::vector<TcRec>& stream_m = plan->stream_m;
   stream_p.clear(); stream_m.clear();
-  long long n_mma = 0, n_pad = 0, n_steps = 0, n_bytes = 0;
+  long long n_mma = 0, n_pad = 0, n_issued = 0, n_steps = 0, n_bytes = 0;
   for (size_t pr = 0; pr < lists.size(); ++pr) {
     stream_off[pr] = (uint32_t)stream_m.size();
     // circular operand ring of this CTA pair: sequential allocation, wrap when the step does not fit
@@ -1194,6 +1257,7 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
         stream_p.push_back(p.encode());
         // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
         n_mma += hs.n_rounds * max_b; n_pad += hs.n_rounds * max_b - hs.n_real;
+        n_issued += tc2_issues_zero_ops(max_b, ksub) ? hs.n_rounds * max_b : hs.n_real;
         n_steps += 1; n_bytes += 2LL * hs.nA * tc2_a_bytes(ksub) + (long long)hs.nB * tc2_b_bytes(N, ksub);
       }
     }
@@ -1201,7 +1265,7 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
   stream_off[(size_t)n_pairs] = (uint32_t)stream_m.size();
   plan->hdrs.resize(items.size());
   for (size_t i = 0; i < items.size(); ++i) plan->hdrs[i] = items[i].hdr;
-  plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
+  plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_issued = n_issued; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
   return 0;
 }
 
@@ -1222,7 +1286,8 @@ static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, 
 //  * the first MMA into an accumulator - and only that one - overwrites it;
 //  * every accumulator sums in the canonical order (k-chunk major, input pixel ascending): results then do not
 //    depend on the schedule (batch-size / sharding invariance);
-//  * an op that reads the zero tile never overwrites its accumulator;
+//  * an op that reads the zero tile never overwrites its accumulator, and every round has a real op (the kernel
+//    commits one wgmma group per round);
 //  * ring safety: when a step's loads may start (step k - dep consumed), no earlier step that can still be read
 //    overlaps its region, regions stay inside the ring, dep <= number of barrier slots;
 //  * progress: a step's region is released only once the next step's first round is issued (unless it ends its item), so
@@ -1294,12 +1359,17 @@ static int tc2_check_plan(int N, int K, const PairTable& tab, int n_mpairs, int 
       const TcItem2& hdr = pl.hdrs[win];
       // the kernel issues round by round, accumulator 0 .. max_acc - 1 within a round
       for (int oi = 0; oi < n_rounds * max_acc; ++oi) {
+        if (oi % max_acc == 0) {
+          int real = 0;
+          for (int a = 0; a < max_acc; ++a) real += TcOp::decode(m.ops[oi + a]).slot != (uint32_t)TC2_ZERO_SLOT;
+          if (real == 0) return fail("round without a real op (it would commit an empty wgmma group)");
+        }
         const TcOp op = TcOp::decode(m.ops[oi]);
         const int a_idx = (int)op.a, slot = (int)op.slot, acc = oi % max_acc;
         const bool first = op.first != 0;
         if (m.ops[oi] & ~TcOp::USED) return fail("op field out of range");
         if (slot == TC2_ZERO_SLOT) {
-          if (max_acc == 1) return fail("zero-tile op in an instantiation without a zero tile");
+          // skipped by the instantiations that do not issue zero-tile ops; a zero-tile op never carries First either way
           if (first) return fail("zero-tile op overwrites its accumulator");
           continue;
         }

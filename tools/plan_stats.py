@@ -2,8 +2,11 @@
 Usage: python tools/plan_stats.py [mnist|celeba] [batch] [R] [CTA pairs] [library] [--slots DIR=MAXB] [--window DIR=WH,WW,SY,SX]
                                  [--latent_dim N] [--net_dim N] [--use_bn]
 --latent_dim / --net_dim / --use_bn plan that generator (default 128 / 64 / no BN); the handle pads each width (see
-DESIGN.md section 2), and the last two columns show the share of each direction's k16 MMAs that multiply real channels
-and its steps per CTA pair (what each consumer warp pays a fixed per-step cost for);
+DESIGN.md section 2), and the next two columns show the share of each direction's k16 MMAs that multiply real channels
+and its steps per CTA pair (what each consumer warp pays a fixed per-step cost for).  The MMA columns of the table count
+every slot of every round, as the planner's time model does; the last three (default plans only, no --slots or --window)
+give what the kernel issues: the k16 MMAs issued, the zero-tile k16 MMAs it skips (rounds with 2 or 4 slots and
+64-channel ops issue only their real ops) and the busiest pair's estimated tensor time for the MMAs issued;
 --slots plans layer-direction DIR (the row index of the table, from 0) with exactly MAXB accumulator slots per round;
 --window plans it on exactly the window WH x WW with strides (SY, SX), e.g. to compare two builds at the same window."""
 import ctypes
@@ -58,7 +61,17 @@ real = {"Linear.fwd": (4 * nd, latent), "Linear.bwd": (latent, 4 * nd), "Generat
         "Generator.2.bwd": (4 * nd, 2 * nd), "Generator.3.fwd": (nd, 2 * nd), "Generator.3.bwd": (2 * nd, nd),
         "Generator.5.fwd": (nd, nd), "Generator.5.bwd": (nd, nd), "last.fwd": (img, nd), "last.bwd": (nd, img)}
 lines = buf.value.decode().strip().splitlines()
-out = [lines[0] + " | real k16 MMAs (share) | steps per CTA pair"]
+issue = {}
+if window is None and force_dir < 0:
+    ibuf = ctypes.create_string_buffer(1 << 16)
+    lib.dgan_debug_plan_issue_stats.restype = ctypes.c_int
+    lib.dgan_debug_plan_issue_stats.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
+    if lib.dgan_debug_plan_issue_stats(ctypes.byref(desc), batch * R, pairs, ibuf, len(ibuf)) > 0:
+        for row in ibuf.value.decode().strip().splitlines()[1:]:
+            col = row.split(" | ")
+            issue[col[0]] = " | ".join(col[2:])
+out = [lines[0] + " | real k16 MMAs (share) | steps per CTA pair" +
+       (" | k16 MMAs issued | zero-tile k16 MMAs skipped | busiest pair: est. tensor us, issued" if issue else "")]
 for line in lines[1:-1]:
     col = line.split(" | ")
     name, n, k = col[0], int(col[1]), int(col[2])
@@ -67,6 +80,7 @@ for line in lines[1:-1]:
         a, b = (int(v) for v in name[name.index("[") + 1:-1].split(":"))
         rn = max(0, min(b, rn) - a)
     share = min(rn, n) * min(rk, k) / (n * k)
-    out.append(line + " | %d (%.2f) | %.1f" % (round(int(col[14]) * share), share, int(col[6]) / pairs))
+    out.append(line + " | %d (%.2f) | %.1f" % (round(int(col[14]) * share), share, int(col[6]) / pairs) +
+               (" | " + issue[name] if name in issue else ""))
 out.append(lines[-1])
 print("\n".join(out))
