@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "dgan_last_launch_count", "dgan_last_enqueue_count", "dgan_macs_per_row", "dgan_profile_enable", "dgan_profile_num_kinds",
     "dgan_profile_kind_name", "dgan_profile_read",
     "dgan_workspace_bytes_weighted", "dgan_reconstruct_weighted", "dgan_loss_grad_weighted",
+    "dgan_workspace_bytes_measured", "dgan_reconstruct_measured", "dgan_loss_grad_measured",
 ]
 
 
@@ -131,6 +132,12 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_weighted.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_loss_grad_weighted.restype = i32
     lib.dgan_loss_grad_weighted.argtypes = [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_workspace_bytes_measured.restype = sz
+    lib.dgan_workspace_bytes_measured.argtypes = [vp, i32, i32, i32]
+    lib.dgan_reconstruct_measured.restype = i32
+    lib.dgan_reconstruct_measured.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_measured.restype = i32
+    lib.dgan_loss_grad_measured.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -227,9 +234,12 @@ class NativeGenerator:
             pass
 
     # -- helpers -------------------------------------------------------------------------
-    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False):
-        sizer = self.lib.dgan_workspace_bytes_weighted if weighted else self.lib.dgan_workspace_bytes
-        need = int(sizer(self._handle, batch, rec_rr))
+    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0):
+        if m > 0:
+            need = int(self.lib.dgan_workspace_bytes_measured(self._handle, batch, rec_rr, int(m)))
+        else:
+            sizer = self.lib.dgan_workspace_bytes_weighted if weighted else self.lib.dgan_workspace_bytes
+            need = int(sizer(self._handle, batch, rec_rr))
         if need == 0:
             raise RuntimeError("dgan_workspace_bytes returned 0 (invalid batch / rec_rr)")
         if self._ws is None or self._ws.numel() < need + 1024:
@@ -311,6 +321,70 @@ class NativeGenerator:
         if return_aux:
             return rec, loss, idx
         return rec
+
+    def _measured(self, measurements: torch.Tensor, operator: torch.Tensor):
+        """(y, A, batch, m): the measurements as a contiguous CUDA float32 [batch, m] tensor and the operator as [m, H*W*C]
+        (shapes only; the values are not checked here - DefenseGANBase.reconstruct_measured does)."""
+        a = _require_cuda_f32(operator, "operator")
+        y = _require_cuda_f32(measurements, "measurements")
+        if a.dim() != 2 or a.shape[1] != self.hwc or not 1 <= a.shape[0] <= self.hwc:
+            raise ValueError("operator must be [m, %d] with 1 <= m <= %d, got %s" % (self.hwc, self.hwc, tuple(a.shape)))
+        m = a.shape[0]
+        if y.dim() != 2 or y.shape[1] != m or y.shape[0] <= 0:
+            raise ValueError("measurements must be [B, %d] (the operator's m), got %s" % (m, tuple(y.shape)))
+        return y, a, y.shape[0], m
+
+    def reconstruct_measured(self, measurements: torch.Tensor, operator: torch.Tensor, rec_rr: int, rec_iters: int,
+                             rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
+                             momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
+                             return_aux: bool = False, z_row_offset: int = 0):
+        """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
+        [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
+        restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
+        the arg-min restart as [B, H, W, C] (with return_aux also the minimum measured loss [B] and the restart [B])."""
+        y, a, batch, m = self._measured(measurements, operator)
+        if rec_rr <= 0 or rec_iters <= 0:
+            raise ValueError("rec_rr and rec_iters must be positive")
+        z0 = None
+        if z_init_val is not None:
+            z0 = _require_cuda_f32(z_init_val, "z_init_val")
+            if z0.numel() != batch * rec_rr * self.latent_dim:
+                raise ValueError("z_init_val must be [B*rec_rr, latent_dim]")
+        with torch.cuda.device(self.device):
+            rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
+            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
+                raise ValueError("out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements" % self.image_dim)
+            loss = torch.empty(batch, dtype=torch.float32, device=self.device)
+            idx = torch.empty(batch, dtype=torch.int32, device=self.device)
+            ws, need = self._workspace(batch, rec_rr, m=m)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
+                                  seed & (2 ** 64 - 1), int(z_row_offset))
+            rc = self.lib.dgan_reconstruct_measured(self._handle, ctypes.byref(prm), _ptr(a), m, _ptr(y), _ptr(z0),
+                                                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+            _check(self.lib, rc, "dgan_reconstruct_measured")
+        if return_aux:
+            return rec, loss, idx
+        return rec
+
+    def loss_grad_measured(self, measurements: torch.Tensor, operator: torch.Tensor, z: torch.Tensor, rec_rr: int):
+        """(G(z), per-row measured loss, d(sum loss)/dz) at z [B*rec_rr, latent] for measurements [B, m] through operator
+        [m, H*W*C]: one evaluation of reconstruct_measured's loop body (dgan_loss_grad_measured)."""
+        y, a, batch, m = self._measured(measurements, operator)
+        zc = _require_cuda_f32(z, "z")
+        n = batch * rec_rr
+        if zc.shape[0] != n:
+            raise ValueError("z must have batch*rec_rr rows")
+        with torch.cuda.device(self.device):
+            g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
+            loss = torch.empty(n, dtype=torch.float32, device=self.device)
+            grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
+            ws, need = self._workspace(batch, rec_rr, m=m)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _check(self.lib, self.lib.dgan_loss_grad_measured(self._handle, _ptr(a), m, _ptr(y), batch, rec_rr, _ptr(zc),
+                                                              _ptr(g), _ptr(loss), _ptr(grad), ws, need,
+                                                              ctypes.c_void_p(stream)), "dgan_loss_grad_measured")
+        return g, loss, grad
 
     def sample_z0(self, n_rows: int, seed: int, z_row_offset: int = 0) -> torch.Tensor:
         """Rows [z_row_offset, z_row_offset + n_rows) of the N(0, 1/latent_dim) Philox stream `seed` - the z0 that

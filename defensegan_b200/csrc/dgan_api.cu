@@ -14,6 +14,7 @@
 #include "kernels_tc.cuh"
 #include "kernels_tc2.cuh"
 #include "kernels_vjp.cuh"
+#include "kernels_measured.cuh"
 
 namespace dgan {
 
@@ -317,9 +318,10 @@ struct dgan_ctx {
   bool profile = false;
   int n_rows_cur = 0;
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
-  // weighted) on a private stream, replayed with one cudaGraphLaunch per call.
+  // weighted, measured: the m of a measured call, 0 otherwise) on a private stream, replayed with one cudaGraphLaunch per
+  // call.
   struct LoopGraph {
-    const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted; float rec_lr, momentum;
+    const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured; float rec_lr, momentum;
     cudaGraphExec_t exec; int64_t kernels;
   };
   std::vector<LoopGraph> graphs;
@@ -429,13 +431,23 @@ struct Workspace {
   float* loss = nullptr;               // [n_pad] per-row loss; dgan_vjp (which computes no loss) keeps its row scales here
   float* x = nullptr;                  // [batch][H*W*C] copy of the call's images (the captured loop reads them from here)
   float* xw = nullptr;                 // weighted workspaces: [batch][H*W*C] copy of the call's per-pixel weights
+  // measured workspaces (m > 0; kernels_measured.cuh): the call's operator A [m_ld][H*W*C], its transpose At [H*W*C][m_ld]
+  // and measurements y [batch][m_ld], zero-padded to m_ld columns; the residuals r [n_pad][m_ld], dy = (2/m) At r
+  // [n_pad][H*W*C], the measured loss's parts [m_ld / 64][n_pad] and the cotangent's row scales [n_pad] (fp16 path)
+  int m = 0, m_ld = 0;
+  float *am = nullptr, *amt = nullptr, *ym = nullptr, *r = nullptr, *dym = nullptr, *mloss_part = nullptr, *mscale = nullptr;
   size_t bytes = 0;
 };
 
+// The padded measurement count of a measured workspace: m rounded up to the measurement products' N tile.
+static int measured_ld(int m) { return (int)align_up((size_t)m, kMeasTileN); }
+
 // The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer - name, element type, byte
 // offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.  weighted: the workspace of the
-// weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.
-static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false) {
+// weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.  m > 0: the workspace of
+// the measured entries for m measurements, the same buffers at the same offsets and the measured ones after all of them.
+static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
+                       int m = 0) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -512,6 +524,18 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
   else w.loss_part = (float*)take("loss_part", "f32", {np, (size_t)w.n_loss_parts});
   w.loss = (float*)take("loss", "f32", {np});
   if (weighted) w.xw = (float*)take("xw", "f32", {np, hwc});   // batch <= n_pad
+  if (m > 0) {
+    w.m = m;
+    w.m_ld = measured_ld(m);
+    const size_t mld = (size_t)w.m_ld;
+    w.am = (float*)take("am", "f32", {mld, hwc});
+    w.amt = (float*)take("amt", "f32", {hwc, mld});
+    w.ym = (float*)take("ym", "f32", {np, mld});            // batch <= n_pad
+    w.r = (float*)take("r", "f32", {np, mld});
+    w.dym = (float*)take("dym", "f32", {np, hwc});
+    w.mloss_part = (float*)take("mloss_part", "f32", {mld / kMeasTileN, np});
+    w.mscale = (float*)take("mscale", "f32", {np});
+  }
   w.bytes = off;
   return w;
 }
@@ -881,17 +905,19 @@ static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t
 
 // ---- a caller's cotangent dy [n_rows][H*W*C] -> the last layer's d(pre), after a forward that wrote w.y ----------
 // fp16 path: per-row power-of-two scales (one shared scale with BatchNorm) in w.loss, d(pre) * scale in w.dblk;
-// fp32 path: d(pre) unscaled in w.dpre.  See kernels_vjp.cuh.
-static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cudaStream_t s) {
+// fp32 path: d(pre) unscaled in w.dpre.  See kernels_vjp.cuh.  scale: where the fp16 path keeps the row scales (NULL:
+// w.loss).
+static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cudaStream_t s, float* scale = nullptr) {
+  if (scale == nullptr) scale = w.loss;
   const FinalLayer& f = c->fin;
   const bool tc = c->desc.precision == DGAN_PREC_FP16;
   const bool sigmoid = f.C_out == 1 && f.act == ACT_SIGMOID;
   if (!sigmoid && !(f.C_out == 3 && f.act == ACT_TANH)) { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
   if (tc) {
-    if (sigmoid) cotangent_rowmax_kernel<ACT_SIGMOID><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
-    else cotangent_rowmax_kernel<ACT_TANH><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, w.loss);
+    if (sigmoid) cotangent_rowmax_kernel<ACT_SIGMOID><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, scale);
+    else cotangent_rowmax_kernel<ACT_TANH><<<w.n_rows, 256, 0, s>>>(w.y, dy, c->hwc, scale);
     DGAN_LAUNCH_CHECK(c);
-    cotangent_scale_kernel<<<1, 1024, 0, s>>>(w.loss, w.n_rows, c->desc.use_bn ? 1 : 0, 4);
+    cotangent_scale_kernel<<<1, 1024, 0, s>>>(scale, w.n_rows, c->desc.use_bn ? 1 : 0, 4);
     DGAN_LAUNCH_CHECK(c);
   }
   if (tc && w.n_pad > w.n_rows) {
@@ -904,10 +930,63 @@ static int launch_cotangent(dgan_ctx* c, const Workspace& w, const float* dy, cu
   const size_t total = (size_t)w.n_rows * c->hwc;
   const unsigned grid = (unsigned)((total + 255) / 256);
   const int w_out = 2 * f.w_in;
-#define CT(ACT, CO, BLK) cotangent_kernel<ACT, CO, BLK><<<grid, 256, 0, s>>>(w.y, dy, w.n_rows, w_out, w.loss, w.dpre, w.dblk, w.n_pad)
+#define CT(ACT, CO, BLK) cotangent_kernel<ACT, CO, BLK><<<grid, 256, 0, s>>>(w.y, dy, w.n_rows, w_out, scale, w.dpre, w.dblk, w.n_pad)
   if (sigmoid) { if (tc) CT(ACT_SIGMOID, 1, true); else CT(ACT_SIGMOID, 1, false); }
   else { if (tc) CT(ACT_TANH, 3, true); else CT(ACT_TANH, 3, false); }
 #undef CT
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// ---- the measured loss (dgan_reconstruct_measured; kernels_measured.cuh) ----------------------------------------------
+// Copy a call's operator a [m][H*W*C] and measurements y [batch][m] into the measured workspace w: A with m_ld - m zero
+// rows, its transpose, y with m_ld - m zero columns.  The measured loop then reads only the workspace.
+static int stage_measured(dgan_ctx* c, const Workspace& w, const float* a, const float* y, int batch, cudaStream_t s) {
+  const int hwc = c->hwc;
+  const size_t na = (size_t)w.m_ld * hwc, ny = (size_t)batch * w.m_ld;
+  pad_copy_kernel<<<(unsigned)((na + 255) / 256), 256, 0, s>>>(a, w.am, w.m, 1, hwc, w.m_ld, 1, hwc);
+  DGAN_LAUNCH_CHECK(c);
+  transpose_tiles_kernel<<<(unsigned)((na + 255) / 256), 256, 0, s>>>(w.am, w.amt, w.m_ld, hwc, na);
+  DGAN_LAUNCH_CHECK(c);
+  pad_copy_kernel<<<(unsigned)((ny + 255) / 256), 256, 0, s>>>(y, w.ym, batch, 1, w.m, batch, 1, w.m_ld);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// out = EPI(s_ * X W^T) over the real latent rows: TF32 tensor cores on the fp16 path, fp32 FFMA on the fp32 path
+template <int EPI>
+static int launch_measured_gemm(dgan_ctx* c, const Workspace& w, const float* X, int ldx, const float* W, int ldw, int N,
+                                int K, float* out, int ldo, const float* ym, int R, float s_, float* loss_part, cudaStream_t s) {
+  const dim3 grid((unsigned)((w.n_rows + kMeasTileM - 1) / kMeasTileM), (unsigned)((N + kMeasTileN - 1) / kMeasTileN));
+  if (c->desc.precision == DGAN_PREC_FP16)
+    measured_gemm_kernel<true, EPI><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
+  else
+    measured_gemm_kernel<false, EPI><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.
+static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  return launch_measured_gemm<MEAS_RESID>(c, w, w.y, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R, 1.f,
+                                          w.mloss_part, s);
+}
+
+// The rest of a measured step's gradient after launch_measure: dy = (2/m) At r, then the cotangent entry of dgan_vjp (its
+// fp16 row scales in w.mscale: w.loss carries the loss to the select) and the backward-to-z into w.g.
+static int measured_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  int rc;
+  if ((rc = launch_measured_gemm<MEAS_SCALE>(c, w, w.r, w.m_ld, w.amt, w.m_ld, c->hwc, w.m_ld, w.dym, c->hwc, nullptr, 1,
+                                             2.f / (float)w.m, nullptr, s)))
+    return rc;
+  if ((rc = launch_cotangent(c, w, w.dym, s, w.mscale))) return rc;
+  return run_backward(c, w, s);
+}
+
+// loss[n] = (1/m) sum_j r[n][j]^2, from the measurement product's parts (fixed order)
+static int measured_loss_finish(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, s>>>(w.mloss_part, w.m_ld / kMeasTileN, 1, (size_t)w.n_pad,
+                                                            1.0f / (float)w.m, w.n_rows, w.loss);
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
@@ -949,17 +1028,17 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
 
 // Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
 // workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
-// planned and mapped too.
-static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false) {
+// planned and mapped too.  m > 0: the workspace of a measured entry for m measurements.
+static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
   if ((rc = plan_all(c, n_rows))) return rc;
   if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted);
+  *out = carve(c, n_rows, ws, nullptr, weighted, m);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (weighted ? " (dgan_workspace_bytes_weighted)" : ""));
+              (weighted ? " (dgan_workspace_bytes_weighted)" : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
     return DGAN_ERR_WORKSPACE;
   }
   if ((rc = build_maps(c, *out))) return rc;
@@ -1229,6 +1308,12 @@ size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr) {
   return carve(h, batch * rec_rr, nullptr, nullptr, true).bytes;
 }
 
+size_t dgan_workspace_bytes_measured(dgan_handle h, int batch, int rec_rr, int m) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || m <= 0 || m > h->hwc) return 0;
+  if (plan_all(h, batch * rec_rr) != 0) return 0;
+  return carve(h, batch * rec_rr, nullptr, nullptr, false, m).bytes;
+}
+
 int64_t dgan_last_launch_count(dgan_handle h) { return h ? h->last_launches : 0; }
 int64_t dgan_last_enqueue_count(dgan_handle h) { return h ? h->last_enqueues : 0; }
 int64_t dgan_macs_per_row(dgan_handle h) { return h ? h->macs_per_row : 0; }
@@ -1243,6 +1328,20 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
   if ((rc = run_forward(h, w, nullptr, 1, 1, false, s))) return rc;
   DGAN_CUDA_CHECK(cudaMemcpyAsync(y_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
   return DGAN_OK;
+}
+
+// The operator and measurements of a measured call (m = 0: not a measured call).
+struct MeasuredArgs { const float* a = nullptr; const float* y = nullptr; int m = 0; };
+
+// m within 1 .. H*W*C and the operator and measurements given; 0, or DGAN_ERR_INVALID_ARG naming the bad argument
+static int check_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev) {
+  if (m <= 0 || m > h->hwc) {
+    set_error("m = " + std::to_string(m) + " is out of range: 1 <= m <= H*W*C = " + std::to_string(h->hwc));
+    return DGAN_ERR_INVALID_ARG;
+  }
+  if (a_dev == nullptr) { set_error("NULL operator a_dev"); return DGAN_ERR_INVALID_ARG; }
+  if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
+  return 0;
 }
 
 // dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place
@@ -1280,6 +1379,34 @@ int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_de
                             float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   if (w_dev == nullptr) { set_error("NULL weights"); return DGAN_ERR_INVALID_ARG; }
   return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
+}
+
+int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev, int batch, int rec_rr,
+                            const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes,
+                            void* stream) {
+  if (h == nullptr || z_dev == nullptr || loss_dev == nullptr || grad_dev == nullptr || batch <= 0 || rec_rr <= 0) {
+    set_error("invalid argument");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  int rc;
+  if ((rc = check_measured(h, a_dev, m, y_dev))) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int n_rows = batch * rec_rr;
+  Workspace w;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, m))) return rc;
+  h->n_rows_cur = n_rows;
+  if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_measured(h, w, a_dev, y_dev, batch, s))) return rc;
+  if ((rc = run_forward(h, w, nullptr, 1, 1, true, s)) || (rc = launch_measure(h, w, rec_rr, s))) return rc;
+  if ((rc = measured_backward(h, w, s)) || (rc = measured_loss_finish(h, w, s))) return rc;
+  if (g_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(g_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
+  DGAN_CUDA_CHECK(cudaMemcpyAsync(loss_dev, w.loss, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, s));
+  const size_t n = (size_t)n_rows * h->desc.latent_dim;
+  const bool tc = h->desc.precision == DGAN_PREC_FP16;
+  scale_copy_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(w.g, w.n_g_parts, (size_t)w.n_pad * h->wd.latent, grad_dev,
+                                                                1.f, n, tc ? w.mscale : nullptr, h->desc.latent_dim,
+                                                                h->wd.latent);
+  DGAN_LAUNCH_CHECK(h);
+  return DGAN_OK;
 }
 
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev, void* ws,
@@ -1364,12 +1491,14 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
   return DGAN_OK;
 }
 
-// dgan_reconstruct (w_dev NULL) and dgan_reconstruct_weighted: the weights are copied into the workspace next to the
-// images, so the captured loop reads the workspace only
+// dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
+// weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
+// the workspace only
 static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                             const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
-                            void* stream) {
-  if (h == nullptr || prm == nullptr || x_dev == nullptr || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+                            void* stream, MeasuredArgs meas = MeasuredArgs()) {
+  const bool measured = meas.m > 0;
+  if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   const bool weighted = w_dev != nullptr;
   const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters, decay_lr = prm->decay_lr;
   const float rec_lr = prm->rec_lr, momentum = prm->momentum;
@@ -1379,13 +1508,18 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   const int latent = h->wd.latent;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m))) return rc;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
   if ((rc = run_init_z(h, w, z0_dev, seed, s, (size_t)prm->z_row_offset))) return rc;
-  DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  enqueues += (h->launches - launches0) + 1;
+  if (measured) {
+    if ((rc = stage_measured(h, w, meas.a, meas.y, batch, s))) return rc;
+    enqueues += h->launches - launches0;
+  } else {
+    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    enqueues += (h->launches - launches0) + 1;
+  }
   if (weighted) {
     DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
     enqueues += 1;
@@ -1405,6 +1539,19 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
       // The loop returns the pre-update forward of iteration L-1 (models/gan.py:419-421, SURVEY F4):
       // the L-th update is never observed, so its backward pass is not run.
       int r2;
+      if (measured) {
+        // the forward of dgan_vjp (ReLU masks kept, y written every step: the measurement product reads it), then the
+        // measured loss's gradient and the momentum update with the cotangent's row scales divided out
+        if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, rec_rr, ls))) return r2;
+        if (last) continue;
+        if ((r2 = measured_backward(h, w, ls))) return r2;
+        const size_t zcount = (size_t)w.n_pad * latent;
+        momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
+            w.z, w.v, w.g, w.n_g_parts, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr, latent, w.n_rows, lr,
+            momentum, zcount, w.z_h);
+        DGAN_LAUNCH_CHECK(h);
+        continue;
+      }
       if ((r2 = run_forward(h, w, w.x, rec_rr, batch, !last, ls, /*want_y=*/last, w.xw))) return r2;
       if (last) continue;
       MomentumArgs mom;
@@ -1425,7 +1572,7 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
     dgan_ctx::LoopGraph* g = nullptr;
     for (auto& e : h->graphs)
       if (e.ws == ws && e.batch == batch && e.rec_rr == rec_rr && e.rec_iters == rec_iters && e.decay_lr == decay_lr &&
-          e.weighted == (int)weighted && e.rec_lr == rec_lr && e.momentum == momentum) { g = &e; break; }
+          e.weighted == (int)weighted && e.measured == meas.m && e.rec_lr == rec_lr && e.momentum == momentum) { g = &e; break; }
     if (g == nullptr) {
       const int64_t k0 = h->launches;
       cudaGraph_t graph = nullptr;
@@ -1435,7 +1582,8 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
         cudaGraphExec_t exec = nullptr;
         if (crc == 0 && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
           if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, rec_lr, momentum, exec, h->launches - k0});
+          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, meas.m, rec_lr, momentum, exec,
+                               h->launches - k0});
           g = &h->graphs.back();
         }
         if (graph) cudaGraphDestroy(graph);
@@ -1457,8 +1605,12 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   }
   {
     const int n_rows = batch * rec_rr;
-    loss_finish_kernel<<<(n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b, 1.0f / (float)h->hwc, n_rows, w.loss);
-    DGAN_LAUNCH_CHECK(h);
+    if (measured) {
+      if ((rc = measured_loss_finish(h, w, s))) return rc;
+    } else {
+      loss_finish_kernel<<<(n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b, 1.0f / (float)h->hwc, n_rows, w.loss);
+      DGAN_LAUNCH_CHECK(h);
+    }
     select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, rec_rr, h->hwc, rec_dev, loss_dev, idx_dev);
     DGAN_LAUNCH_CHECK(h);
     enqueues += 2;
@@ -1478,6 +1630,16 @@ int dgan_reconstruct_weighted(dgan_handle h, const dgan_rec_params* prm, const f
                               size_t ws_bytes, void* stream) {
   if (w_dev == nullptr) { set_error("NULL weights"); return DGAN_ERR_INVALID_ARG; }
   return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
+}
+
+int dgan_reconstruct_measured(dgan_handle h, const dgan_rec_params* prm, const float* a_dev, int m, const float* y_dev,
+                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                              size_t ws_bytes, void* stream) {
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -1772,10 +1934,10 @@ int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
 // itself - lines "n_rows N", "n_pad N", "widths latent c4 c2 c1" (padded), "g_parts N", then one line per buffer:
 // "name type byte_offset dim0 dim1 ..." (type f32, f16, u64 or u32; dims in storage order, outermost first; the mask
 // words of layer l are "mask.l" [P_out][n_pad][C_out / 64]).  Returns the length, or -1 when buf is too small.
-static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted) {
+static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted, int m = 0) {
   if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   std::string out;
-  carve(h, n_rows, nullptr, &out, weighted);
+  carve(h, n_rows, nullptr, &out, weighted, m);
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();
@@ -1788,6 +1950,14 @@ int dgan_debug_workspace_layout(dgan_handle h, int n_rows, char* buf, int buf_le
 // The same for the workspace of the weighted entries (dgan_workspace_bytes_weighted): the weights are "xw" [n_pad][H*W*C].
 int dgan_debug_workspace_layout_weighted(dgan_handle h, int n_rows, char* buf, int buf_len) {
   return workspace_layout_impl(h, n_rows, buf, buf_len, true);
+}
+
+// The same for the workspace of the measured entries for m measurements (dgan_workspace_bytes_measured): after the
+// unweighted buffers, "am" [m_ld][H*W*C], "amt" [H*W*C][m_ld], "ym" [n_pad][m_ld], "r" [n_pad][m_ld], "dym"
+// [n_pad][H*W*C], "mloss_part" [m_ld / 64][n_pad] and "mscale" [n_pad].
+int dgan_debug_workspace_layout_measured(dgan_handle h, int n_rows, int m, char* buf, int buf_len) {
+  if (h == nullptr || m <= 0 || m > h->hwc) { set_error("invalid argument"); return -1; }
+  return workspace_layout_impl(h, n_rows, buf, buf_len, false, m);
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

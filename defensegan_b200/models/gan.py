@@ -351,6 +351,39 @@ class DefenseGANBase(object):
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
         return res
 
+    def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
+                             z_row_offset=0):
+        """Projection onto the generator's range from linear measurements (an extension; the reference has none), for
+        images that are not held themselves but observed as y = A x: a low-resolution or blurred copy, a
+        compressed-sensing sketch.  `operator` A is [m, H*W*C] (a tensor or array; columns in NHWC pixel order,
+        1 <= m <= H*W*C), one for every image and restart; `measurements` y is [B, m].  The R restarts of image i share
+        y[i], and each minimises (1/m) ||A G(z) - y[i]||^2: the normaliser is m, so A = I gives the loss of `reconstruct`
+        and rec_lr keeps its meaning.  rec_rr, rec_iters, rec_lr, the momentum and decay_lr are read from the object at
+        call time, and z0 is drawn as in `reconstruct` (the same seed gives the same z0) unless `z_init_val`
+        [B*rec_rr, latent_dim] is given.  Returns G(z) [B, H, W, C] of the restart with the lowest measured loss (with
+        return_aux also that loss [B] and the restart [B]).  Shapes and finiteness are checked before any native call -
+        a ValueError that names the bad input - at the cost of one device reduction and one host read."""
+        a = self._as_cuda(operator)
+        hwc = int(np.prod(self.image_dim))
+        if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
+            raise ValueError("operator must be [m, %d] with 1 <= m <= %d (H*W*C), got %s" % (hwc, hwc, tuple(a.shape)))
+        y = self._as_cuda(measurements).to(a.device)
+        if y.dim() != 2 or y.shape[1] != a.shape[0] or y.shape[0] == 0:
+            raise ValueError("measurements must be [B, %d] (one row of m values per image), got %s"
+                             % (a.shape[0], tuple(y.shape)))
+        if batch_size is not None and int(batch_size) != y.shape[0]:
+            raise ValueError("batch_size (%d) does not match measurements.shape[0] (%d)" % (int(batch_size), y.shape[0]))
+        finite = torch.stack([torch.isfinite(a).all(), torch.isfinite(y).all()]).tolist()
+        bad = [name for name, ok in zip(("operator", "measurements"), finite) if not ok]
+        if bad:
+            raise ValueError("%s must be finite" % " and ".join(bad))
+        z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
+        native = self._get_native(a.device)
+        self.last_seed = seed = self._next_seed(0)
+        return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
+                                           seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset))
+
     def _pixel_weights(self, pixel_weights, x):
         """pixel_weights broadcast to x's shape and materialised once, after one check of all values (finite, in [0, 1])."""
         w = self._as_cuda(pixel_weights)

@@ -131,6 +131,43 @@ int dgan_reconstruct_weighted(dgan_handle h, const dgan_rec_params* params, cons
  * weights plans nothing for it). */
 size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr);
 
+/* Projection onto the generator's range from linear measurements (an extension: the reference has none; it is the loop of
+ * compressed sensing with generative models), for observations y = A x of an image x that is not held itself - a
+ * low-resolution copy, a blurred copy, a compressed-sensing sketch:
+ *   a_dev [m, H*W*C] fp32 row-major, columns in NHWC pixel order, 1 <= m <= H*W*C; one operator for every image and restart.
+ *   y_dev [batch, m] fp32; the rec_rr restarts of image i share y[i].
+ *   Row n's loss is (1/m) sum_j ((A G(z_n))_j - y[n / rec_rr]_j)^2: the normaliser is m, so A = I (m = H*W*C) is
+ *   dgan_reconstruct's loss and rec_lr keeps its meaning.  Its gradient enters the generator's backward as the cotangent
+ *   dy_n = (2/m) A^T r_n with r_n = A G(z_n) - y[n / rec_rr], as in dgan_vjp (DGAN_PREC_FP16: a power-of-two scale per
+ *   row, one for the call with use_bn, divided out of the gradient).  The z0 stream, momentum, decay_lr, the pre-update
+ *   forward of iteration L-1 and the arg-min select (lowest index on ties) are dgan_reconstruct's; with the same seed the
+ *   call starts from the same z0.  rec_dev [batch, H, W, C], loss_dev [batch] (the minimum measured loss, nullable) and
+ *   idx_dev [batch] (nullable) as in dgan_reconstruct.
+ * Both measurement products run on the tensor cores in TF32 with DGAN_PREC_FP16 (fp32 accumulate) and in fp32 on the
+ * CUDA cores with DGAN_PREC_FP32.  m <= 0, m > H*W*C or a NULL operator or measurement pointer: DGAN_ERR_INVALID_ARG.
+ * Workspace: dgan_workspace_bytes_measured.  A, its transpose and y are copied into it by three kernels (two stream
+ * operations more than dgan_reconstruct's image copy); the captured loop reads only the workspace.  No host
+ * synchronisation, no allocation once the size has been planned.  Per L-step it runs the kernels of dgan_reconstruct's
+ * plus the measurement product, the adjoint product and the cotangent entry (3 kernels with DGAN_PREC_FP16, 1 with fp32)
+ * and, on DGAN_PREC_FP16, a separate momentum update (dgan_reconstruct's runs in the Linear backward); the last L-step
+ * adds the measurement product.  So dgan_last_launch_count is dgan_reconstruct's + 3 + 6 (L - 1) + 1 with
+ * DGAN_PREC_FP16 and + 3 + 3 (L - 1) + 1 with DGAN_PREC_FP32, and dgan_last_enqueue_count is dgan_reconstruct's + 2. */
+int dgan_reconstruct_measured(dgan_handle h, const dgan_rec_params* params, const float* a_dev, int m, const float* y_dev,
+                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
+                              void* workspace, size_t workspace_bytes, void* stream);
+
+/* Bytes of scratch for dgan_reconstruct_measured / dgan_loss_grad_measured with m measurements: dgan_workspace_bytes plus
+ * the copies of A, A^T and y (m padded to a multiple of 64 with zeros), the residuals, the adjoint product and the measured
+ * loss.  0 for m <= 0 or m > H*W*C.  A handle that never measures carves nothing for it. */
+size_t dgan_workspace_bytes_measured(dgan_handle h, int batch, int rec_rr, int m);
+
+/* One evaluation of dgan_reconstruct_measured's loop body without the update, for known-answer tests: g_dev
+ * [batch*rec_rr, H*W*C] = G(z) (nullable), loss_dev [batch*rec_rr] the measured loss, grad_dev [batch*rec_rr, latent] =
+ * d(sum loss)/dz.  Workspace: dgan_workspace_bytes_measured(h, batch, rec_rr, m). */
+int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev, int batch, int rec_rr,
+                            const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -176,12 +213,14 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
 
 /* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack
  * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
- * 256 channels, 1 + 10 L - 5 + 2). */
+ * 256 channels, 1 + 10 L - 5 + 2).  A dgan_reconstruct_measured call runs 3 + 6 (L - 1) + 1 kernels more with
+ * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there). */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
- * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr) combination is seen and replayed
- * with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy, graph, loss sum, arg-min select. */
+ * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m) combination is
+ * seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy (measured calls: the
+ * three kernels that stage A, A^T and y), graph, loss sum, arg-min select. */
 int64_t dgan_last_enqueue_count(dgan_handle h);
 
 /* Algorithmic multiply-accumulates of one generator forward per latent row (exact in-bounds
