@@ -185,6 +185,13 @@ def _require_cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
+def _require_aligned_out(rec: torch.Tensor) -> None:
+    """The reconstruct entries store rec 16 bytes at a time: a view that starts elsewhere (out=buf[1:]) is refused."""
+    if rec.data_ptr() % 16 != 0:
+        raise ValueError("out must be 16-byte aligned: its data starts %d bytes past a 16-byte boundary"
+                         % (rec.data_ptr() % 16))
+
+
 class NativeGenerator:
     """Owns one dgan_handle (the generator's re-laid-out weights on one GPU)."""
 
@@ -303,6 +310,7 @@ class NativeGenerator:
             rec = out if out is not None else torch.empty_like(x)
             if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == x.numel()):
                 raise ValueError("out must be a contiguous CUDA float32 tensor shaped like images")
+            _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
             ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
@@ -354,6 +362,7 @@ class NativeGenerator:
             rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
             if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
                 raise ValueError("out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements" % self.image_dim)
+            _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
             ws, need = self._workspace(batch, rec_rr, m=m)

@@ -1499,6 +1499,9 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
                             void* stream, MeasuredArgs meas = MeasuredArgs()) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
+  // hyper-parameters, so that a call with batch = 0 tells whether a library refuses a misaligned rec_dev, running nothing
+  if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
   const bool weighted = w_dev != nullptr;
   const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters, decay_lr = prm->decay_lr;
   const float rec_lr = prm->rec_lr, momentum = prm->momentum;

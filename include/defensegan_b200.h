@@ -103,7 +103,8 @@ typedef struct dgan_rec_params {
  *   x_dev     [batch, H, W, C] fp32 NHWC, already input-transformed
  *   z0_dev    [batch*rec_rr, latent] fp32 (the reference's z_init_val, gan.py:395-397) or NULL:
  *             z0 ~ N(0, 1/latent) from the Philox stream (seed, z_row_offset) (gan.py:370-377)
- *   rec_dev   [batch, H, W, C] fp32: G(z_{L-1}) of the arg-min restart (gan.py:438-449)
+ *   rec_dev   [batch, H, W, C] fp32: G(z_{L-1}) of the arg-min restart (gan.py:438-449), 16-byte aligned (it is
+ *             stored 16 bytes at a time); a misaligned rec_dev: DGAN_ERR_INVALID_ARG, nothing enqueued
  *   loss_dev  [batch] fp32 min per-image MSE, nullable;  idx_dev [batch] int32 chosen restart, nullable
  * The call enqueues the whole L-step loop on `stream` (8 kernels per L-step with DGAN_PREC_FP16) and never
  * synchronises the host; it does not allocate either once dgan_workspace_bytes has been called for this batch x rec_rr. */
@@ -141,8 +142,8 @@ size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr);
  *   dy_n = (2/m) A^T r_n with r_n = A G(z_n) - y[n / rec_rr], as in dgan_vjp (DGAN_PREC_FP16: a power-of-two scale per
  *   row, one for the call with use_bn, divided out of the gradient).  The z0 stream, momentum, decay_lr, the pre-update
  *   forward of iteration L-1 and the arg-min select (lowest index on ties) are dgan_reconstruct's; with the same seed the
- *   call starts from the same z0.  rec_dev [batch, H, W, C], loss_dev [batch] (the minimum measured loss, nullable) and
- *   idx_dev [batch] (nullable) as in dgan_reconstruct.
+ *   call starts from the same z0.  rec_dev [batch, H, W, C] (16-byte aligned), loss_dev [batch] (the minimum measured
+ *   loss, nullable) and idx_dev [batch] (nullable) as in dgan_reconstruct.
  * Both measurement products run on the tensor cores in TF32 with DGAN_PREC_FP16 (fp32 accumulate) and in fp32 on the
  * CUDA cores with DGAN_PREC_FP32.  m <= 0, m > H*W*C or a NULL operator or measurement pointer: DGAN_ERR_INVALID_ARG.
  * Workspace: dgan_workspace_bytes_measured.  A, its transpose and y are copied into it by three kernels (two stream

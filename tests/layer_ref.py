@@ -422,9 +422,9 @@ def check_forward(net, ws, n, stats, tag, skip=()):
         check_zero_pad(tag + name + " act", act_store, c)
 
 
-def check_last_fwd(net, ws, n, x_img_rows, stats, tag):
-    """The last layer's forward: y, the loss part of each 4x4 block (tensor cores) and the scaled d(pre) it stores
-    (tensor cores: dblk = RN16(gscale * (y - x) * act'(y)); CUDA cores: dpre = (y - x) * act'(y))."""
+def check_last_y(net, ws, n, stats, tag):
+    """The last layer's output y = act(pre) [n][2fh][2fh][C] from its stored input, to the activation's slope times the
+    accumulation bound plus the activation's own error.  Returns the reference y, act'(y) and that bound."""
     tc = net.precision == "fp16"
     L = net.layers[-1]
     x_store = ws[("act_h.%d" if tc else "act.%d") % (net.nl - 1)]
@@ -436,6 +436,16 @@ def check_last_fwd(net, ws, n, x_img_rows, stats, tag):
     C = net.c_img
     check_close(tag + "last.fwd (y)", ws["y"][:n].reshape(n, w_out, w_out, C), y, torch.zeros_like(y), 0.0, "f32", stats,
                 extra=dy, where=["row", "i", "j", "c"])
+    return y, dact, dy
+
+
+def check_last_fwd(net, ws, n, x_img_rows, stats, tag):
+    """The last layer's forward: y, the loss part of each 4x4 block (tensor cores) and the scaled d(pre) it stores
+    (tensor cores: dblk = RN16(gscale * (y - x) * act'(y)); CUDA cores: dpre = (y - x) * act'(y))."""
+    tc = net.precision == "fp16"
+    y, dact, dy = check_last_y(net, ws, n, stats, tag)
+    w_out = 2 * net.fh
+    C = net.c_img
     x = x_img_rows.double().reshape(n, w_out, w_out, C)
     d = (y - x) * dact
     # d/dy of (y - x) act'(y) is at most 1.25 (sigmoid) or 5 (tanh) in magnitude
@@ -515,30 +525,47 @@ def check_row_scales(name, s, m, top, shared):
         raise AssertionError("%s: row %d has scale %r for a row maximum %r" % (name, r, float(s[r]), float(m[r])))
 
 
-def check_cotangent(net, ws, n, dy, stats, tag):
+def check_pad_rows_zero(name, buf, n, row_axis=0):
+    """Every tile-padding row (index >= n along row_axis) of buf is exactly 0; the failure names the first such row."""
+    tail = buf.narrow(row_axis, n, buf.shape[row_axis] - n)
+    if tail.numel() and bool((tail != 0).any()):
+        idx = [int(i) for i in torch.nonzero(tail != 0)[0]]
+        raise AssertionError("%s: tile-padding row %d is not 0 (%r)" % (name, n + idx[row_axis], float(tail[tuple(idx)])))
+
+
+def check_cotangent(net, ws, n, dy, stats, tag, scale="loss"):
     """dgan_vjp's entry: d(pre) = dy * act'(y) from the stored y; tensor cores: scaled by the power-of-two row scales it
-    keeps in `loss` (max |d(pre)| * s in [8, 16)) into the block tensor, the tile-padding rows 0; CUDA cores: unscaled in
-    dpre, the tile-padding rows 0."""
+    keeps in the workspace buffer `scale` (`loss` for dgan_vjp, `mscale` for the measured entries, whose `loss` holds the
+    loss) with max |d(pre)| * s in [8, 16), into the block tensor, the tile-padding rows 0; CUDA cores: unscaled in dpre,
+    the tile-padding rows 0."""
     w_out = 2 * net.fh
     C = net.c_img
     y = ws["y"][:n].double()
     d = dy.reshape(n, -1).double() * (y * (1 - y) if net.act == "sigmoid" else 1 - y * y)
     if net.precision == "fp16":
-        s = ws["loss"][:n]
+        s = ws[scale][:n]
         check_row_scales(tag + "cotangent (row scales)", s, d.abs().amax(dim=1), 4, net.use_bn)
         ref = (d * s.double().unsqueeze(1)).reshape(n, w_out, w_out, C)
         got = blocks_to_nhwc(ws["dblk"], n, w_out, C)
         check_close(tag + "cotangent (dblk)", got, ref, torch.zeros_like(ref), 0.0, "f16", stats,
                     extra=2.0 ** -21 * ref.abs(), where=["row", "i", "j", "c"])
-        if bool((ws["dblk"][:, n:] != 0).any()):
-            raise AssertionError(tag + "cotangent (dblk): a tile-padding row is not 0")
+        check_pad_rows_zero(tag + "cotangent (dblk)", ws["dblk"], n, row_axis=1)
     else:
         ref = d.reshape(n, w_out, w_out, C)
         got = ws["dpre"][:n].reshape(n, w_out, w_out, C)
         check_close(tag + "cotangent (dpre)", got, ref, torch.zeros_like(ref), 0.0, "f32", stats,
                     extra=2.0 ** -21 * ref.abs(), where=["row", "i", "j", "c"])
-        if bool((ws["dpre"][n:] != 0).any()):
-            raise AssertionError(tag + "cotangent (dpre): a tile-padding row is not 0")
+        check_pad_rows_zero(tag + "cotangent (dpre)", ws["dpre"], n)
+
+
+def check_measured_loss(ws, n, m, stats, tag):
+    """The measured loss of each real row from the stored residuals r [n_pad][m_ld]: loss = (1/m) sum_j r_j^2 (the
+    kernels' fp32 squares, one partial per 64-column tile, the tiles summed in a fixed order, times fl(1/m)), within
+    (m + 3) u of the fp64 value: any order of m non-negative terms, the squares' roundings and the two of the multiply."""
+    r = ws["r"][:n].double()
+    ref = (r * r).sum(dim=1) / m
+    check_close(tag + "measured loss", ws["loss"][:n], ref, torch.zeros_like(ref), 0.0, "f32", stats,
+                extra=(m + 3) * 2.0 ** -24 * ref, where=["row"])
 
 
 def check_tangent(net, ws, n, t, ty, stats, tag):
@@ -610,3 +637,35 @@ def check_momentum(net, ws, z0, lr, mu, hwc, stats, tag):
     if tc:
         assert torch.equal(ws["z_h"], ws["z"].half()), "z_h is not RN16(z) after the update"
         assert not bool((ws["mom_counter"] != 0).any()), "the momentum tail's tile counters are not back at 0"
+
+
+def check_momentum_rows(net, ws, z0, lr, mu, n, stats, tag):
+    """momentum_rows_kernel (the measured loop's update) after one step from v = 0 (dgan_reconstruct_measured with L = 2
+    leaves the first step's partial sums in g, its row scales in mscale and the updated z, v, z_h): on the real rows
+    v = fl(sum of the parts in order) / mscale[row] (tensor cores: power-of-two scales, so the division is exact) or
+    unscaled (CUDA cores), z = z0 - lr * v, both to check_momentum's bound; the tile-padding rows and padded latent
+    channels of v and z exactly 0; z_h = RN16(z) exactly; the split-K tail's counters untouched (0: the measured loop
+    does not run the tail).  mu, the call's momentum, does not enter a step from v = 0."""
+    tc = net.precision == "fp16"
+    lat = net.latent
+    g = ws["g"]
+    gs = g[0].clone()
+    for p in range(1, g.shape[0]):
+        gs = gs + g[p]
+    v_ref = gs[:n, :lat].double()
+    if tc:
+        v_ref = v_ref / ws["mscale"][:n].double().unsqueeze(1)
+    v = ws["v"]
+    check_close(tag + "momentum rows (v)", v[:n, :lat], v_ref, torch.zeros_like(v_ref), 0.0, "f32", stats,
+                extra=4 * half_ulp(v_ref, "f32") + 2.0 ** -149, where=["row", "channel"])
+    z_ref = z0[:n, :lat].double() - lr * v[:n, :lat].double()
+    check_close(tag + "momentum rows (z)", ws["z"][:n, :lat], z_ref, torch.zeros_like(z_ref), 0.0, "f32", stats,
+                extra=4 * (half_ulp(z_ref, "f32") + half_ulp(lr * v[:n, :lat].double(), "f32")), where=["row", "channel"])
+    for nm in ("v", "z"):
+        check_pad_rows_zero(tag + "momentum rows (%s)" % nm, ws[nm], n)
+        check_zero_pad(tag + "momentum rows (%s)" % nm, ws[nm], lat)
+    if tc:
+        if not torch.equal(ws["z_h"], ws["z"].half()):
+            r = int(torch.nonzero(ws["z_h"] != ws["z"].half())[0][0])
+            raise AssertionError(tag + "momentum rows (z_h): row %d is not RN16(z)" % r)
+        assert not bool((ws["mom_counter"] != 0).any()), tag + "momentum rows: the split-K tail's counters are not 0"

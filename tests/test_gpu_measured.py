@@ -227,30 +227,42 @@ def test_each_measurement_product_on_its_stored_operands(arch, precision, m):
         assert m_ld % 64 == 0 and m_ld >= m
         assert torch.equal(ws["am"][:m], a) and not ws["am"][m:].any()
         assert torch.equal(ws["amt"], ws["am"].t()) and torch.equal(ws["ym"][:B, :m], y) and not ws["ym"][:B, m:].any()
-        u = 2.0 ** -24
-        rnd = 2.0 ** -10 if precision == "fp16" else 0.0      # two operands rounded to TF32, 2^-11 each
-
-        def bound(x, wt, k):
-            g = k * u / (1 - k * u)
-            return (rnd + g) * (x.abs().double() @ wt.abs().double().t())
-
-        g = ws["y"][:n]
-        y_rows = ws["ym"][:B].repeat_interleave(R_, dim=0)
-        r64 = g.double() @ ws["am"].double().t() - y_rows.double()
-        r = ws["r"][:n]
-        err = (r.double() - r64).abs()
-        lim = bound(g, ws["am"], hwc) + u * r64.abs() + 1e-30
-        print("\n%s %s m=%d: r max err / bound %.3g" % (precision, arch, m, float((err / lim).max())))
-        assert bool((err <= lim).all())
-        assert not r[:, m:].any()                              # padded measurements are exact zeros
-        dy64 = (2.0 / m) * (r.double() @ ws["amt"].double().t())
-        dy = ws["dym"][:n]
-        err = (dy.double() - dy64).abs()
-        lim = (2.0 / m) * bound(r, ws["amt"], m_ld) * (1 + 2 * u) + 2 * u * dy64.abs() + 1e-30
-        print("%s %s m=%d: dy max err / bound %.3g" % (precision, arch, m, float((err / lim).max())))
-        assert bool((err <= lim).all())
+        r_ratio, dy_ratio = check_products(ws, n, R_, m, hwc, precision)
+        print("\n%s %s m=%d: r max err / bound %.3g" % (precision, arch, m, r_ratio))
+        print("%s %s m=%d: dy max err / bound %.3g" % (precision, arch, m, dy_ratio))
     finally:
         gen.close()
+
+
+def check_products(ws, n, rec_rr, m, hwc, precision):
+    """r = A G - y and dy = (2/m) A^T r of the last measured call on n latent rows (rec_rr restarts per image) against
+    fp64 on the operands the kernels read (the workspace buffers of _buffers), each within the bound of its arithmetic
+    (test_each_measurement_product_on_its_stored_operands); the padded measurements of r exact zeros.  Returns the
+    largest error over its bound of r and of dy."""
+    u = 2.0 ** -24
+    rnd = 2.0 ** -10 if precision == "fp16" else 0.0      # two operands rounded to TF32, 2^-11 each
+    m_ld = ws["am"].shape[0]
+
+    def bound(x, wt, k):
+        g = k * u / (1 - k * u)
+        return (rnd + g) * (x.abs().double() @ wt.abs().double().t())
+
+    g = ws["y"][:n]
+    y_rows = ws["ym"][:n // rec_rr].repeat_interleave(rec_rr, dim=0)
+    r64 = g.double() @ ws["am"].double().t() - y_rows.double()
+    r = ws["r"][:n]
+    err = (r.double() - r64).abs()
+    lim = bound(g, ws["am"], hwc) + u * r64.abs() + 1e-30
+    r_ratio = float((err / lim).max())
+    assert bool((err <= lim).all()), "measurement product (r): max err / bound %.3g" % r_ratio
+    assert not r[:, m:].any()                              # padded measurements are exact zeros
+    dy64 = (2.0 / m) * (r.double() @ ws["amt"].double().t())
+    dy = ws["dym"][:n]
+    err = (dy.double() - dy64).abs()
+    lim = (2.0 / m) * bound(r, ws["amt"], m_ld) * (1 + 2 * u) + 2 * u * dy64.abs() + 1e-30
+    dy_ratio = float((err / lim).max())
+    assert bool((err <= lim).all()), "adjoint product (dy): max err / bound %.3g" % dy_ratio
+    return r_ratio, dy_ratio
 
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
