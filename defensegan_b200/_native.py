@@ -37,6 +37,7 @@ ABI_SYMBOLS = [
     "dgan_profile_kind_name", "dgan_profile_read",
     "dgan_workspace_bytes_weighted", "dgan_reconstruct_weighted", "dgan_loss_grad_weighted",
     "dgan_workspace_bytes_measured", "dgan_reconstruct_measured", "dgan_loss_grad_measured",
+    "dgan_workspace_bytes_measured_csr", "dgan_reconstruct_measured_csr", "dgan_loss_grad_measured_csr",
 ]
 
 
@@ -138,6 +139,13 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_measured.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, i32, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_loss_grad_measured.restype = i32
     lib.dgan_loss_grad_measured.argtypes = [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_workspace_bytes_measured_csr.restype = sz
+    lib.dgan_workspace_bytes_measured_csr.argtypes = [vp, i32, i32, i32, i32]
+    lib.dgan_reconstruct_measured_csr.restype = i32
+    lib.dgan_reconstruct_measured_csr.argtypes = [vp, ctypes.POINTER(dgan_rec_params), vp, vp, vp, i32, i32, vp, vp, vp, vp,
+                                                  vp, vp, sz, vp]
+    lib.dgan_loss_grad_measured_csr.restype = i32
+    lib.dgan_loss_grad_measured_csr.argtypes = [vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -183,6 +191,18 @@ def _require_cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     if t.dtype != torch.float32:
         t = t.to(torch.float32)
     return t.contiguous()
+
+
+def _require_cuda_i32(t: torch.Tensor, name: str) -> torch.Tensor:
+    """A CUDA index tensor as contiguous int32; int64 indices must fit."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor (there is no CPU path)" % name)
+    if t.dtype != torch.int32:
+        t = t.to(torch.int32)
+    return t.contiguous()
+
+
+INT32_MAX = 2 ** 31 - 1
 
 
 def _require_aligned_out(rec: torch.Tensor) -> None:
@@ -241,8 +261,10 @@ class NativeGenerator:
             pass
 
     # -- helpers -------------------------------------------------------------------------
-    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0):
-        if m > 0:
+    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1):
+        if m > 0 and nnz >= 0:
+            need = int(self.lib.dgan_workspace_bytes_measured_csr(self._handle, batch, rec_rr, int(m), int(nnz)))
+        elif m > 0:
             need = int(self.lib.dgan_workspace_bytes_measured(self._handle, batch, rec_rr, int(m)))
         else:
             sizer = self.lib.dgan_workspace_bytes_weighted if weighted else self.lib.dgan_workspace_bytes
@@ -342,6 +364,29 @@ class NativeGenerator:
             raise ValueError("measurements must be [B, %d] (the operator's m), got %s" % (m, tuple(y.shape)))
         return y, a, y.shape[0], m
 
+    def _measured_csr(self, measurements: torch.Tensor, operator: torch.Tensor):
+        """(y, (row_ptr, col_idx, val, nnz), batch, m) for a torch sparse CSR operator [m, H*W*C]: the indices as int32
+        (an nnz int32 cannot hold is refused), the values as float32, all contiguous on the GPU (shapes only; the
+        contents are not checked here - DefenseGANBase.reconstruct_measured does, and the library stages an invalid
+        CSR as the empty operator with NaN measurements)."""
+        if operator.dim() != 2 or operator.dense_dim() != 0:
+            raise ValueError("operator must be a 2-D, non-batched, non-hybrid CSR tensor, got %d dims (%d dense)"
+                             % (operator.dim(), operator.dense_dim()))
+        if operator.shape[1] != self.hwc or not 1 <= operator.shape[0] <= self.hwc:
+            raise ValueError("operator must be [m, %d] with 1 <= m <= %d, got %s"
+                             % (self.hwc, self.hwc, tuple(operator.shape)))
+        m = operator.shape[0]
+        crow, col, val = operator.crow_indices(), operator.col_indices(), operator.values()
+        nnz = int(col.numel())
+        if nnz > INT32_MAX:
+            raise ValueError("operator has %d non-zeros; at most %d are supported (int32 indices)" % (nnz, INT32_MAX))
+        y = _require_cuda_f32(measurements, "measurements")
+        if y.dim() != 2 or y.shape[1] != m or y.shape[0] <= 0:
+            raise ValueError("measurements must be [B, %d] (the operator's m), got %s" % (m, tuple(y.shape)))
+        csr = (_require_cuda_i32(crow, "operator.crow_indices()"), _require_cuda_i32(col, "operator.col_indices()"),
+               _require_cuda_f32(val, "operator.values()"), nnz)
+        return y, csr, y.shape[0], m
+
     def reconstruct_measured(self, measurements: torch.Tensor, operator: torch.Tensor, rec_rr: int, rec_iters: int,
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
@@ -349,8 +394,14 @@ class NativeGenerator:
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
-        the arg-min restart as [B, H, W, C] (with return_aux also the minimum measured loss [B] and the restart [B])."""
-        y, a, batch, m = self._measured(measurements, operator)
+        the arg-min restart as [B, H, W, C] (with return_aux also the minimum measured loss [B] and the restart [B]).
+        A torch sparse CSR operator (operator.layout == torch.sparse_csr, columns strictly ascending within each row)
+        runs dgan_reconstruct_measured_csr: the same semantics, at a cost set by its non-zeros."""
+        csr = operator.layout == torch.sparse_csr
+        if csr:
+            y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
+        else:
+            y, a, batch, m = self._measured(measurements, operator)
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
         z0 = None
@@ -365,21 +416,32 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m)
+            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            rc = self.lib.dgan_reconstruct_measured(self._handle, ctypes.byref(prm), _ptr(a), m, _ptr(y), _ptr(z0),
-                                                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-            _check(self.lib, rc, "dgan_reconstruct_measured")
+            if csr:
+                rc = self.lib.dgan_reconstruct_measured_csr(self._handle, ctypes.byref(prm), _ptr(rp), _ptr(ci), _ptr(val),
+                                                            m, nnz, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
+                                                            ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_csr")
+            else:
+                rc = self.lib.dgan_reconstruct_measured(self._handle, ctypes.byref(prm), _ptr(a), m, _ptr(y), _ptr(z0),
+                                                        _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured")
         if return_aux:
             return rec, loss, idx
         return rec
 
     def loss_grad_measured(self, measurements: torch.Tensor, operator: torch.Tensor, z: torch.Tensor, rec_rr: int):
         """(G(z), per-row measured loss, d(sum loss)/dz) at z [B*rec_rr, latent] for measurements [B, m] through operator
-        [m, H*W*C]: one evaluation of reconstruct_measured's loop body (dgan_loss_grad_measured)."""
-        y, a, batch, m = self._measured(measurements, operator)
+        [m, H*W*C]: one evaluation of reconstruct_measured's loop body (dgan_loss_grad_measured, or
+        dgan_loss_grad_measured_csr for a torch sparse CSR operator)."""
+        csr = operator.layout == torch.sparse_csr
+        if csr:
+            y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
+        else:
+            y, a, batch, m = self._measured(measurements, operator)
         zc = _require_cuda_f32(z, "z")
         n = batch * rec_rr
         if zc.shape[0] != n:
@@ -388,11 +450,17 @@ class NativeGenerator:
             g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
             loss = torch.empty(n, dtype=torch.float32, device=self.device)
             grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m)
+            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            _check(self.lib, self.lib.dgan_loss_grad_measured(self._handle, _ptr(a), m, _ptr(y), batch, rec_rr, _ptr(zc),
-                                                              _ptr(g), _ptr(loss), _ptr(grad), ws, need,
-                                                              ctypes.c_void_p(stream)), "dgan_loss_grad_measured")
+            if csr:
+                _check(self.lib, self.lib.dgan_loss_grad_measured_csr(self._handle, _ptr(rp), _ptr(ci), _ptr(val), m, nnz,
+                                                                      _ptr(y), batch, rec_rr, _ptr(zc), _ptr(g), _ptr(loss),
+                                                                      _ptr(grad), ws, need, ctypes.c_void_p(stream)),
+                       "dgan_loss_grad_measured_csr")
+            else:
+                _check(self.lib, self.lib.dgan_loss_grad_measured(self._handle, _ptr(a), m, _ptr(y), batch, rec_rr,
+                                                                  _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
+                                                                  ctypes.c_void_p(stream)), "dgan_loss_grad_measured")
         return g, loss, grad
 
     def sample_z0(self, n_rows: int, seed: int, z_row_offset: int = 0) -> torch.Tensor:

@@ -15,6 +15,7 @@
 #include "kernels_tc2.cuh"
 #include "kernels_vjp.cuh"
 #include "kernels_measured.cuh"
+#include "kernels_measured_csr.cuh"
 
 namespace dgan {
 
@@ -318,10 +319,10 @@ struct dgan_ctx {
   bool profile = false;
   int n_rows_cur = 0;
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
-  // weighted, measured: the m of a measured call, 0 otherwise) on a private stream, replayed with one cudaGraphLaunch per
-  // call.
+  // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise)
+  // on a private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
-    const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured; float rec_lr, momentum;
+    const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     cudaGraphExec_t exec; int64_t kernels;
   };
   std::vector<LoopGraph> graphs;
@@ -436,6 +437,13 @@ struct Workspace {
   // [n_pad][H*W*C], the measured loss's parts [m_ld / 64][n_pad] and the cotangent's row scales [n_pad] (fp16 path)
   int m = 0, m_ld = 0;
   float *am = nullptr, *amt = nullptr, *ym = nullptr, *r = nullptr, *dym = nullptr, *mloss_part = nullptr, *mscale = nullptr;
+  // CSR-measured workspaces (csr; kernels_measured_csr.cuh): no am / amt; the staged operator A (a_rp [m_ld + 1], a_ci /
+  // a_v [nnz]) and its transpose At (at_rp [H*W*C + 1], at_ci / at_v [nnz]), the rows the validation found bad [m_ld]
+  // and the validity flag [1], after all the buffers above
+  bool csr = false;
+  int nnz = 0;
+  int *a_rp = nullptr, *a_ci = nullptr, *at_rp = nullptr, *at_ci = nullptr, *csr_bad = nullptr, *csr_valid = nullptr;
+  float *a_v = nullptr, *at_v = nullptr;
   size_t bytes = 0;
 };
 
@@ -446,8 +454,10 @@ static int measured_ld(int m) { return (int)align_up((size_t)m, kMeasTileN); }
 // offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.  weighted: the workspace of the
 // weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.  m > 0: the workspace of
 // the measured entries for m measurements, the same buffers at the same offsets and the measured ones after all of them.
+// csr_nnz >= 0 (with m > 0): the workspace of the CSR-measured entries for nnz non-zeros, the measured buffers without
+// am / amt and the CSR ones after all of them.
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
-                       int m = 0) {
+                       int m = 0, int csr_nnz = -1) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -455,7 +465,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
   char* b = (char*)base;
   // a buffer of the dims' product of elements of type `type`, one of the element types below
   struct ElemType { const char* name; size_t bytes; };
-  static const ElemType kTypes[] = {{"f32", 4}, {"f16", 2}, {"u64", 8}, {"u32", 4}};
+  static const ElemType kTypes[] = {{"f32", 4}, {"f16", 2}, {"u64", 8}, {"u32", 4}, {"i32", 4}};
   auto take = [&](const std::string& name, const char* type, std::initializer_list<size_t> dims) -> void* {
     size_t bytes = 0;
     for (const ElemType& t : kTypes)
@@ -528,13 +538,28 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.m = m;
     w.m_ld = measured_ld(m);
     const size_t mld = (size_t)w.m_ld;
-    w.am = (float*)take("am", "f32", {mld, hwc});
-    w.amt = (float*)take("amt", "f32", {hwc, mld});
+    w.csr = csr_nnz >= 0;
+    if (!w.csr) {
+      w.am = (float*)take("am", "f32", {mld, hwc});
+      w.amt = (float*)take("amt", "f32", {hwc, mld});
+    }
     w.ym = (float*)take("ym", "f32", {np, mld});            // batch <= n_pad
     w.r = (float*)take("r", "f32", {np, mld});
     w.dym = (float*)take("dym", "f32", {np, hwc});
     w.mloss_part = (float*)take("mloss_part", "f32", {mld / kMeasTileN, np});
     w.mscale = (float*)take("mscale", "f32", {np});
+    if (w.csr) {
+      const size_t nnz = (size_t)csr_nnz;
+      w.nnz = csr_nnz;
+      w.a_rp = (int*)take("a_rp", "i32", {mld + 1});
+      w.a_ci = (int*)take("a_ci", "i32", {nnz});
+      w.a_v = (float*)take("a_v", "f32", {nnz});
+      w.at_rp = (int*)take("at_rp", "i32", {hwc + 1});
+      w.at_ci = (int*)take("at_ci", "i32", {nnz});
+      w.at_v = (float*)take("at_v", "f32", {nnz});
+      w.csr_bad = (int*)take("csr_bad", "i32", {mld});
+      w.csr_valid = (int*)take("csr_valid", "i32", {1});
+    }
   }
   w.bytes = off;
   return w;
@@ -966,8 +991,55 @@ static int launch_measured_gemm(dgan_ctx* c, const Workspace& w, const float* X,
   return 0;
 }
 
+// Copy a call's CSR operator (row_ptr [m + 1], col_idx / val [nnz]) and measurements y [batch][m] into the CSR-measured
+// workspace w, validated, with its transpose built and y padded as stage_measured does (kernels_measured_csr.cuh): five
+// kernels.  An invalid CSR is staged as the empty operator with NaN measurements.
+static int stage_measured_csr(dgan_ctx* c, const Workspace& w, const int* row_ptr, const int* col_idx, const float* val,
+                              const float* y, int batch, cudaStream_t s) {
+  const int hwc = c->hwc, m = w.m;
+  // the products stage kCsrRows rows of H*W*C (measurement) or m_ld (adjoint) floats; the opt-in limit is per kernel, not
+  // per handle, so it is only ever raised
+  const int smem = kCsrRows * std::max(hwc, w.m_ld) * (int)sizeof(float);
+  cudaFuncAttributes fa;
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_csr_kernel<MEAS_RESID>));
+  if (fa.maxDynamicSharedSizeBytes < smem)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_csr_kernel<MEAS_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_csr_kernel<MEAS_SCALE>));
+  if (fa.maxDynamicSharedSizeBytes < smem)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_csr_kernel<MEAS_SCALE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  csr_validate_kernel<<<(m + 255) / 256, 256, 0, s>>>(row_ptr, col_idx, m, w.nnz, hwc, w.csr_bad);
+  DGAN_LAUNCH_CHECK(c);
+  csr_stage_rows_kernel<<<1, 1024, 0, s>>>(row_ptr, w.csr_bad, m, w.m_ld, w.nnz, w.csr_valid, w.a_rp);
+  DGAN_LAUNCH_CHECK(c);
+  const size_t n = std::max({(size_t)w.nnz, (size_t)batch * w.m_ld, (size_t)hwc});
+  csr_stage_entries_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(col_idx, val, w.nnz, y, batch, m, w.m_ld, w.a_rp,
+                                                                       w.csr_valid, hwc, w.a_ci, w.a_v, w.ym, w.at_rp);
+  DGAN_LAUNCH_CHECK(c);
+  csr_scan_kernel<<<1, 1024, 0, s>>>(w.at_rp, hwc);
+  DGAN_LAUNCH_CHECK(c);
+  csr_fill_transpose_kernel<<<(hwc + 127) / 128, 128, 0, s>>>(w.a_rp, w.a_ci, w.a_v, m, hwc, w.at_rp, w.at_ci, w.at_v);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// out = EPI(s_ * X A^T) over the real latent rows through a staged CSR operator (rp, ci, val; N output columns): fp32
+// FFMA on both precisions.  X rows of K floats at stride ldx are staged in shared memory.
+template <int EPI>
+static int launch_measured_csr(dgan_ctx* c, const Workspace& w, const float* X, int ldx, int K, const int* rp,
+                               const int* ci, const float* val, int N, float* out, int ldo, const float* ym, int R,
+                               float s_, float* loss_part, cudaStream_t s) {
+  const unsigned grid = (unsigned)((w.n_rows + kCsrRows - 1) / kCsrRows);
+  measured_csr_kernel<EPI><<<grid, kCsrThreads, kCsrRows * K * sizeof(float), s>>>(X, ldx, w.n_rows, K, rp, ci, val, N, out,
+                                                                                    ldo, ym, R, s_, loss_part, w.n_pad);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
 // The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.
 static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  if (w.csr)
+    return launch_measured_csr<MEAS_RESID>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld, w.ym, R,
+                                           1.f, w.mloss_part, s);
   return launch_measured_gemm<MEAS_RESID>(c, w, w.y, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R, 1.f,
                                           w.mloss_part, s);
 }
@@ -976,9 +1048,11 @@ static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s
 // fp16 row scales in w.mscale: w.loss carries the loss to the select) and the backward-to-z into w.g.
 static int measured_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   int rc;
-  if ((rc = launch_measured_gemm<MEAS_SCALE>(c, w, w.r, w.m_ld, w.amt, w.m_ld, c->hwc, w.m_ld, w.dym, c->hwc, nullptr, 1,
-                                             2.f / (float)w.m, nullptr, s)))
-    return rc;
+  if (w.csr) rc = launch_measured_csr<MEAS_SCALE>(c, w, w.r, w.m_ld, w.m_ld, w.at_rp, w.at_ci, w.at_v, c->hwc, w.dym,
+                                                  c->hwc, nullptr, 1, 2.f / (float)w.m, nullptr, s);
+  else rc = launch_measured_gemm<MEAS_SCALE>(c, w, w.r, w.m_ld, w.amt, w.m_ld, c->hwc, w.m_ld, w.dym, c->hwc, nullptr, 1,
+                                             2.f / (float)w.m, nullptr, s);
+  if (rc) return rc;
   if ((rc = launch_cotangent(c, w, w.dym, s, w.mscale))) return rc;
   return run_backward(c, w, s);
 }
@@ -1029,16 +1103,18 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
 // Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
 // workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
 // planned and mapped too.  m > 0: the workspace of a measured entry for m measurements.
-static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0) {
+static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0,
+                    int csr_nnz = -1) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
   if ((rc = plan_all(c, n_rows))) return rc;
   if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted, m);
+  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (weighted ? " (dgan_workspace_bytes_weighted)" : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
+              (weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
+                                                             : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
     return DGAN_ERR_WORKSPACE;
   }
   if ((rc = build_maps(c, *out))) return rc;
@@ -1314,6 +1390,15 @@ size_t dgan_workspace_bytes_measured(dgan_handle h, int batch, int rec_rr, int m
   return carve(h, batch * rec_rr, nullptr, nullptr, false, m).bytes;
 }
 
+// nnz within 0 .. m * H*W*C (the non-zeros an m-row operator can hold)
+static bool csr_nnz_ok(dgan_handle h, int m, int nnz) { return nnz >= 0 && (int64_t)nnz <= (int64_t)m * h->hwc; }
+
+size_t dgan_workspace_bytes_measured_csr(dgan_handle h, int batch, int rec_rr, int m, int nnz) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || m <= 0 || m > h->hwc || !csr_nnz_ok(h, m, nnz)) return 0;
+  if (plan_all(h, batch * rec_rr) != 0) return 0;
+  return carve(h, batch * rec_rr, nullptr, nullptr, false, m, nnz).bytes;
+}
+
 int64_t dgan_last_launch_count(dgan_handle h) { return h ? h->last_launches : 0; }
 int64_t dgan_last_enqueue_count(dgan_handle h) { return h ? h->last_enqueues : 0; }
 int64_t dgan_macs_per_row(dgan_handle h) { return h ? h->macs_per_row : 0; }
@@ -1330,8 +1415,11 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
   return DGAN_OK;
 }
 
-// The operator and measurements of a measured call (m = 0: not a measured call).
-struct MeasuredArgs { const float* a = nullptr; const float* y = nullptr; int m = 0; };
+// The operator and measurements of a measured call (m = 0: not a measured call): dense a, or (nnz >= 0) the CSR rp, ci, val.
+struct MeasuredArgs {
+  const float* a = nullptr; const float* y = nullptr; int m = 0;
+  const int* rp = nullptr; const int* ci = nullptr; const float* val = nullptr; int nnz = -1;
+};
 
 // m within 1 .. H*W*C and the operator and measurements given; 0, or DGAN_ERR_INVALID_ARG naming the bad argument
 static int check_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev) {
@@ -1342,6 +1430,30 @@ static int check_measured(dgan_handle h, const float* a_dev, int m, const float*
   if (a_dev == nullptr) { set_error("NULL operator a_dev"); return DGAN_ERR_INVALID_ARG; }
   if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
   return 0;
+}
+
+// The same for a CSR operator: nnz within 0 .. m * H*W*C, row_ptr given, col_idx and val given unless nnz == 0.  The
+// contents are validated on the device while they are staged (stage_measured_csr).
+static int check_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m,
+                              int nnz, const float* y_dev) {
+  if (m <= 0 || m > h->hwc) {
+    set_error("m = " + std::to_string(m) + " is out of range: 1 <= m <= H*W*C = " + std::to_string(h->hwc));
+    return DGAN_ERR_INVALID_ARG;
+  }
+  if (!csr_nnz_ok(h, m, nnz)) {
+    set_error("nnz = " + std::to_string(nnz) + " is out of range: 0 <= nnz <= m * H*W*C");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  if (row_ptr == nullptr) { set_error("NULL row_ptr"); return DGAN_ERR_INVALID_ARG; }
+  if (nnz > 0 && (col_idx == nullptr || val == nullptr)) { set_error("NULL col_idx or val with nnz > 0"); return DGAN_ERR_INVALID_ARG; }
+  if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
+  return 0;
+}
+
+// Stage a measured call's operator and measurements: dense or CSR
+static int stage_meas(dgan_ctx* c, const Workspace& w, const MeasuredArgs& meas, int batch, cudaStream_t s) {
+  if (w.csr) return stage_measured_csr(c, w, meas.rp, meas.ci, meas.val, meas.y, batch, s);
+  return stage_measured(c, w, meas.a, meas.y, batch, s);
 }
 
 // dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place
@@ -1381,21 +1493,16 @@ int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_de
   return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
-int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev, int batch, int rec_rr,
-                            const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes,
-                            void* stream) {
-  if (h == nullptr || z_dev == nullptr || loss_dev == nullptr || grad_dev == nullptr || batch <= 0 || rec_rr <= 0) {
-    set_error("invalid argument");
-    return DGAN_ERR_INVALID_ARG;
-  }
+// dgan_loss_grad_measured and dgan_loss_grad_measured_csr, after their operator checks
+static int loss_grad_measured_impl(dgan_handle h, const MeasuredArgs& meas, int batch, int rec_rr, const float* z_dev,
+                                   float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   int rc;
-  if ((rc = check_measured(h, a_dev, m, y_dev))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
   Workspace w;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, m))) return rc;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, meas.m, meas.nnz))) return rc;
   h->n_rows_cur = n_rows;
-  if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_measured(h, w, a_dev, y_dev, batch, s))) return rc;
+  if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_meas(h, w, meas, batch, s))) return rc;
   if ((rc = run_forward(h, w, nullptr, 1, 1, true, s)) || (rc = launch_measure(h, w, rec_rr, s))) return rc;
   if ((rc = measured_backward(h, w, s)) || (rc = measured_loss_finish(h, w, s))) return rc;
   if (g_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(g_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
@@ -1407,6 +1514,34 @@ int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const floa
                                                                 h->wd.latent);
   DGAN_LAUNCH_CHECK(h);
   return DGAN_OK;
+}
+
+static bool loss_grad_args_ok(dgan_handle h, const float* z_dev, float* loss_dev, float* grad_dev, int batch, int rec_rr) {
+  if (h == nullptr || z_dev == nullptr || loss_dev == nullptr || grad_dev == nullptr || batch <= 0 || rec_rr <= 0) {
+    set_error("invalid argument");
+    return false;
+  }
+  return true;
+}
+
+int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev, int batch, int rec_rr,
+                            const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes,
+                            void* stream) {
+  if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
+}
+
+int dgan_loss_grad_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m,
+                                int nnz, const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
+                                float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev, void* ws,
@@ -1511,13 +1646,13 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   const int latent = h->wd.latent;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz))) return rc;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
   if ((rc = run_init_z(h, w, z0_dev, seed, s, (size_t)prm->z_row_offset))) return rc;
   if (measured) {
-    if ((rc = stage_measured(h, w, meas.a, meas.y, batch, s))) return rc;
+    if ((rc = stage_meas(h, w, meas, batch, s))) return rc;
     enqueues += h->launches - launches0;
   } else {
     DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -1575,7 +1710,8 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
     dgan_ctx::LoopGraph* g = nullptr;
     for (auto& e : h->graphs)
       if (e.ws == ws && e.batch == batch && e.rec_rr == rec_rr && e.rec_iters == rec_iters && e.decay_lr == decay_lr &&
-          e.weighted == (int)weighted && e.measured == meas.m && e.rec_lr == rec_lr && e.momentum == momentum) { g = &e; break; }
+          e.weighted == (int)weighted && e.measured == meas.m && e.csr_nnz == meas.nnz && e.rec_lr == rec_lr &&
+          e.momentum == momentum) { g = &e; break; }
     if (g == nullptr) {
       const int64_t k0 = h->launches;
       cudaGraph_t graph = nullptr;
@@ -1585,8 +1721,8 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
         cudaGraphExec_t exec = nullptr;
         if (crc == 0 && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
           if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, meas.m, rec_lr, momentum, exec,
-                               h->launches - k0});
+          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, meas.m, meas.nnz, rec_lr, momentum,
+                               exec, h->launches - k0});
           g = &h->graphs.back();
         }
         if (graph) cudaGraphDestroy(graph);
@@ -1642,6 +1778,16 @@ int dgan_reconstruct_measured(dgan_handle h, const dgan_rec_params* prm, const f
   if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
   MeasuredArgs meas;
   meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
+}
+
+int dgan_reconstruct_measured_csr(dgan_handle h, const dgan_rec_params* prm, const int32_t* row_ptr, const int32_t* col_idx,
+                                  const float* val, int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                  float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
   return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
 }
 
@@ -1937,10 +2083,11 @@ int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
 // itself - lines "n_rows N", "n_pad N", "widths latent c4 c2 c1" (padded), "g_parts N", then one line per buffer:
 // "name type byte_offset dim0 dim1 ..." (type f32, f16, u64 or u32; dims in storage order, outermost first; the mask
 // words of layer l are "mask.l" [P_out][n_pad][C_out / 64]).  Returns the length, or -1 when buf is too small.
-static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted, int m = 0) {
+static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted, int m = 0,
+                                 int csr_nnz = -1) {
   if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   std::string out;
-  carve(h, n_rows, nullptr, &out, weighted, m);
+  carve(h, n_rows, nullptr, &out, weighted, m, csr_nnz);
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();
@@ -1961,6 +2108,16 @@ int dgan_debug_workspace_layout_weighted(dgan_handle h, int n_rows, char* buf, i
 int dgan_debug_workspace_layout_measured(dgan_handle h, int n_rows, int m, char* buf, int buf_len) {
   if (h == nullptr || m <= 0 || m > h->hwc) { set_error("invalid argument"); return -1; }
   return workspace_layout_impl(h, n_rows, buf, buf_len, false, m);
+}
+
+// The same for the workspace of the CSR-measured entries for m measurements and nnz non-zeros
+// (dgan_workspace_bytes_measured_csr): after the unweighted buffers, the measured ones without "am" and "amt", then the
+// staged operator "a_rp" i32 [m_ld + 1], "a_ci" i32 [nnz], "a_v" f32 [nnz], its transpose "at_rp" i32 [H*W*C + 1],
+// "at_ci" i32 [nnz], "at_v" f32 [nnz], the bad-row marks "csr_bad" i32 [m_ld] and the validity flag "csr_valid" i32 [1]
+// (1: the caller's CSR was valid; 0: it was staged as the empty operator with NaN measurements).
+int dgan_debug_workspace_layout_measured_csr(dgan_handle h, int n_rows, int m, int nnz, char* buf, int buf_len) {
+  if (h == nullptr || m <= 0 || m > h->hwc || !csr_nnz_ok(h, m, nnz)) { set_error("invalid argument"); return -1; }
+  return workspace_layout_impl(h, n_rows, buf, buf_len, false, m, nnz);
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -362,7 +362,17 @@ class DefenseGANBase(object):
         call time, and z0 is drawn as in `reconstruct` (the same seed gives the same z0) unless `z_init_val`
         [B*rec_rr, latent_dim] is given.  Returns G(z) [B, H, W, C] of the restart with the lowest measured loss (with
         return_aux also that loss [B] and the restart [B]).  Shapes and finiteness are checked before any native call -
-        a ValueError that names the bad input - at the cost of one device reduction and one host read."""
+        a ValueError that names the bad input - at the cost of one device reduction and one host read.
+
+        `operator` may also be a torch sparse tensor, COO (coalesced: duplicates summed) or CSR: the same semantics as the
+        dense matrix it represents, at a cost set by its non-zeros - a block average, a blur kernel or pixel subsampling
+        have a few non-zeros per row.  A CSR operator is checked too (2-D, not batched or hybrid, crow_indices rising
+        from 0 to nnz, column indices in range and strictly ascending within each row).  On fp32 the result is
+        bit-identical to the dense call on the same matrix; on fp16 a sparse operator is applied in fp32, so it differs
+        from the dense call (TF32) by the TF32 rounding of the operator and the operands."""
+        if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
+            return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
+                                                     z_row_offset)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -377,6 +387,53 @@ class DefenseGANBase(object):
         bad = [name for name, ok in zip(("operator", "measurements"), finite) if not ok]
         if bad:
             raise ValueError("%s must be finite" % " and ".join(bad))
+        z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
+        native = self._get_native(a.device)
+        self.last_seed = seed = self._next_seed(0)
+        return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
+                                           seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset))
+
+    def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset):
+        """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements."""
+        a = operator
+        if a.layout == torch.sparse_coo:
+            if a.dim() != 2 or a.dense_dim() != 0:
+                raise ValueError("operator must be a 2-D, non-hybrid sparse tensor, got %d dims (%d dense)"
+                                 % (a.dim(), a.dense_dim()))
+            a = a.coalesce().to_sparse_csr()
+        if a.crow_indices().dim() != 1:
+            raise ValueError("operator must not be a batched CSR tensor, got shape %s" % (tuple(a.shape),))
+        if a.values().dim() != 1:
+            raise ValueError("operator must not be a hybrid CSR tensor (values of shape %s)" % (tuple(a.values().shape),))
+        hwc = int(np.prod(self.image_dim))
+        if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
+            raise ValueError("operator must be [m, %d] with 1 <= m <= %d (H*W*C), got %s" % (hwc, hwc, tuple(a.shape)))
+        a = self._as_cuda(a)
+        m = a.shape[0]
+        y = self._as_cuda(measurements).to(a.device)
+        if y.dim() != 2 or y.shape[1] != m or y.shape[0] == 0:
+            raise ValueError("measurements must be [B, %d] (one row of m values per image), got %s" % (m, tuple(y.shape)))
+        if batch_size is not None and int(batch_size) != y.shape[0]:
+            raise ValueError("batch_size (%d) does not match measurements.shape[0] (%d)" % (int(batch_size), y.shape[0]))
+        crow, col, val = a.crow_indices(), a.col_indices(), a.values()
+        nnz = col.numel()
+        # row starts: entry e + 1 opens a row when it is some row's first entry; otherwise its column must exceed e's
+        start = torch.zeros(nnz + 1, dtype=torch.bool, device=col.device)
+        start[crow.clamp(0, nnz)] = True
+        checks = [
+            ("operator crow_indices must rise from 0 to nnz = %d" % nnz,
+             (crow[0] == 0) & (crow[-1] == nnz) & (crow[1:] >= crow[:-1]).all()),
+            ("operator column indices must be in [0, %d)" % hwc, ((col >= 0) & (col < hwc)).all()),
+            ("operator column indices must be strictly ascending within each row (no duplicates)",
+             ((col[1:] > col[:-1]) | start[1:nnz]).all()),
+            ("operator values must be finite", torch.isfinite(val).all()),
+            ("measurements must be finite", torch.isfinite(y).all()),
+        ]
+        ok = torch.stack([c for _, c in checks]).tolist()
+        bad = [name for (name, _), good in zip(checks, ok) if not good]
+        if bad:
+            raise ValueError("; ".join(bad))
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)

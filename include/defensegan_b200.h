@@ -169,6 +169,41 @@ int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const floa
                             const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* workspace,
                             size_t workspace_bytes, void* stream);
 
+/* dgan_reconstruct_measured with a sparse operator: A [m, H*W*C] in CSR, row_ptr [m + 1], col_idx [nnz] and val [nnz]
+ * (int32, int32, fp32, on the device), the columns of each row strictly ascending.  The semantics are exactly those of
+ * dgan_reconstruct_measured for the dense matrix the CSR represents; the two measurement products cost in proportion to
+ * the non-zeros instead of m * H*W*C.  They run in fp32 on the CUDA cores on both precisions: with DGAN_PREC_FP32 every
+ * output is bit-identical to dgan_reconstruct_measured's on that dense matrix; with DGAN_PREC_FP16 A is applied in fp32,
+ * so the result differs from the dense call's (TF32) by the TF32 rounding of A and of the operands.
+ * m <= 0, m > H*W*C, nnz < 0, nnz > m * H*W*C, a NULL row_ptr or y_dev, a NULL col_idx or val with nnz > 0, or a
+ * rec_dev that is not 16-byte aligned: DGAN_ERR_INVALID_ARG before anything is enqueued.  The CSR's contents are
+ * validated on the device while it is staged (row_ptr from 0 to nnz, never decreasing; columns in [0, H*W*C) and
+ * strictly ascending within each row); reading only row_ptr[0..m] and col_idx / val[0..nnz).  A CSR that breaks one of
+ * them is never used: the call returns DGAN_OK with NaN losses and reconstructions.
+ * Workspace: dgan_workspace_bytes_measured_csr.  The operator is validated and copied into it with its transpose, and y
+ * with it, by five kernels (four stream operations more than dgan_reconstruct's image copy); the captured loop reads only
+ * the workspace.  No host synchronisation, no allocation once the size has been planned.  Per L-step it runs the kernels
+ * of dgan_reconstruct_measured (one kernel per product).  So dgan_last_launch_count is dgan_reconstruct's
+ * + 5 + 6 (L - 1) + 1 with DGAN_PREC_FP16 and + 5 + 3 (L - 1) + 1 with DGAN_PREC_FP32, and dgan_last_enqueue_count is
+ * dgan_reconstruct's + 4. */
+int dgan_reconstruct_measured_csr(dgan_handle h, const dgan_rec_params* params, const int32_t* row_ptr,
+                                  const int32_t* col_idx, const float* val, int m, int nnz, const float* y_dev,
+                                  const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+
+/* Bytes of scratch for dgan_reconstruct_measured_csr / dgan_loss_grad_measured_csr with m measurements and nnz
+ * non-zeros: dgan_workspace_bytes plus the copies of the CSR and of its transpose, y (m padded to a multiple of 64), the
+ * residuals, the adjoint product and the measured loss - no dense copy of A.  0 for m <= 0, m > H*W*C, nnz < 0 or
+ * nnz > m * H*W*C.  A handle that never uses a CSR operator carves nothing for it. */
+size_t dgan_workspace_bytes_measured_csr(dgan_handle h, int batch, int rec_rr, int m, int nnz);
+
+/* dgan_loss_grad_measured with the CSR operator of dgan_reconstruct_measured_csr.
+ * Workspace: dgan_workspace_bytes_measured_csr(h, batch, rec_rr, m, nnz). */
+int dgan_loss_grad_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m,
+                                int nnz, const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
+                                float* loss_dev, float* grad_dev, void* workspace, size_t workspace_bytes,
+                                void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -215,13 +250,15 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
 /* Kernels run by the most recent dgan_reconstruct on this handle (1 + 8 L - 4 + 2 with DGAN_PREC_FP16 on the MNIST stack
  * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
  * 256 channels, 1 + 10 L - 5 + 2).  A dgan_reconstruct_measured call runs 3 + 6 (L - 1) + 1 kernels more with
- * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there). */
+ * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there); a dgan_reconstruct_measured_csr call
+ * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
- * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m) combination is
- * seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy (measured calls: the
- * three kernels that stage A, A^T and y), graph, loss sum, arg-min select. */
+ * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind and
+ * nnz) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them),
+ * graph, loss sum, arg-min select. */
 int64_t dgan_last_enqueue_count(dgan_handle h);
 
 /* Algorithmic multiply-accumulates of one generator forward per latent row (exact in-bounds

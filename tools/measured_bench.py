@@ -9,7 +9,12 @@
     and their rate against the TF32 data-sheet figure (495 TFLOP/s dense, H100 SXM);
   - the card name and power limit.
 Writes <out_dir>/measured_bench.json.
-Usage: python tools/measured_bench.py OUT_DIR [--reps N] [--warmup N] [--precision fp16|fp32] [--user-steps N]"""
+With --sparse instead: sparse operators (a 2x2 block average, a full-resolution 5 x 5 blur, pixel subsampling at two m)
+at MNIST B = 256 and CelebA B = 128, R = 10, L = 200, passed dense and as CSR; plain, dense and CSR calls alternate
+repeat by repeat.  Reports images/s of each call, the device time of the CSR products (torch.profiler) with their
+algorithmic bytes over it as a share of 3.35 TB/s (HBM3, H100 SXM data sheet), and the workspace bytes of both calls.
+A dense call that does not fit in memory is reported as not run.  Writes <out_dir>/measured_bench_sparse.json.
+Usage: python tools/measured_bench.py OUT_DIR [--reps N] [--warmup N] [--precision fp16|fp32] [--user-steps N] [--sparse]"""
 import argparse
 import json
 import os
@@ -25,10 +30,13 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 from defensegan_b200 import _native  # noqa: E402
 from oracle import defensegan_oracle as O  # noqa: E402
 import measured_oracle as MO  # noqa: E402
+import sparse_operators as SO  # noqa: E402
 
 # (arch, images, restarts, steps, measurement counts)
 CASES = [("mnist", 256, 10, 200, (100, 392, 784)), ("celeba", 128, 10, 200, (500, 2000))]
 TF32_TFLOPS = 495.0
+HBM_TBPS = 3.35
+SHAPES = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 
 
 def card():
@@ -91,6 +99,107 @@ def kernel_times(gen, y, a, z, R, calls=10):
     return out
 
 
+def csr_kernel_times(gen, y, a, z, R, calls=10):
+    """Mean device time per call of each CSR product over dgan_loss_grad_measured_csr calls (torch.profiler)."""
+    from torch.profiler import ProfilerActivity, profile
+    gen.loss_grad_measured(y, a, z, R)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            gen.loss_grad_measured(y, a, z, R)
+        torch.cuda.synchronize()
+    out = {"measure": 0.0, "adjoint": 0.0}
+    for ka in prof.key_averages():
+        if "measured_csr_kernel" not in ka.key:           # <0>: the measurement product, <1>: the adjoint
+            continue
+        out["measure" if "<0>" in ka.key else "adjoint"] += ka.device_time_total / 1e3 / calls
+    return out
+
+
+def csr_product_bytes(n, m, hwc, nnz):
+    """Algorithmic bytes of the two CSR products of one L-step on n latent rows: G (or r) read once, r (or dy) written once,
+    the staged operator (int32 row pointers, int32 columns, fp32 values) and the measurements read once."""
+    m_ld = (m + 63) // 64 * 64
+    measure = 4 * (n * hwc + n * m_ld + (m_ld + 1) + 2 * nnz + n // 10 * m_ld)
+    adjoint = 4 * (n * m_ld + n * hwc + (hwc + 1) + 2 * nnz)
+    return measure, adjoint
+
+
+def sparse_main(args, dev):
+    from defensegan_b200 import _native as N
+    res = {"card": card(), "reps": args.reps, "warmup": args.warmup, "precision": args.precision, "results": []}
+    for arch, B, R, L, subs in (("mnist", 256, 10, 200, (100, 392)), ("celeba", 128, 10, 200, (1024, 4096))):
+        w = O.init_generator_weights(arch)
+        x = torch.tensor(O.synthetic_images(arch, w, B)).to(dev)
+        h, w_, c = SHAPES[arch]
+        hwc = h * w_ * c
+        z0 = torch.tensor(O.sample_z0(B * R, 128)).to(dev)
+        gen = N.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], precision=args.precision,
+                                device=dev)
+        ops = {"block2": MO.block_average_operator(h, w_, c, 2), "blur5": SO.blur_operator(h, w_, c)}
+        for m in subs:
+            ops["sub%d" % m] = SO.subsample_operator(m, hwc, seed=m)
+        r = {"arch": arch, "images": B, "restarts": R, "steps": L, "precision": args.precision, "operators": []}
+        t_plain = []
+        for name, a_np in ops.items():
+            m = a_np.shape[0]
+            lr = 10.0 * min(1.0, 4.0 * m / hwc) if m < hwc else 10.0
+            dense = torch.tensor(a_np).to(dev)
+            csr = dense.to_sparse_csr()
+            nnz = csr.values().numel()
+            y = x.reshape(B, -1) @ dense.t()
+            ws_dense = int(gen.lib.dgan_workspace_bytes_measured(gen._handle, B, R, m))
+            ws_csr = int(gen.lib.dgan_workspace_bytes_measured_csr(gen._handle, B, R, m, nnz))
+            calls = {"plain": lambda: gen.reconstruct(x, R, L, 10.0, z_init_val=z0),
+                     "csr": lambda: gen.reconstruct_measured(y, csr, R, L, lr, z_init_val=z0)}
+            dense_note = None
+            try:
+                gen.reconstruct_measured(y, dense, R, 1, lr, z_init_val=z0)
+                torch.cuda.synchronize()
+                calls["dense"] = lambda: gen.reconstruct_measured(y, dense, R, L, lr, z_init_val=z0)
+            except (RuntimeError, torch.OutOfMemoryError) as e:
+                dense_note = "not run: %s" % str(e).splitlines()[0][:200]
+                gen._ws = None
+                torch.cuda.empty_cache()
+            times = {k: [] for k in calls}
+            for i in range(args.warmup + args.reps):
+                for k, fn in calls.items():
+                    t = timed(fn)
+                    if i >= args.warmup:
+                        times[k].append(t)
+            t_plain += times["plain"]
+            med = {k: float(np.median(v)) for k, v in times.items()}
+            kt = csr_kernel_times(gen, y, csr, z0, R)
+            bm, ba = csr_product_bytes(B * R, m, hwc, nnz)
+            e = {"operator": name, "m": m, "nnz": nnz,
+                 "plain_ms": round(med["plain"], 3), "plain_images_per_s": round(B / med["plain"] * 1e3, 1),
+                 "csr_ms": round(med["csr"], 3), "csr_images_per_s": round(B / med["csr"] * 1e3, 1),
+                 "csr_spread_ms": [round(min(times["csr"]), 3), round(max(times["csr"]), 3)],
+                 "csr_over_plain": round(med["csr"] / med["plain"], 4),
+                 "csr_overhead_per_step_ms": round((med["csr"] - med["plain"]) / L, 4),
+                 "csr_measure_product_ms": round(kt["measure"], 4), "csr_adjoint_product_ms": round(kt["adjoint"], 4),
+                 "csr_measure_bytes": bm, "csr_adjoint_bytes": ba,
+                 "csr_measure_hbm_share": round(bm / (kt["measure"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["measure"] else None,
+                 "csr_adjoint_hbm_share": round(ba / (kt["adjoint"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["adjoint"] else None,
+                 "workspace_bytes_dense": ws_dense, "workspace_bytes_csr": ws_csr}
+            if "dense" in med:
+                e.update({"dense_ms": round(med["dense"], 3), "dense_images_per_s": round(B / med["dense"] * 1e3, 1),
+                          "dense_over_csr": round(med["dense"] / med["csr"], 3)})
+            else:
+                e["dense"] = dense_note
+            print(json.dumps(e), flush=True)
+            r["operators"].append(e)
+            del dense, csr, calls
+            gen._ws = None
+            torch.cuda.empty_cache()
+        r["plain_ms_all"] = [round(t, 3) for t in t_plain]
+        gen.close()
+        res["results"].append(r)
+    os.makedirs(args.out_dir, exist_ok=True)
+    with open(os.path.join(args.out_dir, "measured_bench_sparse.json"), "w") as f:
+        json.dump(res, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("out_dir")
@@ -98,10 +207,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--precision", default="fp16", choices=["fp16", "fp32"])
     ap.add_argument("--user-steps", type=int, default=10)
+    ap.add_argument("--sparse", action="store_true", help="compare plain, dense and CSR calls on sparse operators")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("measured_bench needs a CUDA device")
     dev = torch.device("cuda", 0)
+    if args.sparse:
+        return sparse_main(args, dev)
     res = {"card": card(), "reps": args.reps, "warmup": args.warmup, "precision": args.precision, "results": []}
     for arch, B, R, L, ms in CASES:
         w = O.init_generator_weights(arch)
