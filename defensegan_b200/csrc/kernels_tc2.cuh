@@ -331,8 +331,10 @@ __device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
 // tail included; [8] excludes [12]).  What is left of the warp's cycles after those spans: [12] record wait (full barrier
 // passed -> the step's MMA record read from shared memory and first used), [13] item head (end of the previous item's
 // epilogue, or the PDL wait, -> the first step's operand wait), [14] end wait (end of the last epilogue -> every warp of
-// the CTA has finished, the producer's drain included).  [15] steps the CTA ran.
-constexpr int TC2_PROBE_WORDS = 16;
+// the CTA has finished, the producer's drain included).  [15] steps the CTA ran.  Inside the epilogues [11]: [16] waiting
+// for the epilogue's global inputs (mask words, bias, image and weight pairs: from the point a unit or accumulator needs
+// them to their arrival), [17] waiting for a staging buffer of the TMA store (bulk_wait_read1).
+constexpr int TC2_PROBE_WORDS = 18;
 __device__ unsigned long long g_tc2_probe[48][160][TC2_PROBE_WORDS];
 __device__ __forceinline__ unsigned long long probe_gtime() {
   unsigned long long t;
@@ -345,6 +347,16 @@ __device__ __forceinline__ long long probe_clock_after(uint32_t w0) {
   long long t;
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ge.s32 p, %1, 0;\n\tmov.u64 %0, 0;\n\t@p mov.u64 %0, %%clock64;\n\t}" : "=l"(t) : "r"(w0) : "memory");
   return t;
+}
+// clock64() once `v` has arrived, whatever its bits: both predicated reads depend on it.
+__device__ __forceinline__ long long probe_clock_after64(unsigned long long v) {
+  long long t;
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u64 p, %1, 0;\n\t@p mov.u64 %0, %%clock64;\n\t@!p mov.u64 %0, %%clock64;\n\t}"
+               : "=l"(t) : "l"(v) : "memory");
+  return t;
+}
+__device__ __forceinline__ unsigned long long probe_bits(float2 v) {
+  return ((unsigned long long)__float_as_uint(v.y) << 32) | __float_as_uint(v.x);
 }
 __host__ __device__ constexpr int tc2_probe_key(int n_tile, int epi, int out_bytes) {
   return (n_tile == 256 ? 0 : n_tile == 128 ? 1 : n_tile == 64 ? 2 : n_tile == 48 ? 3 : 4) * 8 + (out_bytes == 4 ? 6 : (epi < 4 ? epi : epi - 4));
@@ -371,7 +383,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #ifdef DGAN_PROBE
   const long long probe_t_start = clock64();
   const unsigned long long probe_g_start = probe_gtime();
-  long long probe_wait_full = 0, probe_issue = 0, probe_wait1 = 0, probe_wait0 = 0, probe_epi = 0;
+  long long probe_wait_full = 0, probe_issue = 0, probe_wait1 = 0, probe_wait0 = 0, probe_epi = 0, probe_in = 0, probe_stage = 0;
   unsigned probe_rec = 0, probe_head = 0, probe_steps = 0;     // 32-bit cycle counts: a launch is far shorter than 2^32 cycles
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -502,12 +514,109 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     for (int i = 0; i < Cfg::ACC_REGS; ++i) acc[i] = 0.f;
     uint32_t item_count = 0, store_count = 0;
     uint32_t ri = rbeg, it = 0;
+    // What the epilogue reads besides the accumulators is requested before the MMAs it follows, so that no global
+    // round trip sits between the item's last MMA and its output.  The item descriptors run one item ahead: item i's
+    // word, window size and pixels arrive during item i-1, and item i's head requests from them, without waiting, its
+    // mask words, its pixel's bias or its image pairs; the epilogue of item i reads registers and shared memory.
+    // (Each TMA store is preceded by fence.proxy.async, which waits for ALL of the warp's outstanding loads: what is
+    // requested at an item's head has long arrived by its epilogue, nothing is requested later.)
+    auto item_desc = [&](int e, int& n, uint32_t& qm) {     // window size and pixels of item word e (-1: none)
+      n = 0; qm = 0u;
+      if (e < 0) return;
+      const TcItem2* ip = items + tc2_item_window(e);
+      n = (int)__ldg(&ip->n_acc);
+      if (lane < 16) qm = (uint32_t)__ldg(&ip->q[lane]);
+    };
+    int e_cur = tc2_item_at(eitems, 0, pair, n_pairs, n_slots), e_nx = tc2_item_at(eitems, 1, pair, n_pairs, n_slots), n_acc_cur;
+    uint32_t q_cur;
+    item_desc(e_cur, n_acc_cur, q_cur);
+    // Per-channel bias (the launch validator gives a per-pixel bias only to N = 256): copied once per CTA into the zero
+    // tile, which these instantiations keep but never write (tc2_issues_zero_ops), and read from there by the epilogue.
+    constexpr bool BIAS_CH = HAS_BIAS && TMA_EPI && N_TILE < 256, BIAS_PX = HAS_BIAS && TMA_EPI && !BIAS_CH;
+    static_assert(!BIAS_CH || (Cfg::ZERO_BYTES >= N_TILE * 4 && !tc2_issues_zero_ops(MAXB, KSUB)), "the bias copy's space");
+    static_assert(!BIAS_PX || MAXB == 1, "a per-pixel bias is held for one accumulator");
+    if constexpr (BIAS_CH) {
+      if (threadIdx.x < N_TILE / 2) {     // float2: the epilogue's loads needed 8-byte alignment only
+        const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias) + threadIdx.x);
+        ptx::st_shared_u32(zero_base + 8u * threadIdx.x, __float_as_uint(b2.x));
+        ptx::st_shared_u32(zero_base + 8u * threadIdx.x + 4u, __float_as_uint(b2.y));
+      }
+      ptx::named_bar_sync(4, TC2_CONSUMERS);
+    }
+    // final kinds: output channels, the bias of each, pairs per row and accumulator
+    constexpr int CO = SIGMOID1 ? 1 : 3, FJ = FINAL ? N_TILE / 8 : 1;
+    // CelebA's weighted kind has no registers for a second set of pairs (it would spill): it requests the pairs of a
+    // row of an accumulator where it uses them.
+    constexpr bool FINAL_PREFETCH = !(WEIGHTED && N_TILE > 32);
+    constexpr int FINAL_HELD = FINAL && N_TILE <= 32 && !(WEIGHTED && MAXB > 4) ? MAXB : 1;
+    const int hwc = fa.w_out * fa.w_out * CO;
+    float bsv[CO];
+    if constexpr (FINAL) {
+#pragma unroll
+      for (int co = 0; co < CO; ++co) bsv[co] = __ldg(bias + co);
+    }
     while (ri < rend) {
-      const int item_e = tc2_item_at(eitems, (int)item_count, pair, n_pairs, n_slots);
-      // what the epilogue needs to know of the item, requested now: two chained global loads that overlap the item's MMAs
-      const TcItem2* ip = items + tc2_item_window(item_e);
-      const int n_acc = (int)__ldg(&ip->n_acc);
-      const uint32_t q_mine = lane < 16 ? (uint32_t)__ldg(&ip->q[lane]) : 0u;
+      const int item_e = e_cur, n_acc = n_acc_cur;
+      const uint32_t q_mine = q_cur;
+      const int mp = tc2_item_mp(item_e);
+      const int tile_row0 = (2 * mp + (int)rank) * kRowTile;
+      const size_t n_lo = (size_t)(tile_row0 + r_lo);
+      // EPI_MASK: the item's mask words, 8 per quad (the four lanes holding the same two rows): lane k of the quad
+      // requests both row words of unit k (accumulator k / G, 64-column group k % G), the epilogue shuffles them.
+      constexpr int G_UNITS = TMA_EPI ? N_TILE / 64 : 1;
+      static_assert(EPI != EPI_MASK || MAXB * G_UNITS == 4, "one mask unit per lane of a quad");
+      unsigned long long mk_pre[2] = {~0ull, ~0ull};
+      if constexpr (EPI == EPI_MASK) {
+        const int ua = (lane & 3) / G_UNITS, ug = (lane & 3) % G_UNITS;
+        const size_t qa = (size_t)__shfl_sync(0xffffffffu, q_mine, ua);
+        if (ua < n_acc) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) mk_pre[h] = __ldg(fa.mb_in + (qa * n_pad + n_lo + 8 * h) * (size_t)(fa.out_ld >> 6) + ug);
+        }
+      }
+      // N = 256 (one accumulator): the bias of its pixel, which may be per pixel (Linear.fwd).  The lanes with the same
+      // lane % 4 need the same columns: lane L requests column pair (g * 8 + L / 4) * 8 + (L % 4) * 2 of every
+      // 64-column group g, and the epilogue shuffles them.
+      float2 bias_px[BIAS_PX ? G_UNITS : 1];
+      if constexpr (BIAS_PX) {
+        const size_t q0 = (size_t)__shfl_sync(0xffffffffu, q_mine, 0);
+        if (n_acc > 0) {
+#pragma unroll
+          for (int g = 0; g < G_UNITS; ++g)
+            bias_px[g] = __ldg(reinterpret_cast<const float2*>(bias + q0 * bias_pstride + (g * 8 + (lane >> 2)) * 8 + (lane & 3) * 2));
+        }
+      }
+      // Final kinds: the image (and weight) pairs of row r_lo + 8 h of accumulator a.  With N = 16 every accumulator's
+      // are requested now (FINAL_HELD = MAXB sets of registers).  Otherwise accumulator 0's are requested now and
+      // accumulator a + 1's row h while accumulator a's row h is used: a row of 16 columns is shorter than a round trip.
+      auto final_pairs = [&](int a, int h, float2 (&xv)[FJ], float2 (&wv)[FJ]) {
+        const int blk = (int)__shfl_sync(0xffffffffu, q_mine, a);
+        const int by = blk / fa.nbx, bx = blk % fa.nbx;
+        const int img = min((int)((n_lo + 8 * h) / fa.R), fa.B - 1);
+#pragma unroll
+        for (int j = 0; j < FJ; ++j) {
+          const int col = j * 8 + (lane & 3) * 2;     // (li * 4 + lj) * CO + co of the 4x4 block
+          const int li = col / (4 * CO), e = col % (4 * CO);
+          const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * CO + e;
+          xv[j] = make_float2(0.f, 0.f);
+          if (fa.x != nullptr) xv[j] = __ldg(reinterpret_cast<const float2*>(fa.x + (size_t)img * hwc + off));
+          wv[j] = make_float2(1.f, 1.f);      // the weight pair next to the image pair (weighted kinds)
+          if (WEIGHTED) wv[j] = __ldg(reinterpret_cast<const float2*>(fa.xw + (size_t)img * hwc + off));
+        }
+      };
+      float2 xp[FINAL_HELD][2][FJ], wp[FINAL_HELD][2][FJ];
+      if constexpr (FINAL && FINAL_PREFETCH) {
+#pragma unroll
+        for (int a = 0; a < FINAL_HELD; ++a) {
+          if (a >= n_acc) break;
+          final_pairs(a, 0, xp[a][0], wp[a][0]);
+          final_pairs(a, 1, xp[a][1], wp[a][1]);
+        }
+      }
+      // the next item's window size and pixels (its word was requested one item earlier), and the word after it
+      item_desc(e_nx, n_acc_cur, q_cur);
+      e_cur = e_nx;
+      e_nx = tc2_item_at(eitems, (int)item_count + 2, pair, n_pairs, n_slots);
       uint32_t flags;
       do {    // the steps of one item
         const uint32_t slot = it & (TC2_NSLOT - 1), phase = (it >> 3) & 1;
@@ -586,35 +695,37 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       // ---- epilogue of the item: accumulator registers -> (bias | ReLU | mask | last layer) -> global memory.
       //      Register i of accumulator a holds column (i % (N_TILE/2)) / 4 * 8 + (lane % 4) * 2 + (i % 2) of row
       //      r_lo + 8 * ((i / 2) % 2) (the m64nNk16 accumulator fragment).
-      const int mp = tc2_item_mp(item_e);
       auto q_of = [&](int a) { return (int)__shfl_sync(0xffffffffu, q_mine, a); };
-      const int tile_row0 = (2 * mp + (int)rank) * kRowTile;
-      const size_t n_lo = (size_t)(tile_row0 + r_lo);
       if constexpr (FINAL) {
-        constexpr int CO = SIGMOID1 ? 1 : 3;
-        const int hwc = fa.w_out * fa.w_out * CO;
-        float bsv[CO];
-#pragma unroll
-        for (int co = 0; co < CO; ++co) bsv[co] = __ldg(bias + co);
 #pragma unroll
         for (int a = 0; a < Cfg::MAXB; ++a) {
           if (a >= n_acc) break;
           const int blk = q_of(a);
           const int by = blk / fa.nbx, bx = blk % fa.nbx;
+#ifdef DGAN_PROBE
+          const long long probe_a0 = clock64();
+#endif
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
+            float2 xa[FJ], wa[FJ];
+            if constexpr (FINAL_PREFETCH) {
+#pragma unroll
+              for (int j = 0; j < FJ; ++j) { xa[j] = xp[a % FINAL_HELD][h][j]; wa[j] = wp[a % FINAL_HELD][h][j]; }
+              if (FINAL_HELD == 1 && a + 1 < Cfg::MAXB && a + 1 < n_acc) final_pairs(a + 1, h, xp[0][h], wp[0][h]);
+            } else {
+              final_pairs(a, h, xa, wa);
+            }
+#ifdef DGAN_PROBE
+            if (h == 0) probe_in += probe_clock_after64(probe_bits(xa[0]) ^ probe_bits(wa[0])) - probe_a0;
+#endif
             const size_t n = n_lo + 8 * h;
-            const int img = min((int)(n / fa.R), fa.B - 1);
             float lsum = 0.f;
 #pragma unroll
             for (int j = 0; j < N_TILE / 8; ++j) {
               const int col = j * 8 + (lane & 3) * 2;     // (li * 4 + lj) * CO + co of the 4x4 block
               const int li = col / (4 * CO), e = col % (4 * CO);
               const size_t off = (size_t)((4 * by + li) * fa.w_out + 4 * bx) * CO + e;
-              float2 xv = make_float2(0.f, 0.f);
-              if (fa.x != nullptr) xv = __ldg(reinterpret_cast<const float2*>(fa.x + (size_t)img * hwc + off));
-              float2 wv = make_float2(1.f, 1.f);      // the weight pair next to the image pair (weighted kinds)
-              if (WEIGHTED) wv = __ldg(reinterpret_cast<const float2*>(fa.xw + (size_t)img * hwc + off));
+              const float2 xv = xa[j], wv = wa[j];
               float yv[2], dv[2];
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
@@ -656,17 +767,33 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           const int q = q_of(a);
 #pragma unroll
           for (int g = 0; g < G; ++g) {
+#ifdef DGAN_PROBE
+            const long long probe_u0 = clock64();
+#endif
             unsigned long long mk[2] = {~0ull, ~0ull}, bits[2] = {0ull, 0ull};
             if (EPI == EPI_MASK) {
 #pragma unroll
-              for (int h = 0; h < 2; ++h) mk[h] = __ldg(fa.mb_in + ((size_t)q * n_pad + n_lo + 8 * h) * GT + g);
+              for (int h = 0; h < 2; ++h) mk[h] = __shfl_sync(0xffffffffu, mk_pre[h], (lane & ~3) | (a * G + g));
+#ifdef DGAN_PROBE
+              probe_in += probe_clock_after64(mk[0] ^ mk[1]) - probe_u0;
+#endif
             }
             uint32_t pk[2][8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const int cl = j * 8 + (lane & 3) * 2;   // column within the 64-column group
               float2 bv = make_float2(0.f, 0.f);
-              if (HAS_BIAS) bv = __ldg(reinterpret_cast<const float2*>(bias + (size_t)q * bias_pstride + g * 64 + cl));
+              if constexpr (BIAS_CH) {
+                const uint2 b2 = ptx::ld_shared_v2(zero_base + (uint32_t)(g * 64 + cl) * 4u);
+                bv = make_float2(__uint_as_float(b2.x), __uint_as_float(b2.y));
+              }
+              if constexpr (BIAS_PX) {
+                bv.x = __shfl_sync(0xffffffffu, bias_px[g].x, j * 4 + (lane & 3));
+                bv.y = __shfl_sync(0xffffffffu, bias_px[g].y, j * 4 + (lane & 3));
+              }
+#ifdef DGAN_PROBE
+              if (HAS_BIAS && j == 0) probe_in += probe_clock_after64(probe_bits(bv)) - probe_u0;
+#endif
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 float v0 = acc[a * (N_TILE / 2) + (g * 8 + j) * 4 + h * 2];
@@ -684,8 +811,14 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
               }
             }
             const uint32_t buf = s_warp + (store_count & 1u) * 2048u;
+#ifdef DGAN_PROBE
+            const long long probe_s0 = clock64();
+#endif
             if (lane == 0) ptx::bulk_wait_read1();     // the store that used this buffer two units ago has read it
             __syncwarp();
+#ifdef DGAN_PROBE
+            probe_stage += clock64() - probe_s0;
+#endif
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -806,6 +939,8 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       atomicAdd(&g_tc2_probe[key][blockIdx.x][9], (unsigned long long)probe_wait1);
       atomicAdd(&g_tc2_probe[key][blockIdx.x][10], (unsigned long long)probe_wait0);
       atomicAdd(&g_tc2_probe[key][blockIdx.x][11], (unsigned long long)probe_epi);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][16], (unsigned long long)probe_in);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][17], (unsigned long long)probe_stage);
     }
     __syncthreads();
     if (threadIdx.x == 0) {

@@ -5,7 +5,9 @@ The second table splits the first consumer warp's cycles into the operand wait, 
 round, the wgmma_wait0 at the end of each item and the epilogues, as shares of its busy cycles, and what is left ("rest")
 into the record wait (operands landed -> the step's MMA record read and first used), the item head (end of an epilogue
 -> the next item's first operand wait), the end wait (last epilogue -> every warp of the CTA done) and the remainder;
-with the steps per CTA and launch, and the record wait in cycles per step.
+with the steps per CTA and launch, and the record wait in cycles per step.  The epilogue's share is split further into
+waiting for its global inputs (mask words, bias, image and weight pairs), waiting for a staging buffer of the TMA store,
+and the rest of it.
 Usage: DGAN_LIB=build_ab/probe.so python tools/probe_step.py [mnist|celeba] [batch] [L] [--json]
 (--json: one JSON object with the time-ordered busy / hand-over table instead of the text tables; bench.py uses it)"""
 import ctypes
@@ -34,7 +36,7 @@ lib = gan._native.lib if hasattr(gan, "_native") and gan._native is not None els
 gan.reconstruct(x, z_init_val=z0)
 torch.cuda.synchronize()
 lib = gan._native.lib
-W = 16                                              # counters per CTA (TC2_PROBE_WORDS)
+W = 18                                              # counters per CTA (TC2_PROBE_WORDS)
 buf = (ctypes.c_ulonglong * (48 * 160 * W))()
 lib.dgan_debug_probe_read.restype = ctypes.c_int
 lib.dgan_debug_probe_read.argtypes = [ctypes.POINTER(ctypes.c_ulonglong)]
@@ -77,9 +79,11 @@ for k in range(48):
     sh = [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (3, 8, 9, 10, 11, 12, 13, 14)]
     steps = a[k, act, 15]
     sh += [float((steps / cnt[act]).mean()), float((a[k, act, 12][steps > 0] / steps[steps > 0]).mean()) if (steps > 0).any() else 0.0]
+    sh += [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (16, 17)]
     split[layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8]))] = dict(
         zip(("operand_wait", "issue", "wgmma_wait1", "wgmma_wait0", "epilogue", "record_wait", "item_head", "end_wait",
-             "steps_per_cta", "record_wait_cycles_per_step"), [round(v, 3) for v in sh]))
+             "steps_per_cta", "record_wait_cycles_per_step", "epilogue_input_wait", "epilogue_staging_wait"),
+            [round(v, 3) for v in sh]))
     timeline.append((int(t0), layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8])), int(g0.max()), float(gf[gf > 0].mean()) if (gf > 0).any() else float(g0.max()),
                      int(g1.max()), 2.0 * kind_flops.get((NT[k // 8], EP[k % 8]), 0.0)))
 # the last launches of the kernels, in time order: how long each was busy and what the hand-over from its predecessor cost
@@ -99,12 +103,14 @@ for t0, name, last_entry, first_full, last_end, flops in timeline:
 print("sum | %.1f | %.1f |" % (tot_busy, tot_gap))
 print()
 print("first consumer warp, share of its busy cycles | operand wait | MMA issue | wgmma_wait1 | wgmma_wait0 | epilogue | rest"
-      " | of rest: record wait | item head | end wait | remainder | steps per CTA | record wait, cycles per step")
+      " | of rest: record wait | item head | end wait | remainder | steps per CTA | record wait, cycles per step"
+      " | of epilogue: input wait | staging wait | rest")
 for name, d in split.items():
     v = list(d.values())
     rest = 1.0 - sum(v[:5])
-    print("%s | %s | %.3f | %s | %.3f | %.1f | %.0f" % (name, " | ".join("%.3f" % x for x in v[:5]), rest,
-                                                      " | ".join("%.3f" % x for x in v[5:8]), rest - sum(v[5:8]), v[8], v[9]))
+    print("%s | %s | %.3f | %s | %.3f | %.1f | %.0f | %.3f | %.3f | %.3f" % (
+        name, " | ".join("%.3f" % x for x in v[:5]), rest, " | ".join("%.3f" % x for x in v[5:8]), rest - sum(v[5:8]), v[8], v[9],
+        v[10], v[11], v[4] - v[10] - v[11]))
 if as_json:
     import json
     rows_out, prev_end = [], None
