@@ -11,6 +11,7 @@ import subprocess
 import sys
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 import torch.autograd.forward_ad as fwAD
 from torch.autograd.function import once_differentiable
@@ -38,6 +39,7 @@ ABI_SYMBOLS = [
     "dgan_workspace_bytes_weighted", "dgan_reconstruct_weighted", "dgan_loss_grad_weighted",
     "dgan_workspace_bytes_measured", "dgan_reconstruct_measured", "dgan_loss_grad_measured",
     "dgan_workspace_bytes_measured_csr", "dgan_reconstruct_measured_csr", "dgan_loss_grad_measured_csr",
+    "dgan_workspace_bytes_pruned", "dgan_reconstruct_pruned",
 ]
 
 
@@ -52,7 +54,44 @@ class dgan_rec_params(ctypes.Structure):
                 ("seed", ctypes.c_uint64), ("z_row_offset", ctypes.c_uint64)]
 
 
+class dgan_prune_point(ctypes.Structure):
+    _fields_ = [("iter", ctypes.c_int32), ("keep", ctypes.c_int32)]
+
+
 ABI_VERSION = 2
+
+
+def check_prune_schedule(prune, rec_rr: int, rec_iters: int):
+    """A restart-pruning schedule as a list of (iter, keep) int pairs, after the rules of dgan_reconstruct_pruned:
+    1 <= iter_1 < iter_2 < ... <= rec_iters - 1 and rec_rr >= keep_1 >= keep_2 >= ... >= 1.  A ValueError names the
+    first bad point."""
+    try:
+        points = [tuple(p) for p in prune]
+    except TypeError:
+        raise ValueError("a prune schedule is a sequence of (iter, keep) pairs, got %r" % (prune,)) from None
+    if not points:
+        raise ValueError("a prune schedule needs at least one (iter, keep) point")
+    out = []
+    prev_it, prev_keep = 0, int(rec_rr)
+    for k, p in enumerate(points):
+        if len(p) != 2 or not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in p):
+            raise ValueError("prune point %d %r: expected a pair of integers (iter, keep)" % (k, p))
+        it, keep = int(p[0]), int(p[1])
+        bad = None
+        if it <= prev_it:
+            bad = "iter must be >= 1" if k == 0 else "iter must exceed the previous point's (%d)" % prev_it
+        elif it > rec_iters - 1:
+            bad = "iter must be <= rec_iters - 1 = %d" % (rec_iters - 1)
+        elif keep < 1:
+            bad = "keep must be >= 1"
+        elif keep > prev_keep:
+            bad = ("keep must be <= rec_rr = %d" % rec_rr) if k == 0 else \
+                "keep must not exceed the previous point's (%d)" % prev_keep
+        if bad is not None:
+            raise ValueError("prune point %d (iter %d, keep %d): %s" % (k, it, keep, bad))
+        out.append((it, keep))
+        prev_it, prev_keep = it, keep
+    return out
 
 
 def _compile(out_path: str, extra_flags: List[str], verbose: bool, force: bool) -> str:
@@ -146,6 +185,11 @@ def load_library() -> ctypes.CDLL:
                                                   vp, vp, sz, vp]
     lib.dgan_loss_grad_measured_csr.restype = i32
     lib.dgan_loss_grad_measured_csr.argtypes = [vp, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_workspace_bytes_pruned.restype = sz
+    lib.dgan_workspace_bytes_pruned.argtypes = [vp, i32, i32, ctypes.POINTER(dgan_prune_point), i32, i32]
+    lib.dgan_reconstruct_pruned.restype = i32
+    lib.dgan_reconstruct_pruned.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ctypes.POINTER(dgan_prune_point), i32, vp,
+                                            vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -261,8 +305,10 @@ class NativeGenerator:
             pass
 
     # -- helpers -------------------------------------------------------------------------
-    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1):
-        if m > 0 and nnz >= 0:
+    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None):
+        if sched is not None:
+            need = int(self.lib.dgan_workspace_bytes_pruned(self._handle, batch, rec_rr, sched, len(sched), int(weighted)))
+        elif m > 0 and nnz >= 0:
             need = int(self.lib.dgan_workspace_bytes_measured_csr(self._handle, batch, rec_rr, int(m), int(nnz)))
         elif m > 0:
             need = int(self.lib.dgan_workspace_bytes_measured(self._handle, batch, rec_rr, int(m)))
@@ -312,10 +358,14 @@ class NativeGenerator:
     def reconstruct(self, images: torch.Tensor, rec_rr: int, rec_iters: int, rec_lr: float = 10.0,
                     z_init_val: Optional[torch.Tensor] = None, seed: int = 0, momentum: float = 0.7,
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
-                    z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None):
+                    z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None,
+                    prune: Optional[Sequence[Sequence[int]]] = None):
         """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
         the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
-        (dgan_reconstruct_weighted)."""
+        (dgan_reconstruct_weighted).
+        prune (a sequence of (iter, keep) pairs, see check_prune_schedule): from iteration iter on, each image keeps only
+        its `keep` restarts of lowest loss at iteration iter - 1 (dgan_reconstruct_pruned); idx is the chosen restart's
+        original index.  None runs every restart to the end."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
@@ -323,6 +373,12 @@ class NativeGenerator:
         if rec_rr <= 0 or rec_iters <= 0 or batch <= 0:
             raise ValueError("batch, rec_rr and rec_iters must be positive")
         pw = self._pixel_weights(pixel_weights, batch)
+        sched = None
+        if prune is not None:
+            if self.use_bn:
+                raise ValueError("restart pruning is not supported with use_bn: the batch statistics couple the rows")
+            points = check_prune_schedule(prune, int(rec_rr), int(rec_iters))
+            sched = (dgan_prune_point * len(points))(*[dgan_prune_point(it, keep) for it, keep in points])
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -335,11 +391,16 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
+            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if pw is None:
+            if sched is not None:
+                rc = self.lib.dgan_reconstruct_pruned(self._handle, ctypes.byref(prm), sched, len(sched), _ptr(x), _ptr(pw),
+                                                      _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                      ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_pruned")
+            elif pw is None:
                 rc = self.lib.dgan_reconstruct(self._handle, ctypes.byref(prm), _ptr(x), _ptr(z0), _ptr(rec), _ptr(loss),
                                                _ptr(idx), ws, need, ctypes.c_void_p(stream))
                 _check(self.lib, rc, "dgan_reconstruct")

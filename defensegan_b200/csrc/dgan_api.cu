@@ -6,6 +6,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <new>
 
@@ -16,6 +17,7 @@
 #include "kernels_vjp.cuh"
 #include "kernels_measured.cuh"
 #include "kernels_measured_csr.cuh"
+#include "kernels_prune.cuh"
 
 namespace dgan {
 
@@ -319,11 +321,18 @@ struct dgan_ctx {
   bool profile = false;
   int n_rows_cur = 0;
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
-  // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise)
-  // on a private stream, replayed with one cudaGraphLaunch per call.
+  // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise,
+  // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise) on a private stream,
+  // replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
+    std::vector<int> prune;
     cudaGraphExec_t exec; int64_t kernels;
+    bool same_key(const LoopGraph& o) const {
+      return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
+             weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
+             momentum == o.momentum && prune == o.prune;
+    }
   };
   std::vector<LoopGraph> graphs;
   cudaStream_t cap_stream = nullptr;
@@ -444,6 +453,11 @@ struct Workspace {
   int nnz = 0;
   int *a_rp = nullptr, *a_ci = nullptr, *at_rp = nullptr, *at_ci = nullptr, *csr_bad = nullptr, *csr_valid = nullptr;
   float *a_v = nullptr, *at_v = nullptr;
+  // the regions of a pruned workspace (prune_maps; kernels_prune.cuh), after all the buffers above: each row's original
+  // restart index [n_pad] (written by the prune point that fills the region; the first region's rows are restarts
+  // 0 .. R-1 of each image and leave it unwritten), the row of the previous region each row was gathered from [n_pad],
+  // and select_kernel's choice per image among its survivors [n_pad] (the last region's only)
+  int *orig = nullptr, *src = nullptr, *sel = nullptr;
   size_t bytes = 0;
 };
 
@@ -455,9 +469,10 @@ static int measured_ld(int m) { return (int)align_up((size_t)m, kMeasTileN); }
 // weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.  m > 0: the workspace of
 // the measured entries for m measurements, the same buffers at the same offsets and the measured ones after all of them.
 // csr_nnz >= 0 (with m > 0): the workspace of the CSR-measured entries for nnz non-zeros, the measured buffers without
-// am / amt and the CSR ones after all of them.
+// am / amt and the CSR ones after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
+// "orig", "src" and "sel" after all the other buffers.
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
-                       int m = 0, int csr_nnz = -1) {
+                       int m = 0, int csr_nnz = -1, bool prune_maps = false) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -560,6 +575,11 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
       w.csr_bad = (int*)take("csr_bad", "i32", {mld});
       w.csr_valid = (int*)take("csr_valid", "i32", {1});
     }
+  }
+  if (prune_maps) {
+    w.orig = (int*)take("orig", "i32", {np});
+    w.src = (int*)take("src", "i32", {np});
+    w.sel = (int*)take("sel", "i32", {np});     // batch <= n_pad
   }
   w.bytes = off;
   return w;
@@ -913,15 +933,22 @@ static int run_tangent(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   return 0;
 }
 
-// z (at the padded latent width) from the caller's z0 [n_rows][latent_dim] or the Philox stream, v = 0
-static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t seed, cudaStream_t s, size_t row_offset = 0) {
-  const int latent = c->desc.latent_dim, ld = c->wd.latent;
-  const size_t total = (size_t)w.n_pad * ld;
+// The state a fresh workspace needs besides z and v: zeroed momentum tickets (fp16 path) and zeroed tile-padding rows of
+// d(pre) (fp32 path).  Memsets only.
+static int clear_start_state(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   if (w.mom_counter != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.mom_counter, 0, (size_t)w.n_pad / kRowTile * sizeof(unsigned), s));
   // fp32 path: the last layer's forward writes dL/dpre for the real rows only while its backward walks all n_pad rows;
   // the tile-padding rows are never observed, but they must not be read uninitialised
   if (w.dblk == nullptr && w.n_pad > w.n_rows)
     DGAN_CUDA_CHECK(cudaMemsetAsync(w.dpre + (size_t)w.n_rows * c->hwc, 0, (size_t)(w.n_pad - w.n_rows) * c->hwc * sizeof(float), s));
+  return 0;
+}
+
+// z (at the padded latent width) from the caller's z0 [n_rows][latent_dim] or the Philox stream, v = 0
+static int run_init_z(dgan_ctx* c, const Workspace& w, const float* z0, uint64_t seed, cudaStream_t s, size_t row_offset = 0) {
+  const int latent = c->desc.latent_dim, ld = c->wd.latent;
+  const size_t total = (size_t)w.n_pad * ld;
+  if (int rc = clear_start_state(c, w, s)) return rc;
   init_z_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w.z, w.v, w.z_h, z0, w.n_rows, w.n_pad, latent, ld, seed,
                                                                 sqrtf(1.0f / (float)latent), row_offset * latent);
   DGAN_LAUNCH_CHECK(c);
@@ -1626,6 +1653,98 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
   return DGAN_OK;
 }
 
+// Iterations t0 .. t1 - 1 of the L-step loop (models/gan.py:409-421) on workspace w, whose rows are `per_image` restarts
+// of each of p.batch images.  Everything it reads or writes lives in the workspace, so it can be captured and replayed.
+// The learning rate follows the global iteration t (decay from ceil(0.8 L) of the full L); iteration L-1, when it is in
+// the range, is its forward alone.  loss_at_end: the forward of iteration t1 - 1 leaves its per-row loss parts in
+// w.loss_part, as the forward of iteration L-1 does (the fp16 path's last-layer forward writes them, and y, only when it
+// is asked for y).
+static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params& p, int per_image, int t0, int t1,
+                         bool measured, cudaStream_t ls, bool loss_at_end = false) {
+  const int latent = h->wd.latent;
+  const int decay_iter = (int)std::ceil(p.rec_iters * 0.8);
+  // fp16: the momentum update (tf.train.MomentumOptimizer, models/gan.py:389-391) runs in the tail of the split-K Linear
+  // backward - the CTA that completes a 128-row tile's partial sums applies it - so an L-step is 8 launches; bit-identical
+  // to the separate kernel the fp32 path uses (same arithmetic, parts summed in the same order)
+  const bool tail = h->desc.precision == DGAN_PREC_FP16;
+  for (int t = t0; t < t1; ++t) {
+    const bool last = (t == p.rec_iters - 1);
+    float lr = p.rec_lr;
+    if (p.decay_lr) lr = p.rec_lr * std::pow(0.1f, (float)(t / decay_iter));
+    // The loop returns the pre-update forward of iteration L-1 (models/gan.py:419-421, SURVEY F4):
+    // the L-th update is never observed, so its backward pass is not run.
+    int r2;
+    if (measured) {
+      // the forward of dgan_vjp (ReLU masks kept, y written every step: the measurement product reads it), then the
+      // measured loss's gradient and the momentum update with the cotangent's row scales divided out
+      if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, per_image, ls))) return r2;
+      if (last) continue;
+      if ((r2 = measured_backward(h, w, ls))) return r2;
+      const size_t zcount = (size_t)w.n_pad * latent;
+      momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
+          w.z, w.v, w.g, w.n_g_parts, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr, latent, w.n_rows, lr,
+          p.momentum, zcount, w.z_h);
+      DGAN_LAUNCH_CHECK(h);
+      continue;
+    }
+    const bool want_y = last || (loss_at_end && t == t1 - 1);
+    if ((r2 = run_forward(h, w, w.x, per_image, p.batch, !last, ls, want_y, w.xw))) return r2;
+    if (last) continue;
+    MomentumArgs mom;
+    mom.lr = lr; mom.mu = p.momentum; mom.tail = tail;
+    if ((r2 = run_backward(h, w, ls, mom))) return r2;
+    if (!tail) {
+      const size_t zcount = (size_t)w.n_pad * latent;
+      ProfScope ps(h, 2 * (int)h->layers.size() + 2, ls);
+      DGAN_CUDA_CHECK(launch_pdl(momentum_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v,
+                                 (const float*)w.g, w.n_g_parts, grad_multiplier(h), lr, p.momentum, zcount, w.z_h));
+      DGAN_LAUNCH_CHECK(h);
+    }
+  }
+  return 0;
+}
+
+// Run a call's loop, enqueue_loop(stream), on s: captured into a CUDA graph the first time `key` (exec and kernels unset)
+// is seen and replayed with one cudaGraphLaunch afterwards, or launched plainly when per-kernel profiling is on or the
+// capture fails.  Adds the stream operations the host issued to *enqueues.
+static int run_loop(dgan_ctx* h, const dgan_ctx::LoopGraph& key, const std::function<int(cudaStream_t)>& enqueue_loop,
+                    cudaStream_t s, int64_t* enqueues) {
+  if (!h->profile && h->cap_stream != nullptr) {      // per-kernel event timing needs the plain launches
+    dgan_ctx::LoopGraph* g = nullptr;
+    for (auto& e : h->graphs)
+      if (e.same_key(key)) { g = &e; break; }
+    if (g == nullptr) {
+      const int64_t k0 = h->launches;
+      cudaGraph_t graph = nullptr;
+      if (cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+        const int crc = enqueue_loop(h->cap_stream);
+        const cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &graph);
+        cudaGraphExec_t exec = nullptr;
+        if (crc == 0 && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
+          if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
+          h->graphs.push_back(key);
+          h->graphs.back().exec = exec;
+          h->graphs.back().kernels = h->launches - k0;
+          g = &h->graphs.back();
+        }
+        if (graph) cudaGraphDestroy(graph);
+      }
+      cudaGetLastError();                     // a failed capture falls back to plain launches below
+      h->launches = k0;                       // captured nodes are counted when they run
+    }
+    if (g != nullptr) {
+      DGAN_CUDA_CHECK(cudaGraphLaunch(g->exec, s));
+      h->launches += g->kernels;
+      *enqueues += 1;
+      return 0;
+    }
+  }
+  const int64_t k0 = h->launches;
+  if (int rc = enqueue_loop(s)) return rc;
+  *enqueues += h->launches - k0;
+  return 0;
+}
+
 // dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
 // weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
 // the workspace only
@@ -1638,12 +1757,10 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   // hyper-parameters, so that a call with batch = 0 tells whether a library refuses a misaligned rec_dev, running nothing
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
   const bool weighted = w_dev != nullptr;
-  const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters, decay_lr = prm->decay_lr;
-  const float rec_lr = prm->rec_lr, momentum = prm->momentum;
+  const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters;
   const uint64_t seed = prm->seed;
   if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
-  const int latent = h->wd.latent;
   Workspace w;
   int rc;
   if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz))) return rc;
@@ -1662,86 +1779,11 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
     DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
     enqueues += 1;
   }
-  // The L-step loop (a function of the workspace and the hyper-parameters only): everything it reads or writes lives in
-  // the workspace, so it can be captured once and replayed.
-  auto enqueue_loop = [&](cudaStream_t ls) -> int {
-    const int decay_iter = (int)std::ceil(rec_iters * 0.8);
-    // fp16: the momentum update (tf.train.MomentumOptimizer, models/gan.py:389-391) runs in the tail of the split-K Linear
-    // backward - the CTA that completes a 128-row tile's partial sums applies it - so an L-step is 8 launches; bit-identical
-    // to the separate kernel the fp32 path uses (same arithmetic, parts summed in the same order)
-    const bool tail = h->desc.precision == DGAN_PREC_FP16;
-    for (int t = 0; t < rec_iters; ++t) {
-      const bool last = (t == rec_iters - 1);
-      float lr = rec_lr;
-      if (decay_lr) lr = rec_lr * std::pow(0.1f, (float)(t / decay_iter));
-      // The loop returns the pre-update forward of iteration L-1 (models/gan.py:419-421, SURVEY F4):
-      // the L-th update is never observed, so its backward pass is not run.
-      int r2;
-      if (measured) {
-        // the forward of dgan_vjp (ReLU masks kept, y written every step: the measurement product reads it), then the
-        // measured loss's gradient and the momentum update with the cotangent's row scales divided out
-        if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, rec_rr, ls))) return r2;
-        if (last) continue;
-        if ((r2 = measured_backward(h, w, ls))) return r2;
-        const size_t zcount = (size_t)w.n_pad * latent;
-        momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
-            w.z, w.v, w.g, w.n_g_parts, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr, latent, w.n_rows, lr,
-            momentum, zcount, w.z_h);
-        DGAN_LAUNCH_CHECK(h);
-        continue;
-      }
-      if ((r2 = run_forward(h, w, w.x, rec_rr, batch, !last, ls, /*want_y=*/last, w.xw))) return r2;
-      if (last) continue;
-      MomentumArgs mom;
-      mom.lr = lr; mom.mu = momentum; mom.tail = tail;
-      if ((r2 = run_backward(h, w, ls, mom))) return r2;
-      if (!tail) {
-        const size_t zcount = (size_t)w.n_pad * latent;
-        ProfScope ps(h, 2 * (int)h->layers.size() + 2, ls);
-        DGAN_CUDA_CHECK(launch_pdl(momentum_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v,
-                                   (const float*)w.g, w.n_g_parts, grad_multiplier(h), lr, momentum, zcount, w.z_h));
-        DGAN_LAUNCH_CHECK(h);
-      }
-    }
-    return 0;
-  };
-  bool replayed = false;
-  if (!h->profile && h->cap_stream != nullptr) {      // per-kernel event timing needs the plain launches
-    dgan_ctx::LoopGraph* g = nullptr;
-    for (auto& e : h->graphs)
-      if (e.ws == ws && e.batch == batch && e.rec_rr == rec_rr && e.rec_iters == rec_iters && e.decay_lr == decay_lr &&
-          e.weighted == (int)weighted && e.measured == meas.m && e.csr_nnz == meas.nnz && e.rec_lr == rec_lr &&
-          e.momentum == momentum) { g = &e; break; }
-    if (g == nullptr) {
-      const int64_t k0 = h->launches;
-      cudaGraph_t graph = nullptr;
-      if (cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-        const int crc = enqueue_loop(h->cap_stream);
-        const cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &graph);
-        cudaGraphExec_t exec = nullptr;
-        if (crc == 0 && ce == cudaSuccess && graph != nullptr && cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess) {
-          if (h->graphs.size() >= 8) { cudaGraphExecDestroy(h->graphs.front().exec); h->graphs.erase(h->graphs.begin()); }
-          h->graphs.push_back({ws, batch, rec_rr, rec_iters, decay_lr, (int)weighted, meas.m, meas.nnz, rec_lr, momentum,
-                               exec, h->launches - k0});
-          g = &h->graphs.back();
-        }
-        if (graph) cudaGraphDestroy(graph);
-      }
-      cudaGetLastError();                     // a failed capture falls back to plain launches below
-      h->launches = k0;                       // captured nodes are counted when they run
-    }
-    if (g != nullptr) {
-      DGAN_CUDA_CHECK(cudaGraphLaunch(g->exec, s));
-      h->launches += g->kernels;
-      enqueues += 1;
-      replayed = true;
-    }
-  }
-  if (!replayed) {
-    const int64_t k0 = h->launches;
-    if ((rc = enqueue_loop(s))) return rc;
-    enqueues += h->launches - k0;
-  }
+  // The L-step loop (a function of the workspace and the hyper-parameters only)
+  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
+                          prm->momentum, {}, nullptr, 0};
+  auto enqueue_loop = [&](cudaStream_t ls) -> int { return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls); };
+  if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
   {
     const int n_rows = batch * rec_rr;
     if (measured) {
@@ -1757,6 +1799,165 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   h->last_enqueues = enqueues;
   h->last_launches = h->launches - launches0;
   return DGAN_OK;
+}
+
+// ---- restart pruning (dgan_reconstruct_pruned; kernels_prune.cuh) ------------------------------------------------------
+// A schedule of n_points prune points: 1 <= iter_1 < iter_2 < ... (<= L - 1 when rec_iters > 0: the sizer does not know L)
+// and rec_rr >= keep_1 >= keep_2 >= ... >= 1.  0, or DGAN_ERR_INVALID_ARG naming the bad point.
+static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_rr, int rec_iters) {
+  if (sched == nullptr || n_points < 1) { set_error("a prune schedule needs at least one point (sched NULL or n_points < 1)"); return DGAN_ERR_INVALID_ARG; }
+  if (rec_rr > kPruneMaxRestarts) {
+    set_error("rec_rr = " + std::to_string(rec_rr) + ": a pruned call takes at most " + std::to_string(kPruneMaxRestarts) + " restarts");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  for (int k = 0; k < n_points; ++k) {
+    const int it = sched[k].iter, keep = sched[k].keep;
+    const int prev_it = k == 0 ? 0 : sched[k - 1].iter, prev_keep = k == 0 ? rec_rr : sched[k - 1].keep;
+    std::string bad;
+    if (it <= prev_it) bad = k == 0 ? "iter must be >= 1" : "iter must exceed the previous point's";
+    else if (rec_iters > 0 && it > rec_iters - 1) bad = "iter must be <= rec_iters - 1 = " + std::to_string(rec_iters - 1);
+    else if (keep < 1) bad = "keep must be >= 1";
+    else if (keep > prev_keep) bad = k == 0 ? "keep must be <= rec_rr = " + std::to_string(rec_rr) : "keep must not exceed the previous point's";
+    if (!bad.empty()) {
+      set_error("prune point " + std::to_string(k) + " (iter " + std::to_string(it) + ", keep " + std::to_string(keep) + "): " + bad);
+      return DGAN_ERR_INVALID_ARG;
+    }
+  }
+  return 0;
+}
+
+// The regions of a pruned workspace: region 0 for batch * rec_rr rows, region k for batch * keep_k rows, each a carve()
+// with the prune maps, one after the other (every carve is a multiple of 1024 bytes).  *bytes: the total; layout (not
+// NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
+static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
+                                           int n_points, void* base, bool weighted, size_t* bytes,
+                                           std::string* layout = nullptr) {
+  std::vector<Workspace> regs;
+  size_t off = 0;
+  for (int k = 0; k <= n_points; ++k) {
+    const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
+    if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
+    regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, 0, -1, true));
+    off += regs.back().bytes;
+  }
+  *bytes = off;
+  return regs;
+}
+
+// Plan every stage's row count (and the weighted pass).
+static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched, int n_points, bool weighted) {
+  int rc;
+  for (int k = 0; k <= n_points; ++k) {
+    const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
+    if ((rc = plan_all(c, rows))) return rc;
+    if (weighted && (rc = plan_pass(c, rows, TC_PASS_WEIGHTED))) return rc;
+  }
+  return 0;
+}
+
+static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
+                                   const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
+                                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (h == nullptr || prm == nullptr || x_dev == nullptr || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
+  const bool weighted = w_dev != nullptr;
+  const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters;
+  if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
+  int rc;
+  if ((rc = check_schedule(sched, n_points, rec_rr, rec_iters))) return rc;
+  if (h->desc.use_bn) {
+    set_error("restart pruning is not supported with use_bn: the batch statistics couple the rows, so dropping restarts "
+              "would change the survivors' trajectories");
+    return DGAN_ERR_UNSUPPORTED;
+  }
+  if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
+  if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
+  if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, weighted))) return rc;
+  size_t need = 0;
+  std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need);
+  if (need > ws_bytes) {
+    set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
+              " (dgan_workspace_bytes_pruned)");
+    return DGAN_ERR_WORKSPACE;
+  }
+  for (Workspace& w : regs) {
+    if ((rc = build_maps(h, w))) return rc;
+    if (weighted && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t launches0 = h->launches;
+  int64_t enqueues = 0;
+  // every region starts as a fresh workspace would: region 0 from z0, the others' z and v come from the prune points
+  for (int k = 0; k <= n_points; ++k) {
+    const Workspace& w = regs[(size_t)k];
+    const int64_t l0 = h->launches;
+    if (k == 0) {
+      if ((rc = run_init_z(h, w, z0_dev, prm->seed, s, (size_t)prm->z_row_offset))) return rc;
+    } else if ((rc = clear_start_state(h, w, s))) {
+      return rc;
+    }
+    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (weighted) DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    enqueues += (h->launches - l0) + 1 + (weighted ? 1 : 0);
+  }
+  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, 0, -1, prm->rec_lr, prm->momentum,
+                          {}, nullptr, 0};
+  for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
+  // the stages and, between them, the prune points: the loss of iteration iter_k - 1 per row (still in loss_part after
+  // that iteration's update), the survivors' maps and the gather of their z, v (and z_h) into the next region
+  auto enqueue_loop = [&](cudaStream_t ls) -> int {
+    int r2;
+    for (int k = 0; k <= n_points; ++k) {
+      const Workspace& w = regs[(size_t)k];
+      const int per = k == 0 ? rec_rr : sched[k - 1].keep;
+      const int t0 = k == 0 ? 0 : sched[k - 1].iter, t1 = k == n_points ? rec_iters : sched[k].iter;
+      h->n_rows_cur = w.n_rows;
+      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, false, ls, k < n_points))) return r2;
+      if (k == n_points) break;
+      const Workspace& nx = regs[(size_t)k + 1];
+      loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, ls>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
+                                                                 1.0f / (float)h->hwc, w.n_rows, w.loss);
+      DGAN_LAUNCH_CHECK(h);
+      prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sched[k].keep, nx.src, nx.orig);
+      DGAN_LAUNCH_CHECK(h);
+      const size_t total = (size_t)nx.n_pad * h->wd.latent;
+      prune_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.z_h, nx.src, nx.n_rows, nx.n_pad,
+                                                                          h->wd.latent, nx.z, nx.v, nx.z_h);
+      DGAN_LAUNCH_CHECK(h);
+    }
+    return 0;
+  };
+  if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
+  const Workspace& w = regs.back();
+  const int per = sched[n_points - 1].keep;
+  h->n_rows_cur = w.n_rows;
+  loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
+                                                            1.0f / (float)h->hwc, w.n_rows, w.loss);
+  DGAN_LAUNCH_CHECK(h);
+  select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, w.sel);
+  DGAN_LAUNCH_CHECK(h);
+  prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
+  DGAN_LAUNCH_CHECK(h);
+  enqueues += 3;
+  h->last_enqueues = enqueues;
+  h->last_launches = h->launches - launches0;
+  return DGAN_OK;
+}
+
+size_t dgan_workspace_bytes_pruned(dgan_handle h, int batch, int rec_rr, const dgan_prune_point* sched, int n_points,
+                                   int weighted) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, weighted != 0) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes);
+  return bytes;
+}
+
+int dgan_reconstruct_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
+                            const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                            int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                                 stream);
 }
 
 int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* z0_dev, float* rec_dev,
@@ -2118,6 +2319,21 @@ int dgan_debug_workspace_layout_measured(dgan_handle h, int n_rows, int m, char*
 int dgan_debug_workspace_layout_measured_csr(dgan_handle h, int n_rows, int m, int nnz, char* buf, int buf_len) {
   if (h == nullptr || m <= 0 || m > h->hwc || !csr_nnz_ok(h, m, nnz)) { set_error("invalid argument"); return -1; }
   return workspace_layout_impl(h, n_rows, buf, buf_len, false, m, nnz);
+}
+
+// The same for the workspace of dgan_reconstruct_pruned (dgan_workspace_bytes_pruned): per region a line
+// "region k byte_offset n_rows" (the offset from the workspace's start), then that region's lines as above - offsets
+// relative to the region - ending with the prune maps "orig", "src" and "sel", i32 [n_pad] each.
+int dgan_debug_workspace_layout_pruned(dgan_handle h, int batch, int rec_rr, const dgan_prune_point* sched, int n_points,
+                                       int weighted, char* buf, int buf_len) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
+  if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
+  std::string out;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out);
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -117,6 +117,7 @@ class DefenseGANBase(object):
         self.precision = "fp32"            # 'fp32' (CUDA-core, reference arithmetic) | 'fp16' (wgmma operands)
         self.rec_momentum = 0.7            # tf.train.MomentumOptimizer(momentum=0.7), models/gan.py:389-391
         self.rec_decay_lr = False          # the reference's decay is dead code (SURVEY F3); True = intended schedule
+        self.rec_prune = None              # restart pruning: [(iter, keep), ...] (cfg REC_PRUNE); None = every restart to the end
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
 
         self.test_mode = test_mode
@@ -335,7 +336,16 @@ class DefenseGANBase(object):
         no renormalisation).  The returned loss and the arg-min restart use the weighted loss; an image whose weights are
         all 0 keeps its z0 and restart 0 is chosen.  With weights of 1 the result is bit-identical to the unweighted
         call.  The weights are checked before any native call - a ValueError for non-finite values or values outside
-        [0, 1] - at the cost of one device reduction and one host read, on the weighted path only."""
+        [0, 1] - at the cost of one device reduction and one host read, on the weighted path only.
+
+        `rec_prune` (an extension, read at call time; None by default): a list of (iter, keep) pairs,
+        1 <= iter_1 < iter_2 < ... <= rec_iters - 1 and rec_rr >= keep_1 >= keep_2 >= ... >= 1.  From iteration iter_k on,
+        each image runs only its keep_k restarts of lowest loss at iteration iter_k - 1 (ties: the lower restart index;
+        NaN last); the survivors follow exactly the trajectories they would follow unpruned, and the arg-min picks among
+        the last survivors (`return_aux`'s restart is the original index).  It cuts the row-steps of a call, at the risk of
+        dropping a restart that would have won.  The schedule is checked before any native call (a ValueError naming the
+        bad point), and refused with use_bn, whose batch statistics couple the restarts."""
+        prune = self._prune_schedule()
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
@@ -346,10 +356,21 @@ class DefenseGANBase(object):
         native = self._get_native(x.device)
         self.last_seed = seed = self._next_seed(reconstructor_id)
         kw = {} if pw is None else {"pixel_weights": pw}
+        if prune is not None:
+            kw["prune"] = prune
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
         return res
+
+    def _prune_schedule(self):
+        """`rec_prune` checked against rec_rr and rec_iters (None when unset); ValueError before any native call."""
+        if self.rec_prune is None:
+            return None
+        if bool(self.use_bn):
+            raise ValueError("rec_prune is not supported with use_bn: the batch statistics couple the restarts, so "
+                             "dropping some would change the others' trajectories")
+        return _native.check_prune_schedule(self.rec_prune, int(self.rec_rr), int(self.rec_iters))
 
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
                              z_row_offset=0):
@@ -369,7 +390,11 @@ class DefenseGANBase(object):
         have a few non-zeros per row.  A CSR operator is checked too (2-D, not batched or hybrid, crow_indices rising
         from 0 to nnz, column indices in range and strictly ascending within each row).  On fp32 the result is
         bit-identical to the dense call on the same matrix; on fp16 a sparse operator is applied in fp32, so it differs
-        from the dense call (TF32) by the TF32 rounding of the operator and the operands."""
+        from the dense call (TF32) by the TF32 rounding of the operator and the operands.
+
+        Restart pruning (`rec_prune`) is not available here: a call with it set raises a ValueError."""
+        if self.rec_prune is not None:
+            raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts: set rec_prune = None")
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
                                                      z_row_offset)
@@ -467,13 +492,16 @@ class DefenseGANBase(object):
             self.test_gen_test = test
 
     def rec_cache_dir(self, split: str, max_num: int = -1) -> str:
-        """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}]/<split>[_debug]` - the directory name the
-        callers parse back with `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651)."""
+        """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]/<split>[_debug]`
+        - the directory name the callers parse back with `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the
+        `_prune` part (only with `rec_prune` set) keeps pruned and unpruned reconstructions apart."""
         if max_num > 0:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}_num{:d}'.format(int(self.rec_rr), float(self.rec_lr),
                                                                    int(self.rec_iters), int(max_num))
         else:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}'.format(int(self.rec_rr), float(self.rec_lr), int(self.rec_iters))
+        if self.rec_prune is not None:
+            name += '_prune' + '-'.join('{:d}x{:d}'.format(int(it), int(keep)) for it, keep in self.rec_prune)
         out = os.path.join(self.checkpoint_dir, name, split)
         if self.debug:
             out += '_debug'

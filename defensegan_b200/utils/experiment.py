@@ -169,12 +169,14 @@ def get_cached_gan_data(gan, test_on_dev, orig_data_flag=None, flags: Optional[F
 # reconstruction hyper-parameters and result files
 # ------------------------------------------------------------------------------------------------------------------
 _REC_DIR_RE = re.compile(r"recs_rr(.*)_lr(.*)_iters(.*)")
+_REC_PRUNE_RE = re.compile(r"_prune(\d+x\d+(?:-\d+x\d+)*)")
 
 
 def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
     """blackbox.py:639-658 / whitebox.py:245-264: with `--rec_path` and `--defense_type defense_gan` the projection's
-    hyper-parameters are parsed back from the cache directory name (`rec_cache_dir`); `--override` applies the
-    `--rec_rr / --rec_lr / --rec_iters` values instead of the model cfg's."""
+    hyper-parameters are parsed back from the cache directory name (`rec_cache_dir`), the restart-pruning schedule
+    (`_prune<it>x<keep>[-<it>x<keep>...]`) included: `gan.rec_prune` becomes that schedule, or None when the name has
+    none; `--override` applies the `--rec_rr / --rec_lr / --rec_iters` values instead of the model cfg's."""
     cfg = cfg or {}
     rr = cfg.get("REC_RR", gan.rec_rr)
     lr = cfg.get("REC_LR", gan.rec_lr)
@@ -188,6 +190,8 @@ def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
             rr, lr, iters = found[0]
             iters = re.split(r"[/_]", str(iters))[0]            # `..._iters200/train`, `..._iters200_num500`
             gan.rec_rr, gan.rec_lr, gan.rec_iters = int(rr), float(lr), int(iters)
+            prune = _REC_PRUNE_RE.findall(flags.rec_path)
+            gan.rec_prune = [tuple(int(v) for v in p.split("x")) for p in prune[0].split("-")] if prune else None
         elif defense == "defense_gan":
             assert flags.online_training or not flags.train_on_recs
     if flags.override:

@@ -204,6 +204,44 @@ int dgan_loss_grad_measured_csr(dgan_handle h, const int32_t* row_ptr, const int
                                 float* loss_dev, float* grad_dev, void* workspace, size_t workspace_bytes,
                                 void* stream);
 
+/* One prune point of a pruned projection, in host memory. */
+typedef struct dgan_prune_point {
+  int32_t iter; /* the iteration from which on the image's survivors run alone */
+  int32_t keep; /* restarts each image keeps */
+} dgan_prune_point;
+
+/* Bytes of scratch for dgan_reconstruct_pruned with this schedule (weighted != 0: with per-pixel weights): one region
+ * per stage, one after the other, each the workspace that dgan_workspace_bytes or dgan_workspace_bytes_weighted carves
+ * for that stage's rows - batch * rec_rr, then batch * keep_k - plus three int32 maps of its rows.  Also plans every
+ * stage's row count.  0 for a handle with use_bn and for a schedule that breaks the rules of dgan_reconstruct_pruned,
+ * except iter <= rec_iters - 1, as L is not known here. */
+size_t dgan_workspace_bytes_pruned(dgan_handle h, int batch, int rec_rr, const dgan_prune_point* sched, int n_points,
+                                   int weighted);
+
+/* dgan_reconstruct with w_dev NULL, dgan_reconstruct_weighted otherwise (w_dev as there), that drops each image's worst restarts
+ * partway through the loop (an extension: the reference runs every restart to the end).  sched [n_points] in host
+ * memory: 1 <= iter_1 < iter_2 < ... < iter_n <= rec_iters - 1 and rec_rr >= keep_1 >= ... >= keep_n >= 1.
+ *   At prune point k, after iteration iter_k - 1 has run with its update: each image's surviving restarts are ranked by
+ *   their loss at iteration iter_k - 1 (lower first; ties by the lower original restart index; NaN after every number)
+ *   and the first keep_k go on, with their z and momentum unchanged, image-major and in ascending original restart
+ *   index.  Iterations iter_k .. run on batch * keep_k rows; the learning rate follows the global iteration (decay_lr
+ *   from ceil(0.8 rec_iters)).  The arg-min select of dgan_reconstruct then picks among the last survivors: rec_dev and
+ *   loss_dev are that survivor's G(z_{L-1}) and loss, idx_dev its original restart index in [0, rec_rr).
+ * Rows are independent without BatchNorm, so each survivor follows exactly its unpruned trajectory: keep_k = rec_rr at
+ * every point gives dgan_reconstruct's bits.  use_bn couples the rows: DGAN_ERR_UNSUPPORTED.  A schedule that breaks the
+ * rules, NULL arguments or a misaligned rec_dev: DGAN_ERR_INVALID_ARG; a workspace smaller than
+ * dgan_workspace_bytes_pruned: DGAN_ERR_WORKSPACE; nothing is enqueued in either case.
+ * Before the captured loop the host enqueues the z0 initialiser (into region 0), the zeroing of each later region's
+ * momentum tickets or d(pre) padding rows (memsets, not counted, as in dgan_reconstruct) and one image copy per region
+ * (with w_dev, one weight copy per region too).  The loop - every stage's L-steps and, at each prune point, the loss sum,
+ * prune_select_kernel and prune_gather_kernel - is one CUDA graph per (workspace, hyper-parameters, schedule).  After it:
+ * loss sum, arg-min select and the mapping of the chosen survivor to its original index.  So, with P = n_points,
+ * dgan_last_launch_count is that of dgan_reconstruct or dgan_reconstruct_weighted with the same rec_iters + 3 P + 1, and
+ * dgan_last_enqueue_count is theirs + P (image copies; 2 P with w_dev) + 1. */
+int dgan_reconstruct_pruned(dgan_handle h, const dgan_rec_params* params, const dgan_prune_point* sched, int n_points,
+                            const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                            int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -251,12 +289,12 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
  * 256 channels, 1 + 10 L - 5 + 2).  A dgan_reconstruct_measured call runs 3 + 6 (L - 1) + 1 kernels more with
  * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there); a dgan_reconstruct_measured_csr call
- * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more. */
+ * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more; a dgan_reconstruct_pruned call with P prune points 3 P + 1 more. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
- * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind and
- * nnz) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
+ * nnz and prune schedule) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
  * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them),
  * graph, loss sum, arg-min select. */
 int64_t dgan_last_enqueue_count(dgan_handle h);
