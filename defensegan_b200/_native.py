@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "dgan_workspace_bytes_measured", "dgan_reconstruct_measured", "dgan_loss_grad_measured",
     "dgan_workspace_bytes_measured_csr", "dgan_reconstruct_measured_csr", "dgan_loss_grad_measured_csr",
     "dgan_workspace_bytes_pruned", "dgan_reconstruct_pruned",
+    "dgan_workspace_bytes_measured_pruned", "dgan_reconstruct_measured_pruned", "dgan_reconstruct_measured_csr_pruned",
 ]
 
 
@@ -190,6 +191,14 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_pruned.restype = i32
     lib.dgan_reconstruct_pruned.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ctypes.POINTER(dgan_prune_point), i32, vp,
                                             vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_workspace_bytes_measured_pruned.restype = sz
+    lib.dgan_workspace_bytes_measured_pruned.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(dgan_prune_point), i32]
+    lib.dgan_reconstruct_measured_pruned.restype = i32
+    lib.dgan_reconstruct_measured_pruned.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ctypes.POINTER(dgan_prune_point), i32,
+                                                     vp, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_csr_pruned.restype = i32
+    lib.dgan_reconstruct_measured_csr_pruned.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ctypes.POINTER(dgan_prune_point),
+                                                         i32, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -306,7 +315,10 @@ class NativeGenerator:
 
     # -- helpers -------------------------------------------------------------------------
     def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None):
-        if sched is not None:
+        if sched is not None and m > 0:
+            need = int(self.lib.dgan_workspace_bytes_measured_pruned(self._handle, batch, rec_rr, int(m), int(nnz), sched,
+                                                                     len(sched)))
+        elif sched is not None:
             need = int(self.lib.dgan_workspace_bytes_pruned(self._handle, batch, rec_rr, sched, len(sched), int(weighted)))
         elif m > 0 and nnz >= 0:
             need = int(self.lib.dgan_workspace_bytes_measured_csr(self._handle, batch, rec_rr, int(m), int(nnz)))
@@ -373,12 +385,7 @@ class NativeGenerator:
         if rec_rr <= 0 or rec_iters <= 0 or batch <= 0:
             raise ValueError("batch, rec_rr and rec_iters must be positive")
         pw = self._pixel_weights(pixel_weights, batch)
-        sched = None
-        if prune is not None:
-            if self.use_bn:
-                raise ValueError("restart pruning is not supported with use_bn: the batch statistics couple the rows")
-            points = check_prune_schedule(prune, int(rec_rr), int(rec_iters))
-            sched = (dgan_prune_point * len(points))(*[dgan_prune_point(it, keep) for it, keep in points])
+        sched = self._schedule(prune, rec_rr, rec_iters)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -412,6 +419,16 @@ class NativeGenerator:
         if return_aux:
             return rec, loss, idx
         return rec
+
+    def _schedule(self, prune, rec_rr: int, rec_iters: int):
+        """A prune schedule as the dgan_prune_point array of the pruned entries (None stays None), checked with
+        check_prune_schedule and refused with use_bn."""
+        if prune is None:
+            return None
+        if self.use_bn:
+            raise ValueError("restart pruning is not supported with use_bn: the batch statistics couple the rows")
+        points = check_prune_schedule(prune, int(rec_rr), int(rec_iters))
+        return (dgan_prune_point * len(points))(*[dgan_prune_point(it, keep) for it, keep in points])
 
     def _measured(self, measurements: torch.Tensor, operator: torch.Tensor):
         """(y, A, batch, m): the measurements as a contiguous CUDA float32 [batch, m] tensor and the operator as [m, H*W*C]
@@ -451,13 +468,17 @@ class NativeGenerator:
     def reconstruct_measured(self, measurements: torch.Tensor, operator: torch.Tensor, rec_rr: int, rec_iters: int,
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
-                             return_aux: bool = False, z_row_offset: int = 0):
+                             return_aux: bool = False, z_row_offset: int = 0,
+                             prune: Optional[Sequence[Sequence[int]]] = None):
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
         the arg-min restart as [B, H, W, C] (with return_aux also the minimum measured loss [B] and the restart [B]).
         A torch sparse CSR operator (operator.layout == torch.sparse_csr, columns strictly ascending within each row)
-        runs dgan_reconstruct_measured_csr: the same semantics, at a cost set by its non-zeros."""
+        runs dgan_reconstruct_measured_csr: the same semantics, at a cost set by its non-zeros.
+        prune (a sequence of (iter, keep) pairs, see check_prune_schedule): restart pruning as in reconstruct, ranked by
+        the measured loss (dgan_reconstruct_measured_pruned, or dgan_reconstruct_measured_csr_pruned for a CSR operator).
+        None runs every restart to the end."""
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -465,6 +486,7 @@ class NativeGenerator:
             y, a, batch, m = self._measured(measurements, operator)
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
+        sched = self._schedule(prune, rec_rr, rec_iters)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -477,11 +499,22 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1)
+            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if csr:
+            if sched is not None and csr:
+                rc = self.lib.dgan_reconstruct_measured_csr_pruned(self._handle, ctypes.byref(prm), sched, len(sched),
+                                                                   _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
+                                                                   _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                                   ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_csr_pruned")
+            elif sched is not None:
+                rc = self.lib.dgan_reconstruct_measured_pruned(self._handle, ctypes.byref(prm), sched, len(sched), _ptr(a), m,
+                                                               _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                               ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_pruned")
+            elif csr:
                 rc = self.lib.dgan_reconstruct_measured_csr(self._handle, ctypes.byref(prm), _ptr(rp), _ptr(ci), _ptr(val),
                                                             m, nnz, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
                                                             ws, need, ctypes.c_void_p(stream))

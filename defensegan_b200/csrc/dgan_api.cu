@@ -464,36 +464,60 @@ struct Workspace {
 // The padded measurement count of a measured workspace: m rounded up to the measurement products' N tile.
 static int measured_ld(int m) { return (int)align_up((size_t)m, kMeasTileN); }
 
-// The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer - name, element type, byte
-// offset and dims in storage order (outermost first) - for dgan_debug_workspace_layout.  weighted: the workspace of the
-// weighted entries, the same buffers at the same offsets and the weights "xw" after all of them.  m > 0: the workspace of
-// the measured entries for m measurements, the same buffers at the same offsets and the measured ones after all of them.
+// The next buffer of a workspace being carved from b (NULL: sizes only) at *off: the dims' product of elements of type
+// `type`, one of the element types below, 1024-byte aligned.  layout (not NULL) receives its line: name, element type,
+// byte offset and dims in storage order (outermost first).
+static void* carve_take(char* b, size_t* off, std::string* layout, const std::string& name, const char* type,
+                        std::initializer_list<size_t> dims) {
+  struct ElemType { const char* name; size_t bytes; };
+  static const ElemType kTypes[] = {{"f32", 4}, {"f16", 2}, {"u64", 8}, {"u32", 4}, {"i32", 4}};
+  size_t bytes = 0;
+  for (const ElemType& t : kTypes)
+    if (strcmp(t.name, type) == 0) bytes = t.bytes;
+  for (size_t d : dims) bytes *= d;
+  if (layout != nullptr) {
+    *layout += name + " " + type + " " + std::to_string(*off);
+    for (size_t d : dims) *layout += " " + std::to_string(d);
+    *layout += "\n";
+  }
+  void* p = b ? (void*)(b + *off) : nullptr;
+  *off += align_up(bytes, 1024);
+  return p;
+}
+
+// The staged CSR operator of a workspace w whose m_ld is set, for nnz non-zeros: a_rp [m_ld + 1], a_ci / a_v [nnz], the
+// transpose's at_rp [H*W*C + 1], at_ci / at_v [nnz], csr_bad [m_ld] and csr_valid [1] (carve_take's arguments).
+static void carve_csr(const dgan_ctx* c, Workspace* w, int nnz_, char* b, size_t* off, std::string* layout) {
+  const size_t mld = (size_t)w->m_ld, hwc = (size_t)c->hwc, nnz = (size_t)nnz_;
+  w->nnz = nnz_;
+  w->a_rp = (int*)carve_take(b, off, layout, "a_rp", "i32", {mld + 1});
+  w->a_ci = (int*)carve_take(b, off, layout, "a_ci", "i32", {nnz});
+  w->a_v = (float*)carve_take(b, off, layout, "a_v", "f32", {nnz});
+  w->at_rp = (int*)carve_take(b, off, layout, "at_rp", "i32", {hwc + 1});
+  w->at_ci = (int*)carve_take(b, off, layout, "at_ci", "i32", {nnz});
+  w->at_v = (float*)carve_take(b, off, layout, "at_v", "f32", {nnz});
+  w->csr_bad = (int*)carve_take(b, off, layout, "csr_bad", "i32", {mld});
+  w->csr_valid = (int*)carve_take(b, off, layout, "csr_valid", "i32", {1});
+}
+
+// The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer (carve_take) for
+// dgan_debug_workspace_layout.  weighted: the workspace of the weighted entries, the same buffers at the same offsets and
+// the weights "xw" after all of them.  m > 0: the workspace of the measured entries for m measurements, the same buffers
+// at the same offsets and the measured ones after all of them.
 // csr_nnz >= 0 (with m > 0): the workspace of the CSR-measured entries for nnz non-zeros, the measured buffers without
 // am / amt and the CSR ones after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
-// "orig", "src" and "sel" after all the other buffers.
+// "orig", "src" and "sel" after all the other buffers.  op (not NULL, with m > 0): a region of a pruned measured
+// workspace, whose operator - am / amt or the CSR buffers - and ym live in the operator block op (carve_operator): only
+// the row-sized measured buffers are carved, the others are op's.
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
-                       int m = 0, int csr_nnz = -1, bool prune_maps = false) {
+                       int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
   size_t off = 0;
   char* b = (char*)base;
-  // a buffer of the dims' product of elements of type `type`, one of the element types below
-  struct ElemType { const char* name; size_t bytes; };
-  static const ElemType kTypes[] = {{"f32", 4}, {"f16", 2}, {"u64", 8}, {"u32", 4}, {"i32", 4}};
   auto take = [&](const std::string& name, const char* type, std::initializer_list<size_t> dims) -> void* {
-    size_t bytes = 0;
-    for (const ElemType& t : kTypes)
-      if (strcmp(t.name, type) == 0) bytes = t.bytes;
-    for (size_t d : dims) bytes *= d;
-    if (layout != nullptr) {
-      *layout += name + " " + type + " " + std::to_string(off);
-      for (size_t d : dims) *layout += " " + std::to_string(d);
-      *layout += "\n";
-    }
-    void* p = b ? (void*)(b + off) : nullptr;
-    off += align_up(bytes, 1024);
-    return p;
+    return carve_take(b, &off, layout, name, type, dims);
   };
   const size_t np = (size_t)w.n_pad;
   const size_t latent = (size_t)c->wd.latent;      // z, v, g and z_h are stored at the padded latent width
@@ -554,26 +578,23 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.m_ld = measured_ld(m);
     const size_t mld = (size_t)w.m_ld;
     w.csr = csr_nnz >= 0;
-    if (!w.csr) {
+    if (!w.csr && op == nullptr) {
       w.am = (float*)take("am", "f32", {mld, hwc});
       w.amt = (float*)take("amt", "f32", {hwc, mld});
     }
-    w.ym = (float*)take("ym", "f32", {np, mld});            // batch <= n_pad
+    if (op == nullptr) w.ym = (float*)take("ym", "f32", {np, mld});            // batch <= n_pad
     w.r = (float*)take("r", "f32", {np, mld});
     w.dym = (float*)take("dym", "f32", {np, hwc});
     w.mloss_part = (float*)take("mloss_part", "f32", {mld / kMeasTileN, np});
     w.mscale = (float*)take("mscale", "f32", {np});
-    if (w.csr) {
-      const size_t nnz = (size_t)csr_nnz;
-      w.nnz = csr_nnz;
-      w.a_rp = (int*)take("a_rp", "i32", {mld + 1});
-      w.a_ci = (int*)take("a_ci", "i32", {nnz});
-      w.a_v = (float*)take("a_v", "f32", {nnz});
-      w.at_rp = (int*)take("at_rp", "i32", {hwc + 1});
-      w.at_ci = (int*)take("at_ci", "i32", {nnz});
-      w.at_v = (float*)take("at_v", "f32", {nnz});
-      w.csr_bad = (int*)take("csr_bad", "i32", {mld});
-      w.csr_valid = (int*)take("csr_valid", "i32", {1});
+    if (op != nullptr) {
+      w.am = op->am; w.amt = op->amt; w.ym = op->ym;
+      w.nnz = op->nnz;
+      w.a_rp = op->a_rp; w.a_ci = op->a_ci; w.a_v = op->a_v;
+      w.at_rp = op->at_rp; w.at_ci = op->at_ci; w.at_v = op->at_v;
+      w.csr_bad = op->csr_bad; w.csr_valid = op->csr_valid;
+    } else if (w.csr) {
+      carve_csr(c, &w, csr_nnz, b, &off, layout);
     }
   }
   if (prune_maps) {
@@ -581,6 +602,32 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.src = (int*)take("src", "i32", {np});
     w.sel = (int*)take("sel", "i32", {np});     // batch <= n_pad
   }
+  w.bytes = off;
+  return w;
+}
+
+// The operator block of a pruned measured workspace, shared by all its regions: the staged operator - "am" / "amt" as in
+// carve, or (csr_nnz >= 0) carve's CSR buffers - then the measurements "ym" [batch][m_ld].  Only the operator's buffers,
+// m, m_ld, csr and nnz are set.
+static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz, void* base, std::string* layout) {
+  Workspace w;
+  size_t off = 0;
+  char* b = (char*)base;
+  auto take = [&](const std::string& name, const char* type, std::initializer_list<size_t> dims) -> void* {
+    return carve_take(b, &off, layout, name, type, dims);
+  };
+  const size_t hwc = (size_t)c->hwc;
+  w.m = m;
+  w.m_ld = measured_ld(m);
+  const size_t mld = (size_t)w.m_ld;
+  w.csr = csr_nnz >= 0;
+  if (w.csr) {
+    carve_csr(c, &w, csr_nnz, b, &off, layout);
+  } else {
+    w.am = (float*)take("am", "f32", {mld, hwc});
+    w.amt = (float*)take("amt", "f32", {hwc, mld});
+  }
+  w.ym = (float*)take("ym", "f32", {(size_t)batch, mld});
   w.bytes = off;
   return w;
 }
@@ -1829,15 +1876,25 @@ static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_r
 // The regions of a pruned workspace: region 0 for batch * rec_rr rows, region k for batch * keep_k rows, each a carve()
 // with the prune maps, one after the other (every carve is a multiple of 1024 bytes).  *bytes: the total; layout (not
 // NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
+// m > 0: a pruned measured workspace (csr_nnz >= 0: CSR): first the operator block (carve_operator; layout: a line
+// "operator 0 batch", then its lines), staged once for every stage, then the regions, each with the row-sized measured
+// buffers and the operator block's pointers.
 static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
                                            int n_points, void* base, bool weighted, size_t* bytes,
-                                           std::string* layout = nullptr) {
+                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1) {
   std::vector<Workspace> regs;
   size_t off = 0;
+  Workspace op;
+  if (m > 0) {
+    if (layout != nullptr) *layout += "operator 0 " + std::to_string(batch) + "\n";
+    op = carve_operator(c, batch, m, csr_nnz, base, layout);
+    off = op.bytes;
+  }
   for (int k = 0; k <= n_points; ++k) {
     const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
     if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
-    regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, 0, -1, true));
+    regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, m, csr_nnz, true,
+                         m > 0 ? &op : nullptr));
     off += regs.back().bytes;
   }
   *bytes = off;
@@ -1855,10 +1912,16 @@ static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_poin
   return 0;
 }
 
+// dgan_reconstruct_pruned and, with meas.m > 0 (x_dev and w_dev NULL), dgan_reconstruct_measured[_csr]_pruned: the
+// operator and measurements are staged once into the operator block that every region shares, and every stage runs the
+// measured loop; the measured forward leaves each iteration's loss parts in mloss_part, so a prune point sums them as
+// the plain loop's do loss_part
 static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                    const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
-                                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (h == nullptr || prm == nullptr || x_dev == nullptr || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+                                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
+                                   MeasuredArgs meas = MeasuredArgs()) {
+  const bool measured = meas.m > 0;
+  if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
   const bool weighted = w_dev != nullptr;
   const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters;
@@ -1874,10 +1937,11 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, weighted))) return rc;
   size_t need = 0;
-  std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need);
+  std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need, nullptr, meas.m,
+                                             meas.nnz);
   if (need > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
-              " (dgan_workspace_bytes_pruned)");
+              (measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
   for (Workspace& w : regs) {
@@ -1896,15 +1960,30 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
     } else if ((rc = clear_start_state(h, w, s))) {
       return rc;
     }
+    if (measured) {              // the operator block, once for every region
+      if (k == 0 && (rc = stage_meas(h, w, meas, batch, s))) return rc;
+      enqueues += h->launches - l0;
+      continue;
+    }
     DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
     if (weighted) DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
     enqueues += (h->launches - l0) + 1 + (weighted ? 1 : 0);
   }
-  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, 0, -1, prm->rec_lr, prm->momentum,
-                          {}, nullptr, 0};
+  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
+                          prm->momentum, {}, nullptr, 0};
   for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
-  // the stages and, between them, the prune points: the loss of iteration iter_k - 1 per row (still in loss_part after
-  // that iteration's update), the survivors' maps and the gather of their z, v (and z_h) into the next region
+  // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
+  // (measured) left
+  auto loss_finish = [&](const Workspace& w, cudaStream_t ls) -> int {
+    if (measured) return measured_loss_finish(h, w, ls);
+    loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, ls>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
+                                                               1.0f / (float)h->hwc, w.n_rows, w.loss);
+    DGAN_LAUNCH_CHECK(h);
+    return 0;
+  };
+  // the stages and, between them, the prune points: the loss of iteration iter_k - 1 per row (its parts are still in
+  // loss_part or mloss_part after that iteration's update), the survivors' maps and the gather of their z, v (and z_h)
+  // into the next region
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
     int r2;
     for (int k = 0; k <= n_points; ++k) {
@@ -1912,12 +1991,10 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
       const int per = k == 0 ? rec_rr : sched[k - 1].keep;
       const int t0 = k == 0 ? 0 : sched[k - 1].iter, t1 = k == n_points ? rec_iters : sched[k].iter;
       h->n_rows_cur = w.n_rows;
-      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, false, ls, k < n_points))) return r2;
+      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured, ls, k < n_points))) return r2;
       if (k == n_points) break;
       const Workspace& nx = regs[(size_t)k + 1];
-      loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, ls>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
-                                                                 1.0f / (float)h->hwc, w.n_rows, w.loss);
-      DGAN_LAUNCH_CHECK(h);
+      if ((r2 = loss_finish(w, ls))) return r2;
       prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sched[k].keep, nx.src, nx.orig);
       DGAN_LAUNCH_CHECK(h);
       const size_t total = (size_t)nx.n_pad * h->wd.latent;
@@ -1931,9 +2008,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   const Workspace& w = regs.back();
   const int per = sched[n_points - 1].keep;
   h->n_rows_cur = w.n_rows;
-  loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
-                                                            1.0f / (float)h->hwc, w.n_rows, w.loss);
-  DGAN_LAUNCH_CHECK(h);
+  if ((rc = loss_finish(w, s))) return rc;
   select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, w.sel);
   DGAN_LAUNCH_CHECK(h);
   prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
@@ -1958,6 +2033,45 @@ int dgan_reconstruct_pruned(dgan_handle h, const dgan_rec_params* prm, const dga
                             int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
   return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
                                  stream);
+}
+
+// m within 1 .. H*W*C and nnz -1 (a dense operator) or within 0 .. m * H*W*C (a CSR one)
+static bool measured_pruned_args_ok(dgan_handle h, int m, int nnz) {
+  return m > 0 && m <= h->hwc && (nnz == -1 || csr_nnz_ok(h, m, nnz));
+}
+
+size_t dgan_workspace_bytes_measured_pruned(dgan_handle h, int batch, int rec_rr, int m, int nnz,
+                                            const dgan_prune_point* sched, int n_points) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || h->desc.use_bn || !measured_pruned_args_ok(h, m, nnz) ||
+      check_schedule(sched, n_points, rec_rr, 0) != 0)
+    return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, nnz);
+  return bytes;
+}
+
+int dgan_reconstruct_measured_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
+                                     const float* a_dev, int m, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                     float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_pruned_impl(h, prm, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                                 ws_bytes, stream, meas);
+}
+
+int dgan_reconstruct_measured_csr_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched,
+                                         int n_points, const int32_t* row_ptr, const int32_t* col_idx, const float* val,
+                                         int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                         float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return reconstruct_pruned_impl(h, prm, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                                 ws_bytes, stream, meas);
 }
 
 int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* z0_dev, float* rec_dev,
@@ -2331,6 +2445,26 @@ int dgan_debug_workspace_layout_pruned(dgan_handle h, int batch, int rec_rr, con
   std::string out;
   size_t bytes = 0;
   carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out);
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
+}
+
+// The same for the workspace of dgan_reconstruct_measured[_csr]_pruned (dgan_workspace_bytes_measured_pruned; nnz -1 for
+// a dense operator): first a line "operator 0 batch" and the operator block's lines - "am" f32 [m_ld][H*W*C] and "amt"
+// f32 [H*W*C][m_ld], or the CSR buffers of dgan_debug_workspace_layout_measured_csr, then "ym" f32 [batch][m_ld] - then
+// per region a line "region k byte_offset n_rows" and that region's lines: the unweighted buffers, the row-sized measured
+// ones "r", "dym", "mloss_part" and "mscale", and the prune maps.
+int dgan_debug_workspace_layout_measured_pruned(dgan_handle h, int batch, int rec_rr, int m, int nnz,
+                                                const dgan_prune_point* sched, int n_points, char* buf, int buf_len) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || buf == nullptr || buf_len <= 0 || !measured_pruned_args_ok(h, m, nnz)) {
+    set_error("invalid argument");
+    return -1;
+  }
+  if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
+  std::string out;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, &out, m, nnz);
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();

@@ -32,6 +32,8 @@ from ..utils.config import load_config, packaged_cfg_path
 
 __all__ = ["RecCache", "DefenseGANBase", "MnistDefenseGAN", "FmnistDefenseDefenseGAN", "CelebADefenseGAN", "dataset_gan_dict"]
 
+_NOT_GIVEN = object()      # reconstruct_measured's prune when the caller passed none (None means "do not prune")
+
 
 class RecCache(object):
     """On-disk cache of one split's reconstructions, in the reference's layout (models/gan.py:466-478,503-507) so that
@@ -373,7 +375,7 @@ class DefenseGANBase(object):
         return _native.check_prune_schedule(self.rec_prune, int(self.rec_rr), int(self.rec_iters))
 
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
-                             z_row_offset=0):
+                             z_row_offset=0, prune=_NOT_GIVEN):
         """Projection onto the generator's range from linear measurements (an extension; the reference has none), for
         images that are not held themselves but observed as y = A x: a low-resolution or blurred copy, a
         compressed-sensing sketch.  `operator` A is [m, H*W*C] (a tensor or array; columns in NHWC pixel order,
@@ -392,12 +394,27 @@ class DefenseGANBase(object):
         bit-identical to the dense call on the same matrix; on fp16 a sparse operator is applied in fp32, so it differs
         from the dense call (TF32) by the TF32 rounding of the operator and the operands.
 
-        Restart pruning (`rec_prune`) is not available here: a call with it set raises a ValueError."""
-        if self.rec_prune is not None:
-            raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts: set rec_prune = None")
+        `prune` (an extension): a list of (iter, keep) pairs with the rules of `rec_prune`, to prune restarts in this call:
+        from iteration iter_k on each image runs only its keep_k restarts of lowest measured loss at iteration iter_k - 1
+        (ties: the lower restart index; NaN last), and the arg-min picks among the last survivors (`return_aux`'s restart
+        is the original index).  The survivors follow exactly their unpruned trajectories.  The schedule is checked
+        before any native call (a ValueError naming the bad point) and refused with use_bn.  The measured call takes its
+        schedule per call rather than from `rec_prune`, which is tuned for the image loss and names the reconstruction
+        cache: without `prune`, a call with `rec_prune` set raises a ValueError; `prune=None` runs every restart to the
+        end whatever `rec_prune` holds."""
+        if prune is _NOT_GIVEN:
+            if self.rec_prune is not None:
+                raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts from it: set "
+                                 "rec_prune = None, or pass prune= to prune this call")
+            prune = None
+        if prune is not None:
+            if bool(self.use_bn):
+                raise ValueError("prune is not supported with use_bn: the batch statistics couple the restarts, so "
+                                 "dropping some would change the others' trajectories")
+            prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                     z_row_offset)
+                                                     z_row_offset, prune)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -417,10 +434,12 @@ class DefenseGANBase(object):
         self.last_seed = seed = self._next_seed(0)
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
-                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset))
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune)
 
-    def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset):
-        """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements."""
+    def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
+                                     prune):
+        """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements
+        (prune: the checked schedule, or None)."""
         a = operator
         if a.layout == torch.sparse_coo:
             if a.dim() != 2 or a.dense_dim() != 0:
@@ -464,7 +483,7 @@ class DefenseGANBase(object):
         self.last_seed = seed = self._next_seed(0)
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
-                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset))
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune)
 
     def _pixel_weights(self, pixel_weights, x):
         """pixel_weights broadcast to x's shape and materialised once, after one check of all values (finite, in [0, 1])."""

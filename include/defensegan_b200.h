@@ -242,6 +242,45 @@ int dgan_reconstruct_pruned(dgan_handle h, const dgan_rec_params* params, const 
                             const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                             int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
 
+/* Bytes of scratch for dgan_reconstruct_measured_pruned with nnz = -1, or dgan_reconstruct_measured_csr_pruned with
+ * nnz >= 0 non-zeros, for m measurements and this schedule: one operator block - the copies of A and A^T, or of the CSR and its
+ * transpose, and y for batch images - shared by every stage, then one region per stage, each the workspace that
+ * dgan_workspace_bytes carves for that stage's rows plus the residuals, the adjoint product, the measured loss and three
+ * int32 maps of its rows.  Also plans every stage's row count.  0 for a handle with use_bn, for a schedule that breaks the
+ * rules of dgan_reconstruct_pruned (except iter <= rec_iters - 1, as L is not known here), for m <= 0 or m > H*W*C and
+ * for nnz < -1 or nnz > m * H*W*C. */
+size_t dgan_workspace_bytes_measured_pruned(dgan_handle h, int batch, int rec_rr, int m, int nnz,
+                                            const dgan_prune_point* sched, int n_points);
+
+/* dgan_reconstruct_measured with the restart pruning of dgan_reconstruct_pruned - a_dev, m and y_dev as in the first,
+ * sched and n_points as in the second: at prune point k each image's survivors are ranked by their measured loss (1/m) ||A G(z) - y||^2
+ * at iteration iter_k - 1, with the same order, ties and NaN rule, and the arg-min select picks among the last
+ * survivors; idx_dev is the original restart index.  Without BatchNorm each survivor follows exactly its unpruned
+ * trajectory: keep_k = rec_rr at every point gives dgan_reconstruct_measured's bits, and any schedule gives the result
+ * composed from rec_rr = 1 calls.  use_bn: DGAN_ERR_UNSUPPORTED.  The argument checks of dgan_reconstruct_measured and
+ * dgan_reconstruct_pruned apply, before anything is enqueued; a workspace smaller than
+ * dgan_workspace_bytes_measured_pruned: DGAN_ERR_WORKSPACE.
+ * Before the captured loop the host enqueues the z0 initialiser (into region 0), the memsets of each later region and
+ * the three kernels that stage A, A^T and y into the operator block, once.  The loop - every stage's measured L-steps on
+ * its rows and, at each prune point, the measured loss sum, prune_select_kernel and prune_gather_kernel - is one CUDA
+ * graph; after it: measured loss sum, arg-min select and the mapping to the original index.  So, with P = n_points,
+ * dgan_last_launch_count is dgan_reconstruct_measured's with the same rec_iters + 3 P + 1, and dgan_last_enqueue_count
+ * is dgan_reconstruct_measured's + 1. */
+int dgan_reconstruct_measured_pruned(dgan_handle h, const dgan_rec_params* params, const dgan_prune_point* sched,
+                                     int n_points, const float* a_dev, int m, const float* y_dev, const float* z0_dev,
+                                     float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                                     void* stream);
+
+/* dgan_reconstruct_measured_pruned with the CSR operator of dgan_reconstruct_measured_csr - row_ptr, col_idx, val, m,
+ * nnz and their checks as there: it is validated and staged once, by five kernels, into the operator block; a malformed
+ * CSR is staged as the empty operator with NaN measurements, so every loss is NaN and each image keeps survivors 0 ..
+ * keep - 1 by the NaN rule.  dgan_last_launch_count is dgan_reconstruct_measured_csr's + 3 P + 1, and
+ * dgan_last_enqueue_count is dgan_reconstruct_measured_csr's + 1. */
+int dgan_reconstruct_measured_csr_pruned(dgan_handle h, const dgan_rec_params* params, const dgan_prune_point* sched,
+                                         int n_points, const int32_t* row_ptr, const int32_t* col_idx, const float* val,
+                                         int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                         float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -289,7 +328,8 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * without BatchNorm; with net_dim > 64 the Linear's forward and Generator.2's backward each run as two column blocks of
  * 256 channels, 1 + 10 L - 5 + 2).  A dgan_reconstruct_measured call runs 3 + 6 (L - 1) + 1 kernels more with
  * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there); a dgan_reconstruct_measured_csr call
- * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more; a dgan_reconstruct_pruned call with P prune points 3 P + 1 more. */
+ * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more; a dgan_reconstruct_pruned call with P prune points 3 P + 1 more, and a
+ * dgan_reconstruct_measured[_csr]_pruned call 3 P + 1 more than the unpruned measured call with the same operator kind. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
