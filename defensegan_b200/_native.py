@@ -41,6 +41,8 @@ ABI_SYMBOLS = [
     "dgan_workspace_bytes_measured_csr", "dgan_reconstruct_measured_csr", "dgan_loss_grad_measured_csr",
     "dgan_workspace_bytes_pruned", "dgan_reconstruct_pruned",
     "dgan_workspace_bytes_measured_pruned", "dgan_reconstruct_measured_pruned", "dgan_reconstruct_measured_csr_pruned",
+    "dgan_workspace_bytes_adam", "dgan_workspace_bytes_measured_adam", "dgan_reconstruct_adam", "dgan_reconstruct_measured_adam",
+    "dgan_reconstruct_measured_csr_adam",
 ]
 
 
@@ -59,7 +61,35 @@ class dgan_prune_point(ctypes.Structure):
     _fields_ = [("iter", ctypes.c_int32), ("keep", ctypes.c_int32)]
 
 
+class dgan_adam_params(ctypes.Structure):
+    _fields_ = [("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float)]
+
+
 ABI_VERSION = 2
+
+
+def check_adam_params(adam):
+    """Adam's (beta1, beta2, eps) as a tuple of floats, after the rules of dgan_reconstruct_adam: 0 <= beta1 < 1,
+    0 <= beta2 < 1 and a finite eps > 0 (as fp32, the type the library reads).  A ValueError names the bad value."""
+    try:
+        vals = tuple(adam)
+    except TypeError:
+        raise ValueError("adam is a (beta1, beta2, eps) triple, got %r" % (adam,)) from None
+    if len(vals) != 3:
+        raise ValueError("adam is a (beta1, beta2, eps) triple, got %r" % (adam,))
+    out = []
+    for name, v in zip(("beta1", "beta2", "eps"), vals):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)):
+            raise ValueError("adam %s = %r is not a number" % (name, v))
+        out.append(float(np.float32(v)))
+    b1, b2, eps = out
+    if not 0.0 <= b1 < 1.0:
+        raise ValueError("adam beta1 = %r must be in [0, 1)" % (vals[0],))
+    if not 0.0 <= b2 < 1.0:
+        raise ValueError("adam beta2 = %r must be in [0, 1)" % (vals[1],))
+    if not (np.isfinite(eps) and eps > 0.0):
+        raise ValueError("adam eps = %r must be finite and > 0" % (vals[2],))
+    return b1, b2, eps
 
 
 def check_prune_schedule(prune, rec_rr: int, rec_iters: int):
@@ -199,6 +229,19 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_measured_csr_pruned.restype = i32
     lib.dgan_reconstruct_measured_csr_pruned.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ctypes.POINTER(dgan_prune_point),
                                                          i32, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    pp, ap = ctypes.POINTER(dgan_prune_point), ctypes.POINTER(dgan_adam_params)
+    lib.dgan_workspace_bytes_adam.restype = sz
+    lib.dgan_workspace_bytes_adam.argtypes = [vp, i32, i32, i32, pp, i32]
+    lib.dgan_workspace_bytes_measured_adam.restype = sz
+    lib.dgan_workspace_bytes_measured_adam.argtypes = [vp, i32, i32, i32, i32, pp, i32]
+    lib.dgan_reconstruct_adam.restype = i32
+    lib.dgan_reconstruct_adam.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, pp, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_adam.restype = i32
+    lib.dgan_reconstruct_measured_adam.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, pp, i32, vp, i32, vp, vp, vp, vp,
+                                                   vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_csr_adam.restype = i32
+    lib.dgan_reconstruct_measured_csr_adam.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, pp, i32, vp, vp, vp, i32, i32,
+                                                       vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -314,8 +357,15 @@ class NativeGenerator:
             pass
 
     # -- helpers -------------------------------------------------------------------------
-    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None):
-        if sched is not None and m > 0:
+    def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None,
+                   adam: bool = False):
+        if adam and m > 0:
+            need = int(self.lib.dgan_workspace_bytes_measured_adam(self._handle, batch, rec_rr, int(m), int(nnz), sched,
+                                                                   len(sched) if sched is not None else 0))
+        elif adam:
+            need = int(self.lib.dgan_workspace_bytes_adam(self._handle, batch, rec_rr, int(weighted), sched,
+                                                          len(sched) if sched is not None else 0))
+        elif sched is not None and m > 0:
             need = int(self.lib.dgan_workspace_bytes_measured_pruned(self._handle, batch, rec_rr, int(m), int(nnz), sched,
                                                                      len(sched)))
         elif sched is not None:
@@ -371,13 +421,16 @@ class NativeGenerator:
                     z_init_val: Optional[torch.Tensor] = None, seed: int = 0, momentum: float = 0.7,
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
                     z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None,
-                    prune: Optional[Sequence[Sequence[int]]] = None):
+                    prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None):
         """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
         the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
         (dgan_reconstruct_weighted).
         prune (a sequence of (iter, keep) pairs, see check_prune_schedule): from iteration iter on, each image keeps only
         its `keep` restarts of lowest loss at iteration iter - 1 (dgan_reconstruct_pruned); idx is the chosen restart's
-        original index.  None runs every restart to the end."""
+        original index.  None runs every restart to the end.
+        adam ((beta1, beta2, eps), see check_adam_params): update z with Adam instead of momentum (dgan_reconstruct_adam,
+        with or without pixel_weights and prune); momentum is then ignored, and rec_lr is Adam's step in z units, so the
+        momentum path's values do not carry over.  None runs the momentum update."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
@@ -386,6 +439,7 @@ class NativeGenerator:
             raise ValueError("batch, rec_rr and rec_iters must be positive")
         pw = self._pixel_weights(pixel_weights, batch)
         sched = self._schedule(prune, rec_rr, rec_iters)
+        ap = self._adam(adam)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -398,11 +452,16 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched)
+            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched, adam=ap is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if sched is not None:
+            if ap is not None:
+                rc = self.lib.dgan_reconstruct_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
+                                                    len(sched) if sched is not None else 0, _ptr(x), _ptr(pw), _ptr(z0),
+                                                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_adam")
+            elif sched is not None:
                 rc = self.lib.dgan_reconstruct_pruned(self._handle, ctypes.byref(prm), sched, len(sched), _ptr(x), _ptr(pw),
                                                       _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
                                                       ctypes.c_void_p(stream))
@@ -429,6 +488,14 @@ class NativeGenerator:
             raise ValueError("restart pruning is not supported with use_bn: the batch statistics couple the rows")
         points = check_prune_schedule(prune, int(rec_rr), int(rec_iters))
         return (dgan_prune_point * len(points))(*[dgan_prune_point(it, keep) for it, keep in points])
+
+    @staticmethod
+    def _adam(adam):
+        """Adam's parameters as the dgan_adam_params of the Adam entries (None stays None), checked with
+        check_adam_params."""
+        if adam is None:
+            return None
+        return dgan_adam_params(*check_adam_params(adam))
 
     def _measured(self, measurements: torch.Tensor, operator: torch.Tensor):
         """(y, A, batch, m): the measurements as a contiguous CUDA float32 [batch, m] tensor and the operator as [m, H*W*C]
@@ -469,7 +536,7 @@ class NativeGenerator:
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
                              return_aux: bool = False, z_row_offset: int = 0,
-                             prune: Optional[Sequence[Sequence[int]]] = None):
+                             prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None):
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
@@ -478,7 +545,9 @@ class NativeGenerator:
         runs dgan_reconstruct_measured_csr: the same semantics, at a cost set by its non-zeros.
         prune (a sequence of (iter, keep) pairs, see check_prune_schedule): restart pruning as in reconstruct, ranked by
         the measured loss (dgan_reconstruct_measured_pruned, or dgan_reconstruct_measured_csr_pruned for a CSR operator).
-        None runs every restart to the end."""
+        None runs every restart to the end.
+        adam ((beta1, beta2, eps)): the Adam update of reconstruct (dgan_reconstruct_measured_adam, or
+        dgan_reconstruct_measured_csr_adam for a CSR operator), with or without prune."""
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -487,6 +556,7 @@ class NativeGenerator:
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
         sched = self._schedule(prune, rec_rr, rec_iters)
+        ap = self._adam(adam)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -499,11 +569,23 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched)
+            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched, adam=ap is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if sched is not None and csr:
+            n_points = len(sched) if sched is not None else 0
+            if ap is not None and csr:
+                rc = self.lib.dgan_reconstruct_measured_csr_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
+                                                                 n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
+                                                                 _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                                 ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_csr_adam")
+            elif ap is not None:
+                rc = self.lib.dgan_reconstruct_measured_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
+                                                             n_points, _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss),
+                                                             _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_adam")
+            elif sched is not None and csr:
                 rc = self.lib.dgan_reconstruct_measured_csr_pruned(self._handle, ctypes.byref(prm), sched, len(sched),
                                                                    _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
                                                                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need,

@@ -18,6 +18,7 @@
 #include "kernels_measured.cuh"
 #include "kernels_measured_csr.cuh"
 #include "kernels_prune.cuh"
+#include "kernels_adam.cuh"
 
 namespace dgan {
 
@@ -322,16 +323,18 @@ struct dgan_ctx {
   int n_rows_cur = 0;
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
   // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise,
-  // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise) on a private stream,
-  // replayed with one cudaGraphLaunch per call.
+  // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise; adam: 1 for the Adam
+  // update with beta1, beta2 and eps, 0 for momentum) on a private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     std::vector<int> prune;
     cudaGraphExec_t exec; int64_t kernels;
+    int adam = 0; float beta1 = 0.f, beta2 = 0.f, eps = 0.f;
     bool same_key(const LoopGraph& o) const {
       return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
              weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
-             momentum == o.momentum && prune == o.prune;
+             momentum == o.momentum && prune == o.prune && adam == o.adam && beta1 == o.beta1 && beta2 == o.beta2 &&
+             eps == o.eps;
     }
   };
   std::vector<LoopGraph> graphs;
@@ -458,6 +461,9 @@ struct Workspace {
   // 0 .. R-1 of each image and leave it unwritten), the row of the previous region each row was gathered from [n_pad],
   // and select_kernel's choice per image among its survivors [n_pad] (the last region's only)
   int *orig = nullptr, *src = nullptr, *sel = nullptr;
+  // Adam workspaces (kernels_adam.cuh), after all the buffers above: the second moment s [n_pad][latent_pad]; the first
+  // moment lives in v, the momentum buffer
+  float* s = nullptr;
   size_t bytes = 0;
 };
 
@@ -508,9 +514,11 @@ static void carve_csr(const dgan_ctx* c, Workspace* w, int nnz_, char* b, size_t
 // am / amt and the CSR ones after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
 // "orig", "src" and "sel" after all the other buffers.  op (not NULL, with m > 0): a region of a pruned measured
 // workspace, whose operator - am / amt or the CSR buffers - and ym live in the operator block op (carve_operator): only
-// the row-sized measured buffers are carved, the others are op's.
+// the row-sized measured buffers are carved, the others are op's.  adam: the workspace of the Adam entries, the same
+// buffers at the same offsets and the second moment "s" after all of them.
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
-                       int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr) {
+                       int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr,
+                       bool adam = false) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -602,6 +610,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.src = (int*)take("src", "i32", {np});
     w.sel = (int*)take("sel", "i32", {np});     // batch <= n_pad
   }
+  if (adam) w.s = (float*)take("s", "f32", {np, latent});
   w.bytes = off;
   return w;
 }
@@ -980,9 +989,10 @@ static int run_tangent(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   return 0;
 }
 
-// The state a fresh workspace needs besides z and v: zeroed momentum tickets (fp16 path) and zeroed tile-padding rows of
-// d(pre) (fp32 path).  Memsets only.
+// The state a fresh workspace needs besides z and v: zeroed momentum tickets (fp16 path), zeroed tile-padding rows of
+// d(pre) (fp32 path) and, in an Adam workspace, a zeroed second moment.  Memsets only.
 static int clear_start_state(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  if (w.s != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.s, 0, (size_t)w.n_pad * c->wd.latent * sizeof(float), s));
   if (w.mom_counter != nullptr) DGAN_CUDA_CHECK(cudaMemsetAsync(w.mom_counter, 0, (size_t)w.n_pad / kRowTile * sizeof(unsigned), s));
   // fp32 path: the last layer's forward writes dL/dpre for the real rows only while its backward walks all n_pad rows;
   // the tile-padding rows are never observed, but they must not be read uninitialised
@@ -1178,17 +1188,18 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
 // workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
 // planned and mapped too.  m > 0: the workspace of a measured entry for m measurements.
 static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0,
-                    int csr_nnz = -1) {
+                    int csr_nnz = -1, bool adam = false) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
   if ((rc = plan_all(c, n_rows))) return rc;
   if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz);
+  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
-                                                             : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
+              (adam ? (m > 0 ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
+               : weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
+               : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
     return DGAN_ERR_WORKSPACE;
   }
   if ((rc = build_maps(c, *out))) return rc;
@@ -1705,10 +1716,24 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
 // The learning rate follows the global iteration t (decay from ceil(0.8 L) of the full L); iteration L-1, when it is in
 // the range, is its forward alone.  loss_at_end: the forward of iteration t1 - 1 leaves its per-row loss parts in
 // w.loss_part, as the forward of iteration L-1 does (the fp16 path's last-layer forward writes them, and y, only when it
-// is asked for y).
+// is asked for y).  adam (not NULL): the Adam update (adam_kernel, with m in w.v and s in w.s) instead of the momentum
+// update; on the fp16 image loss the Linear backward then runs without its momentum tail and adam_kernel follows it.
 static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params& p, int per_image, int t0, int t1,
-                         bool measured, cudaStream_t ls, bool loss_at_end = false) {
+                         bool measured, cudaStream_t ls, bool loss_at_end = false, const dgan_adam_params* adam = nullptr) {
   const int latent = h->wd.latent;
+  // Adam at iteration t (k = t + 1): c1 = lr_t / (1 - beta1^k) and c2 = 1 / sqrt(1 - beta2^k), in double, rounded to fp32
+  auto launch_adam = [&](int t, float lr, float gmul, const float* row_scale) -> int {
+    const double k = (double)t + 1.0;
+    const float c1 = (float)((double)lr / (1.0 - std::pow((double)adam->beta1, k)));
+    const float c2 = (float)(1.0 / std::sqrt(1.0 - std::pow((double)adam->beta2, k)));
+    const size_t zcount = (size_t)w.n_pad * latent;
+    ProfScope ps(h, 2 * (int)h->layers.size() + 2, ls);     // the profile kind of the latent update
+    DGAN_CUDA_CHECK(launch_pdl(adam_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v, w.s,
+                               (const float*)w.g, w.n_g_parts, gmul, row_scale, latent, w.n_rows, adam->beta1, adam->beta2,
+                               adam->eps, c1, c2, zcount, w.z_h));
+    DGAN_LAUNCH_CHECK(h);
+    return 0;
+  };
   const int decay_iter = (int)std::ceil(p.rec_iters * 0.8);
   // fp16: the momentum update (tf.train.MomentumOptimizer, models/gan.py:389-391) runs in the tail of the split-K Linear
   // backward - the CTA that completes a 128-row tile's partial sums applies it - so an L-step is 8 launches; bit-identical
@@ -1727,6 +1752,10 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
       if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, per_image, ls))) return r2;
       if (last) continue;
       if ((r2 = measured_backward(h, w, ls))) return r2;
+      if (adam != nullptr) {
+        if ((r2 = launch_adam(t, lr, 1.f, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr))) return r2;
+        continue;
+      }
       const size_t zcount = (size_t)w.n_pad * latent;
       momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
           w.z, w.v, w.g, w.n_g_parts, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr, latent, w.n_rows, lr,
@@ -1737,6 +1766,10 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
     const bool want_y = last || (loss_at_end && t == t1 - 1);
     if ((r2 = run_forward(h, w, w.x, per_image, p.batch, !last, ls, want_y, w.xw))) return r2;
     if (last) continue;
+    if (adam != nullptr) {
+      if ((r2 = run_backward(h, w, ls)) || (r2 = launch_adam(t, lr, grad_multiplier(h), nullptr))) return r2;
+      continue;
+    }
     MomentumArgs mom;
     mom.lr = lr; mom.mu = p.momentum; mom.tail = tail;
     if ((r2 = run_backward(h, w, ls, mom))) return r2;
@@ -1792,12 +1825,31 @@ static int run_loop(dgan_ctx* h, const dgan_ctx::LoopGraph& key, const std::func
   return 0;
 }
 
+// The optimiser part of a loop's graph-cache key: the Adam hyper-parameters, or none for the momentum update.
+static void set_optimizer_key(dgan_ctx::LoopGraph* key, const dgan_adam_params* adam) {
+  if (adam == nullptr) return;
+  key->adam = 1; key->beta1 = adam->beta1; key->beta2 = adam->beta2; key->eps = adam->eps;
+}
+
+// Adam's hyper-parameters: 0 <= beta1 < 1, 0 <= beta2 < 1 and a finite eps > 0; 0, or DGAN_ERR_INVALID_ARG naming the bad
+// value.
+static int check_adam(const dgan_adam_params* a) {
+  if (a == nullptr) { set_error("NULL Adam parameters"); return DGAN_ERR_INVALID_ARG; }
+  std::string bad;
+  if (!(a->beta1 >= 0.f && a->beta1 < 1.f)) bad = "beta1 = " + std::to_string(a->beta1) + " must be in [0, 1)";
+  else if (!(a->beta2 >= 0.f && a->beta2 < 1.f)) bad = "beta2 = " + std::to_string(a->beta2) + " must be in [0, 1)";
+  else if (!(a->eps > 0.f && std::isfinite(a->eps))) bad = "eps = " + std::to_string(a->eps) + " must be finite and > 0";
+  if (bad.empty()) return 0;
+  set_error("invalid Adam parameters: " + bad);
+  return DGAN_ERR_INVALID_ARG;
+}
+
 // dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
 // weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
-// the workspace only
+// the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).
 static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                             const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
-                            void* stream, MeasuredArgs meas = MeasuredArgs()) {
+                            void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
@@ -1810,7 +1862,7 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   cudaStream_t s = (cudaStream_t)stream;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr))) return rc;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
@@ -1829,7 +1881,10 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   // The L-step loop (a function of the workspace and the hyper-parameters only)
   dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
                           prm->momentum, {}, nullptr, 0};
-  auto enqueue_loop = [&](cudaStream_t ls) -> int { return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls); };
+  set_optimizer_key(&key, adam);
+  auto enqueue_loop = [&](cudaStream_t ls) -> int {
+    return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls, false, adam);
+  };
   if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
   {
     const int n_rows = batch * rec_rr;
@@ -1878,10 +1933,10 @@ static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_r
 // NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
 // m > 0: a pruned measured workspace (csr_nnz >= 0: CSR): first the operator block (carve_operator; layout: a line
 // "operator 0 batch", then its lines), staged once for every stage, then the regions, each with the row-sized measured
-// buffers and the operator block's pointers.
+// buffers and the operator block's pointers.  adam: every region an Adam carve (its second moment "s" last).
 static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
                                            int n_points, void* base, bool weighted, size_t* bytes,
-                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1) {
+                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1, bool adam = false) {
   std::vector<Workspace> regs;
   size_t off = 0;
   Workspace op;
@@ -1894,7 +1949,7 @@ static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec
     const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
     if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
     regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, m, csr_nnz, true,
-                         m > 0 ? &op : nullptr));
+                         m > 0 ? &op : nullptr, adam));
     off += regs.back().bytes;
   }
   *bytes = off;
@@ -1915,11 +1970,12 @@ static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_poin
 // dgan_reconstruct_pruned and, with meas.m > 0 (x_dev and w_dev NULL), dgan_reconstruct_measured[_csr]_pruned: the
 // operator and measurements are staged once into the operator block that every region shares, and every stage runs the
 // measured loop; the measured forward leaves each iteration's loss parts in mloss_part, so a prune point sums them as
-// the plain loop's do loss_part
+// the plain loop's do loss_part.  adam (not NULL, checked by the caller): the Adam entries; a prune point gathers the
+// survivors' second moment with their z, m and z_h.
 static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                    const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
-                                   MeasuredArgs meas = MeasuredArgs()) {
+                                   MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
@@ -1938,10 +1994,11 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, weighted))) return rc;
   size_t need = 0;
   std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need, nullptr, meas.m,
-                                             meas.nnz);
+                                             meas.nnz, adam != nullptr);
   if (need > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
-              (measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
+              (adam != nullptr ? (measured ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
+               : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
   for (Workspace& w : regs) {
@@ -1972,6 +2029,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
                           prm->momentum, {}, nullptr, 0};
   for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
+  set_optimizer_key(&key, adam);
   // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
   // (measured) left
   auto loss_finish = [&](const Workspace& w, cudaStream_t ls) -> int {
@@ -1991,15 +2049,20 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
       const int per = k == 0 ? rec_rr : sched[k - 1].keep;
       const int t0 = k == 0 ? 0 : sched[k - 1].iter, t1 = k == n_points ? rec_iters : sched[k].iter;
       h->n_rows_cur = w.n_rows;
-      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured, ls, k < n_points))) return r2;
+      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured, ls, k < n_points, adam))) return r2;
       if (k == n_points) break;
       const Workspace& nx = regs[(size_t)k + 1];
       if ((r2 = loss_finish(w, ls))) return r2;
       prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sched[k].keep, nx.src, nx.orig);
       DGAN_LAUNCH_CHECK(h);
       const size_t total = (size_t)nx.n_pad * h->wd.latent;
-      prune_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.z_h, nx.src, nx.n_rows, nx.n_pad,
-                                                                          h->wd.latent, nx.z, nx.v, nx.z_h);
+      if (adam != nullptr)
+        prune_gather_adam_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.s, w.z_h, nx.src, nx.n_rows,
+                                                                                 nx.n_pad, h->wd.latent, nx.z, nx.v, nx.s,
+                                                                                 nx.z_h);
+      else
+        prune_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.z_h, nx.src, nx.n_rows, nx.n_pad,
+                                                                            h->wd.latent, nx.z, nx.v, nx.z_h);
       DGAN_LAUNCH_CHECK(h);
     }
     return 0;
@@ -2104,6 +2167,87 @@ int dgan_reconstruct_measured_csr(dgan_handle h, const dgan_rec_params* prm, con
   MeasuredArgs meas;
   meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
   return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
+}
+
+// ---- Adam (kernels_adam.cuh): each entry is its momentum counterpart's code path with the Adam update -----------------
+// sched NULL with n_points 0: unpruned; anything else is a schedule under the rules of dgan_reconstruct_pruned
+static bool unpruned(const dgan_prune_point* sched, int n_points) { return sched == nullptr && n_points == 0; }
+
+size_t dgan_workspace_bytes_adam(dgan_handle h, int batch, int rec_rr, int weighted, const dgan_prune_point* sched,
+                                 int n_points) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
+  if (unpruned(sched, n_points)) {
+    if (plan_all(h, batch * rec_rr) != 0 || (weighted && plan_pass(h, batch * rec_rr, TC_PASS_WEIGHTED) != 0)) return 0;
+    return carve(h, batch * rec_rr, nullptr, nullptr, weighted != 0, 0, -1, false, nullptr, true).bytes;
+  }
+  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, weighted != 0) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, nullptr, 0, -1, true);
+  return bytes;
+}
+
+size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_prune_point* sched,
+                                          int n_points) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || !measured_pruned_args_ok(h, m, nnz)) return 0;
+  if (unpruned(sched, n_points)) {
+    if (plan_all(h, batch * rec_rr) != 0) return 0;
+    return carve(h, batch * rec_rr, nullptr, nullptr, false, m, nnz, false, nullptr, true).bytes;
+  }
+  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, nnz, true);
+  return bytes;
+}
+
+// The image and measured Adam entries after their own checks: unpruned through reconstruct_impl, pruned through
+// reconstruct_pruned_impl, as their momentum counterparts
+static int reconstruct_adam_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                 const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                                 const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                 size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs()) {
+  if (unpruned(sched, n_points))
+    return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam);
+  return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                                 stream, meas, adam);
+}
+
+int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                          const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                          const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                          void* stream) {
+  if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                               stream);
+}
+
+int dgan_reconstruct_measured_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                   const dgan_prune_point* sched, int n_points, const float* a_dev, int m, const float* y_dev,
+                                   const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                   size_t ws_bytes, void* stream) {
+  if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas);
+}
+
+int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                       const dgan_prune_point* sched, int n_points, const int32_t* row_ptr,
+                                       const int32_t* col_idx, const float* val, int m, int nnz, const float* y_dev,
+                                       const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                       size_t ws_bytes, void* stream) {
+  if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -2465,6 +2609,31 @@ int dgan_debug_workspace_layout_measured_pruned(dgan_handle h, int batch, int re
   std::string out;
   size_t bytes = 0;
   carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, &out, m, nnz);
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
+}
+
+// The same for the workspace of the Adam entries (dgan_workspace_bytes_adam with m = 0, dgan_workspace_bytes_measured_adam
+// with m > 0; nnz -1 for a dense operator): unpruned (sched NULL, n_points 0), the layout of
+// dgan_debug_workspace_layout[_weighted / _measured / _measured_csr] with one line more at its end, the second moment
+// "s" f32 [n_pad][latent_pad]; pruned, that of dgan_debug_workspace_layout[_measured]_pruned with "s" at the end of each
+// region (so each later region starts that much further on).
+int dgan_debug_workspace_layout_adam(dgan_handle h, int batch, int rec_rr, int weighted, int m, int nnz,
+                                     const dgan_prune_point* sched, int n_points, char* buf, int buf_len) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || buf == nullptr || buf_len <= 0 ||
+      (m != 0 && !measured_pruned_args_ok(h, m, nnz)) || (m > 0 && weighted)) {
+    set_error("invalid argument");
+    return -1;
+  }
+  std::string out;
+  if (unpruned(sched, n_points)) {
+    carve(h, batch * rec_rr, nullptr, &out, weighted != 0, m, m > 0 ? nnz : -1, false, nullptr, true);
+  } else {
+    if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
+    size_t bytes = 0;
+    carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out, m, m > 0 ? nnz : -1, true);
+  }
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();

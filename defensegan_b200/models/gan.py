@@ -120,6 +120,9 @@ class DefenseGANBase(object):
         self.rec_momentum = 0.7            # tf.train.MomentumOptimizer(momentum=0.7), models/gan.py:389-391
         self.rec_decay_lr = False          # the reference's decay is dead code (SURVEY F3); True = intended schedule
         self.rec_prune = None              # restart pruning: [(iter, keep), ...] (cfg REC_PRUNE); None = every restart to the end
+        self.rec_optimizer = "momentum"    # update of z: "momentum" (the reference's) | "adam" (cfg REC_OPTIMIZER)
+        self.rec_adam_betas = (0.9, 0.999)  # Adam's (beta1, beta2) (cfg REC_ADAM_BETAS), read with rec_optimizer "adam"
+        self.rec_adam_eps = 1e-8           # Adam's eps (cfg REC_ADAM_EPS)
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
 
         self.test_mode = test_mode
@@ -346,8 +349,16 @@ class DefenseGANBase(object):
         NaN last); the survivors follow exactly the trajectories they would follow unpruned, and the arg-min picks among
         the last survivors (`return_aux`'s restart is the original index).  It cuts the row-steps of a call, at the risk of
         dropping a restart that would have won.  The schedule is checked before any native call (a ValueError naming the
-        bad point), and refused with use_bn, whose batch statistics couple the restarts."""
+        bad point), and refused with use_bn, whose batch statistics couple the restarts.
+
+        `rec_optimizer` (an extension, read at call time; "momentum" by default, the reference's
+        MomentumOptimizer(rec_lr, rec_momentum)): "adam" updates z with Adam, rec_adam_betas = (beta1, beta2) and
+        rec_adam_eps, with m and s reset on every call and bias correction at step k = t + 1; rec_momentum is then
+        ignored.  Adam's rec_lr is a step in z units (each coordinate moves by about rec_lr per step early on), so the
+        reference's rec_lr = 10.0 does not carry over: choose it for the problem.  It combines with pixel_weights and
+        rec_prune.  The values are checked before any native call (a ValueError naming the bad value)."""
         prune = self._prune_schedule()
+        adam = self._adam_params()
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
@@ -360,6 +371,8 @@ class DefenseGANBase(object):
         kw = {} if pw is None else {"pixel_weights": pw}
         if prune is not None:
             kw["prune"] = prune
+        if adam is not None:
+            kw["adam"] = adam
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
@@ -373,6 +386,23 @@ class DefenseGANBase(object):
             raise ValueError("rec_prune is not supported with use_bn: the batch statistics couple the restarts, so "
                              "dropping some would change the others' trajectories")
         return _native.check_prune_schedule(self.rec_prune, int(self.rec_rr), int(self.rec_iters))
+
+    def _adam_params(self):
+        """None for rec_optimizer "momentum", else Adam's (beta1, beta2, eps) from rec_adam_betas and rec_adam_eps,
+        checked; ValueError naming the bad value before any native call."""
+        opt = self.rec_optimizer
+        if opt not in ("momentum", "adam"):
+            raise ValueError("rec_optimizer = %r: expected 'momentum' or 'adam'" % (opt,))
+        if opt == "momentum":
+            return None
+        betas = self.rec_adam_betas
+        try:
+            betas = tuple(betas)
+        except TypeError:
+            raise ValueError("rec_adam_betas = %r: expected a pair (beta1, beta2)" % (betas,)) from None
+        if len(betas) != 2:
+            raise ValueError("rec_adam_betas = %r: expected a pair (beta1, beta2)" % (betas,))
+        return _native.check_adam_params((betas[0], betas[1], self.rec_adam_eps))
 
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
                              z_row_offset=0, prune=_NOT_GIVEN):
@@ -401,7 +431,11 @@ class DefenseGANBase(object):
         before any native call (a ValueError naming the bad point) and refused with use_bn.  The measured call takes its
         schedule per call rather than from `rec_prune`, which is tuned for the image loss and names the reconstruction
         cache: without `prune`, a call with `rec_prune` set raises a ValueError; `prune=None` runs every restart to the
-        end whatever `rec_prune` holds."""
+        end whatever `rec_prune` holds.
+
+        `rec_optimizer`, `rec_adam_betas` and `rec_adam_eps` are read at call time as in `reconstruct`: with "adam" the
+        measured loop updates z with Adam (rec_lr is then a step in z units), pruned or not."""
+        adam = self._adam_params()
         if prune is _NOT_GIVEN:
             if self.rec_prune is not None:
                 raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts from it: set "
@@ -414,7 +448,7 @@ class DefenseGANBase(object):
             prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                     z_row_offset, prune)
+                                                     z_row_offset, prune, adam)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -432,14 +466,16 @@ class DefenseGANBase(object):
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
+        kw = {} if adam is None else {"adam": adam}
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
-                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune)
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
+                                           **kw)
 
     def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                     prune):
+                                     prune, adam=None):
         """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements
-        (prune: the checked schedule, or None)."""
+        (prune: the checked schedule, or None; adam: the checked Adam parameters, or None)."""
         a = operator
         if a.layout == torch.sparse_coo:
             if a.dim() != 2 or a.dense_dim() != 0:
@@ -481,9 +517,11 @@ class DefenseGANBase(object):
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
+        kw = {} if adam is None else {"adam": adam}
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
-                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune)
+                                           out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
+                                           **kw)
 
     def _pixel_weights(self, pixel_weights, x):
         """pixel_weights broadcast to x's shape and materialised once, after one check of all values (finite, in [0, 1])."""
@@ -511,9 +549,11 @@ class DefenseGANBase(object):
             self.test_gen_test = test
 
     def rec_cache_dir(self, split: str, max_num: int = -1) -> str:
-        """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]/<split>[_debug]`
-        - the directory name the callers parse back with `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the
-        `_prune` part (only with `rec_prune` set) keeps pruned and unpruned reconstructions apart."""
+        """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]
+        [_adam{b1:g}-{b2:g}-{eps:g}]/<split>[_debug]` - the directory name the callers parse back with
+        `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the `_prune` part (only with `rec_prune` set) keeps pruned
+        and unpruned reconstructions apart, and the `_adam` part (only with rec_optimizer "adam") Adam's from
+        momentum's."""
         if max_num > 0:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}_num{:d}'.format(int(self.rec_rr), float(self.rec_lr),
                                                                    int(self.rec_iters), int(max_num))
@@ -521,6 +561,9 @@ class DefenseGANBase(object):
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}'.format(int(self.rec_rr), float(self.rec_lr), int(self.rec_iters))
         if self.rec_prune is not None:
             name += '_prune' + '-'.join('{:d}x{:d}'.format(int(it), int(keep)) for it, keep in self.rec_prune)
+        adam = self._adam_params()
+        if adam is not None:
+            name += '_adam{:g}-{:g}-{:g}'.format(*adam)
         out = os.path.join(self.checkpoint_dir, name, split)
         if self.debug:
             out += '_debug'

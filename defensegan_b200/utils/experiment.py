@@ -170,13 +170,16 @@ def get_cached_gan_data(gan, test_on_dev, orig_data_flag=None, flags: Optional[F
 # ------------------------------------------------------------------------------------------------------------------
 _REC_DIR_RE = re.compile(r"recs_rr(.*)_lr(.*)_iters(.*)")
 _REC_PRUNE_RE = re.compile(r"_prune(\d+x\d+(?:-\d+x\d+)*)")
+_G = r"(\d+(?:\.\d*)?(?:e[-+]\d+)?)"            # a number as '{:g}' writes it
+_REC_ADAM_RE = re.compile(r"_adam%s-%s-%s" % (_G, _G, _G))
 
 
 def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
     """blackbox.py:639-658 / whitebox.py:245-264: with `--rec_path` and `--defense_type defense_gan` the projection's
     hyper-parameters are parsed back from the cache directory name (`rec_cache_dir`), the restart-pruning schedule
     (`_prune<it>x<keep>[-<it>x<keep>...]`) included: `gan.rec_prune` becomes that schedule, or None when the name has
-    none; `--override` applies the `--rec_rr / --rec_lr / --rec_iters` values instead of the model cfg's."""
+    none; so is the optimiser (`_adam<b1>-<b2>-<eps>`): "adam" with those betas and eps, or "momentum" when the name
+    has none; `--override` applies the `--rec_rr / --rec_lr / --rec_iters` values instead of the model cfg's."""
     cfg = cfg or {}
     rr = cfg.get("REC_RR", gan.rec_rr)
     lr = cfg.get("REC_LR", gan.rec_lr)
@@ -192,6 +195,12 @@ def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
             gan.rec_rr, gan.rec_lr, gan.rec_iters = int(rr), float(lr), int(iters)
             prune = _REC_PRUNE_RE.findall(flags.rec_path)
             gan.rec_prune = [tuple(int(v) for v in p.split("x")) for p in prune[0].split("-")] if prune else None
+            adam = _REC_ADAM_RE.findall(flags.rec_path)
+            if adam:
+                b1, b2, eps = (float(v) for v in adam[0])
+                gan.rec_optimizer, gan.rec_adam_betas, gan.rec_adam_eps = "adam", (b1, b2), eps
+            else:
+                gan.rec_optimizer = "momentum"
         elif defense == "defense_gan":
             assert flags.online_training or not flags.train_on_recs
     if flags.override:

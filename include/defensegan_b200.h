@@ -281,6 +281,64 @@ int dgan_reconstruct_measured_csr_pruned(dgan_handle h, const dgan_rec_params* p
                                          int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
                                          float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
 
+/* Hyper-parameters of the Adam update (an extension: the reference optimises z with tf.train.MomentumOptimizer only). */
+typedef struct dgan_adam_params {
+  float beta1; /* [0, 1): decay of the first moment m */
+  float beta2; /* [0, 1): decay of the second moment s */
+  float eps;   /* finite, > 0 */
+} dgan_adam_params;
+
+/* Bytes of scratch for dgan_reconstruct_adam, with per-pixel weights when weighted != 0.  sched NULL and n_points 0: the
+ * workspace of dgan_workspace_bytes or dgan_workspace_bytes_weighted plus Adam's second moment s [n_pad][latent] fp32;
+ * a schedule: that of dgan_workspace_bytes_pruned with s in every region.  0 where those sizers return 0. */
+size_t dgan_workspace_bytes_adam(dgan_handle h, int batch, int rec_rr, int weighted, const dgan_prune_point* sched,
+                                 int n_points);
+
+/* Bytes of scratch for dgan_reconstruct_measured_adam with nnz = -1, or dgan_reconstruct_measured_csr_adam with nnz >= 0
+ * non-zeros.  Unpruned (sched NULL, n_points 0), the workspace of dgan_workspace_bytes_measured[_csr] plus s; a schedule:
+ * that of dgan_workspace_bytes_measured_pruned with s in every region.  0 where those sizers return 0. */
+size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_prune_point* sched,
+                                          int n_points);
+
+/* dgan_reconstruct (w_dev NULL) or dgan_reconstruct_weighted, with sched NULL and n_points 0, or dgan_reconstruct_pruned
+ * with a schedule, that updates z with Adam instead of momentum (an extension: GAN inversion and compressed sensing with
+ * generative models commonly use Adam).  For latent row n at iteration t, with k = t + 1 and g the gradient the momentum
+ * update uses (the split-K parts summed in order, times the loss's multiplier):
+ *   m = beta1 m + (1 - beta1) g;  s = beta2 s + (1 - beta2) g^2;  z = z - c1 m / (sqrt(s) c2 + eps)
+ *   c1 = lr_t / (1 - beta1^k), c2 = 1 / sqrt(1 - beta2^k), computed on the host in double and rounded to fp32;
+ * lr_t is rec_lr or its decay_lr schedule, as in dgan_reconstruct.  rec_lr is therefore a step in z units: the
+ * momentum path's values do not carry over.  params->momentum is ignored.  m and s start at 0 on every call; iteration
+ * L-1 runs no update.  The fp32 evaluation order is in kernels_adam.cuh (adam_kernel).  A coordinate whose gradient is
+ * always 0 - padded latent columns, an image whose pixel weights are all 0 - keeps its z0.  Loss, select, ties, the NaN rule and the
+ * prune ranking are those of the momentum entries; without BatchNorm each pruned survivor follows exactly its unpruned
+ * trajectory.  adam NULL, beta1 or beta2 outside [0, 1) or eps not finite and > 0: DGAN_ERR_INVALID_ARG, nothing
+ * enqueued; the checks of the momentum counterpart apply too (use_bn with a schedule: DGAN_ERR_UNSUPPORTED).
+ * Workspace: dgan_workspace_bytes_adam; s is zeroed by a memset with z0, and a prune point gathers it with z and m.
+ * Counts: dgan_last_enqueue_count is the momentum counterpart's; dgan_last_launch_count is the momentum counterpart's
+ * with DGAN_PREC_FP32, and L - 1 more with DGAN_PREC_FP16 (the momentum update runs in the Linear backward's tail there,
+ * the Adam update in a kernel of its own). */
+int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                          const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                          const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                          void* stream);
+
+/* dgan_reconstruct_measured, or dgan_reconstruct_measured_pruned with a schedule, with the Adam update of
+ * dgan_reconstruct_adam; g is the measured loop's gradient with the cotangent's row scales divided out.  Workspace:
+ * dgan_workspace_bytes_measured_adam with nnz = -1.  dgan_last_launch_count and dgan_last_enqueue_count equal the momentum
+ * counterpart's on both precisions (adam_kernel replaces the measured loop's momentum kernel). */
+int dgan_reconstruct_measured_adam(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                   const dgan_prune_point* sched, int n_points, const float* a_dev, int m, const float* y_dev,
+                                   const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                   size_t ws_bytes, void* stream);
+
+/* The same with the CSR operator of dgan_reconstruct_measured_csr (dgan_reconstruct_measured_csr_pruned with a
+ * schedule).  Workspace: dgan_workspace_bytes_measured_adam with this nnz; counts as the momentum counterpart's. */
+int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                       const dgan_prune_point* sched, int n_points, const int32_t* row_ptr,
+                                       const int32_t* col_idx, const float* val, int m, int nnz, const float* y_dev,
+                                       const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                       size_t ws_bytes, void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -329,12 +387,14 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * 256 channels, 1 + 10 L - 5 + 2).  A dgan_reconstruct_measured call runs 3 + 6 (L - 1) + 1 kernels more with
  * DGAN_PREC_FP16 and 3 + 3 (L - 1) + 1 more with DGAN_PREC_FP32 (see there); a dgan_reconstruct_measured_csr call
  * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more; a dgan_reconstruct_pruned call with P prune points 3 P + 1 more, and a
- * dgan_reconstruct_measured[_csr]_pruned call 3 P + 1 more than the unpruned measured call with the same operator kind. */
+ * dgan_reconstruct_measured[_csr]_pruned call 3 P + 1 more than the unpruned measured call with the same operator kind.
+ * An Adam call (dgan_reconstruct_adam, dgan_reconstruct_measured[_csr]_adam) runs as many as its momentum counterpart,
+ * plus L - 1 on the DGAN_PREC_FP16 image loss, whose Adam update is a kernel of its own. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
  * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
- * nnz and prune schedule) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * nnz, prune schedule and optimiser: momentum, or Adam with its beta1, beta2 and eps) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
  * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them),
  * graph, loss sum, arg-min select. */
 int64_t dgan_last_enqueue_count(dgan_handle h);
