@@ -43,6 +43,8 @@ ABI_SYMBOLS = [
     "dgan_workspace_bytes_measured_pruned", "dgan_reconstruct_measured_pruned", "dgan_reconstruct_measured_csr_pruned",
     "dgan_workspace_bytes_adam", "dgan_workspace_bytes_measured_adam", "dgan_reconstruct_adam", "dgan_reconstruct_measured_adam",
     "dgan_reconstruct_measured_csr_adam",
+    "dgan_reconstruct_huber", "dgan_reconstruct_measured_huber", "dgan_reconstruct_measured_csr_huber",
+    "dgan_loss_grad_huber", "dgan_loss_grad_measured_huber", "dgan_loss_grad_measured_csr_huber",
 ]
 
 
@@ -90,6 +92,21 @@ def check_adam_params(adam):
     if not (np.isfinite(eps) and eps > 0.0):
         raise ValueError("adam eps = %r must be finite and > 0" % (vals[2],))
     return b1, b2, eps
+
+
+def check_huber_delta(huber_delta):
+    """The Huber loss's delta as a float, after the rule of dgan_reconstruct_huber: > 0 as fp32 (the type the library
+    reads), +inf allowed.  A ValueError names the bad value (NaN, 0, a negative or a non-number)."""
+    if isinstance(huber_delta, bool) or not isinstance(huber_delta, (int, float, np.integer, np.floating)):
+        raise ValueError("huber_delta = %r is not a number" % (huber_delta,))
+    try:
+        with np.errstate(over="ignore"):   # beyond fp32's range: +-inf, as the library would read it
+            d = float(np.float32(huber_delta))
+    except OverflowError:                  # an int beyond a double's range
+        d = float("inf") if huber_delta > 0 else float("-inf")
+    if not d > 0.0:
+        raise ValueError("huber_delta = %r must be > 0 (+inf allowed)" % (huber_delta,))
+    return d
 
 
 def check_prune_schedule(prune, rec_rr: int, rec_iters: int):
@@ -242,6 +259,22 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_measured_csr_adam.restype = i32
     lib.dgan_reconstruct_measured_csr_adam.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, pp, i32, vp, vp, vp, i32, i32,
                                                        vp, vp, vp, vp, vp, vp, sz, vp]
+    f32 = ctypes.c_float
+    lib.dgan_reconstruct_huber.restype = i32
+    lib.dgan_reconstruct_huber.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, f32, pp, i32, vp, vp, vp, vp, vp, vp, vp,
+                                           sz, vp]
+    lib.dgan_reconstruct_measured_huber.restype = i32
+    lib.dgan_reconstruct_measured_huber.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, f32, pp, i32, vp, i32, vp, vp,
+                                                    vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_csr_huber.restype = i32
+    lib.dgan_reconstruct_measured_csr_huber.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, f32, pp, i32, vp, vp, vp,
+                                                        i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_huber.restype = i32
+    lib.dgan_loss_grad_huber.argtypes = [vp, f32, vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_measured_huber.restype = i32
+    lib.dgan_loss_grad_measured_huber.argtypes = [vp, f32, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_measured_csr_huber.restype = i32
+    lib.dgan_loss_grad_measured_csr_huber.argtypes = [vp, f32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
@@ -421,7 +454,8 @@ class NativeGenerator:
                     z_init_val: Optional[torch.Tensor] = None, seed: int = 0, momentum: float = 0.7,
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
                     z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None,
-                    prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None):
+                    prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
+                    huber_delta: Optional[float] = None):
         """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
         the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
         (dgan_reconstruct_weighted).
@@ -430,7 +464,12 @@ class NativeGenerator:
         original index.  None runs every restart to the end.
         adam ((beta1, beta2, eps), see check_adam_params): update z with Adam instead of momentum (dgan_reconstruct_adam,
         with or without pixel_weights and prune); momentum is then ignored, and rec_lr is Adam's step in z units, so the
-        momentum path's values do not carry over.  None runs the momentum update."""
+        momentum path's values do not carry over.  None runs the momentum update.
+        huber_delta (> 0, +inf allowed; see check_huber_delta): the Huber data term instead of the squared error
+        (dgan_reconstruct_huber, with any of pixel_weights, prune and adam): residuals beyond delta count linearly, so a
+        few badly wrong pixels pull the fit less.  With momentum the gradient of clipped residuals shrinks with delta, so
+        rec_lr has to grow as delta falls; Adam is invariant to that scale.  None runs the squared error, through exactly
+        the entry and arguments it always did."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
@@ -440,6 +479,7 @@ class NativeGenerator:
         pw = self._pixel_weights(pixel_weights, batch)
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
+        delta = None if huber_delta is None else check_huber_delta(huber_delta)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -456,7 +496,13 @@ class NativeGenerator:
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if ap is not None:
+            if delta is not None:
+                rc = self.lib.dgan_reconstruct_huber(self._handle, ctypes.byref(prm), ctypes.byref(ap) if ap is not None
+                                                     else None, delta, sched, len(sched) if sched is not None else 0,
+                                                     _ptr(x), _ptr(pw), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                     ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_huber")
+            elif ap is not None:
                 rc = self.lib.dgan_reconstruct_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
                                                     len(sched) if sched is not None else 0, _ptr(x), _ptr(pw), _ptr(z0),
                                                     _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
@@ -536,7 +582,8 @@ class NativeGenerator:
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
                              return_aux: bool = False, z_row_offset: int = 0,
-                             prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None):
+                             prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
+                             huber_delta: Optional[float] = None):
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
@@ -547,7 +594,10 @@ class NativeGenerator:
         the measured loss (dgan_reconstruct_measured_pruned, or dgan_reconstruct_measured_csr_pruned for a CSR operator).
         None runs every restart to the end.
         adam ((beta1, beta2, eps)): the Adam update of reconstruct (dgan_reconstruct_measured_adam, or
-        dgan_reconstruct_measured_csr_adam for a CSR operator), with or without prune."""
+        dgan_reconstruct_measured_csr_adam for a CSR operator), with or without prune.
+        huber_delta: the Huber loss of reconstruct on the measurement residuals, (1/m) sum_j rho_delta(r_j)
+        (dgan_reconstruct_measured_huber, or dgan_reconstruct_measured_csr_huber for a CSR operator), with any of prune
+        and adam.  None runs the squared error as before."""
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -557,6 +607,7 @@ class NativeGenerator:
             raise ValueError("rec_rr and rec_iters must be positive")
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
+        delta = None if huber_delta is None else check_huber_delta(huber_delta)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -574,7 +625,19 @@ class NativeGenerator:
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
             n_points = len(sched) if sched is not None else 0
-            if ap is not None and csr:
+            apr = ctypes.byref(ap) if ap is not None else None
+            if delta is not None and csr:
+                rc = self.lib.dgan_reconstruct_measured_csr_huber(self._handle, ctypes.byref(prm), apr, delta, sched, n_points,
+                                                                  _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
+                                                                  _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                                  ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_csr_huber")
+            elif delta is not None:
+                rc = self.lib.dgan_reconstruct_measured_huber(self._handle, ctypes.byref(prm), apr, delta, sched, n_points,
+                                                              _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
+                                                              ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_huber")
+            elif ap is not None and csr:
                 rc = self.lib.dgan_reconstruct_measured_csr_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
                                                                  n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
                                                                  _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
@@ -609,10 +672,12 @@ class NativeGenerator:
             return rec, loss, idx
         return rec
 
-    def loss_grad_measured(self, measurements: torch.Tensor, operator: torch.Tensor, z: torch.Tensor, rec_rr: int):
+    def loss_grad_measured(self, measurements: torch.Tensor, operator: torch.Tensor, z: torch.Tensor, rec_rr: int,
+                           huber_delta: Optional[float] = None):
         """(G(z), per-row measured loss, d(sum loss)/dz) at z [B*rec_rr, latent] for measurements [B, m] through operator
         [m, H*W*C]: one evaluation of reconstruct_measured's loop body (dgan_loss_grad_measured, or
-        dgan_loss_grad_measured_csr for a torch sparse CSR operator)."""
+        dgan_loss_grad_measured_csr for a torch sparse CSR operator).  huber_delta: with the Huber loss of
+        reconstruct_measured (dgan_loss_grad_measured[_csr]_huber); None: the squared error."""
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -622,13 +687,25 @@ class NativeGenerator:
         n = batch * rec_rr
         if zc.shape[0] != n:
             raise ValueError("z must have batch*rec_rr rows")
+        delta = None if huber_delta is None else check_huber_delta(huber_delta)
         with torch.cuda.device(self.device):
             g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
             loss = torch.empty(n, dtype=torch.float32, device=self.device)
             grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
             ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            if csr:
+            if delta is not None and csr:
+                _check(self.lib, self.lib.dgan_loss_grad_measured_csr_huber(self._handle, delta, _ptr(rp), _ptr(ci), _ptr(val),
+                                                                            m, nnz, _ptr(y), batch, rec_rr, _ptr(zc), _ptr(g),
+                                                                            _ptr(loss), _ptr(grad), ws, need,
+                                                                            ctypes.c_void_p(stream)),
+                       "dgan_loss_grad_measured_csr_huber")
+            elif delta is not None:
+                _check(self.lib, self.lib.dgan_loss_grad_measured_huber(self._handle, delta, _ptr(a), m, _ptr(y), batch, rec_rr,
+                                                                        _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
+                                                                        ctypes.c_void_p(stream)),
+                       "dgan_loss_grad_measured_huber")
+            elif csr:
                 _check(self.lib, self.lib.dgan_loss_grad_measured_csr(self._handle, _ptr(rp), _ptr(ci), _ptr(val), m, nnz,
                                                                       _ptr(y), batch, rec_rr, _ptr(zc), _ptr(g), _ptr(loss),
                                                                       _ptr(grad), ws, need, ctypes.c_void_p(stream)),
@@ -670,9 +747,11 @@ class NativeGenerator:
             raise ValueError("pixel_weights must be [B,%d,%d,%d] like the images" % self.image_dim)
         return pw
 
-    def loss_grad(self, images: torch.Tensor, z: torch.Tensor, rec_rr: int, pixel_weights: Optional[torch.Tensor] = None):
+    def loss_grad(self, images: torch.Tensor, z: torch.Tensor, rec_rr: int, pixel_weights: Optional[torch.Tensor] = None,
+                  huber_delta: Optional[float] = None):
         """(G(z), per-row loss, d(sum loss)/dz) at z [batch*rec_rr, latent]; with pixel_weights [B,H,W,C] the loss is the
-        weighted one of reconstruct (dgan_loss_grad_weighted)."""
+        weighted one of reconstruct (dgan_loss_grad_weighted); with huber_delta the Huber loss of reconstruct, weighted or
+        not (dgan_loss_grad_huber)."""
         x = _require_cuda_f32(images, "images")
         zc = _require_cuda_f32(z, "z")
         batch = x.shape[0]
@@ -680,13 +759,18 @@ class NativeGenerator:
         if zc.shape[0] != n:
             raise ValueError("z must have batch*rec_rr rows")
         pw = self._pixel_weights(pixel_weights, batch)
+        delta = None if huber_delta is None else check_huber_delta(huber_delta)
         with torch.cuda.device(self.device):
             y = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
             loss = torch.empty(n, dtype=torch.float32, device=self.device)
             grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
             ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            if pw is None:
+            if delta is not None:
+                _check(self.lib, self.lib.dgan_loss_grad_huber(self._handle, delta, _ptr(x), _ptr(pw), batch, rec_rr, _ptr(zc),
+                                                               _ptr(y), _ptr(loss), _ptr(grad), ws, need,
+                                                               ctypes.c_void_p(stream)), "dgan_loss_grad_huber")
+            elif pw is None:
                 _check(self.lib, self.lib.dgan_loss_grad(self._handle, _ptr(x), batch, rec_rr, _ptr(zc), _ptr(y), _ptr(loss),
                                                          _ptr(grad), ws, need, ctypes.c_void_p(stream)), "dgan_loss_grad")
             else:

@@ -324,17 +324,19 @@ struct dgan_ctx {
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
   // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise,
   // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise; adam: 1 for the Adam
-  // update with beta1, beta2 and eps, 0 for momentum) on a private stream, replayed with one cudaGraphLaunch per call.
+  // update with beta1, beta2 and eps, 0 for momentum; huber: the Huber entries' delta, 0 for the squared error) on a
+  // private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     std::vector<int> prune;
     cudaGraphExec_t exec; int64_t kernels;
     int adam = 0; float beta1 = 0.f, beta2 = 0.f, eps = 0.f;
+    float huber = 0.f;
     bool same_key(const LoopGraph& o) const {
       return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
              weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
              momentum == o.momentum && prune == o.prune && adam == o.adam && beta1 == o.beta1 && beta2 == o.beta2 &&
-             eps == o.eps;
+             eps == o.eps && huber == o.huber;
     }
   };
   std::vector<LoopGraph> graphs;
@@ -465,6 +467,9 @@ struct Workspace {
   // moment lives in v, the momentum buffer
   float* s = nullptr;
   size_t bytes = 0;
+  // The data term of the call the workspace serves: the Huber loss at this delta (> 0, +inf allowed; the Huber entries),
+  // or 0 for the squared error.  Set by the call, not carved: a Huber call's workspace is its counterpart's.
+  float huber = 0.f;
 };
 
 // The padded measurement count of a measured workspace: m rounded up to the measurement products' N tile.
@@ -680,7 +685,8 @@ static int launch_bsgemm_f32(dgan_ctx* c, int epi, const float* in, int C_in, in
   return 0;
 }
 
-// xw (not NULL, with x): the per-pixel weights of the squared error (the WEIGHTED instantiations)
+// xw (not NULL, with x): the per-pixel weights of the squared error (the WEIGHTED instantiations).  w.huber > 0 (with x):
+// the Huber loss (final_fwd_huber_kernel) instead of the squared error.
 template <typename TIN>
 static int launch_final_fwd(dgan_ctx* c, const TIN* hin, const Workspace& w, const float* x, int R, int B,
                             bool want_grad, cudaStream_t s, const float* xw = nullptr) {
@@ -692,11 +698,20 @@ static int launch_final_fwd(dgan_ctx* c, const TIN* hin, const Workspace& w, con
 #define FF(CO, ACT, WT)                                                                                         \
   final_fwd_loss_kernel<TIN, CO, ACT, WT><<<grid, block, smem, s>>>(hin, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, \
                                                                     f.bias, x, R, B, w.y, dpre ? dpre : w.dpre, lp, xw)
+#define FH(CO, ACT, WT)                                                                                          \
+  final_fwd_huber_kernel<TIN, CO, ACT, WT><<<grid, block, smem, s>>>(hin, w.n_pad, f.h_in, f.w_in, f.C_in, f.w, f.bias, x, R, \
+                                                                     B, w.y, dpre ? dpre : w.dpre, lp, xw, w.huber)
   const bool wt = xw != nullptr && x != nullptr;
-  if (f.C_out == 1 && f.act == ACT_SIGMOID) { if (wt) FF(1, ACT_SIGMOID, true); else FF(1, ACT_SIGMOID, false); }
-  else if (f.C_out == 3 && f.act == ACT_TANH) { if (wt) FF(3, ACT_TANH, true); else FF(3, ACT_TANH, false); }
-  else { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
+  const bool hub = w.huber > 0.f && x != nullptr;
+  if (f.C_out == 1 && f.act == ACT_SIGMOID) {
+    if (hub) { if (wt) FH(1, ACT_SIGMOID, true); else FH(1, ACT_SIGMOID, false); }
+    else if (wt) FF(1, ACT_SIGMOID, true); else FF(1, ACT_SIGMOID, false);
+  } else if (f.C_out == 3 && f.act == ACT_TANH) {
+    if (hub) { if (wt) FH(3, ACT_TANH, true); else FH(3, ACT_TANH, false); }
+    else if (wt) FF(3, ACT_TANH, true); else FF(3, ACT_TANH, false);
+  } else { set_error("unsupported final layer"); return DGAN_ERR_UNSUPPORTED; }
 #undef FF
+#undef FH
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
@@ -877,6 +892,7 @@ static int run_forward(dgan_ctx* c, const Workspace& w, const float* x, int R, i
     fa.nbx = c->fin.w_in / 2; fa.w_out = 2 * c->fin.w_in; fa.gscale = c->tc.grad_scale; fa.write_y = want_y ? 1 : 0;
     const bool weighted = x != nullptr && xw != nullptr;
     fa.xw = weighted ? xw : nullptr;
+    fa.huber = x != nullptr ? w.huber : 0.f;      // > 0: tc2_launch runs the Huber kind of the direction's final kind
     return tc_launch(c, w, 2 * nl, s, false, fa, weighted ? TC_PASS_WEIGHTED : TC_PASS_PROJ);
   }
   const float* in = w.z;
@@ -1067,7 +1083,12 @@ template <int EPI>
 static int launch_measured_gemm(dgan_ctx* c, const Workspace& w, const float* X, int ldx, const float* W, int ldw, int N,
                                 int K, float* out, int ldo, const float* ym, int R, float s_, float* loss_part, cudaStream_t s) {
   const dim3 grid((unsigned)((w.n_rows + kMeasTileM - 1) / kMeasTileM), (unsigned)((N + kMeasTileN - 1) / kMeasTileN));
-  if (c->desc.precision == DGAN_PREC_FP16)
+  if constexpr (EPI == MEAS_RESID_HUBER) {
+    if (c->desc.precision == DGAN_PREC_FP16)
+      measured_gemm_huber_kernel<true><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
+    else
+      measured_gemm_huber_kernel<false><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
+  } else if (c->desc.precision == DGAN_PREC_FP16)
     measured_gemm_kernel<true, EPI><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
   else
     measured_gemm_kernel<false, EPI><<<grid, 256, 0, s>>>(X, ldx, w.n_rows, W, ldw, N, K, out, ldo, ym, R, s_, loss_part, w.n_pad);
@@ -1091,6 +1112,9 @@ static int stage_measured_csr(dgan_ctx* c, const Workspace& w, const int* row_pt
   DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_csr_kernel<MEAS_SCALE>));
   if (fa.maxDynamicSharedSizeBytes < smem)
     DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_csr_kernel<MEAS_SCALE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_csr_huber_kernel));
+  if (fa.maxDynamicSharedSizeBytes < smem)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_csr_huber_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   csr_validate_kernel<<<(m + 255) / 256, 256, 0, s>>>(row_ptr, col_idx, m, w.nnz, hwc, w.csr_bad);
   DGAN_LAUNCH_CHECK(c);
   csr_stage_rows_kernel<<<1, 1024, 0, s>>>(row_ptr, w.csr_bad, m, w.m_ld, w.nnz, w.csr_valid, w.a_rp);
@@ -1113,14 +1137,26 @@ static int launch_measured_csr(dgan_ctx* c, const Workspace& w, const float* X, 
                                const int* ci, const float* val, int N, float* out, int ldo, const float* ym, int R,
                                float s_, float* loss_part, cudaStream_t s) {
   const unsigned grid = (unsigned)((w.n_rows + kCsrRows - 1) / kCsrRows);
-  measured_csr_kernel<EPI><<<grid, kCsrThreads, kCsrRows * K * sizeof(float), s>>>(X, ldx, w.n_rows, K, rp, ci, val, N, out,
-                                                                                    ldo, ym, R, s_, loss_part, w.n_pad);
+  if constexpr (EPI == MEAS_RESID_HUBER)
+    measured_csr_huber_kernel<<<grid, kCsrThreads, kCsrRows * K * sizeof(float), s>>>(X, ldx, w.n_rows, K, rp, ci, val, N,
+                                                                                      out, ldo, ym, R, s_, loss_part, w.n_pad);
+  else
+    measured_csr_kernel<EPI><<<grid, kCsrThreads, kCsrRows * K * sizeof(float), s>>>(X, ldx, w.n_rows, K, rp, ci, val, N,
+                                                                                      out, ldo, ym, R, s_, loss_part, w.n_pad);
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
 
-// The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.
+// The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.  w.huber > 0:
+// the Huber residual psi(r) and the Huber loss's parts (MEAS_RESID_HUBER, delta passed as the scale).
 static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  if (w.huber > 0.f) {
+    if (w.csr)
+      return launch_measured_csr<MEAS_RESID_HUBER>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld,
+                                                   w.ym, R, w.huber, w.mloss_part, s);
+    return launch_measured_gemm<MEAS_RESID_HUBER>(c, w, w.y, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R,
+                                                  w.huber, w.mloss_part, s);
+  }
   if (w.csr)
     return launch_measured_csr<MEAS_RESID>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld, w.ym, R,
                                            1.f, w.mloss_part, s);
@@ -1357,6 +1393,10 @@ static int create_impl(dgan_ctx* c, const dgan_desc* d, const float* const* weig
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<float, 1, ACT_SIGMOID, true>), kFinalSmemMax);   // the weighted loss
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_TANH, true>), kFinalSmemMax);
+  OPTIN((final_fwd_huber_kernel<float, 1, ACT_SIGMOID, false>), kFinalSmemMax);   // the Huber loss
+  OPTIN((final_fwd_huber_kernel<float, 3, ACT_TANH, false>), kFinalSmemMax);
+  OPTIN((final_fwd_huber_kernel<float, 1, ACT_SIGMOID, true>), kFinalSmemMax);
+  OPTIN((final_fwd_huber_kernel<float, 3, ACT_TANH, true>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<float, 1, ACT_NONE>), kFinalSmemMax);    // dgan_jvp's tangent of the last layer
   OPTIN((final_fwd_loss_kernel<float, 3, ACT_NONE>), kFinalSmemMax);
   OPTIN((final_fwd_loss_kernel<__half, 1, ACT_SIGMOID>), 100 * 1024);
@@ -1541,15 +1581,28 @@ static int stage_meas(dgan_ctx* c, const Workspace& w, const MeasuredArgs& meas,
   return stage_measured(c, w, meas.a, meas.y, batch, s);
 }
 
-// dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place
+// The Huber entries' delta: > 0, +inf allowed (NaN, 0 and negative values are refused).  huber NULL: a squared-error
+// call, nothing to check.  0, or DGAN_ERR_INVALID_ARG naming the bad value; the callers check it after every other
+// argument and before anything is enqueued.
+static int check_huber(const float* huber) {
+  if (huber == nullptr || *huber > 0.f) return 0;
+  set_error("invalid Huber delta = " + std::to_string(*huber) + ": it must be > 0 (+inf allowed)");
+  return DGAN_ERR_INVALID_ARG;
+}
+
+// dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place.
+// huber (not NULL): dgan_loss_grad_huber, the Huber loss at *huber.
 static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
-                          float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+                          float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream,
+                          const float* huber = nullptr) {
   if (h == nullptr || x_dev == nullptr || z_dev == nullptr || batch <= 0 || rec_rr <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
   Workspace w;
   int rc;
   if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, w_dev != nullptr))) return rc;
+  if ((rc = check_huber(huber))) return rc;
+  if (huber != nullptr) w.huber = *huber;
   if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
   if ((rc = run_forward(h, w, x_dev, rec_rr, batch, true, s, true, w_dev))) return rc;
   if ((rc = run_backward(h, w, s))) return rc;
@@ -1578,14 +1631,18 @@ int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_de
   return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
-// dgan_loss_grad_measured and dgan_loss_grad_measured_csr, after their operator checks
+// dgan_loss_grad_measured and dgan_loss_grad_measured_csr, after their operator checks; huber (not NULL): their Huber
+// entries, the Huber loss at *huber
 static int loss_grad_measured_impl(dgan_handle h, const MeasuredArgs& meas, int batch, int rec_rr, const float* z_dev,
-                                   float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+                                   float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream,
+                                   const float* huber = nullptr) {
   int rc;
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
   Workspace w;
   if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, meas.m, meas.nnz))) return rc;
+  if ((rc = check_huber(huber))) return rc;
+  if (huber != nullptr) w.huber = *huber;
   h->n_rows_cur = n_rows;
   if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_meas(h, w, meas, batch, s))) return rc;
   if ((rc = run_forward(h, w, nullptr, 1, 1, true, s)) || (rc = launch_measure(h, w, rec_rr, s))) return rc;
@@ -1846,10 +1903,12 @@ static int check_adam(const dgan_adam_params* a) {
 
 // dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
 // weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
-// the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).
+// the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).  huber
+// (not NULL): the Huber entries, the Huber loss at *huber on the counterpart's workspace.
 static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                             const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
-                            void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr) {
+                            void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
+                            const float* huber = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
@@ -1863,6 +1922,8 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   Workspace w;
   int rc;
   if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr))) return rc;
+  if ((rc = check_huber(huber))) return rc;
+  if (huber != nullptr) w.huber = *huber;
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
@@ -1882,6 +1943,7 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
                           prm->momentum, {}, nullptr, 0};
   set_optimizer_key(&key, adam);
+  key.huber = w.huber;
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
     return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls, false, adam);
   };
@@ -1971,11 +2033,13 @@ static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_poin
 // operator and measurements are staged once into the operator block that every region shares, and every stage runs the
 // measured loop; the measured forward leaves each iteration's loss parts in mloss_part, so a prune point sums them as
 // the plain loop's do loss_part.  adam (not NULL, checked by the caller): the Adam entries; a prune point gathers the
-// survivors' second moment with their z, m and z_h.
+// survivors' second moment with their z, m and z_h.  huber (not NULL): the Huber entries, every stage and the ranking on
+// the Huber loss at *huber.
 static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                    const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
-                                   MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr) {
+                                   MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
+                                   const float* huber = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
@@ -2001,9 +2065,11 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
                : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
+  if ((rc = check_huber(huber))) return rc;
   for (Workspace& w : regs) {
     if ((rc = build_maps(h, w))) return rc;
     if (weighted && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
+    if (huber != nullptr) w.huber = *huber;
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t launches0 = h->launches;
@@ -2030,6 +2096,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
                           prm->momentum, {}, nullptr, 0};
   for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
   set_optimizer_key(&key, adam);
+  key.huber = huber != nullptr ? *huber : 0.f;
   // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
   // (measured) left
   auto loss_finish = [&](const Workspace& w, cudaStream_t ls) -> int {
@@ -2201,16 +2268,18 @@ size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, 
   return bytes;
 }
 
-// The image and measured Adam entries after their own checks: unpruned through reconstruct_impl, pruned through
-// reconstruct_pruned_impl, as their momentum counterparts
+// The image and measured Adam and Huber entries after their own checks: unpruned through reconstruct_impl, pruned through
+// reconstruct_pruned_impl, as their momentum and squared-error counterparts (adam NULL: momentum; huber NULL: squared error)
 static int reconstruct_adam_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                  const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                                  const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
-                                 size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs()) {
+                                 size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs(),
+                                 const float* huber = nullptr) {
   if (unpruned(sched, n_points))
-    return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam);
+    return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam,
+                            huber);
   return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                                 stream, meas, adam);
+                                 stream, meas, adam, huber);
 }
 
 int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2248,6 +2317,77 @@ int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* prm
   meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
   return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
                                ws_bytes, stream, meas);
+}
+
+// ---- the Huber loss: each entry is its squared-error counterpart's code path with delta -------------------------------
+// adam NULL: the momentum counterpart; sched NULL with n_points 0: the unpruned one.  The counterpart's checks come first.
+int dgan_reconstruct_huber(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam, float huber_delta,
+                           const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                           const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                           void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                               stream, MeasuredArgs(), &huber_delta);
+}
+
+int dgan_reconstruct_measured_huber(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                    float huber_delta, const dgan_prune_point* sched, int n_points, const float* a_dev, int m,
+                                    const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                    int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, &huber_delta);
+}
+
+int dgan_reconstruct_measured_csr_huber(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                        float huber_delta, const dgan_prune_point* sched, int n_points,
+                                        const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                        const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                        int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, &huber_delta);
+}
+
+int dgan_loss_grad_huber(dgan_handle h, float huber_delta, const float* x_dev, const float* w_dev, int batch, int rec_rr,
+                         const float* z_dev, float* y_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes,
+                         void* stream) {
+  return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream, &huber_delta);
+}
+
+int dgan_loss_grad_measured_huber(dgan_handle h, float huber_delta, const float* a_dev, int m, const float* y_dev, int batch,
+                                  int rec_rr, const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws,
+                                  size_t ws_bytes, void* stream) {
+  if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
+                                 &huber_delta);
+}
+
+int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const int32_t* row_ptr, const int32_t* col_idx,
+                                      const float* val, int m, int nnz, const float* y_dev, int batch, int rec_rr,
+                                      const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws,
+                                      size_t ws_bytes, void* stream) {
+  if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
+                                 &huber_delta);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {

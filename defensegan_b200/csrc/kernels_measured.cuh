@@ -23,7 +23,18 @@
 namespace dgan {
 
 constexpr int kMeasTileM = 128, kMeasTileN = 64, kMeasTileK = 16;
-enum MeasEpi : int { MEAS_RESID = 0, MEAS_SCALE = 1 };
+// MEAS_RESID_HUBER (dgan_reconstruct_measured_huber): the Huber loss at delta = s > 0 instead of the squared error, see
+// meas_huber.
+enum MeasEpi : int { MEAS_RESID = 0, MEAS_SCALE = 1, MEAS_RESID_HUBER = 2 };
+
+// The Huber residual of r at delta: r is replaced by c = |r| > delta ? copysign(delta, r) : r (what the adjoint product
+// reads) and its loss term c (2 r - c) returned.  When |r| <= delta, c == r and the term is r * r to the bit.
+__device__ __forceinline__ float meas_huber(float& r, float delta) {
+  const float c = fabsf(r) > delta ? copysignf(delta, r) : r;
+  const float t = 2.f * r - c;
+  r = c;
+  return c * t;
+}
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t r;
@@ -38,12 +49,13 @@ __device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], 
 }
 
 // MEAS_RESID: out = acc - ym[row / R][col] (ym at row stride ldo), loss_part[blockIdx.y * loss_ld + row] = the block's
-// sum of out^2 over its columns.  MEAS_SCALE: out = s * acc.
+// sum of out^2 over its columns.  MEAS_RESID_HUBER: the same with out and its square replaced by meas_huber's c and term
+// at delta = s (measured_gemm_huber_kernel).  MEAS_SCALE: out = s * acc.
 template <bool TC, int EPI>
-__global__ void __launch_bounds__(256)
-measured_gemm_kernel(const float* __restrict__ X, int ldx, int M, const float* __restrict__ W, int ldw, int N, int K,
-                     float* __restrict__ out, int ldo, const float* __restrict__ ym, int R, float s,
-                     float* __restrict__ loss_part, int loss_ld) {
+__device__ __forceinline__ void
+measured_gemm_body(const float* __restrict__ X, int ldx, int M, const float* __restrict__ W, int ldw, int N, int K,
+                   float* __restrict__ out, int ldo, const float* __restrict__ ym, int R, float s,
+                   float* __restrict__ loss_part, int loss_ld) {
   // TC: [buf][row][k] at stride 20 (conflict-free fragment reads); not TC: [buf][k][row] at strides 132 and 68
   constexpr int kLd = kMeasTileK + 4;
   constexpr int kStage = TC ? (kMeasTileM + kMeasTileN) * kLd : kMeasTileK * (kMeasTileM + 4 + kMeasTileN + 4);
@@ -141,6 +153,10 @@ measured_gemm_kernel(const float* __restrict__ X, int ldx, int M, const float* _
       v -= ym[(size_t)(row / R) * ldo + col];
       return v * v;
     }
+    if (EPI == MEAS_RESID_HUBER) {
+      v -= ym[(size_t)(row / R) * ldo + col];
+      return meas_huber(v, s);
+    }
     v *= s;
     return 0.f;
   };
@@ -159,7 +175,7 @@ measured_gemm_kernel(const float* __restrict__ X, int ldx, int M, const float* _
           rs[mi][h] += epi(row, col, v0) + epi(row, col + 1, v1);
           *reinterpret_cast<float2*>(out + (size_t)row * ldo + col) = make_float2(v0, v1);
         }
-    if (EPI == MEAS_RESID) {
+    if (EPI != MEAS_SCALE) {
 #pragma unroll
       for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
@@ -183,13 +199,30 @@ measured_gemm_kernel(const float* __restrict__ X, int ldx, int M, const float* _
         for (int j = 0; j < 4; ++j) rsum += epi(row, col + j, v[j]);
         *reinterpret_cast<float4*>(out + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
       }
-      if (EPI == MEAS_RESID) {
+      if (EPI != MEAS_SCALE) {
 #pragma unroll
         for (int o = 1; o < 16; o <<= 1) rsum += __shfl_xor_sync(0xffffffffu, rsum, o);
         if (tx == 0 && row < M) loss_part[(size_t)blockIdx.y * loss_ld + row] = rsum;
       }
     }
   }
+}
+
+template <bool TC, int EPI>
+__global__ void __launch_bounds__(256)
+measured_gemm_kernel(const float* __restrict__ X, int ldx, int M, const float* __restrict__ W, int ldw, int N, int K,
+                     float* __restrict__ out, int ldo, const float* __restrict__ ym, int R, float s,
+                     float* __restrict__ loss_part, int loss_ld) {
+  measured_gemm_body<TC, EPI>(X, ldx, M, W, ldw, N, K, out, ldo, ym, R, s, loss_part, loss_ld);
+}
+
+// The measurement product with the Huber residual (MEAS_RESID_HUBER) at delta = s
+template <bool TC>
+__global__ void __launch_bounds__(256)
+measured_gemm_huber_kernel(const float* __restrict__ X, int ldx, int M, const float* __restrict__ W, int ldw, int N, int K,
+                           float* __restrict__ out, int ldo, const float* __restrict__ ym, int R, float s,
+                           float* __restrict__ loss_part, int loss_ld) {
+  measured_gemm_body<TC, MEAS_RESID_HUBER>(X, ldx, M, W, ldw, N, K, out, ldo, ym, R, s, loss_part, loss_ld);
 }
 
 // The momentum update of tf.train.MomentumOptimizer (as momentum_kernel) with a multiplier per latent row: the gradient of

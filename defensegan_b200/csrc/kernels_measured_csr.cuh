@@ -32,13 +32,16 @@ constexpr int kCsrThreads = 256;
 
 // EPI(X A^T) of kCsrRows rows of X [M][K] (row stride ldx) through a CSR operator (rp [N + 1], ci / val) with N output
 // columns: out [M][ldo].  MEAS_RESID: out = acc - ym[row / R][col] (ym at row stride ldo) and
-// loss_part[(col / 64) * loss_ld + row] = the 64-column tile's sum of out^2 (N % 64 == 0).  MEAS_SCALE: out = s * acc.
+// loss_part[(col / 64) * loss_ld + row] = the 64-column tile's sum of out^2 (N % 64 == 0).  MEAS_RESID_HUBER: the same
+// with out and its square replaced by meas_huber's c and term at delta = s, as the dense kernel's
+// (measured_csr_huber_kernel).  MEAS_SCALE:
+// out = s * acc.
 // K % 4 == 0, N % 4 == 0, ldx % 4 == 0.  Dynamic shared memory: kCsrRows * K floats.
 template <int EPI>
-__global__ void __launch_bounds__(kCsrThreads)
-measured_csr_kernel(const float* __restrict__ X, int ldx, int M, int K, const int* __restrict__ rp,
-                    const int* __restrict__ ci, const float* __restrict__ val, int N, float* __restrict__ out, int ldo,
-                    const float* __restrict__ ym, int R, float s, float* __restrict__ loss_part, int loss_ld) {
+__device__ __forceinline__ void
+measured_csr_body(const float* __restrict__ X, int ldx, int M, int K, const int* __restrict__ rp,
+                  const int* __restrict__ ci, const float* __restrict__ val, int N, float* __restrict__ out, int ldo,
+                  const float* __restrict__ ym, int R, float s, float* __restrict__ loss_part, int loss_ld) {
   extern __shared__ __align__(16) float xs[];        // [kCsrRows][K]
   const int tid = threadIdx.x;
   const int m0 = blockIdx.x * kCsrRows;
@@ -87,19 +90,40 @@ measured_csr_kernel(const float* __restrict__ X, int ldx, int M, int K, const in
           if (EPI == MEAS_RESID) {
             v[j] = acc[r][j] - ym[(size_t)(row / R) * ldo + col + j];
             rsum = fmaf(v[j], v[j], rsum);
+          } else if (EPI == MEAS_RESID_HUBER) {
+            const float rj = acc[r][j] - ym[(size_t)(row / R) * ldo + col + j];
+            v[j] = fabsf(rj) > s ? copysignf(s, rj) : rj;
+            rsum = fmaf(v[j], 2.f * rj - v[j], rsum);
           } else {
             v[j] = acc[r][j] * s;
           }
         }
         *reinterpret_cast<float4*>(out + (size_t)row * ldo + col) = make_float4(v[0], v[1], v[2], v[3]);
       }
-      if (EPI == MEAS_RESID) {
+      if (EPI != MEAS_SCALE) {
 #pragma unroll
         for (int o = 1; o < 16; o <<= 1) rsum += __shfl_xor_sync(0xffffffffu, rsum, o);
         if (active && (q & 15) == 0) loss_part[(size_t)(q / 16) * loss_ld + row] = rsum;
       }
     }
   }
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(kCsrThreads)
+measured_csr_kernel(const float* __restrict__ X, int ldx, int M, int K, const int* __restrict__ rp,
+                    const int* __restrict__ ci, const float* __restrict__ val, int N, float* __restrict__ out, int ldo,
+                    const float* __restrict__ ym, int R, float s, float* __restrict__ loss_part, int loss_ld) {
+  measured_csr_body<EPI>(X, ldx, M, K, rp, ci, val, N, out, ldo, ym, R, s, loss_part, loss_ld);
+}
+
+// The measurement product with the Huber residual (MEAS_RESID_HUBER) at delta = s
+__global__ void __launch_bounds__(kCsrThreads)
+measured_csr_huber_kernel(const float* __restrict__ X, int ldx, int M, int K, const int* __restrict__ rp,
+                          const int* __restrict__ ci, const float* __restrict__ val, int N, float* __restrict__ out,
+                          int ldo, const float* __restrict__ ym, int R, float s, float* __restrict__ loss_part,
+                          int loss_ld) {
+  measured_csr_body<MEAS_RESID_HUBER>(X, ldx, M, K, rp, ci, val, N, out, ldo, ym, R, s, loss_part, loss_ld);
 }
 
 // ---- staging ---------------------------------------------------------------------------------------------------------

@@ -130,15 +130,14 @@ constexpr int kBandRows = 4;
 
 // WEIGHTED (dgan_reconstruct_weighted): xw [B][P_out*C_OUT] weights each pixel's squared error, e = xw (y - x): the loss
 // takes e (y - x) and dpre = e act'(y).  With xw = 1, e == y - x, so every output is the unweighted kernel's.
-template <typename TIN, int C_OUT, int ACT, bool WEIGHTED = false>
-__global__ void __launch_bounds__(128)
-final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in, int C_in,
-                      const float* __restrict__ w /*[25][C_OUT][C_in]*/, const float* __restrict__ bias,
-                      const float* __restrict__ x /*[B][P_out*C_OUT] or null*/, int R, int B,
-                      float* __restrict__ y /*[n_pad][P_out*C_OUT]*/,
-                      float* __restrict__ dpre /*[n_pad][P_out*C_OUT] or null*/,
-                      float* __restrict__ loss_part /*[n_pad][n_bands] or null*/,
-                      const float* __restrict__ xw = nullptr /*[B][P_out*C_OUT], WEIGHTED only*/) {
+// HUBER (dgan_reconstruct_huber; x not null): the Huber loss at delta = huber > 0 instead of the squared error.  With
+// d = y - x and c = |d| > delta ? copysign(delta, d) : d, e = xw c (e = c unweighted): the loss takes e (2 d - c) and
+// dpre = e act'(y).  When no |d| exceeds delta, c == d and 2 d - c == d, so every output is the squared-error kernel's.
+template <typename TIN, int C_OUT, int ACT, bool WEIGHTED, bool HUBER>
+__device__ __forceinline__ void
+final_fwd_loss_body(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in, int C_in, const float* __restrict__ w,
+                    const float* __restrict__ bias, const float* __restrict__ x, int R, int B, float* __restrict__ y,
+                    float* __restrict__ dpre, float* __restrict__ loss_part, const float* __restrict__ xw, float huber) {
   extern __shared__ __align__(16) float smem_f[];
   const int ldh = C_in + 4;
   float* ws = smem_f;                                  // [25*C_OUT][C_in]
@@ -202,7 +201,14 @@ final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in
       else if (ACT == ACT_TANH) { yv = tanhf(acc[co]); dact = 1.f - yv * yv; }
       else { yv = acc[co]; dact = 1.f; }
       y[ob + co] = yv;
-      if (WEIGHTED) {
+      if (HUBER) {
+        const size_t xi = (size_t)img * h_out * px_per_row + (size_t)i * px_per_row + j * C_OUT + co;
+        const float d = yv - x[xi];
+        const float c = fabsf(d) > huber ? copysignf(huber, d) : d;
+        const float e = WEIGHTED ? xw[xi] * c : c;
+        lsum = fmaf(e, 2.f * d - c, lsum);
+        dpre[ob + co] = e * dact;
+      } else if (WEIGHTED) {
         const size_t xi = (size_t)img * h_out * px_per_row + (size_t)i * px_per_row + j * C_OUT + co;
         const float d = yv - x[xi];
         const float e = xw[xi] * d;
@@ -222,6 +228,29 @@ final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in
     __syncthreads();
     if (tid == 0) loss_part[(size_t)n * gridDim.y + band] = (red[0] + red[1]) + (red[2] + red[3]);
   }
+}
+
+template <typename TIN, int C_OUT, int ACT, bool WEIGHTED = false>
+__global__ void __launch_bounds__(128)
+final_fwd_loss_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in, int C_in,
+                      const float* __restrict__ w /*[25][C_OUT][C_in]*/, const float* __restrict__ bias,
+                      const float* __restrict__ x /*[B][P_out*C_OUT] or null*/, int R, int B,
+                      float* __restrict__ y /*[n_pad][P_out*C_OUT]*/,
+                      float* __restrict__ dpre /*[n_pad][P_out*C_OUT] or null*/,
+                      float* __restrict__ loss_part /*[n_pad][n_bands] or null*/,
+                      const float* __restrict__ xw = nullptr /*[B][P_out*C_OUT], WEIGHTED only*/) {
+  final_fwd_loss_body<TIN, C_OUT, ACT, WEIGHTED, false>(hin, n_pad, h_in, w_in, C_in, w, bias, x, R, B, y, dpre, loss_part,
+                                                        xw, 0.f);
+}
+
+// The Huber loss of final_fwd_loss_kernel (x, dpre and loss_part not null; xw too when WEIGHTED)
+template <typename TIN, int C_OUT, int ACT, bool WEIGHTED>
+__global__ void __launch_bounds__(128)
+final_fwd_huber_kernel(const TIN* __restrict__ hin, int n_pad, int h_in, int w_in, int C_in, const float* __restrict__ w,
+                       const float* __restrict__ bias, const float* __restrict__ x, int R, int B, float* __restrict__ y,
+                       float* __restrict__ dpre, float* __restrict__ loss_part, const float* __restrict__ xw, float huber) {
+  final_fwd_loss_body<TIN, C_OUT, ACT, WEIGHTED, true>(hin, n_pad, h_in, w_in, C_in, w, bias, x, R, B, y, dpre, loss_part,
+                                                       xw, huber);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -150,7 +150,18 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 // (models/dataset_models.py:68-69,161-163; models/gan.py:411-414).
 // The _W kinds weight the squared error per pixel (dgan_reconstruct_weighted): e = w (y - x), loss part += e (y - x),
 // d(pre) = e act'(y); with w = 1, e == y - x and every stored value is the unweighted kind's.
-enum TcEpilogue : int { EPI_FINAL_SIGMOID1 = 8, EPI_FINAL_TANH3 = 9, EPI_FINAL_SIGMOID1_W = 10, EPI_FINAL_TANH3_W = 11 };
+// The _H kinds (and _WH, weighted) replace the squared error by the Huber loss at delta = TcFinalArgs::huber
+// (dgan_reconstruct_huber): with d = y - x, c = |d| > delta ? copysign(delta, d) : d, e = w c (e = c unweighted), the loss
+// part takes e (2 d - c) and d(pre) = e act'(y).  When no |d| exceeds delta, c == d and 2 d - c == d, so every stored
+// value is the squared-error kind's.  They run on the plans of the kinds they replace (tc2_launch selects them).
+enum TcEpilogue : int { EPI_FINAL_SIGMOID1 = 8, EPI_FINAL_TANH3 = 9, EPI_FINAL_SIGMOID1_W = 10, EPI_FINAL_TANH3_W = 11,
+                        EPI_FINAL_SIGMOID1_H = 12, EPI_FINAL_TANH3_H = 13, EPI_FINAL_SIGMOID1_WH = 14, EPI_FINAL_TANH3_WH = 15 };
+// The Huber kind that replaces final kind epi (any other epilogue is returned unchanged)
+__host__ __device__ constexpr int tc_huber_epi(int epi) {
+  return epi == EPI_FINAL_SIGMOID1 ? EPI_FINAL_SIGMOID1_H : epi == EPI_FINAL_TANH3 ? EPI_FINAL_TANH3_H
+       : epi == EPI_FINAL_SIGMOID1_W ? EPI_FINAL_SIGMOID1_WH : epi == EPI_FINAL_TANH3_W ? EPI_FINAL_TANH3_WH : epi;
+}
+__host__ __device__ constexpr bool tc_final_epi(int epi) { return epi >= EPI_FINAL_SIGMOID1 && epi <= EPI_FINAL_TANH3_WH; }
 
 struct TcFinalArgs {
   const float* x;        // [B][H*W*C] target images (NULL: forward only)
@@ -180,6 +191,8 @@ struct TcFinalArgs {
   // The weighted last-layer epilogues: [B][H*W*C] per-pixel weights of the squared error, indexed as x.  Last, so that
   // every other field keeps its offset.
   const float* xw;
+  // The Huber final kinds: delta (> 0, +inf allowed); 0 selects the squared-error kinds.  After xw for the same reason.
+  float huber;
 };
 
 // ------------------------------------------------------------------------------------------

@@ -57,8 +57,7 @@ __host__ __device__ constexpr int tc2_acc_stride(int n_tile) { return n_tile <= 
 
 // Does this instantiation stage its output tiles through shared memory + TMA?
 __host__ __device__ constexpr bool tc2_tma_epilogue(int n_tile, int epi, int out_bytes) {
-  return out_bytes == 2 && n_tile >= 64 && epi != EPI_FINAL_SIGMOID1 && epi != EPI_FINAL_TANH3 && epi != EPI_FINAL_SIGMOID1_W &&
-         epi != EPI_FINAL_TANH3_W;
+  return out_bytes == 2 && n_tile >= 64 && !tc_final_epi(epi);
 }
 
 constexpr int TC2_REC_BATCH = 16;
@@ -127,7 +126,9 @@ struct Tc2Cfg {
 // backward: K = 16 (MNIST: EPI_MASK, or EPI_NONE with BatchNorm) and K = 48 (CelebA), at N = 64 (net_dim <= 64) and
 // N = 128 (64 < net_dim <= 128).  N = 16 / 48 with EPI_NONE and fp32 output: dgan_jvp's tangent of the last layer's
 // pre-activation (last.jvp), on the last layer's forward geometry.  The _W final kinds: the weighted last-layer forward
-// (last.fwd.w, dgan_reconstruct_weighted), at the N / slots / k16 of the unweighted final kinds.
+// (last.fwd.w, dgan_reconstruct_weighted), at the N / slots / k16 of the unweighted final kinds.  The _H / _WH kinds: the
+// Huber loss of the final kinds (dgan_reconstruct_huber), at the N / slots / k16 of the kinds they replace; tc2_launch runs
+// them on those kinds' plans when TcFinalArgs::huber > 0.
 #define TC2_KINDS(X)                                                                                                   \
   X(256, 1, 4, EPI_BIAS_RELU, __half) X(256, 1, 4, EPI_BIAS, __half) X(256, 1, 4, EPI_MASK, __half)                    \
   X(256, 1, 4, EPI_NONE, __half) X(256, 1, 4, EPI_NONE, float) X(256, 1, 4, EPI_BIAS, float)                           \
@@ -140,7 +141,9 @@ struct Tc2Cfg {
   X(128, 2, 1, EPI_MASK, __half) X(128, 2, 1, EPI_NONE, __half) X(128, 2, 3, EPI_NONE, __half)                         \
   X(16, 8, 4, EPI_FINAL_SIGMOID1, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1, __half) X(48, 4, 4, EPI_FINAL_TANH3, __half)   \
   X(16, 8, 4, EPI_NONE, float) X(48, 4, 4, EPI_NONE, float)                                                              \
-  X(16, 8, 4, EPI_FINAL_SIGMOID1_W, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1_W, __half) X(48, 4, 4, EPI_FINAL_TANH3_W, __half)
+  X(16, 8, 4, EPI_FINAL_SIGMOID1_W, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1_W, __half) X(48, 4, 4, EPI_FINAL_TANH3_W, __half)   \
+  X(16, 8, 4, EPI_FINAL_SIGMOID1_H, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1_H, __half) X(48, 4, 4, EPI_FINAL_TANH3_H, __half)   \
+  X(16, 8, 4, EPI_FINAL_SIGMOID1_WH, __half) X(16, 4, 4, EPI_FINAL_SIGMOID1_WH, __half) X(48, 4, 4, EPI_FINAL_TANH3_WH, __half)
 
 struct Tc2Kind { int n, maxb, ksub, epi, out_bytes; };
 #define TC2_KIND_ROW(NT, MB, KS, EP, T) {NT, MB, KS, EP, (int)sizeof(T)},
@@ -358,7 +361,9 @@ __device__ __forceinline__ long long probe_clock_after64(unsigned long long v) {
 __device__ __forceinline__ unsigned long long probe_bits(float2 v) {
   return ((unsigned long long)__float_as_uint(v.y) << 32) | __float_as_uint(v.x);
 }
+// Keys 0 - 39: (N class) * 8 + epilogue; 40 - 43: the Huber final kinds, one key each (tools/probe_step.py decodes both).
 __host__ __device__ constexpr int tc2_probe_key(int n_tile, int epi, int out_bytes) {
+  if (epi >= EPI_FINAL_SIGMOID1_H) return 40 + epi - EPI_FINAL_SIGMOID1_H;
   return (n_tile == 256 ? 0 : n_tile == 128 ? 1 : n_tile == 64 ? 2 : n_tile == 48 ? 3 : 4) * 8 + (out_bytes == 4 ? 6 : (epi < 4 ? epi : epi - 4));
 }
 #endif
@@ -373,9 +378,13 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                   TOUT* __restrict__ out, int n_pad, const float* __restrict__ bias, int bias_pstride, const TcFinalArgs fa) {
   using Cfg = Tc2Cfg<N_TILE, MAXB, KSUB, EPI, (int)sizeof(TOUT)>;
   constexpr bool TMA_EPI = Cfg::TMA_EPI;
-  constexpr bool WEIGHTED = (EPI == EPI_FINAL_SIGMOID1_W || EPI == EPI_FINAL_TANH3_W);
-  constexpr bool FINAL = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_TANH3 || WEIGHTED);
-  constexpr bool SIGMOID1 = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_SIGMOID1_W);
+  constexpr bool HUBER = (EPI == EPI_FINAL_SIGMOID1_H || EPI == EPI_FINAL_TANH3_H || EPI == EPI_FINAL_SIGMOID1_WH ||
+                          EPI == EPI_FINAL_TANH3_WH);
+  constexpr bool WEIGHTED = (EPI == EPI_FINAL_SIGMOID1_W || EPI == EPI_FINAL_TANH3_W || EPI == EPI_FINAL_SIGMOID1_WH ||
+                             EPI == EPI_FINAL_TANH3_WH);
+  constexpr bool FINAL = tc_final_epi(EPI);
+  constexpr bool SIGMOID1 = (EPI == EPI_FINAL_SIGMOID1 || EPI == EPI_FINAL_SIGMOID1_W || EPI == EPI_FINAL_SIGMOID1_H ||
+                             EPI == EPI_FINAL_SIGMOID1_WH);
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS);
   constexpr int B_TILE = Cfg::B_TILE, A_BYTES = Cfg::A_BYTES;
   constexpr int PRODUCER = TC2_CONSUMERS / 32;     // warp index of the TMA producer
@@ -735,7 +744,13 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                 else { const float t = __expf(-2.f * fabsf(pre)); yy = copysignf(__fdividef(1.f - t, 1.f + t), pre); dact = 1.f - yy * yy; }
                 yv[c] = yy;
                 float d = 0.f;
-                if (WEIGHTED) {           // e = w d: the loss part takes e d, d(pre) e act'(y)
+                if (HUBER) {              // c = psi_delta(d), e = w c: the loss part takes e (2 d - c), d(pre) e act'(y)
+                  d = yy - (c ? xv.y : xv.x);
+                  const float cl = fabsf(d) > fa.huber ? copysignf(fa.huber, d) : d;
+                  const float ew = WEIGHTED ? (c ? wv.y : wv.x) * cl : cl;
+                  lsum = fmaf(ew, 2.f * d - cl, lsum);
+                  d = ew;
+                } else if (WEIGHTED) {    // e = w d: the loss part takes e d, d(pre) e act'(y)
                   d = yy - (c ? xv.y : xv.x);
                   const float ew = (c ? wv.y : wv.x) * d;
                   lsum = fmaf(ew, d, lsum);
@@ -1586,7 +1601,8 @@ static int tc2_optin_all() {
 }
 
 // Launch layer-direction d on n_pad rows with the schedule tc2_get_schedule made for them.  tm_a, tm_out: the tensor
-// maps of its input and output; out: its output, of d.out_bytes per element.
+// maps of its input and output; out: its output, of d.out_bytes per element.  fa.huber > 0: the Huber kind of d's final
+// kind (tc_huber_epi), on d's plan.
 static int tc2_launch(int64_t* launches, const TcDir& d, const CUtensorMap& tm_a, const CUtensorMap& tm_out, void* out,
                       int n_pad, const float* bias, cudaStream_t s, const TcFinalArgs& fa) {
   if (n_pad % (2 * kRowTile) != 0) { set_error("pair kernel needs n_pad % 256 == 0"); return DGAN_ERR_INVALID_ARG; }
@@ -1599,8 +1615,9 @@ static int tc2_launch(int64_t* launches, const TcDir& d, const CUtensorMap& tm_a
   cudaError_t le = cudaSuccess;
   bool found = false;
   const int ksub = tc2_ksub(d.K);
+  const int epi = fa.huber > 0.f ? tc_huber_epi(d.epi) : d.epi;
 #define TC2_GO(NT, MB, KS, EP, T)                                                                                      \
-  if (!found && d.N == NT && sc->maxb == MB && ksub == KS && d.epi == EP && d.out_bytes == (int)sizeof(T)) {           \
+  if (!found && d.N == NT && sc->maxb == MB && ksub == KS && epi == EP && d.out_bytes == (int)sizeof(T)) {             \
     found = true;                                                                                                     \
     le = launch_pdl(tc_bsgemm2_kernel<NT, MB, KS, EP, T>, dim3(grid), dim3(TC2_THREADS), Tc2Cfg<NT, MB, KS, EP, (int)sizeof(T)>::SMEM_BYTES, s, \
                     tm_a, d.tm_b, tm_out, sc->items, sc->stream_p, sc->stream_m, sc->heads, sc->eitems, sc->n_slots,     \

@@ -123,6 +123,7 @@ class DefenseGANBase(object):
         self.rec_optimizer = "momentum"    # update of z: "momentum" (the reference's) | "adam" (cfg REC_OPTIMIZER)
         self.rec_adam_betas = (0.9, 0.999)  # Adam's (beta1, beta2) (cfg REC_ADAM_BETAS), read with rec_optimizer "adam"
         self.rec_adam_eps = 1e-8           # Adam's eps (cfg REC_ADAM_EPS)
+        self.rec_huber_delta = None        # data term: None = squared error (the reference's) | Huber delta > 0 (cfg REC_HUBER_DELTA)
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
 
         self.test_mode = test_mode
@@ -356,9 +357,19 @@ class DefenseGANBase(object):
         rec_adam_eps, with m and s reset on every call and bias correction at step k = t + 1; rec_momentum is then
         ignored.  Adam's rec_lr is a step in z units (each coordinate moves by about rec_lr per step early on), so the
         reference's rec_lr = 10.0 does not carry over: choose it for the problem.  It combines with pixel_weights and
-        rec_prune.  The values are checked before any native call (a ValueError naming the bad value)."""
+        rec_prune.  The values are checked before any native call (a ValueError naming the bad value).
+
+        `rec_huber_delta` (an extension, read at call time; None by default, the reference's squared error): a delta > 0
+        (+inf allowed) replaces the squared error by the Huber loss, quadratic for |G(z)_p - x_p| <= delta and linear
+        beyond, so a few badly wrong pixels - impulse noise, dead pixels, an occluder whose place is not known - pull the
+        fit much less; pixel_weights would need to know where they are.  The loss stays (1/HWC) sum_p w_p rho(d_p) with
+        rho = 2 huber_loss, so delta = +inf, or delta >= 2 on images in the generator's output range, gives the squared
+        error's bits.  With momentum the gradient of clipped residuals shrinks with delta, so rec_lr has to grow as delta
+        falls; with rec_optimizer "adam" it does not.  It combines with pixel_weights, rec_prune and Adam, and is checked
+        before any native call (a ValueError naming the bad value)."""
         prune = self._prune_schedule()
         adam = self._adam_params()
+        huber = self._huber_delta()
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
@@ -373,6 +384,8 @@ class DefenseGANBase(object):
             kw["prune"] = prune
         if adam is not None:
             kw["adam"] = adam
+        if huber is not None:
+            kw["huber_delta"] = huber
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
@@ -404,6 +417,15 @@ class DefenseGANBase(object):
             raise ValueError("rec_adam_betas = %r: expected a pair (beta1, beta2)" % (betas,))
         return _native.check_adam_params((betas[0], betas[1], self.rec_adam_eps))
 
+    def _huber_delta(self):
+        """`rec_huber_delta` checked (None when unset): a float > 0, +inf allowed; ValueError before any native call."""
+        if self.rec_huber_delta is None:
+            return None
+        try:
+            return _native.check_huber_delta(self.rec_huber_delta)
+        except ValueError as e:
+            raise ValueError("rec_huber_delta: %s" % e) from None
+
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
                              z_row_offset=0, prune=_NOT_GIVEN):
         """Projection onto the generator's range from linear measurements (an extension; the reference has none), for
@@ -434,8 +456,12 @@ class DefenseGANBase(object):
         end whatever `rec_prune` holds.
 
         `rec_optimizer`, `rec_adam_betas` and `rec_adam_eps` are read at call time as in `reconstruct`: with "adam" the
-        measured loop updates z with Adam (rec_lr is then a step in z units), pruned or not."""
+        measured loop updates z with Adam (rec_lr is then a step in z units), pruned or not.
+
+        `rec_huber_delta` is read at call time as in `reconstruct`: a delta replaces the squared error of each measurement
+        residual by the Huber loss, (1/m) sum_j rho(r_j), for a few corrupted measurements, dense or sparse, pruned or not."""
         adam = self._adam_params()
+        huber = self._huber_delta()
         if prune is _NOT_GIVEN:
             if self.rec_prune is not None:
                 raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts from it: set "
@@ -448,7 +474,7 @@ class DefenseGANBase(object):
             prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                     z_row_offset, prune, adam)
+                                                     z_row_offset, prune, adam, huber)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -467,15 +493,18 @@ class DefenseGANBase(object):
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
         kw = {} if adam is None else {"adam": adam}
+        if huber is not None:
+            kw["huber_delta"] = huber
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
                                            **kw)
 
     def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                     prune, adam=None):
+                                     prune, adam=None, huber=None):
         """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements
-        (prune: the checked schedule, or None; adam: the checked Adam parameters, or None)."""
+        (prune: the checked schedule, or None; adam: the checked Adam parameters, or None; huber: the checked Huber delta,
+        or None)."""
         a = operator
         if a.layout == torch.sparse_coo:
             if a.dim() != 2 or a.dense_dim() != 0:
@@ -518,6 +547,8 @@ class DefenseGANBase(object):
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
         kw = {} if adam is None else {"adam": adam}
+        if huber is not None:
+            kw["huber_delta"] = huber
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
@@ -550,10 +581,10 @@ class DefenseGANBase(object):
 
     def rec_cache_dir(self, split: str, max_num: int = -1) -> str:
         """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]
-        [_adam{b1:g}-{b2:g}-{eps:g}]/<split>[_debug]` - the directory name the callers parse back with
+        [_adam{b1:g}-{b2:g}-{eps:g}][_huber{delta:g}]/<split>[_debug]` - the directory name the callers parse back with
         `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the `_prune` part (only with `rec_prune` set) keeps pruned
-        and unpruned reconstructions apart, and the `_adam` part (only with rec_optimizer "adam") Adam's from
-        momentum's."""
+        and unpruned reconstructions apart, the `_adam` part (only with rec_optimizer "adam") Adam's from momentum's, and
+        the `_huber` part (only with rec_huber_delta set) the Huber loss's from the squared error's."""
         if max_num > 0:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}_num{:d}'.format(int(self.rec_rr), float(self.rec_lr),
                                                                    int(self.rec_iters), int(max_num))
@@ -564,6 +595,9 @@ class DefenseGANBase(object):
         adam = self._adam_params()
         if adam is not None:
             name += '_adam{:g}-{:g}-{:g}'.format(*adam)
+        huber = self._huber_delta()
+        if huber is not None:
+            name += '_huber{:g}'.format(huber)
         out = os.path.join(self.checkpoint_dir, name, split)
         if self.debug:
             out += '_debug'

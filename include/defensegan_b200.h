@@ -339,6 +339,56 @@ int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* par
                                        const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                        size_t ws_bytes, void* stream);
 
+/* The projection with a Huber data term instead of the squared error (an extension: the reference's loss is the squared
+ * error only).  A few badly wrong pixels or measurements - impulse noise, dead pixels, occluders whose place is not known,
+ * corrupted measurements - then pull G(z) much less far from the point that fits the rest.
+ * For a residual d in fp32 (d = y - x per pixel on the image loss, r = (A G(z))_j - y_j per measurement on the measured
+ * loss) and huber_delta = delta > 0 (+inf allowed):
+ *   c = |d| > delta ? copysign(delta, d) : d      (psi_delta(d); NaN passes through)
+ *   e = w c (weighted image loss; e = c without weights)
+ *   term = e (2 d - c)                             (= w rho_delta(d): d^2 for |d| <= delta, 2 delta |d| - delta^2 beyond)
+ *   d(pre) = e act'(y) on the image loss (times the fp16 path's fixed gradient scale, as in dgan_reconstruct);
+ *   the measured loss stores c as the residual, so the adjoint product gives (2/m) A^T psi(r).
+ * The row loss is (1/HWC) sum_p w_p rho_delta(d_p) on the image loss and (1/m) sum_j rho_delta(r_j) on the measured loss:
+ * the normalisers of the squared error, so rho = 2 torch.nn.functional.huber_loss(..., delta, reduction='none').  When no
+ * residual exceeds delta, c == d and 2 d - c == d exactly, so every stored value, and the whole call, has the bits of
+ * its squared-error counterpart: always at delta = +inf, and on the image loss at any delta >= 2 when the images lie in
+ * the generator's output range (|y - x| < 2).  |c| <= |d|, so the fp16 path's fixed d(pre) scale saturates nowhere it
+ * did not before.  The Huber loss is what loss_dev, the arg-min select, ties, the NaN rule and the prune ranking use;
+ * z0, the momentum or Adam update, decay_lr, the pre-update forward of iteration L-1 and BatchNorm are unchanged.
+ * With momentum the gradient of a clipped residual shrinks with delta, so rec_lr has to grow as delta falls; Adam is
+ * invariant to the gradient's scale and needs no re-tuning.
+ * Each entry runs its counterpart's code path with delta as one argument more: adam NULL selects the momentum update,
+ * otherwise the Adam update of dgan_reconstruct_adam; sched NULL with n_points 0 runs unpruned, any other schedule follows
+ * the rules of dgan_reconstruct_pruned (BatchNorm runs unpruned only; with a schedule: DGAN_ERR_UNSUPPORTED).  So
+ * dgan_reconstruct_huber's counterpart is dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted, dgan_reconstruct_pruned
+ * or dgan_reconstruct_adam.  Workspace: the counterpart's sizer, unchanged (dgan_workspace_bytes[_weighted | _pruned], or
+ * dgan_workspace_bytes_adam when adam is not NULL).  dgan_last_launch_count and dgan_last_enqueue_count equal the
+ * counterpart's; the graph cache keys on delta too.  A delta that is NaN, 0 or negative: DGAN_ERR_INVALID_ARG, after
+ * the counterpart's other checks and before anything is enqueued. */
+int dgan_reconstruct_huber(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam, float huber_delta,
+                           const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                           const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                           void* stream);
+
+/* dgan_reconstruct_measured (dgan_reconstruct_measured_pruned with a schedule, dgan_reconstruct_measured_adam with adam)
+ * with the Huber loss of dgan_reconstruct_huber on the measurement residuals.  Workspace: the counterpart's
+ * (dgan_workspace_bytes_measured[_pruned], or dgan_workspace_bytes_measured_adam with nnz = -1). */
+int dgan_reconstruct_measured_huber(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                    float huber_delta, const dgan_prune_point* sched, int n_points, const float* a_dev, int m,
+                                    const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                    int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* The same with the CSR operator of dgan_reconstruct_measured_csr.  With DGAN_PREC_FP32 every output is bit-identical to
+ * dgan_reconstruct_measured_huber's on the dense matrix the CSR represents.  Workspace: the counterpart's
+ * (dgan_workspace_bytes_measured_csr, dgan_workspace_bytes_measured_pruned or dgan_workspace_bytes_measured_adam with this
+ * nnz). */
+int dgan_reconstruct_measured_csr_huber(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                        float huber_delta, const dgan_prune_point* sched, int n_points,
+                                        const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                        const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                        int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
 /* The z_hat initialiser alone (models/gan.py:370-377): z_dev [n_rows, latent] ~ N(0, 1/latent), rows
  * [z_row_offset, z_row_offset + n_rows) of the Philox stream keyed by `seed` - exactly what dgan_reconstruct
  * draws when z0_dev == NULL. */
@@ -360,6 +410,22 @@ int dgan_loss_grad(dgan_handle h, const float* x_dev, int batch, int rec_rr, con
 int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr,
                             const float* z_dev, float* y_dev, float* loss_dev, float* grad_dev, void* workspace,
                             size_t workspace_bytes, void* stream);
+
+/* dgan_loss_grad (w_dev NULL) or dgan_loss_grad_weighted with the Huber loss of dgan_reconstruct_huber at huber_delta.
+ * Workspace: the counterpart's.  A bad delta: DGAN_ERR_INVALID_ARG after the counterpart's other checks. */
+int dgan_loss_grad_huber(dgan_handle h, float huber_delta, const float* x_dev, const float* w_dev, int batch, int rec_rr,
+                         const float* z_dev, float* y_dev, float* loss_dev, float* grad_dev, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
+/* dgan_loss_grad_measured and dgan_loss_grad_measured_csr with the Huber loss of dgan_reconstruct_huber at huber_delta.
+ * Workspace: the counterpart's.  A bad delta: DGAN_ERR_INVALID_ARG after the counterpart's other checks. */
+int dgan_loss_grad_measured_huber(dgan_handle h, float huber_delta, const float* a_dev, int m, const float* y_dev, int batch,
+                                  int rec_rr, const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const int32_t* row_ptr, const int32_t* col_idx,
+                                      const float* val, int m, int nnz, const float* y_dev, int batch, int rec_rr,
+                                      const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* workspace,
+                                      size_t workspace_bytes, void* stream);
 
 /* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
  *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
@@ -389,12 +455,14 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * 5 + 6 (L - 1) + 1 and 5 + 3 (L - 1) + 1 more; a dgan_reconstruct_pruned call with P prune points 3 P + 1 more, and a
  * dgan_reconstruct_measured[_csr]_pruned call 3 P + 1 more than the unpruned measured call with the same operator kind.
  * An Adam call (dgan_reconstruct_adam, dgan_reconstruct_measured[_csr]_adam) runs as many as its momentum counterpart,
- * plus L - 1 on the DGAN_PREC_FP16 image loss, whose Adam update is a kernel of its own. */
+ * plus L - 1 on the DGAN_PREC_FP16 image loss, whose Adam update is a kernel of its own.  A Huber call
+ * (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber) runs as many as its squared-error counterpart. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
  * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
- * nnz, prune schedule and optimiser: momentum, or Adam with its beta1, beta2 and eps) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * nnz, prune schedule, optimiser: momentum, or Adam with its beta1, beta2 and eps, and data term: the squared error, or
+ * the Huber loss with its delta) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
  * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them),
  * graph, loss sum, arg-min select. */
 int64_t dgan_last_enqueue_count(dgan_handle h);

@@ -57,6 +57,14 @@ if dataset != "celeba":
                   (16, "final-sigmoid"): 287296.0 * rows, (64, "mask"): 287296.0 * rows}
 NT = [256, 128, 64, 48, 16]
 EP = ["bias+relu", "bias", "mask", "none", "final-sigmoid", "final-tanh", "float-out", "?"]
+# keys 40 - 43: the Huber final kinds (tc2_probe_key)
+HUBER = [(16, "final-sigmoid-huber"), (48, "final-tanh-huber"), (16, "final-sigmoid-huber-w"), (48, "final-tanh-huber-w")]
+
+
+def kind(k):
+    return HUBER[k - 40] if k >= 40 else (NT[k // 8], EP[k % 8])
+
+
 raw = np.frombuffer(buf, dtype=np.uint64).reshape(48, 160, W)
 print("kernel <N, epilogue> | launches | cycles from PDL wait to CTA end: mean / min / max over CTAs | (max-mean)/max | trigger->wait mean | MMA operand wait mean (leaders) | set-up cycles mean | last launch, ns from its first CTA entry: last entry / first operands (mean, leaders) / first CTA end / last CTA end")
 timeline, split = [], {}
@@ -73,19 +81,19 @@ for k in range(48):
     g0 = raw[k, act, 5].astype(np.int64); g1 = raw[k, act, 6].astype(np.int64); gf = raw[k, act, 7].astype(np.int64)
     t0 = g0.min()
     print("<%d, %s> | %d | %.0f / %.0f / %.0f | %.3f | %.0f | %.0f | %.0f | %d / %.0f / %d / %d   [abs first entry %d, last end %d]" % (
-        NT[k // 8], EP[k % 8], int(cnt[act].max()), dur.mean(), dur.min(), dur.max(), (dur.max() - dur.mean()) / dur.max(), pre.mean(),
+        *kind(k), int(cnt[act].max()), dur.mean(), dur.min(), dur.max(), (dur.max() - dur.mean()) / dur.max(), pre.mean(),
         wf[lead].mean() if lead.any() else 0, setup.mean(), g0.max() - t0, (gf[gf > 0] - t0).mean() if (gf > 0).any() else -1, g1.min() - t0, g1.max() - t0, t0, g1.max()))
     # the first consumer warp of each CTA (thread 0): shares of its busy cycles, means over CTAs
     sh = [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (3, 8, 9, 10, 11, 12, 13, 14)]
     steps = a[k, act, 15]
     sh += [float((steps / cnt[act]).mean()), float((a[k, act, 12][steps > 0] / steps[steps > 0]).mean()) if (steps > 0).any() else 0.0]
     sh += [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (16, 17)]
-    split[layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8]))] = dict(
+    split[layer_names.get(kind(k), "<%d, %s>" % kind(k))] = dict(
         zip(("operand_wait", "issue", "wgmma_wait1", "wgmma_wait0", "epilogue", "record_wait", "item_head", "end_wait",
              "steps_per_cta", "record_wait_cycles_per_step", "epilogue_input_wait", "epilogue_staging_wait"),
             [round(v, 3) for v in sh]))
-    timeline.append((int(t0), layer_names.get((NT[k // 8], EP[k % 8]), "<%d, %s>" % (NT[k // 8], EP[k % 8])), int(g0.max()), float(gf[gf > 0].mean()) if (gf > 0).any() else float(g0.max()),
-                     int(g1.max()), 2.0 * kind_flops.get((NT[k // 8], EP[k % 8]), 0.0)))
+    timeline.append((int(t0), layer_names.get(kind(k), "<%d, %s>" % kind(k)), int(g0.max()), float(gf[gf > 0].mean()) if (gf > 0).any() else float(g0.max()),
+                     int(g1.max()), 2.0 * kind_flops.get(kind(k), 0.0)))
 # the last launches of the kernels, in time order: how long each was busy and what the hand-over from its predecessor cost
 timeline.sort()
 print()
