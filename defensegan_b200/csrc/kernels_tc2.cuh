@@ -172,6 +172,16 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// Four 8x8 fp16 matrices from the m64nNk16 accumulator fragment into shared memory: lane L names a row of matrix L / 8.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+// prmt.b32 (default mode): selector nibble n picks byte n & 7 of {b, a}; with bit 3 set, that byte's sign fills the byte
+__device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
+  uint32_t r;
+  asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
+  return r;
+}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -336,8 +346,11 @@ __device__ __forceinline__ void tc2_pop_round(uint32_t (&q)[6]) {
 // epilogue, or the PDL wait, -> the first step's operand wait), [14] end wait (end of the last epilogue -> every warp of
 // the CTA has finished, the producer's drain included).  [15] steps the CTA ran.  Inside the epilogues [11]: [16] waiting
 // for the epilogue's global inputs (mask words, bias, image and weight pairs: from the point a unit or accumulator needs
-// them to their arrival), [17] waiting for a staging buffer of the TMA store (bulk_wait_read1).
-constexpr int TC2_PROBE_WORDS = 18;
+// them to their arrival), [17] waiting for a staging buffer of the TMA store (bulk_wait_read1).  Inside the TMA-store
+// epilogues, per 64-column unit: [18] the register work (bias, ReLU or mask, fp16 conversion, and in the ReLU kinds the
+// mask words: packing, combining across the quad, storing), [19] writing the staging buffer, [20] the
+// fence.proxy.async before the TMA store.
+constexpr int TC2_PROBE_WORDS = 21;
 __device__ unsigned long long g_tc2_probe[48][160][TC2_PROBE_WORDS];
 __device__ __forceinline__ unsigned long long probe_gtime() {
   unsigned long long t;
@@ -393,6 +406,7 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   const long long probe_t_start = clock64();
   const unsigned long long probe_g_start = probe_gtime();
   long long probe_wait_full = 0, probe_issue = 0, probe_wait1 = 0, probe_wait0 = 0, probe_epi = 0, probe_in = 0, probe_stage = 0;
+  long long probe_regs = 0, probe_sts = 0, probe_fence = 0;
   unsigned probe_rec = 0, probe_head = 0, probe_steps = 0;     // 32-bit cycle counts: a launch is far shorter than 2^32 cycles
 #endif
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -775,7 +789,14 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         const int GT = fa.out_ld >> 6;                 // 64-column groups per output row (mask words)
         const int row_w = tile_row0 + wg * 64 + wl * 16;
         const uint32_t s_warp = epi_base + (uint32_t)warp * 4096u;
-        const uint32_t swz = (uint32_t)(lane >> 2);
+        const uint32_t l2 = 2u * (uint32_t)(lane & 3);  // this lane's first column in each 8-column chunk
+        // stmatrix: lane L gives the address of row L % 8 of 8x8 matrix L / 8, and matrix m of store p is the chunk
+        // (row half h = m % 2, column chunk j = 2p + m / 2) of the 128B-swizzled slice, chunk j of row r at (j ^ r) * 16
+        const uint32_t sm_row = (uint32_t)(lane & 7) + 8u * (uint32_t)((lane >> 3) & 1);
+        const uint32_t sm_x = (((uint32_t)(lane >> 4) ^ (uint32_t)(lane & 7)) << 4);
+        // EPI_BIAS_RELU: lane k of a quad ends a unit holding 32-bit half k % 2 of row r_lo + 8 (k / 2)'s mask word; the
+        // words are stored after the item's last TMA store, so that no global store precedes a fence.proxy.async.
+        uint32_t mw[Cfg::MAXB * G];
 #pragma unroll
         for (int a = 0; a < Cfg::MAXB; ++a) {
           if (a >= n_acc) break;
@@ -783,17 +804,29 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #pragma unroll
           for (int g = 0; g < G; ++g) {
 #ifdef DGAN_PROBE
-            const long long probe_u0 = clock64();
+            const long long probe_u0 = clock64(), probe_in0 = probe_in;
 #endif
-            unsigned long long mk[2] = {~0ull, ~0ull}, bits[2] = {0ull, 0ull};
-            if (EPI == EPI_MASK) {
+            // EPI_MASK: the unit's bits of this lane, bit 8j + c of row h's word in column 8j + l2 + c, placed as the
+            // sign bits of bytes (c = 0: keep7, c = 1: keep6; 32-bit halves lo: j < 4, hi: j >= 4)
+            uint32_t keep7[2][2], keep6[2][2];
+            if constexpr (EPI == EPI_MASK) {
+              unsigned long long mk[2];
 #pragma unroll
               for (int h = 0; h < 2; ++h) mk[h] = __shfl_sync(0xffffffffu, mk_pre[h], (lane & ~3) | (a * G + g));
 #ifdef DGAN_PROBE
               probe_in += probe_clock_after64(mk[0] ^ mk[1]) - probe_u0;
 #endif
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int hi = 0; hi < 2; ++hi) {
+                  const uint32_t w = (uint32_t)(mk[h] >> (32 * hi));
+                  keep7[h][hi] = w << (7u - l2);
+                  keep6[h][hi] = w << (6u - l2);
+                }
             }
             uint32_t pk[2][8];
+            uint32_t bits[2][2] = {{0u, 0u}, {0u, 0u}};     // EPI_BIAS_RELU: [row half][32-bit half], lane's bits at 8j + c
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
               const int cl = j * 8 + (lane & 3) * 2;   // column within the 64-column group
@@ -815,46 +848,74 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
                 float v1 = acc[a * (N_TILE / 2) + (g * 8 + j) * 4 + h * 2 + 1];
                 if (HAS_BIAS) { v0 += bv.x; v1 += bv.y; }
                 if (EPI == EPI_BIAS_RELU) {
+                  // the mask bit is (value after ReLU > 0), i.e. v > 0 (false for NaN and -0, which fmaxf makes 0); a
+                  // predicated add of the bit at a compile-time position, shifted to this lane's columns once per unit
+                  const uint32_t b = 8u * (uint32_t)(j & 3);
+                  if (v0 > 0.f) bits[h][j >> 2] |= 1u << b;
+                  if (v1 > 0.f) bits[h][j >> 2] |= 2u << b;
                   v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
-                  bits[h] |= ((unsigned long long)(v0 > 0.f) << cl) | ((unsigned long long)(v1 > 0.f) << (cl + 1));
-                }
-                if (EPI == EPI_MASK) {
-                  if (!((mk[h] >> cl) & 1ull)) v0 = 0.f;
-                  if (!((mk[h] >> (cl + 1)) & 1ull)) v1 = 0.f;
                 }
                 pk[h][j] = pack_half2(v0, v1);
+                // a masked-out value becomes +0
+                if (EPI == EPI_MASK) pk[h][j] &= ptx::prmt(keep7[h][j >> 2], keep6[h][j >> 2], 0xCC88u + 0x1111u * (uint32_t)(j & 3));
               }
+            }
+            if constexpr (EPI == EPI_BIAS_RELU) {
+              // the quad's words: lane k keeps row half k / 2 (exchange with lane k ^ 2), then 32-bit half k % 2 (k ^ 1)
+              const bool up = (lane & 2) != 0, odd = (lane & 1) != 0;
+              uint32_t k0 = (up ? bits[1][0] : bits[0][0]) << l2, k1 = (up ? bits[1][1] : bits[0][1]) << l2;
+              const uint32_t s0 = (up ? bits[0][0] : bits[1][0]) << l2, s1 = (up ? bits[0][1] : bits[1][1]) << l2;
+              k0 |= __shfl_xor_sync(0xffffffffu, s0, 2);
+              k1 |= __shfl_xor_sync(0xffffffffu, s1, 2);
+              mw[a * G + g] = (odd ? k1 : k0) | __shfl_xor_sync(0xffffffffu, odd ? k0 : k1, 1);
             }
             const uint32_t buf = s_warp + (store_count & 1u) * 2048u;
 #ifdef DGAN_PROBE
-            const long long probe_s0 = clock64();
+            const long long probe_s0 = probe_clock_after64((((unsigned long long)pk[0][7] << 32) | pk[1][7]) ^
+                                                           (EPI == EPI_BIAS_RELU ? mw[a * G + g] : 0u));
+            probe_regs += probe_s0 - probe_u0 - (probe_in - probe_in0);
 #endif
             if (lane == 0) ptx::bulk_wait_read1();     // the store that used this buffer two units ago has read it
             __syncwarp();
 #ifdef DGAN_PROBE
-            probe_stage += clock64() - probe_s0;
+            const long long probe_s1 = clock64();
+            probe_stage += probe_s1 - probe_s0;
 #endif
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                ptx::st_shared_u32(buf + (swz + 8u * h) * 128u + (((uint32_t)j ^ swz) << 4) + (uint32_t)(lane & 3) * 4u, pk[h][j]);
+            for (int p = 0; p < 4; ++p)
+              ptx::stmatrix_x4(buf + sm_row * 128u + ((32u * (uint32_t)p) ^ sm_x), pk[0][2 * p], pk[1][2 * p], pk[0][2 * p + 1], pk[1][2 * p + 1]);
+#ifdef DGAN_PROBE
+            const long long probe_f0 = clock64();
+            probe_sts += probe_f0 - probe_s1;
+#endif
             ptx::fence_proxy_async_smem();
+#ifdef DGAN_PROBE
+            probe_fence += clock64() - probe_f0;
+#endif
             __syncwarp();
             if (lane == 0) {
               ptx::tma_store_3d(&tm_out, buf, fa.col0 + g * 64, row_w, q);
               ptx::bulk_commit();
             }
             ++store_count;
-            if (EPI == EPI_BIAS_RELU && fa.mb_out != nullptr) {
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 1);
-                bits[h] |= __shfl_xor_sync(0xffffffffu, bits[h], 2);
-              }
-              if ((lane & 3) < 2) fa.mb_out[((size_t)q * n_pad + n_lo + 8 * (lane & 1)) * GT + g] = (lane & 1) ? bits[1] : bits[0];
-            }
           }
+        }
+        if (EPI == EPI_BIAS_RELU && fa.mb_out != nullptr) {
+#ifdef DGAN_PROBE
+          const long long probe_m0 = clock64();
+#endif
+          uint32_t* __restrict__ mb32 = reinterpret_cast<uint32_t*>(fa.mb_out);
+          const size_t row = n_lo + 8 * ((lane >> 1) & 1);
+#pragma unroll
+          for (int a = 0; a < Cfg::MAXB; ++a) {
+            if (a >= n_acc) break;
+            const int q = q_of(a);
+#pragma unroll
+            for (int g = 0; g < G; ++g) mb32[(((size_t)q * n_pad + row) * GT + g) * 2 + (lane & 1)] = mw[a * G + g];
+          }
+#ifdef DGAN_PROBE
+          probe_regs += clock64() - probe_m0;
+#endif
         }
       } else {
         // fp32 outputs (BatchNorm pre-activations, the Linear backward's partial sums): straight from the registers
@@ -956,6 +1017,9 @@ tc_bsgemm2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       atomicAdd(&g_tc2_probe[key][blockIdx.x][11], (unsigned long long)probe_epi);
       atomicAdd(&g_tc2_probe[key][blockIdx.x][16], (unsigned long long)probe_in);
       atomicAdd(&g_tc2_probe[key][blockIdx.x][17], (unsigned long long)probe_stage);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][18], (unsigned long long)probe_regs);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][19], (unsigned long long)probe_sts);
+      atomicAdd(&g_tc2_probe[key][blockIdx.x][20], (unsigned long long)probe_fence);
     }
     __syncthreads();
     if (threadIdx.x == 0) {

@@ -7,7 +7,8 @@ into the record wait (operands landed -> the step's MMA record read and first us
 -> the next item's first operand wait), the end wait (last epilogue -> every warp of the CTA done) and the remainder;
 with the steps per CTA and launch, and the record wait in cycles per step.  The epilogue's share is split further into
 waiting for its global inputs (mask words, bias, image and weight pairs), waiting for a staging buffer of the TMA store,
-and the rest of it.
+and the rest of it; in the TMA-store epilogues that rest splits into the register work of each 64-column unit (bias, ReLU
+or mask, fp16 conversion, the ReLU mask words), writing its staging buffer, and the fence.proxy.async before its store.
 Usage: DGAN_LIB=build_ab/probe.so python tools/probe_step.py [mnist|celeba] [batch] [L] [--json]
 (--json: one JSON object with the time-ordered busy / hand-over table instead of the text tables; bench.py uses it)"""
 import ctypes
@@ -36,7 +37,7 @@ lib = gan._native.lib if hasattr(gan, "_native") and gan._native is not None els
 gan.reconstruct(x, z_init_val=z0)
 torch.cuda.synchronize()
 lib = gan._native.lib
-W = 18                                              # counters per CTA (TC2_PROBE_WORDS)
+W = 21                                              # counters per CTA (TC2_PROBE_WORDS)
 buf = (ctypes.c_ulonglong * (48 * 160 * W))()
 lib.dgan_debug_probe_read.restype = ctypes.c_int
 lib.dgan_debug_probe_read.argtypes = [ctypes.POINTER(ctypes.c_ulonglong)]
@@ -87,10 +88,11 @@ for k in range(48):
     sh = [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (3, 8, 9, 10, 11, 12, 13, 14)]
     steps = a[k, act, 15]
     sh += [float((steps / cnt[act]).mean()), float((a[k, act, 12][steps > 0] / steps[steps > 0]).mean()) if (steps > 0).any() else 0.0]
-    sh += [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (16, 17)]
+    sh += [float((a[k, act, c] / a[k, act, 0]).mean()) for c in (16, 17, 18, 19, 20)]
     split[layer_names.get(kind(k), "<%d, %s>" % kind(k))] = dict(
         zip(("operand_wait", "issue", "wgmma_wait1", "wgmma_wait0", "epilogue", "record_wait", "item_head", "end_wait",
-             "steps_per_cta", "record_wait_cycles_per_step", "epilogue_input_wait", "epilogue_staging_wait"),
+             "steps_per_cta", "record_wait_cycles_per_step", "epilogue_input_wait", "epilogue_staging_wait",
+             "epilogue_registers", "epilogue_staging_stores", "epilogue_fence"),
             [round(v, 3) for v in sh]))
     timeline.append((int(t0), layer_names.get(kind(k), "<%d, %s>" % kind(k)), int(g0.max()), float(gf[gf > 0].mean()) if (gf > 0).any() else float(g0.max()),
                      int(g1.max()), 2.0 * kind_flops.get(kind(k), 0.0)))
@@ -112,13 +114,15 @@ print("sum | %.1f | %.1f |" % (tot_busy, tot_gap))
 print()
 print("first consumer warp, share of its busy cycles | operand wait | MMA issue | wgmma_wait1 | wgmma_wait0 | epilogue | rest"
       " | of rest: record wait | item head | end wait | remainder | steps per CTA | record wait, cycles per step"
-      " | of epilogue: input wait | staging wait | rest")
+      " | of epilogue: input wait | staging wait | rest | of rest (TMA-store epilogues): register work | staging stores"
+      " | fence | remainder")
 for name, d in split.items():
     v = list(d.values())
     rest = 1.0 - sum(v[:5])
-    print("%s | %s | %.3f | %s | %.3f | %.1f | %.0f | %.3f | %.3f | %.3f" % (
+    e_rest = v[4] - v[10] - v[11]
+    print("%s | %s | %.3f | %s | %.3f | %.1f | %.0f | %.3f | %.3f | %.3f | %.3f | %.3f | %.3f | %.3f" % (
         name, " | ".join("%.3f" % x for x in v[:5]), rest, " | ".join("%.3f" % x for x in v[5:8]), rest - sum(v[5:8]), v[8], v[9],
-        v[10], v[11], v[4] - v[10] - v[11]))
+        v[10], v[11], e_rest, v[12], v[13], v[14], e_rest - sum(v[12:15])))
 if as_json:
     import json
     rows_out, prev_end = [], None
