@@ -16,6 +16,8 @@ import torch
 import torch.autograd.forward_ad as fwAD
 from torch.autograd.function import once_differentiable
 
+from .operators import ConvOperator
+
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 LIB_NAME = "libdefensegan_b200.so"
 LIB_PATH = os.environ.get("DGAN_LIB", os.path.join(_PKG_DIR, LIB_NAME))   # DGAN_LIB: A/B-test another build
@@ -45,6 +47,7 @@ ABI_SYMBOLS = [
     "dgan_reconstruct_measured_csr_adam",
     "dgan_reconstruct_huber", "dgan_reconstruct_measured_huber", "dgan_reconstruct_measured_csr_huber",
     "dgan_loss_grad_huber", "dgan_loss_grad_measured_huber", "dgan_loss_grad_measured_csr_huber",
+    "dgan_conv_op_m", "dgan_workspace_bytes_measured_conv", "dgan_reconstruct_measured_conv", "dgan_loss_grad_measured_conv",
 ]
 
 
@@ -65,6 +68,11 @@ class dgan_prune_point(ctypes.Structure):
 
 class dgan_adam_params(ctypes.Structure):
     _fields_ = [("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float)]
+
+
+class dgan_conv_op(ctypes.Structure):
+    _fields_ = [("kh", ctypes.c_int32), ("kw", ctypes.c_int32), ("pad_h", ctypes.c_int32), ("pad_w", ctypes.c_int32),
+                ("stride", ctypes.c_int32)]
 
 
 ABI_VERSION = 2
@@ -276,6 +284,16 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_loss_grad_measured_csr_huber.restype = i32
     lib.dgan_loss_grad_measured_csr_huber.argtypes = [vp, f32, vp, vp, vp, i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.restype = i32
+    cp, fp = ctypes.POINTER(dgan_conv_op), ctypes.POINTER(ctypes.c_float)
+    lib.dgan_conv_op_m.restype = i32
+    lib.dgan_conv_op_m.argtypes = [vp, cp]
+    lib.dgan_workspace_bytes_measured_conv.restype = sz
+    lib.dgan_workspace_bytes_measured_conv.argtypes = [vp, i32, i32, cp, pp, i32, i32]
+    lib.dgan_reconstruct_measured_conv.restype = i32
+    lib.dgan_reconstruct_measured_conv.argtypes = [vp, ctypes.POINTER(dgan_rec_params), ap, fp, pp, i32, cp, vp, vp, vp, vp,
+                                                   vp, vp, vp, sz, vp]
+    lib.dgan_loss_grad_measured_conv.restype = i32
+    lib.dgan_loss_grad_measured_conv.argtypes = [vp, fp, cp, vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
     lib.dgan_forward.argtypes = [vp, vp, i32, vp, vp, sz, vp]
@@ -391,8 +409,11 @@ class NativeGenerator:
 
     # -- helpers -------------------------------------------------------------------------
     def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None,
-                   adam: bool = False):
-        if adam and m > 0:
+                   adam: bool = False, conv: Optional[dgan_conv_op] = None):
+        if conv is not None:
+            need = int(self.lib.dgan_workspace_bytes_measured_conv(self._handle, batch, rec_rr, ctypes.byref(conv), sched,
+                                                                   len(sched) if sched is not None else 0, int(adam)))
+        elif adam and m > 0:
             need = int(self.lib.dgan_workspace_bytes_measured_adam(self._handle, batch, rec_rr, int(m), int(nnz), sched,
                                                                    len(sched) if sched is not None else 0))
         elif adam:
@@ -578,6 +599,56 @@ class NativeGenerator:
                _require_cuda_f32(val, "operator.values()"), nnz)
         return y, csr, y.shape[0], m
 
+    def _measured_conv(self, measurements: torch.Tensor, operator):
+        """(y, kernels, op, batch, m) for a ConvOperator: the measurements as a contiguous CUDA float32 [batch, m] tensor,
+        the kernels broadcast to [batch, kh, kw] on the GPU and the geometry as a dgan_conv_op (shapes only; the values
+        are not checked here - DefenseGANBase.reconstruct_measured does)."""
+        m = operator.num_measurements(self.image_dim)
+        y = _require_cuda_f32(measurements, "measurements")
+        if y.dim() != 2 or y.shape[1] != m or y.shape[0] <= 0:
+            raise ValueError("measurements must be [B, %d] (the operator's m), got %s" % (m, tuple(y.shape)))
+        batch = y.shape[0]
+        k = _require_cuda_f32(operator.kernels(batch, y.device), "operator kernels")
+        kh, kw = operator.kernel_size
+        op = dgan_conv_op(kh, kw, operator.padding[0], operator.padding[1], operator.stride)
+        return y, k, op, batch, m
+
+    def _reconstruct_measured_conv(self, measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed, momentum,
+                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta):
+        """reconstruct_measured for a ConvOperator (dgan_reconstruct_measured_conv)."""
+        y, k, op, batch, m = self._measured_conv(measurements, operator)
+        if rec_rr <= 0 or rec_iters <= 0:
+            raise ValueError("rec_rr and rec_iters must be positive")
+        sched = self._schedule(prune, rec_rr, rec_iters)
+        ap = self._adam(adam)
+        delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
+        z0 = None
+        if z_init_val is not None:
+            z0 = _require_cuda_f32(z_init_val, "z_init_val")
+            if z0.numel() != batch * rec_rr * self.latent_dim:
+                raise ValueError("z_init_val must be [B*rec_rr, latent_dim]")
+        with torch.cuda.device(self.device):
+            rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
+            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
+                raise ValueError("out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements" % self.image_dim)
+            _require_aligned_out(rec)
+            loss = torch.empty(batch, dtype=torch.float32, device=self.device)
+            idx = torch.empty(batch, dtype=torch.int32, device=self.device)
+            ws, need = self._workspace(batch, rec_rr, sched=sched, adam=ap is not None, conv=op)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
+                                  seed & (2 ** 64 - 1), int(z_row_offset))
+            rc = self.lib.dgan_reconstruct_measured_conv(self._handle, ctypes.byref(prm),
+                                                         ctypes.byref(ap) if ap is not None else None,
+                                                         ctypes.byref(delta) if delta is not None else None, sched,
+                                                         len(sched) if sched is not None else 0, ctypes.byref(op), _ptr(k),
+                                                         _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                         ctypes.c_void_p(stream))
+            _check(self.lib, rc, "dgan_reconstruct_measured_conv")
+        if return_aux:
+            return rec, loss, idx
+        return rec
+
     def reconstruct_measured(self, measurements: torch.Tensor, operator: torch.Tensor, rec_rr: int, rec_iters: int,
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
@@ -597,7 +668,13 @@ class NativeGenerator:
         dgan_reconstruct_measured_csr_adam for a CSR operator), with or without prune.
         huber_delta: the Huber loss of reconstruct on the measurement residuals, (1/m) sum_j rho_delta(r_j)
         (dgan_reconstruct_measured_huber, or dgan_reconstruct_measured_csr_huber for a CSR operator), with any of prune
-        and adam.  None runs the squared error as before."""
+        and adam.  None runs the squared error as before.
+        A defensegan_b200.operators.ConvOperator runs dgan_reconstruct_measured_conv: a convolution with one kernel per
+        image (a shared kernel is passed as B copies), applied as a stencil, with any of prune, adam and huber_delta."""
+        if isinstance(operator, ConvOperator):
+            return self._reconstruct_measured_conv(measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed,
+                                                   momentum, decay_lr, out, return_aux, z_row_offset, prune, adam,
+                                                   huber_delta)
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -677,7 +754,10 @@ class NativeGenerator:
         """(G(z), per-row measured loss, d(sum loss)/dz) at z [B*rec_rr, latent] for measurements [B, m] through operator
         [m, H*W*C]: one evaluation of reconstruct_measured's loop body (dgan_loss_grad_measured, or
         dgan_loss_grad_measured_csr for a torch sparse CSR operator).  huber_delta: with the Huber loss of
-        reconstruct_measured (dgan_loss_grad_measured[_csr]_huber); None: the squared error."""
+        reconstruct_measured (dgan_loss_grad_measured[_csr]_huber); None: the squared error.  A ConvOperator runs
+        dgan_loss_grad_measured_conv."""
+        if isinstance(operator, ConvOperator):
+            return self._loss_grad_measured_conv(measurements, operator, z, rec_rr, huber_delta)
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -714,6 +794,28 @@ class NativeGenerator:
                 _check(self.lib, self.lib.dgan_loss_grad_measured(self._handle, _ptr(a), m, _ptr(y), batch, rec_rr,
                                                                   _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
                                                                   ctypes.c_void_p(stream)), "dgan_loss_grad_measured")
+        return g, loss, grad
+
+    def _loss_grad_measured_conv(self, measurements, operator, z, rec_rr, huber_delta):
+        """loss_grad_measured for a ConvOperator (dgan_loss_grad_measured_conv)."""
+        y, k, op, batch, m = self._measured_conv(measurements, operator)
+        zc = _require_cuda_f32(z, "z")
+        n = batch * rec_rr
+        if zc.shape[0] != n:
+            raise ValueError("z must have batch*rec_rr rows")
+        delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
+        with torch.cuda.device(self.device):
+            g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
+            loss = torch.empty(n, dtype=torch.float32, device=self.device)
+            grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
+            ws, need = self._workspace(batch, rec_rr, conv=op)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _check(self.lib, self.lib.dgan_loss_grad_measured_conv(self._handle,
+                                                                   ctypes.byref(delta) if delta is not None else None,
+                                                                   ctypes.byref(op), _ptr(k), _ptr(y), batch, rec_rr,
+                                                                   _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
+                                                                   ctypes.c_void_p(stream)),
+                   "dgan_loss_grad_measured_conv")
         return g, loss, grad
 
     def sample_z0(self, n_rows: int, seed: int, z_row_offset: int = 0) -> torch.Tensor:

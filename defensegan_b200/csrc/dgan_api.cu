@@ -17,6 +17,7 @@
 #include "kernels_vjp.cuh"
 #include "kernels_measured.cuh"
 #include "kernels_measured_csr.cuh"
+#include "kernels_measured_conv.cuh"
 #include "kernels_prune.cuh"
 #include "kernels_adam.cuh"
 
@@ -324,19 +325,21 @@ struct dgan_ctx {
   // The L-step loop of a projection as a CUDA graph: captured once per (workspace, batch, R, L, lr, momentum, decay,
   // weighted, measured: the m of a measured call, 0 otherwise, csr_nnz: the non-zeros of a CSR operator, -1 otherwise,
   // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise; adam: 1 for the Adam
-  // update with beta1, beta2 and eps, 0 for momentum; huber: the Huber entries' delta, 0 for the squared error) on a
-  // private stream, replayed with one cudaGraphLaunch per call.
+  // update with beta1, beta2 and eps, 0 for momentum; huber: the Huber entries' delta, 0 for the squared error; conv:
+  // a convolution operator's kh, kw, ph, pw and stride, empty otherwise - not its kernel values, which are staged outside
+  // the graph) on a private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     std::vector<int> prune;
     cudaGraphExec_t exec; int64_t kernels;
     int adam = 0; float beta1 = 0.f, beta2 = 0.f, eps = 0.f;
     float huber = 0.f;
+    std::vector<int> conv;
     bool same_key(const LoopGraph& o) const {
       return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
              weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
              momentum == o.momentum && prune == o.prune && adam == o.adam && beta1 == o.beta1 && beta2 == o.beta2 &&
-             eps == o.eps && huber == o.huber;
+             eps == o.eps && huber == o.huber && conv == o.conv;
     }
   };
   std::vector<LoopGraph> graphs;
@@ -458,6 +461,11 @@ struct Workspace {
   int nnz = 0;
   int *a_rp = nullptr, *a_ci = nullptr, *at_rp = nullptr, *at_ci = nullptr, *csr_bad = nullptr, *csr_valid = nullptr;
   float *a_v = nullptr, *at_v = nullptr;
+  // convolution-measured workspaces (conv; kernels_measured_conv.cuh): no am / amt and no CSR; the geometry and the staged
+  // kernels ck [batch][kh][kw], after all the buffers above
+  bool conv = false;
+  ConvGeom cg{};
+  float* ck = nullptr;
   // the regions of a pruned workspace (prune_maps; kernels_prune.cuh), after all the buffers above: each row's original
   // restart index [n_pad] (written by the prune point that fills the region; the first region's rows are restarts
   // 0 .. R-1 of each image and leave it unwritten), the row of the previous region each row was gathered from [n_pad],
@@ -516,14 +524,15 @@ static void carve_csr(const dgan_ctx* c, Workspace* w, int nnz_, char* b, size_t
 // the weights "xw" after all of them.  m > 0: the workspace of the measured entries for m measurements, the same buffers
 // at the same offsets and the measured ones after all of them.
 // csr_nnz >= 0 (with m > 0): the workspace of the CSR-measured entries for nnz non-zeros, the measured buffers without
-// am / amt and the CSR ones after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
+// am / amt and the CSR ones after all of them.  conv (not NULL, with m > 0 and csr_nnz -1): the workspace of the
+// convolution-measured entries, the measured buffers without am / amt and the staged kernels "ck" after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
 // "orig", "src" and "sel" after all the other buffers.  op (not NULL, with m > 0): a region of a pruned measured
 // workspace, whose operator - am / amt or the CSR buffers - and ym live in the operator block op (carve_operator): only
 // the row-sized measured buffers are carved, the others are op's.  adam: the workspace of the Adam entries, the same
 // buffers at the same offsets and the second moment "s" after all of them.
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
                        int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr,
-                       bool adam = false) {
+                       bool adam = false, const ConvGeom* conv = nullptr) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -591,7 +600,8 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.m_ld = measured_ld(m);
     const size_t mld = (size_t)w.m_ld;
     w.csr = csr_nnz >= 0;
-    if (!w.csr && op == nullptr) {
+    w.conv = conv != nullptr;
+    if (!w.csr && !w.conv && op == nullptr) {
       w.am = (float*)take("am", "f32", {mld, hwc});
       w.amt = (float*)take("amt", "f32", {hwc, mld});
     }
@@ -606,8 +616,12 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
       w.a_rp = op->a_rp; w.a_ci = op->a_ci; w.a_v = op->a_v;
       w.at_rp = op->at_rp; w.at_ci = op->at_ci; w.at_v = op->at_v;
       w.csr_bad = op->csr_bad; w.csr_valid = op->csr_valid;
+      w.cg = op->cg; w.ck = op->ck;
     } else if (w.csr) {
       carve_csr(c, &w, csr_nnz, b, &off, layout);
+    } else if (w.conv) {
+      w.cg = *conv;
+      w.ck = (float*)take("ck", "f32", {np, (size_t)conv->kh * conv->kw});      // batch <= n_pad
     }
   }
   if (prune_maps) {
@@ -621,9 +635,10 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
 }
 
 // The operator block of a pruned measured workspace, shared by all its regions: the staged operator - "am" / "amt" as in
-// carve, or (csr_nnz >= 0) carve's CSR buffers - then the measurements "ym" [batch][m_ld].  Only the operator's buffers,
-// m, m_ld, csr and nnz are set.
-static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz, void* base, std::string* layout) {
+// carve, or (csr_nnz >= 0) carve's CSR buffers, or (conv not NULL) the kernels "ck" [batch][kh][kw] - then the
+// measurements "ym" [batch][m_ld].  Only the operator's buffers, m, m_ld, csr, nnz, conv and cg are set.
+static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz, void* base, std::string* layout,
+                                const ConvGeom* conv = nullptr) {
   Workspace w;
   size_t off = 0;
   char* b = (char*)base;
@@ -635,8 +650,12 @@ static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz
   w.m_ld = measured_ld(m);
   const size_t mld = (size_t)w.m_ld;
   w.csr = csr_nnz >= 0;
+  w.conv = conv != nullptr;
   if (w.csr) {
     carve_csr(c, &w, csr_nnz, b, &off, layout);
+  } else if (w.conv) {
+    w.cg = *conv;
+    w.ck = (float*)take("ck", "f32", {(size_t)batch, (size_t)conv->kh * conv->kw});
   } else {
     w.am = (float*)take("am", "f32", {mld, hwc});
     w.amt = (float*)take("amt", "f32", {hwc, mld});
@@ -1147,9 +1166,62 @@ static int launch_measured_csr(dgan_ctx* c, const Workspace& w, const float* X, 
   return 0;
 }
 
+// Dynamic shared memory of a convolution product over the workspace's operator: the kernel's taps and the most operand
+// rows any chunk stages (kernels_measured_conv.cuh).  adjoint: the adjoint product's, else the measurement product's.
+static size_t conv_smem(const dgan_ctx* c, const Workspace& w, bool adjoint) {
+  const ConvGeom& g = w.cg;
+  const int n = adjoint ? c->hwc : w.m_ld, row = adjoint ? g.Wo * g.C : g.W * g.C;
+  int most = 0;
+  for (int x0 = 0; x0 < n; x0 += kConvCols) {
+    int lo, hi;
+    if (adjoint) conv_adj_span(g, x0, std::min(n, x0 + kConvCols), &lo, &hi);
+    else conv_meas_span(g, x0, std::min(std::min(n, x0 + kConvCols), w.m), &lo, &hi);
+    most = std::max(most, hi - lo + 1);
+  }
+  return ((size_t)conv_taps_ld(g) + (size_t)most * row) * sizeof(float);
+}
+
+// Copy a call's kernels k [batch][kh][kw] and measurements y [batch][m] into the convolution-measured workspace w, y
+// padded as stage_measured does: one kernel.  Raises the products' shared-memory limit where a geometry needs more than
+// the default (never lowered: the opt-in limit is per kernel, not per handle).
+static int stage_measured_conv(dgan_ctx* c, const Workspace& w, const float* k, const float* y, int batch, cudaStream_t s) {
+  const size_t meas = conv_smem(c, w, false), adj = conv_smem(c, w, true);
+  cudaFuncAttributes fa;
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_conv_kernel));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < meas)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)meas));
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_conv_huber_kernel));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < meas)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_conv_huber_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)meas));
+  DGAN_CUDA_CHECK(cudaFuncGetAttributes(&fa, measured_conv_adjoint_kernel));
+  if ((size_t)fa.maxDynamicSharedSizeBytes < adj)
+    DGAN_CUDA_CHECK(cudaFuncSetAttribute(measured_conv_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)adj));
+  const int taps = w.cg.kh * w.cg.kw;
+  const size_t n = std::max((size_t)batch * taps, (size_t)batch * w.m_ld);
+  conv_stage_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(k, y, batch, taps, w.m, w.m_ld, w.ck, w.ym);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
+// The measurement product through the staged convolution operator: r = A_{n / R} G(z) - y[n / R] and the loss parts
+// (huber: MEAS_RESID_HUBER at delta = w.huber)
+static int launch_measured_conv(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  const unsigned grid = (unsigned)((size_t)w.n_rows * ((w.m_ld + kConvCols - 1) / kConvCols));
+  const size_t smem = conv_smem(c, w, false);
+  if (w.huber > 0.f)
+    measured_conv_huber_kernel<<<grid, kConvThreads, smem, s>>>(w.y, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R,
+                                                                w.huber, w.mloss_part, w.n_pad);
+  else
+    measured_conv_kernel<<<grid, kConvThreads, smem, s>>>(w.y, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R, 1.f,
+                                                          w.mloss_part, w.n_pad);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
 // The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.  w.huber > 0:
 // the Huber residual psi(r) and the Huber loss's parts (MEAS_RESID_HUBER, delta passed as the scale).
 static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  if (w.conv) return launch_measured_conv(c, w, R, s);
   if (w.huber > 0.f) {
     if (w.csr)
       return launch_measured_csr<MEAS_RESID_HUBER>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld,
@@ -1165,10 +1237,17 @@ static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s
 }
 
 // The rest of a measured step's gradient after launch_measure: dy = (2/m) At r, then the cotangent entry of dgan_vjp (its
-// fp16 row scales in w.mscale: w.loss carries the loss to the select) and the backward-to-z into w.g.
-static int measured_backward(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+// fp16 row scales in w.mscale: w.loss carries the loss to the select) and the backward-to-z into w.g.  R: the rows per
+// image, which pick a convolution operator's kernel.
+static int measured_backward(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
   int rc;
-  if (w.csr) rc = launch_measured_csr<MEAS_SCALE>(c, w, w.r, w.m_ld, w.m_ld, w.at_rp, w.at_ci, w.at_v, c->hwc, w.dym,
+  if (w.conv) {
+    const unsigned grid = (unsigned)((size_t)w.n_rows * ((c->hwc + kConvCols - 1) / kConvCols));
+    measured_conv_adjoint_kernel<<<grid, kConvThreads, conv_smem(c, w, true), s>>>(w.r, w.m_ld, w.cg, w.ck, c->hwc, w.dym,
+                                                                                 c->hwc, R, 2.f / (float)w.m);
+    DGAN_LAUNCH_CHECK(c);
+    rc = 0;
+  } else if (w.csr) rc = launch_measured_csr<MEAS_SCALE>(c, w, w.r, w.m_ld, w.m_ld, w.at_rp, w.at_ci, w.at_v, c->hwc, w.dym,
                                                   c->hwc, nullptr, 1, 2.f / (float)w.m, nullptr, s);
   else rc = launch_measured_gemm<MEAS_SCALE>(c, w, w.r, w.m_ld, w.amt, w.m_ld, c->hwc, w.m_ld, w.dym, c->hwc, nullptr, 1,
                                              2.f / (float)w.m, nullptr, s);
@@ -1222,18 +1301,19 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
 
 // Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
 // workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
-// planned and mapped too.  m > 0: the workspace of a measured entry for m measurements.
+// planned and mapped too.  m > 0: the workspace of a measured entry for m measurements (conv: a convolution operator).
 static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0,
-                    int csr_nnz = -1, bool adam = false) {
+                    int csr_nnz = -1, bool adam = false, const ConvGeom* conv = nullptr) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
   if ((rc = plan_all(c, n_rows))) return rc;
   if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam);
+  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam, conv);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (adam ? (m > 0 ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
+              (conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
+               : adam ? (m > 0 ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
                : weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
                : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
     return DGAN_ERR_WORKSPACE;
@@ -1540,10 +1620,12 @@ int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, vo
   return DGAN_OK;
 }
 
-// The operator and measurements of a measured call (m = 0: not a measured call): dense a, or (nnz >= 0) the CSR rp, ci, val.
+// The operator and measurements of a measured call (m = 0: not a measured call): dense a, or (nnz >= 0) the CSR rp, ci, val,
+// or (conv not NULL) a convolution's geometry and kernels k [batch][kh][kw].
 struct MeasuredArgs {
   const float* a = nullptr; const float* y = nullptr; int m = 0;
   const int* rp = nullptr; const int* ci = nullptr; const float* val = nullptr; int nnz = -1;
+  const ConvGeom* conv = nullptr; const float* k = nullptr;
 };
 
 // m within 1 .. H*W*C and the operator and measurements given; 0, or DGAN_ERR_INVALID_ARG naming the bad argument
@@ -1575,8 +1657,9 @@ static int check_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32
   return 0;
 }
 
-// Stage a measured call's operator and measurements: dense or CSR
+// Stage a measured call's operator and measurements: dense, CSR or convolution
 static int stage_meas(dgan_ctx* c, const Workspace& w, const MeasuredArgs& meas, int batch, cudaStream_t s) {
+  if (w.conv) return stage_measured_conv(c, w, meas.k, meas.y, batch, s);
   if (w.csr) return stage_measured_csr(c, w, meas.rp, meas.ci, meas.val, meas.y, batch, s);
   return stage_measured(c, w, meas.a, meas.y, batch, s);
 }
@@ -1640,13 +1723,13 @@ static int loss_grad_measured_impl(dgan_handle h, const MeasuredArgs& meas, int 
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
   Workspace w;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, meas.m, meas.nnz))) return rc;
+  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, meas.m, meas.nnz, false, meas.conv))) return rc;
   if ((rc = check_huber(huber))) return rc;
   if (huber != nullptr) w.huber = *huber;
   h->n_rows_cur = n_rows;
   if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_meas(h, w, meas, batch, s))) return rc;
   if ((rc = run_forward(h, w, nullptr, 1, 1, true, s)) || (rc = launch_measure(h, w, rec_rr, s))) return rc;
-  if ((rc = measured_backward(h, w, s)) || (rc = measured_loss_finish(h, w, s))) return rc;
+  if ((rc = measured_backward(h, w, rec_rr, s)) || (rc = measured_loss_finish(h, w, s))) return rc;
   if (g_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(g_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
   DGAN_CUDA_CHECK(cudaMemcpyAsync(loss_dev, w.loss, (size_t)n_rows * 4, cudaMemcpyDeviceToDevice, s));
   const size_t n = (size_t)n_rows * h->desc.latent_dim;
@@ -1808,7 +1891,7 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
       // measured loss's gradient and the momentum update with the cotangent's row scales divided out
       if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, per_image, ls))) return r2;
       if (last) continue;
-      if ((r2 = measured_backward(h, w, ls))) return r2;
+      if ((r2 = measured_backward(h, w, per_image, ls))) return r2;
       if (adam != nullptr) {
         if ((r2 = launch_adam(t, lr, 1.f, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr))) return r2;
         continue;
@@ -1888,6 +1971,11 @@ static void set_optimizer_key(dgan_ctx::LoopGraph* key, const dgan_adam_params* 
   key->adam = 1; key->beta1 = adam->beta1; key->beta2 = adam->beta2; key->eps = adam->eps;
 }
 
+// The operator part of a loop's graph-cache key: a convolution's geometry (its kernels are staged outside the graph).
+static void set_conv_key(dgan_ctx::LoopGraph* key, const ConvGeom* g) {
+  if (g != nullptr) key->conv = {g->kh, g->kw, g->ph, g->pw, g->s};
+}
+
 // Adam's hyper-parameters: 0 <= beta1 < 1, 0 <= beta2 < 1 and a finite eps > 0; 0, or DGAN_ERR_INVALID_ARG naming the bad
 // value.
 static int check_adam(const dgan_adam_params* a) {
@@ -1921,7 +2009,7 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   cudaStream_t s = (cudaStream_t)stream;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr, meas.conv))) return rc;
   if ((rc = check_huber(huber))) return rc;
   if (huber != nullptr) w.huber = *huber;
   const int64_t launches0 = h->launches;
@@ -1944,6 +2032,7 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
                           prm->momentum, {}, nullptr, 0};
   set_optimizer_key(&key, adam);
   key.huber = w.huber;
+  set_conv_key(&key, meas.conv);
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
     return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls, false, adam);
   };
@@ -1993,25 +2082,26 @@ static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_r
 // The regions of a pruned workspace: region 0 for batch * rec_rr rows, region k for batch * keep_k rows, each a carve()
 // with the prune maps, one after the other (every carve is a multiple of 1024 bytes).  *bytes: the total; layout (not
 // NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
-// m > 0: a pruned measured workspace (csr_nnz >= 0: CSR): first the operator block (carve_operator; layout: a line
+// m > 0: a pruned measured workspace (csr_nnz >= 0: CSR; conv not NULL: convolution): first the operator block (carve_operator; layout: a line
 // "operator 0 batch", then its lines), staged once for every stage, then the regions, each with the row-sized measured
 // buffers and the operator block's pointers.  adam: every region an Adam carve (its second moment "s" last).
 static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
                                            int n_points, void* base, bool weighted, size_t* bytes,
-                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1, bool adam = false) {
+                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1, bool adam = false,
+                                           const ConvGeom* conv = nullptr) {
   std::vector<Workspace> regs;
   size_t off = 0;
   Workspace op;
   if (m > 0) {
     if (layout != nullptr) *layout += "operator 0 " + std::to_string(batch) + "\n";
-    op = carve_operator(c, batch, m, csr_nnz, base, layout);
+    op = carve_operator(c, batch, m, csr_nnz, base, layout, conv);
     off = op.bytes;
   }
   for (int k = 0; k <= n_points; ++k) {
     const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
     if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
     regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, m, csr_nnz, true,
-                         m > 0 ? &op : nullptr, adam));
+                         m > 0 ? &op : nullptr, adam, conv));
     off += regs.back().bytes;
   }
   *bytes = off;
@@ -2058,10 +2148,11 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, weighted))) return rc;
   size_t need = 0;
   std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need, nullptr, meas.m,
-                                             meas.nnz, adam != nullptr);
+                                             meas.nnz, adam != nullptr, meas.conv);
   if (need > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
-              (adam != nullptr ? (measured ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
+              (meas.conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
+               : adam != nullptr ? (measured ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
                : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
@@ -2097,6 +2188,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
   set_optimizer_key(&key, adam);
   key.huber = huber != nullptr ? *huber : 0.f;
+  set_conv_key(&key, meas.conv);
   // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
   // (measured) left
   auto loss_finish = [&](const Workspace& w, cudaStream_t ls) -> int {
@@ -2388,6 +2480,86 @@ int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const in
   meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
   return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
                                  &huber_delta);
+}
+
+// ---- convolution operators (kernels_measured_conv.cuh): a third operator kind through the measured drivers ----------
+// The geometry of op on h's image: 1 <= kh <= min(H, 32), 1 <= kw <= min(W, 32), 0 <= 2 ph <= kh - 1,
+// 0 <= 2 pw <= kw - 1, 1 <= stride <= 16.  false (with *why naming the bad value) outside that range.
+static bool conv_geom(const dgan_ctx* h, const dgan_conv_op* op, ConvGeom* g, std::string* why = nullptr) {
+  std::string bad;
+  if (op->kh < 1 || op->kh > std::min(h->H, 32)) bad = "kh = " + std::to_string(op->kh) + " must be in [1, " + std::to_string(std::min(h->H, 32)) + "]";
+  else if (op->kw < 1 || op->kw > std::min(h->W, 32)) bad = "kw = " + std::to_string(op->kw) + " must be in [1, " + std::to_string(std::min(h->W, 32)) + "]";
+  else if (op->pad_h < 0 || 2 * op->pad_h > op->kh - 1) bad = "pad_h = " + std::to_string(op->pad_h) + " must satisfy 0 <= 2 pad_h <= kh - 1";
+  else if (op->pad_w < 0 || 2 * op->pad_w > op->kw - 1) bad = "pad_w = " + std::to_string(op->pad_w) + " must satisfy 0 <= 2 pad_w <= kw - 1";
+  else if (op->stride < 1 || op->stride > 16) bad = "stride = " + std::to_string(op->stride) + " must be in [1, 16]";
+  if (!bad.empty()) {
+    if (why != nullptr) *why = "invalid convolution operator: " + bad;
+    return false;
+  }
+  *g = ConvGeom{h->H, h->W, h->C, op->kh, op->kw, op->pad_h, op->pad_w, op->stride,
+                (h->H + 2 * op->pad_h - op->kh) / op->stride + 1, (h->W + 2 * op->pad_w - op->kw) / op->stride + 1};
+  return true;
+}
+
+// A convolution call's operator arguments: op given with a geometry in range, k_dev and y_dev given.  0 (meas filled in,
+// its conv pointing at *g), or DGAN_ERR_INVALID_ARG naming the bad argument.
+static int check_measured_conv(dgan_handle h, const dgan_conv_op* op, const float* k_dev, const float* y_dev, ConvGeom* g,
+                               MeasuredArgs* meas) {
+  if (op == nullptr) { set_error("NULL convolution operator op"); return DGAN_ERR_INVALID_ARG; }
+  std::string why;
+  if (!conv_geom(h, op, g, &why)) { set_error(why); return DGAN_ERR_INVALID_ARG; }
+  if (k_dev == nullptr) { set_error("NULL kernels k_dev"); return DGAN_ERR_INVALID_ARG; }
+  if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
+  meas->y = y_dev; meas->m = g->Ho * g->Wo * g->C; meas->k = k_dev; meas->conv = g;
+  return 0;
+}
+
+int dgan_conv_op_m(dgan_handle h, const dgan_conv_op* op) {
+  ConvGeom g;
+  if (h == nullptr || op == nullptr || !conv_geom(h, op, &g)) return 0;
+  return g.Ho * g.Wo * g.C;
+}
+
+size_t dgan_workspace_bytes_measured_conv(dgan_handle h, int batch, int rec_rr, const dgan_conv_op* op,
+                                          const dgan_prune_point* sched, int n_points, int adam) {
+  ConvGeom g;
+  if (h == nullptr || op == nullptr || batch <= 0 || rec_rr <= 0 || !conv_geom(h, op, &g)) return 0;
+  const int m = g.Ho * g.Wo * g.C;
+  if (unpruned(sched, n_points)) {
+    if (plan_all(h, batch * rec_rr) != 0) return 0;
+    return carve(h, batch * rec_rr, nullptr, nullptr, false, m, -1, false, nullptr, adam != 0, &g).bytes;
+  }
+  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, -1, adam != 0, &g);
+  return bytes;
+}
+
+int dgan_reconstruct_measured_conv(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                   const float* huber_delta, const dgan_prune_point* sched, int n_points,
+                                   const dgan_conv_op* op, const float* k_dev, const float* y_dev, const float* z0_dev,
+                                   float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                                   void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  ConvGeom g;
+  MeasuredArgs meas;
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta);
+}
+
+int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const dgan_conv_op* op, const float* k_dev,
+                                 const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
+                                 float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  ConvGeom g;
+  MeasuredArgs meas;
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
+  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
+                                 huber_delta);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -2774,6 +2946,23 @@ int dgan_debug_workspace_layout_adam(dgan_handle h, int batch, int rec_rr, int w
     size_t bytes = 0;
     carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out, m, m > 0 ? nnz : -1, true);
   }
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
+}
+
+// The same for the workspace of the convolution-measured entries (dgan_workspace_bytes_measured_conv, unpruned, without
+// Adam): after the unweighted buffers, the measured ones without "am" and "amt" - "ym" [n_pad][m_ld], "r" [n_pad][m_ld],
+// "dym" [n_pad][H*W*C], "mloss_part" [m_ld / 64][n_pad], "mscale" [n_pad] - then the staged kernels "ck" f32
+// [n_pad][kh * kw] (image b's at row b).
+int dgan_debug_workspace_layout_measured_conv(dgan_handle h, int n_rows, const dgan_conv_op* op, char* buf, int buf_len) {
+  ConvGeom g;
+  if (h == nullptr || op == nullptr || !conv_geom(h, op, &g) || n_rows <= 0 || buf == nullptr || buf_len <= 0) {
+    set_error("invalid argument");
+    return -1;
+  }
+  std::string out;
+  carve(h, n_rows, nullptr, &out, false, g.Ho * g.Wo * g.C, -1, false, nullptr, false, &g);
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();

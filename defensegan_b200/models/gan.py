@@ -26,6 +26,7 @@ import numpy as np
 import torch
 
 from .. import _native
+from ..operators import ConvOperator
 from .. import tf_bundle as _tf_bundle
 from .. import weights as _weights
 from ..utils.config import load_config, packaged_cfg_path
@@ -459,7 +460,13 @@ class DefenseGANBase(object):
         measured loop updates z with Adam (rec_lr is then a step in z units), pruned or not.
 
         `rec_huber_delta` is read at call time as in `reconstruct`: a delta replaces the squared error of each measurement
-        residual by the Huber loss, (1/m) sum_j rho(r_j), for a few corrupted measurements, dense or sparse, pruned or not."""
+        residual by the Huber loss, (1/m) sum_j rho(r_j), for a few corrupted measurements, dense or sparse, pruned or not.
+
+        `operator` may also be a `defensegan_b200.operators.ConvOperator`: a blur, box downsample or blurred decimation,
+        with one kernel for every image or one per image (deblurring photos with their own point-spread functions), applied
+        as a stencil.  m is its num_measurements(image_dim); a per-image kernel count must equal B.  On both precisions
+        the result is bit-identical to the call with its to_sparse_csr matrix (one call per image for per-image kernels),
+        and it runs with prune, rec_optimizer and rec_huber_delta as the other operator kinds do."""
         adam = self._adam_params()
         huber = self._huber_delta()
         if prune is _NOT_GIVEN:
@@ -472,6 +479,9 @@ class DefenseGANBase(object):
                 raise ValueError("prune is not supported with use_bn: the batch statistics couple the restarts, so "
                                  "dropping some would change the others' trajectories")
             prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
+        if isinstance(operator, ConvOperator):
+            return self._reconstruct_measured_conv(measurements, operator, batch_size, z_init_val, return_aux, out,
+                                                   z_row_offset, prune, adam, huber)
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
                                                      z_row_offset, prune, adam, huber)
@@ -499,6 +509,37 @@ class DefenseGANBase(object):
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
                                            **kw)
+
+    def _reconstruct_measured_conv(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
+                                   prune, adam=None, huber=None):
+        """reconstruct_measured for a ConvOperator, after one check of the kernels and the measurements (prune, adam and
+        huber as in _reconstruct_measured_sparse).  The native call gets the kernels broadcast to [B, kh, kw]."""
+        m = operator.num_measurements(self.image_dim)
+        y = self._as_cuda(measurements)
+        if y.dim() != 2 or y.shape[1] != m or y.shape[0] == 0:
+            raise ValueError("measurements must be [B, %d] (one row of the operator's m values per image), got %s"
+                             % (m, tuple(y.shape)))
+        b = y.shape[0]
+        if batch_size is not None and int(batch_size) != b:
+            raise ValueError("batch_size (%d) does not match measurements.shape[0] (%d)" % (int(batch_size), b))
+        if operator.per_image and operator.kernel.shape[0] != b:
+            raise ValueError("operator has %d per-image kernels for %d images (measurements.shape[0])"
+                             % (operator.kernel.shape[0], b))
+        k = operator.kernels(b, y.device)
+        finite = torch.stack([torch.isfinite(k).all(), torch.isfinite(y).all()]).tolist()
+        bad = [name for name, ok in zip(("operator kernels", "measurements"), finite) if not ok]
+        if bad:
+            raise ValueError("%s must be finite" % " and ".join(bad))
+        z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
+        native = self._get_native(y.device)
+        self.last_seed = seed = self._next_seed(0)
+        kw = {} if adam is None else {"adam": adam}
+        if huber is not None:
+            kw["huber_delta"] = huber
+        return native.reconstruct_measured(y, operator._with_kernels(k), int(self.rec_rr), int(self.rec_iters),
+                                           float(self.rec_lr), z_init_val=z0, seed=seed,
+                                           momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
+                                           return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune, **kw)
 
     def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
                                      prune, adam=None, huber=None):

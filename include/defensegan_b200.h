@@ -427,6 +427,69 @@ int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const in
                                       const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* workspace,
                                       size_t workspace_bytes, void* stream);
 
+/* A convolution operator: for an image x [H, W, C] (NHWC) and a kernel k [kh, kw] (fp32, one per image, the same for
+ * every channel), stride s and zero padding (pad_h, pad_w):
+ *   Ho = (H + 2 pad_h - kh) / s + 1,  Wo = (W + 2 pad_w - kw) / s + 1,  m = Ho * Wo * C,
+ *   (A x)[(u * Wo + v) * C + c] = sum over a < kh, b < kw with 0 <= i < H, 0 <= j < W of k[a][b] x[i][j][c],
+ *                                 i = s u + a - pad_h, j = s v + b - pad_w
+ * (a cross-correlation: the kernel is not flipped; torch's conv2d with groups = C and the kernel repeated per channel).
+ * A blur is (5, 5, 2, 2, 1), a 2x2 block average (2, 2, 0, 0, 2) with 0.25 everywhere.  Accepted geometry:
+ * 1 <= kh <= min(H, 32), 1 <= kw <= min(W, 32), 0 <= 2 pad_h <= kh - 1, 0 <= 2 pad_w <= kw - 1, 1 <= stride <= 16. */
+typedef struct dgan_conv_op {
+  int32_t kh, kw, pad_h, pad_w, stride;
+} dgan_conv_op;
+
+/* m = Ho * Wo * C for this handle's image, or 0 for a geometry outside the accepted range (or a NULL handle or op). */
+int dgan_conv_op_m(dgan_handle h, const dgan_conv_op* op);
+
+/* Bytes of scratch for dgan_reconstruct_measured_conv / dgan_loss_grad_measured_conv: unpruned (sched NULL, n_points 0)
+ * the workspace of dgan_workspace_bytes_measured without the copies of A and A^T, plus the kernels [batch][kh][kw]; a
+ * schedule: that of dgan_workspace_bytes_measured_pruned with this operator block.  adam != 0 adds Adam's s, as
+ * dgan_workspace_bytes_measured_adam does.  0 for a geometry outside the accepted range and where those sizers return 0. */
+size_t dgan_workspace_bytes_measured_conv(dgan_handle h, int batch, int rec_rr, const dgan_conv_op* op,
+                                          const dgan_prune_point* sched, int n_points, int adam);
+
+/* dgan_reconstruct_measured with the convolution operator op: image i's operator A_i uses its own kernel
+ * k_dev [batch][kh][kw] (fp32, on the device; a shared kernel is passed as batch copies), y_dev [batch][m].  The loss,
+ * its normaliser m, z0, decay_lr, the pre-update forward of iteration L-1 and the select (ties, NaN rule) are those of
+ * dgan_reconstruct_measured for A_i; the restarts of image i share k_i and y_i.  adam NULL: the momentum update, else
+ * the Adam update of dgan_reconstruct_adam; huber_delta NULL: the squared error, else the Huber loss of
+ * dgan_reconstruct_huber at *huber_delta (checked as there); sched NULL with n_points 0: unpruned, else the restart
+ * pruning of dgan_reconstruct_measured_pruned (use_bn with a schedule: DGAN_ERR_UNSUPPORTED).
+ * Both products run in fp32 on the CUDA cores on both precisions, as a stencil: each reads G or r once and writes r or
+ * dy once.  Their evaluation order is the CSR products' on the matrix the stencil represents, so every output is
+ * bit-identical to dgan_reconstruct_measured_csr's (and its _adam, _huber and _pruned variants') on that matrix:
+ *   measurement output j: one fmaf chain from +0 over the in-bounds taps in ascending (a, b) (ascending input column),
+ *     then the residual and loss parts of the CSR product (per quad of columns, then a butterfly over each 64-column
+ *     tile; padded columns give r = 0);
+ *   adjoint output p = (i, j, c): one chain from +0 over the output pixels (u, v) whose window covers (i, j), in
+ *     ascending order (ascending row of A), then the multiply by 2/m.
+ * A tap whose value is 0 adds a term the CSR does not hold; the chains start at +0 and G and r are finite, so no bit
+ * changes.  The kernels and measurements are not checked for finiteness here.
+ * A geometry outside the accepted range, a NULL op, k_dev or y_dev, or a rec_dev that is not 16-byte aligned:
+ * DGAN_ERR_INVALID_ARG naming the bad value; a workspace smaller than dgan_workspace_bytes_measured_conv:
+ * DGAN_ERR_WORKSPACE; nothing is enqueued in any of these cases.
+ * Workspace: dgan_workspace_bytes_measured_conv.  The kernels and y are copied into it by one kernel (no stream
+ * operation more than dgan_reconstruct's image copy), outside the captured loop; the graph cache keys on the geometry,
+ * not on the kernel values, so new kernels with the same geometry replay the graph.  No host synchronisation, no
+ * allocation once the size has been planned.  Per L-step it runs the kernels of dgan_reconstruct_measured (one kernel
+ * per product).  So dgan_last_launch_count is dgan_reconstruct's + 1 + 6 (L - 1) + 1 with DGAN_PREC_FP16 and
+ * + 1 + 3 (L - 1) + 1 with DGAN_PREC_FP32 (dgan_reconstruct_measured_csr's - 4), plus 3 P + 1 with P prune points and
+ * L - 1 nowhere for Adam, as for the other operator kinds; dgan_last_enqueue_count is dgan_reconstruct's, + 1 with a
+ * schedule. */
+int dgan_reconstruct_measured_conv(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                   const float* huber_delta, const dgan_prune_point* sched, int n_points,
+                                   const dgan_conv_op* op, const float* k_dev, const float* y_dev, const float* z0_dev,
+                                   float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                                   void* stream);
+
+/* dgan_loss_grad_measured with the convolution operator of dgan_reconstruct_measured_conv (huber_delta NULL: the squared
+ * error, else the Huber loss at *huber_delta).  Workspace: dgan_workspace_bytes_measured_conv(h, batch, rec_rr, op,
+ * NULL, 0, 0). */
+int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const dgan_conv_op* op, const float* k_dev,
+                                 const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
+                                 float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream);
+
 /* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
  *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
  *   y_dev [n_rows, H*W*C] = G(z) (nullable; bit-identical to dgan_forward).  The forward is recomputed.
@@ -456,15 +519,17 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * dgan_reconstruct_measured[_csr]_pruned call 3 P + 1 more than the unpruned measured call with the same operator kind.
  * An Adam call (dgan_reconstruct_adam, dgan_reconstruct_measured[_csr]_adam) runs as many as its momentum counterpart,
  * plus L - 1 on the DGAN_PREC_FP16 image loss, whose Adam update is a kernel of its own.  A Huber call
- * (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber) runs as many as its squared-error counterpart. */
+ * (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber) runs as many as its squared-error counterpart.  A
+ * dgan_reconstruct_measured_conv call runs 4 fewer than the dgan_reconstruct_measured_csr call with the same options. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
  * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
  * nnz, prune schedule, optimiser: momentum, or Adam with its beta1, beta2 and eps, and data term: the squared error, or
  * the Huber loss with its delta) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
- * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them),
- * graph, loss sum, arg-min select. */
+ * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them;
+ * convolution-measured calls: the one that stages the kernels and y), graph, loss sum, arg-min select.  A convolution
+ * operator's geometry is part of the key; its kernel values are not. */
 int64_t dgan_last_enqueue_count(dgan_handle h);
 
 /* Algorithmic multiply-accumulates of one generator forward per latent row (exact in-bounds

@@ -13,9 +13,14 @@ With --sparse instead: sparse operators (a 2x2 block average, a full-resolution 
 at MNIST B = 256 and CelebA B = 128, R = 10, L = 200, passed dense and as CSR; plain, dense and CSR calls alternate
 repeat by repeat.  Reports images/s of each call, the device time of the CSR products (torch.profiler) with their
 algorithmic bytes over it as a share of 3.35 TB/s (HBM3, H100 SXM data sheet), and the workspace bytes of both calls.
-A dense call that does not fit in memory is reported as not run.  Writes <out_dir>/measured_bench_sparse.json.
+A dense call that does not fit in memory is reported as not run.  The block averages and the blur also run as a
+ConvOperator (the stencil products of dgan_reconstruct_measured_conv), timed in the same alternation, and two more rows
+run plain and convolution calls only: a 4x box downsample and per-image random 9 x 9 motion-blur kernels.  The product
+times of the CSR and convolution calls are each set against the same byte count - G or r read once, r or dy written
+once - as a share of 3.35 TB/s.  Writes <out_dir>/measured_bench_sparse.json.
 Usage: python tools/measured_bench.py OUT_DIR [--reps N] [--warmup N] [--precision fp16|fp32] [--user-steps N] [--sparse]"""
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -116,6 +121,44 @@ def csr_kernel_times(gen, y, a, z, R, calls=10):
     return out
 
 
+def conv_kernel_times(gen, y, op, z, R, calls=10):
+    """Mean device time per call of each convolution product over dgan_loss_grad_measured_conv calls (torch.profiler)."""
+    from torch.profiler import ProfilerActivity, profile
+    gen.loss_grad_measured(y, op, z, R)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            gen.loss_grad_measured(y, op, z, R)
+        torch.cuda.synchronize()
+    out = {"measure": 0.0, "adjoint": 0.0}
+    for ka in prof.key_averages():
+        if "measured_conv_adjoint_kernel" in ka.key:
+            out["adjoint"] += ka.device_time_total / 1e3 / calls
+        elif "measured_conv_kernel" in ka.key:
+            out["measure"] += ka.device_time_total / 1e3 / calls
+    return out
+
+
+def motion_kernels(B, size=9, seed=0):
+    """B random motion-blur kernels: a random walk of 2 size steps from the centre, its visits counted and normalised."""
+    rs = np.random.RandomState(seed)
+    ks = np.zeros((B, size, size), dtype=np.float64)
+    for b in range(B):
+        i = j = size // 2
+        for _ in range(2 * size):
+            ks[b, i, j] += 1.0
+            di, dj = rs.randint(-1, 2, size=2)
+            i, j = min(size - 1, max(0, i + di)), min(size - 1, max(0, j + dj))
+        ks[b] /= ks[b].sum()
+    return ks.astype(np.float32)
+
+
+def stream_bytes(n, m, hwc):
+    """Bytes each product has to move on n latent rows: G (or r) read once, r (or dy) written once."""
+    m_ld = (m + 63) // 64 * 64
+    return 4 * (n * hwc + n * m_ld), 4 * (n * m_ld + n * hwc)
+
+
 def csr_product_bytes(n, m, hwc, nnz):
     """Algorithmic bytes of the two CSR products of one L-step on n latent rows: G (or r) read once, r (or dy) written once,
     the staged operator (int32 row pointers, int32 columns, fp32 values) and the measurements read once."""
@@ -127,6 +170,7 @@ def csr_product_bytes(n, m, hwc, nnz):
 
 def sparse_main(args, dev):
     from defensegan_b200 import _native as N
+    from defensegan_b200.operators import ConvOperator
     res = {"card": card(), "reps": args.reps, "warmup": args.warmup, "precision": args.precision, "results": []}
     for arch, B, R, L, subs in (("mnist", 256, 10, 200, (100, 392)), ("celeba", 128, 10, 200, (1024, 4096))):
         w = O.init_generator_weights(arch)
@@ -139,9 +183,34 @@ def sparse_main(args, dev):
         ops = {"block2": MO.block_average_operator(h, w_, c, 2), "blur5": SO.blur_operator(h, w_, c)}
         for m in subs:
             ops["sub%d" % m] = SO.subsample_operator(m, hwc, seed=m)
+        convs = {"block2": ConvOperator.box(2), "blur5": ConvOperator.gaussian(5, 1.0), "box4": ConvOperator.box(4),
+                 "motion9": ConvOperator(motion_kernels(B), stride=1, padding=4)}
+        ops["box4"] = ops["motion9"] = None
         r = {"arch": arch, "images": B, "restarts": R, "steps": L, "precision": args.precision, "operators": []}
         t_plain = []
         for name, a_np in ops.items():
+            conv = convs.get(name)
+            if a_np is None:                         # a convolution only: plain and conv calls
+                m = conv.num_measurements((h, w_, c))
+                lr = 10.0 * min(1.0, 4.0 * m / hwc) if m < hwc else 10.0
+                y = conv(x.reshape(B, h, w_, c).double()).float()
+                calls = {"plain": lambda: gen.reconstruct(x, R, L, 10.0, z_init_val=z0),
+                         "conv": lambda: gen.reconstruct_measured(y, conv, R, L, lr, z_init_val=z0)}
+                times = {k: [] for k in calls}
+                for i in range(args.warmup + args.reps):
+                    for k, fn in calls.items():
+                        t = timed(fn)
+                        if i >= args.warmup:
+                            times[k].append(t)
+                t_plain += times["plain"]
+                med = {k: float(np.median(v)) for k, v in times.items()}
+                e = {"operator": name, "m": m, "plain_ms": round(med["plain"], 3)}
+                e.update(conv_entry(gen, conv, y, z0, B, R, L, m, hwc, med, times, h, w_, c))
+                print(json.dumps(e), flush=True)
+                r["operators"].append(e)
+                gen._ws = None
+                torch.cuda.empty_cache()
+                continue
             m = a_np.shape[0]
             lr = 10.0 * min(1.0, 4.0 * m / hwc) if m < hwc else 10.0
             dense = torch.tensor(a_np).to(dev)
@@ -152,6 +221,8 @@ def sparse_main(args, dev):
             ws_csr = int(gen.lib.dgan_workspace_bytes_measured_csr(gen._handle, B, R, m, nnz))
             calls = {"plain": lambda: gen.reconstruct(x, R, L, 10.0, z_init_val=z0),
                      "csr": lambda: gen.reconstruct_measured(y, csr, R, L, lr, z_init_val=z0)}
+            if conv is not None:
+                calls["conv"] = lambda: gen.reconstruct_measured(y, conv, R, L, lr, z_init_val=z0)
             dense_note = None
             try:
                 gen.reconstruct_measured(y, dense, R, 1, lr, z_init_val=z0)
@@ -182,6 +253,12 @@ def sparse_main(args, dev):
                  "csr_measure_hbm_share": round(bm / (kt["measure"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["measure"] else None,
                  "csr_adjoint_hbm_share": round(ba / (kt["adjoint"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["adjoint"] else None,
                  "workspace_bytes_dense": ws_dense, "workspace_bytes_csr": ws_csr}
+            if conv is not None:
+                e.update(conv_entry(gen, conv, y, z0, B, R, L, m, hwc, med, times, h, w_, c))
+                e["conv_over_csr"] = round(med["conv"] / med["csr"], 4)
+                sm, sa = stream_bytes(B * R, m, hwc)
+                e["csr_measure_stream_share"] = round(sm / (kt["measure"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["measure"] else None
+                e["csr_adjoint_stream_share"] = round(sa / (kt["adjoint"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["adjoint"] else None
             if "dense" in med:
                 e.update({"dense_ms": round(med["dense"], 3), "dense_images_per_s": round(B / med["dense"] * 1e3, 1),
                           "dense_over_csr": round(med["dense"] / med["csr"], 3)})
@@ -198,6 +275,26 @@ def sparse_main(args, dev):
     os.makedirs(args.out_dir, exist_ok=True)
     with open(os.path.join(args.out_dir, "measured_bench_sparse.json"), "w") as f:
         json.dump(res, f, indent=1)
+
+
+def conv_entry(gen, conv, y, z0, B, R, L, m, hwc, med, times, h, w_, c):
+    """The convolution call's columns of a --sparse row: its time, its products' times and their share of HBM on the
+    stream byte count, and its workspace bytes."""
+    from defensegan_b200 import _native as N
+    kt = conv_kernel_times(gen, y, conv, z0, R)
+    sm, sa = stream_bytes(B * R, m, hwc)
+    kh, kw = conv.kernel_size
+    op = N.dgan_conv_op(kh, kw, conv.padding[0], conv.padding[1], conv.stride)
+    return {"kernel": [kh, kw], "stride": conv.stride, "padding": list(conv.padding), "per_image": conv.per_image,
+            "conv_ms": round(med["conv"], 3), "conv_images_per_s": round(B / med["conv"] * 1e3, 1),
+            "conv_spread_ms": [round(min(times["conv"]), 3), round(max(times["conv"]), 3)],
+            "conv_over_plain": round(med["conv"] / med["plain"], 4),
+            "conv_measure_product_ms": round(kt["measure"], 4), "conv_adjoint_product_ms": round(kt["adjoint"], 4),
+            "stream_measure_bytes": sm, "stream_adjoint_bytes": sa,
+            "conv_measure_hbm_share": round(sm / (kt["measure"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["measure"] else None,
+            "conv_adjoint_hbm_share": round(sa / (kt["adjoint"] * 1e-3) / (HBM_TBPS * 1e12), 4) if kt["adjoint"] else None,
+            "workspace_bytes_conv": int(gen.lib.dgan_workspace_bytes_measured_conv(gen._handle, B, R, ctypes.byref(op),
+                                                                                    None, 0, 0))}
 
 
 def main():
