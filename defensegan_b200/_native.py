@@ -48,6 +48,8 @@ ABI_SYMBOLS = [
     "dgan_reconstruct_huber", "dgan_reconstruct_measured_huber", "dgan_reconstruct_measured_csr_huber",
     "dgan_loss_grad_huber", "dgan_loss_grad_measured_huber", "dgan_loss_grad_measured_csr_huber",
     "dgan_conv_op_m", "dgan_workspace_bytes_measured_conv", "dgan_reconstruct_measured_conv", "dgan_loss_grad_measured_conv",
+    "dgan_reconstruct_prior", "dgan_reconstruct_measured_prior", "dgan_reconstruct_measured_csr_prior",
+    "dgan_reconstruct_measured_conv_prior",
 ]
 
 
@@ -115,6 +117,24 @@ def check_huber_delta(huber_delta):
     if not d > 0.0:
         raise ValueError("huber_delta = %r must be > 0 (+inf allowed)" % (huber_delta,))
     return d
+
+
+def check_z_prior(z_prior):
+    """The latent prior's weight lambda as a float, after the rule of dgan_reconstruct_prior: as fp32 (the type the
+    library reads) finite and >= 0, with 2 lambda finite in fp32.  A ValueError names the bad value (NaN, an infinity, a
+    negative value, one whose double overflows fp32, or a non-number)."""
+    if isinstance(z_prior, bool) or not isinstance(z_prior, (int, float, np.integer, np.floating)):
+        raise ValueError("z_prior = %r is not a number" % (z_prior,))
+    try:
+        with np.errstate(over="ignore"):   # beyond fp32's range: +-inf, as the library would read it
+            lam = np.float32(z_prior)
+    except OverflowError:                  # an int beyond a double's range
+        lam = np.float32(np.inf)
+    with np.errstate(over="ignore"):
+        two = lam * np.float32(2.0)
+    if not (np.isfinite(lam) and lam >= 0.0 and np.isfinite(two)):
+        raise ValueError("z_prior = %r must be finite and >= 0, with 2 z_prior finite in fp32" % (z_prior,))
+    return float(lam)
 
 
 def check_prune_schedule(prune, rec_rr: int, rec_iters: int):
@@ -294,6 +314,17 @@ def load_library() -> ctypes.CDLL:
                                                    vp, vp, vp, sz, vp]
     lib.dgan_loss_grad_measured_conv.restype = i32
     lib.dgan_loss_grad_measured_conv.argtypes = [vp, fp, cp, vp, vp, i32, i32, vp, vp, vp, vp, vp, sz, vp]
+    rp = ctypes.POINTER(dgan_rec_params)
+    lib.dgan_reconstruct_prior.restype = i32
+    lib.dgan_reconstruct_prior.argtypes = [vp, rp, ap, fp, f32, pp, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_prior.restype = i32
+    lib.dgan_reconstruct_measured_prior.argtypes = [vp, rp, ap, fp, f32, pp, i32, vp, i32, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_csr_prior.restype = i32
+    lib.dgan_reconstruct_measured_csr_prior.argtypes = [vp, rp, ap, fp, f32, pp, i32, vp, vp, vp, i32, i32, vp, vp, vp, vp,
+                                                        vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_conv_prior.restype = i32
+    lib.dgan_reconstruct_measured_conv_prior.argtypes = [vp, rp, ap, fp, f32, pp, i32, cp, vp, vp, vp, vp, vp, vp, vp, sz,
+                                                         vp]
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
     lib.dgan_forward.argtypes = [vp, vp, i32, vp, vp, sz, vp]
@@ -330,6 +361,11 @@ def _check(lib, rc: int, what: str):
 
 def _ptr(t: Optional[torch.Tensor]):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
+
+
+def _byref_or_none(obj):
+    """ctypes.byref(obj) for a nullable pointer argument, None (NULL) for None."""
+    return ctypes.byref(obj) if obj is not None else None
 
 
 def _require_cuda_f32(t: torch.Tensor, name: str) -> torch.Tensor:
@@ -476,7 +512,7 @@ class NativeGenerator:
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
                     z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None,
                     prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
-                    huber_delta: Optional[float] = None):
+                    huber_delta: Optional[float] = None, z_prior: Optional[float] = None):
         """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
         the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
         (dgan_reconstruct_weighted).
@@ -490,7 +526,13 @@ class NativeGenerator:
         (dgan_reconstruct_huber, with any of pixel_weights, prune and adam): residuals beyond delta count linearly, so a
         few badly wrong pixels pull the fit less.  With momentum the gradient of clipped residuals shrinks with delta, so
         rec_lr has to grow as delta falls; Adam is invariant to that scale.  None runs the squared error, through exactly
-        the entry and arguments it always did."""
+        the entry and arguments it always did.
+        z_prior (lambda >= 0, see check_z_prior): each restart minimises J = D + lambda ||z||^2, a Gaussian prior on z that
+        keeps it where the generator was trained (dgan_reconstruct_prior, with any of pixel_weights, prune, adam and
+        huber_delta).  D keeps its 1/HWC normaliser, so lambda is relative to the mean loss: the lambda of a formulation on
+        the unnormalised sum does not carry over.  The returned loss is J, the restart is J's arg-min and prune ranks by
+        J.  0.0 runs the prior entry and gives the bits of the call without it; None runs the call without the prior,
+        through exactly the entry and arguments it always did."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
@@ -501,6 +543,7 @@ class NativeGenerator:
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
         delta = None if huber_delta is None else check_huber_delta(huber_delta)
+        lam = None if z_prior is None else check_z_prior(z_prior)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -517,7 +560,14 @@ class NativeGenerator:
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if delta is not None:
+            if lam is not None:
+                rc = self.lib.dgan_reconstruct_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
+                                                     _byref_or_none(None if delta is None else ctypes.c_float(delta)), lam,
+                                                     sched, len(sched) if sched is not None else 0, _ptr(x), _ptr(pw),
+                                                     _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                     ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_prior")
+            elif delta is not None:
                 rc = self.lib.dgan_reconstruct_huber(self._handle, ctypes.byref(prm), ctypes.byref(ap) if ap is not None
                                                      else None, delta, sched, len(sched) if sched is not None else 0,
                                                      _ptr(x), _ptr(pw), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
@@ -614,14 +664,16 @@ class NativeGenerator:
         return y, k, op, batch, m
 
     def _reconstruct_measured_conv(self, measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed, momentum,
-                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta):
-        """reconstruct_measured for a ConvOperator (dgan_reconstruct_measured_conv)."""
+                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta, z_prior):
+        """reconstruct_measured for a ConvOperator (dgan_reconstruct_measured_conv, or dgan_reconstruct_measured_conv_prior
+        with z_prior)."""
         y, k, op, batch, m = self._measured_conv(measurements, operator)
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
         delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
+        lam = None if z_prior is None else check_z_prior(z_prior)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -638,13 +690,21 @@ class NativeGenerator:
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            rc = self.lib.dgan_reconstruct_measured_conv(self._handle, ctypes.byref(prm),
-                                                         ctypes.byref(ap) if ap is not None else None,
-                                                         ctypes.byref(delta) if delta is not None else None, sched,
-                                                         len(sched) if sched is not None else 0, ctypes.byref(op), _ptr(k),
-                                                         _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                         ctypes.c_void_p(stream))
-            _check(self.lib, rc, "dgan_reconstruct_measured_conv")
+            n_points = len(sched) if sched is not None else 0
+            if lam is not None:
+                rc = self.lib.dgan_reconstruct_measured_conv_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
+                                                                   _byref_or_none(delta), lam, sched, n_points,
+                                                                   ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0), _ptr(rec),
+                                                                   _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_conv_prior")
+            else:
+                rc = self.lib.dgan_reconstruct_measured_conv(self._handle, ctypes.byref(prm),
+                                                             ctypes.byref(ap) if ap is not None else None,
+                                                             ctypes.byref(delta) if delta is not None else None, sched,
+                                                             n_points, ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0),
+                                                             _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                             ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_conv")
         if return_aux:
             return rec, loss, idx
         return rec
@@ -654,7 +714,7 @@ class NativeGenerator:
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
                              return_aux: bool = False, z_row_offset: int = 0,
                              prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
-                             huber_delta: Optional[float] = None):
+                             huber_delta: Optional[float] = None, z_prior: Optional[float] = None):
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
@@ -670,11 +730,15 @@ class NativeGenerator:
         (dgan_reconstruct_measured_huber, or dgan_reconstruct_measured_csr_huber for a CSR operator), with any of prune
         and adam.  None runs the squared error as before.
         A defensegan_b200.operators.ConvOperator runs dgan_reconstruct_measured_conv: a convolution with one kernel per
-        image (a shared kernel is passed as B copies), applied as a stencil, with any of prune, adam and huber_delta."""
+        image (a shared kernel is passed as B copies), applied as a stencil, with any of prune, adam and huber_delta.
+        z_prior: the latent prior of reconstruct, J = D + lambda ||z||^2 with D the measured loss and its 1/m normaliser
+        (dgan_reconstruct_measured[_csr / _conv]_prior, with any of prune, adam and huber_delta); the lambda of a
+        formulation on the unnormalised ||A G(z) - y||^2 is m times this one.  None runs the call without the prior as
+        before."""
         if isinstance(operator, ConvOperator):
             return self._reconstruct_measured_conv(measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed,
                                                    momentum, decay_lr, out, return_aux, z_row_offset, prune, adam,
-                                                   huber_delta)
+                                                   huber_delta, z_prior)
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -685,6 +749,7 @@ class NativeGenerator:
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
         delta = None if huber_delta is None else check_huber_delta(huber_delta)
+        lam = None if z_prior is None else check_z_prior(z_prior)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -703,7 +768,19 @@ class NativeGenerator:
                                   seed & (2 ** 64 - 1), int(z_row_offset))
             n_points = len(sched) if sched is not None else 0
             apr = ctypes.byref(ap) if ap is not None else None
-            if delta is not None and csr:
+            dpr = _byref_or_none(None if delta is None else ctypes.c_float(delta))
+            if lam is not None and csr:
+                rc = self.lib.dgan_reconstruct_measured_csr_prior(self._handle, ctypes.byref(prm), apr, dpr, lam, sched,
+                                                                  n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
+                                                                  _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                                                                  ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_csr_prior")
+            elif lam is not None:
+                rc = self.lib.dgan_reconstruct_measured_prior(self._handle, ctypes.byref(prm), apr, dpr, lam, sched, n_points,
+                                                              _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
+                                                              ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_prior")
+            elif delta is not None and csr:
                 rc = self.lib.dgan_reconstruct_measured_csr_huber(self._handle, ctypes.byref(prm), apr, delta, sched, n_points,
                                                                   _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
                                                                   _ptr(rec), _ptr(loss), _ptr(idx), ws, need,

@@ -327,7 +327,8 @@ struct dgan_ctx {
   // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise; adam: 1 for the Adam
   // update with beta1, beta2 and eps, 0 for momentum; huber: the Huber entries' delta, 0 for the squared error; conv:
   // a convolution operator's kh, kw, ph, pw and stride, empty otherwise - not its kernel values, which are staged outside
-  // the graph) on a private stream, replayed with one cudaGraphLaunch per call.
+  // the graph; prior: 1 for the latent prior with its lambda z_prior, 0 otherwise) on a private stream, replayed with one
+  // cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     std::vector<int> prune;
@@ -335,11 +336,12 @@ struct dgan_ctx {
     int adam = 0; float beta1 = 0.f, beta2 = 0.f, eps = 0.f;
     float huber = 0.f;
     std::vector<int> conv;
+    int prior = 0; float z_prior = 0.f;
     bool same_key(const LoopGraph& o) const {
       return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
              weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
              momentum == o.momentum && prune == o.prune && adam == o.adam && beta1 == o.beta1 && beta2 == o.beta2 &&
-             eps == o.eps && huber == o.huber && conv == o.conv;
+             eps == o.eps && huber == o.huber && conv == o.conv && prior == o.prior && z_prior == o.z_prior;
     }
   };
   std::vector<LoopGraph> graphs;
@@ -478,6 +480,10 @@ struct Workspace {
   // The data term of the call the workspace serves: the Huber loss at this delta (> 0, +inf allowed; the Huber entries),
   // or 0 for the squared error.  Set by the call, not carved: a Huber call's workspace is its counterpart's.
   float huber = 0.f;
+  // The latent prior of the call (the prior entries): each row's objective is J = D + z_prior ||z||^2 with z_prior >= 0.
+  // Set by the call, not carved: the prior term lives in `loss` between its evaluation and the loss's finish.
+  bool prior = false;
+  float z_prior = 0.f;
 };
 
 // The padded measurement count of a measured workspace: m rounded up to the measurement products' N tile.
@@ -1256,12 +1262,27 @@ static int measured_backward(dgan_ctx* c, const Workspace& w, int R, cudaStream_
   return run_backward(c, w, s);
 }
 
-// loss[n] = (1/m) sum_j r[n][j]^2, from the measurement product's parts (fixed order)
-static int measured_loss_finish(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
-  loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, s>>>(w.mloss_part, w.m_ld / kMeasTileN, 1, (size_t)w.n_pad,
-                                                            1.0f / (float)w.m, w.n_rows, w.loss);
+// w.loss[n] = inv * (the row's n_parts loss parts at part index n * stride_n + part * stride_b, fixed order); with the
+// latent prior (w.prior) the prior term prior_term_kernel left in w.loss is added (loss_finish_prior_kernel)
+static int loss_finish(dgan_ctx* c, const Workspace& w, const float* parts, int n_parts, size_t stride_n,
+                       size_t stride_b, float inv, cudaStream_t s) {
+  const unsigned grid = (unsigned)((w.n_rows + 255) / 256);
+  if (w.prior)
+    loss_finish_prior_kernel<<<grid, 256, 0, s>>>(parts, n_parts, stride_n, stride_b, inv, w.n_rows, w.loss);
+  else
+    loss_finish_kernel<<<grid, 256, 0, s>>>(parts, n_parts, stride_n, stride_b, inv, w.n_rows, w.loss);
   DGAN_LAUNCH_CHECK(c);
   return 0;
+}
+
+// loss[n] = (1/m) sum_j r[n][j]^2, from the measurement product's parts (fixed order)
+static int measured_loss_finish(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  return loss_finish(c, w, w.mloss_part, w.m_ld / kMeasTileN, 1, (size_t)w.n_pad, 1.0f / (float)w.m, s);
+}
+
+// loss[n] = (1/HWC) (sum of the image loss's parts), as the last forward left them
+static int image_loss_finish(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  return loss_finish(c, w, w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b, 1.0f / (float)c->hwc, s);
 }
 
 // fp16 path: plan and upload the schedules of every layer-direction for this many latent rows (cached in the handle).
@@ -1673,6 +1694,24 @@ static int check_huber(const float* huber) {
   return DGAN_ERR_INVALID_ARG;
 }
 
+// The prior entries' lambda: finite, >= 0, and 2 lambda finite (the gradient's coefficient, rounded on the host).
+// z_prior NULL: a call without the prior, nothing to check.  0, or DGAN_ERR_INVALID_ARG naming the bad value; the callers
+// check it after every other argument and before anything is enqueued.
+static int check_z_prior(const float* z_prior) {
+  if (z_prior == nullptr) return 0;
+  const float l = *z_prior;
+  if (std::isfinite(l) && l >= 0.f && std::isfinite(2.f * l)) return 0;
+  set_error("invalid latent prior z_prior = " + std::to_string(l) + ": it must be finite and >= 0, with 2 z_prior finite");
+  return DGAN_ERR_INVALID_ARG;
+}
+
+// The latent prior's part of a call's workspace and graph-cache key (z_prior not NULL, checked by check_z_prior).
+static void set_prior(Workspace* w, dgan_ctx::LoopGraph* key, const float* z_prior) {
+  if (z_prior == nullptr) return;
+  if (w != nullptr) { w->prior = true; w->z_prior = *z_prior; }
+  if (key != nullptr) { key->prior = 1; key->z_prior = *z_prior; }
+}
+
 // dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place.
 // huber (not NULL): dgan_loss_grad_huber, the Huber loss at *huber.
 static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
@@ -1858,9 +1897,13 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
 // w.loss_part, as the forward of iteration L-1 does (the fp16 path's last-layer forward writes them, and y, only when it
 // is asked for y).  adam (not NULL): the Adam update (adam_kernel, with m in w.v and s in w.s) instead of the momentum
 // update; on the fp16 image loss the Linear backward then runs without its momentum tail and adam_kernel follows it.
+// w.prior (the prior entries): iteration t1 - 1 first leaves each row's prior term on its z in w.loss (prior_term_kernel)
+// for the loss finish that follows the range, and every update is the prior form of its kernel (the fp16 image loss's
+// momentum runs as on the Adam path: the Linear backward without its tail, then momentum_prior_kernel).
 static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params& p, int per_image, int t0, int t1,
                          bool measured, cudaStream_t ls, bool loss_at_end = false, const dgan_adam_params* adam = nullptr) {
   const int latent = h->wd.latent;
+  const float two_lambda = 2.f * w.z_prior;     // finite: check_z_prior
   // Adam at iteration t (k = t + 1): c1 = lr_t / (1 - beta1^k) and c2 = 1 / sqrt(1 - beta2^k), in double, rounded to fp32
   auto launch_adam = [&](int t, float lr, float gmul, const float* row_scale) -> int {
     const double k = (double)t + 1.0;
@@ -1868,9 +1911,14 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
     const float c2 = (float)(1.0 / std::sqrt(1.0 - std::pow((double)adam->beta2, k)));
     const size_t zcount = (size_t)w.n_pad * latent;
     ProfScope ps(h, 2 * (int)h->layers.size() + 2, ls);     // the profile kind of the latent update
-    DGAN_CUDA_CHECK(launch_pdl(adam_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v, w.s,
-                               (const float*)w.g, w.n_g_parts, gmul, row_scale, latent, w.n_rows, adam->beta1, adam->beta2,
-                               adam->eps, c1, c2, zcount, w.z_h));
+    if (w.prior)
+      DGAN_CUDA_CHECK(launch_pdl(adam_prior_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v, w.s,
+                                 (const float*)w.g, w.n_g_parts, gmul, row_scale, latent, w.n_rows, adam->beta1,
+                                 adam->beta2, adam->eps, c1, c2, zcount, w.z_h, two_lambda));
+    else
+      DGAN_CUDA_CHECK(launch_pdl(adam_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v, w.s,
+                                 (const float*)w.g, w.n_g_parts, gmul, row_scale, latent, w.n_rows, adam->beta1,
+                                 adam->beta2, adam->eps, c1, c2, zcount, w.z_h));
     DGAN_LAUNCH_CHECK(h);
     return 0;
   };
@@ -1878,11 +1926,16 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
   // fp16: the momentum update (tf.train.MomentumOptimizer, models/gan.py:389-391) runs in the tail of the split-K Linear
   // backward - the CTA that completes a 128-row tile's partial sums applies it - so an L-step is 8 launches; bit-identical
   // to the separate kernel the fp32 path uses (same arithmetic, parts summed in the same order)
-  const bool tail = h->desc.precision == DGAN_PREC_FP16;
+  const bool tail = h->desc.precision == DGAN_PREC_FP16 && !w.prior;
   for (int t = t0; t < t1; ++t) {
     const bool last = (t == p.rec_iters - 1);
     float lr = p.rec_lr;
     if (p.decay_lr) lr = p.rec_lr * std::pow(0.1f, (float)(t / decay_iter));
+    if (w.prior && t == t1 - 1) {      // the z of the range's last iteration, before that iteration's update
+      prior_term_kernel<<<(w.n_rows + 255) / 256, 256, 0, ls>>>(w.z, latent, h->desc.latent_dim, w.n_rows, w.z_prior,
+                                                                 w.loss);
+      DGAN_LAUNCH_CHECK(h);
+    }
     // The loop returns the pre-update forward of iteration L-1 (models/gan.py:419-421, SURVEY F4):
     // the L-th update is never observed, so its backward pass is not run.
     int r2;
@@ -1897,9 +1950,13 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
         continue;
       }
       const size_t zcount = (size_t)w.n_pad * latent;
-      momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
-          w.z, w.v, w.g, w.n_g_parts, h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr, latent, w.n_rows, lr,
-          p.momentum, zcount, w.z_h);
+      const float* row_scale = h->desc.precision == DGAN_PREC_FP16 ? w.mscale : nullptr;
+      if (w.prior)
+        momentum_rows_prior_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
+            w.z, w.v, w.g, w.n_g_parts, row_scale, latent, w.n_rows, lr, p.momentum, zcount, w.z_h, two_lambda);
+      else
+        momentum_rows_kernel<<<(unsigned)((zcount + 255) / 256), 256, 0, ls>>>(
+            w.z, w.v, w.g, w.n_g_parts, row_scale, latent, w.n_rows, lr, p.momentum, zcount, w.z_h);
       DGAN_LAUNCH_CHECK(h);
       continue;
     }
@@ -1916,8 +1973,13 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
     if (!tail) {
       const size_t zcount = (size_t)w.n_pad * latent;
       ProfScope ps(h, 2 * (int)h->layers.size() + 2, ls);
-      DGAN_CUDA_CHECK(launch_pdl(momentum_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v,
-                                 (const float*)w.g, w.n_g_parts, grad_multiplier(h), lr, p.momentum, zcount, w.z_h));
+      if (w.prior)
+        DGAN_CUDA_CHECK(launch_pdl(momentum_prior_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z,
+                                   w.v, (const float*)w.g, w.n_g_parts, grad_multiplier(h), lr, p.momentum, zcount, w.z_h,
+                                   two_lambda));
+      else
+        DGAN_CUDA_CHECK(launch_pdl(momentum_kernel, dim3((unsigned)((zcount + 255) / 256)), dim3(256), 0, ls, w.z, w.v,
+                                   (const float*)w.g, w.n_g_parts, grad_multiplier(h), lr, p.momentum, zcount, w.z_h));
       DGAN_LAUNCH_CHECK(h);
     }
   }
@@ -1992,11 +2054,12 @@ static int check_adam(const dgan_adam_params* a) {
 // dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
 // weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
 // the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).  huber
-// (not NULL): the Huber entries, the Huber loss at *huber on the counterpart's workspace.
+// (not NULL): the Huber entries, the Huber loss at *huber on the counterpart's workspace.  z_prior (not NULL): the prior
+// entries, J = D + *z_prior ||z||^2 on the counterpart's workspace.
 static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                             const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                             void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                            const float* huber = nullptr) {
+                            const float* huber = nullptr, const float* z_prior = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
@@ -2010,8 +2073,9 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   Workspace w;
   int rc;
   if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr, meas.conv))) return rc;
-  if ((rc = check_huber(huber))) return rc;
+  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior))) return rc;
   if (huber != nullptr) w.huber = *huber;
+  set_prior(&w, nullptr, z_prior);
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
@@ -2033,18 +2097,13 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   set_optimizer_key(&key, adam);
   key.huber = w.huber;
   set_conv_key(&key, meas.conv);
+  set_prior(nullptr, &key, z_prior);
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
     return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls, false, adam);
   };
   if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
   {
-    const int n_rows = batch * rec_rr;
-    if (measured) {
-      if ((rc = measured_loss_finish(h, w, s))) return rc;
-    } else {
-      loss_finish_kernel<<<(n_rows + 255) / 256, 256, 0, s>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b, 1.0f / (float)h->hwc, n_rows, w.loss);
-      DGAN_LAUNCH_CHECK(h);
-    }
+    if ((rc = measured ? measured_loss_finish(h, w, s) : image_loss_finish(h, w, s))) return rc;
     select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, rec_rr, h->hwc, rec_dev, loss_dev, idx_dev);
     DGAN_LAUNCH_CHECK(h);
     enqueues += 2;
@@ -2124,12 +2183,13 @@ static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_poin
 // measured loop; the measured forward leaves each iteration's loss parts in mloss_part, so a prune point sums them as
 // the plain loop's do loss_part.  adam (not NULL, checked by the caller): the Adam entries; a prune point gathers the
 // survivors' second moment with their z, m and z_h.  huber (not NULL): the Huber entries, every stage and the ranking on
-// the Huber loss at *huber.
+// the Huber loss at *huber.  z_prior (not NULL): the prior entries, every stage and the ranking on J = D + *z_prior ||z||^2,
+// a prune point's prior term on the z of iteration iter_k - 1 (before that iteration's update, as its D).
 static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                    const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
                                    MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                                   const float* huber = nullptr) {
+                                   const float* huber = nullptr, const float* z_prior = nullptr) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
@@ -2156,11 +2216,12 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
                : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
-  if ((rc = check_huber(huber))) return rc;
+  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior))) return rc;
   for (Workspace& w : regs) {
     if ((rc = build_maps(h, w))) return rc;
     if (weighted && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
     if (huber != nullptr) w.huber = *huber;
+    set_prior(&w, nullptr, z_prior);
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t launches0 = h->launches;
@@ -2189,14 +2250,11 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   set_optimizer_key(&key, adam);
   key.huber = huber != nullptr ? *huber : 0.f;
   set_conv_key(&key, meas.conv);
+  set_prior(nullptr, &key, z_prior);
   // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
   // (measured) left
-  auto loss_finish = [&](const Workspace& w, cudaStream_t ls) -> int {
-    if (measured) return measured_loss_finish(h, w, ls);
-    loss_finish_kernel<<<(w.n_rows + 255) / 256, 256, 0, ls>>>(w.loss_part, w.n_loss_parts, w.loss_stride_n, w.loss_stride_b,
-                                                               1.0f / (float)h->hwc, w.n_rows, w.loss);
-    DGAN_LAUNCH_CHECK(h);
-    return 0;
+  auto finish = [&](const Workspace& w, cudaStream_t ls) -> int {
+    return measured ? measured_loss_finish(h, w, ls) : image_loss_finish(h, w, ls);
   };
   // the stages and, between them, the prune points: the loss of iteration iter_k - 1 per row (its parts are still in
   // loss_part or mloss_part after that iteration's update), the survivors' maps and the gather of their z, v (and z_h)
@@ -2211,7 +2269,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
       if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured, ls, k < n_points, adam))) return r2;
       if (k == n_points) break;
       const Workspace& nx = regs[(size_t)k + 1];
-      if ((r2 = loss_finish(w, ls))) return r2;
+      if ((r2 = finish(w, ls))) return r2;
       prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sched[k].keep, nx.src, nx.orig);
       DGAN_LAUNCH_CHECK(h);
       const size_t total = (size_t)nx.n_pad * h->wd.latent;
@@ -2230,7 +2288,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   const Workspace& w = regs.back();
   const int per = sched[n_points - 1].keep;
   h->n_rows_cur = w.n_rows;
-  if ((rc = loss_finish(w, s))) return rc;
+  if ((rc = finish(w, s))) return rc;
   select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, w.sel);
   DGAN_LAUNCH_CHECK(h);
   prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
@@ -2360,18 +2418,19 @@ size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, 
   return bytes;
 }
 
-// The image and measured Adam and Huber entries after their own checks: unpruned through reconstruct_impl, pruned through
-// reconstruct_pruned_impl, as their momentum and squared-error counterparts (adam NULL: momentum; huber NULL: squared error)
+// The image and measured Adam, Huber and prior entries after their own checks: unpruned through reconstruct_impl, pruned
+// through reconstruct_pruned_impl, as their momentum and squared-error counterparts (adam NULL: momentum; huber NULL:
+// squared error; z_prior NULL: no prior)
 static int reconstruct_adam_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                  const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                                  const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                  size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs(),
-                                 const float* huber = nullptr) {
+                                 const float* huber = nullptr, const float* z_prior = nullptr) {
   if (unpruned(sched, n_points))
     return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam,
-                            huber);
+                            huber, z_prior);
   return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                                 stream, meas, adam, huber);
+                                 stream, meas, adam, huber, z_prior);
 }
 
 int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2549,6 +2608,64 @@ int dgan_reconstruct_measured_conv(dgan_handle h, const dgan_rec_params* prm, co
   if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
   return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
                                ws_bytes, stream, meas, huber_delta);
+}
+
+// ---- the latent prior: each entry is its counterpart's code path with lambda = z_prior -------------------------------
+// adam NULL: momentum; huber_delta NULL: the squared error; sched NULL with n_points 0: unpruned.  The counterpart's checks
+// come first, then lambda's (check_z_prior), before anything is enqueued.
+int dgan_reconstruct_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam, const float* huber_delta,
+                           float z_prior, const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
+                           const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
+                           void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                               stream, MeasuredArgs(), huber_delta, &z_prior);
+}
+
+int dgan_reconstruct_measured_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                    const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
+                                    const float* a_dev, int m, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, &z_prior);
+}
+
+int dgan_reconstruct_measured_csr_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                        const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
+                                        const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                        const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                        int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, &z_prior);
+}
+
+int dgan_reconstruct_measured_conv_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                         const float* huber_delta, float z_prior, const dgan_prune_point* sched,
+                                         int n_points, const dgan_conv_op* op, const float* k_dev, const float* y_dev,
+                                         const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                         size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  ConvGeom g;
+  MeasuredArgs meas;
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, &z_prior);
 }
 
 int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const dgan_conv_op* op, const float* k_dev,

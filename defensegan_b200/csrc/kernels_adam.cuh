@@ -17,9 +17,14 @@ namespace dgan {
 // on the host.  eps > 0: a coordinate whose gradient is 0 on every step (padded latent columns, an image whose pixel
 // weights are all 0) keeps m = s = 0 and moves by 0 / eps = 0.  Optionally refreshes the fp16 copy of z
 // that feeds the tensor-core Linear.
-__global__ void adam_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ s, const float* __restrict__ g,
-                            int n_parts, float gmul, const float* __restrict__ row_scale, int ld, int n_rows, float b1,
-                            float b2, float eps, float c1, float c2, size_t count, __half* __restrict__ z_h) {
+// PRIOR (adam_prior_kernel, the prior entries): g = fmaf(two_lambda, z, g) on the pre-update z, the gradient of
+// J = D + lambda ||z||^2; the rest is unchanged.
+template <bool PRIOR>
+__device__ __forceinline__ void adam_body(float* __restrict__ z, float* __restrict__ m, float* __restrict__ s,
+                                          const float* __restrict__ g, int n_parts, float gmul,
+                                          const float* __restrict__ row_scale, int ld, int n_rows, float b1, float b2,
+                                          float eps, float c1, float c2, size_t count, __half* __restrict__ z_h,
+                                          float two_lambda) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -28,7 +33,8 @@ __global__ void adam_kernel(float* __restrict__ z, float* __restrict__ m, float*
   for (int p = 1; p < n_parts; ++p) gs += g[i + (size_t)p * count];   // split-K partials, fixed order
   const size_t row = i / ld;
   const float gm = row_scale != nullptr && row < (size_t)n_rows ? gmul / row_scale[row] : gmul;
-  const float gg = gm * gs;
+  float gg = gm * gs;
+  if (PRIOR) gg = fmaf(two_lambda, z[i], gg);
   const float mm = fmaf(b1, m[i], (1.f - b1) * gg);
   const float ss = fmaf(b2, s[i], (1.f - b2) * (gg * gg));
   const float zz = z[i] - (c1 * mm) / fmaf(sqrtf(ss), c2, eps);
@@ -36,6 +42,19 @@ __global__ void adam_kernel(float* __restrict__ z, float* __restrict__ m, float*
   s[i] = ss;
   z[i] = zz;
   if (z_h != nullptr) z_h[i] = __float2half_rn(zz);
+}
+
+__global__ void adam_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ s, const float* __restrict__ g,
+                            int n_parts, float gmul, const float* __restrict__ row_scale, int ld, int n_rows, float b1,
+                            float b2, float eps, float c1, float c2, size_t count, __half* __restrict__ z_h) {
+  adam_body<false>(z, m, s, g, n_parts, gmul, row_scale, ld, n_rows, b1, b2, eps, c1, c2, count, z_h, 0.f);
+}
+
+__global__ void adam_prior_kernel(float* __restrict__ z, float* __restrict__ m, float* __restrict__ s,
+                                  const float* __restrict__ g, int n_parts, float gmul, const float* __restrict__ row_scale,
+                                  int ld, int n_rows, float b1, float b2, float eps, float c1, float c2, size_t count,
+                                  __half* __restrict__ z_h, float two_lambda) {
+  adam_body<true>(z, m, s, g, n_parts, gmul, row_scale, ld, n_rows, b1, b2, eps, c1, c2, count, z_h, two_lambda);
 }
 
 // prune_gather_kernel with Adam's second state: the survivors' z, m (in v), s and (fp16 path, z_h != NULL) z_h into the

@@ -228,21 +228,36 @@ measured_gemm_huber_kernel(const float* __restrict__ X, int ldx, int M, const fl
 // The momentum update of tf.train.MomentumOptimizer (as momentum_kernel) with a multiplier per latent row: the gradient of
 // row i / ld is g / row_scale[row] (the fp16 path's power-of-two cotangent scales, so the division is exact), or g itself
 // when row_scale is NULL (the fp32 path) and on the tile-padding rows (>= n_rows: no scale, and a gradient of 0).  The
-// measured loop's d(pre) already carries the 2/m of its loss.
-__global__ void momentum_rows_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g, int n_parts,
-                                     const float* __restrict__ row_scale, int ld, int n_rows, float lr, float mu,
-                                     size_t count, __half* __restrict__ z_h) {
+// measured loop's d(pre) already carries the 2/m of its loss.  PRIOR (momentum_rows_prior_kernel, the prior entries): the
+// gradient of J = D + lambda ||z||^2, g = fmaf(two_lambda, z, g) on the pre-update z after the scale is divided out.
+template <bool PRIOR>
+__device__ __forceinline__ void momentum_rows_body(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g,
+                                                   int n_parts, const float* __restrict__ row_scale, int ld, int n_rows,
+                                                   float lr, float mu, size_t count, __half* __restrict__ z_h,
+                                                   float two_lambda) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   float gs = g[i];
   for (int p = 1; p < n_parts; ++p) gs += g[i + (size_t)p * count];   // split-K partials, fixed order
   const size_t row = i / ld;
   const float gmul = row_scale != nullptr && row < (size_t)n_rows ? 1.f / row_scale[row] : 1.f;
-  const float vv = fmaf(mu, v[i], gmul * gs);
+  const float vv = fmaf(mu, v[i], PRIOR ? fmaf(two_lambda, z[i], gmul * gs) : gmul * gs);
   const float zz = z[i] - lr * vv;
   v[i] = vv;
   z[i] = zz;
   if (z_h != nullptr) z_h[i] = __float2half_rn(zz);
+}
+
+__global__ void momentum_rows_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g, int n_parts,
+                                     const float* __restrict__ row_scale, int ld, int n_rows, float lr, float mu,
+                                     size_t count, __half* __restrict__ z_h) {
+  momentum_rows_body<false>(z, v, g, n_parts, row_scale, ld, n_rows, lr, mu, count, z_h, 0.f);
+}
+
+__global__ void momentum_rows_prior_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g,
+                                           int n_parts, const float* __restrict__ row_scale, int ld, int n_rows, float lr,
+                                           float mu, size_t count, __half* __restrict__ z_h, float two_lambda) {
+  momentum_rows_body<true>(z, v, g, n_parts, row_scale, ld, n_rows, lr, mu, count, z_h, two_lambda);
 }
 
 }  // namespace dgan

@@ -314,20 +314,37 @@ final_bwd_kernel(const float* __restrict__ dpre /*[n_pad][P_out*C_OUT]*/, int n_
 //   v <- mu*v + g ;  z <- z - lr*v,   g = gmul * (accumulated J^T dpre)
 // gmul carries the 2/(HWC) of the mean (gan.py:411-413) and undoes any fp16 gradient scaling.
 // Optionally refreshes the fp16 copy of z that feeds the tensor-core Linear.
+// PRIOR (momentum_prior_kernel, the prior entries): the gradient of J = D + lambda ||z||^2, g = fmaf(two_lambda, z, g)
+// on the pre-update z, with two_lambda = 2 lambda rounded on the host.
 // ------------------------------------------------------------------------------------------
-__global__ void momentum_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g, int n_parts,
-                                float gmul, float lr, float mu, size_t count, __half* __restrict__ z_h) {
+template <bool PRIOR>
+__device__ __forceinline__ void momentum_body(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g,
+                                              int n_parts, float gmul, float lr, float mu, size_t count,
+                                              __half* __restrict__ z_h, float two_lambda) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   float gs = g[i];
   for (int p = 1; p < n_parts; ++p) gs += g[i + (size_t)p * count];   // split-K partials, fixed order
-  const float vv = fmaf(mu, v[i], gmul * gs);
+  float gg = gmul * gs;
+  if (PRIOR) gg = fmaf(two_lambda, z[i], gg);
+  const float vv = fmaf(mu, v[i], gg);
   const float zz = z[i] - lr * vv;
   v[i] = vv;
   z[i] = zz;
   if (z_h != nullptr) z_h[i] = __float2half_rn(zz);
+}
+
+__global__ void momentum_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g, int n_parts,
+                                float gmul, float lr, float mu, size_t count, __half* __restrict__ z_h) {
+  momentum_body<false>(z, v, g, n_parts, gmul, lr, mu, count, z_h, 0.f);
+}
+
+__global__ void momentum_prior_kernel(float* __restrict__ z, float* __restrict__ v, const float* __restrict__ g,
+                                      int n_parts, float gmul, float lr, float mu, size_t count, __half* __restrict__ z_h,
+                                      float two_lambda) {
+  momentum_body<true>(z, v, g, n_parts, gmul, lr, mu, count, z_h, two_lambda);
 }
 
 // Philox4x32-10 counter-based generator (public algorithm, Salmon et al. 2011) + Box-Muller.
@@ -380,13 +397,41 @@ __global__ void init_z_kernel(float* __restrict__ z, float* __restrict__ v, __ha
 }
 
 // loss[n] = (sum of band partials, fixed order) / (H*W*C)            (models/gan.py:411-413)
-__global__ void loss_finish_kernel(const float* __restrict__ loss_part, int n_bands, size_t stride_n, size_t stride_b,
-                                   float inv_hwc, int n_rows, float* __restrict__ loss) {
+// PRIOR (loss_finish_prior_kernel): loss[n] holds the row's prior term p (prior_term_kernel) on entry and receives
+// J = D + p, one fp32 add after the rounded D.
+template <bool PRIOR>
+__device__ __forceinline__ void loss_finish_body(const float* __restrict__ loss_part, int n_bands, size_t stride_n,
+                                                 size_t stride_b, float inv_hwc, int n_rows, float* __restrict__ loss) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= n_rows) return;
   float s = 0.f;
   for (int b = 0; b < n_bands; ++b) s += loss_part[(size_t)n * stride_n + (size_t)b * stride_b];
-  loss[n] = s * inv_hwc;
+  if (PRIOR) loss[n] = __fadd_rn(__fmul_rn(s, inv_hwc), loss[n]);
+  else loss[n] = s * inv_hwc;
+}
+
+__global__ void loss_finish_kernel(const float* __restrict__ loss_part, int n_bands, size_t stride_n, size_t stride_b,
+                                   float inv_hwc, int n_rows, float* __restrict__ loss) {
+  loss_finish_body<false>(loss_part, n_bands, stride_n, stride_b, inv_hwc, n_rows, loss);
+}
+
+__global__ void loss_finish_prior_kernel(const float* __restrict__ loss_part, int n_bands, size_t stride_n,
+                                         size_t stride_b, float inv_hwc, int n_rows, float* __restrict__ loss) {
+  loss_finish_body<true>(loss_part, n_bands, stride_n, stride_b, inv_hwc, n_rows, loss);
+}
+
+// The latent prior's term of each real row (the prior entries): p[n] = lambda * sum_{j < latent} z[n][j]^2, the sum one
+// fmaf chain from +0 in ascending column j over the real latent columns (z is [n_pad][ld]).  Launched on the z the data
+// term of the same evaluation is computed on; p lands in the workspace's per-row loss, which loss_finish_prior_kernel
+// then completes.
+__global__ void prior_term_kernel(const float* __restrict__ z, int ld, int latent, int n_rows, float lambda,
+                                  float* __restrict__ p) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= n_rows) return;
+  const float* zr = z + (size_t)n * ld;
+  float acc = 0.f;
+  for (int j = 0; j < latent; ++j) acc = fmaf(zr[j], zr[j], acc);
+  p[n] = lambda * acc;
 }
 
 // Arg-min restart per image and gather (models/gan.py:438-449): lowest index wins ties

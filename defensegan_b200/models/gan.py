@@ -125,6 +125,7 @@ class DefenseGANBase(object):
         self.rec_adam_betas = (0.9, 0.999)  # Adam's (beta1, beta2) (cfg REC_ADAM_BETAS), read with rec_optimizer "adam"
         self.rec_adam_eps = 1e-8           # Adam's eps (cfg REC_ADAM_EPS)
         self.rec_huber_delta = None        # data term: None = squared error (the reference's) | Huber delta > 0 (cfg REC_HUBER_DELTA)
+        self.rec_z_prior = None            # latent prior: None = none (the reference's) | lambda >= 0 of D + lambda ||z||^2 (cfg REC_Z_PRIOR)
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
 
         self.test_mode = test_mode
@@ -367,10 +368,20 @@ class DefenseGANBase(object):
         rho = 2 huber_loss, so delta = +inf, or delta >= 2 on images in the generator's output range, gives the squared
         error's bits.  With momentum the gradient of clipped residuals shrinks with delta, so rec_lr has to grow as delta
         falls; with rec_optimizer "adam" it does not.  It combines with pixel_weights, rec_prune and Adam, and is checked
-        before any native call (a ValueError naming the bad value)."""
+        before any native call (a ValueError naming the bad value).
+
+        `rec_z_prior` (an extension, read at call time; None by default, the reference's loss alone): a lambda >= 0 adds a
+        Gaussian prior on z, so each restart minimises J = D + lambda ||z||^2 with D the data term above.  It keeps z where
+        the generator was trained, so G(z) cannot fit noise or an adversarial perturbation with a latent of a norm the
+        generator never saw.  D keeps its 1/HWC normaliser, so lambda is relative to the mean loss: the lambda of a
+        formulation on the unnormalised sum does not carry over.  The returned loss is J (the detection statistic then
+        includes the prior), the chosen restart is J's arg-min and rec_prune ranks by J.  lambda = 0 gives the bits of
+        the call without it.  It combines with pixel_weights, rec_prune, Adam and rec_huber_delta, and is checked before
+        any native call (a ValueError naming the bad value)."""
         prune = self._prune_schedule()
         adam = self._adam_params()
         huber = self._huber_delta()
+        prior = self._z_prior()
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
@@ -387,6 +398,8 @@ class DefenseGANBase(object):
             kw["adam"] = adam
         if huber is not None:
             kw["huber_delta"] = huber
+        if prior is not None:
+            kw["z_prior"] = prior
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
@@ -427,6 +440,15 @@ class DefenseGANBase(object):
         except ValueError as e:
             raise ValueError("rec_huber_delta: %s" % e) from None
 
+    def _z_prior(self):
+        """`rec_z_prior` checked (None when unset): a finite float >= 0; ValueError before any native call."""
+        if self.rec_z_prior is None:
+            return None
+        try:
+            return _native.check_z_prior(self.rec_z_prior)
+        except ValueError as e:
+            raise ValueError("rec_z_prior: %s" % e) from None
+
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
                              z_row_offset=0, prune=_NOT_GIVEN):
         """Projection onto the generator's range from linear measurements (an extension; the reference has none), for
@@ -466,9 +488,15 @@ class DefenseGANBase(object):
         with one kernel for every image or one per image (deblurring photos with their own point-spread functions), applied
         as a stencil.  m is its num_measurements(image_dim); a per-image kernel count must equal B.  On both precisions
         the result is bit-identical to the call with its to_sparse_csr matrix (one call per image for per-image kernels),
-        and it runs with prune, rec_optimizer and rec_huber_delta as the other operator kinds do."""
+        and it runs with prune, rec_optimizer and rec_huber_delta as the other operator kinds do.
+
+        `rec_z_prior` is read at call time as in `reconstruct`: a lambda >= 0 adds lambda ||z||^2 to the measured loss,
+        (1/m) ||A G(z) - y||^2 + lambda ||z||^2 - the latent prior of compressed sensing with generative models, with the
+        data term normalised by m (the lambda of the unnormalised formulation is m times this one) - for every operator
+        kind, pruned or not."""
         adam = self._adam_params()
         huber = self._huber_delta()
+        prior = self._z_prior()
         if prune is _NOT_GIVEN:
             if self.rec_prune is not None:
                 raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts from it: set "
@@ -481,10 +509,10 @@ class DefenseGANBase(object):
             prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
         if isinstance(operator, ConvOperator):
             return self._reconstruct_measured_conv(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                   z_row_offset, prune, adam, huber)
+                                                   z_row_offset, prune, adam, huber, prior)
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                     z_row_offset, prune, adam, huber)
+                                                     z_row_offset, prune, adam, huber, prior)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -505,15 +533,17 @@ class DefenseGANBase(object):
         kw = {} if adam is None else {"adam": adam}
         if huber is not None:
             kw["huber_delta"] = huber
+        if prior is not None:
+            kw["z_prior"] = prior
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
                                            **kw)
 
     def _reconstruct_measured_conv(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                   prune, adam=None, huber=None):
-        """reconstruct_measured for a ConvOperator, after one check of the kernels and the measurements (prune, adam and
-        huber as in _reconstruct_measured_sparse).  The native call gets the kernels broadcast to [B, kh, kw]."""
+                                   prune, adam=None, huber=None, prior=None):
+        """reconstruct_measured for a ConvOperator, after one check of the kernels and the measurements (prune, adam,
+        huber and prior as in _reconstruct_measured_sparse).  The native call gets the kernels broadcast to [B, kh, kw]."""
         m = operator.num_measurements(self.image_dim)
         y = self._as_cuda(measurements)
         if y.dim() != 2 or y.shape[1] != m or y.shape[0] == 0:
@@ -536,16 +566,18 @@ class DefenseGANBase(object):
         kw = {} if adam is None else {"adam": adam}
         if huber is not None:
             kw["huber_delta"] = huber
+        if prior is not None:
+            kw["z_prior"] = prior
         return native.reconstruct_measured(y, operator._with_kernels(k), int(self.rec_rr), int(self.rec_iters),
                                            float(self.rec_lr), z_init_val=z0, seed=seed,
                                            momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                            return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune, **kw)
 
     def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                     prune, adam=None, huber=None):
+                                     prune, adam=None, huber=None, prior=None):
         """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements
         (prune: the checked schedule, or None; adam: the checked Adam parameters, or None; huber: the checked Huber delta,
-        or None)."""
+        or None; prior: the checked latent prior's lambda, or None)."""
         a = operator
         if a.layout == torch.sparse_coo:
             if a.dim() != 2 or a.dense_dim() != 0:
@@ -590,6 +622,8 @@ class DefenseGANBase(object):
         kw = {} if adam is None else {"adam": adam}
         if huber is not None:
             kw["huber_delta"] = huber
+        if prior is not None:
+            kw["z_prior"] = prior
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
@@ -622,10 +656,11 @@ class DefenseGANBase(object):
 
     def rec_cache_dir(self, split: str, max_num: int = -1) -> str:
         """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]
-        [_adam{b1:g}-{b2:g}-{eps:g}][_huber{delta:g}]/<split>[_debug]` - the directory name the callers parse back with
-        `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the `_prune` part (only with `rec_prune` set) keeps pruned
-        and unpruned reconstructions apart, the `_adam` part (only with rec_optimizer "adam") Adam's from momentum's, and
-        the `_huber` part (only with rec_huber_delta set) the Huber loss's from the squared error's."""
+        [_adam{b1:g}-{b2:g}-{eps:g}][_huber{delta:g}][_zprior{lambda:g}]/<split>[_debug]` - the directory name the callers
+        parse back with `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the `_prune` part (only with `rec_prune` set)
+        keeps pruned and unpruned reconstructions apart, the `_adam` part (only with rec_optimizer "adam") Adam's from
+        momentum's, the `_huber` part (only with rec_huber_delta set) the Huber loss's from the squared error's, and the
+        `_zprior` part (only with rec_z_prior set) those with the latent prior from those without."""
         if max_num > 0:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}_num{:d}'.format(int(self.rec_rr), float(self.rec_lr),
                                                                    int(self.rec_iters), int(max_num))
@@ -639,6 +674,9 @@ class DefenseGANBase(object):
         huber = self._huber_delta()
         if huber is not None:
             name += '_huber{:g}'.format(huber)
+        prior = self._z_prior()
+        if prior is not None:
+            name += '_zprior{:g}'.format(prior)
         out = os.path.join(self.checkpoint_dir, name, split)
         if self.debug:
             out += '_debug'

@@ -490,6 +490,60 @@ int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const 
                                  const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
                                  float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream);
 
+/* The projection with a Gaussian prior on the latent vector (an extension: the reference has none; compressed sensing with
+ * generative models adds it to keep z where the generator was trained).  For lambda = z_prior (fp32, finite, >= 0, and
+ * 2 lambda finite) each restart minimises
+ *   J(z) = D(z) + lambda ||z||^2
+ * where D is the counterpart's data term exactly as it computes it (squared error or Huber, weighted or not, image or
+ * measured), with its normaliser 1/(H*W*C) or 1/m: lambda is relative to the normalised data term, so the lambda of a
+ * formulation on the unnormalised ||A G(z) - y||^2 does not carry over (divide it by m).
+ *   - ||z||^2 runs over the latent_dim real columns in fp32 as one fmaf chain from +0 in ascending column order;
+ *     p = lambda * sum, J = D + p as one fp32 add.
+ *   - The update takes g' = fmaf(2 lambda, z, g) instead of the counterpart's gradient g (after its multiplier, and with
+ *     DGAN_PREC_FP16's measured row scales divided out; split-K parts summed in the same order), on the pre-update z,
+ *     with 2 lambda rounded on the host.  The momentum or Adam arithmetic that follows is the counterpart's.  Padded
+ *     latent columns stay 0.
+ *   - J is evaluated on the z its D is computed on: the z of iteration L-1 for loss_dev and the arg-min select, and at a
+ *     prune point the z of iteration iter_k - 1, before that iteration's update.  J is what loss_dev, the select (ties,
+ *     NaN rule) and the prune ranking use; rec_dev is G(z) of the chosen restart.
+ *   - lambda = 0 gives the counterpart's rec_dev, loss_dev and idx_dev bit for bit.
+ *   - use_bn is allowed unpruned (the prior is per row); with a schedule it is refused as by the counterpart.
+ * Each entry runs its counterpart's code path with the counterpart's option arguments: adam NULL for momentum, else the
+ * Adam update of dgan_reconstruct_adam; huber_delta NULL for the squared error, else the Huber loss of
+ * dgan_reconstruct_huber at *huber_delta; sched NULL with n_points 0 unpruned, else the restart pruning of the pruned
+ * entries.  Workspace: the counterpart's (dgan_workspace_bytes[_weighted / _pruned / _adam] and their measured forms);
+ * the prior needs no buffer of its own.  A lambda that is NaN, infinite or negative, or whose double 2 lambda overflows fp32:
+ * DGAN_ERR_INVALID_ARG naming the value, checked after the counterpart's checks and before anything is enqueued.
+ * Counts: dgan_last_enqueue_count is the counterpart's.  dgan_last_launch_count is the counterpart's + 1 + P (the prior
+ * term, at iteration L-1 and at each of P prune points), + L - 1 on the DGAN_PREC_FP16 image loss with momentum, whose
+ * update then runs as a kernel of its own after the Linear backward, as Adam's does.  The graph cache keys on lambda.
+ *
+ * dgan_reconstruct_prior: the image loss; w_dev NULL for dgan_reconstruct's loss, else dgan_reconstruct_weighted's. */
+int dgan_reconstruct_prior(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                           const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
+                           const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                           int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured (a dense operator) with the latent prior of dgan_reconstruct_prior. */
+int dgan_reconstruct_measured_prior(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                    const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
+                                    const float* a_dev, int m, const float* y_dev, const float* z0_dev, float* rec_dev,
+                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured_csr with the latent prior of dgan_reconstruct_prior. */
+int dgan_reconstruct_measured_csr_prior(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                        const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
+                                        const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                        const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                        int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured_conv with the latent prior of dgan_reconstruct_prior. */
+int dgan_reconstruct_measured_conv_prior(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                         const float* huber_delta, float z_prior, const dgan_prune_point* sched,
+                                         int n_points, const dgan_conv_op* op, const float* k_dev, const float* y_dev,
+                                         const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                         size_t ws_bytes, void* stream);
+
 /* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
  *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
  *   y_dev [n_rows, H*W*C] = G(z) (nullable; bit-identical to dgan_forward).  The forward is recomputed.
@@ -520,13 +574,15 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * An Adam call (dgan_reconstruct_adam, dgan_reconstruct_measured[_csr]_adam) runs as many as its momentum counterpart,
  * plus L - 1 on the DGAN_PREC_FP16 image loss, whose Adam update is a kernel of its own.  A Huber call
  * (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber) runs as many as its squared-error counterpart.  A
- * dgan_reconstruct_measured_conv call runs 4 fewer than the dgan_reconstruct_measured_csr call with the same options. */
+ * dgan_reconstruct_measured_conv call runs 4 fewer than the dgan_reconstruct_measured_csr call with the same options.  A
+ * prior call (dgan_reconstruct[_measured[_csr / _conv]]_prior) runs its counterpart's + 1 + P with P prune points, + L - 1
+ * on the DGAN_PREC_FP16 image loss with momentum. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
  * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
  * nnz, prune schedule, optimiser: momentum, or Adam with its beta1, beta2 and eps, and data term: the squared error, or
- * the Huber loss with its delta) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * the Huber loss with its delta, and latent prior: none, or lambda) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
  * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them;
  * convolution-measured calls: the one that stages the kernels and y), graph, loss sum, arg-min select.  A convolution
  * operator's geometry is part of the key; its kernel values are not. */
