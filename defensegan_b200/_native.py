@@ -50,6 +50,9 @@ ABI_SYMBOLS = [
     "dgan_conv_op_m", "dgan_workspace_bytes_measured_conv", "dgan_reconstruct_measured_conv", "dgan_loss_grad_measured_conv",
     "dgan_reconstruct_prior", "dgan_reconstruct_measured_prior", "dgan_reconstruct_measured_csr_prior",
     "dgan_reconstruct_measured_conv_prior",
+    "dgan_workspace_bytes_sparse_dev", "dgan_workspace_bytes_measured_sparse_dev", "dgan_reconstruct_sparse_dev",
+    "dgan_reconstruct_measured_sparse_dev", "dgan_reconstruct_measured_csr_sparse_dev",
+    "dgan_reconstruct_measured_conv_sparse_dev",
 ]
 
 
@@ -75,6 +78,10 @@ class dgan_adam_params(ctypes.Structure):
 class dgan_conv_op(ctypes.Structure):
     _fields_ = [("kh", ctypes.c_int32), ("kw", ctypes.c_int32), ("pad_h", ctypes.c_int32), ("pad_w", ctypes.c_int32),
                 ("stride", ctypes.c_int32)]
+
+
+class dgan_sparse_dev(ctypes.Structure):
+    _fields_ = [("l1", ctypes.c_float), ("step", ctypes.c_float)]
 
 
 ABI_VERSION = 2
@@ -135,6 +142,39 @@ def check_z_prior(z_prior):
     if not (np.isfinite(lam) and lam >= 0.0 and np.isfinite(two)):
         raise ValueError("z_prior = %r must be finite and >= 0, with 2 z_prior finite in fp32" % (z_prior,))
     return float(lam)
+
+
+def check_sparse_dev(sparse_dev, n: Optional[int] = None):
+    """Sparse deviations' (l1, step) as a tuple of floats, after the rules of dgan_reconstruct_sparse_dev: both as fp32
+    (the type the library reads) finite and >= 0; with n (H*W*C for the image loss, m for a measured one) also
+    eta = step n / 2 and tau = eta l1, in double, finite in fp32.  A ValueError names the bad value."""
+    try:
+        vals = tuple(sparse_dev)
+    except TypeError:
+        raise ValueError("sparse_dev is an (l1, step) pair, got %r" % (sparse_dev,)) from None
+    if len(vals) != 2:
+        raise ValueError("sparse_dev is an (l1, step) pair, got %r" % (sparse_dev,))
+    out = []
+    for name, v in zip(("l1", "step"), vals):
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.integer, np.floating)):
+            raise ValueError("sparse_dev %s = %r is not a number" % (name, v))
+        try:
+            with np.errstate(over="ignore"):   # beyond fp32's range: +-inf, as the library would read it
+                f = float(np.float32(v))
+        except OverflowError:                  # an int beyond a double's range
+            f = float("inf")
+        if not (np.isfinite(f) and f >= 0.0):
+            raise ValueError("sparse_dev %s = %r must be finite and >= 0" % (name, v))
+        out.append(f)
+    l1, step = out
+    if n is not None:
+        eta = step * float(n) / 2.0
+        with np.errstate(over="ignore"):
+            if not np.isfinite(np.float32(eta)):
+                raise ValueError("sparse_dev step = %r: eta = step * n / 2 = %r overflows fp32" % (vals[1], eta))
+            if not np.isfinite(np.float32(eta * l1)):
+                raise ValueError("sparse_dev l1 = %r: tau = eta * l1 = %r overflows fp32" % (vals[0], eta * l1))
+    return l1, step
 
 
 def check_prune_schedule(prune, rec_rr: int, rec_iters: int):
@@ -325,6 +365,22 @@ def load_library() -> ctypes.CDLL:
     lib.dgan_reconstruct_measured_conv_prior.restype = i32
     lib.dgan_reconstruct_measured_conv_prior.argtypes = [vp, rp, ap, fp, f32, pp, i32, cp, vp, vp, vp, vp, vp, vp, vp, sz,
                                                          vp]
+    sdp = ctypes.POINTER(dgan_sparse_dev)
+    lib.dgan_workspace_bytes_sparse_dev.restype = sz
+    lib.dgan_workspace_bytes_sparse_dev.argtypes = [vp, i32, i32, i32, i32, pp, i32]
+    lib.dgan_workspace_bytes_measured_sparse_dev.restype = sz
+    lib.dgan_workspace_bytes_measured_sparse_dev.argtypes = [vp, i32, i32, i32, i32, cp, i32, pp, i32]
+    lib.dgan_reconstruct_sparse_dev.restype = i32
+    lib.dgan_reconstruct_sparse_dev.argtypes = [vp, rp, ap, fp, fp, pp, i32, sdp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_sparse_dev.restype = i32
+    lib.dgan_reconstruct_measured_sparse_dev.argtypes = [vp, rp, ap, fp, fp, pp, i32, sdp, vp, vp, i32, vp, vp, vp, vp, vp,
+                                                         vp, sz, vp]
+    lib.dgan_reconstruct_measured_csr_sparse_dev.restype = i32
+    lib.dgan_reconstruct_measured_csr_sparse_dev.argtypes = [vp, rp, ap, fp, fp, pp, i32, sdp, vp, vp, vp, vp, i32, i32, vp,
+                                                             vp, vp, vp, vp, vp, sz, vp]
+    lib.dgan_reconstruct_measured_conv_sparse_dev.restype = i32
+    lib.dgan_reconstruct_measured_conv_sparse_dev.argtypes = [vp, rp, ap, fp, fp, pp, i32, sdp, vp, cp, vp, vp, vp, vp, vp,
+                                                              vp, vp, sz, vp]
     lib.dgan_sample_z0.argtypes = [vp, u64, u64, i32, vp, vp]
     lib.dgan_forward.restype = i32
     lib.dgan_forward.argtypes = [vp, vp, i32, vp, vp, sz, vp]
@@ -445,8 +501,16 @@ class NativeGenerator:
 
     # -- helpers -------------------------------------------------------------------------
     def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None,
-                   adam: bool = False, conv: Optional[dgan_conv_op] = None):
-        if conv is not None:
+                   adam: bool = False, conv: Optional[dgan_conv_op] = None, sdev: bool = False):
+        n_points = len(sched) if sched is not None else 0
+        if sdev and (m > 0 or conv is not None):
+            need = int(self.lib.dgan_workspace_bytes_measured_sparse_dev(
+                self._handle, batch, rec_rr, int(m), int(nnz), ctypes.byref(conv) if conv is not None else None, int(adam),
+                sched, n_points))
+        elif sdev:
+            need = int(self.lib.dgan_workspace_bytes_sparse_dev(self._handle, batch, rec_rr, int(weighted), int(adam), sched,
+                                                                n_points))
+        elif conv is not None:
             need = int(self.lib.dgan_workspace_bytes_measured_conv(self._handle, batch, rec_rr, ctypes.byref(conv), sched,
                                                                    len(sched) if sched is not None else 0, int(adam)))
         elif adam and m > 0:
@@ -512,7 +576,8 @@ class NativeGenerator:
                     decay_lr: bool = False, out: Optional[torch.Tensor] = None, return_aux: bool = False,
                     z_row_offset: int = 0, pixel_weights: Optional[torch.Tensor] = None,
                     prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
-                    huber_delta: Optional[float] = None, z_prior: Optional[float] = None):
+                    huber_delta: Optional[float] = None, z_prior: Optional[float] = None, sparse_dev=None,
+                    deviation_out: Optional[torch.Tensor] = None):
         """pixel_weights ([B,H,W,C], finite, in [0, 1]; the values are not checked here - DefenseGANBase.reconstruct does):
         the projection minimises the weighted loss (1/HWC) sum_p w_p (G(z)_p - x_p)^2 instead
         (dgan_reconstruct_weighted).
@@ -532,7 +597,14 @@ class NativeGenerator:
         huber_delta).  D keeps its 1/HWC normaliser, so lambda is relative to the mean loss: the lambda of a formulation on
         the unnormalised sum does not carry over.  The returned loss is J, the restart is J's arg-min and prune ranks by
         J.  0.0 runs the prior entry and gives the bits of the call without it; None runs the call without the prior,
-        through exactly the entry and arguments it always did."""
+        through exactly the entry and arguments it always did.
+        sparse_dev ((l1, step), see check_sparse_dev): fit G(z) + nu with an l1 penalty on a per-pixel deviation nu
+        (Sparse-Gen; dgan_reconstruct_sparse_dev, with any of pixel_weights, prune, adam, huber_delta and z_prior): a few
+        pixels G cannot produce (occluders, dead pixels, impulse noise) go into nu instead of dragging z.  The returned
+        image stays G(z) of the chosen restart, the returned loss is J = D(G(z) + nu) [+ lambda ||z||^2] + l1 ||nu||_1;
+        deviation_out (a [B,H,W,C] float32 CUDA tensor, 16-byte aligned) receives that restart's nu.  step = 1 with the
+        squared error is the exact minimiser over nu per step, which treats residuals beyond l1 * H*W*C / 2 as
+        deviations.  None runs the call without deviations, through exactly the entry and arguments it always did."""
         x = _require_cuda_f32(images, "images")
         batch = x.shape[0]
         if x.numel() != batch * self.hwc:
@@ -544,6 +616,7 @@ class NativeGenerator:
         ap = self._adam(adam)
         delta = None if huber_delta is None else check_huber_delta(huber_delta)
         lam = None if z_prior is None else check_z_prior(z_prior)
+        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, self.hwc)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -556,11 +629,20 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched, adam=ap is not None)
+            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched, adam=ap is not None,
+                                       sdev=sd is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if lam is not None:
+            if sd is not None:
+                rc = self.lib.dgan_reconstruct_sparse_dev(
+                    self._handle, ctypes.byref(prm), _byref_or_none(ap),
+                    _byref_or_none(None if delta is None else ctypes.c_float(delta)),
+                    _byref_or_none(None if lam is None else ctypes.c_float(lam)), sched,
+                    len(sched) if sched is not None else 0, ctypes.byref(sd), _ptr(dev), _ptr(x), _ptr(pw), _ptr(z0),
+                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_sparse_dev")
+            elif lam is not None:
                 rc = self.lib.dgan_reconstruct_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
                                                      _byref_or_none(None if delta is None else ctypes.c_float(delta)), lam,
                                                      sched, len(sched) if sched is not None else 0, _ptr(x), _ptr(pw),
@@ -605,6 +687,26 @@ class NativeGenerator:
             raise ValueError("restart pruning is not supported with use_bn: the batch statistics couple the rows")
         points = check_prune_schedule(prune, int(rec_rr), int(rec_iters))
         return (dgan_prune_point * len(points))(*[dgan_prune_point(it, keep) for it, keep in points])
+
+    def _sparse_dev(self, sparse_dev, deviation_out, batch: int, n: int):
+        """(dgan_sparse_dev or None, deviation_out or None) for the sparse-deviation entries: sparse_dev checked with
+        check_sparse_dev for n values per row (H*W*C, or the measured m); deviation_out, which needs sparse_dev, a
+        contiguous CUDA float32 tensor of batch * H*W*C elements, 16-byte aligned."""
+        if sparse_dev is None:
+            if deviation_out is not None:
+                raise ValueError("deviation_out needs sparse_dev: without deviations there is nothing to return")
+            return None, None
+        sd = dgan_sparse_dev(*check_sparse_dev(sparse_dev, n))
+        if deviation_out is not None:
+            d = deviation_out
+            if not (isinstance(d, torch.Tensor) and d.is_cuda and d.dtype == torch.float32 and d.is_contiguous() and
+                    d.numel() == batch * self.hwc):
+                raise ValueError("deviation_out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements"
+                                 % self.image_dim)
+            if d.data_ptr() % 16 != 0:
+                raise ValueError("deviation_out must be 16-byte aligned: its data starts %d bytes past a 16-byte boundary"
+                                 % (d.data_ptr() % 16))
+        return sd, deviation_out
 
     @staticmethod
     def _adam(adam):
@@ -664,9 +766,10 @@ class NativeGenerator:
         return y, k, op, batch, m
 
     def _reconstruct_measured_conv(self, measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed, momentum,
-                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta, z_prior):
+                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta, z_prior, sparse_dev,
+                                   deviation_out):
         """reconstruct_measured for a ConvOperator (dgan_reconstruct_measured_conv, or dgan_reconstruct_measured_conv_prior
-        with z_prior)."""
+        with z_prior, or dgan_reconstruct_measured_conv_sparse_dev with sparse_dev)."""
         y, k, op, batch, m = self._measured_conv(measurements, operator)
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
@@ -674,6 +777,7 @@ class NativeGenerator:
         ap = self._adam(adam)
         delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
         lam = None if z_prior is None else check_z_prior(z_prior)
+        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, m)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -686,12 +790,19 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, sched=sched, adam=ap is not None, conv=op)
+            ws, need = self._workspace(batch, rec_rr, m=m, sched=sched, adam=ap is not None, conv=op, sdev=sd is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
             n_points = len(sched) if sched is not None else 0
-            if lam is not None:
+            if sd is not None:
+                rc = self.lib.dgan_reconstruct_measured_conv_sparse_dev(
+                    self._handle, ctypes.byref(prm), _byref_or_none(ap), _byref_or_none(delta),
+                    _byref_or_none(None if lam is None else ctypes.c_float(lam)), sched, n_points, ctypes.byref(sd),
+                    _ptr(dev), ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
+                    ctypes.c_void_p(stream))
+                _check(self.lib, rc, "dgan_reconstruct_measured_conv_sparse_dev")
+            elif lam is not None:
                 rc = self.lib.dgan_reconstruct_measured_conv_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
                                                                    _byref_or_none(delta), lam, sched, n_points,
                                                                    ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0), _ptr(rec),
@@ -714,7 +825,8 @@ class NativeGenerator:
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
                              return_aux: bool = False, z_row_offset: int = 0,
                              prune: Optional[Sequence[Sequence[int]]] = None, adam: Optional[Sequence[float]] = None,
-                             huber_delta: Optional[float] = None, z_prior: Optional[float] = None):
+                             huber_delta: Optional[float] = None, z_prior: Optional[float] = None, sparse_dev=None,
+                             deviation_out: Optional[torch.Tensor] = None):
         """The projection of reconstruct fitted to linear measurements (dgan_reconstruct_measured): measurements y
         [B, m] of images through operator A [m, H*W*C] (NHWC pixel order, 1 <= m <= H*W*C, shared by every image and
         restart).  Each restart minimises (1/m) ||A G(z) - y_i||^2; the R restarts of image i share y_i.  Returns G(z) of
@@ -734,11 +846,14 @@ class NativeGenerator:
         z_prior: the latent prior of reconstruct, J = D + lambda ||z||^2 with D the measured loss and its 1/m normaliser
         (dgan_reconstruct_measured[_csr / _conv]_prior, with any of prune, adam and huber_delta); the lambda of a
         formulation on the unnormalised ||A G(z) - y||^2 is m times this one.  None runs the call without the prior as
-        before."""
+        before.
+        sparse_dev, deviation_out: the sparse deviations of reconstruct, fitting A (G(z) + nu) to y with D's 1/m
+        normaliser (dgan_reconstruct_measured[_csr / _conv]_sparse_dev, with any of prune, adam, huber_delta and z_prior);
+        nu lives in pixel space.  None runs the call without deviations as before."""
         if isinstance(operator, ConvOperator):
             return self._reconstruct_measured_conv(measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed,
                                                    momentum, decay_lr, out, return_aux, z_row_offset, prune, adam,
-                                                   huber_delta, z_prior)
+                                                   huber_delta, z_prior, sparse_dev, deviation_out)
         csr = operator.layout == torch.sparse_csr
         if csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
@@ -750,6 +865,7 @@ class NativeGenerator:
         ap = self._adam(adam)
         delta = None if huber_delta is None else check_huber_delta(huber_delta)
         lam = None if z_prior is None else check_z_prior(z_prior)
+        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, m)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
@@ -762,14 +878,28 @@ class NativeGenerator:
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched, adam=ap is not None)
+            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched, adam=ap is not None,
+                                       sdev=sd is not None)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
             n_points = len(sched) if sched is not None else 0
             apr = ctypes.byref(ap) if ap is not None else None
             dpr = _byref_or_none(None if delta is None else ctypes.c_float(delta))
-            if lam is not None and csr:
+            if sd is not None:
+                lpr = _byref_or_none(None if lam is None else ctypes.c_float(lam))
+                if csr:
+                    rc = self.lib.dgan_reconstruct_measured_csr_sparse_dev(
+                        self._handle, ctypes.byref(prm), apr, dpr, lpr, sched, n_points, ctypes.byref(sd), _ptr(dev),
+                        _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws,
+                        need, ctypes.c_void_p(stream))
+                    _check(self.lib, rc, "dgan_reconstruct_measured_csr_sparse_dev")
+                else:
+                    rc = self.lib.dgan_reconstruct_measured_sparse_dev(
+                        self._handle, ctypes.byref(prm), apr, dpr, lpr, sched, n_points, ctypes.byref(sd), _ptr(dev),
+                        _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
+                    _check(self.lib, rc, "dgan_reconstruct_measured_sparse_dev")
+            elif lam is not None and csr:
                 rc = self.lib.dgan_reconstruct_measured_csr_prior(self._handle, ctypes.byref(prm), apr, dpr, lam, sched,
                                                                   n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
                                                                   _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,

@@ -20,6 +20,7 @@
 #include "kernels_measured_conv.cuh"
 #include "kernels_prune.cuh"
 #include "kernels_adam.cuh"
+#include "kernels_sparse_dev.cuh"
 
 namespace dgan {
 
@@ -327,8 +328,8 @@ struct dgan_ctx {
   // prune: the prune points of a pruned call as iter, keep, iter, keep, ..., empty otherwise; adam: 1 for the Adam
   // update with beta1, beta2 and eps, 0 for momentum; huber: the Huber entries' delta, 0 for the squared error; conv:
   // a convolution operator's kh, kw, ph, pw and stride, empty otherwise - not its kernel values, which are staged outside
-  // the graph; prior: 1 for the latent prior with its lambda z_prior, 0 otherwise) on a private stream, replayed with one
-  // cudaGraphLaunch per call.
+  // the graph; prior: 1 for the latent prior with its lambda z_prior, 0 otherwise; sdev: 1 for sparse deviations with
+  // their l1 and step, 0 otherwise) on a private stream, replayed with one cudaGraphLaunch per call.
   struct LoopGraph {
     const void* ws; int batch, rec_rr, rec_iters, decay_lr, weighted, measured, csr_nnz; float rec_lr, momentum;
     std::vector<int> prune;
@@ -337,11 +338,13 @@ struct dgan_ctx {
     float huber = 0.f;
     std::vector<int> conv;
     int prior = 0; float z_prior = 0.f;
+    int sdev = 0; float sdev_l1 = 0.f, sdev_step = 0.f;
     bool same_key(const LoopGraph& o) const {
       return ws == o.ws && batch == o.batch && rec_rr == o.rec_rr && rec_iters == o.rec_iters && decay_lr == o.decay_lr &&
              weighted == o.weighted && measured == o.measured && csr_nnz == o.csr_nnz && rec_lr == o.rec_lr &&
              momentum == o.momentum && prune == o.prune && adam == o.adam && beta1 == o.beta1 && beta2 == o.beta2 &&
-             eps == o.eps && huber == o.huber && conv == o.conv && prior == o.prior && z_prior == o.z_prior;
+             eps == o.eps && huber == o.huber && conv == o.conv && prior == o.prior && z_prior == o.z_prior &&
+             sdev == o.sdev && sdev_l1 == o.sdev_l1 && sdev_step == o.sdev_step;
     }
   };
   std::vector<LoopGraph> graphs;
@@ -484,6 +487,13 @@ struct Workspace {
   // Set by the call, not carved: the prior term lives in `loss` between its evaluation and the loss's finish.
   bool prior = false;
   float z_prior = 0.f;
+  // Sparse deviations (the *_sparse_dev entries; kernels_sparse_dev.cuh), after all the buffers above: each row's
+  // deviation nu [n_pad][H*W*C] and u = G(z) + nu [n_pad][H*W*C], which the data term reads in place of y.  ident: the
+  // image loss run through the measured loop as the identity operator (m = H*W*C), with the measured row buffers dym,
+  // mloss_part and mscale carved before nu.  eta, tau and l1 are set by the call.
+  float *nu = nullptr, *u = nullptr;
+  bool ident = false;
+  float sdev_eta = 0.f, sdev_tau = 0.f, sdev_l1 = 0.f;
 };
 
 // The padded measurement count of a measured workspace: m rounded up to the measurement products' N tile.
@@ -535,10 +545,13 @@ static void carve_csr(const dgan_ctx* c, Workspace* w, int nnz_, char* b, size_t
 // "orig", "src" and "sel" after all the other buffers.  op (not NULL, with m > 0): a region of a pruned measured
 // workspace, whose operator - am / amt or the CSR buffers - and ym live in the operator block op (carve_operator): only
 // the row-sized measured buffers are carved, the others are op's.  adam: the workspace of the Adam entries, the same
-// buffers at the same offsets and the second moment "s" after all of them.
+// buffers at the same offsets and the second moment "s" after all of them.  sdev: the workspace of the sparse-deviation
+// entries, the same buffers at the same offsets and then - for the image loss (m = 0), which runs the measured loop as
+// the identity operator - "dym", "mloss_part" and "mscale" as a measured workspace for m = H*W*C carves them, then "nu"
+// and "u" [n_pad][H*W*C].
 static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
                        int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr,
-                       bool adam = false, const ConvGeom* conv = nullptr) {
+                       bool adam = false, const ConvGeom* conv = nullptr, bool sdev = false) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -636,6 +649,18 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.sel = (int*)take("sel", "i32", {np});     // batch <= n_pad
   }
   if (adam) w.s = (float*)take("s", "f32", {np, latent});
+  if (sdev && m == 0) {
+    w.ident = true;
+    w.m = c->hwc;
+    w.m_ld = measured_ld(c->hwc);
+    w.dym = (float*)take("dym", "f32", {np, hwc});
+    w.mloss_part = (float*)take("mloss_part", "f32", {(size_t)w.m_ld / kMeasTileN, np});
+    w.mscale = (float*)take("mscale", "f32", {np});
+  }
+  if (sdev) {
+    w.nu = (float*)take("nu", "f32", {np, hwc});
+    w.u = (float*)take("u", "f32", {np, hwc});
+  }
   w.bytes = off;
   return w;
 }
@@ -1211,43 +1236,72 @@ static int stage_measured_conv(dgan_ctx* c, const Workspace& w, const float* k, 
 
 // The measurement product through the staged convolution operator: r = A_{n / R} G(z) - y[n / R] and the loss parts
 // (huber: MEAS_RESID_HUBER at delta = w.huber)
-static int launch_measured_conv(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+static int launch_measured_conv(dgan_ctx* c, const Workspace& w, const float* in, int R, cudaStream_t s) {
   const unsigned grid = (unsigned)((size_t)w.n_rows * ((w.m_ld + kConvCols - 1) / kConvCols));
   const size_t smem = conv_smem(c, w, false);
   if (w.huber > 0.f)
-    measured_conv_huber_kernel<<<grid, kConvThreads, smem, s>>>(w.y, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R,
+    measured_conv_huber_kernel<<<grid, kConvThreads, smem, s>>>(in, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R,
                                                                 w.huber, w.mloss_part, w.n_pad);
   else
-    measured_conv_kernel<<<grid, kConvThreads, smem, s>>>(w.y, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R, 1.f,
+    measured_conv_kernel<<<grid, kConvThreads, smem, s>>>(in, c->hwc, w.cg, w.ck, w.m_ld, w.m, w.r, w.m_ld, w.ym, R, 1.f,
                                                           w.mloss_part, w.n_pad);
   DGAN_LAUNCH_CHECK(c);
   return 0;
 }
 
+// The image loss of a sparse-deviation call (w.ident) on u: the loss parts and dy = (2 / H*W*C) w c of the identity
+// operator in one kernel (sdev_image_resid_kernel), against the images in w.x and the weights in w.xw (NULL: unweighted)
+static int launch_image_resid(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
+  const dim3 grid((unsigned)w.n_rows, (unsigned)((w.m_ld / 4 + 255) / 256));
+  const float s_ = 2.f / (float)w.m;
+#define IR(HU, WE) sdev_image_resid_kernel<HU, WE><<<grid, 256, 0, s>>>(w.u, w.x, w.xw, c->hwc, w.m_ld, R, w.huber, s_, \
+                                                                        w.dym, w.mloss_part, w.n_pad)
+  if (w.huber > 0.f) { if (w.xw != nullptr) IR(true, true); else IR(true, false); }
+  else { if (w.xw != nullptr) IR(false, true); else IR(false, false); }
+#undef IR
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
 // The measurement product after a forward that wrote w.y: r = A G(z) - y[n / R] and the measured loss's parts.  w.huber > 0:
-// the Huber residual psi(r) and the Huber loss's parts (MEAS_RESID_HUBER, delta passed as the scale).
+// the Huber residual psi(r) and the Huber loss's parts (MEAS_RESID_HUBER, delta passed as the scale).  With sparse
+// deviations (w.u) the product reads u = G(z) + nu in place of G(z); the image loss's (w.ident) is launch_image_resid.
 static int launch_measure(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
-  if (w.conv) return launch_measured_conv(c, w, R, s);
+  if (w.ident) return launch_image_resid(c, w, R, s);
+  const float* in = w.u != nullptr ? w.u : w.y;
+  if (w.conv) return launch_measured_conv(c, w, in, R, s);
   if (w.huber > 0.f) {
     if (w.csr)
-      return launch_measured_csr<MEAS_RESID_HUBER>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld,
+      return launch_measured_csr<MEAS_RESID_HUBER>(c, w, in, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld,
                                                    w.ym, R, w.huber, w.mloss_part, s);
-    return launch_measured_gemm<MEAS_RESID_HUBER>(c, w, w.y, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R,
+    return launch_measured_gemm<MEAS_RESID_HUBER>(c, w, in, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R,
                                                   w.huber, w.mloss_part, s);
   }
   if (w.csr)
-    return launch_measured_csr<MEAS_RESID>(c, w, w.y, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld, w.ym, R,
+    return launch_measured_csr<MEAS_RESID>(c, w, in, c->hwc, c->hwc, w.a_rp, w.a_ci, w.a_v, w.m_ld, w.r, w.m_ld, w.ym, R,
                                            1.f, w.mloss_part, s);
-  return launch_measured_gemm<MEAS_RESID>(c, w, w.y, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R, 1.f,
+  return launch_measured_gemm<MEAS_RESID>(c, w, in, c->hwc, w.am, c->hwc, w.m_ld, c->hwc, w.r, w.m_ld, w.ym, R, 1.f,
                                           w.mloss_part, s);
+}
+
+// Sparse deviations, iteration t of the loop, after its forward: nu from the previous iteration's dy (t > 0; +0 at
+// t = 0) and u = y + nu (sdev_update_kernel)
+static int launch_sdev_update(dgan_ctx* c, const Workspace& w, int t, cudaStream_t s) {
+  const size_t n4 = (size_t)w.n_rows * c->hwc / 4;
+  sdev_update_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, s>>>(w.y, w.dym, w.nu, w.u, n4, t > 0 ? 1 : 0, w.sdev_eta,
+                                                                  w.sdev_tau);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
 }
 
 // The rest of a measured step's gradient after launch_measure: dy = (2/m) At r, then the cotangent entry of dgan_vjp (its
 // fp16 row scales in w.mscale: w.loss carries the loss to the select) and the backward-to-z into w.g.  R: the rows per
-// image, which pick a convolution operator's kernel.
+// image, which pick a convolution operator's kernel.  The image loss of a sparse-deviation call (w.ident) has its dy from launch_image_resid already.
 static int measured_backward(dgan_ctx* c, const Workspace& w, int R, cudaStream_t s) {
   int rc;
-  if (w.conv) {
+  if (w.ident) {
+    rc = 0;
+  } else if (w.conv) {
     const unsigned grid = (unsigned)((size_t)w.n_rows * ((c->hwc + kConvCols - 1) / kConvCols));
     measured_conv_adjoint_kernel<<<grid, kConvThreads, conv_smem(c, w, true), s>>>(w.r, w.m_ld, w.cg, w.ck, c->hwc, w.dym,
                                                                                  c->hwc, R, 2.f / (float)w.m);
@@ -1323,24 +1377,27 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
 // Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
 // workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
 // planned and mapped too.  m > 0: the workspace of a measured entry for m measurements (conv: a convolution operator).
+// sdev: a sparse-deviation workspace (carve), whose weighted image loss runs in the measured loop, not the weighted pass.
 static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0,
-                    int csr_nnz = -1, bool adam = false, const ConvGeom* conv = nullptr) {
+                    int csr_nnz = -1, bool adam = false, const ConvGeom* conv = nullptr, bool sdev = false) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
+  const bool wpass = weighted && !sdev;
   if ((rc = plan_all(c, n_rows))) return rc;
-  if (weighted && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam, conv);
+  if (wpass && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
+  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam, conv, sdev);
   if (out->bytes > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
+              (sdev ? (m > 0 ? " (dgan_workspace_bytes_measured_sparse_dev)" : " (dgan_workspace_bytes_sparse_dev)")
+               : conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
                : adam ? (m > 0 ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
                : weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
                : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
     return DGAN_ERR_WORKSPACE;
   }
   if ((rc = build_maps(c, *out))) return rc;
-  return weighted ? build_maps(c, *out, TC_PASS_WEIGHTED) : 0;
+  return wpass ? build_maps(c, *out, TC_PASS_WEIGHTED) : 0;
 }
 
 // The weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights) as 3-D arrays: the caller's shape
@@ -1712,6 +1769,48 @@ static void set_prior(Workspace* w, dgan_ctx::LoopGraph* key, const float* z_pri
   if (key != nullptr) { key->prior = 1; key->z_prior = *z_prior; }
 }
 
+// A call's sparse deviations (on: a *_sparse_dev entry, whose sd must not be NULL; dev_out NULL: nu is not returned)
+struct SdevArgs { bool on = false; const dgan_sparse_dev* sd = nullptr; float* dev_out = nullptr; };
+
+// The sparse-deviation entries' l1 and step: finite and >= 0, with eta = step n / 2 and tau = eta l1 (n: H*W*C, or the
+// m of a measured call; both in double, rounded to fp32) finite in fp32, and dev_out 16-byte aligned (sdev_select_kernel
+// stores 16 bytes at a time).  0 (*eta and *tau set), or DGAN_ERR_INVALID_ARG naming the bad value; the callers check it
+// after every other argument and before anything is enqueued.
+static int check_sparse_dev(const SdevArgs& a, int n, float* eta, float* tau) {
+  if (!a.on) return 0;
+  if (a.sd == nullptr) { set_error("NULL sparse_dev"); return DGAN_ERR_INVALID_ARG; }
+  const float l1 = a.sd->l1, step = a.sd->step;
+  std::string bad;
+  if (!(std::isfinite(l1) && l1 >= 0.f)) bad = "l1 = " + std::to_string(l1) + " must be finite and >= 0";
+  else if (!(std::isfinite(step) && step >= 0.f)) bad = "step = " + std::to_string(step) + " must be finite and >= 0";
+  if (bad.empty()) {
+    const double e = (double)step * (double)n / 2.0, t = e * (double)l1;
+    *eta = (float)e;
+    *tau = (float)t;
+    if (!std::isfinite(*eta)) bad = "eta = step * n / 2 = " + std::to_string(e) + " overflows fp32";
+    else if (!std::isfinite(*tau)) bad = "tau = eta * l1 = " + std::to_string(t) + " overflows fp32";
+  }
+  if (bad.empty() && ((uintptr_t)a.dev_out & 15) != 0) bad = "dev_out must be 16-byte aligned";
+  if (bad.empty()) return 0;
+  set_error("invalid sparse deviations: " + bad);
+  return DGAN_ERR_INVALID_ARG;
+}
+
+// The sparse deviations' part of a call's workspace and graph-cache key (a.on, checked by check_sparse_dev)
+static void set_sdev(Workspace* w, dgan_ctx::LoopGraph* key, const SdevArgs& a, float eta, float tau) {
+  if (!a.on) return;
+  if (w != nullptr) { w->sdev_eta = eta; w->sdev_tau = tau; w->sdev_l1 = a.sd->l1; }
+  if (key != nullptr) { key->sdev = 1; key->sdev_l1 = a.sd->l1; key->sdev_step = a.sd->step; }
+}
+
+// After a loss finish of a sparse-deviation workspace (w.nu): J = loss + l1 sum |nu| per row (sdev_term_kernel)
+static int sdev_term(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
+  if (w.nu == nullptr) return 0;
+  sdev_term_kernel<<<(unsigned)((w.n_rows + 7) / 8), 256, 0, s>>>(w.nu, c->hwc, w.n_rows, w.sdev_l1, w.loss);
+  DGAN_LAUNCH_CHECK(c);
+  return 0;
+}
+
 // dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place.
 // huber (not NULL): dgan_loss_grad_huber, the Huber loss at *huber.
 static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
@@ -1900,6 +1999,8 @@ int dgan_sample_z0(dgan_handle h, uint64_t seed, uint64_t z_row_offset, int n_ro
 // w.prior (the prior entries): iteration t1 - 1 first leaves each row's prior term on its z in w.loss (prior_term_kernel)
 // for the loss finish that follows the range, and every update is the prior form of its kernel (the fp16 image loss's
 // momentum runs as on the Adam path: the Linear backward without its tail, then momentum_prior_kernel).
+// w.nu (the sparse-deviation entries, measured loop only): after each forward, nu's update from the previous iteration's
+// dy and u = G(z) + nu (launch_sdev_update), which the data term reads.
 static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params& p, int per_image, int t0, int t1,
                          bool measured, cudaStream_t ls, bool loss_at_end = false, const dgan_adam_params* adam = nullptr) {
   const int latent = h->wd.latent;
@@ -1942,7 +2043,9 @@ static int enqueue_steps(dgan_ctx* h, const Workspace& w, const dgan_rec_params&
     if (measured) {
       // the forward of dgan_vjp (ReLU masks kept, y written every step: the measurement product reads it), then the
       // measured loss's gradient and the momentum update with the cotangent's row scales divided out
-      if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls)) || (r2 = launch_measure(h, w, per_image, ls))) return r2;
+      if ((r2 = run_forward(h, w, nullptr, 1, 1, !last, ls))) return r2;
+      if (w.nu != nullptr && (r2 = launch_sdev_update(h, w, t, ls))) return r2;
+      if ((r2 = launch_measure(h, w, per_image, ls))) return r2;
       if (last) continue;
       if ((r2 = measured_backward(h, w, per_image, ls))) return r2;
       if (adam != nullptr) {
@@ -2055,11 +2158,13 @@ static int check_adam(const dgan_adam_params* a) {
 // weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
 // the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).  huber
 // (not NULL): the Huber entries, the Huber loss at *huber on the counterpart's workspace.  z_prior (not NULL): the prior
-// entries, J = D + *z_prior ||z||^2 on the counterpart's workspace.
+// entries, J = D + *z_prior ||z||^2 on the counterpart's workspace.  sdev.on: the sparse-deviation entries on a
+// sparse-deviation workspace (carve), every loss on the measured loop (the image loss as the identity operator) and
+// J + l1 ||nu||_1 the returned loss and the arg-min.
 static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                             const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                             void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                            const float* huber = nullptr, const float* z_prior = nullptr) {
+                            const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
@@ -2072,10 +2177,15 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   cudaStream_t s = (cudaStream_t)stream;
   Workspace w;
   int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr, meas.conv))) return rc;
-  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior))) return rc;
+  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr, meas.conv, sdev.on)))
+    return rc;
+  float eta = 0.f, tau = 0.f;
+  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior)) ||
+      (rc = check_sparse_dev(sdev, measured ? meas.m : h->hwc, &eta, &tau)))
+    return rc;
   if (huber != nullptr) w.huber = *huber;
   set_prior(&w, nullptr, z_prior);
+  set_sdev(&w, nullptr, sdev, eta, tau);
   const int64_t launches0 = h->launches;
   int64_t enqueues = 0;
   h->n_rows_cur = batch * rec_rr;
@@ -2098,15 +2208,21 @@ static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const flo
   key.huber = w.huber;
   set_conv_key(&key, meas.conv);
   set_prior(nullptr, &key, z_prior);
+  set_sdev(nullptr, &key, sdev, eta, tau);
   auto enqueue_loop = [&](cudaStream_t ls) -> int {
-    return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured, ls, false, adam);
+    return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured || sdev.on, ls, false, adam);
   };
   if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
   {
-    if ((rc = measured ? measured_loss_finish(h, w, s) : image_loss_finish(h, w, s))) return rc;
+    const int64_t l0 = h->launches;
+    if ((rc = w.m > 0 ? measured_loss_finish(h, w, s) : image_loss_finish(h, w, s)) || (rc = sdev_term(h, w, s))) return rc;
     select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, rec_rr, h->hwc, rec_dev, loss_dev, idx_dev);
     DGAN_LAUNCH_CHECK(h);
-    enqueues += 2;
+    if (sdev.dev_out != nullptr) {
+      sdev_select_kernel<<<batch, 256, 0, s>>>(w.loss, w.nu, rec_rr, h->hwc, sdev.dev_out);
+      DGAN_LAUNCH_CHECK(h);
+    }
+    enqueues += h->launches - l0;
   }
   h->last_enqueues = enqueues;
   h->last_launches = h->launches - launches0;
@@ -2143,11 +2259,12 @@ static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_r
 // NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
 // m > 0: a pruned measured workspace (csr_nnz >= 0: CSR; conv not NULL: convolution): first the operator block (carve_operator; layout: a line
 // "operator 0 batch", then its lines), staged once for every stage, then the regions, each with the row-sized measured
-// buffers and the operator block's pointers.  adam: every region an Adam carve (its second moment "s" last).
+// buffers and the operator block's pointers.  adam: every region an Adam carve (its second moment "s" last).  sdev: every
+// region a sparse-deviation carve (its deviation buffers last).
 static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
                                            int n_points, void* base, bool weighted, size_t* bytes,
                                            std::string* layout = nullptr, int m = 0, int csr_nnz = -1, bool adam = false,
-                                           const ConvGeom* conv = nullptr) {
+                                           const ConvGeom* conv = nullptr, bool sdev = false) {
   std::vector<Workspace> regs;
   size_t off = 0;
   Workspace op;
@@ -2160,7 +2277,7 @@ static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec
     const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
     if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
     regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, m, csr_nnz, true,
-                         m > 0 ? &op : nullptr, adam, conv));
+                         m > 0 ? &op : nullptr, adam, conv, sdev));
     off += regs.back().bytes;
   }
   *bytes = off;
@@ -2184,12 +2301,14 @@ static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_poin
 // the plain loop's do loss_part.  adam (not NULL, checked by the caller): the Adam entries; a prune point gathers the
 // survivors' second moment with their z, m and z_h.  huber (not NULL): the Huber entries, every stage and the ranking on
 // the Huber loss at *huber.  z_prior (not NULL): the prior entries, every stage and the ranking on J = D + *z_prior ||z||^2,
-// a prune point's prior term on the z of iteration iter_k - 1 (before that iteration's update, as its D).
+// a prune point's prior term on the z of iteration iter_k - 1 (before that iteration's update, as its D).  sdev.on: the
+// sparse-deviation entries, every region a sparse-deviation carve; a prune point ranks by J + l1 ||nu||_1 on the nu of
+// iteration iter_k - 1 and gathers the survivors' nu and dy, whose update the next region's first iteration applies.
 static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                    const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
                                    float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
                                    MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                                   const float* huber = nullptr, const float* z_prior = nullptr) {
+                                   const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
   const bool measured = meas.m > 0;
   if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
@@ -2205,23 +2324,29 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   }
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
-  if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, weighted))) return rc;
+  const bool wpass = weighted && !sdev.on;      // a sparse-deviation image loss runs in the measured loop
+  if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, wpass))) return rc;
   size_t need = 0;
   std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need, nullptr, meas.m,
-                                             meas.nnz, adam != nullptr, meas.conv);
+                                             meas.nnz, adam != nullptr, meas.conv, sdev.on);
   if (need > ws_bytes) {
     set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
-              (meas.conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
+              (sdev.on ? (measured ? " (dgan_workspace_bytes_measured_sparse_dev)" : " (dgan_workspace_bytes_sparse_dev)")
+               : meas.conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
                : adam != nullptr ? (measured ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
                : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
     return DGAN_ERR_WORKSPACE;
   }
-  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior))) return rc;
+  float eta = 0.f, tau = 0.f;
+  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior)) ||
+      (rc = check_sparse_dev(sdev, measured ? meas.m : h->hwc, &eta, &tau)))
+    return rc;
   for (Workspace& w : regs) {
     if ((rc = build_maps(h, w))) return rc;
-    if (weighted && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
+    if (wpass && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
     if (huber != nullptr) w.huber = *huber;
     set_prior(&w, nullptr, z_prior);
+    set_sdev(&w, nullptr, sdev, eta, tau);
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t launches0 = h->launches;
@@ -2251,10 +2376,12 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   key.huber = huber != nullptr ? *huber : 0.f;
   set_conv_key(&key, meas.conv);
   set_prior(nullptr, &key, z_prior);
+  set_sdev(nullptr, &key, sdev, eta, tau);
   // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
-  // (measured) left
+  // (measured, and every sparse-deviation loss) left, with the deviations' term
   auto finish = [&](const Workspace& w, cudaStream_t ls) -> int {
-    return measured ? measured_loss_finish(h, w, ls) : image_loss_finish(h, w, ls);
+    const int r2 = w.m > 0 ? measured_loss_finish(h, w, ls) : image_loss_finish(h, w, ls);
+    return r2 ? r2 : sdev_term(h, w, ls);
   };
   // the stages and, between them, the prune points: the loss of iteration iter_k - 1 per row (its parts are still in
   // loss_part or mloss_part after that iteration's update), the survivors' maps and the gather of their z, v (and z_h)
@@ -2266,7 +2393,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
       const int per = k == 0 ? rec_rr : sched[k - 1].keep;
       const int t0 = k == 0 ? 0 : sched[k - 1].iter, t1 = k == n_points ? rec_iters : sched[k].iter;
       h->n_rows_cur = w.n_rows;
-      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured, ls, k < n_points, adam))) return r2;
+      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured || sdev.on, ls, k < n_points, adam))) return r2;
       if (k == n_points) break;
       const Workspace& nx = regs[(size_t)k + 1];
       if ((r2 = finish(w, ls))) return r2;
@@ -2281,6 +2408,12 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
         prune_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.z_h, nx.src, nx.n_rows, nx.n_pad,
                                                                             h->wd.latent, nx.z, nx.v, nx.z_h);
       DGAN_LAUNCH_CHECK(h);
+      if (sdev.on) {
+        const size_t n4 = (size_t)nx.n_rows * h->hwc / 4;
+        sdev_gather_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, ls>>>(w.nu, w.dym, nx.src, nx.n_rows, h->hwc, nx.nu,
+                                                                         nx.dym);
+        DGAN_LAUNCH_CHECK(h);
+      }
     }
     return 0;
   };
@@ -2288,12 +2421,17 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   const Workspace& w = regs.back();
   const int per = sched[n_points - 1].keep;
   h->n_rows_cur = w.n_rows;
+  const int64_t l0 = h->launches;
   if ((rc = finish(w, s))) return rc;
   select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, w.sel);
   DGAN_LAUNCH_CHECK(h);
   prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
   DGAN_LAUNCH_CHECK(h);
-  enqueues += 3;
+  if (sdev.dev_out != nullptr) {
+    sdev_select_kernel<<<batch, 256, 0, s>>>(w.loss, w.nu, per, h->hwc, sdev.dev_out);
+    DGAN_LAUNCH_CHECK(h);
+  }
+  enqueues += h->launches - l0;
   h->last_enqueues = enqueues;
   h->last_launches = h->launches - launches0;
   return DGAN_OK;
@@ -2420,17 +2558,17 @@ size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, 
 
 // The image and measured Adam, Huber and prior entries after their own checks: unpruned through reconstruct_impl, pruned
 // through reconstruct_pruned_impl, as their momentum and squared-error counterparts (adam NULL: momentum; huber NULL:
-// squared error; z_prior NULL: no prior)
+// squared error; z_prior NULL: no prior; sdev.on false: no sparse deviations)
 static int reconstruct_adam_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                  const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                                  const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                  size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs(),
-                                 const float* huber = nullptr, const float* z_prior = nullptr) {
+                                 const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
   if (unpruned(sched, n_points))
     return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam,
-                            huber, z_prior);
+                            huber, z_prior, sdev);
   return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                                 stream, meas, adam, huber, z_prior);
+                                 stream, meas, adam, huber, z_prior, sdev);
 }
 
 int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2677,6 +2815,106 @@ int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const 
   if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
   return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
                                  huber_delta);
+}
+
+// ---- sparse deviations (kernels_sparse_dev.cuh): each entry is its prior entry's code path on the measured loop --------
+// with u = G(z) + nu in place of G(z).  adam NULL: momentum; huber_delta NULL: the squared error; z_prior NULL: no prior;
+// sched NULL with n_points 0: unpruned.  The counterpart's checks come first, then check_sparse_dev's, before anything
+// is enqueued.
+
+// The bytes of a sparse-deviation workspace (m 0: the image loss, weighted or not; m > 0: measured, nnz -1 dense or the
+// CSR non-zeros, conv not NULL a convolution), planning every stage; layout (not NULL) receives its lines.  0 when an
+// argument is out of range.
+static size_t sdev_bytes(dgan_handle h, int batch, int rec_rr, bool weighted, int m, int nnz, const ConvGeom* conv,
+                         bool adam, const dgan_prune_point* sched, int n_points, std::string* layout) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
+  if (m != 0 && (weighted || (conv == nullptr && !measured_pruned_args_ok(h, m, nnz)))) return 0;
+  if (unpruned(sched, n_points)) {
+    if (plan_all(h, batch * rec_rr) != 0) return 0;
+    return carve(h, batch * rec_rr, nullptr, layout, weighted, m, conv != nullptr ? -1 : nnz, false, nullptr, adam, conv,
+                 true).bytes;
+  }
+  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
+  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
+  size_t bytes = 0;
+  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted, &bytes, layout, m, conv != nullptr ? -1 : nnz, adam,
+               conv, true);
+  return bytes;
+}
+
+size_t dgan_workspace_bytes_sparse_dev(dgan_handle h, int batch, int rec_rr, int weighted, int adam,
+                                       const dgan_prune_point* sched, int n_points) {
+  return sdev_bytes(h, batch, rec_rr, weighted != 0, 0, -1, nullptr, adam != 0, sched, n_points, nullptr);
+}
+
+size_t dgan_workspace_bytes_measured_sparse_dev(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_conv_op* op,
+                                                int adam, const dgan_prune_point* sched, int n_points) {
+  ConvGeom g;
+  if (op != nullptr) {
+    if (h == nullptr || !conv_geom(h, op, &g) || m != g.Ho * g.Wo * g.C) return 0;
+  } else if (m <= 0) {
+    return 0;
+  }
+  return sdev_bytes(h, batch, rec_rr, false, m, nnz, op != nullptr ? &g : nullptr, adam != 0, sched, n_points, nullptr);
+}
+
+int dgan_reconstruct_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                const float* huber_delta, const float* z_prior, const dgan_prune_point* sched, int n_points,
+                                const dgan_sparse_dev* sparse_dev, float* dev_out, const float* x_dev, const float* w_dev,
+                                const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
+                               stream, MeasuredArgs(), huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+}
+
+int dgan_reconstruct_measured_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                         const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                         int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out, const float* a_dev,
+                                         int m, const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                         int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.a = a_dev; meas.y = y_dev; meas.m = m;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+}
+
+int dgan_reconstruct_measured_csr_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                             const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                             int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out,
+                                             const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                             const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                             int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
+  MeasuredArgs meas;
+  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+}
+
+int dgan_reconstruct_measured_conv_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
+                                              const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                              int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out,
+                                              const dgan_conv_op* op, const float* k_dev, const float* y_dev,
+                                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
+                                              void* ws, size_t ws_bytes, void* stream) {
+  if (adam != nullptr)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  ConvGeom g;
+  MeasuredArgs meas;
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
+  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
+                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -3080,6 +3318,29 @@ int dgan_debug_workspace_layout_measured_conv(dgan_handle h, int n_rows, const d
   }
   std::string out;
   carve(h, n_rows, nullptr, &out, false, g.Ho * g.Wo * g.C, -1, false, nullptr, false, &g);
+  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
+  memcpy(buf, out.c_str(), out.size() + 1);
+  return (int)out.size();
+}
+
+// The same for the workspace of the sparse-deviation entries (dgan_workspace_bytes_sparse_dev with m = 0,
+// dgan_workspace_bytes_measured_sparse_dev with m > 0; nnz -1 for a dense or convolution operator, op not NULL for a
+// convolution): the layout of the counterpart - unpruned or pruned, Adam or not - with, at the end of the workspace or of
+// each region, for the image loss "dym" f32 [n_pad][H*W*C], "mloss_part" f32 [m_ld / 64][n_pad] and "mscale" f32 [n_pad]
+// (m_ld: H*W*C rounded up to 64), then "nu" and "u", f32 [n_pad][H*W*C] each.
+int dgan_debug_workspace_layout_sparse_dev(dgan_handle h, int batch, int rec_rr, int weighted, int m, int nnz,
+                                           const dgan_conv_op* op, int adam, const dgan_prune_point* sched, int n_points,
+                                           char* buf, int buf_len) {
+  ConvGeom g;
+  if (h == nullptr || buf == nullptr || buf_len <= 0 || (op != nullptr && (!conv_geom(h, op, &g) || m != g.Ho * g.Wo * g.C))) {
+    set_error("invalid argument");
+    return -1;
+  }
+  std::string out;
+  if (sdev_bytes(h, batch, rec_rr, weighted != 0, m, nnz, op != nullptr ? &g : nullptr, adam != 0, sched, n_points, &out) == 0) {
+    set_error("invalid argument");
+    return -1;
+  }
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();

@@ -126,6 +126,7 @@ class DefenseGANBase(object):
         self.rec_adam_eps = 1e-8           # Adam's eps (cfg REC_ADAM_EPS)
         self.rec_huber_delta = None        # data term: None = squared error (the reference's) | Huber delta > 0 (cfg REC_HUBER_DELTA)
         self.rec_z_prior = None            # latent prior: None = none (the reference's) | lambda >= 0 of D + lambda ||z||^2 (cfg REC_Z_PRIOR)
+        self.rec_sparse_dev = None         # sparse deviations: None = none (the reference's) | (l1, step) of G(z) + nu (cfg REC_SPARSE_DEV)
         self.seed = 11241990               # callers use tf.set_random_seed(11241990) (blackbox.py:464)
 
         self.test_mode = test_mode
@@ -327,7 +328,7 @@ class DefenseGANBase(object):
         return (int(self.seed) * 1000003 + int(reconstructor_id) * 7919 + self._call_counter) & (2 ** 63 - 1)
 
     def reconstruct(self, images, batch_size=None, back_prop=True, reconstructor_id=0, z_init_val=None,
-                    return_aux=False, out=None, z_row_offset=0, pixel_weights=None):
+                    return_aux=False, out=None, z_row_offset=0, pixel_weights=None, deviation_out=None):
         """Defense-GAN projection of `images` onto the generator's range (reference
         models/gan.py:333-449): rec_rr restarts x rec_iters momentum-GD steps on
         ||G(z) - x||^2, returns G(z) of the min-loss restart.  Hyper-parameters are read from the
@@ -377,11 +378,25 @@ class DefenseGANBase(object):
         formulation on the unnormalised sum does not carry over.  The returned loss is J (the detection statistic then
         includes the prior), the chosen restart is J's arg-min and rec_prune ranks by J.  lambda = 0 gives the bits of
         the call without it.  It combines with pixel_weights, rec_prune, Adam and rec_huber_delta, and is checked before
-        any native call (a ValueError naming the bad value)."""
+        any native call (a ValueError naming the bad value).
+
+        `rec_sparse_dev` (an extension, read at call time; None by default, the reference's range projection alone): an
+        (l1, step) pair with both >= 0 fits G(z) + nu, with nu a per-pixel deviation under an l1 penalty (Sparse-Gen,
+        Dhar, Grover and Ermon 2018): each restart minimises D(G(z) + nu) [+ lambda ||z||^2] + l1 ||nu||_1, nu taking an
+        ISTA step of size step * H*W*C / 2 each iteration.  A few pixels the generator cannot produce - an occluder, dead
+        or saturated pixels, impulse noise, a patch - then go into nu instead of dragging z to a wrong latent.  The
+        returned image is still G(z) of the chosen restart (the defense's output); `deviation_out` (a [B,H,W,C] float32
+        CUDA tensor) receives that restart's nu, a per-pixel map of where the input left the generator's range.  step = 1
+        on the squared error moves nu to its exact minimiser each step, counting residuals beyond l1 * H*W*C / 2 as
+        deviations.  The returned loss is J with the l1 term, the arg-min and rec_prune rank by it.  It combines with
+        pixel_weights, rec_prune, Adam, rec_huber_delta and rec_z_prior, and is checked before any native call (a
+        ValueError naming the bad value).  The image loss then runs in the measured loop rather than the fused one, so
+        it costs more per step."""
         prune = self._prune_schedule()
         adam = self._adam_params()
         huber = self._huber_delta()
         prior = self._z_prior()
+        sdev = self._sparse_dev(deviation_out)
         x = self._as_cuda(images)
         if x.dim() != 4 or list(x.shape[1:]) != list(self.image_dim):
             raise ValueError("images must be [B,%d,%d,%d], got %s" % (tuple(self.image_dim) + (tuple(x.shape),)))
@@ -400,6 +415,9 @@ class DefenseGANBase(object):
             kw["huber_delta"] = huber
         if prior is not None:
             kw["z_prior"] = prior
+        if sdev is not None:
+            kw["sparse_dev"] = sdev
+            kw["deviation_out"] = deviation_out
         res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
                                  momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                  return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
@@ -449,8 +467,20 @@ class DefenseGANBase(object):
         except ValueError as e:
             raise ValueError("rec_z_prior: %s" % e) from None
 
+    def _sparse_dev(self, deviation_out=None):
+        """`rec_sparse_dev` checked (None when unset): an (l1, step) pair of finite floats >= 0; ValueError before any
+        native call, also for a deviation_out given without it."""
+        if self.rec_sparse_dev is None:
+            if deviation_out is not None:
+                raise ValueError("deviation_out needs rec_sparse_dev: without deviations there is nothing to return")
+            return None
+        try:
+            return _native.check_sparse_dev(self.rec_sparse_dev)
+        except ValueError as e:
+            raise ValueError("rec_sparse_dev: %s" % e) from None
+
     def reconstruct_measured(self, measurements, operator, batch_size=None, z_init_val=None, return_aux=False, out=None,
-                             z_row_offset=0, prune=_NOT_GIVEN):
+                             z_row_offset=0, prune=_NOT_GIVEN, deviation_out=None):
         """Projection onto the generator's range from linear measurements (an extension; the reference has none), for
         images that are not held themselves but observed as y = A x: a low-resolution or blurred copy, a
         compressed-sensing sketch.  `operator` A is [m, H*W*C] (a tensor or array; columns in NHWC pixel order,
@@ -493,10 +523,16 @@ class DefenseGANBase(object):
         `rec_z_prior` is read at call time as in `reconstruct`: a lambda >= 0 adds lambda ||z||^2 to the measured loss,
         (1/m) ||A G(z) - y||^2 + lambda ||z||^2 - the latent prior of compressed sensing with generative models, with the
         data term normalised by m (the lambda of the unnormalised formulation is m times this one) - for every operator
-        kind, pruned or not."""
+        kind, pruned or not.
+
+        `rec_sparse_dev` is read at call time as in `reconstruct`: each restart fits A (G(z) + nu) to y with an l1 penalty
+        on the pixel-space deviation nu, whose step is step * m / 2 (step = 1 is the 1/Lipschitz step for ||A||_2 <= 1,
+        such as the normalised blurs and box averages of ConvOperator), for every operator kind, pruned or not;
+        `deviation_out` receives the chosen restart's nu."""
         adam = self._adam_params()
         huber = self._huber_delta()
         prior = self._z_prior()
+        sdev = self._sparse_dev(deviation_out)
         if prune is _NOT_GIVEN:
             if self.rec_prune is not None:
                 raise ValueError("rec_prune is set, but reconstruct_measured does not prune restarts from it: set "
@@ -509,10 +545,10 @@ class DefenseGANBase(object):
             prune = _native.check_prune_schedule(prune, int(self.rec_rr), int(self.rec_iters))
         if isinstance(operator, ConvOperator):
             return self._reconstruct_measured_conv(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                   z_row_offset, prune, adam, huber, prior)
+                                                   z_row_offset, prune, adam, huber, prior, sdev, deviation_out)
         if isinstance(operator, torch.Tensor) and operator.layout in (torch.sparse_coo, torch.sparse_csr):
             return self._reconstruct_measured_sparse(measurements, operator, batch_size, z_init_val, return_aux, out,
-                                                     z_row_offset, prune, adam, huber, prior)
+                                                     z_row_offset, prune, adam, huber, prior, sdev, deviation_out)
         a = self._as_cuda(operator)
         hwc = int(np.prod(self.image_dim))
         if a.dim() != 2 or a.shape[1] != hwc or not 1 <= a.shape[0] <= hwc:
@@ -535,15 +571,18 @@ class DefenseGANBase(object):
             kw["huber_delta"] = huber
         if prior is not None:
             kw["z_prior"] = prior
+        if sdev is not None:
+            kw["sparse_dev"] = sdev
+            kw["deviation_out"] = deviation_out
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
                                            **kw)
 
     def _reconstruct_measured_conv(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                   prune, adam=None, huber=None, prior=None):
+                                   prune, adam=None, huber=None, prior=None, sdev=None, deviation_out=None):
         """reconstruct_measured for a ConvOperator, after one check of the kernels and the measurements (prune, adam,
-        huber and prior as in _reconstruct_measured_sparse).  The native call gets the kernels broadcast to [B, kh, kw]."""
+        huber, prior, sdev and deviation_out as in _reconstruct_measured_sparse).  The native call gets the kernels broadcast to [B, kh, kw]."""
         m = operator.num_measurements(self.image_dim)
         y = self._as_cuda(measurements)
         if y.dim() != 2 or y.shape[1] != m or y.shape[0] == 0:
@@ -568,16 +607,20 @@ class DefenseGANBase(object):
             kw["huber_delta"] = huber
         if prior is not None:
             kw["z_prior"] = prior
+        if sdev is not None:
+            kw["sparse_dev"] = sdev
+            kw["deviation_out"] = deviation_out
         return native.reconstruct_measured(y, operator._with_kernels(k), int(self.rec_rr), int(self.rec_iters),
                                            float(self.rec_lr), z_init_val=z0, seed=seed,
                                            momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
                                            return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune, **kw)
 
     def _reconstruct_measured_sparse(self, measurements, operator, batch_size, z_init_val, return_aux, out, z_row_offset,
-                                     prune, adam=None, huber=None, prior=None):
+                                     prune, adam=None, huber=None, prior=None, sdev=None, deviation_out=None):
         """reconstruct_measured for a sparse COO or CSR operator, after one check of the CSR and the measurements
         (prune: the checked schedule, or None; adam: the checked Adam parameters, or None; huber: the checked Huber delta,
-        or None; prior: the checked latent prior's lambda, or None)."""
+        or None; prior: the checked latent prior's lambda, or None; sdev: the checked sparse deviations' (l1, step), or
+        None, with deviation_out)."""
         a = operator
         if a.layout == torch.sparse_coo:
             if a.dim() != 2 or a.dense_dim() != 0:
@@ -624,6 +667,9 @@ class DefenseGANBase(object):
             kw["huber_delta"] = huber
         if prior is not None:
             kw["z_prior"] = prior
+        if sdev is not None:
+            kw["sparse_dev"] = sdev
+            kw["deviation_out"] = deviation_out
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
@@ -656,11 +702,13 @@ class DefenseGANBase(object):
 
     def rec_cache_dir(self, split: str, max_num: int = -1) -> str:
         """`<checkpoint_dir>/recs_rr{R}_lr{lr:.5f}_iters{L}[_num{n}][_prune{it}x{keep}[-{it}x{keep}...]]
-        [_adam{b1:g}-{b2:g}-{eps:g}][_huber{delta:g}][_zprior{lambda:g}]/<split>[_debug]` - the directory name the callers
+        [_adam{b1:g}-{b2:g}-{eps:g}][_huber{delta:g}][_zprior{lambda:g}][_sdev{l1:g}_{step:g}]/<split>[_debug]` - the
+        directory name the callers
         parse back with `recs_rr(.*)_lr(.*)_iters(.*)` (blackbox.py:646-651); the `_prune` part (only with `rec_prune` set)
         keeps pruned and unpruned reconstructions apart, the `_adam` part (only with rec_optimizer "adam") Adam's from
         momentum's, the `_huber` part (only with rec_huber_delta set) the Huber loss's from the squared error's, and the
-        `_zprior` part (only with rec_z_prior set) those with the latent prior from those without."""
+        `_zprior` part (only with rec_z_prior set) those with the latent prior from those without, and the `_sdev` part
+        (only with rec_sparse_dev set) those with sparse deviations from those without."""
         if max_num > 0:
             name = 'recs_rr{:d}_lr{:.5f}_iters{:d}_num{:d}'.format(int(self.rec_rr), float(self.rec_lr),
                                                                    int(self.rec_iters), int(max_num))
@@ -677,6 +725,9 @@ class DefenseGANBase(object):
         prior = self._z_prior()
         if prior is not None:
             name += '_zprior{:g}'.format(prior)
+        sdev = self._sparse_dev()
+        if sdev is not None:
+            name += '_sdev{:g}_{:g}'.format(*sdev)
         out = os.path.join(self.checkpoint_dir, name, split)
         if self.debug:
             out += '_debug'

@@ -74,6 +74,9 @@ def reconstruct_sharded(gan, images: torch.Tensor, z_init_val: Optional[torch.Te
     if bool(gan.use_bn):
         raise RuntimeError("use_bn=True couples all latent rows through batch statistics (SURVEY F2); "
                            "sharding the batch would change the result - run replicas instead")
+    if getattr(gan, "rec_sparse_dev", None) is not None:
+        raise RuntimeError("rec_sparse_dev is set: the projection with sparse deviations runs on one GPU only; call "
+                           "gan.reconstruct per device, or set rec_sparse_dev = None to shard")
 
     # every rank advances the model's call counter identically, so all shards draw from ONE Philox stream; the shard's
     # first row in that stream is (first image) * rec_rr: row for row the single-GPU draw

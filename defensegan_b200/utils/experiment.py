@@ -174,6 +174,7 @@ _G = r"(\d+(?:\.\d*)?(?:e[-+]\d+)?)"            # a number as '{:g}' writes it
 _REC_ADAM_RE = re.compile(r"_adam%s-%s-%s" % (_G, _G, _G))
 _REC_HUBER_RE = re.compile(r"_huber(inf|\d+(?:\.\d*)?(?:e[-+]\d+)?)")
 _REC_ZPRIOR_RE = re.compile(r"_zprior%s" % _G)
+_REC_SDEV_RE = re.compile(r"_sdev%s_%s" % (_G, _G))
 
 
 def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
@@ -182,7 +183,8 @@ def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
     (`_prune<it>x<keep>[-<it>x<keep>...]`) included: `gan.rec_prune` becomes that schedule, or None when the name has
     none; so is the optimiser (`_adam<b1>-<b2>-<eps>`): "adam" with those betas and eps, or "momentum" when the name
     has none; and the data term (`_huber<delta>`): the Huber loss at that delta, or the squared error (None) when the name
-    has none; and the latent prior (`_zprior<lambda>`): that lambda, or no prior (None) when the name has none;
+    has none; and the latent prior (`_zprior<lambda>`): that lambda, or no prior (None) when the name has none; and the
+    sparse deviations (`_sdev<l1>_<step>`): that (l1, step), or none (None) when the name has none;
     `--override` applies the `--rec_rr / --rec_lr / --rec_iters` values instead of the model cfg's."""
     cfg = cfg or {}
     rr = cfg.get("REC_RR", gan.rec_rr)
@@ -209,6 +211,8 @@ def set_test_time_rec_params(gan, flags: Flags, cfg=None) -> None:
             gan.rec_huber_delta = float(huber.group(1)) if huber else None
             prior = _REC_ZPRIOR_RE.search(flags.rec_path)
             gan.rec_z_prior = float(prior.group(1)) if prior else None
+            sdev = _REC_SDEV_RE.search(flags.rec_path)
+            gan.rec_sparse_dev = (float(sdev.group(1)), float(sdev.group(2))) if sdev else None
         elif defense == "defense_gan":
             assert flags.online_training or not flags.train_on_recs
     if flags.override:

@@ -544,6 +544,96 @@ int dgan_reconstruct_measured_conv_prior(dgan_handle h, const dgan_rec_params* p
                                          const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                          size_t ws_bytes, void* stream);
 
+/* The projection with sparse deviations (an extension: the reference has none; Sparse-Gen, Dhar, Grover and Ermon, ICML
+ * 2018).  Each restart row carries nu in R^{H*W*C}, starting at +0, and fits u = G(z) + nu (one fp32 add per element):
+ * the data term D is the counterpart's, computed on u in place of G(z) - the image loss (1/n) sum w l(u - x) with
+ * n = H*W*C, or the measured loss (1/m) sum l(A_i u - y_i) - squared error or Huber, weighted or not.  Each restart
+ * minimises
+ *   J(z, nu) = D(u) + lambda ||z||^2 + l1 ||nu||_1          (the lambda term only with a prior)
+ * for l1 >= 0 and step >= 0, both finite.
+ *   - p_nu = l1 * S, S = sum |nu_p| over the H*W*C pixels of the row in fp32: lane l of a warp adds |nu_l|, |nu_{l+32}|,
+ *     ... in ascending p from +0, then a butterfly over the 32 lanes at offsets 16, 8, 4, 2, 1.  J = ((D + p_z) + p_nu)
+ *     as fp32 adds, or D + p_nu without a prior.
+ *   - g = dD/du: (2/n) w c for the image loss (c the residual u - x, or for Huber its clip to delta), or the measured
+ *     path's fp32 dy = (2/m) A^T c before its cotangent entry.  The generator's backward receives g as the counterpart's
+ *     does; the update of z is the counterpart's (momentum or Adam, with or without the prior's term).
+ *   - The update of nu is one proximal-gradient (ISTA) step on the same iterate:
+ *       nu <- S_tau(fmaf(-eta, g, nu)),  S_tau(a) = |a| > tau ? a - copysign(tau, a) : +0
+ *     with eta = step n / 2 (step m / 2 measured) and tau = eta l1, both in double on the host, rounded to fp32.  With
+ *     step = 1 on the unweighted squared-error image loss one step is the exact minimiser over nu, S_tau(x - G(z)), and
+ *     tau = l1 n / 2 is the residual beyond which a pixel counts as a deviation; Sparse-Gen's unnormalised lambda is n l1.
+ *     step = 1 is the 1/Lipschitz step for ||A||_2 <= 1 (the normalised blurs and box averages of a convolution
+ *     operator).  nu's step is constant: decay_lr and Adam apply to z only.
+ *   - Iteration t computes D, g and J at (z_t, nu_t) and, if t < L - 1, moves both to (z_{t+1}, nu_{t+1}).  loss_dev and
+ *     the arg-min use J at iteration L - 1; a prune point iter_k ranks by J at iteration iter_k - 1, before that
+ *     iteration's update.  Survivors carry their nu, and each follows its unpruned trajectory exactly.
+ *   - rec_dev is G(z) of the chosen restart (the range projection); dev_out [batch, H, W, C] (nullable, 16-byte aligned)
+ *     receives that restart's nu.  The full estimate is their sum.
+ *   - step = 0 keeps nu and p_nu at +0: every measured entry (dense, CSR, convolution) then gives its counterpart's
+ *     rec_dev, loss_dev and idx_dev bit for bit.  The image entry without weights equals the CSR entry on the identity
+ *     (m = n) bit for bit at any step on both precisions: its data term is that operator fused (the CSR measurement
+ *     product's loss reduction, the adjoint's fmaf chain from +0).  w = 1 everywhere gives the unweighted bits.
+ *   - use_bn is allowed unpruned; with a schedule it is refused as by the counterpart.
+ * Each entry takes the options of its prior entry - adam NULL for momentum, huber_delta NULL for the squared error,
+ * z_prior NULL for no prior (else lambda = *z_prior, checked as dgan_reconstruct_prior checks it), sched NULL with
+ * n_points 0 unpruned - then sparse_dev (not NULL) and dev_out.  Every loss, the image loss included, runs the measured
+ * loop: the image loss leaves the fused last-layer epilogue of dgan_reconstruct.
+ * Workspace: dgan_workspace_bytes_sparse_dev / dgan_workspace_bytes_measured_sparse_dev, the counterpart's layout with nu
+ * and u appended (and, for the image loss, the measured row buffers of m = n): 2 * rows * H*W*C * 4 bytes more, where rows
+ * is batch * rec_rr rounded up to the row tile, per region when pruned - 126 MB at CelebA batch 128, rec_rr 10.
+ * l1 or step NaN, infinite or negative, eta or tau not finite in fp32, a misaligned dev_out or a NULL sparse_dev:
+ * DGAN_ERR_INVALID_ARG naming the value, checked after the counterpart's checks and before anything is enqueued.
+ * Counts, with L iterations and P prune points, against the counterpart (the same call without sparse deviations):
+ * dgan_last_enqueue_count is the counterpart's + 1, + 1 more with dev_out.
+ * dgan_last_launch_count is, for a measured entry, the counterpart's + L (the nu update) + 1 + P (p_nu, at
+ * iteration L - 1 and at each prune point) + P (the survivors' nu gather), + 1 with dev_out; for the image entry, that of
+ * dgan_reconstruct_measured_sparse_dev on a dense operator with m = H*W*C and the same options - 3 (the operator's
+ * staging) - (L - 1) (the adjoint products, fused into the image residual).  The graph cache keys on l1 and step. */
+typedef struct dgan_sparse_dev {
+  float l1;     /* >= 0: the weight of ||nu||_1 in J */
+  float step;   /* >= 0: nu's step, in units of 2/n (2/m): step = 1 is eta = n / 2 */
+} dgan_sparse_dev;
+
+/* The workspace of dgan_reconstruct_sparse_dev (weighted: with w_dev; adam: with the Adam update; sched / n_points as
+ * there).  0 for an invalid argument. */
+size_t dgan_workspace_bytes_sparse_dev(dgan_handle h, int batch, int rec_rr, int weighted, int adam,
+                                       const dgan_prune_point* sched, int n_points);
+
+/* The workspace of dgan_reconstruct_measured[_csr / _conv]_sparse_dev: nnz -1 for a dense operator, else the CSR
+ * non-zeros; op not NULL for a convolution (nnz -1 and m = dgan_conv_op_m(h, op)).  0 for an invalid argument. */
+size_t dgan_workspace_bytes_measured_sparse_dev(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_conv_op* op,
+                                                int adam, const dgan_prune_point* sched, int n_points);
+
+/* dgan_reconstruct_sparse_dev: the image loss; w_dev NULL for dgan_reconstruct's loss, else dgan_reconstruct_weighted's. */
+int dgan_reconstruct_sparse_dev(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                const float* huber_delta, const float* z_prior, const dgan_prune_point* sched, int n_points,
+                                const dgan_sparse_dev* sparse_dev, float* dev_out, const float* x_dev, const float* w_dev,
+                                const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
+                                size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured (a dense operator) with the sparse deviations of dgan_reconstruct_sparse_dev. */
+int dgan_reconstruct_measured_sparse_dev(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                         const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                         int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out, const float* a_dev,
+                                         int m, const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                         int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured_csr with the sparse deviations of dgan_reconstruct_sparse_dev. */
+int dgan_reconstruct_measured_csr_sparse_dev(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                             const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                             int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out,
+                                             const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
+                                             const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
+                                             int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream);
+
+/* dgan_reconstruct_measured_conv with the sparse deviations of dgan_reconstruct_sparse_dev. */
+int dgan_reconstruct_measured_conv_sparse_dev(dgan_handle h, const dgan_rec_params* params, const dgan_adam_params* adam,
+                                              const float* huber_delta, const float* z_prior, const dgan_prune_point* sched,
+                                              int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out,
+                                              const dgan_conv_op* op, const float* k_dev, const float* y_dev,
+                                              const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
+                                              void* ws, size_t ws_bytes, void* stream);
+
 /* tf.gradients(generator_fn(z), z, grad_ys=dy) (models/gan.py:657-665,726-735 through tflib's ops):
  *   z_dev [n_rows, latent] fp32, dy_dev [n_rows, H*W*C] fp32 -> dz_dev [n_rows, latent] fp32,
  *   y_dev [n_rows, H*W*C] = G(z) (nullable; bit-identical to dgan_forward).  The forward is recomputed.
@@ -576,13 +666,13 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
  * (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber) runs as many as its squared-error counterpart.  A
  * dgan_reconstruct_measured_conv call runs 4 fewer than the dgan_reconstruct_measured_csr call with the same options.  A
  * prior call (dgan_reconstruct[_measured[_csr / _conv]]_prior) runs its counterpart's + 1 + P with P prune points, + L - 1
- * on the DGAN_PREC_FP16 image loss with momentum. */
+ * on the DGAN_PREC_FP16 image loss with momentum.  A sparse-deviation call: see dgan_reconstruct_sparse_dev. */
 int64_t dgan_last_launch_count(dgan_handle h);
 
 /* Stream operations the HOST issued for it.  The L-step loop only touches the workspace, so it is captured into a CUDA
  * graph the first time a (workspace, batch, rec_rr, rec_iters, rec_lr, momentum, decay_lr, weighted, m, operator kind,
  * nnz, prune schedule, optimiser: momentum, or Adam with its beta1, beta2 and eps, and data term: the squared error, or
- * the Huber loss with its delta, and latent prior: none, or lambda) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
+ * the Huber loss with its delta, and latent prior: none, or lambda, and sparse deviations: none, or l1 and step) combination is seen and replayed with one cudaGraphLaunch afterwards: z0 initialiser (+ its memsets), image copy
  * (measured calls: the three kernels that stage A, A^T and y; CSR-measured calls: the five that validate and stage them;
  * convolution-measured calls: the one that stages the kernels and y), graph, loss sum, arg-min select.  A convolution
  * operator's geometry is part of the key; its kernel values are not. */
