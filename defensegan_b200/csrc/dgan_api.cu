@@ -319,6 +319,7 @@ struct dgan_ctx {
   // fp16 path: the weighted last-layer forward (tc_directions(desc, TC_PASS_WEIGHTED)) on last.fwd's weight tiles; made on
   // the first weighted call
   std::vector<TcDir> tc_w_dirs;
+  int tc_order = TC2_ORDER_BAND;       // item order of every fp16 plan (Tc2Order; dgan_debug_force_order)
   // optional per-launch CUDA-event timing (dgan_profile_*): serialises nothing by itself but
   // adds two event records per launch, so it is never enabled in a timed benchmark pass
   bool profile = false;
@@ -1365,6 +1366,7 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
       if ((rc = tc_dir_supported(t))) return rc;
       for (const TcDir& p : c->tc_dirs)
         if (p.ld == t.ld && p.col0 == t.col0) { t.w = p.w; t.tm_b = p.tm_b; }
+      t.order = c->tc_order;
     }
     have = std::move(dirs);
   }
@@ -2963,7 +2965,9 @@ static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mut
   for (const TcDir& dr : tc_directions(d, pass)) {
     if (int rc = tc_dir_supported(dr)) return rc;
     Tc2Plan plan;
-    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan);
+    const bool rev = tc2_band_reverse(dr.ld);
+    int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs,
+                      dr.order, rev, &plan);
     if (rc) { set_error(dr.name + ": " + dgan_last_error()); return rc; }
     // self-test of the validator: damage one plan in one specific way - faults 1-11 and 14-15 that of Generator.3 fwd (of
     // its tangent direction Generator.3.jvp for the tangent pass), faults 12-13 (specific to narrow ops) that of the last
@@ -3026,11 +3030,23 @@ static int check_plans_impl(const dgan_desc* d, int n_rows, int n_pairs, int mut
     std::string err;
     if ((rc = tc2_check_plan(dr.N, dr.K, dr.tab, n_mpairs, dr.epi, dr.out_bytes, plan, &err))) { set_error(dr.name + ": " + err); return rc; }
     if (mutate != 0) continue;
+    // the plan in the other order (dgan_debug_force_order)
+    Tc2Plan lpt;
+    if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs,
+                       TC2_ORDER_LPT, rev, &lpt))) {
+      set_error(dr.name + " (LPT order): " + dgan_last_error());
+      return rc;
+    }
+    if ((rc = tc2_check_plan(dr.N, dr.K, dr.tab, n_mpairs, dr.epi, dr.out_bytes, lpt, &err))) {
+      set_error(dr.name + " (LPT order): " + err);
+      return rc;
+    }
     // the plans dgan_debug_force_slots can select: every other slot count this direction has an instantiation for
     for (const Tc2Kind& k : kTc2Kinds) {
       if (k.n != dr.N || k.ksub != plan.ksub || k.epi != dr.epi || k.out_bytes != dr.out_bytes || k.maxb == plan.maxb) continue;
       Tc2Plan forced;
-      if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &forced))) {
+      if ((rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, k.maxb, dr.epi, dr.out_bytes, n_mpairs, n_pairs,
+                         dr.order, rev, &forced))) {
         set_error(dr.name + " (" + std::to_string(k.maxb) + " slots): " + dgan_last_error());
         return rc;
       }
@@ -3072,6 +3088,25 @@ int dgan_debug_force_slots(dgan_handle h, int dir, int maxb) {
   }
   d.force_maxb = maxb;
   d.by_mpairs.clear();                      // the uploaded tables stay in h->allocs until dgan_destroy
+  for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
+  h->graphs.clear();
+  return DGAN_OK;
+}
+
+// Host-side test aid (not in the public header): plan every layer-direction of an fp16 handle in item order `order`
+// (Tc2Order: 0 LPT, 1 banded, the default) from now on.  Schedules and captured loops are re-made on the next call.  The
+// results must not change: the order only decides which CTA pair computes an item, and when.
+int dgan_debug_force_order(dgan_handle h, int order) {
+  if (h == nullptr || h->desc.precision != DGAN_PREC_FP16 || (order != TC2_ORDER_LPT && order != TC2_ORDER_BAND)) {
+    set_error("invalid argument");
+    return DGAN_ERR_INVALID_ARG;
+  }
+  h->tc_order = order;
+  for (std::vector<TcDir>* dirs : {&h->tc_dirs, &h->tc_jvp_dirs, &h->tc_w_dirs})
+    for (TcDir& d : *dirs) {
+      d.order = order;
+      d.by_mpairs.clear();                    // the uploaded tables stay in h->allocs until dgan_destroy
+    }
   for (auto& g : h->graphs) cudaGraphExecDestroy(g.exec);
   h->graphs.clear();
   return DGAN_OK;
@@ -3135,7 +3170,7 @@ static int plan_stats_impl(const dgan_desc* d, int n_rows, int n_pairs, int forc
     Tc2Plan plan;
     const bool forced = (int)di == force_dir;
     const int rc = tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, forced ? force_maxb : 0, dr.epi, dr.out_bytes,
-                            n_mpairs, n_pairs, &plan, forced ? force_shape : nullptr);
+                            n_mpairs, n_pairs, dr.order, tc2_band_reverse(dr.ld), &plan, forced ? force_shape : nullptr);
     if (rc) return -1;
     char line[320];
     const double mb = (double)plan.n_bytes / 1e6;
@@ -3168,6 +3203,43 @@ int dgan_debug_plan_stats_window(const dgan_desc* d, int n_rows, int n_pairs, in
   return plan_stats_impl(d, n_rows, n_pairs, force_dir, force_maxb, shape, buf, buf_len);
 }
 
+// Host-only developer aid (not in the public header): the item order of every layer-direction's plan in item order
+// `order` (Tc2Order) - the order the planner kept (it falls back to LPT when bands would unbalance the pairs), the row
+// pairs per band, the busiest CTA pair's load under LPT and under the kept order (cost-model us), the bytes staged into
+// shared memory as activation tiles (both CTAs) and as weight tiles, the distinct activation tiles read (the input
+// tensor), and the working set: the peak, over the cost model's timeline of every pair, of the bytes of activation tiles
+// between their first and last load - as text, one line per layer-direction in the order of dgan_debug_plan_stats.
+// Returns the length, or -1.
+int dgan_debug_plan_order_stats(const dgan_desc* d, int n_rows, int n_pairs, int order, char* buf, int buf_len) {
+  using namespace dgan;
+  if (d == nullptr || n_rows <= 0 || n_pairs <= 0 || buf == nullptr || buf_len <= 0 ||
+      (order != TC2_ORDER_LPT && order != TC2_ORDER_BAND)) {
+    set_error("invalid argument");
+    return -1;
+  }
+  const int n_pad = ((n_rows + 2 * kRowTile - 1) / (2 * kRowTile)) * 2 * kRowTile, n_mpairs = n_pad / (2 * kRowTile);
+  Widths wd;
+  if (padded_widths(d, &wd) != 0) return -1;
+  std::string out = "direction | order | band row pairs | busiest pair: LPT us | busiest pair: order us | staged A MB"
+                    " | staged weight MB | unique input MB | working set MB\n";
+  for (const TcDir& dr : tc_directions(d)) {
+    Tc2Plan plan;
+    if (tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, order,
+                 tc2_band_reverse(dr.ld), &plan))
+      return -1;
+    char line[240];
+    snprintf(line, sizeof line, "%s | %s | %d | %.1f | %.1f | %.1f | %.1f | %.1f | %.1f\n", dr.name.c_str(),
+             plan.order == TC2_ORDER_BAND ? (tc2_band_reverse(dr.ld) ? "band-" : "band+") : "lpt", plan.band_rows,
+             plan.load_max / 1e3, plan.load_max_order / 1e3, plan.n_bytes_a / 1e6, plan.n_bytes_b / 1e6,
+             plan.uniq_a_bytes / 1e6, plan.ws_a_bytes / 1e6);
+    out += line;
+  }
+  const int n = (int)std::min(out.size(), (size_t)buf_len - 1);
+  memcpy(buf, out.data(), (size_t)n);
+  buf[n] = 0;
+  return n;
+}
+
 // Host-only developer aid (not in the public header): what the kernel issues for the plan of every layer-direction -
 // the slots per round, the k16 MMAs issued (the real ones, and the zero-tile ones where the round is fixed:
 // tc2_issues_zero_ops), the zero-tile k16 MMAs the kernel skips, and the MMA term of the busiest CTA pair's load for the
@@ -3182,7 +3254,9 @@ int dgan_debug_plan_issue_stats(const dgan_desc* d, int n_rows, int n_pairs, cha
   std::string out = "direction | slots | k16 MMAs issued | zero-tile k16 MMAs skipped | busiest pair: est. tensor us, issued\n";
   for (const TcDir& dr : tc_directions(d)) {
     Tc2Plan plan;
-    if (tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, &plan)) return -1;
+    if (tc2_plan(dr.N, dr.K, dr.tab, dr.h_grid, dr.w_grid, dr.max_acc, 0, dr.epi, dr.out_bytes, n_mpairs, n_pairs, dr.order,
+                 tc2_band_reverse(dr.ld), &plan))
+      return -1;
     char line[200];
     snprintf(line, sizeof line, "%s | %d | %lld | %lld | %.1f\n", dr.name.c_str(), plan.maxb, plan.n_issued * plan.ksub,
              (plan.n_mma - plan.n_issued) * plan.ksub, plan.op_ns_issued_max / 1e3);

@@ -22,6 +22,8 @@
 //     step the consumer waits for all MMAs and runs the epilogue straight from the registers.  Each consumer warp
 //     stores the 16 rows it holds with its own TMA store.
 #pragma once
+#include <unordered_map>
+
 #include "kernels_tc.cuh"
 #include "tc_records.cuh"
 
@@ -1053,6 +1055,10 @@ struct Tc2Schedule {           // one window tiling of a layer-direction + its i
 };
 // 64-channel or 16-channel TMA box for operands of K channels (tc_make_map)
 static uint32_t tc2_box_k(int K) { return tc2_ksub(K) == 4 ? 64u : 16u; }
+// The order in which the CTA pairs take a layer-direction's items (window, row pair), see tc2_search.  LPT: largest
+// first over the whole batch.  BAND: row pairs in bands that every pair walks in the same order, so an activation
+// tile's re-reads fall close together in time and hit L2; the default.
+enum Tc2Order { TC2_ORDER_LPT = 0, TC2_ORDER_BAND = 1 };
 // One layer-direction of the fp16 path: out[P_out][rows][N] = epi(pixel graph `tab` over in[P_in][rows][K] and n_tiles
 // [N][K] weight tiles).  dgan_api.cu's tc_directions() fills the description from the generator's desc alone; a handle
 // adds the weight tiles, their tensor map and the schedules planned for its row counts.
@@ -1072,6 +1078,7 @@ struct TcDir {
   __half* w = nullptr;         // [n_tiles][N][K] fp16, K contiguous
   CUtensorMap tm_b{};          // box {64 | 16, N/2, 1}: the half of a weight tile (sub-tile) one CTA of the pair loads
   int force_maxb = 0;          // > 0: plan with exactly this many accumulator slots per round (dgan_debug_force_slots)
+  int order = TC2_ORDER_BAND;  // item order (Tc2Order; dgan_debug_force_order)
   std::vector<std::pair<int, Tc2Schedule>> by_mpairs;   // uploaded schedule per n_mpairs (tc2_get_schedule)
 };
 
@@ -1264,6 +1271,21 @@ static void tc2_enumerate_windows(int h_grid, int w_grid, int wh, int ww, int sy
 #ifndef TC2_REFINE_BUDGET
 #define TC2_REFINE_BUDGET (1LL << 26)    // candidate evaluations of the assignment refinement per window shape (tc2_search)
 #endif
+// Banded order (tc2_search): the input and output bytes of one band's row pairs stay within this share of the 50 MB L2,
+// and the banded assignment is kept while its makespan is within TC2_BAND_TOLERANCE of LPT's.  On an H100 (DESIGN.md
+// section 6) the banded directions ran up to 16 % faster and none slower while their makespans were up to 1.7 % worse.
+// A direction whose whole input is smaller than TC2_BAND_MIN_INPUT stays in L2 in any order and keeps LPT: the last
+// layer's backward on MNIST (4 and 8 MB of input) ran 5 - 7 % slower in bands, CelebA's Generator.2 forward (10.5 MB)
+// 2 - 3 % faster.
+#ifndef TC2_BAND_L2_BYTES
+#define TC2_BAND_L2_BYTES (16 << 20)
+#endif
+#ifndef TC2_BAND_TOLERANCE
+#define TC2_BAND_TOLERANCE 0.02
+#endif
+#ifndef TC2_BAND_MIN_INPUT
+#define TC2_BAND_MIN_INPUT (9 << 20)
+#endif
 
 // The planner.  tc2_search picks the accumulator slots per round and the window tiling for `n_mpairs` row pairs on
 // `n_pairs` CTA pairs and assigns the items to the pairs; tc2_encode_streams lays each pair's steps out in its operand
@@ -1278,9 +1300,16 @@ struct Tc2Plan {               // host result of the planner (what tc2_get_sched
   // ops of the rounds' slots (rounds x slots, KSUB k16 MMAs each), the zero-tile ones among them, ops issued (the real
   // ones, and the zero-tile ones where the instantiation issues them)
   long long n_mma = 0, n_pad = 0, n_issued = 0, n_steps = 0, n_bytes = 0;
-  double load_max = 0.0, load_mean = 0.0;   // cost-model load of the busiest CTA pair / the mean over pairs (balance of the LPT assignment)
-  double op_ns_max = 0.0;      // the MMA term of the busiest pair's load (estimated tensor time, ns)
+  long long n_bytes_a = 0, n_bytes_b = 0;   // n_bytes split: activation tiles (both CTAs) and weight tiles (multicast)
+  long long uniq_a_bytes = 0;  // the distinct activation tiles the plan reads (both CTAs): its input tensor
+  // peak, over the cost model's timeline of every pair, of the bytes of activation tiles between their first and last load
+  long long ws_a_bytes = 0;
+  // cost-model load of the busiest CTA pair / the mean over pairs of the LPT assignment (the window shape's score)
+  double load_max = 0.0, load_mean = 0.0;
+  double op_ns_max = 0.0;      // the MMA term of that busiest pair's load (estimated tensor time, ns)
   double op_ns_issued_max = 0.0;   // the same term for the ops the kernel issues (n_issued)
+  int order = TC2_ORDER_LPT, band_rows = 0;   // the order the plan uses (Tc2Order) and its row pairs per band
+  double load_max_order = 0.0;  // the busiest pair's load under that order
   int maxb = 1, ring_bytes = 0;   // accumulator slots per round of the chosen instantiation, its operand ring
   int ksub = 4;                   // k16 MMAs per op of the instantiation (tc2_ksub)
 };
@@ -1289,16 +1318,115 @@ static double tc2_op_ns(int N, int ksub) {
   return DGAN_COST_OP_NS * (double)std::max(N, DGAN_COST_OP_MIN_N) / 64.0 * (double)ksub / 4.0;
 }
 
+// The time model's cost of one item (ns)
+static double tc2_item_cost(const Tc2HostItem& it, int N, double op_ns) {
+  return DGAN_COST_NS_PER_KB / 1024.0 *
+             (it.stage_bytes + DGAN_COST_EPI_KB * 1024.0 * it.hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0) +
+         op_ns * (double)it.n_ops + DGAN_COST_STEP_NS * (double)it.steps.size();
+}
+
+// Band of item idx (window * n_mpairs + row pair) in time order: row pairs [b * band_rows, (b + 1) * band_rows) form band
+// b, walked from the last band to the first when `reverse`.
+static int tc2_band_of(int idx, int n_mpairs, int band_rows, bool reverse) {
+  const int b = (idx % n_mpairs) / band_rows, n_bands = (n_mpairs + band_rows - 1) / band_rows;
+  return reverse ? n_bands - 1 - b : b;
+}
+
+// Assign the items (window w, row pair mp; index w * n_mpairs + mp, cost icost[w]) to the CTA pairs: each in turn to the
+// currently least-loaded pair, then refine, then order each pair's list.  band_rows = 0 (LPT): items in index order
+// (windows sorted by staged bytes, mp the fast index: cost-descending), each pair's list largest first.  band_rows > 0
+// (BAND): items by (band, cost descending), so every pair works through the bands in the same order; the refinement
+// swaps items of one band only, and each list is sorted by (band, cost descending).  No pair takes more than max_items
+// items (0: no limit).  Returns the makespan.
+static double tc2_assign(const std::vector<double>& icost, int n_mpairs, int n_pairs, int band_rows, bool reverse,
+                         size_t max_items, std::vector<std::vector<int>>* lists_out, std::vector<double>* load_out) {
+  const long long total = (long long)icost.size() * n_mpairs;
+  auto cost_of = [&](int idx) { return icost[(size_t)(idx / n_mpairs)]; };
+  auto band_of = [&](int idx) { return band_rows > 0 ? tc2_band_of(idx, n_mpairs, band_rows, reverse) : 0; };
+  std::vector<int> seq((size_t)total);
+  std::iota(seq.begin(), seq.end(), 0);
+  if (band_rows > 0)
+    std::stable_sort(seq.begin(), seq.end(), [&](int a, int b) {
+      return band_of(a) != band_of(b) ? band_of(a) < band_of(b) : cost_of(a) > cost_of(b);
+    });
+  std::vector<double>& load = *load_out;
+  std::vector<std::vector<int>>& lists = *lists_out;
+  load.assign((size_t)n_pairs, 0.0);
+  lists.assign((size_t)n_pairs, {});
+  const size_t cap = max_items > 0 ? max_items : (size_t)total;
+  for (int idx : seq) {
+    size_t best = (size_t)n_pairs;
+    for (size_t pr = 0; pr < (size_t)n_pairs; ++pr)
+      if (lists[pr].size() < cap && (best == (size_t)n_pairs || load[pr] < load[best])) best = pr;
+    load[best] += cost_of(idx);
+    lists[best].push_back(idx);
+  }
+  // Refinement: while the busiest pair can hand an item to - or swap one with - another pair so that both end
+  // up below its load, do the best such move (LPT alone leaves e.g. 35 on a mean of 30.4 for Generator.2 bwd's
+  // 160 items of cost 4..25).
+  // One pass looks at |P| x (1 + |Q|) candidates for every other pair Q: quadratic in the items per pair.  With many
+  // items per pair (large batches: 160 row pairs x 1024 windows) LPT alone is already within one small item of
+  // the mean and the search would take minutes, so it runs on a budget of candidate evaluations that the
+  // benchmarked sizes (<= 20 row pairs) never reach.
+  long long work = 0;
+  for (int iter = 0; iter < 4096 && work < TC2_REFINE_BUDGET; ++iter) {
+    const size_t P = (size_t)(std::max_element(load.begin(), load.end()) - load.begin());
+    double best_peak = load[P];
+    size_t bq = P; int bi = -1, bj = -1;
+    for (size_t Q = 0; Q < (size_t)n_pairs; ++Q) {
+      if (Q == P) continue;
+      work += (long long)lists[P].size() * (long long)(1 + lists[Q].size());
+      for (size_t i = 0; i < lists[P].size(); ++i) {
+        const double ci = cost_of(lists[P][i]);
+        double peak = std::max(load[P] - ci, load[Q] + ci);           // move i: P -> Q
+        if (lists[Q].size() < cap && peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = -1; }
+        for (size_t j = 0; j < lists[Q].size(); ++j) {                 // swap i <-> j
+          const double cj = cost_of(lists[Q][j]);
+          if (cj >= ci || band_of(lists[Q][j]) != band_of(lists[P][i])) continue;
+          peak = std::max(load[P] - ci + cj, load[Q] + ci - cj);
+          if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = (int)j; }
+        }
+      }
+    }
+    if (bi < 0) break;
+    const int it_i = lists[P][(size_t)bi];
+    const double ci = cost_of(it_i);
+    if (bj < 0) {
+      lists[P].erase(lists[P].begin() + bi);
+      lists[bq].push_back(it_i);
+      load[P] -= ci; load[bq] += ci;
+    } else {
+      const int it_j = lists[bq][(size_t)bj];
+      const double cj = cost_of(it_j);
+      lists[P][(size_t)bi] = it_j; lists[bq][(size_t)bj] = it_i;
+      load[P] += cj - ci; load[bq] += ci - cj;
+    }
+  }
+  // biggest first within a band: a pair's last item is its smallest (shortest un-overlapped epilogue)
+  for (auto& l : lists)
+    std::stable_sort(l.begin(), l.end(), [&](int a, int b) {
+      return band_of(a) != band_of(b) ? band_of(a) < band_of(b) : cost_of(a) > cost_of(b);
+    });
+  return *std::max_element(load.begin(), load.end());
+}
+
 // Every candidate - an instantiation of TC2_KINDS for (N, epilogue, output type) and a shape of wh x ww <= its slots
 // accumulators, strides 1 or 2 - is scored by an LPT assignment of its items (window, row pair) to the CTA pairs with
 // the time model above (operand bytes staged, a per-accumulator epilogue charge, a fixed per-item charge, and the ops
 // of the rounds' slots, zero-tile ones included even where the kernel skips them: the constants were fitted to kernels
-// that issued them); the smallest makespan wins.  Fills the plan's shape, slots, ring and loads, and
-// returns the winner's items and, per CTA pair, its item indices (window * n_mpairs + row pair) in issue order.
-// force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
+// that issued them); the smallest makespan wins.  With order BAND the winner's items are then assigned again in bands
+// of row pairs (tc2_assign): as few row pairs per band as give every CTA pair about one item, and no more than keep the
+// band's input and output within TC2_BAND_L2_BYTES.  Under LPT every pair works on windows of similar cost across all
+// row pairs at once, so a tile read by an early (interior) and a late (boundary) window is fetched from L2 twice only if
+// the whole input stays there; in bands it is re-read while its band runs.  The banded assignment is kept unless its
+// makespan exceeds LPT's by more than TC2_BAND_TOLERANCE.  `reverse` walks the bands from the last row pair down:
+// alternated from one layer-direction to the next, a kernel starts on the rows its predecessor wrote last.  Fills the
+// plan's shape, slots, ring, order and loads, and returns the winner's items and, per CTA pair, its item indices
+// (window * n_mpairs + row pair) in issue order.  force_shape (statistics only): consider only this window shape
+// {wh, ww, sy, sx}.
 static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
-                      int out_bytes, int n_mpairs, int n_pairs, const int* force_shape, Tc2Plan* plan,
-                      std::vector<Tc2HostItem>* best_items, std::vector<std::vector<int>>* best_lists) {
+                      int out_bytes, int n_mpairs, int n_pairs, int order, bool reverse, const int* force_shape,
+                      Tc2Plan* plan, std::vector<Tc2HostItem>* best_items, std::vector<std::vector<int>>* best_lists) {
   const int max_a = TC2_MAX_A;
   // Step size: a step is consumed only once all of it has landed, so big steps cost pipeline depth (4 x 48 KB fit the
   // ring); 48 KB holds one activation tile and one whole N = 256 weight tile.  The N = 64, K = 128 layer (Generator.3
@@ -1311,6 +1439,7 @@ static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid
   double best_cost = 1e300;
   plan->maxb = 0;
   std::vector<std::vector<int>> wins;
+  std::vector<double> best_load;
   for (const Tc2Kind& kind : kTc2Kinds) {
     if (kind.n != N || kind.ksub != ksub || kind.epi != epi || kind.out_bytes != out_bytes) continue;
     if (force_maxb > 0 && kind.maxb != force_maxb) continue;
@@ -1325,92 +1454,71 @@ static int tc2_search(int N, int K, const PairTable& tab, int h_grid, int w_grid
             tc2_enumerate_windows(h_grid, std::max(w_grid, 1), wh, ww, sy, sx, &wins);
             std::vector<Tc2HostItem> items(wins.size());
             for (size_t i = 0; i < wins.size(); ++i) tc2_build_item(tab, wins[i], N, K, mb, max_a, step_max, &items[i]);
-            std::vector<double> icost(items.size());
-            auto cost_item = [&](const Tc2HostItem& it) {
-              return DGAN_COST_NS_PER_KB / 1024.0 *
-                         (it.stage_bytes + DGAN_COST_EPI_KB * 1024.0 * it.hdr.n_acc * std::max(1, N / 64) + DGAN_COST_FIXED_KB * 1024.0) +
-                     op_ns * (double)it.n_ops + DGAN_COST_STEP_NS * (double)it.steps.size();
-            };
             std::stable_sort(items.begin(), items.end(), [](const Tc2HostItem& l, const Tc2HostItem& r) { return l.stage_bytes > r.stage_bytes; });
-            for (size_t i = 0; i < items.size(); ++i) icost[i] = cost_item(items[i]);
-            // LPT: items (window, mp) largest-first, each to the currently least-loaded CTA pair
-            const long long total = (long long)items.size() * n_mpairs;
-            std::vector<double> load((size_t)n_pairs, 0.0);
-            std::vector<std::vector<int>> lists((size_t)n_pairs);
-            for (long long idx = 0; idx < total; ++idx) {        // items[] is sorted by cost, mp is the fast index: cost-descending
-              size_t best = 0;
-              for (size_t pr = 1; pr < (size_t)n_pairs; ++pr)
-                if (load[pr] < load[best]) best = pr;
-              load[best] += icost[(size_t)(idx / n_mpairs)];
-              lists[best].push_back((int)idx);
-            }
-            // Refinement: while the busiest pair can hand an item to - or swap one with - another pair so that both end
-            // up below its load, do the best such move (LPT alone leaves e.g. 35 on a mean of 30.4 for Generator.2 bwd's
-            // 160 items of cost 4..25).
-            auto cost_of = [&](int idx) { return icost[(size_t)(idx / n_mpairs)]; };
-            // One pass looks at |P| x (1 + |Q|) candidates for every other pair Q: quadratic in the items per pair.  With many
-            // items per pair (large batches: 160 row pairs x 1024 windows) LPT alone is already within one small item of
-            // the mean and the search would take minutes, so it runs on a budget of candidate evaluations that the
-            // benchmarked sizes (<= 20 row pairs) never reach.
-            long long work = 0;
-            for (int iter = 0; iter < 4096 && work < TC2_REFINE_BUDGET; ++iter) {
-              const size_t P = (size_t)(std::max_element(load.begin(), load.end()) - load.begin());
-              double best_peak = load[P];
-              size_t bq = P; int bi = -1, bj = -1;
-              for (size_t Q = 0; Q < (size_t)n_pairs; ++Q) {
-                if (Q == P) continue;
-                work += (long long)lists[P].size() * (long long)(1 + lists[Q].size());
-                for (size_t i = 0; i < lists[P].size(); ++i) {
-                  const double ci = cost_of(lists[P][i]);
-                  double peak = std::max(load[P] - ci, load[Q] + ci);           // move i: P -> Q
-                  if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = -1; }
-                  for (size_t j = 0; j < lists[Q].size(); ++j) {                 // swap i <-> j
-                    const double cj = cost_of(lists[Q][j]);
-                    if (cj >= ci) continue;
-                    peak = std::max(load[P] - ci + cj, load[Q] + ci - cj);
-                    if (peak < best_peak - 1e-9) { best_peak = peak; bq = Q; bi = (int)i; bj = (int)j; }
-                  }
-                }
-              }
-              if (bi < 0) break;
-              const int it_i = lists[P][(size_t)bi];
-              const double ci = cost_of(it_i);
-              if (bj < 0) {
-                lists[P].erase(lists[P].begin() + bi);
-                lists[bq].push_back(it_i);
-                load[P] -= ci; load[bq] += ci;
-              } else {
-                const int it_j = lists[bq][(size_t)bj];
-                const double cj = cost_of(it_j);
-                lists[P][(size_t)bi] = it_j; lists[bq][(size_t)bj] = it_i;
-                load[P] += cj - ci; load[bq] += ci - cj;
-              }
-            }
-            for (auto& l : lists)      // biggest first: a pair's last item is its smallest (shortest un-overlapped epilogue)
-              std::stable_sort(l.begin(), l.end(), [&](int a, int b) { return cost_of(a) > cost_of(b); });
-            const double makespan = *std::max_element(load.begin(), load.end());
+            std::vector<double> icost(items.size());
+            for (size_t i = 0; i < items.size(); ++i) icost[i] = tc2_item_cost(items[i], N, op_ns);
+            std::vector<std::vector<int>> lists;
+            std::vector<double> load;
+            const double makespan = tc2_assign(icost, n_mpairs, n_pairs, 0, false, 0, &lists, &load);
             if (makespan < best_cost) {
               best_cost = makespan;
-              plan->load_max = makespan;
-              plan->load_mean = std::accumulate(load.begin(), load.end(), 0.0) / (double)n_pairs;
               plan->shape[0] = wh; plan->shape[1] = ww; plan->shape[2] = sy; plan->shape[3] = sx;
               plan->maxb = mb; plan->ring_bytes = ring;
-              plan->op_ns_max = 0.0;
-              plan->op_ns_issued_max = 0.0;
-              for (size_t pr = 0; pr < lists.size(); ++pr)
-                if (load[pr] == makespan) {
-                  for (int idx : lists[pr]) {
-                    plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
-                    plan->op_ns_issued_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_issued;
-                  }
-                  break;
-                }
-              best_items->swap(items); best_lists->swap(lists);
+              best_items->swap(items); best_lists->swap(lists); best_load.swap(load);
             }
           }
   }
   if (plan->maxb == 0) { set_error("no tensor-core kernel instantiation for this layer-direction"); return DGAN_ERR_UNSUPPORTED; }
   plan->ksub = ksub;
+  const std::vector<Tc2HostItem>& items = *best_items;
+  plan->load_max = best_cost;
+  plan->load_mean = std::accumulate(best_load.begin(), best_load.end(), 0.0) / (double)n_pairs;
+  plan->op_ns_max = 0.0;
+  plan->op_ns_issued_max = 0.0;
+  for (size_t pr = 0; pr < best_lists->size(); ++pr)
+    if (best_load[pr] == best_cost) {
+      for (int idx : (*best_lists)[pr]) {
+        plan->op_ns_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_ops;
+        plan->op_ns_issued_max += op_ns * (double)items[(size_t)(idx / n_mpairs)].n_issued;
+      }
+      break;
+    }
+  plan->order = TC2_ORDER_LPT;
+  plan->band_rows = 0;
+  plan->load_max_order = best_cost;
+  std::vector<double> icost(items.size());
+  for (size_t i = 0; i < items.size(); ++i) icost[i] = tc2_item_cost(items[i], N, op_ns);
+  if (order == TC2_ORDER_BAND && n_mpairs > 1) {
+    // one row pair's input (the distinct pixels the steps stage, K channels) and output, in bytes
+    std::vector<int> pix;
+    long long n_out = 0;
+    for (const Tc2HostItem& it : items) {
+      n_out += it.hdr.n_acc;
+      for (const Tc2HostStep& st : it.steps) pix.insert(pix.end(), st.a_pix, st.a_pix + st.nA);
+    }
+    std::sort(pix.begin(), pix.end());
+    const long long n_in = std::unique(pix.begin(), pix.end()) - pix.begin();
+    const long long mp_bytes = 2LL * kRowTile * (2LL * K * n_in + (long long)out_bytes * N * n_out);
+    const int fill = (n_pairs + (int)items.size() - 1) / (int)items.size();
+    const int fit = (int)std::max(1LL, (long long)TC2_BAND_L2_BYTES / std::max(mp_bytes, 1LL));
+    const int band_rows = std::min(n_mpairs, std::max(1, std::min(fill, fit)));
+    const long long in_bytes = 2LL * kRowTile * n_mpairs * 2LL * K * n_in;
+    if (band_rows < n_mpairs && in_bytes >= (long long)TC2_BAND_MIN_INPUT) {
+      std::vector<std::vector<int>> lists;
+      std::vector<double> load;
+      // no pair takes more items than the most LPT gives one: each item is an epilogue and an item head more for its
+      // pair, which the time model charges only as a fixed cost, and the epilogue item list keeps LPT's slots
+      size_t lpt_items = 0;
+      for (const auto& l : *best_lists) lpt_items = std::max(lpt_items, l.size());
+      const double makespan = tc2_assign(icost, n_mpairs, n_pairs, band_rows, reverse, lpt_items, &lists, &load);
+      if (makespan <= best_cost * (1.0 + TC2_BAND_TOLERANCE)) {
+        plan->order = TC2_ORDER_BAND;
+        plan->band_rows = band_rows;
+        plan->load_max_order = makespan;
+        best_lists->swap(lists);
+      }
+    }
+  }
   return 0;
 }
 
@@ -1431,9 +1539,14 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
   std::vector<TcRec>& stream_p = plan->stream_p;
   std::vector<TcRec>& stream_m = plan->stream_m;
   stream_p.clear(); stream_m.clear();
-  long long n_mma = 0, n_pad = 0, n_issued = 0, n_steps = 0, n_bytes = 0;
+  long long n_mma = 0, n_pad = 0, n_issued = 0, n_steps = 0, n_bytes_a = 0, n_bytes_b = 0;
+  // statistics: per activation tile (row pair, k-chunk, pixel) the first and last time a step loads it, on the time
+  // model's timeline of its CTA pair (a step at its share of the item's cost)
+  const double op_ns = tc2_op_ns(N, ksub);
+  std::unordered_map<long long, std::pair<double, double>> a_span;
   for (size_t pr = 0; pr < lists.size(); ++pr) {
     stream_off[pr] = (uint32_t)stream_m.size();
+    double t_item = 0.0;
     // circular operand ring of this CTA pair: sequential allocation, wrap when the step does not fit
     std::vector<std::pair<int, int>> region;     // [begin, end) in KB of every step of this stream
     int cursor = 0;
@@ -1442,8 +1555,15 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
       if ((uint32_t)win > TcItemWindow::mask || (uint32_t)mp > TcItemMp::mask) { set_error("tensor-core schedule limits exceeded"); return DGAN_ERR_UNSUPPORTED; }
       eitems[k * (size_t)n_pairs + pr] = tc2_item_word(win, mp);
       const Tc2HostItem& itm = items[(size_t)win];
+      const double c_item = tc2_item_cost(itm, N, op_ns);
       for (size_t j = 0; j < itm.steps.size(); ++j) {
         const Tc2HostStep& hs = itm.steps[j];
+        const double t = t_item + c_item * (double)j / (double)itm.steps.size();
+        for (int a = 0; a < hs.nA; ++a) {
+          const long long key = ((long long)mp * 16 + hs.kc) * 65536 + hs.a_pix[a];
+          auto ins = a_span.insert({key, {t, t}});
+          if (!ins.second) ins.first->second.second = t;
+        }
         const int kb = (hs.bytes + 1023) / 1024;
         if (kb * 1024 > ring_bytes) { set_error("tensor-core step larger than the operand ring"); return DGAN_ERR_UNSUPPORTED; }
         if (cursor + kb > ring_bytes / 1024) cursor = 0;
@@ -1472,24 +1592,40 @@ static int tc2_encode_streams(int N, int n_mpairs, int n_pairs, const std::vecto
         // bytes read from L2 by the pair: both activation tiles, each weight tile once (multicast)
         n_mma += hs.n_rounds * max_b; n_pad += hs.n_rounds * max_b - hs.n_real;
         n_issued += tc2_issues_zero_ops(max_b, ksub) ? hs.n_rounds * max_b : hs.n_real;
-        n_steps += 1; n_bytes += 2LL * hs.nA * tc2_a_bytes(ksub) + (long long)hs.nB * tc2_b_bytes(N, ksub);
+        n_steps += 1; n_bytes_a += 2LL * hs.nA * tc2_a_bytes(ksub); n_bytes_b += (long long)hs.nB * tc2_b_bytes(N, ksub);
       }
+      t_item += c_item;
     }
   }
+  std::vector<std::pair<double, int>> ev;       // (time, +1 first load / -1 after the last)
+  for (const auto& kv : a_span) { ev.push_back({kv.second.first, 1}); ev.push_back({kv.second.second, -1}); }
+  std::sort(ev.begin(), ev.end(), [](const auto& l, const auto& r) { return l.first != r.first ? l.first < r.first : l.second > r.second; });
+  long long live = 0, peak = 0;
+  for (const auto& e : ev) { live += e.second; peak = std::max(peak, live); }
+  plan->uniq_a_bytes = 2LL * tc2_a_bytes(ksub) * (long long)a_span.size();
+  plan->ws_a_bytes = 2LL * tc2_a_bytes(ksub) * peak;
   stream_off[(size_t)n_pairs] = (uint32_t)stream_m.size();
   plan->hdrs.resize(items.size());
   for (size_t i = 0; i < items.size(); ++i) plan->hdrs[i] = items[i].hdr;
-  plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_issued = n_issued; plan->n_steps = n_steps; plan->n_bytes = n_bytes;
+  plan->n_mma = n_mma; plan->n_pad = n_pad; plan->n_issued = n_issued; plan->n_steps = n_steps;
+  plan->n_bytes_a = n_bytes_a; plan->n_bytes_b = n_bytes_b; plan->n_bytes = n_bytes_a + n_bytes_b;
   return 0;
 }
 
-// The plan of one layer-direction.  force_shape (statistics only): consider only this window shape {wh, ww, sy, sx}.
+// Whether layer-direction ld (layer l forward = 2l, backward = 2l + 1) walks its bands in reverse: the directions run
+// forward l = 0, 1, .., then backward from the last layer down, so the position in that sequence alternates with
+// l + (ld & 1) - also from one L-step's last direction (Linear backward) to the next one's first.
+static bool tc2_band_reverse(int ld) { return (((ld >> 1) + (ld & 1)) & 1) != 0; }
+
+// The plan of one layer-direction (tc2_search).  force_shape (statistics only): consider only this window shape
+// {wh, ww, sy, sx}.
 static int tc2_plan(int N, int K, const PairTable& tab, int h_grid, int w_grid, int max_acc, int force_maxb, int epi,
-                    int out_bytes, int n_mpairs, int n_pairs, Tc2Plan* plan, const int* force_shape = nullptr) {
+                    int out_bytes, int n_mpairs, int n_pairs, int order, bool reverse, Tc2Plan* plan,
+                    const int* force_shape = nullptr) {
   std::vector<Tc2HostItem> items;
   std::vector<std::vector<int>> lists;
-  const int rc = tc2_search(N, K, tab, h_grid, w_grid, max_acc, force_maxb, epi, out_bytes, n_mpairs, n_pairs, force_shape,
-                            plan, &items, &lists);
+  const int rc = tc2_search(N, K, tab, h_grid, w_grid, max_acc, force_maxb, epi, out_bytes, n_mpairs, n_pairs, order,
+                            reverse, force_shape, plan, &items, &lists);
   return rc ? rc : tc2_encode_streams(N, n_mpairs, n_pairs, items, lists, plan);
 }
 
@@ -1635,7 +1771,8 @@ static int tc2_get_schedule(TcDir& d, int n_mpairs, int n_pairs, std::vector<voi
     if (kv.first == n_mpairs) return 0;
   Tc2Plan plan;
   int rc;
-  if ((rc = tc2_plan(d.N, d.K, d.tab, d.h_grid, d.w_grid, d.max_acc, d.force_maxb, d.epi, d.out_bytes, n_mpairs, n_pairs, &plan)))
+  if ((rc = tc2_plan(d.N, d.K, d.tab, d.h_grid, d.w_grid, d.max_acc, d.force_maxb, d.epi, d.out_bytes, n_mpairs, n_pairs,
+                     d.order, tc2_band_reverse(d.ld), &plan)))
     return rc;
   const cudaStream_t s = 0;
   Tc2Schedule sc;

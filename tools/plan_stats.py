@@ -8,7 +8,13 @@ every slot of every round, as the planner's time model does; the last three (def
 give what the kernel issues: the k16 MMAs issued, the zero-tile k16 MMAs it skips (rounds with 2 or 4 slots and
 64-channel ops issue only their real ops) and the busiest pair's estimated tensor time for the MMAs issued;
 --slots plans layer-direction DIR (the row index of the table, from 0) with exactly MAXB accumulator slots per round;
---window plans it on exactly the window WH x WW with strides (SY, SX), e.g. to compare two builds at the same window."""
+--window plans it on exactly the window WH x WW with strides (SY, SX), e.g. to compare two builds at the same window.
+A second table (default plans only) gives the item order of each plan (lpt, or band+ / band- with the direction the
+bands are walked in), its row pairs per band, the busiest pair's cost-model load under LPT and under that order, the
+bytes staged as activation tiles and as weight tiles, the unique input (the distinct activation tiles read) and the
+working set: the peak, over the cost model's timeline of every pair, of the bytes of activation tiles between their first
+and last load.  Set against the 50 MB L2, it shows without a GPU which directions the order can help; --order lpt gives
+the table for the LPT order."""
 import ctypes
 import os
 import sys
@@ -35,6 +41,11 @@ if "--window" in sys.argv:
     i = sys.argv.index("--window")
     d, shape = sys.argv[i + 1].split("=")
     force_dir, window = int(d), [int(v) for v in shape.split(",")]
+    del sys.argv[i:i + 2]
+order = 1
+if "--order" in sys.argv:
+    i = sys.argv.index("--order")
+    order = {"lpt": 0, "band": 1}[sys.argv[i + 1]]
     del sys.argv[i:i + 2]
 dataset = sys.argv[1] if len(sys.argv) > 1 else "mnist"
 batch = int(sys.argv[2]) if len(sys.argv) > 2 else 256
@@ -84,3 +95,11 @@ for line in lines[1:-1]:
                (" | " + issue[name] if name in issue else ""))
 out.append(lines[-1])
 print("\n".join(out))
+if window is None and force_dir < 0:
+    obuf = ctypes.create_string_buffer(1 << 16)
+    lib.dgan_debug_plan_order_stats.restype = ctypes.c_int
+    lib.dgan_debug_plan_order_stats.argtypes = [ctypes.POINTER(_native.dgan_desc), ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                ctypes.c_char_p, ctypes.c_int]
+    if lib.dgan_debug_plan_order_stats(ctypes.byref(desc), batch * R, pairs, order, obuf, len(obuf)) > 0:
+        print()
+        print(obuf.value.decode().strip())
