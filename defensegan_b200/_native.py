@@ -451,6 +451,73 @@ def _require_aligned_out(rec: torch.Tensor) -> None:
                          % (rec.data_ptr() % 16))
 
 
+def _float_ref(v: Optional[float]):
+    """A nullable const float* argument: NULL for None."""
+    return _byref_or_none(None if v is None else ctypes.c_float(v))
+
+
+_ENTRY_OF_KIND = {"image": "", "dense": "_measured", "csr": "_measured_csr", "conv": "_measured_conv"}
+
+
+def _route(kind: str, operands=(), m: int = 0, nnz: int = -1, conv: Optional[dgan_conv_op] = None, weighted: bool = False,
+           sched=None, ap: Optional[dgan_adam_params] = None, delta: Optional[float] = None, lam: Optional[float] = None,
+           sd: Optional[dgan_sparse_dev] = None, dev: Optional[torch.Tensor] = None):
+    """The sizer and the C entry of a projection with checked options, for an operator kind "image" (operands: the
+    images and the weights, or NULL), "dense" (a, m, y), "csr" (row_ptr, col_idx, val, m, nnz, y) or "conv" (op, k, y):
+    (sizer, its arguments after (handle, batch, rec_rr), entry, its arguments between dgan_rec_params and z0).  The
+    entry follows sparse_dev > z_prior > huber_delta > adam > prune > weighted / plain.  Huber and the prior run on
+    their counterpart's workspace, so the sizer follows sparse_dev > conv > adam > prune > the operator's own."""
+    measured = kind != "image"
+    n_points = len(sched) if sched is not None else 0
+    if sd is not None and measured:
+        sizer = ("dgan_workspace_bytes_measured_sparse_dev",
+                 (int(m), int(nnz), _byref_or_none(conv), int(ap is not None), sched, n_points))
+    elif sd is not None:
+        sizer = ("dgan_workspace_bytes_sparse_dev", (int(weighted), int(ap is not None), sched, n_points))
+    elif kind == "conv":
+        sizer = ("dgan_workspace_bytes_measured_conv", (ctypes.byref(conv), sched, n_points, int(ap is not None)))
+    elif ap is not None and measured:
+        sizer = ("dgan_workspace_bytes_measured_adam", (int(m), int(nnz), sched, n_points))
+    elif ap is not None:
+        sizer = ("dgan_workspace_bytes_adam", (int(weighted), sched, n_points))
+    elif sched is not None and measured:
+        sizer = ("dgan_workspace_bytes_measured_pruned", (int(m), int(nnz), sched, n_points))
+    elif sched is not None:
+        sizer = ("dgan_workspace_bytes_pruned", (sched, n_points, int(weighted)))
+    elif kind == "csr":
+        sizer = ("dgan_workspace_bytes_measured_csr", (int(m), int(nnz)))
+    elif kind == "dense":
+        sizer = ("dgan_workspace_bytes_measured", (int(m),))
+    else:
+        sizer = ("dgan_workspace_bytes_weighted" if weighted else "dgan_workspace_bytes", ())
+    entry = "dgan_reconstruct" + _ENTRY_OF_KIND[kind]
+    operands = tuple(operands)
+    if sd is not None:
+        options = (_byref_or_none(ap), _float_ref(delta), _float_ref(lam), sched, n_points, ctypes.byref(sd), _ptr(dev))
+        entry += "_sparse_dev"
+    elif lam is not None:
+        options = (_byref_or_none(ap), _float_ref(delta), lam, sched, n_points)
+        entry += "_prior"
+    elif kind == "conv":
+        options = (_byref_or_none(ap), _float_ref(delta), sched, n_points)
+    elif delta is not None:
+        options = (_byref_or_none(ap), delta, sched, n_points)
+        entry += "_huber"
+    elif ap is not None:
+        options = (ctypes.byref(ap), sched, n_points)
+        entry += "_adam"
+    elif sched is not None:
+        options = (sched, n_points)
+        entry += "_pruned"
+    else:
+        options = ()
+        if weighted:
+            entry += "_weighted"
+        elif not measured:
+            operands = operands[:1]              # dgan_reconstruct takes no weights
+    return sizer + (entry, options + operands)
+
+
 class NativeGenerator:
     """Owns one dgan_handle (the generator's re-laid-out weights on one GPU)."""
 
@@ -502,35 +569,15 @@ class NativeGenerator:
     # -- helpers -------------------------------------------------------------------------
     def _workspace(self, batch: int, rec_rr: int, weighted: bool = False, m: int = 0, nnz: int = -1, sched=None,
                    adam: bool = False, conv: Optional[dgan_conv_op] = None, sdev: bool = False):
-        n_points = len(sched) if sched is not None else 0
-        if sdev and (m > 0 or conv is not None):
-            need = int(self.lib.dgan_workspace_bytes_measured_sparse_dev(
-                self._handle, batch, rec_rr, int(m), int(nnz), ctypes.byref(conv) if conv is not None else None, int(adam),
-                sched, n_points))
-        elif sdev:
-            need = int(self.lib.dgan_workspace_bytes_sparse_dev(self._handle, batch, rec_rr, int(weighted), int(adam), sched,
-                                                                n_points))
-        elif conv is not None:
-            need = int(self.lib.dgan_workspace_bytes_measured_conv(self._handle, batch, rec_rr, ctypes.byref(conv), sched,
-                                                                   len(sched) if sched is not None else 0, int(adam)))
-        elif adam and m > 0:
-            need = int(self.lib.dgan_workspace_bytes_measured_adam(self._handle, batch, rec_rr, int(m), int(nnz), sched,
-                                                                   len(sched) if sched is not None else 0))
-        elif adam:
-            need = int(self.lib.dgan_workspace_bytes_adam(self._handle, batch, rec_rr, int(weighted), sched,
-                                                          len(sched) if sched is not None else 0))
-        elif sched is not None and m > 0:
-            need = int(self.lib.dgan_workspace_bytes_measured_pruned(self._handle, batch, rec_rr, int(m), int(nnz), sched,
-                                                                     len(sched)))
-        elif sched is not None:
-            need = int(self.lib.dgan_workspace_bytes_pruned(self._handle, batch, rec_rr, sched, len(sched), int(weighted)))
-        elif m > 0 and nnz >= 0:
-            need = int(self.lib.dgan_workspace_bytes_measured_csr(self._handle, batch, rec_rr, int(m), int(nnz)))
-        elif m > 0:
-            need = int(self.lib.dgan_workspace_bytes_measured(self._handle, batch, rec_rr, int(m)))
-        else:
-            sizer = self.lib.dgan_workspace_bytes_weighted if weighted else self.lib.dgan_workspace_bytes
-            need = int(sizer(self._handle, batch, rec_rr))
+        """The workspace of a call with these options, sized by the sizer _route picks: (1024-byte aligned pointer,
+        bytes)."""
+        kind = "conv" if conv is not None else "csr" if m > 0 and nnz >= 0 else "dense" if m > 0 else "image"
+        sizer, args = _route(kind, (), m, nnz, conv, weighted, sched, dgan_adam_params() if adam else None,
+                             sd=dgan_sparse_dev() if sdev else None)[:2]
+        return self._workspace_of(sizer, args, batch, rec_rr)
+
+    def _workspace_of(self, sizer: str, args, batch: int, rec_rr: int):
+        need = int(getattr(self.lib, sizer)(self._handle, batch, rec_rr, *args))
         if need == 0:
             raise RuntimeError("dgan_workspace_bytes returned 0 (invalid batch / rec_rr)")
         if self._ws is None or self._ws.numel() < need + 1024:
@@ -612,71 +659,48 @@ class NativeGenerator:
         if rec_rr <= 0 or rec_iters <= 0 or batch <= 0:
             raise ValueError("batch, rec_rr and rec_iters must be positive")
         pw = self._pixel_weights(pixel_weights, batch)
+        rec, loss, idx = self._project("image", (_ptr(x), _ptr(pw)), batch, self.hwc, rec_rr, rec_iters, rec_lr, z_init_val,
+                                       seed, momentum, decay_lr, out, z_row_offset, prune, adam, huber_delta, z_prior,
+                                       sparse_dev, deviation_out, weighted=pw is not None)
+        rec = rec.view(images.shape) if out is None else rec
+        if return_aux:
+            return rec, loss, idx
+        return rec
+
+    def _project(self, kind: str, operands, batch: int, m: int, rec_rr: int, rec_iters: int, rec_lr: float, z_init_val,
+                 seed: int, momentum: float, decay_lr: bool, out, z_row_offset: int, prune, adam, huber_delta, z_prior,
+                 sparse_dev, deviation_out, weighted: bool = False, nnz: int = -1, conv: Optional[dgan_conv_op] = None):
+        """reconstruct and reconstruct_measured after their operator's checks: the options checked, then the call _route
+        picks for the operator kind and its C arguments `operands` (m: the measurements, H*W*C for images).  Returns
+        (rec [B*H*W*C], loss, idx)."""
         sched = self._schedule(prune, rec_rr, rec_iters)
         ap = self._adam(adam)
         delta = None if huber_delta is None else check_huber_delta(huber_delta)
         lam = None if z_prior is None else check_z_prior(z_prior)
-        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, self.hwc)
+        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, m)
         z0 = None
         if z_init_val is not None:
             z0 = _require_cuda_f32(z_init_val, "z_init_val")
             if z0.numel() != batch * rec_rr * self.latent_dim:
                 raise ValueError("z_init_val must be [B*rec_rr, latent_dim]")
         with torch.cuda.device(self.device):
-            rec = out if out is not None else torch.empty_like(x)
-            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == x.numel()):
-                raise ValueError("out must be a contiguous CUDA float32 tensor shaped like images")
+            rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
+            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
+                raise ValueError("out must be a contiguous CUDA float32 tensor " +
+                                 ("shaped like images" if kind == "image" else
+                                  "of B*%d*%d*%d elements" % self.image_dim))
             _require_aligned_out(rec)
             loss = torch.empty(batch, dtype=torch.float32, device=self.device)
             idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None, sched=sched, adam=ap is not None,
-                                       sdev=sd is not None)
+            sizer, sizer_args, entry, args = _route(kind, operands, m, nnz, conv, weighted, sched, ap, delta, lam, sd, dev)
+            ws, need = self._workspace_of(sizer, sizer_args, batch, rec_rr)
             stream = torch.cuda.current_stream(self.device).cuda_stream
             prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
                                   seed & (2 ** 64 - 1), int(z_row_offset))
-            if sd is not None:
-                rc = self.lib.dgan_reconstruct_sparse_dev(
-                    self._handle, ctypes.byref(prm), _byref_or_none(ap),
-                    _byref_or_none(None if delta is None else ctypes.c_float(delta)),
-                    _byref_or_none(None if lam is None else ctypes.c_float(lam)), sched,
-                    len(sched) if sched is not None else 0, ctypes.byref(sd), _ptr(dev), _ptr(x), _ptr(pw), _ptr(z0),
-                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_sparse_dev")
-            elif lam is not None:
-                rc = self.lib.dgan_reconstruct_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
-                                                     _byref_or_none(None if delta is None else ctypes.c_float(delta)), lam,
-                                                     sched, len(sched) if sched is not None else 0, _ptr(x), _ptr(pw),
-                                                     _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                     ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_prior")
-            elif delta is not None:
-                rc = self.lib.dgan_reconstruct_huber(self._handle, ctypes.byref(prm), ctypes.byref(ap) if ap is not None
-                                                     else None, delta, sched, len(sched) if sched is not None else 0,
-                                                     _ptr(x), _ptr(pw), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                     ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_huber")
-            elif ap is not None:
-                rc = self.lib.dgan_reconstruct_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
-                                                    len(sched) if sched is not None else 0, _ptr(x), _ptr(pw), _ptr(z0),
-                                                    _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_adam")
-            elif sched is not None:
-                rc = self.lib.dgan_reconstruct_pruned(self._handle, ctypes.byref(prm), sched, len(sched), _ptr(x), _ptr(pw),
-                                                      _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                      ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_pruned")
-            elif pw is None:
-                rc = self.lib.dgan_reconstruct(self._handle, ctypes.byref(prm), _ptr(x), _ptr(z0), _ptr(rec), _ptr(loss),
-                                               _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct")
-            else:
-                rc = self.lib.dgan_reconstruct_weighted(self._handle, ctypes.byref(prm), _ptr(x), _ptr(pw), _ptr(z0),
-                                                        _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_weighted")
-        rec = rec.view(images.shape) if out is None else rec
-        if return_aux:
-            return rec, loss, idx
-        return rec
+            rc = getattr(self.lib, entry)(self._handle, ctypes.byref(prm), *args, _ptr(z0), _ptr(rec), _ptr(loss),
+                                          _ptr(idx), ws, need, ctypes.c_void_p(stream))
+            _check(self.lib, rc, entry)
+        return rec, loss, idx
 
     def _schedule(self, prune, rec_rr: int, rec_iters: int):
         """A prune schedule as the dgan_prune_point array of the pruned entries (None stays None), checked with
@@ -765,61 +789,6 @@ class NativeGenerator:
         op = dgan_conv_op(kh, kw, operator.padding[0], operator.padding[1], operator.stride)
         return y, k, op, batch, m
 
-    def _reconstruct_measured_conv(self, measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed, momentum,
-                                   decay_lr, out, return_aux, z_row_offset, prune, adam, huber_delta, z_prior, sparse_dev,
-                                   deviation_out):
-        """reconstruct_measured for a ConvOperator (dgan_reconstruct_measured_conv, or dgan_reconstruct_measured_conv_prior
-        with z_prior, or dgan_reconstruct_measured_conv_sparse_dev with sparse_dev)."""
-        y, k, op, batch, m = self._measured_conv(measurements, operator)
-        if rec_rr <= 0 or rec_iters <= 0:
-            raise ValueError("rec_rr and rec_iters must be positive")
-        sched = self._schedule(prune, rec_rr, rec_iters)
-        ap = self._adam(adam)
-        delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
-        lam = None if z_prior is None else check_z_prior(z_prior)
-        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, m)
-        z0 = None
-        if z_init_val is not None:
-            z0 = _require_cuda_f32(z_init_val, "z_init_val")
-            if z0.numel() != batch * rec_rr * self.latent_dim:
-                raise ValueError("z_init_val must be [B*rec_rr, latent_dim]")
-        with torch.cuda.device(self.device):
-            rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
-            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
-                raise ValueError("out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements" % self.image_dim)
-            _require_aligned_out(rec)
-            loss = torch.empty(batch, dtype=torch.float32, device=self.device)
-            idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, sched=sched, adam=ap is not None, conv=op, sdev=sd is not None)
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
-                                  seed & (2 ** 64 - 1), int(z_row_offset))
-            n_points = len(sched) if sched is not None else 0
-            if sd is not None:
-                rc = self.lib.dgan_reconstruct_measured_conv_sparse_dev(
-                    self._handle, ctypes.byref(prm), _byref_or_none(ap), _byref_or_none(delta),
-                    _byref_or_none(None if lam is None else ctypes.c_float(lam)), sched, n_points, ctypes.byref(sd),
-                    _ptr(dev), ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                    ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_conv_sparse_dev")
-            elif lam is not None:
-                rc = self.lib.dgan_reconstruct_measured_conv_prior(self._handle, ctypes.byref(prm), _byref_or_none(ap),
-                                                                   _byref_or_none(delta), lam, sched, n_points,
-                                                                   ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0), _ptr(rec),
-                                                                   _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_conv_prior")
-            else:
-                rc = self.lib.dgan_reconstruct_measured_conv(self._handle, ctypes.byref(prm),
-                                                             ctypes.byref(ap) if ap is not None else None,
-                                                             ctypes.byref(delta) if delta is not None else None, sched,
-                                                             n_points, ctypes.byref(op), _ptr(k), _ptr(y), _ptr(z0),
-                                                             _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                             ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_conv")
-        if return_aux:
-            return rec, loss, idx
-        return rec
-
     def reconstruct_measured(self, measurements: torch.Tensor, operator: torch.Tensor, rec_rr: int, rec_iters: int,
                              rec_lr: float = 10.0, z_init_val: Optional[torch.Tensor] = None, seed: int = 0,
                              momentum: float = 0.7, decay_lr: bool = False, out: Optional[torch.Tensor] = None,
@@ -850,108 +819,21 @@ class NativeGenerator:
         sparse_dev, deviation_out: the sparse deviations of reconstruct, fitting A (G(z) + nu) to y with D's 1/m
         normaliser (dgan_reconstruct_measured[_csr / _conv]_sparse_dev, with any of prune, adam, huber_delta and z_prior);
         nu lives in pixel space.  None runs the call without deviations as before."""
+        nnz, conv = -1, None
         if isinstance(operator, ConvOperator):
-            return self._reconstruct_measured_conv(measurements, operator, rec_rr, rec_iters, rec_lr, z_init_val, seed,
-                                                   momentum, decay_lr, out, return_aux, z_row_offset, prune, adam,
-                                                   huber_delta, z_prior, sparse_dev, deviation_out)
-        csr = operator.layout == torch.sparse_csr
-        if csr:
+            y, k, conv, batch, m = self._measured_conv(measurements, operator)
+            kind, operands = "conv", (ctypes.byref(conv), _ptr(k), _ptr(y))
+        elif operator.layout == torch.sparse_csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
+            kind, operands = "csr", (_ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y))
         else:
             y, a, batch, m = self._measured(measurements, operator)
+            kind, operands = "dense", (_ptr(a), m, _ptr(y))
         if rec_rr <= 0 or rec_iters <= 0:
             raise ValueError("rec_rr and rec_iters must be positive")
-        sched = self._schedule(prune, rec_rr, rec_iters)
-        ap = self._adam(adam)
-        delta = None if huber_delta is None else check_huber_delta(huber_delta)
-        lam = None if z_prior is None else check_z_prior(z_prior)
-        sd, dev = self._sparse_dev(sparse_dev, deviation_out, batch, m)
-        z0 = None
-        if z_init_val is not None:
-            z0 = _require_cuda_f32(z_init_val, "z_init_val")
-            if z0.numel() != batch * rec_rr * self.latent_dim:
-                raise ValueError("z_init_val must be [B*rec_rr, latent_dim]")
-        with torch.cuda.device(self.device):
-            rec = out if out is not None else torch.empty((batch,) + self.image_dim, dtype=torch.float32, device=self.device)
-            if not (rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == batch * self.hwc):
-                raise ValueError("out must be a contiguous CUDA float32 tensor of B*%d*%d*%d elements" % self.image_dim)
-            _require_aligned_out(rec)
-            loss = torch.empty(batch, dtype=torch.float32, device=self.device)
-            idx = torch.empty(batch, dtype=torch.int32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1, sched=sched, adam=ap is not None,
-                                       sdev=sd is not None)
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            prm = dgan_rec_params(batch, int(rec_rr), int(rec_iters), float(rec_lr), float(momentum), int(bool(decay_lr)),
-                                  seed & (2 ** 64 - 1), int(z_row_offset))
-            n_points = len(sched) if sched is not None else 0
-            apr = ctypes.byref(ap) if ap is not None else None
-            dpr = _byref_or_none(None if delta is None else ctypes.c_float(delta))
-            if sd is not None:
-                lpr = _byref_or_none(None if lam is None else ctypes.c_float(lam))
-                if csr:
-                    rc = self.lib.dgan_reconstruct_measured_csr_sparse_dev(
-                        self._handle, ctypes.byref(prm), apr, dpr, lpr, sched, n_points, ctypes.byref(sd), _ptr(dev),
-                        _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws,
-                        need, ctypes.c_void_p(stream))
-                    _check(self.lib, rc, "dgan_reconstruct_measured_csr_sparse_dev")
-                else:
-                    rc = self.lib.dgan_reconstruct_measured_sparse_dev(
-                        self._handle, ctypes.byref(prm), apr, dpr, lpr, sched, n_points, ctypes.byref(sd), _ptr(dev),
-                        _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                    _check(self.lib, rc, "dgan_reconstruct_measured_sparse_dev")
-            elif lam is not None and csr:
-                rc = self.lib.dgan_reconstruct_measured_csr_prior(self._handle, ctypes.byref(prm), apr, dpr, lam, sched,
-                                                                  n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
-                                                                  _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                                  ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_csr_prior")
-            elif lam is not None:
-                rc = self.lib.dgan_reconstruct_measured_prior(self._handle, ctypes.byref(prm), apr, dpr, lam, sched, n_points,
-                                                              _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
-                                                              ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_prior")
-            elif delta is not None and csr:
-                rc = self.lib.dgan_reconstruct_measured_csr_huber(self._handle, ctypes.byref(prm), apr, delta, sched, n_points,
-                                                                  _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
-                                                                  _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                                  ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_csr_huber")
-            elif delta is not None:
-                rc = self.lib.dgan_reconstruct_measured_huber(self._handle, ctypes.byref(prm), apr, delta, sched, n_points,
-                                                              _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
-                                                              ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_huber")
-            elif ap is not None and csr:
-                rc = self.lib.dgan_reconstruct_measured_csr_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
-                                                                 n_points, _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y),
-                                                                 _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                                 ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_csr_adam")
-            elif ap is not None:
-                rc = self.lib.dgan_reconstruct_measured_adam(self._handle, ctypes.byref(prm), ctypes.byref(ap), sched,
-                                                             n_points, _ptr(a), m, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss),
-                                                             _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_adam")
-            elif sched is not None and csr:
-                rc = self.lib.dgan_reconstruct_measured_csr_pruned(self._handle, ctypes.byref(prm), sched, len(sched),
-                                                                   _ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y), _ptr(z0),
-                                                                   _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                                   ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_csr_pruned")
-            elif sched is not None:
-                rc = self.lib.dgan_reconstruct_measured_pruned(self._handle, ctypes.byref(prm), sched, len(sched), _ptr(a), m,
-                                                               _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx), ws, need,
-                                                               ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_pruned")
-            elif csr:
-                rc = self.lib.dgan_reconstruct_measured_csr(self._handle, ctypes.byref(prm), _ptr(rp), _ptr(ci), _ptr(val),
-                                                            m, nnz, _ptr(y), _ptr(z0), _ptr(rec), _ptr(loss), _ptr(idx),
-                                                            ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured_csr")
-            else:
-                rc = self.lib.dgan_reconstruct_measured(self._handle, ctypes.byref(prm), _ptr(a), m, _ptr(y), _ptr(z0),
-                                                        _ptr(rec), _ptr(loss), _ptr(idx), ws, need, ctypes.c_void_p(stream))
-                _check(self.lib, rc, "dgan_reconstruct_measured")
+        rec, loss, idx = self._project(kind, operands, batch, m, rec_rr, rec_iters, rec_lr, z_init_val, seed, momentum,
+                                       decay_lr, out, z_row_offset, prune, adam, huber_delta, z_prior, sparse_dev,
+                                       deviation_out, nnz=nnz, conv=conv)
         if return_aux:
             return rec, loss, idx
         return rec
@@ -964,65 +846,47 @@ class NativeGenerator:
         reconstruct_measured (dgan_loss_grad_measured[_csr]_huber); None: the squared error.  A ConvOperator runs
         dgan_loss_grad_measured_conv."""
         if isinstance(operator, ConvOperator):
-            return self._loss_grad_measured_conv(measurements, operator, z, rec_rr, huber_delta)
-        csr = operator.layout == torch.sparse_csr
-        if csr:
+            y, k, conv, batch, m = self._measured_conv(measurements, operator)
+            return self._loss_grad("conv", (ctypes.byref(conv), _ptr(k), _ptr(y)), batch, z, rec_rr, huber_delta,
+                                   conv=conv)
+        if operator.layout == torch.sparse_csr:
             y, (rp, ci, val, nnz), batch, m = self._measured_csr(measurements, operator)
-        else:
-            y, a, batch, m = self._measured(measurements, operator)
-        zc = _require_cuda_f32(z, "z")
-        n = batch * rec_rr
-        if zc.shape[0] != n:
-            raise ValueError("z must have batch*rec_rr rows")
-        delta = None if huber_delta is None else check_huber_delta(huber_delta)
-        with torch.cuda.device(self.device):
-            g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
-            loss = torch.empty(n, dtype=torch.float32, device=self.device)
-            grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, m=m, nnz=nnz if csr else -1)
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            if delta is not None and csr:
-                _check(self.lib, self.lib.dgan_loss_grad_measured_csr_huber(self._handle, delta, _ptr(rp), _ptr(ci), _ptr(val),
-                                                                            m, nnz, _ptr(y), batch, rec_rr, _ptr(zc), _ptr(g),
-                                                                            _ptr(loss), _ptr(grad), ws, need,
-                                                                            ctypes.c_void_p(stream)),
-                       "dgan_loss_grad_measured_csr_huber")
-            elif delta is not None:
-                _check(self.lib, self.lib.dgan_loss_grad_measured_huber(self._handle, delta, _ptr(a), m, _ptr(y), batch, rec_rr,
-                                                                        _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
-                                                                        ctypes.c_void_p(stream)),
-                       "dgan_loss_grad_measured_huber")
-            elif csr:
-                _check(self.lib, self.lib.dgan_loss_grad_measured_csr(self._handle, _ptr(rp), _ptr(ci), _ptr(val), m, nnz,
-                                                                      _ptr(y), batch, rec_rr, _ptr(zc), _ptr(g), _ptr(loss),
-                                                                      _ptr(grad), ws, need, ctypes.c_void_p(stream)),
-                       "dgan_loss_grad_measured_csr")
-            else:
-                _check(self.lib, self.lib.dgan_loss_grad_measured(self._handle, _ptr(a), m, _ptr(y), batch, rec_rr,
-                                                                  _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
-                                                                  ctypes.c_void_p(stream)), "dgan_loss_grad_measured")
-        return g, loss, grad
+            return self._loss_grad("csr", (_ptr(rp), _ptr(ci), _ptr(val), m, nnz, _ptr(y)), batch, z, rec_rr, huber_delta,
+                                   m=m, nnz=nnz)
+        y, a, batch, m = self._measured(measurements, operator)
+        return self._loss_grad("dense", (_ptr(a), m, _ptr(y)), batch, z, rec_rr, huber_delta, m=m)
 
-    def _loss_grad_measured_conv(self, measurements, operator, z, rec_rr, huber_delta):
-        """loss_grad_measured for a ConvOperator (dgan_loss_grad_measured_conv)."""
-        y, k, op, batch, m = self._measured_conv(measurements, operator)
+    def _loss_grad(self, kind: str, operands, batch: int, z: torch.Tensor, rec_rr: int, huber_delta, pixel_weights=None,
+                   m: int = 0, nnz: int = -1, conv: Optional[dgan_conv_op] = None):
+        """loss_grad and loss_grad_measured after their operator's checks: (G(z), per-row loss, d(sum loss)/dz) from
+        dgan_loss_grad[_weighted / _huber] for images (operands: the images; pixel_weights are checked here) or
+        dgan_loss_grad_measured[_csr / _conv][_huber] (operands as _route's)."""
         zc = _require_cuda_f32(z, "z")
         n = batch * rec_rr
         if zc.shape[0] != n:
             raise ValueError("z must have batch*rec_rr rows")
-        delta = None if huber_delta is None else ctypes.c_float(check_huber_delta(huber_delta))
+        pw = self._pixel_weights(pixel_weights, batch)
+        delta = None if huber_delta is None else check_huber_delta(huber_delta)
+        if kind == "image":
+            operands = (operands[0], _ptr(pw))
+        entry = "dgan_loss_grad" + _ENTRY_OF_KIND[kind]
+        if kind == "conv":
+            operands = (_float_ref(delta),) + operands
+        elif delta is not None:
+            entry, operands = entry + "_huber", (delta,) + operands
+        elif pw is not None:
+            entry += "_weighted"
+        elif kind == "image":
+            operands = operands[:1]                  # dgan_loss_grad takes no weights
         with torch.cuda.device(self.device):
             g = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
             loss = torch.empty(n, dtype=torch.float32, device=self.device)
             grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, conv=op)
+            ws, need = self._workspace_of(*_route(kind, m=m, nnz=nnz, conv=conv, weighted=pw is not None)[:2], batch,
+                                          rec_rr)
             stream = torch.cuda.current_stream(self.device).cuda_stream
-            _check(self.lib, self.lib.dgan_loss_grad_measured_conv(self._handle,
-                                                                   ctypes.byref(delta) if delta is not None else None,
-                                                                   ctypes.byref(op), _ptr(k), _ptr(y), batch, rec_rr,
-                                                                   _ptr(zc), _ptr(g), _ptr(loss), _ptr(grad), ws, need,
-                                                                   ctypes.c_void_p(stream)),
-                   "dgan_loss_grad_measured_conv")
+            _check(self.lib, getattr(self.lib, entry)(self._handle, *operands, batch, rec_rr, _ptr(zc), _ptr(g),
+                                                      _ptr(loss), _ptr(grad), ws, need, ctypes.c_void_p(stream)), entry)
         return g, loss, grad
 
     def sample_z0(self, n_rows: int, seed: int, z_row_offset: int = 0) -> torch.Tensor:
@@ -1062,31 +926,7 @@ class NativeGenerator:
         weighted one of reconstruct (dgan_loss_grad_weighted); with huber_delta the Huber loss of reconstruct, weighted or
         not (dgan_loss_grad_huber)."""
         x = _require_cuda_f32(images, "images")
-        zc = _require_cuda_f32(z, "z")
-        batch = x.shape[0]
-        n = batch * rec_rr
-        if zc.shape[0] != n:
-            raise ValueError("z must have batch*rec_rr rows")
-        pw = self._pixel_weights(pixel_weights, batch)
-        delta = None if huber_delta is None else check_huber_delta(huber_delta)
-        with torch.cuda.device(self.device):
-            y = torch.empty((n,) + self.image_dim, dtype=torch.float32, device=self.device)
-            loss = torch.empty(n, dtype=torch.float32, device=self.device)
-            grad = torch.empty(n, self.latent_dim, dtype=torch.float32, device=self.device)
-            ws, need = self._workspace(batch, rec_rr, weighted=pw is not None)
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            if delta is not None:
-                _check(self.lib, self.lib.dgan_loss_grad_huber(self._handle, delta, _ptr(x), _ptr(pw), batch, rec_rr, _ptr(zc),
-                                                               _ptr(y), _ptr(loss), _ptr(grad), ws, need,
-                                                               ctypes.c_void_p(stream)), "dgan_loss_grad_huber")
-            elif pw is None:
-                _check(self.lib, self.lib.dgan_loss_grad(self._handle, _ptr(x), batch, rec_rr, _ptr(zc), _ptr(y), _ptr(loss),
-                                                         _ptr(grad), ws, need, ctypes.c_void_p(stream)), "dgan_loss_grad")
-            else:
-                _check(self.lib, self.lib.dgan_loss_grad_weighted(self._handle, _ptr(x), _ptr(pw), batch, rec_rr, _ptr(zc),
-                                                                  _ptr(y), _ptr(loss), _ptr(grad), ws, need,
-                                                                  ctypes.c_void_p(stream)), "dgan_loss_grad_weighted")
-        return y, loss, grad
+        return self._loss_grad("image", (_ptr(x),), x.shape[0], z, rec_rr, huber_delta, pixel_weights)
 
     def vjp(self, z: torch.Tensor, dy: torch.Tensor, want_y: bool = False):
         """Vector-Jacobian product of the generator at z: dz = (dG/dz)^T dy for a cotangent dy shaped like G(z)

@@ -536,23 +536,35 @@ static void carve_csr(const dgan_ctx* c, Workspace* w, int nnz_, char* b, size_t
   w->csr_valid = (int*)carve_take(b, off, layout, "csr_valid", "i32", {1});
 }
 
+// What a projection's workspace holds beyond the generator's buffers, and how it is split into stages (carve,
+// plan_workspace).  weighted: the image loss's per-pixel weights.  m > 0: a measured loss for m measurements; nnz >= 0 a
+// CSR operator with nnz non-zeros, conv (not NULL, nnz -1) a convolution, neither a dense operator.  adam: Adam's second
+// moment.  sdev: the sparse deviations.  n_points > 0: a pruned projection with the prune points sched, one region per
+// stage; 0: unpruned, one workspace.
+struct WsShape {
+  bool weighted = false;
+  int m = 0, nnz = -1;
+  const ConvGeom* conv = nullptr;
+  bool adam = false, sdev = false;
+  const dgan_prune_point* sched = nullptr;
+  int n_points = 0;
+};
+
 // The workspace's buffers, in carve() order: layout (not NULL) receives one line per buffer (carve_take) for
-// dgan_debug_workspace_layout.  weighted: the workspace of the weighted entries, the same buffers at the same offsets and
-// the weights "xw" after all of them.  m > 0: the workspace of the measured entries for m measurements, the same buffers
-// at the same offsets and the measured ones after all of them.
-// csr_nnz >= 0 (with m > 0): the workspace of the CSR-measured entries for nnz non-zeros, the measured buffers without
-// am / amt and the CSR ones after all of them.  conv (not NULL, with m > 0 and csr_nnz -1): the workspace of the
-// convolution-measured entries, the measured buffers without am / amt and the staged kernels "ck" after all of them.  prune_maps: one region of a pruned workspace (carve_pruned), the maps
-// "orig", "src" and "sel" after all the other buffers.  op (not NULL, with m > 0): a region of a pruned measured
-// workspace, whose operator - am / amt or the CSR buffers - and ym live in the operator block op (carve_operator): only
-// the row-sized measured buffers are carved, the others are op's.  adam: the workspace of the Adam entries, the same
-// buffers at the same offsets and the second moment "s" after all of them.  sdev: the workspace of the sparse-deviation
-// entries, the same buffers at the same offsets and then - for the image loss (m = 0), which runs the measured loop as
-// the identity operator - "dym", "mloss_part" and "mscale" as a measured workspace for m = H*W*C carves them, then "nu"
-// and "u" [n_pad][H*W*C].
-static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout = nullptr, bool weighted = false,
-                       int m = 0, int csr_nnz = -1, bool prune_maps = false, const Workspace* op = nullptr,
-                       bool adam = false, const ConvGeom* conv = nullptr, bool sdev = false) {
+// dgan_debug_workspace_layout.  sh.weighted: the workspace of the weighted entries, the same buffers at the same offsets
+// and the weights "xw" after all of them.  sh.m > 0: the workspace of the measured entries for m measurements, the same
+// buffers at the same offsets and the measured ones after all of them.  sh.nnz >= 0: the CSR-measured workspace, the
+// measured buffers without am / amt and the CSR ones after all of them.  sh.conv: the convolution-measured workspace, the
+// measured buffers without am / amt and the staged kernels "ck" after all of them.  sh.n_points > 0: one region of a
+// pruned workspace (plan_workspace), the maps "orig", "src" and "sel" after all the other buffers.  op (not NULL, with
+// m > 0): a region of a pruned measured workspace, whose operator - am / amt, the CSR buffers or ck - and ym live in the
+// operator block op (carve_operator): only the row-sized measured buffers are carved, the others are op's.  sh.adam: the
+// workspace of the Adam entries, the same buffers at the same offsets and the second moment "s" after all of them.
+// sh.sdev: the workspace of the sparse-deviation entries, the same buffers at the same offsets and then - for the image
+// loss (m = 0), which runs the measured loop as the identity operator - "dym", "mloss_part" and "mscale" as a measured
+// workspace for m = H*W*C carves them, then "nu" and "u" [n_pad][H*W*C].
+static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* layout, const WsShape& sh,
+                       const Workspace* op = nullptr) {
   Workspace w;
   w.n_rows = n_rows;
   w.n_pad = (int)align_up((size_t)std::max(n_rows, 1), c->desc.precision == DGAN_PREC_FP16 ? 2 * kRowTile : kRowTile);
@@ -614,13 +626,13 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
   if (tc) w.loss_part = (float*)take("loss_part", "f32", {(size_t)w.n_loss_parts, np});
   else w.loss_part = (float*)take("loss_part", "f32", {np, (size_t)w.n_loss_parts});
   w.loss = (float*)take("loss", "f32", {np});
-  if (weighted) w.xw = (float*)take("xw", "f32", {np, hwc});   // batch <= n_pad
-  if (m > 0) {
-    w.m = m;
-    w.m_ld = measured_ld(m);
+  if (sh.weighted) w.xw = (float*)take("xw", "f32", {np, hwc});   // batch <= n_pad
+  if (sh.m > 0) {
+    w.m = sh.m;
+    w.m_ld = measured_ld(sh.m);
     const size_t mld = (size_t)w.m_ld;
-    w.csr = csr_nnz >= 0;
-    w.conv = conv != nullptr;
+    w.csr = sh.nnz >= 0;
+    w.conv = sh.conv != nullptr;
     if (!w.csr && !w.conv && op == nullptr) {
       w.am = (float*)take("am", "f32", {mld, hwc});
       w.amt = (float*)take("amt", "f32", {hwc, mld});
@@ -638,19 +650,19 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
       w.csr_bad = op->csr_bad; w.csr_valid = op->csr_valid;
       w.cg = op->cg; w.ck = op->ck;
     } else if (w.csr) {
-      carve_csr(c, &w, csr_nnz, b, &off, layout);
+      carve_csr(c, &w, sh.nnz, b, &off, layout);
     } else if (w.conv) {
-      w.cg = *conv;
-      w.ck = (float*)take("ck", "f32", {np, (size_t)conv->kh * conv->kw});      // batch <= n_pad
+      w.cg = *sh.conv;
+      w.ck = (float*)take("ck", "f32", {np, (size_t)sh.conv->kh * sh.conv->kw});      // batch <= n_pad
     }
   }
-  if (prune_maps) {
+  if (sh.n_points > 0) {
     w.orig = (int*)take("orig", "i32", {np});
     w.src = (int*)take("src", "i32", {np});
     w.sel = (int*)take("sel", "i32", {np});     // batch <= n_pad
   }
-  if (adam) w.s = (float*)take("s", "f32", {np, latent});
-  if (sdev && m == 0) {
+  if (sh.adam) w.s = (float*)take("s", "f32", {np, latent});
+  if (sh.sdev && sh.m == 0) {
     w.ident = true;
     w.m = c->hwc;
     w.m_ld = measured_ld(c->hwc);
@@ -658,7 +670,7 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
     w.mloss_part = (float*)take("mloss_part", "f32", {(size_t)w.m_ld / kMeasTileN, np});
     w.mscale = (float*)take("mscale", "f32", {np});
   }
-  if (sdev) {
+  if (sh.sdev) {
     w.nu = (float*)take("nu", "f32", {np, hwc});
     w.u = (float*)take("u", "f32", {np, hwc});
   }
@@ -667,10 +679,9 @@ static Workspace carve(const dgan_ctx* c, int n_rows, void* base, std::string* l
 }
 
 // The operator block of a pruned measured workspace, shared by all its regions: the staged operator - "am" / "amt" as in
-// carve, or (csr_nnz >= 0) carve's CSR buffers, or (conv not NULL) the kernels "ck" [batch][kh][kw] - then the
-// measurements "ym" [batch][m_ld].  Only the operator's buffers, m, m_ld, csr, nnz, conv and cg are set.
-static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz, void* base, std::string* layout,
-                                const ConvGeom* conv = nullptr) {
+// carve, or (sh.nnz >= 0) carve's CSR buffers, or (sh.conv) the kernels "ck" [batch][kh][kw] - then the measurements
+// "ym" [batch][m_ld].  Only the operator's buffers, m, m_ld, csr, nnz, conv and cg are set.
+static Workspace carve_operator(const dgan_ctx* c, int batch, const WsShape& sh, void* base, std::string* layout) {
   Workspace w;
   size_t off = 0;
   char* b = (char*)base;
@@ -678,16 +689,16 @@ static Workspace carve_operator(const dgan_ctx* c, int batch, int m, int csr_nnz
     return carve_take(b, &off, layout, name, type, dims);
   };
   const size_t hwc = (size_t)c->hwc;
-  w.m = m;
-  w.m_ld = measured_ld(m);
+  w.m = sh.m;
+  w.m_ld = measured_ld(sh.m);
   const size_t mld = (size_t)w.m_ld;
-  w.csr = csr_nnz >= 0;
-  w.conv = conv != nullptr;
+  w.csr = sh.nnz >= 0;
+  w.conv = sh.conv != nullptr;
   if (w.csr) {
-    carve_csr(c, &w, csr_nnz, b, &off, layout);
+    carve_csr(c, &w, sh.nnz, b, &off, layout);
   } else if (w.conv) {
-    w.cg = *conv;
-    w.ck = (float*)take("ck", "f32", {(size_t)batch, (size_t)conv->kh * conv->kw});
+    w.cg = *sh.conv;
+    w.ck = (float*)take("ck", "f32", {(size_t)batch, (size_t)sh.conv->kh * sh.conv->kw});
   } else {
     w.am = (float*)take("am", "f32", {mld, hwc});
     w.amt = (float*)take("amt", "f32", {hwc, mld});
@@ -1376,30 +1387,81 @@ static int plan_pass(dgan_ctx* c, int n_rows, TcPass pass) {
   return 0;
 }
 
-// Check the caller's workspace and carve it for n_rows latent rows; on the fp16 path also plan for them and encode the
-// workspace's tensor maps.  weighted: the workspace of a weighted entry (carve), with the weighted last-layer forward
-// planned and mapped too.  m > 0: the workspace of a measured entry for m measurements (conv: a convolution operator).
-// sdev: a sparse-deviation workspace (carve), whose weighted image loss runs in the measured loop, not the weighted pass.
-static int check_ws(dgan_ctx* c, int n_rows, void* ws, size_t ws_bytes, Workspace* out, bool weighted = false, int m = 0,
-                    int csr_nnz = -1, bool adam = false, const ConvGeom* conv = nullptr, bool sdev = false) {
+// A projection's workspace for batch images of rec_rr restarts, at base (NULL: sizes only): every stage's row count
+// planned (with the weighted last-layer forward when the image loss is weighted without sparse deviations, which run it
+// in the measured loop), then carved.  Unpruned (sh.n_points 0): one carve of batch * rec_rr rows, the operator of a
+// measured loss inside it.  Pruned: a measured loss's operator block first (carve_operator; layout: a line
+// "operator 0 batch", then its lines), staged once for every stage, then region k for batch * keep_k rows (region 0:
+// batch * rec_rr), each a carve with the prune maps and the operator block's pointers, one after the other (every carve
+// is a multiple of 1024 bytes); layout: per region a line "region k byte_offset n_rows", then carve's lines with offsets
+// relative to the region.  The schedule has passed check_schedule.  *bytes: the total; regs (not NULL): the carves.
+// 0, or the planner's error code.
+static int plan_workspace(dgan_ctx* c, int batch, int rec_rr, const WsShape& sh, void* base, std::string* layout,
+                          std::vector<Workspace>* regs, size_t* bytes) {
+  auto stage_rows = [&](int k) { return batch * (k == 0 ? rec_rr : sh.sched[k - 1].keep); };
+  int rc;
+  for (int k = 0; k <= sh.n_points; ++k) {
+    if ((rc = plan_all(c, stage_rows(k)))) return rc;
+    if (sh.weighted && !sh.sdev && (rc = plan_pass(c, stage_rows(k), TC_PASS_WEIGHTED))) return rc;
+  }
+  size_t off = 0;
+  Workspace op;
+  const bool op_block = sh.n_points > 0 && sh.m > 0;
+  if (op_block) {
+    if (layout != nullptr) *layout += "operator 0 " + std::to_string(batch) + "\n";
+    op = carve_operator(c, batch, sh, base, layout);
+    off = op.bytes;
+  }
+  for (int k = 0; k <= sh.n_points; ++k) {
+    if (layout != nullptr && sh.n_points > 0)
+      *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(stage_rows(k)) + "\n";
+    Workspace w = carve(c, stage_rows(k), base ? (void*)((char*)base + off) : nullptr, layout, sh, op_block ? &op : nullptr);
+    off += w.bytes;
+    if (regs != nullptr) regs->push_back(std::move(w));
+  }
+  *bytes = off;
+  return 0;
+}
+
+// The sizer that returns a projection's workspace bytes, as the "workspace too small" message names it (none for
+// dgan_workspace_bytes)
+static std::string sizer_name(const WsShape& sh) {
+  const bool measured = sh.m > 0;
+  if (sh.sdev) return measured ? "dgan_workspace_bytes_measured_sparse_dev" : "dgan_workspace_bytes_sparse_dev";
+  if (sh.conv != nullptr) return "dgan_workspace_bytes_measured_conv";
+  if (sh.adam) return measured ? "dgan_workspace_bytes_measured_adam" : "dgan_workspace_bytes_adam";
+  if (sh.n_points > 0) return measured ? "dgan_workspace_bytes_measured_pruned" : "dgan_workspace_bytes_pruned";
+  if (sh.weighted) return "dgan_workspace_bytes_weighted";
+  if (sh.nnz >= 0) return "dgan_workspace_bytes_measured_csr";
+  return measured ? "dgan_workspace_bytes_measured" : "";
+}
+
+// Check the caller's workspace and plan and carve it (plan_workspace) into *regs, one per stage; on the fp16 path also
+// encode each region's tensor maps, and those of the weighted last-layer forward when it was planned.
+static int check_ws(dgan_ctx* c, int batch, int rec_rr, const WsShape& sh, void* ws, size_t ws_bytes,
+                    std::vector<Workspace>* regs) {
   if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
   if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
   int rc;
-  const bool wpass = weighted && !sdev;
-  if ((rc = plan_all(c, n_rows))) return rc;
-  if (wpass && (rc = plan_pass(c, n_rows, TC_PASS_WEIGHTED))) return rc;
-  *out = carve(c, n_rows, ws, nullptr, weighted, m, csr_nnz, false, nullptr, adam, conv, sdev);
-  if (out->bytes > ws_bytes) {
-    set_error("workspace too small: need " + std::to_string(out->bytes) + " bytes, got " + std::to_string(ws_bytes) +
-              (sdev ? (m > 0 ? " (dgan_workspace_bytes_measured_sparse_dev)" : " (dgan_workspace_bytes_sparse_dev)")
-               : conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
-               : adam ? (m > 0 ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
-               : weighted ? " (dgan_workspace_bytes_weighted)" : csr_nnz >= 0 ? " (dgan_workspace_bytes_measured_csr)"
-               : m > 0 ? " (dgan_workspace_bytes_measured)" : ""));
+  size_t need = 0;
+  if ((rc = plan_workspace(c, batch, rec_rr, sh, ws, nullptr, regs, &need))) return rc;
+  if (need > ws_bytes) {
+    const std::string sizer = sizer_name(sh);
+    set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
+              (sizer.empty() ? "" : " (" + sizer + ")"));
     return DGAN_ERR_WORKSPACE;
   }
-  if ((rc = build_maps(c, *out))) return rc;
-  return wpass ? build_maps(c, *out, TC_PASS_WEIGHTED) : 0;
+  for (Workspace& w : *regs) {
+    if ((rc = build_maps(c, w))) return rc;
+    if (sh.weighted && !sh.sdev && (rc = build_maps(c, w, TC_PASS_WEIGHTED))) return rc;
+  }
+  return 0;
+}
+
+// The bytes of a projection's workspace (plan_workspace), or 0 when planning fails
+static size_t workspace_bytes(dgan_ctx* c, int batch, int rec_rr, const WsShape& sh) {
+  size_t bytes = 0;
+  return plan_workspace(c, batch, rec_rr, sh, nullptr, nullptr, nullptr, &bytes) ? 0 : bytes;
 }
 
 // The weight tensors in creation order (include/defensegan_b200.h, dgan_num_weights) as 3-D arrays: the caller's shape
@@ -1659,20 +1721,21 @@ int dgan_destroy(dgan_handle h) {
 
 size_t dgan_workspace_bytes(dgan_handle h, int batch, int rec_rr) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
-  if (plan_all(h, batch * rec_rr) != 0) return 0;
-  return carve(h, batch * rec_rr, nullptr).bytes;
+  return workspace_bytes(h, batch, rec_rr, WsShape());
 }
 
 size_t dgan_workspace_bytes_weighted(dgan_handle h, int batch, int rec_rr) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
-  if (plan_all(h, batch * rec_rr) != 0 || plan_pass(h, batch * rec_rr, TC_PASS_WEIGHTED) != 0) return 0;
-  return carve(h, batch * rec_rr, nullptr, nullptr, true).bytes;
+  WsShape sh;
+  sh.weighted = true;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 size_t dgan_workspace_bytes_measured(dgan_handle h, int batch, int rec_rr, int m) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0 || m <= 0 || m > h->hwc) return 0;
-  if (plan_all(h, batch * rec_rr) != 0) return 0;
-  return carve(h, batch * rec_rr, nullptr, nullptr, false, m).bytes;
+  WsShape sh;
+  sh.m = m;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 // nnz within 0 .. m * H*W*C (the non-zeros an m-row operator can hold)
@@ -1680,8 +1743,10 @@ static bool csr_nnz_ok(dgan_handle h, int m, int nnz) { return nnz >= 0 && (int6
 
 size_t dgan_workspace_bytes_measured_csr(dgan_handle h, int batch, int rec_rr, int m, int nnz) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0 || m <= 0 || m > h->hwc || !csr_nnz_ok(h, m, nnz)) return 0;
-  if (plan_all(h, batch * rec_rr) != 0) return 0;
-  return carve(h, batch * rec_rr, nullptr, nullptr, false, m, nnz).bytes;
+  WsShape sh;
+  sh.m = m;
+  sh.nnz = nnz;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int64_t dgan_last_launch_count(dgan_handle h) { return h ? h->last_launches : 0; }
@@ -1691,9 +1756,10 @@ int64_t dgan_macs_per_row(dgan_handle h) { return h ? h->macs_per_row : 0; }
 int dgan_forward(dgan_handle h, const float* z_dev, int n_rows, float* y_dev, void* ws, size_t ws_bytes, void* stream) {
   if (h == nullptr || z_dev == nullptr || y_dev == nullptr || n_rows <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
-  Workspace w;
+  std::vector<Workspace> regs;
   int rc;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  if ((rc = check_ws(h, n_rows, 1, WsShape(), ws, ws_bytes, &regs))) return rc;
+  const Workspace& w = regs[0];
   if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
   if ((rc = run_forward(h, w, nullptr, 1, 1, false, s))) return rc;
   DGAN_CUDA_CHECK(cudaMemcpyAsync(y_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
@@ -1708,21 +1774,23 @@ struct MeasuredArgs {
   const ConvGeom* conv = nullptr; const float* k = nullptr;
 };
 
-// m within 1 .. H*W*C and the operator and measurements given; 0, or DGAN_ERR_INVALID_ARG naming the bad argument
-static int check_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev) {
+// m within 1 .. H*W*C and the operator and measurements given; 0 (*meas filled in), or DGAN_ERR_INVALID_ARG naming the
+// bad argument
+static int check_measured(dgan_handle h, const float* a_dev, int m, const float* y_dev, MeasuredArgs* meas) {
   if (m <= 0 || m > h->hwc) {
     set_error("m = " + std::to_string(m) + " is out of range: 1 <= m <= H*W*C = " + std::to_string(h->hwc));
     return DGAN_ERR_INVALID_ARG;
   }
   if (a_dev == nullptr) { set_error("NULL operator a_dev"); return DGAN_ERR_INVALID_ARG; }
   if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
+  meas->a = a_dev; meas->y = y_dev; meas->m = m;
   return 0;
 }
 
 // The same for a CSR operator: nnz within 0 .. m * H*W*C, row_ptr given, col_idx and val given unless nnz == 0.  The
 // contents are validated on the device while they are staged (stage_measured_csr).
 static int check_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m,
-                              int nnz, const float* y_dev) {
+                              int nnz, const float* y_dev, MeasuredArgs* meas) {
   if (m <= 0 || m > h->hwc) {
     set_error("m = " + std::to_string(m) + " is out of range: 1 <= m <= H*W*C = " + std::to_string(h->hwc));
     return DGAN_ERR_INVALID_ARG;
@@ -1734,6 +1802,7 @@ static int check_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32
   if (row_ptr == nullptr) { set_error("NULL row_ptr"); return DGAN_ERR_INVALID_ARG; }
   if (nnz > 0 && (col_idx == nullptr || val == nullptr)) { set_error("NULL col_idx or val with nnz > 0"); return DGAN_ERR_INVALID_ARG; }
   if (y_dev == nullptr) { set_error("NULL measurements y_dev"); return DGAN_ERR_INVALID_ARG; }
+  meas->y = y_dev; meas->m = m; meas->rp = row_ptr; meas->ci = col_idx; meas->val = val; meas->nnz = nnz;
   return 0;
 }
 
@@ -1813,6 +1882,33 @@ static int sdev_term(dgan_ctx* c, const Workspace& w, cudaStream_t s) {
   return 0;
 }
 
+// One projection's options, filled in by its entry after that entry's own argument checks.  The loss: the images x, with
+// the per-pixel weights w (NULL: unweighted), or a measured loss (meas.m > 0, x and w NULL).  adam NULL: the momentum
+// update; huber NULL: the squared error; z_prior NULL: no latent prior; sdev.on: sparse deviations.  pruned: the prune
+// points sched (check_schedule); not pruned: one stage of rec_iters iterations.
+struct Projection {
+  const float* x = nullptr;
+  const float* w = nullptr;
+  MeasuredArgs meas;
+  const dgan_adam_params* adam = nullptr;
+  const float* huber = nullptr;
+  const float* z_prior = nullptr;
+  SdevArgs sdev;
+  bool pruned = false;
+  const dgan_prune_point* sched = nullptr;
+  int n_points = 0;
+
+  WsShape shape() const {
+    WsShape sh;
+    sh.weighted = w != nullptr;
+    sh.m = meas.m; sh.nnz = meas.nnz; sh.conv = meas.conv;
+    sh.adam = adam != nullptr;
+    sh.sdev = sdev.on;
+    if (pruned) { sh.sched = sched; sh.n_points = n_points; }
+    return sh;
+  }
+};
+
 // dgan_loss_grad (w_dev NULL) and dgan_loss_grad_weighted: the weighted forward reads the caller's weights in place.
 // huber (not NULL): dgan_loss_grad_huber, the Huber loss at *huber.
 static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev, int batch, int rec_rr, const float* z_dev,
@@ -1821,9 +1917,12 @@ static int loss_grad_impl(dgan_handle h, const float* x_dev, const float* w_dev,
   if (h == nullptr || x_dev == nullptr || z_dev == nullptr || batch <= 0 || rec_rr <= 0) { set_error("invalid argument"); return DGAN_ERR_INVALID_ARG; }
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
-  Workspace w;
+  WsShape sh;
+  sh.weighted = w_dev != nullptr;
+  std::vector<Workspace> regs;
   int rc;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, w_dev != nullptr))) return rc;
+  if ((rc = check_ws(h, batch, rec_rr, sh, ws, ws_bytes, &regs))) return rc;
+  Workspace& w = regs[0];
   if ((rc = check_huber(huber))) return rc;
   if (huber != nullptr) w.huber = *huber;
   if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
@@ -1854,20 +1953,20 @@ int dgan_loss_grad_weighted(dgan_handle h, const float* x_dev, const float* w_de
   return loss_grad_impl(h, x_dev, w_dev, batch, rec_rr, z_dev, y_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
-// dgan_loss_grad_measured and dgan_loss_grad_measured_csr, after their operator checks; huber (not NULL): their Huber
-// entries, the Huber loss at *huber
-static int loss_grad_measured_impl(dgan_handle h, const MeasuredArgs& meas, int batch, int rec_rr, const float* z_dev,
-                                   float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream,
-                                   const float* huber = nullptr) {
+// The measured loss_grad entries after their operator checks (p.meas); p.huber (not NULL): their Huber entries, the
+// Huber loss at *p.huber
+static int loss_grad_measured_impl(dgan_handle h, const Projection& p, int batch, int rec_rr, const float* z_dev,
+                                   float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   int rc;
   cudaStream_t s = (cudaStream_t)stream;
   const int n_rows = batch * rec_rr;
-  Workspace w;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w, false, meas.m, meas.nnz, false, meas.conv))) return rc;
-  if ((rc = check_huber(huber))) return rc;
-  if (huber != nullptr) w.huber = *huber;
+  std::vector<Workspace> regs;
+  if ((rc = check_ws(h, batch, rec_rr, p.shape(), ws, ws_bytes, &regs))) return rc;
+  Workspace& w = regs[0];
+  if ((rc = check_huber(p.huber))) return rc;
+  if (p.huber != nullptr) w.huber = *p.huber;
   h->n_rows_cur = n_rows;
-  if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_meas(h, w, meas, batch, s))) return rc;
+  if ((rc = run_init_z(h, w, z_dev, 0, s)) || (rc = stage_meas(h, w, p.meas, batch, s))) return rc;
   if ((rc = run_forward(h, w, nullptr, 1, 1, true, s)) || (rc = launch_measure(h, w, rec_rr, s))) return rc;
   if ((rc = measured_backward(h, w, rec_rr, s)) || (rc = measured_loss_finish(h, w, s))) return rc;
   if (g_dev) DGAN_CUDA_CHECK(cudaMemcpyAsync(g_dev, w.y, (size_t)n_rows * h->hwc * 4, cudaMemcpyDeviceToDevice, s));
@@ -1893,20 +1992,18 @@ int dgan_loss_grad_measured(dgan_handle h, const float* a_dev, int m, const floa
                             const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes,
                             void* stream) {
   if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
+  Projection p;
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return loss_grad_measured_impl(h, p, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 int dgan_loss_grad_measured_csr(dgan_handle h, const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m,
                                 int nnz, const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
                                 float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
+  Projection p;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return loss_grad_measured_impl(h, p, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev, float* y_dev, float* dz_dev, void* ws,
@@ -1916,9 +2013,10 @@ int dgan_vjp(dgan_handle h, const float* z_dev, int n_rows, const float* dy_dev,
     return DGAN_ERR_INVALID_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
-  Workspace w;
+  std::vector<Workspace> regs;
   int rc;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  if ((rc = check_ws(h, n_rows, 1, WsShape(), ws, ws_bytes, &regs))) return rc;
+  Workspace& w = regs[0];
   h->n_rows_cur = n_rows;     // the FLOPs dgan_profile_read reports refer to this call
   // the forward of dgan_forward, keeping the ReLU masks; the cotangent replaces the loss's (y - x) in the last layer
   if ((rc = run_init_z(h, w, z_dev, 0, s))) return rc;
@@ -1941,9 +2039,10 @@ int dgan_jvp(dgan_handle h, const float* z_dev, int n_rows, const float* t_dev, 
     return DGAN_ERR_INVALID_ARG;
   }
   cudaStream_t s = (cudaStream_t)stream;
-  Workspace w;
+  std::vector<Workspace> regs;
   int rc;
-  if ((rc = check_ws(h, n_rows, ws, ws_bytes, &w))) return rc;
+  if ((rc = check_ws(h, n_rows, 1, WsShape(), ws, ws_bytes, &regs))) return rc;
+  Workspace& w = regs[0];
   if ((rc = plan_pass(h, n_rows, TC_PASS_TANGENT)) || (rc = build_maps(h, w, TC_PASS_TANGENT))) return rc;
   h->n_rows_cur = n_rows;
   const FinalLayer& f = h->fin;
@@ -2156,81 +2255,6 @@ static int check_adam(const dgan_adam_params* a) {
   return DGAN_ERR_INVALID_ARG;
 }
 
-// dgan_reconstruct (w_dev NULL), dgan_reconstruct_weighted and dgan_reconstruct_measured (meas.m > 0, x_dev NULL): the
-// weights, or the operator and measurements, are copied into the workspace next to the images, so the captured loop reads
-// the workspace only.  adam (not NULL, checked by the caller): the Adam entries, on an Adam workspace (carve).  huber
-// (not NULL): the Huber entries, the Huber loss at *huber on the counterpart's workspace.  z_prior (not NULL): the prior
-// entries, J = D + *z_prior ||z||^2 on the counterpart's workspace.  sdev.on: the sparse-deviation entries on a
-// sparse-deviation workspace (carve), every loss on the measured loop (the image loss as the identity operator) and
-// J + l1 ||nu||_1 the returned loss and the arg-min.
-static int reconstruct_impl(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
-                            const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
-                            void* stream, MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                            const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
-  const bool measured = meas.m > 0;
-  if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
-  // hyper-parameters, so that a call with batch = 0 tells whether a library refuses a misaligned rec_dev, running nothing
-  if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
-  const bool weighted = w_dev != nullptr;
-  const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters;
-  const uint64_t seed = prm->seed;
-  if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
-  cudaStream_t s = (cudaStream_t)stream;
-  Workspace w;
-  int rc;
-  if ((rc = check_ws(h, batch * rec_rr, ws, ws_bytes, &w, weighted, meas.m, meas.nnz, adam != nullptr, meas.conv, sdev.on)))
-    return rc;
-  float eta = 0.f, tau = 0.f;
-  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior)) ||
-      (rc = check_sparse_dev(sdev, measured ? meas.m : h->hwc, &eta, &tau)))
-    return rc;
-  if (huber != nullptr) w.huber = *huber;
-  set_prior(&w, nullptr, z_prior);
-  set_sdev(&w, nullptr, sdev, eta, tau);
-  const int64_t launches0 = h->launches;
-  int64_t enqueues = 0;
-  h->n_rows_cur = batch * rec_rr;
-  if ((rc = run_init_z(h, w, z0_dev, seed, s, (size_t)prm->z_row_offset))) return rc;
-  if (measured) {
-    if ((rc = stage_meas(h, w, meas, batch, s))) return rc;
-    enqueues += h->launches - launches0;
-  } else {
-    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    enqueues += (h->launches - launches0) + 1;
-  }
-  if (weighted) {
-    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    enqueues += 1;
-  }
-  // The L-step loop (a function of the workspace and the hyper-parameters only)
-  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
-                          prm->momentum, {}, nullptr, 0};
-  set_optimizer_key(&key, adam);
-  key.huber = w.huber;
-  set_conv_key(&key, meas.conv);
-  set_prior(nullptr, &key, z_prior);
-  set_sdev(nullptr, &key, sdev, eta, tau);
-  auto enqueue_loop = [&](cudaStream_t ls) -> int {
-    return enqueue_steps(h, w, *prm, rec_rr, 0, rec_iters, measured || sdev.on, ls, false, adam);
-  };
-  if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
-  {
-    const int64_t l0 = h->launches;
-    if ((rc = w.m > 0 ? measured_loss_finish(h, w, s) : image_loss_finish(h, w, s)) || (rc = sdev_term(h, w, s))) return rc;
-    select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, rec_rr, h->hwc, rec_dev, loss_dev, idx_dev);
-    DGAN_LAUNCH_CHECK(h);
-    if (sdev.dev_out != nullptr) {
-      sdev_select_kernel<<<batch, 256, 0, s>>>(w.loss, w.nu, rec_rr, h->hwc, sdev.dev_out);
-      DGAN_LAUNCH_CHECK(h);
-    }
-    enqueues += h->launches - l0;
-  }
-  h->last_enqueues = enqueues;
-  h->last_launches = h->launches - launches0;
-  return DGAN_OK;
-}
-
 // ---- restart pruning (dgan_reconstruct_pruned; kernels_prune.cuh) ------------------------------------------------------
 // A schedule of n_points prune points: 1 <= iter_1 < iter_2 < ... (<= L - 1 when rec_iters > 0: the sizer does not know L)
 // and rec_rr >= keep_1 >= keep_2 >= ... >= 1.  0, or DGAN_ERR_INVALID_ARG naming the bad point.
@@ -2256,99 +2280,46 @@ static int check_schedule(const dgan_prune_point* sched, int n_points, int rec_r
   return 0;
 }
 
-// The regions of a pruned workspace: region 0 for batch * rec_rr rows, region k for batch * keep_k rows, each a carve()
-// with the prune maps, one after the other (every carve is a multiple of 1024 bytes).  *bytes: the total; layout (not
-// NULL): per region a line "region k byte_offset n_rows", then carve's lines with offsets relative to the region.
-// m > 0: a pruned measured workspace (csr_nnz >= 0: CSR; conv not NULL: convolution): first the operator block (carve_operator; layout: a line
-// "operator 0 batch", then its lines), staged once for every stage, then the regions, each with the row-sized measured
-// buffers and the operator block's pointers.  adam: every region an Adam carve (its second moment "s" last).  sdev: every
-// region a sparse-deviation carve (its deviation buffers last).
-static std::vector<Workspace> carve_pruned(const dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched,
-                                           int n_points, void* base, bool weighted, size_t* bytes,
-                                           std::string* layout = nullptr, int m = 0, int csr_nnz = -1, bool adam = false,
-                                           const ConvGeom* conv = nullptr, bool sdev = false) {
-  std::vector<Workspace> regs;
-  size_t off = 0;
-  Workspace op;
-  if (m > 0) {
-    if (layout != nullptr) *layout += "operator 0 " + std::to_string(batch) + "\n";
-    op = carve_operator(c, batch, m, csr_nnz, base, layout, conv);
-    off = op.bytes;
-  }
-  for (int k = 0; k <= n_points; ++k) {
-    const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
-    if (layout != nullptr) *layout += "region " + std::to_string(k) + " " + std::to_string(off) + " " + std::to_string(rows) + "\n";
-    regs.push_back(carve(c, rows, base ? (void*)((char*)base + off) : nullptr, layout, weighted, m, csr_nnz, true,
-                         m > 0 ? &op : nullptr, adam, conv, sdev));
-    off += regs.back().bytes;
-  }
-  *bytes = off;
-  return regs;
-}
-
-// Plan every stage's row count (and the weighted pass).
-static int plan_pruned(dgan_ctx* c, int batch, int rec_rr, const dgan_prune_point* sched, int n_points, bool weighted) {
-  int rc;
-  for (int k = 0; k <= n_points; ++k) {
-    const int rows = batch * (k == 0 ? rec_rr : sched[k - 1].keep);
-    if ((rc = plan_all(c, rows))) return rc;
-    if (weighted && (rc = plan_pass(c, rows, TC_PASS_WEIGHTED))) return rc;
-  }
-  return 0;
-}
-
-// dgan_reconstruct_pruned and, with meas.m > 0 (x_dev and w_dev NULL), dgan_reconstruct_measured[_csr]_pruned: the
-// operator and measurements are staged once into the operator block that every region shares, and every stage runs the
-// measured loop; the measured forward leaves each iteration's loss parts in mloss_part, so a prune point sums them as
-// the plain loop's do loss_part.  adam (not NULL, checked by the caller): the Adam entries; a prune point gathers the
-// survivors' second moment with their z, m and z_h.  huber (not NULL): the Huber entries, every stage and the ranking on
-// the Huber loss at *huber.  z_prior (not NULL): the prior entries, every stage and the ranking on J = D + *z_prior ||z||^2,
-// a prune point's prior term on the z of iteration iter_k - 1 (before that iteration's update, as its D).  sdev.on: the
-// sparse-deviation entries, every region a sparse-deviation carve; a prune point ranks by J + l1 ||nu||_1 on the nu of
-// iteration iter_k - 1 and gathers the survivors' nu and dy, whose update the next region's first iteration applies.
-static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
-                                   const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev,
-                                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream,
-                                   MeasuredArgs meas = MeasuredArgs(), const dgan_adam_params* adam = nullptr,
-                                   const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
-  const bool measured = meas.m > 0;
-  if (h == nullptr || prm == nullptr || (x_dev == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+// Every projection after its entry's checks.  The images and weights, or the operator and measurements, are staged into
+// the workspace, so the captured loop reads the workspace only.  The loop runs n_points + 1 stages, stage k on region k
+// of the workspace (plan_workspace): rec_rr restarts per image from z0 in the first, the survivors of prune point k in
+// the others, whose z and v (and z_h, Adam's s, and the sparse deviations' nu and dy) the prune point gathers from the
+// previous region; an unpruned projection is the one stage.  A measured loss (and every sparse-deviation loss, the image
+// loss as the identity operator) runs the measured loop, whose forward leaves each iteration's loss parts in
+// mloss_part, so a prune point sums them as the image loop's do loss_part.  p.adam: the Adam update.  p.huber: the
+// Huber loss at *p.huber.  p.z_prior: J = D + *p.z_prior ||z||^2, a prune point's prior term on the z of iteration
+// iter_k - 1 (before that iteration's update, as its D).  p.sdev.on: every loss J + l1 ||nu||_1, for the ranking and
+// the arg-min.
+static int project(dgan_handle h, const dgan_rec_params* prm, const Projection& p, const float* z0_dev, float* rec_dev,
+                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
+  const bool measured = p.meas.m > 0, weighted = p.w != nullptr;
+  if (h == nullptr || prm == nullptr || (p.x == nullptr && !measured) || rec_dev == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  // the arg-min select stores the reconstructions 16 bytes at a time (select_kernel).  Checked before the
+  // hyper-parameters, so that a call with batch = 0 tells whether a library refuses a misaligned rec_dev, running nothing
   if (((uintptr_t)rec_dev & 15) != 0) { set_error("rec_dev must be 16-byte aligned"); return DGAN_ERR_INVALID_ARG; }
-  const bool weighted = w_dev != nullptr;
   const int batch = prm->batch, rec_rr = prm->rec_rr, rec_iters = prm->rec_iters;
   if (batch <= 0 || rec_rr <= 0 || rec_iters <= 0) { set_error("batch, rec_rr and rec_iters must be positive"); return DGAN_ERR_INVALID_ARG; }
   int rc;
-  if ((rc = check_schedule(sched, n_points, rec_rr, rec_iters))) return rc;
-  if (h->desc.use_bn) {
-    set_error("restart pruning is not supported with use_bn: the batch statistics couple the rows, so dropping restarts "
-              "would change the survivors' trajectories");
-    return DGAN_ERR_UNSUPPORTED;
+  if (p.pruned) {
+    if ((rc = check_schedule(p.sched, p.n_points, rec_rr, rec_iters))) return rc;
+    if (h->desc.use_bn) {
+      set_error("restart pruning is not supported with use_bn: the batch statistics couple the rows, so dropping restarts "
+                "would change the survivors' trajectories");
+      return DGAN_ERR_UNSUPPORTED;
+    }
   }
-  if (ws == nullptr) { set_error("workspace is NULL"); return DGAN_ERR_WORKSPACE; }
-  if (((uintptr_t)ws & 1023) != 0) { set_error("workspace must be 1024-byte aligned"); return DGAN_ERR_WORKSPACE; }
-  const bool wpass = weighted && !sdev.on;      // a sparse-deviation image loss runs in the measured loop
-  if ((rc = plan_pruned(h, batch, rec_rr, sched, n_points, wpass))) return rc;
-  size_t need = 0;
-  std::vector<Workspace> regs = carve_pruned(h, batch, rec_rr, sched, n_points, ws, weighted, &need, nullptr, meas.m,
-                                             meas.nnz, adam != nullptr, meas.conv, sdev.on);
-  if (need > ws_bytes) {
-    set_error("workspace too small: need " + std::to_string(need) + " bytes, got " + std::to_string(ws_bytes) +
-              (sdev.on ? (measured ? " (dgan_workspace_bytes_measured_sparse_dev)" : " (dgan_workspace_bytes_sparse_dev)")
-               : meas.conv != nullptr ? " (dgan_workspace_bytes_measured_conv)"
-               : adam != nullptr ? (measured ? " (dgan_workspace_bytes_measured_adam)" : " (dgan_workspace_bytes_adam)")
-               : measured ? " (dgan_workspace_bytes_measured_pruned)" : " (dgan_workspace_bytes_pruned)"));
-    return DGAN_ERR_WORKSPACE;
-  }
+  const WsShape sh = p.shape();
+  const int n_points = sh.n_points;
+  std::vector<Workspace> regs;
+  if ((rc = check_ws(h, batch, rec_rr, sh, ws, ws_bytes, &regs))) return rc;
   float eta = 0.f, tau = 0.f;
-  if ((rc = check_huber(huber)) || (rc = check_z_prior(z_prior)) ||
-      (rc = check_sparse_dev(sdev, measured ? meas.m : h->hwc, &eta, &tau)))
+  if ((rc = check_huber(p.huber)) || (rc = check_z_prior(p.z_prior)) ||
+      (rc = check_sparse_dev(p.sdev, measured ? p.meas.m : h->hwc, &eta, &tau)))
     return rc;
   for (Workspace& w : regs) {
-    if ((rc = build_maps(h, w))) return rc;
-    if (wpass && (rc = build_maps(h, w, TC_PASS_WEIGHTED))) return rc;
-    if (huber != nullptr) w.huber = *huber;
-    set_prior(&w, nullptr, z_prior);
-    set_sdev(&w, nullptr, sdev, eta, tau);
+    if (p.huber != nullptr) w.huber = *p.huber;
+    set_prior(&w, nullptr, p.z_prior);
+    set_sdev(&w, nullptr, p.sdev, eta, tau);
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t launches0 = h->launches;
@@ -2362,24 +2333,25 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
     } else if ((rc = clear_start_state(h, w, s))) {
       return rc;
     }
-    if (measured) {              // the operator block, once for every region
-      if (k == 0 && (rc = stage_meas(h, w, meas, batch, s))) return rc;
+    if (measured) {              // the operator, once for every region
+      if (k == 0 && (rc = stage_meas(h, w, p.meas, batch, s))) return rc;
       enqueues += h->launches - l0;
       continue;
     }
-    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, x_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if (weighted) DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, w_dev, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    DGAN_CUDA_CHECK(cudaMemcpyAsync(w.x, p.x, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (weighted) DGAN_CUDA_CHECK(cudaMemcpyAsync(w.xw, p.w, (size_t)batch * h->hwc * sizeof(float), cudaMemcpyDeviceToDevice, s));
     enqueues += (h->launches - l0) + 1 + (weighted ? 1 : 0);
   }
-  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, meas.m, meas.nnz, prm->rec_lr,
+  // The loop (a function of the workspace and the hyper-parameters only)
+  dgan_ctx::LoopGraph key{ws, batch, rec_rr, rec_iters, prm->decay_lr, (int)weighted, p.meas.m, p.meas.nnz, prm->rec_lr,
                           prm->momentum, {}, nullptr, 0};
-  for (int k = 0; k < n_points; ++k) { key.prune.push_back(sched[k].iter); key.prune.push_back(sched[k].keep); }
-  set_optimizer_key(&key, adam);
-  key.huber = huber != nullptr ? *huber : 0.f;
-  set_conv_key(&key, meas.conv);
-  set_prior(nullptr, &key, z_prior);
-  set_sdev(nullptr, &key, sdev, eta, tau);
-  // the per-row loss of region w's last iteration, from the parts its last forward (plain) or measurement product
+  for (int k = 0; k < n_points; ++k) { key.prune.push_back(sh.sched[k].iter); key.prune.push_back(sh.sched[k].keep); }
+  set_optimizer_key(&key, p.adam);
+  key.huber = p.huber != nullptr ? *p.huber : 0.f;
+  set_conv_key(&key, p.meas.conv);
+  set_prior(nullptr, &key, p.z_prior);
+  set_sdev(nullptr, &key, p.sdev, eta, tau);
+  // the per-row loss of region w's last iteration, from the parts its last forward (image loss) or measurement product
   // (measured, and every sparse-deviation loss) left, with the deviations' term
   auto finish = [&](const Workspace& w, cudaStream_t ls) -> int {
     const int r2 = w.m > 0 ? measured_loss_finish(h, w, ls) : image_loss_finish(h, w, ls);
@@ -2392,17 +2364,17 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
     int r2;
     for (int k = 0; k <= n_points; ++k) {
       const Workspace& w = regs[(size_t)k];
-      const int per = k == 0 ? rec_rr : sched[k - 1].keep;
-      const int t0 = k == 0 ? 0 : sched[k - 1].iter, t1 = k == n_points ? rec_iters : sched[k].iter;
+      const int per = k == 0 ? rec_rr : sh.sched[k - 1].keep;
+      const int t0 = k == 0 ? 0 : sh.sched[k - 1].iter, t1 = k == n_points ? rec_iters : sh.sched[k].iter;
       h->n_rows_cur = w.n_rows;
-      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured || sdev.on, ls, k < n_points, adam))) return r2;
+      if ((r2 = enqueue_steps(h, w, *prm, per, t0, t1, measured || p.sdev.on, ls, k < n_points, p.adam))) return r2;
       if (k == n_points) break;
       const Workspace& nx = regs[(size_t)k + 1];
       if ((r2 = finish(w, ls))) return r2;
-      prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sched[k].keep, nx.src, nx.orig);
+      prune_select_kernel<<<batch, 256, 0, ls>>>(w.loss, k == 0 ? nullptr : w.orig, per, sh.sched[k].keep, nx.src, nx.orig);
       DGAN_LAUNCH_CHECK(h);
       const size_t total = (size_t)nx.n_pad * h->wd.latent;
-      if (adam != nullptr)
+      if (p.adam != nullptr)
         prune_gather_adam_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.s, w.z_h, nx.src, nx.n_rows,
                                                                                  nx.n_pad, h->wd.latent, nx.z, nx.v, nx.s,
                                                                                  nx.z_h);
@@ -2410,7 +2382,7 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
         prune_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ls>>>(w.z, w.v, w.z_h, nx.src, nx.n_rows, nx.n_pad,
                                                                             h->wd.latent, nx.z, nx.v, nx.z_h);
       DGAN_LAUNCH_CHECK(h);
-      if (sdev.on) {
+      if (p.sdev.on) {
         const size_t n4 = (size_t)nx.n_rows * h->hwc / 4;
         sdev_gather_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, ls>>>(w.nu, w.dym, nx.src, nx.n_rows, h->hwc, nx.nu,
                                                                          nx.dym);
@@ -2420,17 +2392,20 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
     return 0;
   };
   if ((rc = run_loop(h, key, enqueue_loop, s, &enqueues))) return rc;
+  // the arg-min of the last stage; a pruned call maps each image's choice among its survivors to the original restart
   const Workspace& w = regs.back();
-  const int per = sched[n_points - 1].keep;
+  const int per = n_points == 0 ? rec_rr : sh.sched[n_points - 1].keep;
   h->n_rows_cur = w.n_rows;
   const int64_t l0 = h->launches;
   if ((rc = finish(w, s))) return rc;
-  select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, w.sel);
+  select_kernel<<<batch, 256, 0, s>>>(w.loss, w.y, per, h->hwc, rec_dev, loss_dev, n_points == 0 ? idx_dev : w.sel);
   DGAN_LAUNCH_CHECK(h);
-  prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
-  DGAN_LAUNCH_CHECK(h);
-  if (sdev.dev_out != nullptr) {
-    sdev_select_kernel<<<batch, 256, 0, s>>>(w.loss, w.nu, per, h->hwc, sdev.dev_out);
+  if (n_points > 0) {
+    prune_idx_kernel<<<(batch + 255) / 256, 256, 0, s>>>(w.sel, w.orig, per, batch, idx_dev);
+    DGAN_LAUNCH_CHECK(h);
+  }
+  if (p.sdev.dev_out != nullptr) {
+    sdev_select_kernel<<<batch, 256, 0, s>>>(w.loss, w.nu, per, h->hwc, p.sdev.dev_out);
     DGAN_LAUNCH_CHECK(h);
   }
   enqueues += h->launches - l0;
@@ -2439,20 +2414,49 @@ static int reconstruct_pruned_impl(dgan_handle h, const dgan_rec_params* prm, co
   return DGAN_OK;
 }
 
+// sched NULL with n_points 0: unpruned; anything else is a schedule under the rules of dgan_reconstruct_pruned
+static bool unpruned(const dgan_prune_point* sched, int n_points) { return sched == nullptr && n_points == 0; }
+
+// A sizer's schedule: unpruned, or one check_schedule accepts on a handle without use_bn
+static bool sizer_sched_ok(dgan_handle h, int rec_rr, const dgan_prune_point* sched, int n_points) {
+  return unpruned(sched, n_points) || (!h->desc.use_bn && check_schedule(sched, n_points, rec_rr, 0) == 0);
+}
+
+// The first checks of the entries that take Adam's parameters, in their order: adam's (always for the Adam entries,
+// need_adam; otherwise when given), then the handle.
+static int check_entry(dgan_handle h, const dgan_adam_params* adam, bool need_adam = false) {
+  if (adam != nullptr || need_adam)
+    if (int rc = check_adam(adam)) return rc;
+  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  return 0;
+}
+
+// The options an entry passes on besides its loss: adam (NULL: momentum), huber (NULL: squared error), z_prior (NULL: no
+// prior) and the schedule (unpruned: sched NULL with n_points 0)
+static Projection options(const dgan_adam_params* adam, const float* huber, const float* z_prior,
+                          const dgan_prune_point* sched, int n_points) {
+  Projection p;
+  p.adam = adam; p.huber = huber; p.z_prior = z_prior;
+  p.pruned = !unpruned(sched, n_points); p.sched = sched; p.n_points = n_points;
+  return p;
+}
+
 size_t dgan_workspace_bytes_pruned(dgan_handle h, int batch, int rec_rr, const dgan_prune_point* sched, int n_points,
                                    int weighted) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0 || h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, weighted != 0) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes);
-  return bytes;
+  WsShape sh;
+  sh.weighted = weighted != 0;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int dgan_reconstruct_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                             const float* x_dev, const float* w_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                             int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                                 stream);
+  Projection p = options(nullptr, nullptr, nullptr, sched, n_points);
+  p.pruned = true;
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 // m within 1 .. H*W*C and nnz -1 (a dense operator) or within 0 .. m * H*W*C (a CSR one)
@@ -2465,135 +2469,106 @@ size_t dgan_workspace_bytes_measured_pruned(dgan_handle h, int batch, int rec_rr
   if (h == nullptr || batch <= 0 || rec_rr <= 0 || h->desc.use_bn || !measured_pruned_args_ok(h, m, nnz) ||
       check_schedule(sched, n_points, rec_rr, 0) != 0)
     return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, nnz);
-  return bytes;
+  WsShape sh;
+  sh.m = m; sh.nnz = nnz;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int dgan_reconstruct_measured_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched, int n_points,
                                      const float* a_dev, int m, const float* y_dev, const float* z0_dev, float* rec_dev,
                                      float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_pruned_impl(h, prm, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                                 ws_bytes, stream, meas);
+  if (int rc = check_entry(h, nullptr)) return rc;
+  Projection p = options(nullptr, nullptr, nullptr, sched, n_points);
+  p.pruned = true;
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr_pruned(dgan_handle h, const dgan_rec_params* prm, const dgan_prune_point* sched,
                                          int n_points, const int32_t* row_ptr, const int32_t* col_idx, const float* val,
                                          int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
                                          float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_pruned_impl(h, prm, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                                 ws_bytes, stream, meas);
+  if (int rc = check_entry(h, nullptr)) return rc;
+  Projection p = options(nullptr, nullptr, nullptr, sched, n_points);
+  p.pruned = true;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* z0_dev, float* rec_dev,
                      float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  return reconstruct_impl(h, prm, x_dev, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
+  Projection p;
+  p.x = x_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_weighted(dgan_handle h, const dgan_rec_params* prm, const float* x_dev, const float* w_dev,
                               const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                               size_t ws_bytes, void* stream) {
   if (w_dev == nullptr) { set_error("NULL weights"); return DGAN_ERR_INVALID_ARG; }
-  return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
+  Projection p;
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured(dgan_handle h, const dgan_rec_params* prm, const float* a_dev, int m, const float* y_dev,
                               const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                               size_t ws_bytes, void* stream) {
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
+  if (int rc = check_entry(h, nullptr)) return rc;
+  Projection p;
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr(dgan_handle h, const dgan_rec_params* prm, const int32_t* row_ptr, const int32_t* col_idx,
                                   const float* val, int m, int nnz, const float* y_dev, const float* z0_dev, float* rec_dev,
                                   float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_impl(h, prm, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas);
+  if (int rc = check_entry(h, nullptr)) return rc;
+  Projection p;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 // ---- Adam (kernels_adam.cuh): each entry is its momentum counterpart's code path with the Adam update -----------------
-// sched NULL with n_points 0: unpruned; anything else is a schedule under the rules of dgan_reconstruct_pruned
-static bool unpruned(const dgan_prune_point* sched, int n_points) { return sched == nullptr && n_points == 0; }
-
 size_t dgan_workspace_bytes_adam(dgan_handle h, int batch, int rec_rr, int weighted, const dgan_prune_point* sched,
                                  int n_points) {
-  if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
-  if (unpruned(sched, n_points)) {
-    if (plan_all(h, batch * rec_rr) != 0 || (weighted && plan_pass(h, batch * rec_rr, TC_PASS_WEIGHTED) != 0)) return 0;
-    return carve(h, batch * rec_rr, nullptr, nullptr, weighted != 0, 0, -1, false, nullptr, true).bytes;
-  }
-  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, weighted != 0) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, nullptr, 0, -1, true);
-  return bytes;
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || !sizer_sched_ok(h, rec_rr, sched, n_points)) return 0;
+  WsShape sh;
+  sh.weighted = weighted != 0; sh.adam = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 size_t dgan_workspace_bytes_measured_adam(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_prune_point* sched,
                                           int n_points) {
-  if (h == nullptr || batch <= 0 || rec_rr <= 0 || !measured_pruned_args_ok(h, m, nnz)) return 0;
-  if (unpruned(sched, n_points)) {
-    if (plan_all(h, batch * rec_rr) != 0) return 0;
-    return carve(h, batch * rec_rr, nullptr, nullptr, false, m, nnz, false, nullptr, true).bytes;
-  }
-  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, nnz, true);
-  return bytes;
-}
-
-// The image and measured Adam, Huber and prior entries after their own checks: unpruned through reconstruct_impl, pruned
-// through reconstruct_pruned_impl, as their momentum and squared-error counterparts (adam NULL: momentum; huber NULL:
-// squared error; z_prior NULL: no prior; sdev.on false: no sparse deviations)
-static int reconstruct_adam_impl(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
-                                 const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
-                                 const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
-                                 size_t ws_bytes, void* stream, MeasuredArgs meas = MeasuredArgs(),
-                                 const float* huber = nullptr, const float* z_prior = nullptr, SdevArgs sdev = SdevArgs()) {
-  if (unpruned(sched, n_points))
-    return reconstruct_impl(h, prm, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream, meas, adam,
-                            huber, z_prior, sdev);
-  return reconstruct_pruned_impl(h, prm, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                                 stream, meas, adam, huber, z_prior, sdev);
+  if (h == nullptr || batch <= 0 || rec_rr <= 0 || !measured_pruned_args_ok(h, m, nnz) ||
+      !sizer_sched_ok(h, rec_rr, sched, n_points))
+    return 0;
+  WsShape sh;
+  sh.m = m; sh.nnz = nnz; sh.adam = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int dgan_reconstruct_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                           const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                           const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                           void* stream) {
-  if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                               stream);
+  if (int rc = check_entry(h, adam, true)) return rc;
+  Projection p = options(adam, nullptr, nullptr, sched, n_points);
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                    const dgan_prune_point* sched, int n_points, const float* a_dev, int m, const float* y_dev,
                                    const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                    size_t ws_bytes, void* stream) {
-  if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas);
+  if (int rc = check_entry(h, adam, true)) return rc;
+  Projection p = options(adam, nullptr, nullptr, sched, n_points);
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2601,13 +2576,10 @@ int dgan_reconstruct_measured_csr_adam(dgan_handle h, const dgan_rec_params* prm
                                        const int32_t* col_idx, const float* val, int m, int nnz, const float* y_dev,
                                        const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                        size_t ws_bytes, void* stream) {
-  if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas);
+  if (int rc = check_entry(h, adam, true)) return rc;
+  Projection p = options(adam, nullptr, nullptr, sched, n_points);
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 // ---- the Huber loss: each entry is its squared-error counterpart's code path with delta -------------------------------
@@ -2616,25 +2588,20 @@ int dgan_reconstruct_huber(dgan_handle h, const dgan_rec_params* prm, const dgan
                            const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                            const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                            void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                               stream, MeasuredArgs(), &huber_delta);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, &huber_delta, nullptr, sched, n_points);
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_huber(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                     float huber_delta, const dgan_prune_point* sched, int n_points, const float* a_dev, int m,
                                     const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                                     int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, &huber_delta);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, &huber_delta, nullptr, sched, n_points);
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr_huber(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2642,14 +2609,10 @@ int dgan_reconstruct_measured_csr_huber(dgan_handle h, const dgan_rec_params* pr
                                         const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
                                         const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                                         int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, &huber_delta);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, &huber_delta, nullptr, sched, n_points);
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_loss_grad_huber(dgan_handle h, float huber_delta, const float* x_dev, const float* w_dev, int batch, int rec_rr,
@@ -2662,11 +2625,10 @@ int dgan_loss_grad_measured_huber(dgan_handle h, float huber_delta, const float*
                                   int rec_rr, const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws,
                                   size_t ws_bytes, void* stream) {
   if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
-                                 &huber_delta);
+  Projection p;
+  p.huber = &huber_delta;
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return loss_grad_measured_impl(h, p, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const int32_t* row_ptr, const int32_t* col_idx,
@@ -2674,11 +2636,10 @@ int dgan_loss_grad_measured_csr_huber(dgan_handle h, float huber_delta, const in
                                       const float* z_dev, float* g_dev, float* loss_dev, float* grad_dev, void* ws,
                                       size_t ws_bytes, void* stream) {
   if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
-                                 &huber_delta);
+  Projection p;
+  p.huber = &huber_delta;
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return loss_grad_measured_impl(h, p, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 // ---- convolution operators (kernels_measured_conv.cuh): a third operator kind through the measured drivers ----------
@@ -2722,17 +2683,13 @@ int dgan_conv_op_m(dgan_handle h, const dgan_conv_op* op) {
 size_t dgan_workspace_bytes_measured_conv(dgan_handle h, int batch, int rec_rr, const dgan_conv_op* op,
                                           const dgan_prune_point* sched, int n_points, int adam) {
   ConvGeom g;
-  if (h == nullptr || op == nullptr || batch <= 0 || rec_rr <= 0 || !conv_geom(h, op, &g)) return 0;
-  const int m = g.Ho * g.Wo * g.C;
-  if (unpruned(sched, n_points)) {
-    if (plan_all(h, batch * rec_rr) != 0) return 0;
-    return carve(h, batch * rec_rr, nullptr, nullptr, false, m, -1, false, nullptr, adam != 0, &g).bytes;
-  }
-  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, nullptr, m, -1, adam != 0, &g);
-  return bytes;
+  if (h == nullptr || op == nullptr || batch <= 0 || rec_rr <= 0 || !conv_geom(h, op, &g) ||
+      !sizer_sched_ok(h, rec_rr, sched, n_points))
+    return 0;
+  WsShape sh;
+  sh.m = g.Ho * g.Wo * g.C; sh.conv = &g; sh.adam = adam != 0;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int dgan_reconstruct_measured_conv(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2740,14 +2697,11 @@ int dgan_reconstruct_measured_conv(dgan_handle h, const dgan_rec_params* prm, co
                                    const dgan_conv_op* op, const float* k_dev, const float* y_dev, const float* z0_dev,
                                    float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                                    void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, nullptr, sched, n_points);
   ConvGeom g;
-  MeasuredArgs meas;
-  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta);
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 // ---- the latent prior: each entry is its counterpart's code path with lambda = z_prior -------------------------------
@@ -2757,25 +2711,20 @@ int dgan_reconstruct_prior(dgan_handle h, const dgan_rec_params* prm, const dgan
                            float z_prior, const dgan_prune_point* sched, int n_points, const float* x_dev, const float* w_dev,
                            const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes,
                            void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                               stream, MeasuredArgs(), huber_delta, &z_prior);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, &z_prior, sched, n_points);
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
                                     const float* huber_delta, float z_prior, const dgan_prune_point* sched, int n_points,
                                     const float* a_dev, int m, const float* y_dev, const float* z0_dev, float* rec_dev,
                                     float* loss_dev, int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, &z_prior);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, &z_prior, sched, n_points);
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2783,14 +2732,10 @@ int dgan_reconstruct_measured_csr_prior(dgan_handle h, const dgan_rec_params* pr
                                         const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
                                         const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                                         int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, &z_prior);
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, &z_prior, sched, n_points);
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_conv_prior(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2798,25 +2743,22 @@ int dgan_reconstruct_measured_conv_prior(dgan_handle h, const dgan_rec_params* p
                                          int n_points, const dgan_conv_op* op, const float* k_dev, const float* y_dev,
                                          const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                          size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, &z_prior, sched, n_points);
   ConvGeom g;
-  MeasuredArgs meas;
-  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, &z_prior);
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const dgan_conv_op* op, const float* k_dev,
                                  const float* y_dev, int batch, int rec_rr, const float* z_dev, float* g_dev,
                                  float* loss_dev, float* grad_dev, void* ws, size_t ws_bytes, void* stream) {
   if (!loss_grad_args_ok(h, z_dev, loss_dev, grad_dev, batch, rec_rr)) return DGAN_ERR_INVALID_ARG;
+  Projection p;
+  p.huber = huber_delta;
   ConvGeom g;
-  MeasuredArgs meas;
-  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
-  return loss_grad_measured_impl(h, meas, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream,
-                                 huber_delta);
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &p.meas)) return rc;
+  return loss_grad_measured_impl(h, p, batch, rec_rr, z_dev, g_dev, loss_dev, grad_dev, ws, ws_bytes, stream);
 }
 
 // ---- sparse deviations (kernels_sparse_dev.cuh): each entry is its prior entry's code path on the measured loop --------
@@ -2824,29 +2766,22 @@ int dgan_loss_grad_measured_conv(dgan_handle h, const float* huber_delta, const 
 // sched NULL with n_points 0: unpruned.  The counterpart's checks come first, then check_sparse_dev's, before anything
 // is enqueued.
 
-// The bytes of a sparse-deviation workspace (m 0: the image loss, weighted or not; m > 0: measured, nnz -1 dense or the
-// CSR non-zeros, conv not NULL a convolution), planning every stage; layout (not NULL) receives its lines.  0 when an
-// argument is out of range.
-static size_t sdev_bytes(dgan_handle h, int batch, int rec_rr, bool weighted, int m, int nnz, const ConvGeom* conv,
-                         bool adam, const dgan_prune_point* sched, int n_points, std::string* layout) {
-  if (h == nullptr || batch <= 0 || rec_rr <= 0) return 0;
-  if (m != 0 && (weighted || (conv == nullptr && !measured_pruned_args_ok(h, m, nnz)))) return 0;
-  if (unpruned(sched, n_points)) {
-    if (plan_all(h, batch * rec_rr) != 0) return 0;
-    return carve(h, batch * rec_rr, nullptr, layout, weighted, m, conv != nullptr ? -1 : nnz, false, nullptr, adam, conv,
-                 true).bytes;
-  }
-  if (h->desc.use_bn || check_schedule(sched, n_points, rec_rr, 0) != 0) return 0;
-  if (plan_pruned(h, batch, rec_rr, sched, n_points, false) != 0) return 0;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted, &bytes, layout, m, conv != nullptr ? -1 : nnz, adam,
-               conv, true);
-  return bytes;
+// The sparse-deviation sizers' and layout's screening of their arguments (m 0: the image loss, weighted or not; m > 0:
+// measured, nnz -1 dense or the CSR non-zeros, conv not NULL a convolution whose m was checked by the caller)
+static bool sdev_args_ok(dgan_handle h, int batch, int rec_rr, bool weighted, int m, int nnz, const ConvGeom* conv,
+                         const dgan_prune_point* sched, int n_points) {
+  if (h == nullptr || batch <= 0 || rec_rr <= 0) return false;
+  if (m != 0 && (weighted || (conv == nullptr && !measured_pruned_args_ok(h, m, nnz)))) return false;
+  return sizer_sched_ok(h, rec_rr, sched, n_points);
 }
 
 size_t dgan_workspace_bytes_sparse_dev(dgan_handle h, int batch, int rec_rr, int weighted, int adam,
                                        const dgan_prune_point* sched, int n_points) {
-  return sdev_bytes(h, batch, rec_rr, weighted != 0, 0, -1, nullptr, adam != 0, sched, n_points, nullptr);
+  if (!sdev_args_ok(h, batch, rec_rr, weighted != 0, 0, -1, nullptr, sched, n_points)) return 0;
+  WsShape sh;
+  sh.weighted = weighted != 0; sh.adam = adam != 0; sh.sdev = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 size_t dgan_workspace_bytes_measured_sparse_dev(dgan_handle h, int batch, int rec_rr, int m, int nnz, const dgan_conv_op* op,
@@ -2857,7 +2792,12 @@ size_t dgan_workspace_bytes_measured_sparse_dev(dgan_handle h, int batch, int re
   } else if (m <= 0) {
     return 0;
   }
-  return sdev_bytes(h, batch, rec_rr, false, m, nnz, op != nullptr ? &g : nullptr, adam != 0, sched, n_points, nullptr);
+  const ConvGeom* conv = op != nullptr ? &g : nullptr;
+  if (!sdev_args_ok(h, batch, rec_rr, false, m, nnz, conv, sched, n_points)) return 0;
+  WsShape sh;
+  sh.m = m; sh.nnz = conv != nullptr ? -1 : nnz; sh.conv = conv; sh.adam = adam != 0; sh.sdev = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return workspace_bytes(h, batch, rec_rr, sh);
 }
 
 int dgan_reconstruct_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2865,11 +2805,11 @@ int dgan_reconstruct_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const
                                 const dgan_sparse_dev* sparse_dev, float* dev_out, const float* x_dev, const float* w_dev,
                                 const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev, void* ws,
                                 size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, x_dev, w_dev, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes,
-                               stream, MeasuredArgs(), huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, z_prior, sched, n_points);
+  p.sdev = SdevArgs{true, sparse_dev, dev_out};
+  p.x = x_dev; p.w = w_dev;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2877,14 +2817,11 @@ int dgan_reconstruct_measured_sparse_dev(dgan_handle h, const dgan_rec_params* p
                                          int n_points, const dgan_sparse_dev* sparse_dev, float* dev_out, const float* a_dev,
                                          int m, const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                                          int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured(h, a_dev, m, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.a = a_dev; meas.y = y_dev; meas.m = m;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, z_prior, sched, n_points);
+  p.sdev = SdevArgs{true, sparse_dev, dev_out};
+  if (int rc = check_measured(h, a_dev, m, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_csr_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2893,14 +2830,11 @@ int dgan_reconstruct_measured_csr_sparse_dev(dgan_handle h, const dgan_rec_param
                                              const int32_t* row_ptr, const int32_t* col_idx, const float* val, int m, int nnz,
                                              const float* y_dev, const float* z0_dev, float* rec_dev, float* loss_dev,
                                              int32_t* idx_dev, void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
-  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev)) return rc;
-  MeasuredArgs meas;
-  meas.y = y_dev; meas.m = m; meas.rp = row_ptr; meas.ci = col_idx; meas.val = val; meas.nnz = nnz;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, z_prior, sched, n_points);
+  p.sdev = SdevArgs{true, sparse_dev, dev_out};
+  if (int rc = check_measured_csr(h, row_ptr, col_idx, val, m, nnz, y_dev, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_reconstruct_measured_conv_sparse_dev(dgan_handle h, const dgan_rec_params* prm, const dgan_adam_params* adam,
@@ -2909,14 +2843,12 @@ int dgan_reconstruct_measured_conv_sparse_dev(dgan_handle h, const dgan_rec_para
                                               const dgan_conv_op* op, const float* k_dev, const float* y_dev,
                                               const float* z0_dev, float* rec_dev, float* loss_dev, int32_t* idx_dev,
                                               void* ws, size_t ws_bytes, void* stream) {
-  if (adam != nullptr)
-    if (int rc = check_adam(adam)) return rc;
-  if (h == nullptr) { set_error("NULL argument"); return DGAN_ERR_INVALID_ARG; }
+  if (int rc = check_entry(h, adam)) return rc;
+  Projection p = options(adam, huber_delta, z_prior, sched, n_points);
+  p.sdev = SdevArgs{true, sparse_dev, dev_out};
   ConvGeom g;
-  MeasuredArgs meas;
-  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &meas)) return rc;
-  return reconstruct_adam_impl(h, prm, adam, sched, n_points, nullptr, nullptr, z0_dev, rec_dev, loss_dev, idx_dev, ws,
-                               ws_bytes, stream, meas, huber_delta, z_prior, SdevArgs{true, sparse_dev, dev_out});
+  if (int rc = check_measured_conv(h, op, k_dev, y_dev, &g, &p.meas)) return rc;
+  return project(h, prm, p, z0_dev, rec_dev, loss_dev, idx_dev, ws, ws_bytes, stream);
 }
 
 int dgan_profile_enable(dgan_handle h, int enable) {
@@ -3283,23 +3215,32 @@ int dgan_debug_padded_widths(const dgan_desc* d, int* out) {
 // itself - lines "n_rows N", "n_pad N", "widths latent c4 c2 c1" (padded), "g_parts N", then one line per buffer:
 // "name type byte_offset dim0 dim1 ..." (type f32, f16, u64 or u32; dims in storage order, outermost first; the mask
 // words of layer l are "mask.l" [P_out][n_pad][C_out / 64]).  Returns the length, or -1 when buf is too small.
-static int workspace_layout_impl(dgan_handle h, int n_rows, char* buf, int buf_len, bool weighted, int m = 0,
-                                 int csr_nnz = -1) {
-  if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
+// Every layout aid plans its workspace as its sizer does (plan_workspace).
+static int write_layout(dgan_handle h, int batch, int rec_rr, const WsShape& sh, char* buf, int buf_len) {
   std::string out;
-  carve(h, n_rows, nullptr, &out, weighted, m, csr_nnz);
+  size_t bytes = 0;
+  if (plan_workspace(h, batch, rec_rr, sh, nullptr, &out, nullptr, &bytes)) return -1;
   if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();
 }
 
+static bool layout_args_ok(dgan_handle h, int n_rows, char* buf, int buf_len) {
+  if (h == nullptr || n_rows <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return false; }
+  return true;
+}
+
 int dgan_debug_workspace_layout(dgan_handle h, int n_rows, char* buf, int buf_len) {
-  return workspace_layout_impl(h, n_rows, buf, buf_len, false);
+  if (!layout_args_ok(h, n_rows, buf, buf_len)) return -1;
+  return write_layout(h, n_rows, 1, WsShape(), buf, buf_len);
 }
 
 // The same for the workspace of the weighted entries (dgan_workspace_bytes_weighted): the weights are "xw" [n_pad][H*W*C].
 int dgan_debug_workspace_layout_weighted(dgan_handle h, int n_rows, char* buf, int buf_len) {
-  return workspace_layout_impl(h, n_rows, buf, buf_len, true);
+  if (!layout_args_ok(h, n_rows, buf, buf_len)) return -1;
+  WsShape sh;
+  sh.weighted = true;
+  return write_layout(h, n_rows, 1, sh, buf, buf_len);
 }
 
 // The same for the workspace of the measured entries for m measurements (dgan_workspace_bytes_measured): after the
@@ -3307,7 +3248,10 @@ int dgan_debug_workspace_layout_weighted(dgan_handle h, int n_rows, char* buf, i
 // [n_pad][H*W*C], "mloss_part" [m_ld / 64][n_pad] and "mscale" [n_pad].
 int dgan_debug_workspace_layout_measured(dgan_handle h, int n_rows, int m, char* buf, int buf_len) {
   if (h == nullptr || m <= 0 || m > h->hwc) { set_error("invalid argument"); return -1; }
-  return workspace_layout_impl(h, n_rows, buf, buf_len, false, m);
+  if (!layout_args_ok(h, n_rows, buf, buf_len)) return -1;
+  WsShape sh;
+  sh.m = m;
+  return write_layout(h, n_rows, 1, sh, buf, buf_len);
 }
 
 // The same for the workspace of the CSR-measured entries for m measurements and nnz non-zeros
@@ -3317,7 +3261,10 @@ int dgan_debug_workspace_layout_measured(dgan_handle h, int n_rows, int m, char*
 // (1: the caller's CSR was valid; 0: it was staged as the empty operator with NaN measurements).
 int dgan_debug_workspace_layout_measured_csr(dgan_handle h, int n_rows, int m, int nnz, char* buf, int buf_len) {
   if (h == nullptr || m <= 0 || m > h->hwc || !csr_nnz_ok(h, m, nnz)) { set_error("invalid argument"); return -1; }
-  return workspace_layout_impl(h, n_rows, buf, buf_len, false, m, nnz);
+  if (!layout_args_ok(h, n_rows, buf, buf_len)) return -1;
+  WsShape sh;
+  sh.m = m; sh.nnz = nnz;
+  return write_layout(h, n_rows, 1, sh, buf, buf_len);
 }
 
 // The same for the workspace of dgan_reconstruct_pruned (dgan_workspace_bytes_pruned): per region a line
@@ -3327,12 +3274,10 @@ int dgan_debug_workspace_layout_pruned(dgan_handle h, int batch, int rec_rr, con
                                        int weighted, char* buf, int buf_len) {
   if (h == nullptr || batch <= 0 || rec_rr <= 0 || buf == nullptr || buf_len <= 0) { set_error("invalid argument"); return -1; }
   if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
-  std::string out;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out);
-  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
-  memcpy(buf, out.c_str(), out.size() + 1);
-  return (int)out.size();
+  WsShape sh;
+  sh.weighted = weighted != 0;
+  sh.sched = sched; sh.n_points = n_points;
+  return write_layout(h, batch, rec_rr, sh, buf, buf_len);
 }
 
 // The same for the workspace of dgan_reconstruct_measured[_csr]_pruned (dgan_workspace_bytes_measured_pruned; nnz -1 for
@@ -3347,12 +3292,10 @@ int dgan_debug_workspace_layout_measured_pruned(dgan_handle h, int batch, int re
     return -1;
   }
   if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
-  std::string out;
-  size_t bytes = 0;
-  carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, false, &bytes, &out, m, nnz);
-  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
-  memcpy(buf, out.c_str(), out.size() + 1);
-  return (int)out.size();
+  WsShape sh;
+  sh.m = m; sh.nnz = nnz;
+  sh.sched = sched; sh.n_points = n_points;
+  return write_layout(h, batch, rec_rr, sh, buf, buf_len);
 }
 
 // The same for the workspace of the Adam entries (dgan_workspace_bytes_adam with m = 0, dgan_workspace_bytes_measured_adam
@@ -3367,17 +3310,11 @@ int dgan_debug_workspace_layout_adam(dgan_handle h, int batch, int rec_rr, int w
     set_error("invalid argument");
     return -1;
   }
-  std::string out;
-  if (unpruned(sched, n_points)) {
-    carve(h, batch * rec_rr, nullptr, &out, weighted != 0, m, m > 0 ? nnz : -1, false, nullptr, true);
-  } else {
-    if (check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
-    size_t bytes = 0;
-    carve_pruned(h, batch, rec_rr, sched, n_points, nullptr, weighted != 0, &bytes, &out, m, m > 0 ? nnz : -1, true);
-  }
-  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
-  memcpy(buf, out.c_str(), out.size() + 1);
-  return (int)out.size();
+  if (!unpruned(sched, n_points) && check_schedule(sched, n_points, rec_rr, 0) != 0) return -1;
+  WsShape sh;
+  sh.weighted = weighted != 0; sh.m = m; sh.nnz = m > 0 ? nnz : -1; sh.adam = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return write_layout(h, batch, rec_rr, sh, buf, buf_len);
 }
 
 // The same for the workspace of the convolution-measured entries (dgan_workspace_bytes_measured_conv, unpruned, without
@@ -3390,11 +3327,9 @@ int dgan_debug_workspace_layout_measured_conv(dgan_handle h, int n_rows, const d
     set_error("invalid argument");
     return -1;
   }
-  std::string out;
-  carve(h, n_rows, nullptr, &out, false, g.Ho * g.Wo * g.C, -1, false, nullptr, false, &g);
-  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
-  memcpy(buf, out.c_str(), out.size() + 1);
-  return (int)out.size();
+  WsShape sh;
+  sh.m = g.Ho * g.Wo * g.C; sh.conv = &g;
+  return write_layout(h, n_rows, 1, sh, buf, buf_len);
 }
 
 // The same for the workspace of the sparse-deviation entries (dgan_workspace_bytes_sparse_dev with m = 0,
@@ -3410,14 +3345,16 @@ int dgan_debug_workspace_layout_sparse_dev(dgan_handle h, int batch, int rec_rr,
     set_error("invalid argument");
     return -1;
   }
-  std::string out;
-  if (sdev_bytes(h, batch, rec_rr, weighted != 0, m, nnz, op != nullptr ? &g : nullptr, adam != 0, sched, n_points, &out) == 0) {
+  const ConvGeom* conv = op != nullptr ? &g : nullptr;
+  if (!sdev_args_ok(h, batch, rec_rr, weighted != 0, m, nnz, conv, sched, n_points)) {
     set_error("invalid argument");
     return -1;
   }
-  if (out.size() + 1 > (size_t)buf_len) { set_error("buffer too small"); return -1; }
-  memcpy(buf, out.c_str(), out.size() + 1);
-  return (int)out.size();
+  WsShape sh;
+  sh.weighted = weighted != 0; sh.m = m; sh.nnz = m > 0 && conv == nullptr ? nnz : -1; sh.conv = conv;
+  sh.adam = adam != 0; sh.sdev = true;
+  sh.sched = sched; sh.n_points = n_points;
+  return write_layout(h, batch, rec_rr, sh, buf, buf_len);
 }
 
 int dgan_debug_plan_stats(const dgan_desc* d, int n_rows, int n_pairs, char* buf, int buf_len) {

@@ -409,8 +409,17 @@ class DefenseGANBase(object):
         kw = {} if pw is None else {"pixel_weights": pw}
         if prune is not None:
             kw["prune"] = prune
-        if adam is not None:
-            kw["adam"] = adam
+        kw.update(self._option_kwargs(adam, huber, prior, sdev, deviation_out))
+        res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
+                                 momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
+                                 return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
+        return res
+
+    @staticmethod
+    def _option_kwargs(adam, huber, prior, sdev, deviation_out):
+        """The native keyword arguments of the checked options that are set: an option left unset is not passed, so the
+        call reaches the native layer as it did before that option existed."""
+        kw = {} if adam is None else {"adam": adam}
         if huber is not None:
             kw["huber_delta"] = huber
         if prior is not None:
@@ -418,10 +427,7 @@ class DefenseGANBase(object):
         if sdev is not None:
             kw["sparse_dev"] = sdev
             kw["deviation_out"] = deviation_out
-        res = native.reconstruct(x, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0, seed=seed,
-                                 momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
-                                 return_aux=return_aux, z_row_offset=int(z_row_offset), **kw)
-        return res
+        return kw
 
     def _prune_schedule(self):
         """`rec_prune` checked against rec_rr and rec_iters (None when unset); ValueError before any native call."""
@@ -566,14 +572,7 @@ class DefenseGANBase(object):
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
-        kw = {} if adam is None else {"adam": adam}
-        if huber is not None:
-            kw["huber_delta"] = huber
-        if prior is not None:
-            kw["z_prior"] = prior
-        if sdev is not None:
-            kw["sparse_dev"] = sdev
-            kw["deviation_out"] = deviation_out
+        kw = self._option_kwargs(adam, huber, prior, sdev, deviation_out)
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
@@ -602,14 +601,7 @@ class DefenseGANBase(object):
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(y.device)
         self.last_seed = seed = self._next_seed(0)
-        kw = {} if adam is None else {"adam": adam}
-        if huber is not None:
-            kw["huber_delta"] = huber
-        if prior is not None:
-            kw["z_prior"] = prior
-        if sdev is not None:
-            kw["sparse_dev"] = sdev
-            kw["deviation_out"] = deviation_out
+        kw = self._option_kwargs(adam, huber, prior, sdev, deviation_out)
         return native.reconstruct_measured(y, operator._with_kernels(k), int(self.rec_rr), int(self.rec_iters),
                                            float(self.rec_lr), z_init_val=z0, seed=seed,
                                            momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr), out=out,
@@ -662,14 +654,7 @@ class DefenseGANBase(object):
         z0 = self._as_cuda(z_init_val) if z_init_val is not None else None
         native = self._get_native(a.device)
         self.last_seed = seed = self._next_seed(0)
-        kw = {} if adam is None else {"adam": adam}
-        if huber is not None:
-            kw["huber_delta"] = huber
-        if prior is not None:
-            kw["z_prior"] = prior
-        if sdev is not None:
-            kw["sparse_dev"] = sdev
-            kw["deviation_out"] = deviation_out
+        kw = self._option_kwargs(adam, huber, prior, sdev, deviation_out)
         return native.reconstruct_measured(y, a, int(self.rec_rr), int(self.rec_iters), float(self.rec_lr), z_init_val=z0,
                                            seed=seed, momentum=float(self.rec_momentum), decay_lr=bool(self.rec_decay_lr),
                                            out=out, return_aux=return_aux, z_row_offset=int(z_row_offset), prune=prune,
