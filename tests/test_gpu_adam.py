@@ -11,6 +11,7 @@ dgan_reconstruct_measured_csr_adam), on MNIST and CelebA, fp32 and fp16, with Ba
   - the header's launch and enqueue counts, and no allocation in steady state;
   - the layout: the momentum layout plus s."""
 import ctypes
+import functools
 
 import numpy as np
 import pytest
@@ -19,6 +20,9 @@ import torch
 import adam_oracle as AO
 import layer_ref as LR
 import measured_oracle as MO
+from gpu_support import gsum as _gsum, option_layout as _layout, read as _read
+from gpu_support import rec, rec_m, release_cached_memory  # noqa: F401
+from gpu_support import bits as _bits, gen as _gen, images as _images, same as _same, z0 as _z0
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -27,102 +31,10 @@ HWC = {"mnist": 784, "celeba": 12288}
 SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 ADAM = (0.9, 0.999, 1e-8)
 CASES = [(p, a) for p in ("fp32", "fp16") for a in ("mnist", "celeba")]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-def _gen(arch, precision, use_bn=False, latent=128):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent, use_bn=use_bn,
-                                precision=precision, device=dev)
-    return w, g
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return all(torch.equal(_bits(p), _bits(q)) for p, q in zip(a, b))
-
-
-def _images(arch, w, B, seed=2):
-    return torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=seed)).cuda()
-
-
-def _z0(n, latent=128, seed=3):
-    return torch.tensor(O.sample_z0(n, latent, seed=seed)).cuda()
-
-
-def _rec(gen, x, R, L, lr, z0, adam=ADAM, **kw):
-    return [t.clone() for t in gen.reconstruct(x, R, L, lr, z_init_val=z0, adam=adam, return_aux=True, **kw)]
-
-
-def _rec_m(gen, y, a, R, L, lr, z0, adam=ADAM, **kw):
-    return [t.clone() for t in gen.reconstruct_measured(y, a, R, L, lr, z_init_val=z0, adam=adam, return_aux=True, **kw)]
+_rec, _rec_m = functools.partial(rec, adam=ADAM), functools.partial(rec_m, adam=ADAM)
 
 
 # ---- the workspace ----
-
-def _layout(gen, batch, R, weighted=0, m=0, nnz=-1, sched=None, adam=True):
-    """{name: (type, offset, dims)} of an unpruned workspace (adam: dgan_debug_workspace_layout_adam), and the raw text."""
-    from defensegan_b200 import _native
-    buf = ctypes.create_string_buffer(1 << 18)
-    if adam:
-        fn = gen.lib.dgan_debug_workspace_layout_adam
-        fn.restype = ctypes.c_int
-        fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                       ctypes.POINTER(_native.dgan_prune_point), ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-        arr = None
-        if sched:
-            arr = (_native.dgan_prune_point * len(sched))(*[_native.dgan_prune_point(a, b) for a, b in sched])
-        assert fn(gen._handle, batch, R, weighted, m, nnz, arr, len(sched) if sched else 0, buf, len(buf)) > 0
-    elif sched:
-        fn = gen.lib.dgan_debug_workspace_layout_pruned
-        fn.restype = ctypes.c_int
-        fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_native.dgan_prune_point), ctypes.c_int,
-                       ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-        arr = (_native.dgan_prune_point * len(sched))(*[_native.dgan_prune_point(a, b) for a, b in sched])
-        assert fn(gen._handle, batch, R, arr, len(sched), weighted, buf, len(buf)) > 0
-    elif m > 0:
-        name = "dgan_debug_workspace_layout_measured" + ("_csr" if nnz >= 0 else "")
-        fn = getattr(gen.lib, name)
-        fn.restype = ctypes.c_int
-        extra = [ctypes.c_int] if nnz >= 0 else []
-        fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int] + extra + [ctypes.c_char_p, ctypes.c_int]
-        args = (gen._handle, batch * R, m) + ((nnz,) if nnz >= 0 else ()) + (buf, len(buf))
-        assert fn(*args) > 0
-    else:
-        fn = gen.lib.dgan_debug_workspace_layout_weighted if weighted else gen.lib.dgan_debug_workspace_layout
-        fn.restype = ctypes.c_int
-        fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-        assert fn(gen._handle, batch * R, buf, len(buf)) > 0
-    text = buf.value.decode()
-    bufs = {}
-    for line in text.splitlines():
-        f = line.split()
-        if len(f) >= 4 and f[1] in ("f32", "f16", "u64", "u32", "i32"):
-            bufs[f[0]] = (f[1], int(f[2]), [int(v) for v in f[3:]])
-    return bufs, text
-
-
-def _read(gen, bufs, name):
-    typ, off, dims = bufs[name]
-    dt = {"f32": torch.float32, "f16": torch.float16, "i32": torch.int32, "u32": torch.int32}[typ]
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr() + off
-    n = int(np.prod(dims))
-    torch.cuda.synchronize()
-    return gen._ws[base:base + n * dt.itemsize].view(dt).view(*dims).clone()
-
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
 def test_adam_layout_is_the_momentum_layout_plus_s(precision):
@@ -136,10 +48,10 @@ def test_adam_layout_is_the_momentum_layout_plus_s(precision):
             lines = ada.splitlines()
             assert "\n".join(lines[:-1]) + "\n" == mom, kw
             name, typ, off, *dims = lines[-1].split()
-            n_pad = bufs["z"][2][0]
+            n_pad = bufs["bufs"]["z"][2][0]
             assert (name, typ, dims) == ("s", "f32", [str(n_pad), "128"]), kw
             end = max(o + (int(np.prod(d)) * 4 + 1023) // 1024 * 1024 for t, o, d in _layout(gen, B, R, adam=False,
-                                                                                              **kw)[0].values())
+                                                                                              **kw)[0]["bufs"].values())
             assert int(off) == end, kw
         for weighted in (0, 1):
             _, mom = _layout(gen, B, R, weighted=weighted, sched=sched, adam=False)
@@ -152,13 +64,6 @@ def test_adam_layout_is_the_momentum_layout_plus_s(precision):
 
 
 # ---- the update on its stored operands ----
-
-def _gsum(g):
-    gs = g[0].clone()
-    for p in range(1, g.shape[0]):
-        gs = gs + g[p]
-    return gs
-
 
 def _check_update(ws1, ws2, z0p, lr, n, lat, tc, row_mul, pad_rows_zero, tag):
     """ws1 after L = 2 (step k = 1 from m = s = 0), ws2 after L = 3 (step k = 2 from ws1's m, s, z), each step against

@@ -27,6 +27,9 @@ import torch
 
 import huber_oracle as H
 import measured_oracle as MO
+from gpu_support import bits as _bits, gen as _gen, images as _images, same as _same, z0 as _z0
+from gpu_support import rec as _rec, rec_m as _rec_m, release_cached_memory  # noqa: F401
+from gpu_support import layout, read_call, view, views
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -35,48 +38,6 @@ SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 ADAM = (0.9, 0.999, 1e-8)
 CASES = [(p, a) for p in ("fp32", "fp16") for a in ("mnist", "celeba")]
 INF = float("inf")
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-def _gen(arch, precision, use_bn=False, latent=128, net_dim=64):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, net_dim=net_dim, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent,
-                                net_dim=net_dim, use_bn=use_bn, precision=precision, device=dev)
-    return w, g
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return all(torch.equal(_bits(p), _bits(q)) for p, q in zip(a, b))
-
-
-def _images(arch, w, B, seed=2):
-    return torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=seed)).cuda()
-
-
-def _z0(n, latent=128, seed=3):
-    return torch.tensor(O.sample_z0(n, latent, seed=seed)).cuda()
-
-
-def _rec(gen, x, R, L, lr, z0, **kw):
-    return [t.clone() for t in gen.reconstruct(x, R, L, lr, z_init_val=z0, return_aux=True, **kw)]
-
-
-def _rec_m(gen, y, a, R, L, lr, z0, **kw):
-    return [t.clone() for t in gen.reconstruct_measured(y, a, R, L, lr, z_init_val=z0, return_aux=True, **kw)]
 
 
 def _salt_and_pepper(x, arch, p, seed=5):
@@ -334,7 +295,6 @@ def test_huber_loss_grad_each_layer_direction(arch, latent, net_dim, use_bn, pre
     that clips 20 - 80 % of the pixels, the share taken from the fp64 reference."""
     import huber_layer_ref as HR
     import layer_ref as LR
-    from test_gpu_layers import read_call
     w, gen = _gen(arch, precision, use_bn, latent, net_dim)
     try:
         R_ = 1 if n_rows == 1 else 2
@@ -372,8 +332,6 @@ def test_huber_loss_grad_measured_each_layer_direction(arch, latent, net_dim, us
     the residuals."""
     import huber_layer_ref as HR
     import layer_ref as LR
-    from test_gpu_layers import read_call
-    from test_gpu_measured import _buffers
     w, gen = _gen(arch, precision, use_bn, latent, net_dim)
     try:
         R_ = 2
@@ -389,7 +347,7 @@ def test_huber_loss_grad_measured_each_layer_direction(arch, latent, net_dim, us
         gen.loss_grad_measured(y, a, z, R_, huber_delta=delta)
         torch.cuda.synchronize()
         ws, net = read_call(gen, w, arch, latent, net_dim, use_bn, precision, n_rows)
-        wsm = _buffers(gen, n_rows, m)
+        wsm = views(gen, layout(gen, "_measured", n_rows, m)[0][0])
         for k in ("am", "amt", "ym", "r", "dym", "mloss_part", "mscale"):
             ws[k] = wsm[k]
         stats = LR.Stats()
@@ -408,15 +366,6 @@ def test_huber_loss_grad_measured_each_layer_direction(arch, latent, net_dim, us
 
 
 # ---- calls on one handle, counts, steady state ----
-
-def _layout_text(gen, n_rows, weighted):
-    fn = gen.lib.dgan_debug_workspace_layout_weighted if weighted else gen.lib.dgan_debug_workspace_layout
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    assert fn(gen._handle, n_rows, buf, len(buf)) > 0
-    return buf.value.decode()
-
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
 def test_graph_cache_counts_and_steady_state(precision):
@@ -468,14 +417,12 @@ def test_graph_cache_counts_and_steady_state(precision):
         # the workspace is the counterpart's: the same size, the same layout string (dgan_debug_workspace_layout
         # [_weighted]), and a Huber call leaves G(z) where that layout puts y
         for pw in (None, torch.ones_like(x)):
-            lay = _layout_text(gen, B * R, pw is not None)
+            regions, lay = layout(gen, "_weighted" if pw is not None else "", B * R)
             size = gen._workspace(B, R, weighted=pw is not None)[1]
             yh, _, _ = gen.loss_grad(x, z0, R, pixel_weights=pw, huber_delta=0.1)
             assert gen._workspace(B, R, weighted=pw is not None)[1] == size
-            assert _layout_text(gen, B * R, pw is not None) == lay
-            f = next(ln.split() for ln in lay.splitlines() if ln.split()[0] == "y")
-            base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr() + int(f[2])
-            stored = gen._ws[base:base + B * R * 784 * 4].view(torch.float32).view(B * R, 784)
+            assert layout(gen, "_weighted" if pw is not None else "", B * R)[1] == lay
+            stored = view(gen, regions[0], "y").flatten()[:B * R * 784].view(B * R, 784)
             assert torch.equal(_bits(stored), _bits(yh.reshape(B * R, 784)))
     finally:
         gen.close()

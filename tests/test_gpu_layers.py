@@ -36,48 +36,10 @@ import pytest
 import torch
 
 import layer_ref as R
+from gpu_support import MATRIX, ROWS, gen, read_call
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
-
-# (arch, latent_dim, net_dim, use_bn)
-MATRIX = [("mnist", 128, 64, False), ("mnist", 128, 64, True), ("mnist", 100, 32, False), ("mnist", 128, 128, False),
-          ("celeba", 128, 64, False), ("celeba", 200, 48, False), ("celeba", 64, 128, True)]
-ROWS = [1, 300, 2560]
-DTYPES = {"f32": torch.float32, "f16": torch.float16, "u64": torch.int64, "u32": torch.int32}
-
-
-def workspace(native, n_rows):
-    """The buffers of the native handle's workspace for n_rows latent rows, by name, as tensors viewing it."""
-    lib = native.lib
-    lib.dgan_debug_workspace_layout.restype = ctypes.c_int
-    lib.dgan_debug_workspace_layout.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    n = lib.dgan_debug_workspace_layout(native._handle, n_rows, buf, len(buf))
-    assert n > 0, lib.dgan_last_error()
-    ws = native._ws
-    base = (ws.data_ptr() + 1023) // 1024 * 1024 - ws.data_ptr()
-    out, meta = {}, {}
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if f[1] in DTYPES:
-            dt = DTYPES[f[1]]
-            dims = [int(d) for d in f[3:]]
-            size = int(np.prod(dims)) * torch.tensor([], dtype=dt).element_size()
-            off = base + int(f[2])
-            out[f[0]] = ws[off:off + size].view(dt).view(dims)
-        else:
-            meta[f[0]] = [int(v) for v in f[1:]]
-    return out, meta
-
-
-def make(arch, latent, net_dim, use_bn, precision):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, net_dim=net_dim, use_bn=use_bn, random_bias=True)
-    native = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent,
-                                     net_dim=net_dim, use_bn=use_bn, precision=precision, device=dev)
-    return native, w
 
 
 def run_loss_grad(native, w, arch, latent, n_rows, seed=3):
@@ -91,19 +53,11 @@ def run_loss_grad(native, w, arch, latent, n_rows, seed=3):
     return z, x_rows
 
 
-def read_call(native, w, arch, latent, net_dim, use_bn, precision, n_rows):
-    """The workspace a call for n_rows rows left, and the reference network at the handle's padded widths."""
-    ws, meta = workspace(native, n_rows)
-    assert meta["n_rows"] == [n_rows]
-    net = R.Net(arch, latent, net_dim, use_bn, precision, meta["widths"], w, torch.device("cuda", 0))
-    return ws, net
-
-
 @pytest.mark.parametrize("n_rows", ROWS)
 @pytest.mark.parametrize("precision", ["fp16", "fp32"])
 @pytest.mark.parametrize("arch,latent,net_dim,use_bn", MATRIX)
 def test_loss_grad_each_layer_direction(arch, latent, net_dim, use_bn, precision, n_rows):
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         z, x_rows = run_loss_grad(native, w, arch, latent, n_rows)
         ws, net = read_call(native, w, arch, latent, net_dim, use_bn, precision, n_rows)
@@ -122,7 +76,7 @@ def test_every_slot_count_matches_fp64_per_layer():
     """Every instantiation of the tensor-core kernel a layer-direction can be planned on (dgan_debug_force_slots), each
     checked against the fp64 reference rather than only against the default plan."""
     arch, latent, net_dim, use_bn, n_rows = "mnist", 128, 64, False, 300
-    native, w = make(arch, latent, net_dim, use_bn, "fp16")
+    w, native = gen(arch, "fp16", use_bn, latent, net_dim)
     lib = native.lib
     lib.dgan_debug_slot_choices.restype = ctypes.c_int
     lib.dgan_debug_slot_choices.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.c_int]
@@ -156,7 +110,7 @@ def test_every_slot_count_matches_fp64_per_layer():
 def test_vjp_each_layer_direction(arch, latent, net_dim, use_bn, precision, n_rows):
     """dgan_vjp: the cotangent entry (d(pre) from dy and the stored y, its power-of-two row scales, zeroed tile-padding
     rows), the forward it recomputes, and every backward layer-direction from there."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         g = torch.Generator().manual_seed(n_rows)
         z = torch.tensor(O.sample_z0(n_rows, latent, seed=7)).cuda()
@@ -180,7 +134,7 @@ def test_vjp_each_layer_direction(arch, latent, net_dim, use_bn, precision, n_ro
 def test_jvp_each_layer_direction(arch, latent, net_dim, use_bn, precision, n_rows):
     """dgan_jvp: the tangent entry (z_h = RN16(t * s_n), or v = t), every tangent direction on its stored input (masked by
     the primal masks, or through the BatchNorm tangent), the last layer's fp32 tangent of pre and ty."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         g = torch.Generator().manual_seed(n_rows + 1)
         z = torch.tensor(O.sample_z0(n_rows, latent, seed=8)).cuda()
@@ -204,7 +158,7 @@ def test_momentum_update_after_one_step(arch, latent, net_dim, use_bn, precision
     """dgan_reconstruct with L = 2 from a given z0: the first step's partial sums stay in g, and z, v, z_h hold the update
     (the tail of the tensor-core Linear backward, or the fp32 path's momentum kernel); the partial sums themselves are
     checked as the Linear backward of the stored d(pre_0)."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         B, Rr, lr = 150, 2, 10.0
         n = B * Rr

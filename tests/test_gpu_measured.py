@@ -17,34 +17,11 @@ import pytest
 import torch
 
 import measured_oracle as MO
+from gpu_support import HWC, SHAPE, TOL, check_products, layout, release_cached_memory, views  # noqa: F401
+from gpu_support import gen as _gen
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back the blocks this module left
-    cached, so that the handles of later tests find the memory."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-TOL = {"fp32": dict(fwd=2e-5, grad_rel=2e-4, grad_cos=0.999999, loss=1e-6),
-       "fp16": dict(fwd=5e-3, grad_rel=6e-2, grad_cos=0.998, loss=1e-4)}
-HWC = {"mnist": 784, "celeba": 12288}
-SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
-
-
-def _gen(arch, precision, use_bn=False, latent=128, net_dim=64):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, net_dim=net_dim, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent, net_dim=net_dim,
-                                use_bn=use_bn, precision=precision, device=dev)
-    return w, g
 
 
 def _measure(a, x):
@@ -184,26 +161,6 @@ def test_measured_loss_and_grad_match_fp64_oracle(precision, arch):
         gen.close()
 
 
-def _buffers(gen, n_rows, m):
-    """The f32 buffers of the measured workspace of the last call, by name, as views of the workspace."""
-    fn = gen.lib.dgan_debug_workspace_layout_measured
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    assert fn(gen._handle, n_rows, m, buf, len(buf)) > 0
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr()
-    out = {}
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if len(f) < 4 or f[1] != "f32":
-            continue
-        dims = [int(d) for d in f[3:]]
-        n = int(np.prod(dims))
-        off = base + int(f[2])
-        out[f[0]] = gen._ws[off:off + 4 * n].view(torch.float32).view(*dims)
-    return out
-
-
 @pytest.mark.parametrize("m", [1, 50, 200, 784])
 @pytest.mark.parametrize("precision", ["fp16", "fp32"])
 @pytest.mark.parametrize("arch", ["mnist", "celeba"])
@@ -222,7 +179,7 @@ def test_each_measurement_product_on_its_stored_operands(arch, precision, m):
         z = torch.tensor(O.sample_z0(n, 128, seed=4)).cuda()
         gen.loss_grad_measured(y, a, z, R_)
         torch.cuda.synchronize()
-        ws = _buffers(gen, n, m)
+        ws = views(gen, layout(gen, "_measured", n, m)[0][0])
         m_ld = ws["am"].shape[0]
         assert m_ld % 64 == 0 and m_ld >= m
         assert torch.equal(ws["am"][:m], a) and not ws["am"][m:].any()
@@ -232,37 +189,6 @@ def test_each_measurement_product_on_its_stored_operands(arch, precision, m):
         print("%s %s m=%d: dy max err / bound %.3g" % (precision, arch, m, dy_ratio))
     finally:
         gen.close()
-
-
-def check_products(ws, n, rec_rr, m, hwc, precision):
-    """r = A G - y and dy = (2/m) A^T r of the last measured call on n latent rows (rec_rr restarts per image) against
-    fp64 on the operands the kernels read (the workspace buffers of _buffers), each within the bound of its arithmetic
-    (test_each_measurement_product_on_its_stored_operands); the padded measurements of r exact zeros.  Returns the
-    largest error over its bound of r and of dy."""
-    u = 2.0 ** -24
-    rnd = 2.0 ** -10 if precision == "fp16" else 0.0      # two operands rounded to TF32, 2^-11 each
-    m_ld = ws["am"].shape[0]
-
-    def bound(x, wt, k):
-        g = k * u / (1 - k * u)
-        return (rnd + g) * (x.abs().double() @ wt.abs().double().t())
-
-    g = ws["y"][:n]
-    y_rows = ws["ym"][:n // rec_rr].repeat_interleave(rec_rr, dim=0)
-    r64 = g.double() @ ws["am"].double().t() - y_rows.double()
-    r = ws["r"][:n]
-    err = (r.double() - r64).abs()
-    lim = bound(g, ws["am"], hwc) + u * r64.abs() + 1e-30
-    r_ratio = float((err / lim).max())
-    assert bool((err <= lim).all()), "measurement product (r): max err / bound %.3g" % r_ratio
-    assert not r[:, m:].any()                              # padded measurements are exact zeros
-    dy64 = (2.0 / m) * (r.double() @ ws["amt"].double().t())
-    dy = ws["dym"][:n]
-    err = (dy.double() - dy64).abs()
-    lim = (2.0 / m) * bound(r, ws["amt"], m_ld) * (1 + 2 * u) + 2 * u * dy64.abs() + 1e-30
-    dy_ratio = float((err / lim).max())
-    assert bool((err <= lim).all()), "adjoint product (dy): max err / bound %.3g" % dy_ratio
-    return r_ratio, dy_ratio
 
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])

@@ -13,20 +13,12 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_support import gen as _gen, layout, release_cached_memory, views  # noqa: F401
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 def _taps(kh, kw, seed, zeros=False):
@@ -49,15 +41,6 @@ def _ops():
         "box2": ConvOperator.box(2),
         "box4": ConvOperator.box(4),
     }
-
-
-def _gen(arch, precision, use_bn=False):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], use_bn=use_bn,
-                                precision=precision, device=dev)
-    return w, g
 
 
 def _measure(op, arch, w, B, seed=2):
@@ -137,31 +120,12 @@ def test_per_image_kernels_equal_single_image_csr_calls(arch, precision, variant
         gen.close()
 
 
-def _layout_fn(gen):
-    from defensegan_b200 import _native
-    fn = gen.lib.dgan_debug_workspace_layout_measured_conv
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(_native.dgan_conv_op), ctypes.c_char_p, ctypes.c_int]
-    return fn
-
-
 def _buffers(gen, n_rows, op):
     """The buffers of the conv-measured workspace of the last call, by name, as views of the workspace."""
     from defensegan_b200 import _native
     kh, kw = op.kernel_size
     cop = _native.dgan_conv_op(kh, kw, op.padding[0], op.padding[1], op.stride)
-    buf = ctypes.create_string_buffer(1 << 16)
-    assert _layout_fn(gen)(gen._handle, n_rows, ctypes.byref(cop), buf, len(buf)) > 0
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr()
-    out = {}
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if len(f) < 4 or f[1] != "f32":
-            continue
-        dims = [int(d) for d in f[3:]]
-        off = base + int(f[2])
-        out[f[0]] = gen._ws[off:off + 4 * int(np.prod(dims))].view(torch.float32).view(*dims)
-    return out
+    return views(gen, layout(gen, "_measured_conv", n_rows, ctypes.byref(cop))[0][0])
 
 
 @pytest.mark.parametrize("n_rows", [1, 300, 2560])

@@ -18,33 +18,30 @@ import torch
 
 import measured_oracle as MO
 import sparse_operators as SO
+from gpu_support import gen as _gen, layout, release_cached_memory, views  # noqa: F401
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
+def _release_operators(release_cached_memory):
+    """Drop the cached operators before the module's cached memory is handed back."""
     yield
-    import gc
     _OPS.clear()
-    gc.collect()
-    torch.cuda.empty_cache()
+
+
+def _has_guard(gen):
+    """The library validates a CSR before using it: its layout names the validity flag."""
+    try:
+        return "\ncsr_valid i32 " in layout(gen, "_measured_csr", 1, 1, 1)[1]
+    except (AttributeError, AssertionError):
+        return False
 
 
 HWC = {"mnist": 784, "celeba": 12288}
 SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 _OPS = {}
-
-
-def _gen(arch, precision, use_bn=False):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], use_bn=use_bn,
-                                precision=precision, device=dev)
-    return w, g
 
 
 def _operator(arch, kind):
@@ -136,38 +133,6 @@ def test_fp16_long_horizon_parity(arch, kind):
         gen.close()
 
 
-def _buffers(gen, n_rows, m, nnz):
-    """The buffers of the CSR-measured workspace of the last call, by name, as views of the workspace."""
-    fn = gen.lib.dgan_debug_workspace_layout_measured_csr
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    assert fn(gen._handle, n_rows, m, nnz, buf, len(buf)) > 0
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr()
-    out = {}
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if len(f) < 4 or f[1] not in ("f32", "i32"):
-            continue
-        dims = [int(d) for d in f[3:]]
-        n = int(np.prod(dims))
-        off = base + int(f[2])
-        out[f[0]] = gen._ws[off:off + 4 * n].view(torch.float32 if f[1] == "f32" else torch.int32).view(*dims)
-    return out
-
-
-def _has_guard(gen):
-    """The library validates a CSR before using it: its layout names the validity flag."""
-    try:
-        fn = gen.lib.dgan_debug_workspace_layout_measured_csr
-    except AttributeError:
-        return False
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    return fn(gen._handle, 1, 1, 1, buf, len(buf)) > 0 and "\ncsr_valid i32 " in buf.value.decode()
-
-
 def _dense64(rp, ci, v, n_rows, n_cols):
     """The dense fp64 matrix of a staged CSR, and the non-zeros per row."""
     rp = rp.long()
@@ -202,7 +167,7 @@ def test_each_product_on_its_stored_operands(arch, kind, precision, n_rows):
         gen._ws.zero_()
         gen.loss_grad_measured(y, acsr, z, R_)
         torch.cuda.synchronize()
-        ws = _buffers(gen, n_rows, m, nnz)
+        ws = views(gen, layout(gen, "_measured_csr", n_rows, m, nnz)[0][0])
         assert int(ws["csr_valid"][0]) == 1
         m_ld = ws["r"].shape[1]
         # the staged operator and its transpose
@@ -337,7 +302,7 @@ def test_malformed_csr_through_the_c_abi_gives_nan_and_leaves_the_next_call_alon
             assert rc == 0
             torch.cuda.synchronize()
             assert bool(torch.isnan(loss).all())
-            ws_ = _buffers(gen, B * R_, m, nnz)
+            ws_ = views(gen, layout(gen, "_measured_csr", B * R_, m, nnz)[0][0])
             assert int(ws_["csr_valid"][0]) == 0 and not ws_["a_rp"].any() and not ws_["at_rp"].any()
             again = gen.reconstruct_measured(y, acsr, R_, L, 1.0, z_init_val=z0, return_aux=True)
             assert all(torch.equal(p, q) for p, q in zip(again, good))

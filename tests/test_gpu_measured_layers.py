@@ -31,23 +31,13 @@ import torch
 
 import layer_ref as R
 import measured_oracle as MO
+from gpu_support import HWC, MATRIX, ROWS, SHAPE, TOL, check_products, gen, layout, read_call, views
+from gpu_support import release_cached_memory  # noqa: F401
 from oracle import defensegan_oracle as O
-from test_gpu_layers import MATRIX, ROWS, make, read_call
-from test_gpu_measured import HWC, SHAPE, TOL, _buffers, check_products
 
 pytestmark = pytest.mark.gpu
 
 MEASURED = ("am", "amt", "ym", "r", "dym", "mloss_part", "mscale")
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back the blocks this module left
-    cached, so that the handles of later tests find the memory."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 def _m(arch):
@@ -63,7 +53,7 @@ def _measure(a, x):
 def _read(native, w, arch, latent, net_dim, use_bn, precision, n_rows, m):
     """The workspace of the last measured call: the common buffers (typed) and the measured ones, by name."""
     ws, net = read_call(native, w, arch, latent, net_dim, use_bn, precision, n_rows)
-    wsm = _buffers(native, n_rows, m)
+    wsm = views(native, layout(native, "_measured", n_rows, m)[0][0])
     for k in MEASURED:
         ws[k] = wsm[k]
     return ws, net
@@ -72,7 +62,7 @@ def _read(native, w, arch, latent, net_dim, use_bn, precision, n_rows, m):
 @pytest.mark.parametrize("precision", ["fp16", "fp32"])
 @pytest.mark.parametrize("arch,latent,net_dim,use_bn", MATRIX)
 def test_loss_grad_measured_each_layer_direction(arch, latent, net_dim, use_bn, precision):
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         hwc = HWC[arch]
         for n_rows in ROWS:
@@ -110,7 +100,7 @@ def test_momentum_rows_after_one_step(arch, latent, net_dim, use_bn, precision):
     still in the workspace: the L-1 iteration runs only the forward (act, mask, pre, y) and the measurement product
     (r, mloss_part), then the loss finish (loss) and the select.  So g, dact.0, mscale and the updated z, v, z_h are
     step 0's: the partial sums are checked as the Linear backward of the stored d(pre_0), then the update."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         B, Rr, m = 150, 2, _m(arch)
         n = B * Rr
@@ -145,7 +135,7 @@ def test_measured_calls_at_padded_widths(arch, latent, net_dim, use_bn, precisio
     test_gpu_parity.py's BatchNorm tolerances.  The BatchNorm rows run 8 MNIST or 4 CelebA images: with the 6 rows of
     3 MNIST images the problem itself is ill-conditioned (the fp32 and fp64 oracles' gradients differ by 1% of their
     largest element), and so is the CelebA loop of 2 images (0.8% between the oracles' reconstructions)."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         if use_bn:
             B, R_ = (8, 2) if arch == "mnist" else (4, 2)
@@ -198,7 +188,7 @@ def test_operator_scale_is_exact(arch, latent, net_dim, use_bn, precision):
     absorbs the 4^k of d(pre) exactly (on the fp32 path the backward is linear in it), no value leaves the normal fp32
     range at these k - so G is bit-identical and loss and gradient are exactly 4^k times the k = 0 result; with rec_lr
     4^-k times, every step moves z by the same bits, and rec, idx are bit-identical, the loss exactly 4^k times."""
-    native, w = make(arch, latent, net_dim, use_bn, precision)
+    w, native = gen(arch, precision, use_bn, latent, net_dim)
     try:
         B, R_, L, m = 4, 3, 5, _m(arch)
         lr = 0.5 if use_bn else 10.0 * m / HWC[arch]
@@ -229,7 +219,7 @@ def test_zero_operator(precision):
     as the kernels sum it: one partial per 64-column tile, the tiles in a fixed order - within the fp32 bound of any
     order of m + 1 additions and the two roundings of the 1/m multiply."""
     arch, latent, B, R_, m = "mnist", 128, 4, 3, 50
-    native, w = make(arch, latent, 64, False, precision)
+    w, native = gen(arch, precision, False, latent, 64)
     try:
         a = torch.zeros(m, HWC[arch], device="cuda")
         y = torch.randn(B, m, generator=torch.Generator().manual_seed(12)).cuda()
@@ -254,7 +244,7 @@ def test_repeated_row_is_the_row_scaled_by_sqrt2(precision):
     """A with row j repeated (and y_j) is, at the normaliser m + 1, the m-row operator with row j and y_j scaled by
     sqrt(2): its loss is m / (m + 1) times that one's, and with rec_lr (m + 1) / m times it takes the same steps."""
     arch, B, R_, L, m, j = "mnist", 4, 3, 8, 64, 5
-    native, w = make(arch, 128, 64, False, precision)
+    w, native = gen(arch, precision, False, 128, 64)
     try:
         x = torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=2)).cuda()
         z0 = torch.tensor(O.sample_z0(B * R_, 128, seed=4)).cuda()
@@ -287,7 +277,7 @@ def test_misaligned_out_is_refused(precision):
     before."""
     from defensegan_b200 import _native
     arch, B, R_, L, m = "mnist", 3, 2, 3, 100
-    native, w = make(arch, 128, 64, False, precision)
+    w, native = gen(arch, precision, False, 128, 64)
     lib = native.lib
     try:
         hwc = HWC[arch]

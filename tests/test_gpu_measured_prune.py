@@ -20,6 +20,8 @@ import torch
 
 import measured_oracle as MO
 import sparse_operators as SO
+from gpu_support import bits as _bits, gen as _gen, layout
+from gpu_support import read as _read, release_cached_memory, same as _same, ws_base  # noqa: F401
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -31,24 +33,6 @@ THREE = [(3, 3), (6, 2), (9, 1)]
 # (operator kind, passed as CSR): a dense Gaussian sketch, the 2x2 block average and pixel subsampling as CSR
 OPS = [("gauss", False), ("block2", True), ("sub", True)]
 CASES = [(p, a, k, c) for p in ("fp32", "fp16") for a in ("mnist", "celeba") for k, c in OPS]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-def _gen(arch, precision, use_bn=False):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], use_bn=use_bn,
-                                precision=precision, device=dev)
-    return w, g
 
 
 def _operator(arch, kind):
@@ -69,14 +53,6 @@ def _problem(arch, kind, csr, w, B, R, seed=2):
     z0 = torch.tensor(O.sample_z0(B * R, 128, seed=seed + 1)).cuda()
     lr = 10.0 * min(1.0, 4.0 * a.shape[0] / a.shape[1])
     return (ad.to_sparse_csr() if csr else ad), torch.tensor(y).cuda(), z0, lr
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return all(torch.equal(_bits(p), _bits(q)) for p, q in zip(a, b))
 
 
 def _call(gen, y, op, R, L, z0, lr, prune, decay=False, **kw):
@@ -215,40 +191,13 @@ def test_malformed_csr_gives_nan_and_leaves_the_next_call_alone():
 # ---- the workspace ----
 
 def _layout(gen, batch, R, m, nnz, sched):
-    """[{kind, off, rows, n_pad, bufs: {name: (type, offset, dims)}}] in order: the operator block, then the regions."""
-    from defensegan_b200 import _native
-    fn = gen.lib.dgan_debug_workspace_layout_measured_pruned
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                   ctypes.POINTER(_native.dgan_prune_point), ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    arr = (_native.dgan_prune_point * len(sched))(*[_native.dgan_prune_point(a, b) for a, b in sched])
-    buf = ctypes.create_string_buffer(1 << 18)
-    assert fn(gen._handle, batch, R, m, nnz, arr, len(sched), buf, len(buf)) > 0
-    blocks = []
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if f[0] in ("operator", "region"):
-            blocks.append({"kind": f[0], "off": int(f[1]) if f[0] == "operator" else int(f[2]),
-                           "rows": int(f[2]) if f[0] == "operator" else int(f[3]), "bufs": {}})
-        elif f[0] == "n_pad":
-            blocks[-1]["n_pad"] = int(f[1])
-        elif len(f) >= 4 and f[1] in ("f32", "f16", "u64", "u32", "i32"):
-            blocks[-1]["bufs"][f[0]] = (f[1], int(f[2]), [int(v) for v in f[3:]])
-    return blocks
+    """{"operator": the operator block, k: region k}, each {off, n_rows, n_pad, bufs}, in that order."""
+    return layout(gen, "_measured_pruned", batch, R, m, nnz, list(sched), len(sched))[0]
 
 
 def _block_bytes(block):
     size = {"f32": 4, "f16": 2, "u64": 8, "u32": 4, "i32": 4}
     return max(off + (int(np.prod(d)) * size[t] + 1023) // 1024 * 1024 for t, off, d in block["bufs"].values())
-
-
-def _read(gen, block, name):
-    typ, off, dims = block["bufs"][name]
-    dt = {"f32": torch.float32, "f16": torch.float16, "i32": torch.int32, "u32": torch.int32}[typ]
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr() + block["off"] + off
-    n = int(np.prod(dims))
-    torch.cuda.synchronize()
-    return gen._ws[base:base + n * dt.itemsize].view(dt).view(*dims).clone()
 
 
 @pytest.mark.parametrize("csr", [False, True])
@@ -259,8 +208,9 @@ def test_layout_is_the_operator_block_once_then_the_regions(csr):
         B, R, m = 8, 10, 2000
         nnz = 30000 if csr else -1
         for sched in (ONE, THREE, [(40, 2)], [(20, 5), (60, 2), (120, 1)]):
-            blocks = _layout(gen, B, R, m, nnz, sched)
-            assert [b["kind"] for b in blocks] == ["operator"] + ["region"] * (len(sched) + 1)
+            regions = _layout(gen, B, R, m, nnz, sched)
+            assert list(regions) == ["operator"] + list(range(len(sched) + 1))
+            blocks = list(regions.values())
             op = blocks[0]
             m_ld = (m + 63) // 64 * 64
             if csr:
@@ -268,11 +218,11 @@ def test_layout_is_the_operator_block_once_then_the_regions(csr):
                 assert op["bufs"]["at_rp"][2] == [12288 + 1]
             else:
                 assert op["bufs"]["am"][2] == [m_ld, 12288] and op["bufs"]["amt"][2] == [12288, m_ld]
-            assert op["bufs"]["ym"][2] == [B, m_ld] and op["off"] == 0 and op["rows"] == B
+            assert op["bufs"]["ym"][2] == [B, m_ld] and op["off"] == 0 and op["n_rows"] == B
             off = _block_bytes(op)
             for k, reg in enumerate(blocks[1:]):
                 assert reg["off"] == off, k
-                assert reg["rows"] == B * (R if k == 0 else sched[k - 1][1])
+                assert reg["n_rows"] == B * (R if k == 0 else sched[k - 1][1])
                 names = set(reg["bufs"])
                 assert {"z", "v", "y", "r", "dym", "mloss_part", "mscale", "orig", "src", "sel"} <= names
                 assert not names & {"am", "amt", "ym", "a_rp", "a_ci", "a_v", "at_rp", "at_ci", "at_v", "csr_bad",
@@ -306,9 +256,9 @@ def test_gathered_rows_equal_the_source_rows(precision, arch, kind, csr):
         sched = [(L - 1, keep)]
         got = _call(gen, y, op, R, L, z0, lr, sched)
         nnz = op.values().numel() if csr else -1
-        blocks = _layout(gen, B, R, op.shape[0], nnz, sched)
+        blocks = list(_layout(gen, B, R, op.shape[0], nnz, sched).values())
         r0, r1 = blocks[1], blocks[2]
-        assert (r0["rows"], r1["rows"]) == (B * R, B * keep)
+        assert (r0["n_rows"], r1["n_rows"]) == (B * R, B * keep)
         src = _read(gen, r1, "src")[:B * keep].long()
         orig = _read(gen, r1, "orig")[:B * keep].long()
         assert torch.equal(orig, src % R) and torch.equal(src // R, torch.arange(B, device="cuda").repeat_interleave(keep))
@@ -425,7 +375,7 @@ def test_refused_calls_enqueue_nothing(precision):
         for bad_m, bad_nnz in ((0, -1), (785, -1), (m, -2), (m, m * 784 + 1)):
             assert int(lib.dgan_workspace_bytes_measured_pruned(gen._handle, B, R, bad_m, bad_nnz, good, 1)) == 0
         ws_t = torch.empty(need + 1024, dtype=torch.uint8, device="cuda")
-        ws = ctypes.c_void_p((ws_t.data_ptr() + 1023) // 1024 * 1024)
+        ws = ctypes.c_void_p(ws_base(ws_t))
         prm = _native.dgan_rec_params(B, R, L, lr, 0.7, 0, 1, 0)
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         p = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731

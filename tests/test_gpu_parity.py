@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_support import ws_base
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -179,7 +180,7 @@ def test_error_paths_through_c_abi(gens):
     x = torch.zeros(2, 28, 28, 1, device="cuda")
     rec = torch.empty_like(x)
     small = torch.empty(4096, dtype=torch.uint8, device="cuda")
-    base = (small.data_ptr() + 1023) // 1024 * 1024
+    base = ws_base(small)
     prm = _native.dgan_rec_params(2, 2, 3, 10.0, 0.7, 0, 0, 0)
     rc = lib.dgan_reconstruct(gen._handle, ctypes.byref(prm), x.data_ptr(), None, rec.data_ptr(), None, None,
                               ctypes.c_void_p(base), 1024, None)

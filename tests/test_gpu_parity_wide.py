@@ -28,7 +28,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MSE_BAR = 1e-4     # BASELINE.json: "reconstruction MSE within 1e-4 of the reference"
 
 
-def _gen(arch, weights, precision):
+def _native_gen(arch, weights, precision):
     from defensegan_b200 import _native
     dev = torch.device("cuda", 0)
     return _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in weights.values()], precision=precision,
@@ -42,7 +42,7 @@ def gens():
     def get(arch, precision):
         if (arch, precision) not in cache:
             w = O.init_generator_weights(arch)
-            cache[(arch, precision)] = (w, _gen(arch, w, precision))
+            cache[(arch, precision)] = (w, _native_gen(arch, w, precision))
         return cache[(arch, precision)]
 
     yield get
@@ -240,7 +240,7 @@ def test_large_saturating_weights_stay_finite(gens):
     z0 = O.sample_z0(B * R, 128, seed=4)
     want = O.reconstruct(arch, big, imgs, R, L, rec_lr=1.0, z_init_val=z0)
     for precision, tol in (("fp32", 2e-4), ("fp16", 5e-3)):
-        gen = _gen(arch, big, precision)
+        gen = _native_gen(arch, big, precision)
         rec, loss, idx = gen.reconstruct(torch.tensor(imgs).cuda(), R, L, 1.0, z_init_val=torch.tensor(z0).cuda(), return_aux=True)
         assert torch.isfinite(rec).all() and torch.isfinite(loss).all()
         d = np.abs(loss.cpu().numpy() - want["loss_min"])

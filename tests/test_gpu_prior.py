@@ -20,8 +20,10 @@ import torch
 import layer_ref as LR
 import measured_oracle as MO
 import prior_oracle as P
+from gpu_support import bits as _bits, gen as _gen, images as _images, same as _same, z0 as _z0
+from gpu_support import rec as _rec, rec_m as _rec_m, release_cached_memory  # noqa: F401
+from gpu_support import gsum as _gsum, option_layout as _layout, option_lr as _lr, read as _read
 from oracle import defensegan_oracle as O
-from test_gpu_adam import _gsum, _layout, _read
 
 pytestmark = pytest.mark.gpu
 
@@ -29,52 +31,6 @@ HWC = {"mnist": 784, "celeba": 12288}
 SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 ADAM = (0.9, 0.999, 1e-8)
 CASES = [(p, a) for p in ("fp32", "fp16") for a in ("mnist", "celeba")]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back what this module left cached."""
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
-
-
-def _gen(arch, precision, use_bn=False, latent=128):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent, use_bn=use_bn,
-                                precision=precision, device=dev)
-    return w, g
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return all(torch.equal(_bits(p), _bits(q)) for p, q in zip(a, b))
-
-
-def _images(arch, w, B, seed=2):
-    return torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=seed)).cuda()
-
-
-def _z0(n, latent=128, seed=3):
-    return torch.tensor(O.sample_z0(n, latent, seed=seed)).cuda()
-
-
-def _rec(gen, x, R, L, lr, z0, **kw):
-    return [t.clone() for t in gen.reconstruct(x, R, L, lr, z_init_val=z0, return_aux=True, **kw)]
-
-
-def _rec_m(gen, y, a, R, L, lr, z0, **kw):
-    return [t.clone() for t in gen.reconstruct_measured(y, a, R, L, lr, z_init_val=z0, return_aux=True, **kw)]
-
-
-def _lr(kw):
-    return 0.02 if "adam" in kw else 0.5
 
 
 # ---- lambda = 0: the counterpart's bits ----

@@ -16,6 +16,7 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_support import bits as _bits, gen as _gen, layout, read as _read, same as _same, ws_base
 from oracle import defensegan_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -25,28 +26,11 @@ ONE = [(5, 2)]
 THREE = [(3, 3), (6, 2), (9, 1)]
 
 
-def _gen(arch, precision, use_bn=False):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], use_bn=use_bn, precision=precision,
-                                device=dev)
-    return w, g
-
-
 def _problem(arch, w, B, R, seed=2):
     x = torch.tensor(O.synthetic_images(arch, w, B, kind="S2", seed=seed)).cuda()
     z0 = torch.tensor(O.sample_z0(B * R, 128, seed=seed + 1)).cuda()
     pw = torch.tensor(np.random.RandomState(seed).uniform(0, 1, size=tuple(x.shape)).astype(np.float32)).cuda()
     return x, z0, pw
-
-
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return all(torch.equal(_bits(p), _bits(q)) for p, q in zip(a, b))
 
 
 def _call(gen, x, R, L, z0, pw, prune, lr=10.0, decay=False, **kw):
@@ -167,34 +151,8 @@ def test_batch_split_and_seeded_z0(precision, weighted):
 
 
 def _regions(gen, batch, R, sched, weighted):
-    """{k: (byte offset of region k in the aligned workspace, {name: (type, offset, dims)}, n_rows, n_pad)}."""
-    from defensegan_b200 import _native
-    fn = gen.lib.dgan_debug_workspace_layout_pruned
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_native.dgan_prune_point), ctypes.c_int,
-                   ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    arr = (_native.dgan_prune_point * len(sched))(*[_native.dgan_prune_point(a, b) for a, b in sched])
-    buf = ctypes.create_string_buffer(1 << 18)
-    assert fn(gen._handle, batch, R, arr, len(sched), int(weighted), buf, len(buf)) > 0
-    regs, cur = {}, None
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if f[0] == "region":
-            cur = regs[int(f[1])] = {"off": int(f[2]), "n_rows": int(f[3]), "bufs": {}}
-        elif f[0] == "n_pad":
-            cur["n_pad"] = int(f[1])
-        elif len(f) >= 4 and f[1] in ("f32", "f16", "u64", "u32", "i32"):
-            cur["bufs"][f[0]] = (f[1], int(f[2]), [int(v) for v in f[3:]])
-    return regs
-
-
-def _read(gen, reg, name):
-    typ, off, dims = reg["bufs"][name]
-    dt = {"f32": torch.float32, "f16": torch.float16, "i32": torch.int32, "u32": torch.int32}[typ]
-    base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr() + reg["off"] + off
-    n = int(np.prod(dims))
-    torch.cuda.synchronize()
-    return gen._ws[base:base + n * dt.itemsize].view(dt).view(*dims).clone()
+    """{k: {off, n_rows, n_pad, bufs}} of region k of a pruned workspace."""
+    return layout(gen, "_pruned", batch, R, list(sched), len(sched), int(weighted))[0]
 
 
 @pytest.mark.parametrize("precision,arch,weighted", CASES)
@@ -285,7 +243,7 @@ def test_refused_calls_enqueue_nothing(precision):
         assert int(lib.dgan_workspace_bytes_pruned(bn._handle, B, R, good, 1, 0)) == 0
         assert int(lib.dgan_workspace_bytes_pruned(gen._handle, B, R, sched_of([(4, 5)]), 1, 0)) == 0
         ws_t = torch.empty(need + 1024, dtype=torch.uint8, device="cuda")
-        ws = ctypes.c_void_p((ws_t.data_ptr() + 1023) // 1024 * 1024)
+        ws = ctypes.c_void_p(ws_base(ws_t))
         prm = _native.dgan_rec_params(B, R, L, 10.0, 0.7, 0, 1, 0)
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         p = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731

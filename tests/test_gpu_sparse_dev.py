@@ -19,9 +19,9 @@ import torch
 
 import measured_oracle as MO
 import sparse_dev_oracle as S
+from gpu_support import gen as _gen, images as _images, option_lr as _lr, read as _read, same as _same, z0 as _z0
+from gpu_support import layout, rec as _rec, rec_m as _rec_m, release_cached_memory  # noqa: F401
 from oracle import defensegan_oracle as O
-from test_gpu_adam import _layout, _read  # noqa: F401
-from test_gpu_prior import _gen, _images, _lr, _rec, _rec_m, _same, _z0
 
 pytestmark = pytest.mark.gpu
 
@@ -29,14 +29,6 @@ HWC = {"mnist": 784, "celeba": 12288}
 SHAPE = {"mnist": (28, 28, 1), "celeba": (64, 64, 3)}
 ADAM = (0.9, 0.999, 1e-8)
 CASES = [(p, a) for p in ("fp32", "fp16") for a in ("mnist", "celeba")]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    yield
-    import gc
-    gc.collect()
-    torch.cuda.empty_cache()
 
 
 def _identity_csr(n):
@@ -53,21 +45,8 @@ def _zero_bits(t):
 
 
 def _sdev_layout(gen, B, R, weighted=0, m=0, nnz=-1, adam=0):
-    """{name: (type, offset, dims)} of an unpruned sparse-deviation workspace (dgan_debug_workspace_layout_sparse_dev)."""
-    from defensegan_b200 import _native
-    fn = gen.lib.dgan_debug_workspace_layout_sparse_dev
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p] + [ctypes.c_int] * 5 + [ctypes.c_void_p, ctypes.c_int,
-                                                            ctypes.POINTER(_native.dgan_prune_point), ctypes.c_int,
-                                                            ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 18)
-    assert fn(gen._handle, B, R, weighted, m, nnz, None, adam, None, 0, buf, len(buf)) > 0
-    bufs = {}
-    for line in buf.value.decode().splitlines():
-        f = line.split()
-        if len(f) >= 4 and f[1] in ("f32", "f16", "u64", "u32", "i32"):
-            bufs[f[0]] = (f[1], int(f[2]), [int(v) for v in f[3:]])
-    return bufs
+    """Region 0 of an unpruned sparse-deviation workspace (dgan_debug_workspace_layout_sparse_dev)."""
+    return layout(gen, "_sparse_dev", B, R, weighted, m, nnz, None, adam, [], 0)[0][0]
 
 
 # ---- 1. step = 0: the counterparts' bits ----

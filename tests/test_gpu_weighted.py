@@ -15,36 +15,14 @@ import torch
 import layer_ref as R
 import weighted_layer_ref as WR
 import weighted_oracle as WO
+from gpu_support import gen as _gen, layout, read_call, release_cached_memory, view  # noqa: F401
 from oracle import defensegan_oracle as O
-from test_gpu_layers import read_call
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module", autouse=True)
-def _release_cached_memory():
-    """The library allocates with cudaMalloc, outside torch's caching allocator: hand back the blocks this module's fp64
-    references left cached, so that the handles of later tests find the memory."""
-    yield
-    import gc
-    gc.collect()
-    before = torch.cuda.mem_get_info()[0]
-    torch.cuda.empty_cache()
-    print("\nfree GPU memory: %.1f GB with this module's cache, %.1f GB after releasing it"
-          % (before / 2 ** 30, torch.cuda.mem_get_info()[0] / 2 ** 30))
-
-
 TOL = {"fp32": dict(fwd=2e-5, grad_rel=2e-4, grad_cos=0.999999, loss=1e-6),
        "fp16": dict(fwd=5e-3, grad_rel=6e-2, grad_cos=0.998, loss=1e-4)}
-
-
-def _gen(arch, precision, use_bn=False, latent=128, net_dim=64):
-    from defensegan_b200 import _native
-    dev = torch.device("cuda", 0)
-    w = O.init_generator_weights(arch, latent_dim=latent, net_dim=net_dim, use_bn=use_bn, random_bias=True)
-    g = _native.NativeGenerator(arch, [torch.as_tensor(v).to(dev) for v in w.values()], latent_dim=latent, net_dim=net_dim,
-                                use_bn=use_bn, precision=precision, device=dev)
-    return w, g
 
 
 def _weights(shape, kind, seed=0):
@@ -185,16 +163,6 @@ def test_weighted_loss_grad_each_layer_direction(arch, latent, net_dim, use_bn, 
         gen.close()
 
 
-def _layout(gen, n_rows, weighted):
-    import ctypes
-    fn = gen.lib.dgan_debug_workspace_layout_weighted if weighted else gen.lib.dgan_debug_workspace_layout
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_char_p, ctypes.c_int]
-    buf = ctypes.create_string_buffer(1 << 16)
-    assert fn(gen._handle, n_rows, buf, len(buf)) > 0
-    return buf.value.decode().splitlines()
-
-
 @pytest.mark.parametrize("precision", ["fp16", "fp32"])
 def test_steady_state_and_alternating_calls(precision):
     """A second weighted call at a planned size allocates nothing, replays its captured loop and issues one stream
@@ -234,11 +202,11 @@ def test_steady_state_and_alternating_calls(precision):
         assert torch.cuda.mem_get_info()[0] == free0
         assert plain + 1 <= 11         # the loop is one graph launch, not L-step launches
         # the weighted layout: the unweighted buffers at their offsets, then the copy of the weights the loop read
-        plain_ws, weighted_ws = _layout(gen, B * R_, False), _layout(gen, B * R_, True)
+        plain_ws = layout(gen, "", B * R_)[1].splitlines()
+        regions, weighted_ws = layout(gen, "_weighted", B * R_)
+        weighted_ws = weighted_ws.splitlines()
         assert weighted_ws[:len(plain_ws)] == plain_ws and weighted_ws[len(plain_ws)].split()[0] == "xw"
-        name, _, off, rows, hwc = weighted_ws[-1].split()
-        base = (gen._ws.data_ptr() + 1023) // 1024 * 1024 - gen._ws.data_ptr() + int(off)
-        xw = gen._ws[base:base + int(rows) * int(hwc) * 4].view(torch.float32).view(int(rows), int(hwc))
+        xw = view(gen, regions[0], weighted_ws[-1].split()[0])
         assert torch.equal(xw[:B], pw.reshape(B, -1))
     finally:
         gen.close()

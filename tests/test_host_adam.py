@@ -1,72 +1,18 @@
 """CPU tests (no GPU) of the Adam update of the latent rows (dgan_reconstruct_adam, dgan_reconstruct_measured_adam,
-dgan_reconstruct_measured_csr_adam): the exported symbols against the header, dgan_adam_params against the C compiler,
-the refusal of bad Adam parameters by the C entries and by Python before any native call, the binding's routing (and a
-momentum call's kwargs unchanged), DefenseGANBase's rec_optimizer attributes, the cache name and its parse-back, and
-what ptxas made of the new kernels.  The Adam workspace's layout needs a handle, so tests/test_gpu_adam.py reads it."""
-import contextlib
+dgan_reconstruct_measured_csr_adam): the refusal of bad Adam parameters by the C entries and by Python before any native
+call, the binding's routing (and a momentum call's kwargs unchanged), DefenseGANBase's rec_optimizer attributes, and the
+cache name and its parse-back.  The Adam workspace's layout needs a handle, so tests/test_gpu_adam.py reads it."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_adam", "dgan_workspace_bytes_measured_adam", "dgan_reconstruct_adam",
-               "dgan_reconstruct_measured_adam", "dgan_reconstruct_measured_csr_adam"]
+from recording import Out, cpu_native, recording_gan  # noqa: F401  (the fixture)
+
 BAD = [((1.0, 0.999, 1e-8), "beta1"), ((-0.5, 0.999, 1e-8), "beta1"), ((float("nan"), 0.999, 1e-8), "beta1"),
        ((0.9, 1.0, 1e-8), "beta2"), ((0.9, -1e-3, 1e-8), "beta2"), ((0.9, 0.999, 0.0), "eps"),
        ((0.9, 0.999, -1e-8), "eps"), ((0.9, 0.999, float("inf")), "eps"), ((0.9, 0.999, float("nan")), "eps")]
-
-
-def test_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "dgan_rec_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params))
-            elif "dgan_prune_point" in p:
-                want.append(ctypes.POINTER(_native.dgan_prune_point))
-            elif "dgan_adam_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_adam_params))
-            elif "*" in p or p.startswith("dgan_handle"):
-                want.append(ctypes.c_void_p)
-            else:
-                want.append(ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-    assert lib.dgan_abi_version() == 2
-
-
-def test_adam_params_struct_matches_the_compilers_layout_and_the_header_is_c99(tmp_path):
-    from defensegan_b200 import _native
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "defensegan_b200.h"\n'
-                   'int (*f)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const dgan_prune_point*, int, '
-                   'const int32_t*, const int32_t*, const float*, int, int, const float*, const float*, float*, float*, '
-                   'int32_t*, void*, size_t, void*) = dgan_reconstruct_measured_csr_adam;\n'
-                   'int main(void) { printf("%zu %zu %zu %zu\\n", sizeof(dgan_adam_params), '
-                   'offsetof(dgan_adam_params, beta1), offsetof(dgan_adam_params, beta2), offsetof(dgan_adam_params, eps));'
-                   ' return 0; }\n')
-    exe = tmp_path / "layout"
-    subprocess.run([cc, "-std=c99", "-pedantic", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe),
-                    "-L", os.path.dirname(_native.LIB_PATH), "-Wl,--unresolved-symbols=ignore-all"], check=True)
-    got = tuple(int(v) for v in subprocess.run([str(exe)], stdout=subprocess.PIPE, text=True, check=True).stdout.split())
-    A = _native.dgan_adam_params
-    assert got == (ctypes.sizeof(A), A.beta1.offset, A.beta2.offset, A.eps.offset)
 
 
 # ---- refusals ----
@@ -131,51 +77,6 @@ def test_check_adam_params_accepts_the_edges_as_fp32():
 
 # ---- the binding's routing ----
 
-@pytest.fixture
-def cpu_native(monkeypatch):
-    """A NativeGenerator whose library records its calls (no GPU)."""
-    from defensegan_b200 import _native
-    calls = []
-
-    class FakeLib:
-        def __getattr__(self, name):
-            def f(*args):
-                calls.append((name, args))
-                return 1 << 20 if name.startswith("dgan_workspace_bytes") else 0
-            return f
-
-    class Stream:
-        cuda_stream = 0
-
-    monkeypatch.setattr(_native, "_require_cuda_f32", lambda t, name: t.to(torch.float32).contiguous())
-    monkeypatch.setattr(_native, "_require_cuda_i32", lambda t, name: t.to(torch.int32).contiguous())
-    monkeypatch.setattr(_native, "_require_aligned_out", lambda rec: None)
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda d=None: Stream())
-    g = object.__new__(_native.NativeGenerator)
-    g.lib, g.device, g._ws, g._handle = FakeLib(), torch.device("cpu"), None, ctypes.c_void_p(0)
-    g.image_dim, g.hwc, g.latent_dim, g.use_bn = (28, 28, 1), 784, 8, False
-    g.calls = calls
-    return g
-
-
-class Out:
-    """Stands in for a CUDA `out` tensor of n elements."""
-    is_cuda, dtype = True, torch.float32
-
-    def __init__(self, n):
-        self.n = n
-
-    def is_contiguous(self):
-        return True
-
-    def numel(self):
-        return self.n
-
-    def data_ptr(self):
-        return 0
-
-
 def _adam_of(byref):
     p = byref._obj
     return tuple(round(float(getattr(p, f)), 6) for f in ("beta1", "beta2", "eps"))
@@ -236,26 +137,6 @@ def test_binding_refuses_bad_adam_before_any_native_call(cpu_native):
 
 # ---- DefenseGANBase ----
 
-def _recording_gan(**kw):
-    from defensegan_b200.models.gan import MnistDefenseGAN
-    gan = MnistDefenseGAN(test_mode=True, verbose=False, **kw)
-    seen = []
-
-    class FakeNative:
-        def reconstruct(self, x, *args, **kw):
-            seen.append(("reconstruct", kw))
-            return x
-
-        def reconstruct_measured(self, y, a, *args, **kw):
-            seen.append(("reconstruct_measured", kw))
-            return y
-
-    gan._as_cuda = lambda t: t.to(torch.float32)
-    gan._get_native = lambda device: FakeNative()
-    gan.rec_rr, gan.rec_iters = 4, 50
-    return gan, seen
-
-
 def test_defaults_and_cfg_keys():
     from defensegan_b200.models.gan import MnistDefenseGAN
     gan = MnistDefenseGAN(test_mode=True, verbose=False)
@@ -268,7 +149,7 @@ def test_defaults_and_cfg_keys():
 
 
 def test_momentum_calls_keep_their_kwargs_and_adam_calls_add_adam():
-    gan, seen = _recording_gan()
+    gan, seen = recording_gan()
     a = torch.zeros(10, 784)
     a[torch.arange(10), torch.arange(10)] = 1.0
     gan.reconstruct(torch.rand(2, 28, 28, 1))
@@ -340,32 +221,3 @@ def test_rec_cache_dir_names_adam_and_parses_back(tmp_path):
     E.set_test_time_rec_params(other, E.Flags(defense_type="defense_gan", rec_path=both, override=False,
                                               online_training=False, train_on_recs=False))
     assert other.rec_cache_dir("dev", max_num=100) == both
-
-
-# ---- what ptxas made of the new kernels ----
-
-def test_adam_kernels_compile_for_sm90a_without_spills(tmp_path):
-    from defensegan_b200 import _native
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    src = tmp_path / "adam.cu"
-    src.write_text('#include "%s"\n' % os.path.join(_native.CSRC_DIR, "kernels_adam.cuh"))
-    flags = [f for f in _native.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC")]
-    res = subprocess.run([nvcc] + flags + ["-cubin", "-Xptxas", "-v", str(src), "-o", str(tmp_path / "adam.cubin")],
-                         stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout[-4000:]
-    names = ("adam_kernel", "prune_gather_adam_kernel")
-    spills, fn = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn is not None:
-            spills[fn] = tuple(int(v) for v in m.groups())
-            fn = None
-    assert sorted(n for n in names if any(re.search(r"\d%s" % n, k) for k in spills)) == sorted(names), sorted(spills)
-    bad = {k: v for k, v in spills.items() if v != (0, 0, 0)}
-    assert not bad, bad

@@ -1,68 +1,19 @@
 """CPU tests (no GPU) of the Huber data term (dgan_reconstruct_huber, dgan_reconstruct_measured[_csr]_huber,
-dgan_loss_grad[_measured[_csr]]_huber): the exported symbols against the header, the header as C99, the refusal of a bad
-delta by the C entries and by Python before any native call, the binding's routing (a squared-error call's entry and
-kwargs unchanged), DefenseGANBase's rec_huber_delta, the cache name and its parse-back, the Huber oracle against the
-existing oracles and finite differences, and what ptxas made of the new instantiations."""
+dgan_loss_grad[_measured[_csr]]_huber): the refusal of a bad delta by the C entries and by Python before any native
+call, the binding's routing (a squared-error call's entry and kwargs unchanged), DefenseGANBase's rec_huber_delta, the
+cache name and its parse-back, and the Huber oracle against the existing oracles and finite differences."""
 import ctypes
 import math
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from test_host_adam import Out, cpu_native  # noqa: F401  (the recording NativeGenerator fixture)
+from recording import Out, cpu_native, recording_gan  # noqa: F401  (the fixture)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_reconstruct_huber", "dgan_reconstruct_measured_huber", "dgan_reconstruct_measured_csr_huber",
-               "dgan_loss_grad_huber", "dgan_loss_grad_measured_huber", "dgan_loss_grad_measured_csr_huber"]
+
 BAD = [0.0, -0.0, -1.0, float("nan"), -float("inf"), 1e-50]       # 1e-50 is 0 in fp32
-
-
-def test_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t, "float": ctypes.c_float}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "dgan_rec_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params))
-            elif "dgan_prune_point" in p:
-                want.append(ctypes.POINTER(_native.dgan_prune_point))
-            elif "dgan_adam_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_adam_params))
-            elif "*" in p or p.startswith("dgan_handle"):
-                want.append(ctypes.c_void_p)
-            else:
-                want.append(ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-    assert lib.dgan_abi_version() == 2
-
-
-def test_header_is_c99_with_the_new_entries(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "huber.c"
-    src.write_text('#include "defensegan_b200.h"\n'
-                   'int (*f)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, float, const dgan_prune_point*, '
-                   'int, const float*, const float*, const float*, float*, float*, int32_t*, void*, size_t, void*) = '
-                   'dgan_reconstruct_huber;\n'
-                   'int (*g)(dgan_handle, float, const int32_t*, const int32_t*, const float*, int, int, const float*, int, '
-                   'int, const float*, float*, float*, float*, void*, size_t, void*) = dgan_loss_grad_measured_csr_huber;\n'
-                   'int main(void) { return f == 0 || g == 0; }\n')
-    subprocess.run([cc, "-std=c99", "-pedantic", "-Werror", "-c", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                    str(tmp_path / "huber.o")], check=True)
 
 
 # ---- refusals ----
@@ -193,26 +144,6 @@ def test_binding_refuses_a_bad_delta_before_any_native_call(cpu_native):  # noqa
 
 # ---- DefenseGANBase ----
 
-def _recording_gan(**kw):
-    from defensegan_b200.models.gan import MnistDefenseGAN
-    gan = MnistDefenseGAN(test_mode=True, verbose=False, **kw)
-    seen = []
-
-    class FakeNative:
-        def reconstruct(self, x, *args, **kw):
-            seen.append(("reconstruct", kw))
-            return x
-
-        def reconstruct_measured(self, y, a, *args, **kw):
-            seen.append(("reconstruct_measured", kw))
-            return y
-
-    gan._as_cuda = lambda t: t.to(torch.float32)
-    gan._get_native = lambda device: FakeNative()
-    gan.rec_rr, gan.rec_iters = 4, 50
-    return gan, seen
-
-
 def test_defaults_and_cfg_key():
     from defensegan_b200.models.gan import MnistDefenseGAN
     from defensegan_b200.utils.config import load_config, packaged_cfg_path
@@ -223,7 +154,7 @@ def test_defaults_and_cfg_key():
 
 
 def test_squared_error_calls_keep_their_kwargs_and_huber_calls_add_the_delta():
-    gan, seen = _recording_gan()
+    gan, seen = recording_gan()
     a = torch.zeros(10, 784)
     a[torch.arange(10), torch.arange(10)] = 1.0
     gan.reconstruct(torch.rand(2, 28, 28, 1))
@@ -384,39 +315,3 @@ def test_oracle_gradient_matches_finite_differences(case):
         fd = (lp - lm) / (2 * h)
         assert fd == pytest.approx(float((g * v).sum()), rel=1e-5, abs=1e-9)
     assert math.isfinite(float(loss.sum()))
-
-
-# ---- what ptxas made of the new instantiations ----
-
-def test_huber_instantiations_compile_for_sm90a_without_spills(tmp_path):
-    """Every new kernel is spill-free, except the fp32 CelebA weighted last-layer forward, whose squared-error
-    counterpart already spills: its Huber instantiation may spill no more than that one."""
-    from defensegan_b200 import _native
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    flags = [f for f in _native.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC")]
-    res = subprocess.run([nvcc] + flags + ["-cubin", "-Xptxas", "-v", os.path.join(_native.CSRC_DIR, "dgan_api.cu"), "-o",
-                          str(tmp_path / "dgan_api.cubin")], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout[-4000:]
-    spills, fn = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn is not None:
-            spills[fn] = (int(m.group(1)), int(m.group(2)))
-            fn = None
-    tc = {k: v for k, v in spills.items() if re.search(r"tc_bsgemm2_kernelILi\d+ELi\d+ELi\d+ELi1[2-5]E", k)}
-    meas = {k: v for k, v in spills.items() if re.search(r"measured_(gemm|csr)_huber_kernel", k)}
-    fp32 = {k: v for k, v in spills.items() if "final_fwd_huber_kernel" in k}
-    assert len(tc) == 6 and len(meas) == 3 and len(fp32) == 4, (sorted(tc), sorted(meas), sorted(fp32))
-    assert all(v == (0, 0) for v in list(tc.values()) + list(meas.values())), (tc, meas)
-    for k, v in fp32.items():
-        if "IfLi3ELi1ELb1E" in k:                     # CelebA, tanh, weighted
-            twin = [s for n, s in spills.items() if "final_fwd_loss_kernelIfLi3ELi1ELb1E" in n]
-            assert len(twin) == 1 and v[0] <= twin[0][0] and v[1] <= twin[0][1], (v, twin)
-        else:
-            assert v == (0, 0), (k, v)

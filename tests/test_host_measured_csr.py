@@ -1,12 +1,7 @@
-"""CPU tests (no GPU) of the projection from sparse linear measurements: the exported CSR symbols, the binding's and
-DefenseGANBase's handling of sparse operators, the checks that refuse a malformed CSR before any native call, the test
-operators, and what ptxas made of the new kernels."""
-import contextlib
+"""CPU tests (no GPU) of the projection from sparse linear measurements: the binding's and DefenseGANBase's handling of
+sparse operators, the checks that refuse a malformed CSR before any native call, and the test operators."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,28 +11,7 @@ import measured_oracle as MO
 import sparse_operators as SO
 from oracle import defensegan_oracle as O
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_measured_csr", "dgan_reconstruct_measured_csr", "dgan_loss_grad_measured_csr"]
-
-
-def test_csr_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "*" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params) if "dgan_rec_params" in p else ctypes.c_void_p)
-            else:
-                want.append(ctypes.c_void_p if p.startswith("dgan_handle") else ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
+from recording import Out, cpu_native  # noqa: F401  (the fixture)
 
 
 def test_workspace_bytes_measured_csr_refuses_bad_m_and_nnz_without_a_handle():
@@ -60,66 +34,6 @@ def test_the_debug_layout_names_the_staged_csr():
 
 
 # ---- the binding ----
-
-class FakeLib:
-    """Stands in for the CUDA library under NativeGenerator: logs every entry point it is called through."""
-
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        def fn(*args):
-            self.calls.append((name, args))
-            return 4096 if name.startswith("dgan_workspace_bytes") else 0
-        return fn
-
-
-@pytest.fixture
-def cpu_native(monkeypatch):
-    """A NativeGenerator (MNIST) on the CPU whose library is a FakeLib; the converted index and value tensors it passes
-    are kept in `seen`."""
-    from defensegan_b200 import _native
-
-    class Stream:
-        cuda_stream = 0
-
-    class Out:
-        is_cuda, dtype = True, torch.float32
-
-        def __init__(self, n):
-            self.n = n
-
-        def is_contiguous(self):
-            return True
-
-        def numel(self):
-            return self.n
-
-        def data_ptr(self):
-            return 0
-
-    seen = {}
-
-    def f32(t, name):
-        t = t.to(torch.float32).contiguous()
-        seen[name] = t
-        return t
-
-    def i32(t, name):
-        t = t.to(torch.int32).contiguous()
-        seen[name] = t
-        return t
-
-    monkeypatch.setattr(_native, "_require_cuda_f32", f32)
-    monkeypatch.setattr(_native, "_require_cuda_i32", i32)
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda d=None: Stream())
-    g = object.__new__(_native.NativeGenerator)
-    g.lib, g.device, g._ws, g._handle = FakeLib(), torch.device("cpu"), None, ctypes.c_void_p(0)
-    g.image_dim, g.hwc, g.latent_dim = (28, 28, 1), 784, 8
-    g.Out, g.seen = Out, seen
-    return g
-
 
 def _csr(m=50, seed=0):
     a = torch.tensor(SO.random_sparse_operator(m, 784, density=0.02, seed=seed))
@@ -305,33 +219,3 @@ def test_oracle_is_the_same_for_an_operator_and_its_csr_densified():
     y = (x.reshape(2, -1) @ a.T).astype(np.float32)
     for p, q in zip(MO.loss_and_grad("mnist", w, a, y, z, 2), MO.loss_and_grad("mnist", w, back, y, z, 2)):
         assert np.array_equal(p, q)
-
-
-# ---- what ptxas made of the new kernels ----
-
-def test_csr_kernels_compile_for_sm90a_without_spills(tmp_path):
-    from defensegan_b200 import _native
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    flags = [f for f in _native.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC")]
-    cmd = [nvcc] + flags + ["-cubin", "-Xptxas", "-v", os.path.join(_native.CSRC_DIR, "dgan_api.cu"),
-                            "-o", str(tmp_path / "dgan_api.cubin")]
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout[-4000:]
-    names = ("measured_csr_kernel", "csr_validate_kernel", "csr_stage_rows_kernel", "csr_stage_entries_kernel",
-             "csr_scan_kernel", "csr_fill_transpose_kernel")
-    spills, fn = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn is not None and any(n in fn for n in names):
-            spills[fn] = tuple(int(v) for v in m.groups())
-            fn = None
-    assert sum("measured_csr_kernel" in k for k in spills) == 2, sorted(spills)
-    assert all(sum(n in k for k in spills) >= 1 for n in names), sorted(spills)
-    bad = {k: v for k, v in spills.items() if v != (0, 0, 0)}
-    assert not bad, bad

@@ -1,64 +1,15 @@
 """CPU tests (no GPU) of restart pruning in the projection from linear measurements (dgan_reconstruct_measured_pruned,
-dgan_reconstruct_measured_csr_pruned): the exported symbols against the header, the header as C99, the binding's routing
-of dense, COO and CSR operators with and without a schedule, the three `prune` cases of
-DefenseGANBase.reconstruct_measured with their refusals raised before any native call.  The layout of a pruned measured
-workspace needs a handle, so tests/test_gpu_measured_prune.py reads it; here the printer's refusal without one."""
-import contextlib
+dgan_reconstruct_measured_csr_pruned): the binding's routing of dense, COO and CSR operators with and without a
+schedule, the three `prune` cases of DefenseGANBase.reconstruct_measured with their refusals raised before any native
+call.  The layout of a pruned measured workspace needs a handle, so tests/test_gpu_measured_prune.py reads it; here the
+printer's refusal without one."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_measured_pruned", "dgan_reconstruct_measured_pruned",
-               "dgan_reconstruct_measured_csr_pruned"]
-
-
-def test_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "dgan_rec_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params))
-            elif "dgan_prune_point" in p:
-                want.append(ctypes.POINTER(_native.dgan_prune_point))
-            elif "*" in p or p.startswith("dgan_handle"):
-                want.append(ctypes.c_void_p)
-            else:
-                want.append(ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-    assert lib.dgan_abi_version() == 2
-
-
-def test_header_compiles_as_c99(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "use.c"
-    src.write_text('#include "defensegan_b200.h"\n'
-                   'size_t (*a)(dgan_handle, int, int, int, int, const dgan_prune_point*, int) = '
-                   'dgan_workspace_bytes_measured_pruned;\n'
-                   'int (*b)(dgan_handle, const dgan_rec_params*, const dgan_prune_point*, int, const float*, int, '
-                   'const float*, const float*, float*, float*, int32_t*, void*, size_t, void*) = '
-                   'dgan_reconstruct_measured_pruned;\n'
-                   'int (*c)(dgan_handle, const dgan_rec_params*, const dgan_prune_point*, int, const int32_t*, '
-                   'const int32_t*, const float*, int, int, const float*, const float*, float*, float*, int32_t*, void*, '
-                   'size_t, void*) = dgan_reconstruct_measured_csr_pruned;\n')
-    subprocess.run([cc, "-std=c99", "-pedantic", "-Werror", "-c", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                    str(tmp_path / "use.o")], check=True)
+from recording import Out, cpu_native  # noqa: F401  (the fixture)
 
 
 def _layout_fn(lib):
@@ -82,55 +33,10 @@ def test_sizer_and_layout_refuse_bad_arguments_without_a_handle():
 
 # ---- the binding's routing ----
 
-@pytest.fixture
-def cpu_native(monkeypatch):
-    """A NativeGenerator whose library records its calls (no GPU)."""
-    from defensegan_b200 import _native
-    calls = []
-
-    class FakeLib:
-        def __getattr__(self, name):
-            def f(*args):
-                calls.append((name, args))
-                return 1 << 20 if name.startswith("dgan_workspace_bytes") else 0
-            return f
-
-    class Stream:
-        cuda_stream = 0
-
-    monkeypatch.setattr(_native, "_require_cuda_f32", lambda t, name: t.to(torch.float32).contiguous())
-    monkeypatch.setattr(_native, "_require_cuda_i32", lambda t, name: t.to(torch.int32).contiguous())
-    monkeypatch.setattr(_native, "_require_aligned_out", lambda rec: None)
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda d=None: Stream())
-    g = object.__new__(_native.NativeGenerator)
-    g.lib, g.device, g._ws, g._handle = FakeLib(), torch.device("cpu"), None, ctypes.c_void_p(0)
-    g.image_dim, g.hwc, g.latent_dim, g.use_bn = (28, 28, 1), 784, 8, False
-    g.calls = calls
-    return g
-
-
 def _operators():
     a = torch.zeros(10, 784)
     a[torch.arange(10), torch.arange(10) * 7] = 1.0
     return a, a.to_sparse_csr()
-
-
-class Out:
-    """Stands in for a CUDA `out` tensor of n elements."""
-    is_cuda, dtype = True, torch.float32
-
-    def __init__(self, n):
-        self.n = n
-
-    def is_contiguous(self):
-        return True
-
-    def numel(self):
-        return self.n
-
-    def data_ptr(self):
-        return 0
 
 
 def test_binding_routes_dense_and_csr_with_a_schedule_to_the_pruned_entries(cpu_native):

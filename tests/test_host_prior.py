@@ -1,79 +1,19 @@
 """CPU tests (no GPU) of the latent prior (dgan_reconstruct_prior, dgan_reconstruct_measured[_csr / _conv]_prior): the
-exported symbols against the header, the header as C99, the refusal of a bad lambda by the C entries and by Python
-before any native call, the binding's routing (a call without the prior keeps its entry and kwargs), DefenseGANBase's
-rec_z_prior, the cache name and its parse-back, the prior oracle against finite differences and the existing oracles,
-and what ptxas made of the new kernels."""
+refusal of a bad lambda by the C entries and by Python before any native call, the binding's routing (a call without the
+prior keeps its entry and kwargs), DefenseGANBase's rec_z_prior, the cache name and its parse-back, and the prior oracle
+against finite differences and the existing oracles."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from test_host_adam import Out, cpu_native  # noqa: F401  (the recording NativeGenerator fixture)
+from recording import Out, cpu_native, recording_gan  # noqa: F401  (the fixture)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_reconstruct_prior", "dgan_reconstruct_measured_prior", "dgan_reconstruct_measured_csr_prior",
-               "dgan_reconstruct_measured_conv_prior"]
+
 INF = float("inf")
 BAD = [-1e-3, -INF, INF, float("nan"), 3e38, 1e39]        # 3e38: finite in fp32, 2 lambda is not; 1e39: inf in fp32
-
-
-def test_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t, "float": ctypes.c_float}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "dgan_rec_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params))
-            elif "dgan_prune_point" in p:
-                want.append(ctypes.POINTER(_native.dgan_prune_point))
-            elif "dgan_adam_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_adam_params))
-            elif "dgan_conv_op" in p:
-                want.append(ctypes.POINTER(_native.dgan_conv_op))
-            elif p.startswith("const float*") and "huber_delta" in p:
-                want.append(ctypes.POINTER(ctypes.c_float))
-            elif "*" in p or p.startswith("dgan_handle"):
-                want.append(ctypes.c_void_p)
-            else:
-                want.append(ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-    assert lib.dgan_abi_version() == 2
-
-
-def test_header_is_c99_with_the_new_entries(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "prior.c"
-    src.write_text('#include "defensegan_b200.h"\n'
-                   'int (*f)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, float, '
-                   'const dgan_prune_point*, int, const float*, const float*, const float*, float*, float*, int32_t*, void*, '
-                   'size_t, void*) = dgan_reconstruct_prior;\n'
-                   'int (*g)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, float, '
-                   'const dgan_prune_point*, int, const float*, int, const float*, const float*, float*, float*, int32_t*, '
-                   'void*, size_t, void*) = dgan_reconstruct_measured_prior;\n'
-                   'int (*h)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, float, '
-                   'const dgan_prune_point*, int, const int32_t*, const int32_t*, const float*, int, int, const float*, '
-                   'const float*, float*, float*, int32_t*, void*, size_t, void*) = dgan_reconstruct_measured_csr_prior;\n'
-                   'int (*k)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, float, '
-                   'const dgan_prune_point*, int, const dgan_conv_op*, const float*, const float*, const float*, float*, '
-                   'float*, int32_t*, void*, size_t, void*) = dgan_reconstruct_measured_conv_prior;\n'
-                   'int main(void) { return f == 0 || g == 0 || h == 0 || k == 0; }\n')
-    subprocess.run([cc, "-std=c99", "-pedantic", "-Werror", "-c", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                    str(tmp_path / "prior.o")], check=True)
 
 
 # ---- refusals ----
@@ -200,26 +140,6 @@ def test_binding_refuses_a_bad_lambda_before_any_native_call(cpu_native):  # noq
 
 # ---- DefenseGANBase ----
 
-def _recording_gan(**kw):
-    from defensegan_b200.models.gan import MnistDefenseGAN
-    gan = MnistDefenseGAN(test_mode=True, verbose=False, **kw)
-    seen = []
-
-    class FakeNative:
-        def reconstruct(self, x, *args, **kw):
-            seen.append(("reconstruct", kw))
-            return x
-
-        def reconstruct_measured(self, y, a, *args, **kw):
-            seen.append(("reconstruct_measured", kw))
-            return y
-
-    gan._as_cuda = lambda t: t.to(torch.float32)
-    gan._get_native = lambda device: FakeNative()
-    gan.rec_rr, gan.rec_iters = 4, 50
-    return gan, seen
-
-
 def test_defaults_and_cfg_key():
     from defensegan_b200.models.gan import MnistDefenseGAN
     from defensegan_b200.utils.config import load_config, packaged_cfg_path
@@ -231,7 +151,7 @@ def test_defaults_and_cfg_key():
 
 def test_calls_without_the_prior_keep_their_kwargs_and_prior_calls_add_lambda():
     from defensegan_b200.operators import ConvOperator
-    gan, seen = _recording_gan()
+    gan, seen = recording_gan()
     a = torch.zeros(10, 784)
     a[torch.arange(10), torch.arange(10)] = 1.0
     gan.reconstruct(torch.rand(2, 28, 28, 1))
@@ -360,32 +280,3 @@ def test_oracle_at_zero_reproduces_the_counterpart_oracles(adam):
     # a prior shrinks the chosen restarts' latents
     r2 = P.reconstruct("mnist", weights, 3, 6, lr, 0.5, images=x, z_init_val=z0, adam=adam)
     assert np.linalg.norm(r2["z_final"]) < np.linalg.norm(r1["z_final"])
-
-
-# ---- what ptxas made of the new kernels ----
-
-def test_prior_kernels_compile_for_sm90a_without_spills(tmp_path):
-    from defensegan_b200 import _native
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    flags = [f for f in _native.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC")]
-    cmd = [nvcc] + flags + ["-cubin", "-Xptxas", "-v", os.path.join(_native.CSRC_DIR, "dgan_api.cu"),
-                            "-o", str(tmp_path / "dgan_api.cubin")]
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout[-4000:]
-    names = ("momentum_prior_kernel", "momentum_rows_prior_kernel", "adam_prior_kernel", "prior_term_kernel",
-             "loss_finish_prior_kernel")
-    spills, fn = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn is not None and any(re.search(r"\d%s" % n, fn) for n in names):
-            spills[fn] = tuple(int(v) for v in m.groups())
-            fn = None
-    assert sorted(n for n in names if any(re.search(r"\d%s" % n, k) for k in spills)) == sorted(names), sorted(spills)
-    bad = {k: v for k, v in spills.items() if v != (0, 0, 0)}
-    assert not bad, bad

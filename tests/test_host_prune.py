@@ -1,61 +1,13 @@
-"""CPU tests (no GPU) of restart pruning (dgan_reconstruct_pruned): the exported symbols and the prune-point struct
-against the header and the C compiler, the schedule checks of the binding and of DefenseGANBase (raised before any native
-call), the use_bn and reconstruct_measured refusals, the cache-directory naming and its parse-back, and what ptxas made
-of the new kernels."""
-import contextlib
+"""CPU tests (no GPU) of restart pruning (dgan_reconstruct_pruned): the schedule checks of the binding and of
+DefenseGANBase (raised before any native call), the use_bn and reconstruct_measured refusals, and the cache-directory naming
+and its parse-back."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_pruned", "dgan_reconstruct_pruned"]
-
-
-def test_prune_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        want = []
-        for p in (" ".join(p.split()) for p in m.group(2).split(",")):
-            if "dgan_rec_params" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params))
-            elif "dgan_prune_point" in p:
-                want.append(ctypes.POINTER(_native.dgan_prune_point))
-            elif "*" in p or p.startswith("dgan_handle"):
-                want.append(ctypes.c_void_p)
-            else:
-                want.append(ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-    assert lib.dgan_abi_version() == 2
-
-
-def test_prune_point_struct_matches_the_compilers_layout(tmp_path):
-    from defensegan_b200 import _native
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "defensegan_b200.h"\n'
-                   'int main(void) { printf("%zu %zu %zu\\n", sizeof(dgan_prune_point), offsetof(dgan_prune_point, iter),'
-                   ' offsetof(dgan_prune_point, keep)); return 0; }\n')
-    exe = tmp_path / "layout"
-    subprocess.run([cc, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    size, off_iter, off_keep = (int(v) for v in subprocess.run([str(exe)], stdout=subprocess.PIPE, text=True,
-                                                                 check=True).stdout.split())
-    P = _native.dgan_prune_point
-    assert (size, off_iter, off_keep) == (ctypes.sizeof(P), P.iter.offset, P.keep.offset)
+from recording import Out, cpu_native  # noqa: F401  (the fixture)
 
 
 def test_sizer_and_layout_refuse_bad_schedules_without_a_handle():
@@ -104,48 +56,6 @@ def test_check_prune_schedule_names_the_bad_point(sched, rr, iters, match):
 
 
 # ---- the binding: the schedule reaches the pruned entry unchanged ----
-
-@pytest.fixture
-def cpu_native(monkeypatch):
-    """A NativeGenerator whose library records its calls (no GPU)."""
-    from defensegan_b200 import _native
-    calls = []
-
-    class FakeLib:
-        def __getattr__(self, name):
-            def f(*args):
-                calls.append((name, args))
-                return 1 << 20 if name.startswith("dgan_workspace_bytes") else 0
-            return f
-
-    class Stream:
-        cuda_stream = 0
-
-    class Out:
-        is_cuda, dtype = True, torch.float32
-
-        def __init__(self, n):
-            self.n = n
-
-        def is_contiguous(self):
-            return True
-
-        def numel(self):
-            return self.n
-
-        def data_ptr(self):
-            return 0
-
-    monkeypatch.setattr(_native, "_require_cuda_f32", lambda t, name: t.to(torch.float32).contiguous())
-    monkeypatch.setattr(_native, "_require_aligned_out", lambda rec: None)
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda d=None: Stream())
-    g = object.__new__(_native.NativeGenerator)
-    g.lib, g.device, g._ws, g._handle = FakeLib(), torch.device("cpu"), None, ctypes.c_void_p(0)
-    g.image_dim, g.hwc, g.latent_dim, g.use_bn = (28, 28, 1), 784, 8, False
-    g.calls, g.Out = calls, Out
-    return g
-
 
 @pytest.mark.parametrize("weighted", [False, True])
 def test_binding_passes_the_schedule_to_the_pruned_entry(cpu_native, weighted):
@@ -279,31 +189,3 @@ def test_rec_cache_dir_names_the_schedule_and_parses_back(tmp_path):
     assert parse(one) == (10, 10.0, 200, [(40, 2)])
     assert parse(plain) == (10, 10.0, 200, None)
     assert parse(plain_num) == (10, 10.0, 200, None)
-
-
-# ---- what ptxas made of the new kernels ----
-
-def test_prune_kernels_compile_for_sm90a_without_spills(tmp_path):
-    from defensegan_b200 import _native
-    nvcc = shutil.which(os.environ.get("NVCC", "nvcc"))
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    flags = [f for f in _native.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC")]
-    cmd = [nvcc] + flags + ["-cubin", "-Xptxas", "-v", os.path.join(_native.CSRC_DIR, "dgan_api.cu"),
-                            "-o", str(tmp_path / "dgan_api.cubin")]
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout[-4000:]
-    names = ("prune_select_kernel", "prune_gather_kernel", "prune_idx_kernel")
-    spills, fn = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r"Function properties for (\S+)", line)
-        if m:
-            fn = m.group(1)
-            continue
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and fn is not None and any(n in fn for n in names):
-            spills[fn] = tuple(int(v) for v in m.groups())
-            fn = None
-    assert all(sum(n in k for k in spills) == 1 for n in names), sorted(spills)
-    bad = {k: v for k, v in spills.items() if v != (0, 0, 0)}
-    assert not bad, bad

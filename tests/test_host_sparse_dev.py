@@ -1,76 +1,20 @@
-"""CPU tests (no GPU) of the sparse deviations (dgan_reconstruct[_measured[_csr / _conv]]_sparse_dev): the header as C99
-and the dgan_sparse_dev layout against the compiler's, the exported symbols, the refusals of the C entries and of Python
-before any native call, the binding's routing (None keeps today's entry), DefenseGANBase's rec_sparse_dev, the cache name
-and its parse-back, the sharded call's refusal, and the fp64 oracle against autograd and the closed form at step = 1."""
+"""CPU tests (no GPU) of the sparse deviations (dgan_reconstruct[_measured[_csr / _conv]]_sparse_dev): the refusals of
+the C entries and of Python before any native call, the binding's routing (None keeps today's entry), DefenseGANBase's
+rec_sparse_dev, the cache name and its parse-back, the sharded call's refusal, and the fp64 oracle against autograd and
+the closed form at step = 1."""
 import ctypes
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from test_host_adam import Out, cpu_native  # noqa: F401  (the recording NativeGenerator fixture)
+from recording import Out, cpu_native, recording_gan  # noqa: F401  (the fixture)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_sparse_dev", "dgan_workspace_bytes_measured_sparse_dev", "dgan_reconstruct_sparse_dev",
-               "dgan_reconstruct_measured_sparse_dev", "dgan_reconstruct_measured_csr_sparse_dev",
-               "dgan_reconstruct_measured_conv_sparse_dev"]
+
 INF = float("inf")
 BAD = [(-1e-3, 1.0), (0.1, -1.0), (float("nan"), 1.0), (0.1, float("nan")), (INF, 1.0), (0.1, INF), (1e39, 1.0),
        (0.1, 1e39)]
-
-
-def _cc():
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    return cc
-
-
-def test_header_is_c99_and_the_struct_layout_matches_ctypes(tmp_path):
-    from defensegan_b200 import _native
-    src = tmp_path / "sdev.c"
-    src.write_text(
-        '#include <stddef.h>\n#include <stdio.h>\n#include "defensegan_b200.h"\n#ifdef DECLS\n'
-        'int (*f)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, const float*, '
-        'const dgan_prune_point*, int, const dgan_sparse_dev*, float*, const float*, const float*, const float*, float*, '
-        'float*, int32_t*, void*, size_t, void*) = dgan_reconstruct_sparse_dev;\n'
-        'int (*g)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, const float*, '
-        'const dgan_prune_point*, int, const dgan_sparse_dev*, float*, const float*, int, const float*, const float*, '
-        'float*, float*, int32_t*, void*, size_t, void*) = dgan_reconstruct_measured_sparse_dev;\n'
-        'int (*h)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, const float*, '
-        'const dgan_prune_point*, int, const dgan_sparse_dev*, float*, const int32_t*, const int32_t*, const float*, int, '
-        'int, const float*, const float*, float*, float*, int32_t*, void*, size_t, void*) = '
-        'dgan_reconstruct_measured_csr_sparse_dev;\n'
-        'int (*k)(dgan_handle, const dgan_rec_params*, const dgan_adam_params*, const float*, const float*, '
-        'const dgan_prune_point*, int, const dgan_sparse_dev*, float*, const dgan_conv_op*, const float*, const float*, '
-        'const float*, float*, float*, int32_t*, void*, size_t, void*) = dgan_reconstruct_measured_conv_sparse_dev;\n'
-        'size_t (*s1)(dgan_handle, int, int, int, int, const dgan_prune_point*, int) = dgan_workspace_bytes_sparse_dev;\n'
-        'size_t (*s2)(dgan_handle, int, int, int, int, const dgan_conv_op*, int, const dgan_prune_point*, int) = '
-        'dgan_workspace_bytes_measured_sparse_dev;\n'
-        'int all(void) { return f == 0 || g == 0 || h == 0 || k == 0 || s1 == 0 || s2 == 0; }\n#endif\n'
-        'int main(void) {\n'
-        '  printf("%d %d %d\\n", (int)sizeof(dgan_sparse_dev), (int)offsetof(dgan_sparse_dev, l1), '
-        '(int)offsetof(dgan_sparse_dev, step));\n'
-        '  return 0;\n}\n')
-    exe = tmp_path / "sdev"
-    subprocess.run([_cc(), "-std=c99", "-pedantic", "-Werror", "-DDECLS", "-c", "-I", os.path.join(ROOT, "include"),
-                    str(src), "-o", str(tmp_path / "sdev.o")], check=True)
-    subprocess.run([_cc(), "-std=c99", "-pedantic", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o",
-                    str(exe)], check=True)
-    out = subprocess.run([str(exe)], check=True, stdout=subprocess.PIPE, text=True).stdout.split()
-    S = _native.dgan_sparse_dev
-    assert [int(v) for v in out] == [ctypes.sizeof(S), S.l1.offset, S.step.offset]
-
-
-def test_symbols_are_exported():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym), sym
-    assert lib.dgan_abi_version() == 2
 
 
 # ---- refusals ----
@@ -200,26 +144,6 @@ def test_binding_refuses_bad_arguments_before_any_native_call(cpu_native):  # no
 
 # ---- DefenseGANBase ----
 
-def _recording_gan():
-    from defensegan_b200.models.gan import MnistDefenseGAN
-    gan = MnistDefenseGAN(test_mode=True, verbose=False)
-    seen = []
-
-    class FakeNative:
-        def reconstruct(self, x, *args, **kw):
-            seen.append(kw)
-            return x
-
-        def reconstruct_measured(self, y, a, *args, **kw):
-            seen.append(kw)
-            return y
-
-    gan._as_cuda = lambda t: t.to(torch.float32)
-    gan._get_native = lambda device: FakeNative()
-    gan.rec_rr, gan.rec_iters = 4, 50
-    return gan, seen
-
-
 def test_defaults_cfg_key_and_kwargs():
     from defensegan_b200.models.gan import MnistDefenseGAN
     from defensegan_b200.operators import ConvOperator
@@ -228,19 +152,19 @@ def test_defaults_cfg_key_and_kwargs():
     cfg = dict(load_config(packaged_cfg_path("mnist")))
     cfg["REC_SPARSE_DEV"] = [0.01, 1.0]
     assert MnistDefenseGAN(cfg=cfg, test_mode=True, verbose=False).rec_sparse_dev == [0.01, 1.0]
-    gan, seen = _recording_gan()
+    gan, seen = recording_gan()
     a = torch.eye(784)[:10]
     gan.reconstruct(torch.rand(2, 28, 28, 1))
     gan.reconstruct_measured(torch.rand(2, 10), a)
-    assert "sparse_dev" not in seen[0] and "deviation_out" not in seen[0] and "sparse_dev" not in seen[1]
+    assert "sparse_dev" not in seen[0][1] and "deviation_out" not in seen[0][1] and "sparse_dev" not in seen[1][1]
     gan.rec_sparse_dev = (0.02, 1)
     dev = torch.zeros(2, 28, 28, 1)
     gan.reconstruct(torch.rand(2, 28, 28, 1), deviation_out=dev)
     gan.reconstruct_measured(torch.rand(2, 10), a.to_sparse_csr())
     gan.reconstruct_measured(torch.rand(2, 49), ConvOperator.box(4), deviation_out=dev)
-    for kw in seen[2:]:
+    for _, kw in seen[2:]:
         assert kw["sparse_dev"] == (pytest.approx(0.02), 1.0)
-    assert seen[2]["deviation_out"] is dev and seen[3]["deviation_out"] is None and seen[4]["deviation_out"] is dev
+    assert seen[2][1]["deviation_out"] is dev and seen[3][1]["deviation_out"] is None and seen[4][1]["deviation_out"] is dev
 
 
 @pytest.mark.parametrize("val", [(-0.5, 1.0), (0.1, float("nan")), (INF, 1.0), 0.1, "x"])

@@ -1,10 +1,8 @@
 """CPU tests (no GPU) of the per-pixel weighted projection: the weighted oracle, the binding's routing and checks, the
 sharding of the weights, the per-layer checker on an emulation of the weighted last-layer forward (and its seeded
 defects), and the plans of the fp16 path's weighted last-layer forward (host code of the CUDA library)."""
-import contextlib
 import ctypes
 import os
-import re
 import socket
 
 import numpy as np
@@ -18,8 +16,7 @@ from oracle import defensegan_oracle as O
 from test_host_layers import Emu, N_PAD, N_ROWS
 from test_host_widths import GRID, _desc
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NEW_SYMBOLS = ["dgan_workspace_bytes_weighted", "dgan_reconstruct_weighted", "dgan_loss_grad_weighted"]
+from recording import cpu_native  # noqa: F401  (the fixture)
 
 
 # ---- the weighted oracle ----
@@ -81,57 +78,6 @@ def test_oracle_all_zero_weights_keep_z0_and_choose_restart_0():
 
 
 # ---- the C-ABI and the binding ----
-
-def test_weighted_symbols_are_exported_with_the_header_signatures():
-    from defensegan_b200 import _native
-    lib = _native.load_library()
-    header = open(os.path.join(ROOT, "include", "defensegan_b200.h")).read()
-    ctype = {"int": ctypes.c_int, "size_t": ctypes.c_size_t}
-    for sym in NEW_SYMBOLS:
-        assert sym in _native.ABI_SYMBOLS and hasattr(lib, sym)
-        m = re.search(r"(\w+)\s+%s\s*\(([^)]*)\)" % sym, header)
-        assert m, sym
-        params = [" ".join(p.split()) for p in m.group(2).split(",")]
-        want = []
-        for p in params:
-            if "*" in p:
-                want.append(ctypes.POINTER(_native.dgan_rec_params) if "dgan_rec_params" in p else ctypes.c_void_p)
-            else:
-                want.append(ctypes.c_void_p if p.startswith("dgan_handle") else ctype[p.rsplit(" ", 1)[0]])
-        fn = getattr(lib, sym)
-        assert list(fn.argtypes) == want, sym
-        assert fn.restype == ctype[m.group(1)], sym
-
-
-class FakeLib:
-    """Stands in for the CUDA library under NativeGenerator: logs every entry point it is called through."""
-
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        def fn(*args):
-            self.calls.append((name, args))
-            return 4096 if name.startswith("dgan_workspace_bytes") else 0
-        return fn
-
-
-@pytest.fixture
-def cpu_native(monkeypatch):
-    """A NativeGenerator (MNIST) on the CPU whose library is a FakeLib."""
-    from defensegan_b200 import _native
-
-    class Stream:
-        cuda_stream = 0
-
-    monkeypatch.setattr(_native, "_require_cuda_f32", lambda t, name: t.to(torch.float32).contiguous())
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    monkeypatch.setattr(torch.cuda, "current_stream", lambda d=None: Stream())
-    g = object.__new__(_native.NativeGenerator)
-    g.lib, g.device, g._ws, g._handle = FakeLib(), torch.device("cpu"), None, ctypes.c_void_p(0)
-    g.image_dim, g.hwc, g.latent_dim = (28, 28, 1), 784, 8
-    return g
-
 
 class FakeOut:
     """The `out` buffer of reconstruct as the binding checks it (a contiguous CUDA float32 tensor shaped like x)."""

@@ -12,26 +12,10 @@ one row of an accumulator ahead, so that its round trip to L2 overlaps MMAs or o
   weighted CelebA kind (N = 48) is the exception: it has no registers for a second set of pairs."""
 import re
 
-from test_sass_wgmma_groups import _sass
+import compiled
 
 EPI_FINAL = {8, 9, 10, 11}
 EPI_FINAL_TANH3_W = 11
-
-
-def _instructions(lines):
-    out = []
-    for line in lines:
-        m = re.search(r"/\*([0-9a-f]{4,})\*/\s+(.*?);", line)
-        if m:
-            out.append((int(m.group(1), 16), m.group(2).strip()))
-    return out
-
-
-def _kind(name):
-    m = re.search(r"tc_bsgemm2_kernelILi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)E(6__half|f)", name)
-    assert m, name
-    n, maxb, ksub, epi, t = m.groups()
-    return int(n), int(maxb), int(ksub), int(epi), 2 if t == "6__half" else 4
 
 
 def _regs(op):
@@ -63,10 +47,6 @@ def _is_ldg(text):
     return re.search(r"(^|\s)LDG\b|(^|\s)LDG\.", text) is not None
 
 
-def _is_stg(text):
-    return re.search(r"(^|\s)STG\b|(^|\s)STG\.", text) is not None
-
-
 def tma_epilogue_loads(ins):
     """Global loads between each wait for all MMAs and the last TMA store after it."""
     bad = []
@@ -96,7 +76,7 @@ def final_loads_used_before_a_store(ins):
             continue
         dest = _ldg_dest(t)
         for b, u in ins[i + 1:]:
-            if _is_stg(u):
+            if compiled.is_stg(u):
                 break
             if dest & _sources(u):
                 bad.append("%04x %s  (read at %04x by %s)" % (a, t, b, u))
@@ -106,13 +86,13 @@ def final_loads_used_before_a_store(ins):
     return bad
 
 
-def test_epilogue_does_not_wait_for_global_memory(tmp_path):
-    funcs = _sass(tmp_path)
+def test_epilogue_does_not_wait_for_global_memory():
+    funcs = compiled.sass("tc_bsgemm2_kernel")
     assert len(funcs) >= 20, "too few tc_bsgemm2_kernel instantiations in the SASS: %d" % len(funcs)
     n_tma = n_final = 0
     for name, lines in funcs.items():
-        n, maxb, ksub, epi, out_bytes = _kind(name)
-        ins = _instructions(lines)
+        n, maxb, ksub, epi, out_bytes = compiled.tc_template(name)
+        ins = compiled.instructions(lines)
         if out_bytes == 2 and n >= 64 and epi not in EPI_FINAL:
             n_tma += 1
             bad = tma_epilogue_loads(ins)

@@ -9,8 +9,7 @@ fence.proxy.async (MEMBAR.ALL.CTA) that orders the staging writes before the sto
 - The staging buffer is written with stmatrix (STSM, four 8x8 matrices per instruction), not with scalar STS."""
 import re
 
-from test_sass_epilogue import _instructions, _is_stg, _kind
-from test_sass_wgmma_groups import _sass
+import compiled
 
 EPI_FINAL = {8, 9, 10, 11}
 
@@ -33,17 +32,17 @@ def epilogue_spans(ins):
     return spans
 
 
-def test_tma_epilogue_stores(tmp_path):
-    funcs = _sass(tmp_path)
+def test_tma_epilogue_stores():
+    funcs = compiled.sass("tc_bsgemm2_kernel")
     n_tma = 0
     for name, lines in funcs.items():
-        n, maxb, ksub, epi, out_bytes = _kind(name)
+        n, maxb, ksub, epi, out_bytes = compiled.tc_template(name)
         if not (out_bytes == 2 and n >= 64 and epi not in EPI_FINAL):
             continue
         n_tma += 1
-        ins = _instructions(lines)
+        ins = compiled.instructions(lines)
         for d, fence, hi in epilogue_spans(ins):
-            stg = ["%04x %s" % (a, t) for a, t in ins if d < a < fence and _is_stg(t)]
+            stg = ["%04x %s" % (a, t) for a, t in ins if d < a < fence and compiled.is_stg(t)]
             assert not stg, (name, "global store ahead of the item's last fence.proxy.async", stg)
             ops = [_mnem(t) for a, t in ins if d < a <= hi]
             assert any(o.startswith("STSM") for o in ops), (name, "the staging buffer is not written with stmatrix")

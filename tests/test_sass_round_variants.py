@@ -8,17 +8,10 @@ around each HGMMA and close a group at every one. The 1- and 8-slot and the narr
 and are held to the same group rule."""
 import re
 
-from test_sass_step_loop import _instructions
-from test_sass_wgmma_groups import _sass
+import compiled
 
 _BRANCH = re.compile(r"\bBR[AX]\b|\bBRA\.|\bEXIT\b|\bRET\b")
 _WAIT1 = "WARPGROUP.DEPBAR.LE gsb0, 0x1"
-
-
-def _template_args(name):
-    m = re.search(r"tc_bsgemm2_kernelILi(\d+)ELi(\d+)ELi(\d+)ELi(\d+)E", name)
-    assert m, name
-    return tuple(int(v) for v in m.groups())      # N, slots per round, k16 per op, epilogue
 
 
 def _blocks(ins):
@@ -54,12 +47,12 @@ def _next_wgmma_event(ins, start):
     return None
 
 
-def test_each_round_variant_is_one_wgmma_group(tmp_path):
-    funcs = _sass(tmp_path)
+def test_each_round_variant_is_one_wgmma_group():
+    funcs = compiled.sass("tc_bsgemm2_kernel")
     assert len(funcs) >= 20, "too few tc_bsgemm2_kernel instantiations in the SASS: %d" % len(funcs)
     for name, lines in funcs.items():
-        n, maxb, ksub, _ = _template_args(name)
-        ins = _instructions(lines)
+        n, maxb, ksub, _, _ = compiled.tc_template(name)
+        ins = compiled.instructions(lines)
         blocks = _blocks(ins)
         assert blocks, name
         for b in blocks:

@@ -9,23 +9,14 @@ target) that holds every HGMMA and the last wait on a barrier before the first H
 the step's operands. The loop around it is the item loop, whose head and epilogue may load from global memory."""
 import re
 
-from test_sass_wgmma_groups import _sass
+import compiled
 
 
-def _instructions(lines):
-    out = []
-    for line in lines:
-        m = re.search(r"/\*([0-9a-f]{4,})\*/\s+(.*?);", line)
-        if m:
-            out.append((int(m.group(1), 16), m.group(2)))
-    return out
-
-
-def test_no_global_load_in_the_step_loop(tmp_path):
-    funcs = _sass(tmp_path)
+def test_no_global_load_in_the_step_loop():
+    funcs = compiled.sass("tc_bsgemm2_kernel")
     assert len(funcs) >= 20, "too few tc_bsgemm2_kernel instantiations in the SASS: %d" % len(funcs)
     for name, lines in funcs.items():
-        ins = _instructions(lines)
+        ins = compiled.instructions(lines)
         mma = [a for a, t in ins if "HGMMA" in t]
         waits = [a for a, t in ins if "SYNCS.PHASECHK" in t and a < min(mma)]
         assert mma and waits, name
